@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- disparity volumes/s of the STEREO_GIF hot path (CVC -> CVF -> WTA) on B200.
+"""bench.py -- disparity volumes/s of the STEREO_GIF hot path (CVC -> CVF -> WTA) on H100.
 
-Contract (see the task brief): `python bench.py --gpus N --steps K --warmup W` prints ONE JSON line
+`python bench.py --gpus N --steps K --warmup W` prints ONE JSON line
 on rank 0.  A "step" is one stereo frame through CostConst_GPU + CostFilter_GPU + DispSelect_GPU
 producing BOTH disparity maps.  Workload at every N: BASELINE config C4, synthetic 1920x1080, D=128,
 fp32 (`--workload C3|C5` select the other synthetic BASELINE configs).  N>1 (launched by torchrun, one
@@ -13,13 +13,15 @@ packed (cost,d) minima -> final maps) is a fused reduce-scatter + all-gather ove
   e2e      : same metric through the host-facing C-ABI calls: frames in pinned HOST memory, the H2D copy of
              every frame's two images and the D2H read of both u8 maps inside the timed region (the upload
              of frame k+1 overlaps the computation of frame k: psm_set_images_async)
-  roofline : the fused CVF kernel's algorithmic bytes / its event-timed duration vs the measured HBM peak,
-             plus the pipe that actually limits it (from the committed ncu summary)
+  roofline : the fused CVF kernel's algorithmic bytes / its event-timed duration vs the HBM peak
   parity   : before the line is printed, the maps fetched by the last e2e step are compared with the CPU
              oracle on a row band (exact mode: equal; mixed mode: +-1, flips counted)
   cpu_baseline / --impl reference : the reference's pthreads CPU path on the host cores: oracle/_ref (the
              reference's own CVC/CVF/DispSel sources compiled against an OpenCV shim) when it was built,
              else the C port; a bounded slice sample per step, all cores and the reference's 8-thread cap
+  --dump-outputs DIR : after the timed steps, what the last timed step computed (single GPU): both disparity maps
+             (lDis.npy, rDis.npy) and a fixed seeded sample of both filtered cost volumes (lVol_sample.npy,
+             rVol_sample.npy, with the sampled (d, y, x) in vol_sample_index.npy), all float32, ~38 MB at C4
 """
 import argparse
 import ctypes as C
@@ -55,17 +57,53 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
-def profile_facts(workload, mode):
-    """ncu-derived facts for THIS workload and mode from the committed summary (profiles/cvf_profile_facts.json):
-    DRAM traffic per launch and the limiting pipe.  None when that combination was never profiled."""
-    p = os.path.join(ROOT, "profiles", "cvf_profile_facts.json")
+def device_info(index):
+    """GPU name and power limit: an absolute number is only meaningful with the card it was measured on."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
     try:
-        return json.load(open(p)).get(f"{workload}:{mode}")
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=20).stdout.strip()
+        info["power_limit_w"] = float(out)
     except Exception:
-        return None
+        pass
+    return info
+
+
+L2_BYTES = 50e6   # H100 L2
+DUMP_SAMPLES = 1 << 20   # voxels sampled per filtered volume by --dump-outputs
+
+
+def dump_outputs(out_dir, de, W, H, d_count):
+    """Both u8 disparity maps and a seeded sample of both filtered volumes as they are on the device now, float32 .npy."""
+    import torch
+
+    class DeviceArray:   # zero-copy view of a device buffer the library owns
+        def __init__(self, ptr, n, typestr):
+            self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 3}
+
+    def device(what, n_of_pitch, typestr):
+        from primestereomatch_b200 import capi
+        ptr, pitch = C.c_void_p(), C.c_size_t()
+        capi.check(capi.lib().psm_device_ptr(de.handle, what, C.byref(ptr), C.byref(pitch)), de.handle)
+        return torch.as_tensor(DeviceArray(ptr.value, n_of_pitch(pitch.value), typestr), device="cuda"), pitch.value
+
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(20240601)
+    d = rng.integers(0, d_count, DUMP_SAMPLES)
+    y = rng.integers(0, H, DUMP_SAMPLES)
+    x = rng.integers(0, W, DUMP_SAMPLES)
+    np.save(os.path.join(out_dir, "vol_sample_index.npy"), np.stack([d, y, x]).astype(np.float32))
+    for v, name in enumerate(("l", "r")):
+        m, _ = device(2 + v, lambda p: H * p, "|u1")
+        np.save(os.path.join(out_dir, f"{name}Dis.npy"), m.view(H, W).cpu().numpy().astype(np.float32))
+        vol, pitch = device(v, lambda p: d_count * H * p, "<f4")
+        flat = torch.from_numpy((d * H + y) * pitch + x).to("cuda")
+        np.save(os.path.join(out_dir, f"{name}Vol_sample.npy"), vol[flat].cpu().numpy())
 
 
 class ClockSampler:
@@ -210,6 +248,8 @@ def main():
     ap.add_argument("--upload", default="banded", choices=["banded", "replicated"],
                     help="N>1, e2e: banded = every rank uploads H/N rows of both images and the bands are "
                          "all-gathered over NVLink; replicated = every rank uploads both full images over PCIe")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/*.npy (single GPU)")
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "p2p-barrier", "nccl"],
                     help="N>1: p2p = fused WTA + exchange over NVLink peer memory, ordered by device-side flags; "
                          "p2p-barrier = same kernels separated by NCCL barriers; nccl = local WTA then ncclAllGather")
@@ -232,6 +272,8 @@ def main():
 
     if not torch.cuda.is_available():
         raise SystemExit("bench.py needs a CUDA device: the product has no CPU path")
+    if args.dump_outputs and (world > 1 or args.emulate_shards > 1):
+        raise SystemExit("bench.py: --dump-outputs needs a single-GPU run of the whole frame")
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -367,6 +409,8 @@ def main():
     if rank == 0:
         sampler.start()
     total_ms = timed(False, args.steps)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, de, W, H, d_count)
     launches_per_step = (de.launch_count() - launches0) // (warm + args.steps)
     kms = kernel_times(args.steps)
     clocks = sampler.stop() if rank == 0 else None
@@ -432,7 +476,6 @@ def main():
         kern_ms = float(np.mean(kms))
         achieved = algo_bytes / (kern_ms * 1e-3) / 1e9
         mode = MODES[args.cvf_mode]
-        facts = profile_facts(args.workload, mode) if world == 1 else None
         h2d = banded.h2d_bytes() if banded is not None else 2 * W * H * 3 * 4
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": warm,
@@ -443,14 +486,11 @@ def main():
                        "cvf_mode": mode, "variant": args.variant,
                        **({"emulated_share_of": args.emulate_shards, "NOTE": "tuning run, not a benchmark line"} if args.emulate_shards > 1 else {}),
                        "l2": f"inputs larger than L2: each step streams {4 * V * 4 / 1e9:.2f} GB of volumes (raw+filtered, 2 views) per GPU"
-                             + ("" if 4 * V * 4 > 252e6 else "; NOTE: smaller than 2 x L2, L2 reuse between steps is possible"),
+                             + ("" if 4 * V * 4 > 2 * L2_BYTES else "; NOTE: smaller than 2 x L2, L2 reuse between steps is possible"),
                        "stage_ms_last_step": stage},
             "roofline": {"bound": "hbm", "kernel": "cvf_stream_kernel (fused guided filter, both views per launch)",
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": (facts or {}).get("dram_bytes_per_launch"),
-                         "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": kern_ms, "peak_source": peak_src,
-                         "limiter": (facts or {}).get("limiter",
-                                                      "not profiled for this workload/mode; see profiles/ for C4")},
+                         "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": kern_ms, "peak_source": peak_src},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d * world,
                     "upload": ("banded, two-deep pipeline: each rank uploads H/N rows, NCCL all-gather over NVLink, on a side stream" if banded is not None
                                else "two-deep pipeline: frame k+1 uploads (copy stream) while frame k computes"),
@@ -462,18 +502,8 @@ def main():
             "parity_checked": bool(parity and parity["ok"]),
             "parity": parity,
             "clocks": clocks,
+            "device": device_info(local_rank),
         }
-        if facts and "executed_warp_instructions" in facts:
-            # what actually binds: the instruction stream at 12 warps per SM.  Live: warp instructions of the profiled launch
-            # (committed ncu summary of this workload and mode) / the kernel time measured in THIS run, against 4 warp
-            # instructions per clock per SM at the SM clock sampled in this run.
-            sm_mhz = float((clocks or {}).get("sm_mhz") or 1965.0)
-            peak_ips = 148 * 4 * sm_mhz * 1e6
-            ips = facts["executed_warp_instructions"] / (kern_ms * 1e-3)
-            line["roofline"]["issue"] = {"achieved": ips / 1e12, "peak": peak_ips / 1e12, "unit": "T warp-instructions/s",
-                                         "frac": ips / peak_ips, "issue_active_pct_in_profile": facts.get("issue_active_pct"),
-                                         "warps_per_sm": facts.get("warps_per_sm"),
-                                         "note": "instruction count from the committed ncu capture of this workload/mode; time and clock from this run"}
         if mixed is not None:
             mixed["roofline_frac"] = algo_bytes / (mixed["kernel_ms"] * 1e-3) / 1e9 / peak
             line["tolerance_mode"] = mixed

@@ -1,5 +1,5 @@
 /*
- * prime_stereo_b200.h -- C-ABI of the B200-native STEREO_GIF hot path
+ * prime_stereo_b200.h -- C-ABI of the H100-native (sm_90a) STEREO_GIF hot path
  * (cost-volume construction -> guided-image-filter cost aggregation -> WTA).
  *
  * This is the drop-in boundary that sits under the reference's DispEst "_GPU" stage

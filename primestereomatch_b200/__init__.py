@@ -1,4 +1,4 @@
-"""primestereomatch_b200 -- B200-native (sm_100a) STEREO_GIF hot path: CVC -> CVF -> WTA.
+"""primestereomatch_b200 -- H100-native (sm_90a) STEREO_GIF hot path: CVC -> CVF -> WTA.
 
 The product is the CUDA library `libprime_stereo_b200.so` (sources in csrc/, C-ABI in
 include/prime_stereo_b200.h).  `DispEst` mirrors the reference facade over that C-ABI.

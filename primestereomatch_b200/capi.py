@@ -105,7 +105,7 @@ def check(rc, ctx=None):
 PLAN_FIELDS = ("threads", "nstrips", "ndgroups", "nseg", "seg_rows", "pack_gl", "pack_x0", "pack_ndg", "pack_first", "grid")
 
 
-def cvf_plan(width, height, d_count, sm_count=148, no_pack=False):
+def cvf_plan(width, height, d_count, sm_count=132, no_pack=False):
     """psm_cvf_plan as a dict (needs no device)."""
     out = (C.c_int * 10)()
     rc = lib().psm_cvf_plan(width, height, d_count, sm_count, 1 if no_pack else 0, out, 10)

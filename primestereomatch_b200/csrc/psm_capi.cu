@@ -1,4 +1,4 @@
-// psm_capi.cu -- the C-ABI (include/prime_stereo_b200.h) over the sm_100a kernels.
+// psm_capi.cu -- the C-ABI (include/prime_stereo_b200.h) over the sm_90a kernels.
 // Host logic only: context/buffer ownership, stage ordering, launches, timers.  No CPU
 // compute path exists here: every stage is a CUDA kernel launch or it fails.
 #include "../../include/prime_stereo_b200.h"
@@ -270,8 +270,8 @@ CvfPlan plan_cvf(int W, int H, int d_count, int nsm, int threads_override, int t
             const long rem_ctas = ctas - (waves - 1) * slots;
             const double last = rem_ctas >= slots ? 1.0 : (0.5 + 0.5 * (double)rem_ctas / (double)slots);
             // + half a CTA duration: CTAs do not finish in lock-step, and the shorter they are the shorter the ragged end of the
-            // kernel.  Fitted on measurements (profiles/r2_segrows_ab2.txt, r2_segrows_shards_ab.txt): C4 -> 4 segments, C3 -> 6,
-            // 16 slices of C4 (one of 8 ranks) -> 9, 32 slices of C5 -> 8, each the fastest or within 1 % of it.
+            // kernel.  At 132 SMs (H100): C4 -> 5 segments, C3 -> 6, 16 slices of C4 (one of 8 ranks) -> 8, 32 slices of C5 -> 10,
+            // each the fastest count in an A/B over forced counts or within 1.5 % of it.
             const long cost = (long)(((double)(waves - 1) + last + 0.5) * (rows + 11) * 16);
             if (best_cost < 0 || cost < best_cost) { best_cost = cost; best_ns = ns; best_rows = rows; }
         }
@@ -288,11 +288,11 @@ int launch_cvf_stream(psm_ctx* c)
     CvfParams P;
     for (int v = 0; v < 2; ++v) { P.vol_in[v] = c->vol[v]; P.vol_out[v] = c->vol_alt[v]; P.guide[v] = c->guide[v]; }
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->d_count;
-    // the packed remainder needs the tensor-memory ring and no CTA-level staging (variants 1, 2 and 9 keep the plain
-    // decomposition); option 105 = 1 disables it
+    // the packed remainder needs no CTA-level staging (variant 9 stages the guide rows of one strip); variants 1 and 2
+    // keep the plain decomposition of the round-1 kernel; option 105 = 1 disables it
     const bool plain_variant = c->cvf_variant == 9 || c->cvf_variant == 2 || (c->cvf_mode != PSM_CVF_MIXED && c->cvf_variant == 1);
-    int nsm = 148;
-    cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device);
+    int nsm = 0;
+    PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
     const CvfPlan plan = plan_cvf(c->W, c->H, c->d_count, nsm, c->cvf_threads, c->cvf_target_rows,
                                   !c->cvf_no_pack && !plain_variant && !c->cvf_remap);
     const int nthreads = plan.nthreads;
@@ -300,60 +300,62 @@ int launch_cvf_stream(psm_ctx* c)
     P.pack_gl = plan.pack_gl; P.pack_x0 = plan.pack_x0; P.pack_ndg = plan.pack_ndg; P.pack_first = plan.pack_first;
     P.remap_sms = 0; P.remap_ctas = 0;
     if (c->cvf_remap) {
-        int nsm = 0;
-        PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
         P.remap_sms = nsm;
         P.remap_ctas = (int)((227 * 1024) / ((size_t)8 * 4 * nthreads * sizeof(float4) + 1024));  // resident CTAs by shared memory
         if (P.remap_ctas * nthreads * 170 > 65536) P.remap_ctas = 65536 / (nthreads * 170);      // ... and by registers
     }
-    // kernel selection: mode (exact / mixed) x tuning variant (PSM option 100)
-    //   variant 0 (shipped): integer widening + history ring in tensor memory (+ L1 prefetch of the next guide rows in exact mode)
-    //   variant 1: F2F conversions, ring in shared memory (the round-1 kernel, kept as the A/B baseline; exact only)
-    //   variant 2: integer widening, ring in shared memory
-    //   variant 3: F2F conversions, ring in tensor memory (exact only)
-    //   variant 4: as 0 with <= 128 registers (4 CTAs of 128 threads per SM)
-    //   variants 5-8: experiments recorded in DESIGN.md section 9 (prefetch on/off, stage-2 F2F, 144/152-register builds)
+    // kernel selection: mode (exact / mixed) x tuning variant (PSM option 100); every build keeps its history ring in
+    // shared memory
+    //   variant 0 (shipped): integer widening (+ L1 prefetch of the next guide rows in exact mode)
+    //   variant 1: F2F conversions (the round-1 kernel, kept as the A/B baseline; exact only)
+    //   variant 2: integer widening, plain decomposition
+    //   variant 3: F2F conversions (exact only)
+    //   variant 4: as 0 with <= 128 registers
+    //   variants 5-8: experiments recorded in DESIGN.md (prefetch on/off, stage-2 F2F, 144/152-register builds)
     using kern_t = void (*)(CvfParams);
     kern_t kern = nullptr;
-    bool tm = true, staged = false;
+    bool staged = false;
     if (c->cvf_mode == PSM_CVF_MIXED) {
         switch (c->cvf_variant) {
-        case 2: kern = cvf_stream_kernel<3, 1, kS2Mixed, 0>; tm = false; break;
-        case 4: kern = cvf_stream_kernel<4, 1, kS2Mixed, 1>; break;
-        case 5: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1, 1>; break;
-        case 6: kern = cvf_stream_kernel<4, 1, kS2Mixed, 1, 1>; break;
-        case 7: kern = cvf_stream_kernel<5, 1, kS2Mixed, 1, 0>; break;   // 144 registers
-        case 8: kern = cvf_stream_kernel<6, 1, kS2Mixed, 1, 0>; break;   // 152 registers
-        case 9: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1, 2>; staged = true; break;   // TMA-staged guide rows
-        case 10: kern = cvf_stream_kernel<4, 1, kS2Mixed, 1, 3>; break;  // light prefetch, <= 128 registers: 16 warps per SM with 128-thread CTAs
-        case 11: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1, 3>; break;  // light prefetch, 168 registers
-        case 12: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1, 0, 1>; break;  // packed exact adds
-        case 14: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1, 4, 0>; break;  // coefficient rows one step ahead
-        case 15: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1, 4, 1>; break;  // ... + packed exact adds
-        case 13: kern = cvf_stream_kernel<4, 1, kS2Mixed, 1, 3, 1>; break;  // packed exact adds + light prefetch, 128 registers
-        default: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1>; break;
+        case 2: kern = cvf_stream_kernel<3, 1, kS2Mixed>; break;
+        case 4: kern = cvf_stream_kernel<4, 1, kS2Mixed>; break;
+        case 5: kern = cvf_stream_kernel<3, 1, kS2Mixed, 1>; break;
+        case 6: kern = cvf_stream_kernel<4, 1, kS2Mixed, 1>; break;
+        case 7: kern = cvf_stream_kernel<5, 1, kS2Mixed, 0>; break;   // 144 registers
+        case 8: kern = cvf_stream_kernel<6, 1, kS2Mixed, 0>; break;   // 152 registers
+        case 9: kern = cvf_stream_kernel<3, 1, kS2Mixed, 2>; staged = true; break;   // TMA-staged guide rows
+        case 10: kern = cvf_stream_kernel<4, 1, kS2Mixed, 3>; break;  // light prefetch, <= 128 registers
+        case 11: kern = cvf_stream_kernel<3, 1, kS2Mixed, 3>; break;  // light prefetch, 168 registers
+        case 12: kern = cvf_stream_kernel<3, 1, kS2Mixed, 0, 1>; break;  // exact adds as fma
+        case 14: kern = cvf_stream_kernel<3, 1, kS2Mixed, 4, 0>; break;  // coefficient rows one step ahead
+        case 15: kern = cvf_stream_kernel<3, 1, kS2Mixed, 4, 1>; break;  // ... + exact adds as fma
+        case 13: kern = cvf_stream_kernel<4, 1, kS2Mixed, 3, 1>; break;  // exact adds as fma + light prefetch, 128 registers
+        default: kern = cvf_stream_kernel<3, 1, kS2Mixed>; break;
         }
     } else {
         switch (c->cvf_variant) {
-        case 1: kern = cvf_stream_kernel<3, 0, kS2Exact, 0>; tm = false; break;
-        case 2: kern = cvf_stream_kernel<3, 1, kS2Exact, 0>; tm = false; break;
-        case 3: kern = cvf_stream_kernel<3, 0, kS2Exact, 1>; break;
-        case 4: kern = cvf_stream_kernel<4, 1, kS2Exact, 1>; break;
-        case 6: kern = cvf_stream_kernel<3, 2, kS2Exact, 1, 0>; break;
-        case 7: kern = cvf_stream_kernel<3, 2, kS2Exact, 1, 1>; break;
-        case 8: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 0>; break;
-        case 9: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 2>; staged = true; break;   // TMA-staged guide rows
-        case 10: kern = cvf_stream_kernel<4, 1, kS2Exact, 1, 3>; break;  // light prefetch, <= 128 registers
-        case 11: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 3>; break;  // light prefetch, 168 registers
-        case 12: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 1, 1>; break;  // packed exact adds
-        case 14: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 4, 0>; break;  // coefficient rows one step ahead
-        default: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 1>; break;
+        case 1: kern = cvf_stream_kernel<3, 0, kS2Exact>; break;
+        case 2: kern = cvf_stream_kernel<3, 1, kS2Exact>; break;
+        case 3: kern = cvf_stream_kernel<3, 0, kS2Exact>; break;
+        case 4: kern = cvf_stream_kernel<4, 1, kS2Exact>; break;
+        case 6: kern = cvf_stream_kernel<3, 2, kS2Exact, 0>; break;
+        case 7: kern = cvf_stream_kernel<3, 2, kS2Exact, 1>; break;
+        case 8: kern = cvf_stream_kernel<3, 1, kS2Exact, 0>; break;
+        case 9: kern = cvf_stream_kernel<3, 1, kS2Exact, 2>; staged = true; break;   // TMA-staged guide rows
+        case 10: kern = cvf_stream_kernel<4, 1, kS2Exact, 3>; break;  // light prefetch, <= 128 registers
+        case 11: kern = cvf_stream_kernel<3, 1, kS2Exact, 3>; break;  // light prefetch, 168 registers
+        case 12: kern = cvf_stream_kernel<3, 1, kS2Exact, 1, 1>; break;  // exact adds as fma
+        case 14: kern = cvf_stream_kernel<3, 1, kS2Exact, 4, 0>; break;  // coefficient rows one step ahead
+        default: kern = cvf_stream_kernel<3, 1, kS2Exact, 1>; break;
         }
     }
-    const size_t smem = (tm ? (staged ? (size_t)kStSmemBytes : 0) : (size_t)8 * 4 * nthreads * sizeof(float4)) + (size_t)c->cvf_extra_smem;
+    const size_t smem = (staged ? (size_t)kStSmemBytes : 0) + (size_t)8 * 4 * nthreads * sizeof(float4) + (size_t)c->cvf_extra_smem;
+    int smem_max = 0;
+    PSM_CUDA(c, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    if (smem > (size_t)smem_max)
+        return fail(c, PSM_EINVAL, "streaming filter: %zu bytes of shared memory for %d threads exceed the %d a block may have",
+                    smem, nthreads, smem_max);
     PSM_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (tm && !staged && !c->cvf_extra_smem)  // nothing lives in shared memory: give the whole array to L1 (the guide rows are re-read by every slice)
-        PSM_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxL1));
     P.guide_flags = c->guide_flags;
     P.one = 1.0f; P.mone = -1.0f;
     const unsigned grid = plan.grid;
@@ -384,7 +386,7 @@ int psm_device_count(void)
 
 const char* psm_build_info(void)
 {
-    return "prime_stereo_b200 0.1 (sm_100a; " PSM_BUILD_FLAGS ")";
+    return "prime_stereo_b200 0.1 (sm_90a; " PSM_BUILD_FLAGS ")";
 }
 
 const char* psm_last_error(psm_ctx* ctx) { return ctx ? ctx->err : g_create_error; }
@@ -988,8 +990,8 @@ int psm_post_process_device(psm_ctx* c)
     if (c->p2p_own && c->p2p_seq > 0)
         if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
-    int nsm = 148;
-    cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device);
+    int nsm = 0;
+    PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
     for (int v = 0; v < 2; ++v) {
         const float* g = c->guide[v];
         dim3 blk(256), grd((c->W + 255) / 256, c->H);

@@ -1,4 +1,4 @@
-// psm_common.cuh -- shared device helpers for the B200 (sm_100a) STEREO_GIF path.
+// psm_common.cuh -- shared device helpers for the H100 (sm_90a) STEREO_GIF path.
 //
 // Numerics rule for this library: every float operation that the reference performs as a
 // separate IEEE operation (reference builds with plain -O3 on baseline x86-64, no FMA

@@ -11,16 +11,14 @@
 //     final rounding.  Box sums here are fp64 running column sums (+ newest row, - oldest row) and
 //     8-wide row sums, scaled and rounded once to float.
 //   * every fp32 operation of a, b and q is a separate IEEE round-to-nearest op in the reference's
-//     order (CVF.cpp:87-163).  Multiplies of two columns share one FMUL2; adds that consume a
-//     product stay scalar because ptxas 12.9 contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2
-//     even with --fmad=false.
+//     order (CVF.cpp:87-163): __fmul_rn / __fadd_rn / __fsub_rn, which ptxas never contracts.
 //   * PSM_CVF_EXACT: all eight box sums in fp64 -> q bit-exact.
 //     PSM_CVF_MIXED: the four stage-1 sums in fp64 (a, b stay bit-exact), the four stage-2 sums
 //     (box of a0,a1,a2,b) in fp32 with a FIXED summation tree (below) -> q within ~3e-6 of exact,
 //     deterministic and position-independent (tests/mixed_model.py restates it on the CPU).
 //
-// f32 -> f64 without the conversion (XU) pipe.  F2F runs at 16/clk/SM on B200 and the exact filter
-// needs 24 conversions per voxel; it was the binding pipe (profiles/r1_*).  For a NON-NEGATIVE
+// f32 -> f64 without the conversion (XU) pipe.  F2F has a fraction of the FMA pipe's rate and the exact
+// filter needs 24 conversions per voxel, so it binds when every widening uses it.  For a NON-NEGATIVE
 // finite float with bit pattern u (zero and denormals included) the 64-bit integer u * 2^29, read
 // as a double, is exactly f * 2^-896: the 8-bit exponent field lands in the low bits of the 11-bit
 // field (bias error -896), the mantissa lines up, denormals stay denormals of the same scaled
@@ -33,15 +31,15 @@
 // converts with F2F and rescales, and from then on the warp also widens a,b with F2F, so
 // non-finite data propagates exactly like in the reference.
 //
-// Work decomposition (B200-first; nothing like the reference's per-slice Mat pipeline):
+// Work decomposition (nothing like the reference's per-slice Mat pipeline):
 //   warp   = one strip of 128 input columns (112 output columns) of ONE disparity slice, one row segment
 //   lane   = 4 consecutive columns -> every global access is a 128-bit load/store
 //   CTA    = wpc warps = wpc consecutive slices of the same strip and segment (guide rows hit in L1)
 //   stage 1: S1[4 boxes][4 cols] fp64 running column sums of p, I0*p, I1*p, I2*p;
 //            row sums = per-lane prefix/suffix sums + 4 fp64 shuffles per box (lane+1 total, lane+2 prefixes)
 //   a,b    : CVF.cpp:92-155 with the d-independent adjugate / 1/det precomputed per pixel (K2)
-//   ring   : thread-private 8-slot history (512 B per thread) in TENSOR MEMORY (below; shared memory in the TM = 0
-//            builds), the only on-chip history: stage-1 "oldest rows" are re-read from the raw volume (L1/L2).
+//   ring   : thread-private 8-slot history (512 B per thread) in shared memory, the only on-chip history: stage-1
+//            "oldest rows" are re-read from the raw volume (L1/L2).
 //            EXACT: slots hold a,b rows;  MIXED: slots hold PAIR rows  pair(t) = ab(t-1) + ab(t)
 //   stage 2 EXACT: S2[4 planes][4 cols] fp64 running column sums of a0,a1,a2,b (newest from
 //            registers, oldest from the ring); row sums as in stage 1
@@ -79,7 +77,7 @@ namespace psm {
 constexpr int kStripOut = 112;  // output columns per warp
 constexpr int kStripIn = 128;   // input columns per warp
 constexpr int kCvfThreads = 96;       // CTA size when the slice count is not a multiple of 4: 3 slice-warps, 4 CTAs/SM (else 128 x 3)
-constexpr int kCvfMaxThreads = 512;   // 16 warps: every ring of an SM's tensor memory in one CTA
+constexpr int kCvfMaxThreads = 448;   // 14 warps: 448 rings of 512 B = 224 KB, the most shared memory one CTA may have (227 KB)
 
 // stage-2 modes (template parameter S2M)
 constexpr int kS2Exact = 0;  // fp64 running sums
@@ -96,13 +94,16 @@ struct CvfParams {
     // packed remainder strips (0 = off): blocks >= pack_first filter the W - nstrips*112 rightmost columns with
     // 32 / pack_gl slices per warp (pack_gl = 8 or 16 lanes per slice); see "Packed remainder" in the header comment
     int pack_gl, pack_first, pack_ndg, pack_x0;
-    float one, mone;            // +1.0f / -1.0f, passed at run time so that the compiler cannot fold them (packed exact adds, PA)
+    float one, mone;            // +1.0f / -1.0f, passed at run time so that the compiler cannot fold them (exact adds as fma, PA)
 };
 
-struct f2x2 { float2 lo, hi; };  // four columns as two packed pairs
+struct f2x2 { float2 lo, hi; };  // four columns as two pairs
 __device__ __forceinline__ f2x2 from4(const float4& v) { return {make_float2(v.x, v.y), make_float2(v.z, v.w)}; }
 __device__ __forceinline__ float4 to4(const f2x2& v) { return make_float4(v.lo.x, v.lo.y, v.hi.x, v.hi.y); }
-__device__ __forceinline__ f2x2 mul2(const f2x2& a, const f2x2& b) { return {__fmul2_rn(a.lo, b.lo), __fmul2_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f2x2 mul2(const f2x2& a, const f2x2& b)
+{
+    return {make_float2(__fmul_rn(a.lo.x, b.lo.x), __fmul_rn(a.lo.y, b.lo.y)), make_float2(__fmul_rn(a.hi.x, b.hi.x), __fmul_rn(a.hi.y, b.hi.y))};
+}
 __device__ __forceinline__ f2x2 add2(const f2x2& a, const f2x2& b)
 {
     return {make_float2(fadd(a.lo.x, b.lo.x), fadd(a.lo.y, b.lo.y)), make_float2(fadd(a.hi.x, b.hi.x), fadd(a.hi.y, b.hi.y))};
@@ -111,25 +112,23 @@ __device__ __forceinline__ f2x2 sub2(const f2x2& a, const f2x2& b)
 {
     return {make_float2(fsub(a.lo.x, b.lo.x), fsub(a.lo.y, b.lo.y)), make_float2(fsub(a.hi.x, b.hi.x), fsub(a.hi.y, b.hi.y))};
 }
-// Packed EXACT add / subtract of values that may be products: x + y == fma(x, 1, y) and x - y == fma(y, -1, x) with one
-// rounding each, so an FFMA2 whose multiplier is a RUN-TIME 1.0f / -1.0f (ptxas cannot fold or re-associate it, and an fma
-// is never contracted with the multiply that feeds it) does two IEEE additions per instruction.  This sidesteps the
-// FMUL2 + FADD2 -> FFMA2 contraction of ptxas 12.9 that forces plain adds of products to stay scalar.
+// EXACT add / subtract as an fma: x + y == fma(x, 1, y) and x - y == fma(y, -1, x) with one rounding each; the
+// multiplier is a RUN-TIME 1.0f / -1.0f, so ptxas can neither fold nor re-associate it (PA builds).
 __device__ __forceinline__ float2 fma2(const float2& a, const float2& b, const float2& c)
 {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(*reinterpret_cast<const unsigned long long*>(&a)),
-        "l"(*reinterpret_cast<const unsigned long long*>(&b)), "l"(*reinterpret_cast<const unsigned long long*>(&c)));
-    return *reinterpret_cast<float2*>(&d);
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
-// packed add (FADD2): only for operands that are NOT products (see the contraction note above)
-__device__ __forceinline__ f2x2 addp(const f2x2& a, const f2x2& b) { return {__fadd2_rn(a.lo, b.lo), __fadd2_rn(a.hi, b.hi)}; }
+// add of operands that are not products
+__device__ __forceinline__ f2x2 addp(const f2x2& a, const f2x2& b)
+{
+    return {make_float2(__fadd_rn(a.lo.x, b.lo.x), __fadd_rn(a.lo.y, b.lo.y)), make_float2(__fadd_rn(a.hi.x, b.hi.x), __fadd_rn(a.hi.y, b.hi.y))};
+}
 __device__ __forceinline__ float get(const f2x2& v, int j) { return j == 0 ? v.lo.x : (j == 1 ? v.lo.y : (j == 2 ? v.hi.x : v.hi.y)); }
 
-// PSM_KNOCKOUT (never defined in the product build): tools/cvf_knockout.cu compiles this header with single operation
+// PSM_KNOCKOUT (never defined in the product build): an experiment may compile this header with single operation
 // classes removed -- results are wrong, only the TIME is of interest -- to measure what the kernel is sensitive to.
-// bit 0 shuffles, bit 1 tensor-memory ring, bit 2 guide loads, bit 3 stores, bit 4 stage-1 widening + fp64 running sums,
+// bit 0 shuffles, bit 1 history ring, bit 2 guide loads, bit 3 stores, bit 4 stage-1 widening + fp64 running sums,
 // bit 5 volume (p) loads.
 #ifndef PSM_KNOCKOUT
 #define PSM_KNOCKOUT 0
@@ -180,50 +179,6 @@ __device__ __forceinline__ f2x2 hsum8f(const f2x2& c)
 }
 
 
-// ---- a,b / pair history ring in TENSOR MEMORY ---------------------------------------------------
-// The ring (8 slots x 4 planes x 4 columns per thread = 128 words per thread, 16 KB per warp) is the
-// only per-slice on-chip history and was what capped the kernel at 12 warps per SM when it lived in
-// shared memory (192 KB of rings left ~35 KB of L1 for the guide rows).  On sm_100a each SM has
-// 256 KB of tensor memory (512 columns x 128 lanes x 32 bit) that this kernel does not need for
-// MMA accumulators, and tcgen05.ld/st in the 32x32b shape give every thread of a warp a private
-// row: lane i of warp w addresses TMEM lane 32*(w%4)+i.  One ring = 128 columns of one lane quarter;
-// a CTA allocates 128 columns for its <= 4 warps.  One LDTM / STTM moves a whole slot (16 words per
-// thread) -- 4x fewer instructions than LDS/STS.128 -- and shared memory / L1 is left to the loads.
-__device__ __forceinline__ void tmem_ld16(unsigned taddr, f2x2 (&v)[4])
-{
-    unsigned r[16];
-    if (PSM_KNOCKOUT & 2) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) v[q] = {make_float2(1.f, 2.f), make_float2(3.f, (float)taddr)};
-        return;
-    }
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-        v[q] = {make_float2(__uint_as_float(r[4 * q]), __uint_as_float(r[4 * q + 1])),
-                make_float2(__uint_as_float(r[4 * q + 2]), __uint_as_float(r[4 * q + 3]))};
-}
-__device__ __forceinline__ void tmem_st16(unsigned taddr, const f2x2 (&v)[4])
-{
-    unsigned r[16];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        r[4 * q] = __float_as_uint(v[q].lo.x); r[4 * q + 1] = __float_as_uint(v[q].lo.y);
-        r[4 * q + 2] = __float_as_uint(v[q].hi.x); r[4 * q + 3] = __float_as_uint(v[q].hi.y);
-    }
-    if (PSM_KNOCKOUT & 2) return;
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-                 :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-                    "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-constexpr unsigned kTmemCols = 128;   // one ring = 128 columns of one lane quarter; a CTA allocates one block per 4 warps
-
-
 // ---- TMA (bulk async copy) staging of the guide rows --------------------------------------------
 // The 13 guide rows a step needs (10 coefficient planes at the a,b columns, 3 image planes at the
 // input columns) are identical for every slice-warp of a CTA.  One elected lane of warp 0 copies them
@@ -232,7 +187,7 @@ constexpr unsigned kTmemCols = 128;   // one ring = 128 columns of one lane quar
 // one arrival per warp.  Consumers read with LDS at immediate offsets: no per-load address arithmetic,
 // no L2 latency on the critical path, and the image rows (needed as newest, output and oldest row of
 // the stage-1 window) stay in a 16-row ring, so they are fetched from L2 once per CTA instead of
-// three times per warp.
+// three times per warp.  The staging area lies in front of the rings in the dynamic shared memory.
 constexpr int kStCoefStages = 4;       // coefficient stages in flight (power of two)
 constexpr int kStIRows = 16;           // image-row ring (power of two >= 8 + stages)
 constexpr int kStLook = 2;             // the producer runs this many steps ahead
@@ -266,22 +221,21 @@ __device__ __forceinline__ float4 lds4(unsigned addr)
 // IW  : 0 = F2F everywhere; 1 = integer widening into the scaled domain in both stages; 2 = integer widening in
 //       stage 1 (non-negative values: one instruction each), F2F in the exact stage 2 (signed values would cost three)
 // S2M : kS2Exact / kS2Mixed
-// TM  : 1 = history ring in tensor memory (tcgen05.ld/st), 0 = in shared memory
-// PA  : 1 = adds / subtracts of products as packed FFMA2 with a run-time unit multiplier (exact, see fma2)
+// PA  : 1 = adds / subtracts of products as fma with a run-time unit multiplier (exact, see fma2)
 // PF  : 1 = prefetch the next step's guide rows into L1;  2 = stage the guide rows in shared memory with bulk async
-//       copies (TMA) issued two steps ahead by one lane per CTA (needs TM = 1: the ring is not in shared memory);
-//       3 = light prefetch (only the newest p row a step ahead; everything else is an L1 hit with the ring in TMEM);
+//       copies (TMA) issued two steps ahead by one lane per CTA;
+//       3 = light prefetch (only the newest p row a step ahead; everything else is loaded where it is used);
 //       4 = the ten coefficient rows are loaded one step ahead as well (40 more live registers)
-// register budgets by MINB: 3 -> 168 regs (3 CTAs x 128 thr or 4 x 96: 12 warps/SM); 4 -> 128 regs (16 warps);
-// 5 -> 144 regs (2 CTAs x 224 thr = 14 warps, two TMEM column blocks per lane quarter); 6 -> 152 regs (13 warps)
+// register budgets by MINB: 3 -> 168 regs (3 CTAs x 128 thr or 4 x 96: 12 warps/SM); 4 -> 128 regs; 5 -> 144 regs
+// (2 CTAs x 224 thr = 14 warps); 6 -> 152 regs.  Shared memory (512 B of ring per thread) caps an SM at 3 CTAs of 128.
 constexpr int cvf_max_regs(int minb) { return minb == 3 ? 168 : (minb == 4 ? 128 : (minb == 5 ? 144 : 152)); }
 
-template <int MINB, int IW, int S2M, int TM, int PF = 0, int PA = 0>
+template <int MINB, int IW, int S2M, int PF = 0, int PA = 0>
 __global__ void __maxnreg__(cvf_max_regs(MINB))
 cvf_stream_kernel(const CvfParams P)
 {
-    extern __shared__ float4 ring[];  // TM == 0: [8 slots][4 planes][blockDim.x threads]
-    __shared__ unsigned tmem_base_smem;
+    extern __shared__ float4 smem_dyn[];  // PF == 2: staging area (kStSmemBytes), then the rings
+    float4* ring = smem_dyn + (PF == 2 ? kStSmemBytes / 16 : 0);  // [8 slots][4 planes][blockDim.x threads]
     constexpr bool MIXED = (S2M == kS2Mixed);
     constexpr double kMean1 = IW ? kMeanScaled : kMeanPlain;   // stage-1 mean scale
     constexpr double kMean2 = IW == 1 ? kMeanScaled : kMeanPlain;   // stage-2 (exact) mean scale: IW == 2 keeps S2 unscaled
@@ -329,34 +283,20 @@ cvf_stream_kernel(const CvfParams P)
     const bool active = dlc_raw < P.Dloc;     // warp-uniform unless packed
     const int dlc = active ? dlc_raw : P.Dloc - 1;
     constexpr bool ST = (PF == 2);
-    const unsigned st_base = (unsigned)__cvta_generic_to_shared(ring);   // staging area (ST): barriers, coefficient stages, image-row ring
-    if (ST && tid == 0) {
+    const unsigned st_base = (unsigned)__cvta_generic_to_shared(smem_dyn);   // staging area (ST): barriers, coefficient stages, image-row ring
+    if (ST) {
+        if (tid == 0) {
 #pragma unroll
-        for (int i = 0; i < kStCoefStages; ++i) { mbar_init(st_base + 8 * i, 1); mbar_init(st_base + 8 * (kStCoefStages + i), wpc); }
-        mbar_init(st_base + 8 * 2 * kStCoefStages, 1);   // prologue barrier
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    unsigned tring = 0;   // TMEM address of this warp's ring (lane quarter = warp % 4, column block = warp / 4)
-    // columns this CTA allocates: one 128-column block per group of 4 warps, rounded up to a power of two
-    const unsigned tmem_cols = wpc <= 4 ? kTmemCols : (wpc <= 8 ? 2 * kTmemCols : 4 * kTmemCols);
-    if (TM) {
-        // one warp allocates the CTA's columns, everybody reads the base after a fenced barrier; this
-        // barrier and the one before the deallocation are the only CTA-wide synchronisations
-        if (warp == 0) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                         :: "r"((unsigned)__cvta_generic_to_shared(&tmem_base_smem)), "r"(tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+            for (int i = 0; i < kStCoefStages; ++i) { mbar_init(st_base + 8 * i, 1); mbar_init(st_base + 8 * (kStCoefStages + i), wpc); }
+            mbar_init(st_base + 8 * 2 * kStCoefStages, 1);   // prologue barrier
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // lane field = bits 31..16: (warp%4)*32 << 16; warps 4.. use the next 128-column block of their lane quarter
-        tring = tmem_base_smem + ((unsigned)(warp & 3) << 21) + (unsigned)(warp >> 2) * kTmemCols;
-    } else if (!active) {
-        return;  // warps never synchronise with each other
+        __syncthreads();   // the barriers are initialised before anyone waits on them; the only CTA-wide synchronisation
+        // a surplus warp of the last slice group (Dloc % wpc != 0) redoes the last slice with its stores masked:
+        // every warp arrives on the stage barriers
+    } else if (!__any_sync(0xffffffffu, active)) {
+        return;  // warps never synchronise with each other; lanes of a packed warp do (shuffles), so only whole warps leave
     }
-    // TM: a surplus warp of the last slice group (Dloc % wpc != 0) redoes the last slice with its stores
-    // masked, so that every warp reaches the barrier before the deallocation without a divergent region
 
     const int W = P.W, H = P.H;
     const unsigned Wp = (unsigned)P.Wp;
@@ -413,21 +353,19 @@ cvf_stream_kernel(const CvfParams P)
 
     // history ring accessors (slot = 0..7): a whole slot = 4 planes x 4 columns of this thread
     auto ring_ld = [&](int slot, f2x2 (&v)[4]) {
-        if (TM) tmem_ld16(tring + (unsigned)slot * 16u, v);
-        else {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) v[q] = from4(ring[(slot * 4 + q) * nthr + tid]);
+        for (int q = 0; q < 4; ++q) {
+            if (PSM_KNOCKOUT & 2) v[q] = {make_float2(1.f, 2.f), make_float2(3.f, (float)slot)};
+            else v[q] = from4(ring[(slot * 4 + q) * nthr + tid]);
         }
     };
     auto ring_st = [&](int slot, const f2x2 (&v)[4]) {
-        if (TM) tmem_st16(tring + (unsigned)slot * 16u, v);
-        else {
+        if (PSM_KNOCKOUT & 2) return;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) ring[(slot * 4 + q) * nthr + tid] = to4(v[q]);
-        }
+        for (int q = 0; q < 4; ++q) ring[(slot * 4 + q) * nthr + tid] = to4(v[q]);
     };
-    auto ring_wait_ld = [&]() { if (TM) tmem_wait_ld(); };
-    auto ring_wait_st = [&]() { if (TM) tmem_wait_st(); };
+    auto ring_wait_ld = [&]() {};
+    auto ring_wait_st = [&]() {};
 
     struct RowIn { float4 p, i0, i1, i2; };
     auto load_at = [&](size_t ro) {  // ro: byte offset of the row
@@ -747,9 +685,9 @@ cvf_stream_kernel(const CvfParams P)
             ro_y += rowB;
         };
         if (PF == 3) {
-            // ---- "light prefetch" steady loop: with the ring in tensor memory the whole shared-memory array is L1, so
-            // only the NEWEST p row (which comes from HBM) is loaded a step ahead; the image rows, the oldest p row
-            // (read 7 steps ago by this warp) and the coefficient rows are L1 hits and are loaded where they are used.
+            // ---- "light prefetch" steady loop: only the NEWEST p row (which comes from HBM) is loaded a step ahead; the
+            // image rows, the oldest p row (read 7 steps ago by this warp) and the coefficient rows are mostly cache hits
+            // and are loaded where they are used.
             // 28 fewer live registers than the full prefetch: the build for 16 warps per SM (<= 128 registers).
             float4 pn = xn.p;
             auto steady_lp = [&](auto slow_tag) {
@@ -927,13 +865,6 @@ cvf_stream_kernel(const CvfParams P)
         }
     }
     for (; t <= Tend; ++t) generic_step(t);
-    if (TM) {
-        tmem_wait_st();
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0)
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base_smem), "r"(tmem_cols) : "memory");
-    }
 }
 
 }  // namespace psm

@@ -14,7 +14,7 @@
 // the colours to 256 indices with cv::kmeans (RNG-seeded, un-vendored): parity for natural images is unpinned
 // by the reference itself; this kernel needs no clustering -- it evaluates the weights directly.
 //
-// B200 mapping (nothing like the reference's serial column scan with necklace tables): one WARP per pixel,
+// GPU mapping (nothing like the reference's serial column scan with necklace tables): one WARP per pixel,
 //   the 361 window taps dealt round-robin to the 32 lanes (12 rounds), each tap one 4-byte load of a packed
 //   u32 image (disparity << 24 | R6 << 16 | G6 << 8 | B6);
 //   the taps ((disparity, fixed-point weight) pairs) stay in registers, 12 per lane; the weighted median is found by eight

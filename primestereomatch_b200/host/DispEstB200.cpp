@@ -20,7 +20,7 @@ DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl)
         if (psm_create(&ctx, wid, hei, maxDis, 0) != PSM_OK) {
             // reference logs OpenCL set-up failures and carries on (DispEst.cpp:69-79); so do we, with
             // the GPU stages then returning an error code instead of computing anything on the CPU
-            std::fprintf(stderr, "Failed to create the B200 context: %s\n", psm_last_error(nullptr));
+            std::fprintf(stderr, "Failed to create the GPU context: %s\n", psm_last_error(nullptr));
             ctx = nullptr;
         }
     }

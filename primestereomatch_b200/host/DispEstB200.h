@@ -1,5 +1,5 @@
 // DispEstB200.h -- C++ host facade with the reference's DispEst API surface
-// (/root/reference/include/DispEst.h:21-109) whose "_GPU" stage methods run on the B200 C-ABI
+// (reference include/DispEst.h:21-109) whose "_GPU" stage methods run on the H100 C-ABI
 // library (include/prime_stereo_b200.h) instead of the reference's OpenCL classes.
 //
 // Two ways to use it (INTEGRATION.md):
@@ -106,7 +106,7 @@ public:
 private:
     int not_built(const char* what) const
     {
-        std::fprintf(stderr, "DispEst::%s: CPU stage not built into the B200 facade (use the reference's own)\n", what);
+        std::fprintf(stderr, "DispEst::%s: CPU stage not built into the GPU facade (use the reference's own)\n", what);
         return -1;
     }
     cv::Mat lImg, rImg;

@@ -12,9 +12,9 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the built artefacts are git-ignored: on a fresh checkout compile them once (nvcc cross-compiles
-    # sm_100a without a GPU; the oracle is plain gcc)
+    # sm_90a without a GPU; the oracle is plain gcc)
     lib = os.path.join(ROOT, "primestereomatch_b200", "libprime_stereo_b200.so")
     orc = os.path.join(ROOT, "oracle", "libstereo_oracle.so")
     if not (os.path.exists(lib) and os.path.exists(orc)):

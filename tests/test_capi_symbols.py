@@ -30,7 +30,7 @@ def test_library_exports_every_declared_symbol():
 def test_build_info_and_error_paths_without_gpu():
     L = capi.lib()
     info = L.psm_build_info().decode()
-    assert "sm_100a" in info
+    assert "sm_90a" in info
     n = L.psm_device_count()
     assert n >= 0
     ctx = ctypes.c_void_p()

@@ -70,11 +70,12 @@ def test_row_segments_partition_the_image(H, d_count):
 
 
 def test_measured_plans():
-    """The segment counts the A/B runs found fastest (profiles/r2_segrows_ab2.txt, r2_segrows_shards_ab.txt)."""
-    assert capi.cvf_plan(1920, 1080, 128)["nseg"] == 4           # C4
+    """The segment counts the planner picks for a 132-SM H100.  A/B of the CVF kernel over forced segment counts on an
+    H100 80GB HBM3 (700 W): each pick was the fastest count or within 1.5 % of it."""
+    assert capi.cvf_plan(1920, 1080, 128)["nseg"] == 5           # C4
     assert capi.cvf_plan(1280, 720, 64)["nseg"] == 6             # C3
-    assert capi.cvf_plan(1920, 1080, 16)["nseg"] == 9            # C4 on 8 GPUs
-    assert capi.cvf_plan(1920, 1080, 32)["nseg"] == 8            # C5 on 8 GPUs
+    assert capi.cvf_plan(1920, 1080, 16)["nseg"] == 8            # C4 on 8 GPUs
+    assert capi.cvf_plan(1920, 1080, 32)["nseg"] == 10           # C5 on 8 GPUs
     assert capi.cvf_plan(1920, 1080, 16)["threads"] == 128       # 4 x 4 slices, no idle warp slot
 
 

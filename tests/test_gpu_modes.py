@@ -1,6 +1,6 @@
 """GPU tests of the CVF kernel's modes and paths (all through the C-ABI):
-  * PSM_CVF_EXACT in its four builds (integer widening / F2F conversions x history ring in tensor memory / in
-    shared memory; variant 0 is shipped, variant 1 is the round-1 kernel) -- all bit-exact;
+  * PSM_CVF_EXACT in its builds (integer widening / F2F conversions, prefetch and staging options; variant 0 is
+    shipped, variant 1 is the round-1 kernel) -- all bit-exact;
   * inputs outside the integer-widening domain (negative / -0 costs, negative guide values) -- bit-exact through
     the per-row slow path and the guide flag;
   * PSM_CVF_MIXED -- bit-exact against its CPU model (tests/mixed_model.py), within tolerance of the exact path;

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C-ABI, against the
+"""GPU parity tests (run on an H100): the CUDA path, called through the C-ABI, against the
 CPU oracle on the same inputs.  Bar: bit-exact raw costs, guide planes, a/b, filtered costs and
 u8 disparity maps (north_star tolerance is 1e-4 on a/b and +-1 disparity; we hold the stronger
 bit-exact bar in the default PSM_CVF_EXACT mode)."""
