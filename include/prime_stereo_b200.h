@@ -107,6 +107,18 @@ int psm_destroy(psm_ctx* ctx);
 
 int psm_set_option(psm_ctx* ctx, int key, int value);
 
+/* Guided-filter window (the reference's GIF_R_WIN: box Size(window, window), anchor window/2, BORDER_REFLECT_101)
+ * and regulariser (GIF_EPS) for every later filtering call of this context. Default (8, 0.0001f).
+ * Valid: 1 <= window <= 32, eps finite and > 0; anything else returns PSM_EINVAL and leaves the context unchanged.
+ * Applies to psm_cost_filter, psm_read_guide_plane (planes 3-11), psm_read_ab_slice and psm_cost_filter_fgf (box
+ * K = 2*(window/s)+1 with this eps, as FastGuidedFilter(img, GIF_R_WIN, GIF_EPS, s) does; PSM_EINVAL when the FGF kernel's
+ * shared memory cannot hold that box, e.g. window 16 at s = 1).  Changing either value invalidates the cached guide planes.
+ * At the defaults every call runs exactly the tuned 8 x 8 kernels; any other setting runs a generic-window streaming filter
+ * (PSM_CVF_EXACT only: psm_cost_filter returns PSM_EINVAL in PSM_CVF_MIXED / PSM_CVF_NAIVE mode) whose results are
+ * bit-exact under the same condition as the default path, with 2^23 replaced by 2^(29 - ceil(log2 window^2)).
+ * Sharded contexts filter slice by slice as before: every rank must set the same parameters. */
+int psm_set_guided_filter(psm_ctx* ctx, int window, float eps);
+
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream. */
 int psm_set_stream(psm_ctx* ctx, void* cuda_stream);

@@ -11,6 +11,7 @@
 #include <cmath>
 
 #include "psm_cvf_stream.cuh"
+#include "psm_cvf_window.cuh"
 #include "psm_pp.cuh"
 #include "psm_fgf.cuh"
 
@@ -71,6 +72,9 @@ struct psm_ctx {
     bool ev_valid[kNumStages] = {};
     int cvf_mode = PSM_CVF_EXACT, gray_mode = 0, timing = 1, cvf_variant = 0, cvf_target_rows = 0, cvf_extra_smem = 0, cvf_threads = 0, cvf_remap = 0, cvf_no_pack = 0, cvc_variant = 0, guide_seg_rows = 0, cvc_chunk = 0;
     bool have_images = false, guide_valid = false, have_cvc = false, filtered = false;
+    int gif_win = kBoxK;                    // guided-filter window (GIF_R_WIN) and regulariser (GIF_EPS), psm_set_guided_filter
+    float gif_eps = kGifEps;
+    bool gif_default() const { return gif_win == kBoxK && gif_eps == kGifEps; }
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -187,6 +191,19 @@ int upload_async(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep)
 int ensure_guide(psm_ctx* c)
 {
     if (c->guide_valid) return PSM_OK;
+    if (!c->gif_default()) {   // any other window / eps: the generic precompute (psm_cvf_window.cuh)
+        WinGuideParams P;
+        P.guide[0] = c->guide[0]; P.guide[1] = c->guide[1];
+        P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.K = c->gif_win; P.a = c->gif_win / 2;
+        P.seg_rows = kWinGuideSegRows;
+        P.scale = 1.0 / ((double)P.K * P.K);
+        P.eps = c->gif_eps;
+        dim3 grd((c->W + 127) / 128, (c->H + P.seg_rows - 1) / P.seg_rows, 2);
+        guide_window_kernel<<<grd, 128, 0, c->stream>>>(P);
+        PSM_LAUNCH_CHECK(c);
+        c->guide_valid = true;
+        return PSM_OK;
+    }
     GuideParams P;
     P.guide[0] = c->guide[0]; P.guide[1] = c->guide[1];
     P.guide_flags = c->guide_flags;
@@ -360,6 +377,35 @@ int launch_cvf_stream(psm_ctx* c)
     P.one = 1.0f; P.mone = -1.0f;
     const unsigned grid = plan.grid;
     kern<<<grid, nthreads, smem, c->stream>>>(P);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
+// The guided filter at a non-default window / eps (psm_cvf_window.cuh): strips of kWinThreads - 2K + 2 output columns, and
+// as many row segments (of >= 4K rows, so that the ~2K warm-up rows stay a small share) as it takes to give every SM a few CTAs.
+int launch_cvf_window(psm_ctx* c)
+{
+    WinParams P;
+    for (int v = 0; v < 2; ++v) { P.vol_in[v] = c->vol[v]; P.vol_out[v] = c->vol_alt[v]; P.guide[v] = c->guide[v]; }
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->d_count;
+    P.K = c->gif_win; P.a = c->gif_win / 2;
+    P.scale = 1.0 / ((double)P.K * P.K);
+    P.tw = kWinThreads - 2 * P.K + 2;
+    P.nstrips = (c->W + P.tw - 1) / P.tw;
+    P.ring_stride = (c->W < P.tw ? c->W : P.tw) + P.K - 1;
+    int nsm = 0, smem_max = 0;
+    PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
+    PSM_CUDA(c, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    const long base = 2L * P.Dloc * P.nstrips;
+    int nseg = 1;
+    while (base * nseg < 4L * nsm && c->H / (nseg + 1) >= 4 * P.K) ++nseg;
+    P.seg_rows = (c->H + nseg - 1) / nseg;
+    P.nseg = (c->H + P.seg_rows - 1) / P.seg_rows;
+    const size_t smem = win_smem_bytes(P.K, P.ring_stride);
+    if (smem > (size_t)smem_max)
+        return fail(c, PSM_EINVAL, "guided filter window %d: %zu bytes of shared memory exceed the %d a block may have", P.K, smem, smem_max);
+    PSM_CUDA(c, cudaFuncSetAttribute(cvf_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cvf_window_kernel<<<(unsigned)(base * P.nseg), kWinThreads, smem, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
@@ -557,6 +603,17 @@ int psm_set_option(psm_ctx* c, int key, int value)
     }
 }
 
+int psm_set_guided_filter(psm_ctx* c, int window, float eps)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (window < 1 || window > kWinMax) return fail(c, PSM_EINVAL, "guided-filter window %d outside 1..%d", window, kWinMax);
+    if (!(eps > 0.0f) || !std::isfinite(eps)) return fail(c, PSM_EINVAL, "guided-filter eps %g is not a finite value > 0", (double)eps);
+    if (window != c->gif_win || eps != c->gif_eps) c->guide_valid = false;   // mean_I, var_I and the solve depend on both
+    c->gif_win = window;
+    c->gif_eps = eps;
+    return PSM_OK;
+}
+
 int psm_set_stream(psm_ctx* c, void* cuda_stream)
 {
     if (int rc = bind(c)) return rc;
@@ -666,8 +723,21 @@ int psm_cost_filter(psm_ctx* c)
 {
     if (int rc = bind(c)) return rc;
     if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter before psm_cost_const");
+    if (!c->gif_default() && c->cvf_mode != PSM_CVF_EXACT)
+        return fail(c, PSM_EINVAL, "CVF mode %s exists only for the default guided filter (window 8, eps 1e-4); "
+                    "this context has window %d, eps %g: use PSM_CVF_EXACT", c->cvf_mode == PSM_CVF_MIXED ? "MIXED" : "NAIVE",
+                    c->gif_win, (double)c->gif_eps);
     if (int rc = stage_begin(c, 2)) return rc;
     if (int rc = ensure_guide(c)) return rc;
+    if (!c->gif_default()) {
+        if (int rc = stage_begin(c, 4)) return rc;
+        if (int rc = launch_cvf_window(c)) return rc;
+        if (int rc = stage_end(c, 4)) return rc;
+        for (int v = 0; v < 2; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
+        c->have_cvc = false;
+        c->filtered = true;
+        return stage_end(c, 2);
+    }
     const bool tiny = c->W < 16 || c->H < 16;
     if (c->cvf_mode == PSM_CVF_NAIVE || tiny) {
         if (int rc = ensure_ab(c, (size_t)c->d_count)) return rc;
@@ -702,7 +772,15 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
     if (s != 1 && s != 2 && s != 4 && s != 8) return fail(c, PSM_EINVAL, "sub-sampling rate must be 1, 2, 4 or 8 (got %d)", s);
     if (c->W / s < 1 || c->H / s < 1) return fail(c, PSM_EINVAL, "image smaller than the sub-sampling rate");
     FgfGeom g;
-    g.W = c->W; g.H = c->H; g.Wp = c->Wp; g.s = s; g.w2 = c->W / s; g.h2 = c->H / s; g.K = 2 * (kBoxK / s) + 1;
+    // FastGuidedFilter(img, r = GIF_R_WIN, eps = GIF_EPS, s) (DispEst.cpp:283-284): box K = 2 * (r / s) + 1 at low resolution
+    g.W = c->W; g.H = c->H; g.Wp = c->Wp; g.s = s; g.w2 = c->W / s; g.h2 = c->H / s; g.K = 2 * (c->gif_win / s) + 1;
+    {
+        int smem_max = 0;
+        PSM_CUDA(c, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+        if (fgf_smem_bytes(g.K) > (size_t)smem_max)
+            return fail(c, PSM_EINVAL, "Fast Guided Filter box %d (window %d, rate %d) needs %zu bytes of shared memory, more than "
+                        "the %d a block may have", g.K, c->gif_win, s, fgf_smem_bytes(g.K), smem_max);
+    }
     g.ifx = 1.0 / ((double)g.w2 / g.W); g.ify = 1.0 / ((double)g.h2 / g.H);
     const size_t n2 = (size_t)g.w2 * g.h2;
     if (c->fgf_s != s) {   // (re)build buffers and the INTER_LINEAR plan for this rate
@@ -739,7 +817,7 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
     if (int rc = stage_begin(c, 4)) return rc;
     for (int v = 0; v < 2; ++v) {
         dim3 blk(128), g2((g.w2 + 127) / 128, g.h2);
-        fgf_guide_kernel<<<g2, blk, 0, c->stream>>>(c->guide[v], c->plane, g, kGifEps, c->fgf_lo[v]);
+        fgf_guide_kernel<<<g2, blk, 0, c->stream>>>(c->guide[v], c->plane, g, c->gif_eps, c->fgf_lo[v]);
         PSM_LAUNCH_CHECK(c);
         dim3 g3((g.w2 + kFgfTX - 1) / kFgfTX, (g.h2 + kFgfTY - 1) / kFgfTY, c->d_count);
         const size_t fsmem = fgf_smem_bytes(g.K);
@@ -1073,8 +1151,13 @@ int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
     if (int rc = ensure_guide(c)) return rc;
     if (int rc = ensure_ab(c, 1)) return rc;
     dim3 blk(128), grd((c->W + 127) / 128, c->H, 1);
-    cvf_naive_ab_kernel<<<grd, blk, 0, c->stream>>>(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->guide[view],
-                                                  c->plane, c->W, c->H, c->Wp, 1, c->ab);
+    if (!c->gif_default())
+        ab_window_kernel<<<grd, blk, 0, c->stream>>>(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->guide[view], c->plane,
+                                                     c->W, c->H, c->Wp, c->gif_win, c->gif_win / 2,
+                                                     1.0 / ((double)c->gif_win * c->gif_win), c->ab);
+    else
+        cvf_naive_ab_kernel<<<grd, blk, 0, c->stream>>>(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->guide[view],
+                                                      c->plane, c->W, c->H, c->Wp, 1, c->ab);
     PSM_LAUNCH_CHECK(c);
     const size_t wb = c->W * sizeof(float);
     // scratch is laid out [4][ab_slices][plane]; only slice 0 of each plane group was written with nslices=1

@@ -96,6 +96,14 @@ class DispEst:
     def setSubsampleRate(self, newRate):
         self.subsample_rate = int(newRate)
 
+    def setGuidedFilter(self, window, eps):
+        """Guided-filter window and regulariser (the reference's compile-time GIF_R_WIN and GIF_EPS, include/ComFunc.h:49-50)
+        for every later CostFilter_GPU / CostFilter_FGF_GPU call; default (8, 1e-4).  Raises PsmError on values outside
+        1 <= window <= 32, 0 < eps < inf."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_guided_filter(self._ctx, int(window), float(eps)), self._ctx)
+        return 0
+
     def set_option(self, key, value):
         capi.check(self._lib.psm_set_option(self._ctx, int(key), int(value)), self._ctx)
 

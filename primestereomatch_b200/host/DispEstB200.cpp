@@ -49,6 +49,12 @@ int DispEst::setThreads(unsigned int newThreads)
     return 0;
 }
 
+int DispEst::setGuidedFilter(int window, float eps)
+{
+    if (!ctx) return -1;
+    return psm_set_guided_filter(ctx, window, eps);
+}
+
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
 {

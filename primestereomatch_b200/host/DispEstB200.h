@@ -82,6 +82,9 @@ public:
     int setInputImages(cv::Mat l, cv::Mat r);
     int setThreads(unsigned int newThreads);
     void setSubsampleRate(unsigned int newRate) { subsample_rate = newRate; }
+    // guided-filter window and eps (the reference's GIF_R_WIN / GIF_EPS) for the later CostFilter calls; see
+    // psm_set_guided_filter.  INTEGRATION.md: call setGuidedFilter(GIF_R_WIN, GIF_EPS) so the GPU mode follows the build.
+    int setGuidedFilter(int window, float eps);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
