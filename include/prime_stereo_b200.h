@@ -119,6 +119,18 @@ int psm_set_option(psm_ctx* ctx, int key, int value);
  * Sharded contexts filter slice by slice as before: every rank must set the same parameters. */
 int psm_set_guided_filter(psm_ctx* ctx, int window, float eps);
 
+/* Matching cost (the reference's ALPHA_32F and truncation thresholds TAU_1_32F / TAU_2_32F, include/CVC.h:18-23) for every
+ * later psm_cost_const of this context: src/CVC.cpp:18-39 with the truncation lines 24-25 and 36-37 restored, all in float:
+ *   clr = (|dB| + |dG|) + |dR|,  grd = |dGradX|   (border pixels: the BC_32F differences in double, rounded once)
+ *   if (clr > tau_color) clr = tau_color;  if (grd > tau_grad) grd = tau_grad;   (a NaN difference stays NaN)
+ *   cost = alpha * clr + (1 - alpha) * grd       (every operation rounded separately, no FMA)
+ * Default (0.9f, +inf, +inf): the reference as shipped, with the truncation commented out.  Valid: 0 <= alpha <= 1, each
+ * tau >= 0 or +inf (no truncation); anything else, NaN included, returns PSM_EINVAL and leaves the context unchanged.
+ * The guide planes do not depend on it.  At the default every call runs exactly the tuned cost-volume kernels; any other
+ * setting runs a parameterised build of the shipped one (options 106 and 108 do not apply to it).  Sharded contexts build
+ * their own slices: every rank must set the same values. */
+int psm_set_matching_cost(psm_ctx* ctx, float alpha, float tau_color, float tau_grad);
+
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream. */
 int psm_set_stream(psm_ctx* ctx, void* cuda_stream);

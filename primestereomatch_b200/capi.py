@@ -20,6 +20,7 @@ SYMBOLS = [
     "psm_p2p_set_peers", "psm_disp_select_keys_p2p", "psm_disp_reduce_p2p", "psm_disp_fetch_p2p", "psm_read_cost_slice", "psm_write_cost_slice",
     "psm_read_guide_plane", "psm_read_ab_slice", "psm_device_ptr", "psm_stage_ms",
     "psm_launch_count", "psm_sync", "psm_last_error", "psm_build_info", "psm_cvf_plan", "psm_set_guided_filter",
+    "psm_set_matching_cost",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -54,6 +55,7 @@ def lib():
     L.psm_destroy.argtypes = [vp]
     L.psm_set_option.argtypes = [vp, i, i]
     L.psm_set_guided_filter.argtypes = [vp, i, C.c_float]
+    L.psm_set_matching_cost.argtypes = [vp, C.c_float, C.c_float, C.c_float]
     L.psm_set_stream.argtypes = [vp, vp]
     L.psm_set_images.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_u8.argtypes = [vp, u8p, sz, u8p, sz]

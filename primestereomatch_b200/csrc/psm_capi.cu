@@ -75,6 +75,8 @@ struct psm_ctx {
     int gif_win = kBoxK;                    // guided-filter window (GIF_R_WIN) and regulariser (GIF_EPS), psm_set_guided_filter
     float gif_eps = kGifEps;
     bool gif_default() const { return gif_win == kBoxK && gif_eps == kGifEps; }
+    CvcCost cost = {0.9f, INFINITY, INFINITY};   // matching cost (ALPHA_32F, TAU_1_32F, TAU_2_32F), psm_set_matching_cost
+    bool cost_default() const { return cost.alpha == 0.9f && cost.tau_color == INFINITY && cost.tau_grad == INFINITY; }
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -614,6 +616,16 @@ int psm_set_guided_filter(psm_ctx* c, int window, float eps)
     return PSM_OK;
 }
 
+int psm_set_matching_cost(psm_ctx* c, float alpha, float tau_color, float tau_grad)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (!(alpha >= 0.0f && alpha <= 1.0f)) return fail(c, PSM_EINVAL, "matching-cost alpha %g is not in [0, 1]", (double)alpha);
+    if (!(tau_color >= 0.0f)) return fail(c, PSM_EINVAL, "colour threshold %g is not >= 0 or +inf", (double)tau_color);
+    if (!(tau_grad >= 0.0f)) return fail(c, PSM_EINVAL, "gradient threshold %g is not >= 0 or +inf", (double)tau_grad);
+    c->cost = CvcCost{alpha, tau_color, tau_grad};
+    return PSM_OK;
+}
+
 int psm_set_stream(psm_ctx* c, void* cuda_stream)
 {
     if (int rc = bind(c)) return rc;
@@ -703,11 +715,18 @@ int psm_cost_const(psm_ctx* c)
         dim3 blk(128), grd((((c->W + 3) / 4) + 127) / 128, c->H, 2 * nchunks);
         // option 106 (tuning): 0 shipped = interior fast path + scalar window loads; 2 = no fast path (the round-1 loop);
         // 1 / 3 = fast path + grouped 128-bit window loads for the border warps without / with a register cap (DESIGN.md section 10)
-        switch (c->cvc_variant) {
-        case 1: cvc_both_kernel<4, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        case 2: cvc_both_kernel<7, 2><<<grd, blk, 0, c->stream>>>(P2); break;
-        case 3: cvc_both_kernel<5, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        default: cvc_both_kernel<7, 0><<<grd, blk, 0, c->stream>>>(P2); break;
+        // Any matching cost other than the default runs the parameterised build of the shipped variant, all owned slices
+        // per CTA: options 106 and 108 do not apply to it.
+        if (!c->cost_default()) {
+            grd.z = 2;
+            cvc_cost_kernel<<<grd, blk, 0, c->stream>>>(P2, c->cost);
+        } else {
+            switch (c->cvc_variant) {
+            case 1: cvc_both_kernel<4, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+            case 2: cvc_both_kernel<7, 2><<<grd, blk, 0, c->stream>>>(P2); break;
+            case 3: cvc_both_kernel<5, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+            default: cvc_both_kernel<7, 0><<<grd, blk, 0, c->stream>>>(P2); break;
+            }
         }
         PSM_LAUNCH_CHECK(c);
         if (!P2.v[0].fold_halo)  // narrow images: separate halo pass (general reflection)

@@ -99,25 +99,51 @@ struct CvcParams {
     int fold_halo;          // 1: this kernel also writes the mirrored column halo (W >= 32)
 };
 
+// The weighting of the colour and gradient differences.  CostFixed is the reference's compiled ALPHA_32F = 0.9f without
+// truncation (the shipped kernels); CostParam restores the truncation lines CVC.cpp:24-25, 36-37 with run-time alpha and
+// thresholds (psm_set_matching_cost).  Both round every operation separately; (1 - alpha) is one fsub as in CVC.cpp:26.
+struct CostFixed {
+    __device__ __forceinline__ float operator()(float clr, float grd) const
+    {
+        return fadd(fmul(0.9f, clr), fmul(fsub(1.0f, 0.9f), grd));
+    }
+};
+
+struct CvcCost { float alpha, tau_color, tau_grad; };   // psm_set_matching_cost; +inf = no truncation
+
+struct CostParam {
+    float alpha, one_minus_alpha, tau_color, tau_grad;
+    __device__ __forceinline__ explicit CostParam(const CvcCost& k)
+        : alpha(k.alpha), one_minus_alpha(fsub(1.0f, k.alpha)), tau_color(k.tau_color), tau_grad(k.tau_grad) {}
+    __device__ __forceinline__ float operator()(float clr, float grd) const
+    {
+        clr = clr > tau_color ? tau_color : clr;   // a select, not fminf: a NaN difference stays NaN
+        grd = grd > tau_grad ? tau_grad : grd;
+        return fadd(fmul(alpha, clr), fmul(one_minus_alpha, grd));
+    }
+};
+
+template <class Weigh>
 __device__ __forceinline__ float cost4(float l0, float l1, float l2, float lg,
-                                       float r0, float r1, float r2, float rg)
+                                       float r0, float r1, float r2, float rg, const Weigh& weigh)
 {
     const float clr = fadd(fadd(fabsf(fsub(l0, r0)), fabsf(fsub(l1, r1))), fabsf(fsub(l2, r2)));
     const float grd = fabsf(fsub(lg, rg));
-    return fadd(fmul(0.9f, clr), fmul(fsub(1.0f, 0.9f), grd));
+    return weigh(clr, grd);
 }
 
-__device__ __forceinline__ float cost_border(float l0, float l1, float l2, float lg)
+template <class Weigh>
+__device__ __forceinline__ float cost_border(float l0, float l1, float l2, float lg, const Weigh& weigh)
 {
     const double s = __dadd_rn(__dadd_rn(fabs(__dsub_rn((double)l0, 1.0)), fabs(__dsub_rn((double)l1, 1.0))),
                                fabs(__dsub_rn((double)l2, 1.0)));
     const float clr = (float)s;
     const float grd = (float)fabs(__dsub_rn((double)lg, 1.0));
-    return fadd(fmul(0.9f, clr), fmul(fsub(1.0f, 0.9f), grd));
+    return weigh(clr, grd);
 }
 
-template <int SIGN, int GROUPED>
-__device__ __forceinline__ void cvc_body(const CvcParams& P);
+template <int SIGN, int GROUPED, class Weigh>
+__device__ __forceinline__ void cvc_body(const CvcParams& P, const Weigh& weigh);
 
 // both volumes in ONE launch (blockIdx.z = view): twice the CTAs in flight and no tail between the two views.
 // MINB = resident CTAs per SM the register budget is cut for; GROUPED: 0 = shipped (interior fast path + scalar-load window for the
@@ -137,12 +163,23 @@ __global__ void __launch_bounds__(128, MINB) cvc_both_kernel(const CvcParams2 P2
         P.d_begin += first;
         P.d_count = min(P2.chunk, P.d_count - first);
     }
-    if (view == 0) cvc_body<-1, GROUPED>(P);
-    else cvc_body<+1, GROUPED>(P);
+    if (view == 0) cvc_body<-1, GROUPED>(P, CostFixed());
+    else cvc_body<+1, GROUPED>(P, CostFixed());
 }
 
-template <int SIGN, int GROUPED>
-__device__ __forceinline__ void cvc_body(const CvcParams& P)
+// The same K1 at any psm_set_matching_cost setting other than the default: the shipped decomposition (interior fast path,
+// scalar window loads, all owned slices per CTA; tuning options 106 and 108 do not apply), grid z = view.
+__global__ void __launch_bounds__(128, 7) cvc_cost_kernel(const CvcParams2 P2, const CvcCost K)
+{
+    const int view = blockIdx.z & 1;
+    const CvcParams P = P2.v[view];
+    const CostParam weigh(K);
+    if (view == 0) cvc_body<-1, 0>(P, weigh);
+    else cvc_body<+1, 0>(P, weigh);
+}
+
+template <int SIGN, int GROUPED, class Weigh>
+__device__ __forceinline__ void cvc_body(const CvcParams& P, const Weigh& weigh)
 {
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y;
@@ -157,7 +194,7 @@ __device__ __forceinline__ void cvc_body(const CvcParams& P)
         s[c][0] = v.x; s[c][1] = v.y; s[c][2] = v.z; s[c][3] = v.w;
     }
 #pragma unroll
-    for (int j = 0; j < 4; ++j) bord[j] = cost_border(s[0][j], s[1][j], s[2][j], s[3][j]);
+    for (int j = 0; j < 4; ++j) bord[j] = cost_border(s[0][j], s[1][j], s[2][j], s[3][j], weigh);
 
     const float* o0 = P.other[0] + ro;
     const float* o1 = P.other[1] + ro;
@@ -190,7 +227,7 @@ __device__ __forceinline__ void cvc_body(const CvcParams& P)
         for (int j = 0; j < 4; ++j) {
             const int x = x4 + j;
             const bool interior = (SIGN < 0) ? (x >= dd) : (x < W - dd);
-            const float c = cost4(s[0][j], s[1][j], s[2][j], s[3][j], m[0][j], m[1][j], m[2][j], m[3][j]);
+            const float c = cost4(s[0][j], s[1][j], s[2][j], s[3][j], m[0][j], m[1][j], m[2][j], m[3][j], weigh);
             rp[j] = (x < W) ? (interior ? c : bord[j]) : 0.f;
         }
         float* o = out + (size_t)dl * slice;
@@ -224,10 +261,10 @@ __device__ __forceinline__ void cvc_body(const CvcParams& P)
 #pragma unroll 4
             for (int dl = 0; dl < P.d_count; ++dl, ++d, o += slice) {
                 float4 r;
-                r.x = cost4(s[0][0], s[1][0], s[2][0], s[3][0], w[0][0], w[1][0], w[2][0], w[3][0]);
-                r.y = cost4(s[0][1], s[1][1], s[2][1], s[3][1], w[0][1], w[1][1], w[2][1], w[3][1]);
-                r.z = cost4(s[0][2], s[1][2], s[2][2], s[3][2], w[0][2], w[1][2], w[2][2], w[3][2]);
-                r.w = cost4(s[0][3], s[1][3], s[2][3], s[3][3], w[0][3], w[1][3], w[2][3], w[3][3]);
+                r.x = cost4(s[0][0], s[1][0], s[2][0], s[3][0], w[0][0], w[1][0], w[2][0], w[3][0], weigh);
+                r.y = cost4(s[0][1], s[1][1], s[2][1], s[3][1], w[0][1], w[1][1], w[2][1], w[3][1], weigh);
+                r.z = cost4(s[0][2], s[1][2], s[2][2], s[3][2], w[0][2], w[1][2], w[2][2], w[3][2], weigh);
+                r.w = cost4(s[0][3], s[1][3], s[2][3], s[3][3], w[0][3], w[1][3], w[2][3], w[3][3], weigh);
                 __stcs(reinterpret_cast<float4*>(o), r);
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {

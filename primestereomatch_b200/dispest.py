@@ -104,6 +104,15 @@ class DispEst:
         capi.check(self._lib.psm_set_guided_filter(self._ctx, int(window), float(eps)), self._ctx)
         return 0
 
+    def setMatchingCost(self, alpha, tau_color, tau_grad):
+        """Matching-cost weight and truncation thresholds (the reference's compile-time ALPHA_32F, TAU_1_32F and TAU_2_32F,
+        include/CVC.h:18-23, with the truncation of src/CVC.cpp:24-25,36-37 applied) for every later CostConst_GPU call;
+        default (0.9, inf, inf), the reference as shipped.  Raises PsmError unless 0 <= alpha <= 1 and each tau is >= 0 or
+        inf (no truncation)."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_matching_cost(self._ctx, float(alpha), float(tau_color), float(tau_grad)), self._ctx)
+        return 0
+
     def set_option(self, key, value):
         capi.check(self._lib.psm_set_option(self._ctx, int(key), int(value)), self._ctx)
 

@@ -55,6 +55,12 @@ int DispEst::setGuidedFilter(int window, float eps)
     return psm_set_guided_filter(ctx, window, eps);
 }
 
+int DispEst::setMatchingCost(float alpha, float tau_color, float tau_grad)
+{
+    if (!ctx) return -1;
+    return psm_set_matching_cost(ctx, alpha, tau_color, tau_grad);
+}
+
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
 {

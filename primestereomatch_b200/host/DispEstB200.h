@@ -85,6 +85,9 @@ public:
     // guided-filter window and eps (the reference's GIF_R_WIN / GIF_EPS) for the later CostFilter calls; see
     // psm_set_guided_filter.  INTEGRATION.md: call setGuidedFilter(GIF_R_WIN, GIF_EPS) so the GPU mode follows the build.
     int setGuidedFilter(int window, float eps);
+    // matching-cost alpha and truncation thresholds (the reference's ALPHA_32F / TAU_1_32F / TAU_2_32F) for the later
+    // CostConst calls; see psm_set_matching_cost.  INTEGRATION.md: setMatchingCost(ALPHA_32F, INFINITY, INFINITY).
+    int setMatchingCost(float alpha, float tau_color, float tau_grad);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference

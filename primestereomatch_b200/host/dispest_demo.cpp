@@ -1,8 +1,9 @@
 // dispest_demo.cpp -- drives the C++ DispEst facade exactly like StereoMatch::compute does
 // (reference src/StereoMatch.cpp:198-241): setInputImages -> CostConst_GPU -> CostFilter_GPU ->
 // DispSelect_GPU -> PostProcess_GPU.  Raw I/O so it needs no image library:
-//   dispest_demo W H D left.f32 right.f32 out_left.u8 out_right.u8 [window eps]
-// The optional window / eps go to setGuidedFilter (default: the reference's 8 and 0.0001f).
+//   dispest_demo W H D left.f32 right.f32 out_left.u8 out_right.u8 [window eps [alpha tau_color tau_grad]]
+// The optional window / eps go to setGuidedFilter (default: the reference's 8 and 0.0001f), the optional alpha and
+// thresholds to setMatchingCost (default: 0.9 inf inf, i.e. no truncation).
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -20,7 +21,10 @@ static bool read_all(const char* path, void* dst, size_t n)
 
 int main(int argc, char** argv)
 {
-    if (argc != 8 && argc != 10) { std::fprintf(stderr, "usage: %s W H D left.f32 right.f32 outL.u8 outR.u8 [window eps]\n", argv[0]); return 2; }
+    if (argc != 8 && argc != 10 && argc != 13) {
+        std::fprintf(stderr, "usage: %s W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad]]\n", argv[0]);
+        return 2;
+    }
     const int W = std::atoi(argv[1]), H = std::atoi(argv[2]), D = std::atoi(argv[3]);
     if (b200devicepoll() == 0) { std::fprintf(stderr, "no CUDA device\n"); return 3; }
     cv::Mat l(H, W, CV_32FC3), r(H, W, CV_32FC3);
@@ -29,7 +33,9 @@ int main(int argc, char** argv)
     SMDE->setInputImages(l, r);
     SMDE->setThreads(MAX_CPU_THREADS);
     SMDE->setSubsampleRate(4);
-    int rc = argc == 10 ? SMDE->setGuidedFilter(std::atoi(argv[8]), (float)std::atof(argv[9])) : 0;
+    int rc = argc >= 10 ? SMDE->setGuidedFilter(std::atoi(argv[8]), (float)std::atof(argv[9])) : 0;
+    if (!rc && argc == 13)
+        rc = SMDE->setMatchingCost((float)std::atof(argv[10]), (float)std::atof(argv[11]), (float)std::atof(argv[12]));
     if (!rc) rc = SMDE->CostConst_GPU();
     if (!rc) rc = SMDE->CostFilter_GPU();
     if (!rc) rc = SMDE->DispSelect_GPU();
