@@ -131,6 +131,24 @@ int psm_set_guided_filter(psm_ctx* ctx, int window, float eps);
  * their own slices: every rank must set the same values. */
 int psm_set_matching_cost(psm_ctx* ctx, float alpha, float tau_color, float tau_grad);
 
+/* Post-filter weight types: JointWMF::filter's weightType, numbered as in include/JointWMF.h:503-508 ("cos" = 3 and
+ * "jac" = 4 are not functions of the colour difference and are not supported). */
+enum { PSM_WMF_EXP = 0, PSM_WMF_IV1 = 1, PSM_WMF_IV2 = 2, PSM_WMF_OFF = 5 };
+
+/* Post-filter (JointWMF::filter(disp, img8UC3, radius, sigma, 256, 256, iterations, weight_type), the reference's
+ * PP::processDM with MED_SZ = 2 * radius + 1) for every later psm_post_process / psm_post_process_device of this context.
+ * With s = sigma / 256 * 64 and the 6-bit colour difference (d0, d1, d2), in float with the reference's operation order:
+ *   exp: expf(-(float)(d0^2+d1^2+d2^2) * (1 / ((2*s)*s)))    iv1: 1 / ((float)(|d0|+|d1|+|d2|) + s)
+ *   iv2: 1 / ((float)(d0^2+d1^2+d2^2) + s*s)                  off: 1
+ * held as W = lrintf(w / w(0) * 2^22); out(p) = min { v : 2 * sum_{q, I_q <= v} W >= sum_q W } over the (2r+1)^2 window
+ * clipped at the image border, exact integer sums.  Each iteration filters the previous one's output with the original
+ * feature image.  Default (9, 25.5f, 1, PSM_WMF_EXP): the reference as shipped.  Valid: 1 <= radius <= 32, sigma finite
+ * in [2^-16, 2^16], 1 <= iterations <= 16, one of the four weight types; anything else, NaN included, returns PSM_EINVAL
+ * and leaves the context unchanged.  At radius 9, sigma 25.5 and exp every pass runs exactly the tuned kernel pair; any
+ * other setting runs a generic-radius kernel (two launches per pass and view in both cases).  The weight table is cached
+ * on the context and rebuilt after a change of sigma or weight type.  See DESIGN.md section 13. */
+int psm_set_post_filter(psm_ctx* ctx, int radius, float sigma, int iterations, int weight_type);
+
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream. */
 int psm_set_stream(psm_ctx* ctx, void* cuda_stream);

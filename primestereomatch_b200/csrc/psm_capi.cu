@@ -3,6 +3,7 @@
 // compute path exists here: every stage is a CUDA kernel launch or it fails.
 #include "../../include/prime_stereo_b200.h"
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -13,6 +14,7 @@
 #include "psm_cvf_stream.cuh"
 #include "psm_cvf_window.cuh"
 #include "psm_pp.cuh"
+#include "psm_pp_param.cuh"
 #include "psm_fgf.cuh"
 
 #ifndef PSM_BUILD_FLAGS
@@ -54,6 +56,8 @@ struct psm_ctx {
     uint8_t* dis_pp[2] = {nullptr, nullptr}; // post-processed maps
     uint32_t* pp_packed = nullptr;          // packed (disparity, 6-bit colour) image of one view, lazy
     uint32_t* pp_lut = nullptr;             // weight table indexed by squared colour distance, lazy
+    uint32_t* pp_plut = nullptr;            // weight table of the current post-filter setting (generic kernel), lazy
+    bool pp_plut_valid = false;             // pp_plut holds the table of (pp_sigma, pp_type)
     bool have_maps = false;                 // disparity maps valid (a select / reduce stage ran)
     int* guide_flags = nullptr;             // [2] device flags: guide outside the integer-widening domain (see psm_cvf_stream.cuh)
     unsigned char* p2p_own = nullptr;       // own exchange block: keys [2 views][nranks][chunk] u64, maps [2 views][H*W] u8, flag words
@@ -77,6 +81,10 @@ struct psm_ctx {
     bool gif_default() const { return gif_win == kBoxK && gif_eps == kGifEps; }
     CvcCost cost = {0.9f, INFINITY, INFINITY};   // matching cost (ALPHA_32F, TAU_1_32F, TAU_2_32F), psm_set_matching_cost
     bool cost_default() const { return cost.alpha == 0.9f && cost.tau_color == INFINITY && cost.tau_grad == INFINITY; }
+    int pp_radius = kPpRadius;              // post-filter (JointWMF::filter's r, sigma, iter, weightType), psm_set_post_filter
+    float pp_sigma = 25.5f;
+    int pp_iter = 1, pp_type = PSM_WMF_EXP;
+    bool pp_tuned() const { return pp_radius == kPpRadius && pp_sigma == 25.5f && pp_type == PSM_WMF_EXP; }   // any pp_iter
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -537,7 +545,7 @@ int psm_destroy(psm_ctx* c)
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaFree(c->ab);
     cudaFree(c->guide_flags);
-    cudaFree(c->pp_packed); cudaFree(c->pp_lut);
+    cudaFree(c->pp_packed); cudaFree(c->pp_lut); cudaFree(c->pp_plut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
     for (int v = 0; v < 2; ++v) cudaFree(c->dis_pp[v]);
     for (int s = 0; s < kNumStages; ++s) {
@@ -623,6 +631,22 @@ int psm_set_matching_cost(psm_ctx* c, float alpha, float tau_color, float tau_gr
     if (!(tau_color >= 0.0f)) return fail(c, PSM_EINVAL, "colour threshold %g is not >= 0 or +inf", (double)tau_color);
     if (!(tau_grad >= 0.0f)) return fail(c, PSM_EINVAL, "gradient threshold %g is not >= 0 or +inf", (double)tau_grad);
     c->cost = CvcCost{alpha, tau_color, tau_grad};
+    return PSM_OK;
+}
+
+int psm_set_post_filter(psm_ctx* c, int radius, float sigma, int iterations, int weight_type)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (radius < 1 || radius > kPpParamMaxRadius) return fail(c, PSM_EINVAL, "post-filter radius %d outside 1..%d", radius, kPpParamMaxRadius);
+    if (!(sigma >= 0x1p-16f && sigma <= 0x1p16f)) return fail(c, PSM_EINVAL, "post-filter sigma %g outside [2^-16, 2^16]", (double)sigma);
+    if (iterations < 1 || iterations > 16) return fail(c, PSM_EINVAL, "post-filter iterations %d outside 1..16", iterations);
+    if (weight_type != PSM_WMF_EXP && weight_type != PSM_WMF_IV1 && weight_type != PSM_WMF_IV2 && weight_type != PSM_WMF_OFF)
+        return fail(c, PSM_EINVAL, "post-filter weight type %d is not exp (0), iv1 (1), iv2 (2) or off (5)", weight_type);
+    if (sigma != c->pp_sigma || weight_type != c->pp_type) c->pp_plut_valid = false;   // the table depends on both
+    c->pp_radius = radius;
+    c->pp_sigma = sigma;
+    c->pp_iter = iterations;
+    c->pp_type = weight_type;
     return PSM_OK;
 }
 
@@ -1064,6 +1088,31 @@ static const uint8_t* current_map(const psm_ctx* c, int v)
     return c->dis[v];
 }
 
+static int pp_weight_table_size(int type)
+{
+    return type == PSM_WMF_IV1 ? 3 * 63 + 1 : (type == PSM_WMF_OFF ? 1 : kPpMaxD2 + 1);
+}
+
+// The post-filter's 2^-22 fixed-point weight table: JointWMF.h:620-648's float formulas on the 6-bit colour difference
+// (index: squared distance for exp / iv2, L1 distance for iv1, one entry for off), normalised by w(0) so that the centre
+// tap is always 2^22.  Built with -ffp-contract=off.  At (25.5, exp) equal to the default path's table.  -> entries
+static int pp_weight_table(float sigma, int type, uint32_t* t)
+{
+    const float s = sigma / 256.0f * 64;
+    auto w = [&](int k) -> float {
+        switch (type) {
+        case PSM_WMF_EXP: return expf(-(float)k * (1.0f / (2 * s * s)));
+        case PSM_WMF_IV1: return 1.0f / ((float)k + s);
+        case PSM_WMF_IV2: return 1.0f / ((float)k + s * s);
+        default: return 1.0f;
+        }
+    };
+    const float w0 = w(0);
+    const int n = pp_weight_table_size(type);
+    for (int k = 0; k < n; ++k) t[k] = (uint32_t)lrintf((w(k) / w0) * 4194304.0f);
+    return n;
+}
+
 int psm_post_process_device(psm_ctx* c)
 {
     if (int rc = bind(c)) return rc;
@@ -1084,18 +1133,47 @@ int psm_post_process_device(psm_ctx* c)
         PSM_CUDA(c, cudaMalloc(&c->pp_packed, npix * sizeof(uint32_t)));
         for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->dis_pp[v], npix));
     }
+    const bool tuned = c->pp_tuned();
+    const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
+    if (!tuned && !c->pp_plut_valid) {
+        if (!c->pp_plut) {
+            PSM_CUDA(c, cudaMalloc(&c->pp_plut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
+            PSM_CUDA(c, cudaFuncSetAttribute(pp_wmf_param_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        }
+        uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
+        if (!host) return fail(c, PSM_ENOMEM, "out of host memory");
+        const int n = pp_weight_table(c->pp_sigma, c->pp_type, host);
+        // stream-ordered: a previous frame's filter may still be reading the old table
+        cudaError_t e = cudaMemcpyAsync(c->pp_plut, host, n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        delete[] host;
+        PSM_CUDA(c, e);
+        c->pp_plut_valid = true;
+    }
     if (c->p2p_own && c->p2p_seq > 0)
         if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
     int nsm = 0;
     PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
+    const int lut_n = pp_weight_table_size(c->pp_type);
+    const int idx_mode = c->pp_type == PSM_WMF_IV1 ? kIdxL1 : (c->pp_type == PSM_WMF_OFF ? kIdxOne : kIdxSq);
+    const size_t psmem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)lut_n * sizeof(uint32_t);
+    const long pgrid = std::min<long>((long)nsm * 8, ((long)npix + kPpParamWarps - 1) / kPpParamWarps);
     for (int v = 0; v < 2; ++v) {
         const float* g = c->guide[v];
         dim3 blk(256), grd((c->W + 255) / 256, c->H);
-        pp_pack_kernel<<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, current_map(c, v), c->W, c->H, c->pp_packed);
-        PSM_LAUNCH_CHECK(c);
-        pp_wmf_kernel<<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, c->dis_pp[v]);
-        PSM_LAUNCH_CHECK(c);
+        // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output
+        for (int it = 0; it < c->pp_iter; ++it) {
+            const uint8_t* src = it == 0 ? current_map(c, v) : c->dis_pp[v];
+            pp_pack_kernel<<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
+            PSM_LAUNCH_CHECK(c);
+            if (tuned)
+                pp_wmf_kernel<<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, c->dis_pp[v]);
+            else
+                pp_wmf_param_kernel<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_plut, lut_n, idx_mode,
+                                                                                              c->pp_radius, c->W, c->H, c->dis_pp[v]);
+            PSM_LAUNCH_CHECK(c);
+        }
     }
     return stage_end(c, 5);
 }

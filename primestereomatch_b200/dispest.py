@@ -113,6 +113,18 @@ class DispEst:
         capi.check(self._lib.psm_set_matching_cost(self._ctx, float(alpha), float(tau_color), float(tau_grad)), self._ctx)
         return 0
 
+    _WMF_WEIGHTS = {"exp": capi.PSM_WMF_EXP, "iv1": capi.PSM_WMF_IV1, "iv2": capi.PSM_WMF_IV2, "off": capi.PSM_WMF_OFF}
+
+    def setPostFilter(self, radius, sigma=25.5, iterations=1, weight="exp"):
+        """Joint weighted-median post-filter (JointWMF::filter's r, sigma, iter and weightType; the reference's PP::processDM
+        passes MED_SZ/2 = 9 and the defaults) for every later PostProcess_GPU call; default (9, 25.5, 1, "exp").  weight is
+        "exp", "iv1", "iv2" or "off".  Raises PsmError unless 1 <= radius <= 32, 2^-16 <= sigma <= 2^16 and
+        1 <= iterations <= 16, and on any other weight name."""
+        self._need_gpu()
+        wt = self._WMF_WEIGHTS.get(weight, -1) if isinstance(weight, str) else -1
+        capi.check(self._lib.psm_set_post_filter(self._ctx, int(radius), float(sigma), int(iterations), wt), self._ctx)
+        return 0
+
     def set_option(self, key, value):
         capi.check(self._lib.psm_set_option(self._ctx, int(key), int(value)), self._ctx)
 

@@ -61,6 +61,12 @@ int DispEst::setMatchingCost(float alpha, float tau_color, float tau_grad)
     return psm_set_matching_cost(ctx, alpha, tau_color, tau_grad);
 }
 
+int DispEst::setPostFilter(int radius, float sigma, int iterations, int weight_type)
+{
+    if (!ctx) return -1;
+    return psm_set_post_filter(ctx, radius, sigma, iterations, weight_type);
+}
+
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
 {

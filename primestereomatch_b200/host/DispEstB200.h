@@ -88,6 +88,9 @@ public:
     // matching-cost alpha and truncation thresholds (the reference's ALPHA_32F / TAU_1_32F / TAU_2_32F) for the later
     // CostConst calls; see psm_set_matching_cost.  INTEGRATION.md: setMatchingCost(ALPHA_32F, INFINITY, INFINITY).
     int setMatchingCost(float alpha, float tau_color, float tau_grad);
+    // Weighted-median post-filter (JointWMF::filter's r, sigma, iter, weightType: PSM_WMF_*) for every later PostProcess
+    // call; see psm_set_post_filter.  INTEGRATION.md: setPostFilter(MED_SZ/2, 25.5f, 1, PSM_WMF_EXP).
+    int setPostFilter(int radius, float sigma, int iterations, int weight_type);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
