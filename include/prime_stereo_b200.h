@@ -95,13 +95,30 @@ int psm_device_count(void);
 
 /* Create a context for W x H images and disparities [0, max_disp) on CUDA device `device`.
  * Allocates all device state (planar images, gradients, guide planes, both cost volumes,
- * disparity maps).  max_disp <= 256 (u8 disparity maps). */
+ * disparity maps).  max_disp <= 256 (u8 disparity maps; psm_create_u16 for up to 4096). */
 int psm_create(psm_ctx** out, int width, int height, int max_disp, int device);
 
 /* Disparity-sharded context (multi-GPU, one context per GPU): this context owns the global
  * slices [d_begin, d_begin + d_count) of a max_disp-deep problem.  psm_create == shard [0,max_disp). */
 int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp,
                        int d_begin, int d_count, int device);
+
+/* Context with 16-bit disparity maps (uint16_t), for 2 <= max_disp <= 4096, owning the global slices
+ * [d_begin, d_begin + d_count) ([0, max_disp) = unsharded).  Holds at any D, D <= 256 included; geometry is validated
+ * before any CUDA call (PSM_EINVAL), allocation failure returns PSM_ENOMEM.  The map format is fixed at creation:
+ *   - format-neutral calls work on both kinds of context and write maps in the context's format: psm_disp_select_device,
+ *     psm_disp_select_keys, psm_disp_select_keys_p2p, psm_disp_reduce_p2p, psm_post_process_device and every setter;
+ *   - the map calls with host copies have a _u16 twin (psm_disp_select_u16, psm_disp_select_u16_async,
+ *     psm_disp_reduce_keys_u16, psm_disp_fetch_p2p_u16, psm_post_process_u16); a u8 call on a u16 context, or a _u16
+ *     call on a u8 context, returns PSM_EINVAL and names the right call;
+ *   - psm_device_ptr selectors 2-5 return the 16-bit maps (pitch_elems = W);
+ *   - the exchange block of psm_p2p_create_buffer holds 2-byte maps.
+ * The selection is DispSel::CVSelect's arg-min kept as an int: the low byte of a 16-bit map is the reference's uchar map.
+ * The post-filter is the same weighted median on the wider value range (JointWMF::filter on the map as CV_32F with
+ * nI = max_disp).  4096 keeps a 12-bit disparity and the 18 colour bits in one packed u32; memory is the practical limit
+ * below that (four W x H x d_count float volumes: about 35 GB at 1920 x 1080 x 1024).  See DESIGN.md section 14. */
+int psm_create_u16(psm_ctx** out, int width, int height, int max_disp,
+                   int d_begin, int d_count, int device);
 
 int psm_destroy(psm_ctx* ctx);
 
@@ -207,6 +224,13 @@ int psm_disp_select_async(psm_ctx* ctx, uint8_t* left, size_t left_step,
 /* Stage 3 without the D2H copy: maps stay on the device (see psm_device_ptr). Asynchronous. */
 int psm_disp_select_device(psm_ctx* ctx);
 
+/* Stage 3 on a u16 context (psm_create_u16): as psm_disp_select / psm_disp_select_async with uint16_t maps over
+ * d in [1, max_disp); row steps in bytes (at least 2 * W). */
+int psm_disp_select_u16(psm_ctx* ctx, uint16_t* left, size_t left_step,
+                        uint16_t* right, size_t right_step);
+int psm_disp_select_u16_async(psm_ctx* ctx, uint16_t* left, size_t left_step,
+                              uint16_t* right, size_t right_step);
+
 /* Stage 4: post-processing of both maps -- the joint weighted-median filter of PP::processDM (window 19x19,
  * "exp" colour weights on the 6-bit-quantised left / right image, JointWMF defaults), on the device; the
  * reference runs this stage on the CPU even in GPU mode (src/DispEst.cpp:338-344).  Input: the maps of the last
@@ -218,6 +242,8 @@ int psm_disp_select_device(psm_ctx* ctx);
 int psm_post_process(psm_ctx* ctx, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step);
 /* Same without the D2H copy (maps stay on the device: psm_device_ptr selectors 4, 5). Asynchronous. */
 int psm_post_process_device(psm_ctx* ctx);
+/* Stage 4 on a u16 context: as psm_post_process with uint16_t maps (row steps in bytes). */
+int psm_post_process_u16(psm_ctx* ctx, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step);
 
 /* Sharded stage 3a: per-pixel packed minima over this context's slices, written to DEVICE
  * buffers of H*W uint64 each:  key = (order_preserving_u32(cost) << 32) | global_d.
@@ -229,6 +255,10 @@ int psm_disp_select_keys(psm_ctx* ctx, uint64_t* d_keys_left, uint64_t* d_keys_r
 int psm_disp_reduce_keys(psm_ctx* ctx, const uint64_t* d_gathered_left,
                          const uint64_t* d_gathered_right, int nranks,
                          uint8_t* left, size_t left_step, uint8_t* right, size_t right_step);
+/* Same on a u16 context: the low 16 bits of the winning key. */
+int psm_disp_reduce_keys_u16(psm_ctx* ctx, const uint64_t* d_gathered_left,
+                             const uint64_t* d_gathered_right, int nranks,
+                             uint16_t* left, size_t left_step, uint16_t* right, size_t right_step);
 
 /* ---- Sharded stage 3 fused with its exchange over NVLink peer memory ------------------------------
  * Instead of "local WTA kernel, then library collectives", the min-reduction over ranks is done by two
@@ -255,6 +285,7 @@ int psm_p2p_set_peers(psm_ctx* ctx, void* const* d_buffers, int nranks, int rank
 int psm_disp_select_keys_p2p(psm_ctx* ctx);
 int psm_disp_reduce_p2p(psm_ctx* ctx);
 int psm_disp_fetch_p2p(psm_ctx* ctx, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step);
+int psm_disp_fetch_p2p_u16(psm_ctx* ctx, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step);
 
 /* Debug / parity reads (synchronising). `d` is a GLOBAL disparity index owned by this context. */
 int psm_read_cost_slice(psm_ctx* ctx, int view, int d, float* dst, size_t dst_step);
@@ -266,7 +297,8 @@ int psm_read_guide_plane(psm_ctx* ctx, int view, int plane, float* dst, size_t d
 int psm_read_ab_slice(psm_ctx* ctx, int view, int d, float* a3, float* b);
 
 /* Device pointers for zero-copy callers / benchmarks. what: 0 left volume, 1 right volume,
- * 2 left u8 map, 3 right u8 map, 4 / 5 post-processed left / right u8 map.  pitch_elems receives the row pitch in elements. */
+ * 2 left u8 map, 3 right u8 map, 4 / 5 post-processed left / right u8 map (uint16_t maps on a psm_create_u16 context,
+ * pitch_elems = W).  pitch_elems receives the row pitch in elements. */
 int psm_device_ptr(psm_ctx* ctx, int what, void** ptr, size_t* pitch_elems);
 
 /* Last measured stage durations in milliseconds (cudaEvent pairs on the context stream):

@@ -20,7 +20,8 @@ SYMBOLS = [
     "psm_p2p_set_peers", "psm_disp_select_keys_p2p", "psm_disp_reduce_p2p", "psm_disp_fetch_p2p", "psm_read_cost_slice", "psm_write_cost_slice",
     "psm_read_guide_plane", "psm_read_ab_slice", "psm_device_ptr", "psm_stage_ms",
     "psm_launch_count", "psm_sync", "psm_last_error", "psm_build_info", "psm_cvf_plan", "psm_set_guided_filter",
-    "psm_set_matching_cost", "psm_set_post_filter",
+    "psm_set_matching_cost", "psm_set_post_filter", "psm_create_u16", "psm_disp_select_u16", "psm_disp_select_u16_async",
+    "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -53,6 +54,12 @@ def lib():
     L.psm_cvf_plan.argtypes = [i, i, i, i, i, C.POINTER(C.c_int), i]
     L.psm_create.argtypes = [C.POINTER(vp), i, i, i, i]
     L.psm_create_sharded.argtypes = [C.POINTER(vp), i, i, i, i, i, i]
+    L.psm_create_u16.argtypes = [C.POINTER(vp), i, i, i, i, i, i]
+    L.psm_disp_select_u16.argtypes = [vp, vp, sz, vp, sz]
+    L.psm_disp_select_u16_async.argtypes = [vp, vp, sz, vp, sz]
+    L.psm_disp_reduce_keys_u16.argtypes = [vp, vp, vp, i, vp, sz, vp, sz]
+    L.psm_disp_fetch_p2p_u16.argtypes = [vp, vp, sz, vp, sz]
+    L.psm_post_process_u16.argtypes = [vp, vp, sz, vp, sz]
     L.psm_destroy.argtypes = [vp]
     L.psm_set_option.argtypes = [vp, i, i]
     L.psm_set_guided_filter.argtypes = [vp, i, C.c_float]

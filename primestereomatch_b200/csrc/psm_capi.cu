@@ -16,6 +16,7 @@
 #include "psm_pp.cuh"
 #include "psm_pp_param.cuh"
 #include "psm_fgf.cuh"
+#include "psm_wide.cuh"
 
 #ifndef PSM_BUILD_FLAGS
 #define PSM_BUILD_FLAGS "unknown"
@@ -47,13 +48,14 @@ struct psm_ctx {
     bool ingest_done_valid[2] = {false, false};
     int stage_cur = 0;                      // staging set holding the current frame: 0 = stage_in, 1 = stage_alt
     int up_pending = 0;                     // 0 none, 1 f32 upload pending, 2 u8 upload pending
-    uint8_t* dis[2] = {nullptr, nullptr};
+    uint8_t* dis[2] = {nullptr, nullptr};    // disparity maps: u8, or u16 (map_bytes = 2, psm_create_u16) behind the same pointer
+    int map_bytes = 1;                       // bytes per disparity-map element
     // Fast Guided Filter branch (lazy): low-res guide planes per view, low-res coefficient scratch, up-sampling plan
     float* fgf_lo[2] = {nullptr, nullptr};
     float* fgf_mean = nullptr;
     void* fgf_plan = nullptr;               // FgfTap x[W], y[H]: INTER_LINEAR source indices and weights
     int fgf_s = 0;                          // sub-sampling rate the buffers / plan were built for
-    uint8_t* dis_pp[2] = {nullptr, nullptr}; // post-processed maps
+    uint8_t* dis_pp[2] = {nullptr, nullptr}; // post-processed maps (map_bytes per element)
     uint32_t* pp_packed = nullptr;          // packed (disparity, 6-bit colour) image of one view, lazy
     uint32_t* pp_lut = nullptr;             // weight table indexed by squared colour distance, lazy
     uint32_t* pp_plut = nullptr;            // weight table of the current post-filter setting (generic kernel), lazy
@@ -427,6 +429,29 @@ int copy_map_out(psm_ctx* c, const uint8_t* dsrc, uint8_t* dst, size_t step)
     return PSM_OK;
 }
 
+// u16 maps (psm_create_u16): rows of 2 * W bytes
+int copy_map_out16(psm_ctx* c, const uint8_t* dsrc, uint16_t* dst, size_t step)
+{
+    const size_t row = (size_t)c->W * sizeof(uint16_t);
+    if (!dst || step < row) return fail(c, PSM_EINVAL, "bad disparity map pointer/step (u16 maps need a step of at least %zu bytes)", row);
+    PSM_CUDA(c, cudaMemcpy2DAsync(dst, step, dsrc, row, row, c->H, cudaMemcpyDeviceToHost, c->stream));
+    return PSM_OK;
+}
+
+// the map calls of one format on a context of the other: PSM_EINVAL naming the right call
+int check_u8(psm_ctx* c, const char* call, const char* u16_call)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->map_bytes != 1) return fail(c, PSM_EINVAL, "%s on a context with 16-bit maps (psm_create_u16): use %s", call, u16_call);
+    return PSM_OK;
+}
+int check_u16(psm_ctx* c, const char* call, const char* u8_call)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->map_bytes != 2) return fail(c, PSM_EINVAL, "%s on a context with 8-bit maps (psm_create / psm_create_sharded): use %s", call, u8_call);
+    return PSM_OK;
+}
+
 }  // namespace
 
 // ----------------------------------------------------------------------------------------------
@@ -456,14 +481,11 @@ int psm_cvf_plan(int width, int height, int d_count, int sm_count, int no_pack, 
     return PSM_OK;
 }
 
-int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device)
+}  // extern "C"
+
+// geometry already validated by the caller; map_bytes 1 (u8 maps) or 2 (u16 maps)
+static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device, int map_bytes)
 {
-    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
-    *out = nullptr;
-    if (width < 1 || height < 1 || max_disp < 2 || max_disp > 256)
-        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=256)", width, height, max_disp);
-    if (d_begin < 0 || d_count < 1 || d_begin + d_count > max_disp)
-        return fail(nullptr, PSM_EINVAL, "bad shard [%d,%d) of %d", d_begin, d_begin + d_count, max_disp);
     int ndev = psm_device_count();
     if (device < 0 || device >= ndev) return fail(nullptr, PSM_ECUDA, "CUDA device %d not available (%d devices)", device, ndev);
     psm_ctx* c = new (std::nothrow) psm_ctx();
@@ -471,6 +493,7 @@ int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp, int d
     c->W = width; c->H = height; c->Wp = pitch_for_width(width); c->D = max_disp;
     c->d_begin = d_begin; c->d_count = d_count; c->device = device;
     c->plane = (size_t)c->H * c->Wp;
+    c->map_bytes = map_bytes;
     auto bail = [&](int code) {
         snprintf(g_create_error, sizeof(g_create_error), "%s", c->err);
         psm_destroy(c);
@@ -506,8 +529,8 @@ int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp, int d
         PSM_CREATE_CUDA(halo_alloc(&c->vol[v], vol_rows));
         PSM_CREATE_CUDA(halo_alloc(&c->vol_alt[v], vol_rows));
         PSM_CREATE_CUDA(cudaMalloc(&c->stage_in[v], (size_t)c->W * c->H * 3 * sizeof(float)));
-        PSM_CREATE_CUDA(cudaMalloc(&c->dis[v], (size_t)c->W * c->H));
-        PSM_CREATE_CUDA(cudaMemsetAsync(c->dis[v], 0, (size_t)c->W * c->H, c->stream));
+        PSM_CREATE_CUDA(cudaMalloc(&c->dis[v], (size_t)c->W * c->H * map_bytes));
+        PSM_CREATE_CUDA(cudaMemsetAsync(c->dis[v], 0, (size_t)c->W * c->H * map_bytes, c->stream));
     }
     PSM_CREATE_CUDA(cudaMalloc(&c->guide_flags, 2 * sizeof(int)));
     PSM_CREATE_CUDA(cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
@@ -522,6 +545,30 @@ int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp, int d
 #undef PSM_CREATE_CUDA
     *out = c;
     return PSM_OK;
+}
+
+extern "C" {
+
+int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device)
+{
+    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
+    *out = nullptr;
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > 256)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=256)", width, height, max_disp);
+    if (d_begin < 0 || d_count < 1 || d_begin + d_count > max_disp)
+        return fail(nullptr, PSM_EINVAL, "bad shard [%d,%d) of %d", d_begin, d_begin + d_count, max_disp);
+    return create_ctx(out, width, height, max_disp, d_begin, d_count, device, 1);
+}
+
+int psm_create_u16(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device)
+{
+    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
+    *out = nullptr;
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > kWideMaxDisp)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d)", width, height, max_disp, kWideMaxDisp);
+    if (d_begin < 0 || d_count < 1 || d_begin + d_count > max_disp)
+        return fail(nullptr, PSM_EINVAL, "bad shard [%d,%d) of %d", d_begin, d_begin + d_count, max_disp);
+    return create_ctx(out, width, height, max_disp, d_begin, d_count, device, 2);
 }
 
 int psm_create(psm_ctx** out, int width, int height, int max_disp, int device)
@@ -886,7 +933,11 @@ int psm_disp_select_device(psm_ctx* c)
     if (int rc = stage_begin(c, 3)) return rc;
     for (int v = 0; v < 2; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        wta_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, c->dis[v], nullptr);
+        if (c->map_bytes == 2)
+            wta16_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
+                                                     reinterpret_cast<uint16_t*>(c->dis[v]));
+        else
+            wta_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, c->dis[v], nullptr);
         PSM_LAUNCH_CHECK(c);
     }
     c->have_maps = true;
@@ -895,6 +946,7 @@ int psm_disp_select_device(psm_ctx* c)
 
 int psm_disp_select(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
 {
+    if (int rc = check_u8(c, "psm_disp_select", "psm_disp_select_u16")) return rc;
     if (int rc = psm_disp_select_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
     if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
@@ -904,9 +956,28 @@ int psm_disp_select(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right,
 
 int psm_disp_select_async(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
 {
+    if (int rc = check_u8(c, "psm_disp_select_async", "psm_disp_select_u16_async")) return rc;
     if (int rc = psm_disp_select_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
     return copy_map_out(c, c->dis[1], right, right_step);
+}
+
+int psm_disp_select_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    if (int rc = check_u16(c, "psm_disp_select_u16", "psm_disp_select")) return rc;
+    if (int rc = psm_disp_select_device(c)) return rc;
+    if (int rc = copy_map_out16(c, c->dis[0], left, left_step)) return rc;
+    if (int rc = copy_map_out16(c, c->dis[1], right, right_step)) return rc;
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
+}
+
+int psm_disp_select_u16_async(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    if (int rc = check_u16(c, "psm_disp_select_u16_async", "psm_disp_select_async")) return rc;
+    if (int rc = psm_disp_select_device(c)) return rc;
+    if (int rc = copy_map_out16(c, c->dis[0], left, left_step)) return rc;
+    return copy_map_out16(c, c->dis[1], right, right_step);
 }
 
 int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_right)
@@ -928,6 +999,7 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
 int psm_disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
                          uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
 {
+    if (int rc = check_u8(c, "psm_disp_reduce_keys", "psm_disp_reduce_keys_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
     const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
@@ -946,11 +1018,33 @@ int psm_disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint
     return PSM_OK;
 }
 
-// Exchange block of one rank: [2 views][nranks][chunk] uint64 keys, [2 views][H*W] u8 result maps,
+int psm_disp_reduce_keys_u16(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
+                             uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    if (int rc = check_u16(c, "psm_disp_reduce_keys_u16", "psm_disp_reduce_keys")) return rc;
+    if (int rc = bind(c)) return rc;
+    if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
+    const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
+    const size_t npix = (size_t)c->W * c->H;
+    for (int v = 0; v < 2; ++v) {
+        keys_reduce16_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
+            reinterpret_cast<const unsigned long long*>(g[v]), nranks, npix, reinterpret_cast<uint16_t*>(c->dis[v]));
+        PSM_LAUNCH_CHECK(c);
+    }
+    c->have_maps = true;
+    if (left && right) {
+        if (int rc = copy_map_out16(c, c->dis[0], left, left_step)) return rc;
+        if (int rc = copy_map_out16(c, c->dis[1], right, right_step)) return rc;
+    }
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
+}
+
+// Exchange block of one rank: [2 views][nranks][chunk] uint64 keys, [2 views][H*W] result maps (u8, or u16 on a u16 context),
 // [2 views][2 * kMaxRanks] u32 flag words (ARRIVE per rank, DONE per rank), each part 256-byte aligned.
 static size_t p2p_chunk(const psm_ctx* c, int nranks) { return ((size_t)c->W * c->H + nranks - 1) / nranks; }
 static size_t p2p_keys_bytes(const psm_ctx* c, int nranks) { return (size_t)2 * nranks * p2p_chunk(c, nranks) * sizeof(unsigned long long); }
-static size_t p2p_maps_bytes(const psm_ctx* c) { return (((size_t)2 * c->W * c->H) + 255) & ~(size_t)255; }
+static size_t p2p_maps_bytes(const psm_ctx* c) { return (((size_t)2 * c->W * c->H * c->map_bytes) + 255) & ~(size_t)255; }
 static size_t p2p_flags_bytes() { return (size_t)2 * 2 * kMaxRanks * sizeof(unsigned); }
 
 int psm_p2p_create_buffer(psm_ctx* c, int nranks, void** d_buffer)
@@ -1019,7 +1113,7 @@ static void p2p_fill(const psm_ctx* c, int view, P2pPeers& peers)
     for (int r = 0; r < kMaxRanks; ++r) {
         unsigned char* base = r < c->p2p_nranks ? c->p2p_peer[r] : nullptr;
         peers.keys[r] = base ? reinterpret_cast<unsigned long long*>(base) + (size_t)view * c->p2p_nranks * chunk : nullptr;
-        peers.maps[r] = base ? base + kb + (size_t)view * npix : nullptr;
+        peers.maps[r] = base ? base + kb + (size_t)view * npix * c->map_bytes : nullptr;
         peers.flags[r] = base ? reinterpret_cast<unsigned*>(base + kb + mb) + (size_t)view * 2 * kMaxRanks : nullptr;
     }
 }
@@ -1049,7 +1143,8 @@ int psm_disp_reduce_p2p(psm_ctx* c)
     for (int v = 0; v < 2; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
-        chunk_reduce_kernel<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
+        if (c->map_bytes == 2) chunk_reduce16_kernel<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
+        else chunk_reduce_kernel<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
         PSM_LAUNCH_CHECK(c);
     }
     return PSM_OK;
@@ -1070,6 +1165,7 @@ static int p2p_wait_done(psm_ctx* c)
 
 int psm_disp_fetch_p2p(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
 {
+    if (int rc = check_u8(c, "psm_disp_fetch_p2p", "psm_disp_fetch_p2p_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
     if (int rc = p2p_wait_done(c)) return rc;
@@ -1080,11 +1176,24 @@ int psm_disp_fetch_p2p(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* rig
     return PSM_OK;
 }
 
+int psm_disp_fetch_p2p_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    if (int rc = check_u16(c, "psm_disp_fetch_p2p_u16", "psm_disp_fetch_p2p")) return rc;
+    if (int rc = bind(c)) return rc;
+    if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
+    if (int rc = p2p_wait_done(c)) return rc;
+    const unsigned char* maps = c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks);
+    if (int rc = copy_map_out16(c, maps, left, left_step)) return rc;
+    if (int rc = copy_map_out16(c, maps + (size_t)c->W * c->H * 2, right, right_step)) return rc;
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
+}
+
 // ---- post-processing (PP::processDM) ----------------------------------------------------------------
 static const uint8_t* current_map(const psm_ctx* c, int v)
 {
     if (c->p2p_own && c->p2p_seq > 0)   // sharded: the complete maps live in the exchange block
-        return c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks) + (size_t)v * c->W * c->H;
+        return c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks) + (size_t)v * c->W * c->H * c->map_bytes;
     return c->dis[v];
 }
 
@@ -1131,14 +1240,17 @@ int psm_post_process_device(psm_ctx* c)
         delete[] host;
         PSM_CUDA(c, e);
         PSM_CUDA(c, cudaMalloc(&c->pp_packed, npix * sizeof(uint32_t)));
-        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->dis_pp[v], npix));
+        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->dis_pp[v], npix * c->map_bytes));
     }
     const bool tuned = c->pp_tuned();
     const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
     if (!tuned && !c->pp_plut_valid) {
         if (!c->pp_plut) {
             PSM_CUDA(c, cudaMalloc(&c->pp_plut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
-            PSM_CUDA(c, cudaFuncSetAttribute(pp_wmf_param_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            if (c->map_bytes == 2)
+                PSM_CUDA(c, cudaFuncSetAttribute(pp_wmf16_param_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            else
+                PSM_CUDA(c, cudaFuncSetAttribute(pp_wmf_param_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         }
         uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
         if (!host) return fail(c, PSM_ENOMEM, "out of host memory");
@@ -1163,6 +1275,23 @@ int psm_post_process_device(psm_ctx* c)
         const float* g = c->guide[v];
         dim3 blk(256), grd((c->W + 255) / 256, c->H);
         // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output
+        if (c->map_bytes == 2) {   // u16 maps: the wide twins, the same two launches per pass
+            int steps = 0;
+            while ((1 << steps) < c->D) ++steps;   // ceil(log2 max_disp) bisection steps over [0, max_disp - 1]
+            for (int it = 0; it < c->pp_iter; ++it) {
+                const uint16_t* src = reinterpret_cast<const uint16_t*>(it == 0 ? current_map(c, v) : c->dis_pp[v]);
+                uint16_t* dst = reinterpret_cast<uint16_t*>(c->dis_pp[v]);
+                pp_pack16_kernel<<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
+                PSM_LAUNCH_CHECK(c);
+                if (tuned)
+                    pp_wmf16_kernel<<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, c->D, steps, dst);
+                else
+                    pp_wmf16_param_kernel<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_plut, lut_n,
+                                                                                                      idx_mode, c->pp_radius, c->W, c->H, dst);
+                PSM_LAUNCH_CHECK(c);
+            }
+            continue;
+        }
         for (int it = 0; it < c->pp_iter; ++it) {
             const uint8_t* src = it == 0 ? current_map(c, v) : c->dis_pp[v];
             pp_pack_kernel<<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
@@ -1180,9 +1309,20 @@ int psm_post_process_device(psm_ctx* c)
 
 int psm_post_process(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
 {
+    if (int rc = check_u8(c, "psm_post_process", "psm_post_process_u16")) return rc;
     if (int rc = psm_post_process_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis_pp[0], left, left_step)) return rc;
     if (int rc = copy_map_out(c, c->dis_pp[1], right, right_step)) return rc;
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
+}
+
+int psm_post_process_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    if (int rc = check_u16(c, "psm_post_process_u16", "psm_post_process")) return rc;
+    if (int rc = psm_post_process_device(c)) return rc;
+    if (int rc = copy_map_out16(c, c->dis_pp[0], left, left_step)) return rc;
+    if (int rc = copy_map_out16(c, c->dis_pp[1], right, right_step)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }

@@ -33,9 +33,12 @@ class DispEst:
 
     l, r : HxWx3 images, both float32 in [0,1] (CV_32FC3) or both uint8 (CV_8UC3), BGR order.
     d    : maxDis.   t : CPU threads (kept for API compatibility).   ocl : use the GPU path.
+    map_bits : None (8-bit maps for d <= 256, 16-bit above), 8 or 16 (16-bit maps at any d, d <= 4096).  With 16 bits
+    lDisMap / rDisMap are uint16 (CV_16UC1) and the context comes from psm_create_u16; their low byte is the
+    reference's uchar map.
     """
 
-    def __init__(self, l, r, d, t=MAX_CPU_THREADS, ocl=True, device=0, d_begin=0, d_count=None):
+    def __init__(self, l, r, d, t=MAX_CPU_THREADS, ocl=True, device=0, d_begin=0, d_count=None, map_bits=None):
         l, r = np.asarray(l), np.asarray(r)
         if l.dtype != r.dtype or l.shape != r.shape:
             # reference: "DE: Error - Left & Right images are of different types." then exit(1)
@@ -44,11 +47,15 @@ class DispEst:
             raise ValueError("DispEst expects HxWx3 float32 or uint8 images")
         self.hei, self.wid = int(l.shape[0]), int(l.shape[1])
         self.maxDis = int(d)
+        if map_bits not in (None, 8, 16):
+            raise ValueError(f"map_bits must be None, 8 or 16 (got {map_bits!r})")
+        self.map_bits = map_bits if map_bits is not None else (16 if self.maxDis > 256 else 8)
+        mdt = np.uint16 if self.map_bits == 16 else np.uint8
         self.threads = int(t)
         self.useOCL = bool(ocl)
         self.subsample_rate = 4
-        self.lDisMap = np.zeros((self.hei, self.wid), np.uint8)  # DispEst.cpp:46-47
-        self.rDisMap = np.zeros((self.hei, self.wid), np.uint8)
+        self.lDisMap = np.zeros((self.hei, self.wid), mdt)  # DispEst.cpp:46-47
+        self.rDisMap = np.zeros((self.hei, self.wid), mdt)
         self._lImg, self._rImg = l, r
         self._ctx = C.c_void_p()
         self._lib = None
@@ -56,8 +63,8 @@ class DispEst:
             L = capi.lib()
             self._lib = L
             dc = self.maxDis - d_begin if d_count is None else d_count
-            capi.check(L.psm_create_sharded(C.byref(self._ctx), self.wid, self.hei, self.maxDis,
-                                            int(d_begin), int(dc), int(device)))
+            create = L.psm_create_u16 if self.map_bits == 16 else L.psm_create_sharded
+            capi.check(create(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc), int(device)))
         self.d_begin, self.d_count = d_begin, (self.maxDis - d_begin if d_count is None else d_count)
 
     # -- lifetime ---------------------------------------------------------------------------
@@ -162,16 +169,18 @@ class DispEst:
     def DispSelect_GPU(self):
         """DispEst.cpp:323-328: WTA, results land in lDisMap / rDisMap."""
         self._need_gpu()
-        capi.check(self._lib.psm_disp_select(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
-                                             _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
+        sel = self._lib.psm_disp_select_u16 if self.map_bits == 16 else self._lib.psm_disp_select
+        capi.check(sel(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
+                       _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
         return 0
 
     def PostProcess_GPU(self):
         """DispEst.cpp:338-344 -> PP::processDM (PP.cpp:402-425): joint weighted-median filter of both maps; the
         reference runs it on the CPU even in GPU mode, here it is a device stage.  Results replace lDisMap / rDisMap."""
         self._need_gpu()
-        capi.check(self._lib.psm_post_process(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
-                                              _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
+        pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
+        capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
+                      _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
         return 0
 
     def CostConst(self):

@@ -14,10 +14,13 @@ DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl)
         std::printf("DE: Error - Left & Right images are of different types.\n");
         std::exit(1);
     }
-    lDisMap = cv::Mat::zeros(hei, wid, CV_8UC1);
-    rDisMap = cv::Mat::zeros(hei, wid, CV_8UC1);
+    // maxDis > 256: 16-bit maps (psm_create_u16, maxDis <= 4096)
+    const bool wide = maxDis > 256;
+    lDisMap = cv::Mat::zeros(hei, wid, wide ? CV_16UC1 : CV_8UC1);
+    rDisMap = cv::Mat::zeros(hei, wid, wide ? CV_16UC1 : CV_8UC1);
     if (useOCL) {
-        if (psm_create(&ctx, wid, hei, maxDis, 0) != PSM_OK) {
+        const int rc = wide ? psm_create_u16(&ctx, wid, hei, maxDis, 0, maxDis, 0) : psm_create(&ctx, wid, hei, maxDis, 0);
+        if (rc != PSM_OK) {
             // reference logs OpenCL set-up failures and carries on (DispEst.cpp:69-79); so do we, with
             // the GPU stages then returning an error code instead of computing anything on the CPU
             std::fprintf(stderr, "Failed to create the GPU context: %s\n", psm_last_error(nullptr));
@@ -114,6 +117,8 @@ int DispEst::CostFilter_GPU()
 int DispEst::DispSelect_GPU()
 {
     if (!ctx) return -1;
+    if (lDisMap.type() == CV_16UC1)
+        return psm_disp_select_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, rDisMap.ptr<uint16_t>(), rDisMap.step);
     return psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, rDisMap.ptr<uint8_t>(), rDisMap.step);
 }
 
@@ -122,5 +127,7 @@ int DispEst::DispSelect_GPU()
 int DispEst::PostProcess_GPU()
 {
     if (!ctx) return -1;
+    if (lDisMap.type() == CV_16UC1)
+        return psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, rDisMap.ptr<uint16_t>(), rDisMap.step);
     return psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, rDisMap.ptr<uint8_t>(), rDisMap.step);
 }

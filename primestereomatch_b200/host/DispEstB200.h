@@ -26,11 +26,13 @@
 #ifndef PSM_HAVE_OPENCV
 // Minimal stand-in for the handful of cv::Mat members the facade touches.
 #define CV_8U 0
+#define CV_16U 2
 #define CV_32F 5
 #define CV_MAT_DEPTH_MASK 7
 #define CV_MAKETYPE(depth, cn) ((depth) + (((cn)-1) << 3))
 #define CV_8UC1 CV_MAKETYPE(CV_8U, 1)
 #define CV_8UC3 CV_MAKETYPE(CV_8U, 3)
+#define CV_16UC1 CV_MAKETYPE(CV_16U, 1)
 #define CV_32FC1 CV_MAKETYPE(CV_32F, 1)
 #define CV_32FC3 CV_MAKETYPE(CV_32F, 3)
 namespace cv {
@@ -52,7 +54,7 @@ public:
     }
     int type() const { return type_; }
     int channels() const { return (type_ >> 3) + 1; }
-    size_t elemSize() const { return (size_t)channels() * ((type_ & CV_MAT_DEPTH_MASK) == CV_32F ? 4 : 1); }
+    size_t elemSize() const { return (size_t)channels() * ((type_ & CV_MAT_DEPTH_MASK) == CV_32F ? 4 : (type_ & CV_MAT_DEPTH_MASK) == CV_16U ? 2 : 1); }
     bool empty() const { return data == nullptr; }
     template <typename T> T* ptr(int y = 0) { return (T*)(data + step * y); }
     template <typename T> const T* ptr(int y = 0) const { return (const T*)(data + step * y); }
@@ -76,7 +78,8 @@ public:
     DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl);
     ~DispEst(void);
 
-    cv::Mat lDisMap;  // CV_8UC1, raw disparity index (reference DispEst.h:28-29)
+    cv::Mat lDisMap;  // CV_8UC1, raw disparity index (reference DispEst.h:28-29); CV_16UC1 when maxDis > 256 (psm_create_u16),
+                      // whose low byte is the reference's uchar map
     cv::Mat rDisMap;
 
     int setInputImages(cv::Mat l, cv::Mat r);

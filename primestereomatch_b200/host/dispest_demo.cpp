@@ -5,7 +5,8 @@
 //                [radius sigma iterations weight]]]
 // The optional window / eps go to setGuidedFilter (default: the reference's 8 and 0.0001f), the optional alpha and
 // thresholds to setMatchingCost (default: 0.9 inf inf, i.e. no truncation), the optional post-filter radius, sigma,
-// iterations and weight (exp, iv1, iv2 or off) to setPostFilter (default: 9 25.5 1 exp).
+// iterations and weight (exp, iv1, iv2 or off) to setPostFilter (default: 9 25.5 1 exp).  D up to 4096: above 256
+// the maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -52,8 +53,9 @@ int main(int argc, char** argv)
     if (!rc) rc = SMDE->PostProcess_GPU();
     if (rc) { std::fprintf(stderr, "stage failed (%d): %s\n", rc, SMDE->last_error()); return 1; }
     std::printf("CVC %.3f ms  CVF %.3f ms  DispSel %.3f ms  PP %.3f ms\n", SMDE->stage_ms(1), SMDE->stage_ms(2), SMDE->stage_ms(3), SMDE->stage_ms(5));
-    FILE* f = std::fopen(argv[6], "wb"); std::fwrite(SMDE->lDisMap.data, 1, (size_t)W * H, f); std::fclose(f);
-    f = std::fopen(argv[7], "wb"); std::fwrite(SMDE->rDisMap.data, 1, (size_t)W * H, f); std::fclose(f);
+    const size_t bytes = SMDE->lDisMap.step * H;   // dense rows: W * 1 or W * 2 bytes
+    FILE* f = std::fopen(argv[6], "wb"); std::fwrite(SMDE->lDisMap.data, 1, bytes, f); std::fclose(f);
+    f = std::fopen(argv[7], "wb"); std::fwrite(SMDE->rDisMap.data, 1, bytes, f); std::fclose(f);
     delete SMDE;
     return 0;
 }

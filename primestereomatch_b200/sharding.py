@@ -38,10 +38,15 @@ def bind_to_current_stream(de):
     capi.check(capi.lib().psm_set_stream(de.handle, C.c_void_p(h if h else 1)), de.handle)
 
 
+def _wide(de):
+    """the context has 16-bit maps (DispEst(..., map_bits=16) or maxDis > 256)"""
+    return getattr(de, "map_bits", 8) == 16
+
+
 def gather_and_reduce(de, keys, gathered, world, lmap=None, rmap=None, group=None):
     """Library baseline of the exchange.  keys: int64 CUDA tensor [2, H*W] (this rank's packed minima, written by
     psm_disp_select_keys); gathered: int64 CUDA tensor [2, world, H*W].  One all-gather per view, then the final
-    min -> u8 maps (optionally copied to host arrays).  The context is bound to torch's current stream first:
+    min -> maps (u8, or u16 when de.map_bits == 16; optionally copied to host arrays).  The context is bound to torch's current stream first:
     the all-gathers must not overtake the select kernels."""
     import torch.distributed as dist
     L = capi.lib()
@@ -51,8 +56,9 @@ def gather_and_reduce(de, keys, gathered, world, lmap=None, rmap=None, group=Non
     dist.all_gather_into_tensor(gathered[1].view(-1), keys[1], group=group)
     lp = lmap.ctypes.data_as(C.c_void_p) if lmap is not None else None
     rp = rmap.ctypes.data_as(C.c_void_p) if rmap is not None else None
-    capi.check(L.psm_disp_reduce_keys(de.handle, gathered[0].data_ptr(), gathered[1].data_ptr(), world,
-                                      lp, de.wid, rp, de.wid), de.handle)
+    reduce = L.psm_disp_reduce_keys_u16 if _wide(de) else L.psm_disp_reduce_keys
+    step = de.wid * (2 if _wide(de) else 1)
+    capi.check(reduce(de.handle, gathered[0].data_ptr(), gathered[1].data_ptr(), world, lp, step, rp, step), de.handle)
 
 
 class P2PExchange:
@@ -102,8 +108,13 @@ class P2PExchange:
         capi.check(capi.lib().psm_disp_reduce_p2p(self.de.handle), self.de.handle)
 
     def fetch(self, lmap_ptr, rmap_ptr):
-        capi.check(capi.lib().psm_disp_fetch_p2p(self.de.handle, lmap_ptr, self.de.wid, rmap_ptr, self.de.wid),
-                   self.de.handle)
+        """host maps of the context's format: uint8, or uint16 on a 16-bit context (rows of W elements)"""
+        L = capi.lib()
+        if _wide(self.de):
+            capi.check(L.psm_disp_fetch_p2p_u16(self.de.handle, lmap_ptr, 2 * self.de.wid, rmap_ptr, 2 * self.de.wid),
+                       self.de.handle)
+        else:
+            capi.check(L.psm_disp_fetch_p2p(self.de.handle, lmap_ptr, self.de.wid, rmap_ptr, self.de.wid), self.de.handle)
 
     def frame(self, lmap_ptr=None, rmap_ptr=None):
         """select -> reduce [-> fetch]; with device_sync=False a barrier follows select and reduce."""
