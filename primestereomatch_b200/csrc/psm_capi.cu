@@ -16,7 +16,6 @@
 #include "psm_pp.cuh"
 #include "psm_pp_param.cuh"
 #include "psm_fgf.cuh"
-#include "psm_wide.cuh"
 
 #ifndef PSM_BUILD_FLAGS
 #define PSM_BUILD_FLAGS "unknown"
@@ -422,34 +421,26 @@ int launch_cvf_window(psm_ctx* c)
     return PSM_OK;
 }
 
-int copy_map_out(psm_ctx* c, const uint8_t* dsrc, uint8_t* dst, size_t step)
+// device map -> host rows of W elements of the context's map format
+int copy_map_out(psm_ctx* c, const uint8_t* dsrc, void* dst, size_t step)
 {
-    if (!dst || step < (size_t)c->W) return fail(c, PSM_EINVAL, "bad disparity map pointer/step");
-    PSM_CUDA(c, cudaMemcpy2DAsync(dst, step, dsrc, c->W, c->W, c->H, cudaMemcpyDeviceToHost, c->stream));
-    return PSM_OK;
-}
-
-// u16 maps (psm_create_u16): rows of 2 * W bytes
-int copy_map_out16(psm_ctx* c, const uint8_t* dsrc, uint16_t* dst, size_t step)
-{
-    const size_t row = (size_t)c->W * sizeof(uint16_t);
-    if (!dst || step < row) return fail(c, PSM_EINVAL, "bad disparity map pointer/step (u16 maps need a step of at least %zu bytes)", row);
+    const size_t row = (size_t)c->W * c->map_bytes;
+    if (!dst || step < row)
+        return c->map_bytes == 1 ? fail(c, PSM_EINVAL, "bad disparity map pointer/step")
+                                 : fail(c, PSM_EINVAL, "bad disparity map pointer/step (u16 maps need a step of at least %zu bytes)", row);
     PSM_CUDA(c, cudaMemcpy2DAsync(dst, step, dsrc, row, row, c->H, cudaMemcpyDeviceToHost, c->stream));
     return PSM_OK;
 }
 
-// the map calls of one format on a context of the other: PSM_EINVAL naming the right call
-int check_u8(psm_ctx* c, const char* call, const char* u16_call)
+// a map call for maps of type T, named u8_call / u16_call in its two formats, on a context of the other format:
+// PSM_EINVAL naming the right call
+template <typename T>
+int check_map_format(psm_ctx* c, const char* u8_call, const char* u16_call)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (c->map_bytes != 1) return fail(c, PSM_EINVAL, "%s on a context with 16-bit maps (psm_create_u16): use %s", call, u16_call);
-    return PSM_OK;
-}
-int check_u16(psm_ctx* c, const char* call, const char* u8_call)
-{
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (c->map_bytes != 2) return fail(c, PSM_EINVAL, "%s on a context with 8-bit maps (psm_create / psm_create_sharded): use %s", call, u8_call);
-    return PSM_OK;
+    if (c->map_bytes == (int)sizeof(T)) return PSM_OK;
+    if (sizeof(T) == 1) return fail(c, PSM_EINVAL, "%s on a context with 16-bit maps (psm_create_u16): use %s", u8_call, u16_call);
+    return fail(c, PSM_EINVAL, "%s on a context with 8-bit maps (psm_create / psm_create_sharded): use %s", u16_call, u8_call);
 }
 
 }  // namespace
@@ -553,8 +544,9 @@ int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp, int d
 {
     if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
     *out = nullptr;
-    if (width < 1 || height < 1 || max_disp < 2 || max_disp > 256)
-        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=256)", width, height, max_disp);
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > MapFormat<uint8_t>::kMaxDisp)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d)", width, height, max_disp,
+                    MapFormat<uint8_t>::kMaxDisp);
     if (d_begin < 0 || d_count < 1 || d_begin + d_count > max_disp)
         return fail(nullptr, PSM_EINVAL, "bad shard [%d,%d) of %d", d_begin, d_begin + d_count, max_disp);
     return create_ctx(out, width, height, max_disp, d_begin, d_count, device, 1);
@@ -564,8 +556,9 @@ int psm_create_u16(psm_ctx** out, int width, int height, int max_disp, int d_beg
 {
     if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
     *out = nullptr;
-    if (width < 1 || height < 1 || max_disp < 2 || max_disp > kWideMaxDisp)
-        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d)", width, height, max_disp, kWideMaxDisp);
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > MapFormat<uint16_t>::kMaxDisp)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d)", width, height, max_disp,
+                    MapFormat<uint16_t>::kMaxDisp);
     if (d_begin < 0 || d_count < 1 || d_begin + d_count > max_disp)
         return fail(nullptr, PSM_EINVAL, "bad shard [%d,%d) of %d", d_begin, d_begin + d_count, max_disp);
     return create_ctx(out, width, height, max_disp, d_begin, d_count, device, 2);
@@ -924,89 +917,46 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
     return stage_end(c, 2);
 }
 
-int psm_disp_select_device(psm_ctx* c)
+}  // extern "C"
+
+// the WTA of both views into the context's maps of type T
+template <typename T>
+static int select_maps(psm_ctx* c)
 {
-    if (int rc = bind(c)) return rc;
-    if (c->d_begin != 0 || c->d_count != c->D)
-        return fail(c, PSM_ESTATE, "psm_disp_select on a sharded context: use psm_disp_select_keys + psm_disp_reduce_keys");
-    if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select before psm_cost_filter");
-    if (int rc = stage_begin(c, 3)) return rc;
     for (int v = 0; v < 2; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        if (c->map_bytes == 2)
-            wta16_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
-                                                     reinterpret_cast<uint16_t*>(c->dis[v]));
-        else
-            wta_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, c->dis[v], nullptr);
+        wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
+                                                  reinterpret_cast<T*>(c->dis[v]), nullptr);
         PSM_LAUNCH_CHECK(c);
     }
-    c->have_maps = true;
-    return stage_end(c, 3);
+    return PSM_OK;
 }
 
-int psm_disp_select(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+// psm_disp_select[_u16][_async]: select on the device, copy both maps to the host, then wait for them unless async
+template <typename T>
+static int disp_select(psm_ctx* c, T* left, size_t left_step, T* right, size_t right_step, bool sync)
 {
-    if (int rc = check_u8(c, "psm_disp_select", "psm_disp_select_u16")) return rc;
+    if (int rc = sync ? check_map_format<T>(c, "psm_disp_select", "psm_disp_select_u16")
+                      : check_map_format<T>(c, "psm_disp_select_async", "psm_disp_select_u16_async")) return rc;
     if (int rc = psm_disp_select_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
     if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (sync) PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }
 
-int psm_disp_select_async(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+template <typename T>
+static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
+                            T* left, size_t left_step, T* right, size_t right_step)
 {
-    if (int rc = check_u8(c, "psm_disp_select_async", "psm_disp_select_u16_async")) return rc;
-    if (int rc = psm_disp_select_device(c)) return rc;
-    if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
-    return copy_map_out(c, c->dis[1], right, right_step);
-}
-
-int psm_disp_select_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
-{
-    if (int rc = check_u16(c, "psm_disp_select_u16", "psm_disp_select")) return rc;
-    if (int rc = psm_disp_select_device(c)) return rc;
-    if (int rc = copy_map_out16(c, c->dis[0], left, left_step)) return rc;
-    if (int rc = copy_map_out16(c, c->dis[1], right, right_step)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
-}
-
-int psm_disp_select_u16_async(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
-{
-    if (int rc = check_u16(c, "psm_disp_select_u16_async", "psm_disp_select_async")) return rc;
-    if (int rc = psm_disp_select_device(c)) return rc;
-    if (int rc = copy_map_out16(c, c->dis[0], left, left_step)) return rc;
-    return copy_map_out16(c, c->dis[1], right, right_step);
-}
-
-int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_right)
-{
-    if (int rc = bind(c)) return rc;
-    if (!d_keys_left || !d_keys_right) return fail(c, PSM_EINVAL, "null key buffer");
-    if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
-    if (int rc = stage_begin(c, 3)) return rc;
-    uint64_t* keys[2] = {d_keys_left, d_keys_right};
-    for (int v = 0; v < 2; ++v) {
-        dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        wta_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, nullptr,
-                                               reinterpret_cast<unsigned long long*>(keys[v]));
-        PSM_LAUNCH_CHECK(c);
-    }
-    return stage_end(c, 3);
-}
-
-int psm_disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
-                         uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
-{
-    if (int rc = check_u8(c, "psm_disp_reduce_keys", "psm_disp_reduce_keys_u16")) return rc;
+    if (int rc = check_map_format<T>(c, "psm_disp_reduce_keys", "psm_disp_reduce_keys_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
     const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
     const size_t npix = (size_t)c->W * c->H;
     for (int v = 0; v < 2; ++v) {
-        keys_reduce_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
-            reinterpret_cast<const unsigned long long*>(g[v]), nranks, npix, c->dis[v]);
+        keys_reduce_kernel<T><<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
+            reinterpret_cast<const unsigned long long*>(g[v]), nranks, npix, reinterpret_cast<T*>(c->dis[v]));
         PSM_LAUNCH_CHECK(c);
     }
     c->have_maps = true;
@@ -1018,26 +968,66 @@ int psm_disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint
     return PSM_OK;
 }
 
+extern "C" {
+
+int psm_disp_select_device(psm_ctx* c)
+{
+    if (int rc = bind(c)) return rc;
+    if (c->d_begin != 0 || c->d_count != c->D)
+        return fail(c, PSM_ESTATE, "psm_disp_select on a sharded context: use psm_disp_select_keys + psm_disp_reduce_keys");
+    if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select before psm_cost_filter");
+    if (int rc = stage_begin(c, 3)) return rc;
+    if (int rc = c->map_bytes == 2 ? select_maps<uint16_t>(c) : select_maps<uint8_t>(c)) return rc;
+    c->have_maps = true;
+    return stage_end(c, 3);
+}
+
+int psm_disp_select(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+{
+    return disp_select(c, left, left_step, right, right_step, true);
+}
+
+int psm_disp_select_async(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+{
+    return disp_select(c, left, left_step, right, right_step, false);
+}
+
+int psm_disp_select_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    return disp_select(c, left, left_step, right, right_step, true);
+}
+
+int psm_disp_select_u16_async(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
+{
+    return disp_select(c, left, left_step, right, right_step, false);
+}
+
+int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_right)
+{
+    if (int rc = bind(c)) return rc;
+    if (!d_keys_left || !d_keys_right) return fail(c, PSM_EINVAL, "null key buffer");
+    if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
+    if (int rc = stage_begin(c, 3)) return rc;
+    uint64_t* keys[2] = {d_keys_left, d_keys_right};
+    for (int v = 0; v < 2; ++v) {   // keys only, on either map format
+        dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
+        wta_kernel<uint8_t><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, nullptr,
+                                                        reinterpret_cast<unsigned long long*>(keys[v]));
+        PSM_LAUNCH_CHECK(c);
+    }
+    return stage_end(c, 3);
+}
+
+int psm_disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
+                         uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+{
+    return disp_reduce_keys(c, d_gathered_left, d_gathered_right, nranks, left, left_step, right, right_step);
+}
+
 int psm_disp_reduce_keys_u16(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
                              uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
 {
-    if (int rc = check_u16(c, "psm_disp_reduce_keys_u16", "psm_disp_reduce_keys")) return rc;
-    if (int rc = bind(c)) return rc;
-    if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
-    const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
-    const size_t npix = (size_t)c->W * c->H;
-    for (int v = 0; v < 2; ++v) {
-        keys_reduce16_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
-            reinterpret_cast<const unsigned long long*>(g[v]), nranks, npix, reinterpret_cast<uint16_t*>(c->dis[v]));
-        PSM_LAUNCH_CHECK(c);
-    }
-    c->have_maps = true;
-    if (left && right) {
-        if (int rc = copy_map_out16(c, c->dis[0], left, left_step)) return rc;
-        if (int rc = copy_map_out16(c, c->dis[1], right, right_step)) return rc;
-    }
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    return disp_reduce_keys(c, d_gathered_left, d_gathered_right, nranks, left, left_step, right, right_step);
 }
 
 // Exchange block of one rank: [2 views][nranks][chunk] uint64 keys, [2 views][H*W] result maps (u8, or u16 on a u16 context),
@@ -1140,11 +1130,11 @@ int psm_disp_reduce_p2p(psm_ctx* c)
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "no exchange block");
     const unsigned npix = (unsigned)((size_t)c->W * c->H);
+    const auto reduce = c->map_bytes == 2 ? chunk_reduce_kernel<uint16_t> : chunk_reduce_kernel<uint8_t>;
     for (int v = 0; v < 2; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
-        if (c->map_bytes == 2) chunk_reduce16_kernel<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
-        else chunk_reduce_kernel<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
+        reduce<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
         PSM_LAUNCH_CHECK(c);
     }
     return PSM_OK;
@@ -1163,30 +1153,32 @@ static int p2p_wait_done(psm_ctx* c)
     return PSM_OK;
 }
 
-int psm_disp_fetch_p2p(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+}  // extern "C"
+
+template <typename T>
+static int disp_fetch_p2p(psm_ctx* c, T* left, size_t left_step, T* right, size_t right_step)
 {
-    if (int rc = check_u8(c, "psm_disp_fetch_p2p", "psm_disp_fetch_p2p_u16")) return rc;
+    if (int rc = check_map_format<T>(c, "psm_disp_fetch_p2p", "psm_disp_fetch_p2p_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
     if (int rc = p2p_wait_done(c)) return rc;
     const unsigned char* maps = c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks);
     if (int rc = copy_map_out(c, maps, left, left_step)) return rc;
-    if (int rc = copy_map_out(c, maps + (size_t)c->W * c->H, right, right_step)) return rc;
+    if (int rc = copy_map_out(c, maps + (size_t)c->W * c->H * sizeof(T), right, right_step)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }
 
+extern "C" {
+
+int psm_disp_fetch_p2p(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+{
+    return disp_fetch_p2p(c, left, left_step, right, right_step);
+}
+
 int psm_disp_fetch_p2p_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
 {
-    if (int rc = check_u16(c, "psm_disp_fetch_p2p_u16", "psm_disp_fetch_p2p")) return rc;
-    if (int rc = bind(c)) return rc;
-    if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
-    if (int rc = p2p_wait_done(c)) return rc;
-    const unsigned char* maps = c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks);
-    if (int rc = copy_map_out16(c, maps, left, left_step)) return rc;
-    if (int rc = copy_map_out16(c, maps + (size_t)c->W * c->H * 2, right, right_step)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    return disp_fetch_p2p(c, left, left_step, right, right_step);
 }
 
 // ---- post-processing (PP::processDM) ----------------------------------------------------------------
@@ -1222,9 +1214,16 @@ static int pp_weight_table(float sigma, int type, uint32_t* t)
     return n;
 }
 
-int psm_post_process_device(psm_ctx* c)
+}  // extern "C"
+
+// the post-filter stage on maps of type T
+template <typename T>
+static int post_process_maps(psm_ctx* c)
 {
-    if (int rc = bind(c)) return rc;
+    // the generic kernel: one histogram level over the 256 values of u8 maps, two levels on u16 maps
+    const auto generic = [] {
+        if constexpr (sizeof(T) == 1) return pp_wmf_param_kernel; else return pp_wmf_param_two_level_kernel;
+    }();
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_post_process before psm_set_images");
     if (!c->have_maps && !(c->p2p_own && c->p2p_seq > 0)) return fail(c, PSM_ESTATE, "psm_post_process before a disparity-selection stage");
     const size_t npix = (size_t)c->W * c->H;
@@ -1247,10 +1246,7 @@ int psm_post_process_device(psm_ctx* c)
     if (!tuned && !c->pp_plut_valid) {
         if (!c->pp_plut) {
             PSM_CUDA(c, cudaMalloc(&c->pp_plut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
-            if (c->map_bytes == 2)
-                PSM_CUDA(c, cudaFuncSetAttribute(pp_wmf16_param_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            else
-                PSM_CUDA(c, cudaFuncSetAttribute(pp_wmf_param_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         }
         uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
         if (!host) return fail(c, PSM_ENOMEM, "out of host memory");
@@ -1271,45 +1267,33 @@ int psm_post_process_device(psm_ctx* c)
     const int idx_mode = c->pp_type == PSM_WMF_IV1 ? kIdxL1 : (c->pp_type == PSM_WMF_OFF ? kIdxOne : kIdxSq);
     const size_t psmem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)lut_n * sizeof(uint32_t);
     const long pgrid = std::min<long>((long)nsm * 8, ((long)npix + kPpParamWarps - 1) / kPpParamWarps);
+    int steps = 0;
+    while ((1 << steps) < c->D) ++steps;   // u16 maps: ceil(log2 max_disp) bisection steps over [0, max_disp - 1]
     for (int v = 0; v < 2; ++v) {
         const float* g = c->guide[v];
+        T* dst = reinterpret_cast<T*>(c->dis_pp[v]);
         dim3 blk(256), grd((c->W + 255) / 256, c->H);
         // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output
-        if (c->map_bytes == 2) {   // u16 maps: the wide twins, the same two launches per pass
-            int steps = 0;
-            while ((1 << steps) < c->D) ++steps;   // ceil(log2 max_disp) bisection steps over [0, max_disp - 1]
-            for (int it = 0; it < c->pp_iter; ++it) {
-                const uint16_t* src = reinterpret_cast<const uint16_t*>(it == 0 ? current_map(c, v) : c->dis_pp[v]);
-                uint16_t* dst = reinterpret_cast<uint16_t*>(c->dis_pp[v]);
-                pp_pack16_kernel<<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
-                PSM_LAUNCH_CHECK(c);
-                if (tuned)
-                    pp_wmf16_kernel<<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, c->D, steps, dst);
-                else
-                    pp_wmf16_param_kernel<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_plut, lut_n,
-                                                                                                      idx_mode, c->pp_radius, c->W, c->H, dst);
-                PSM_LAUNCH_CHECK(c);
-            }
-            continue;
-        }
         for (int it = 0; it < c->pp_iter; ++it) {
-            const uint8_t* src = it == 0 ? current_map(c, v) : c->dis_pp[v];
-            pp_pack_kernel<<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
+            const T* src = reinterpret_cast<const T*>(it == 0 ? current_map(c, v) : c->dis_pp[v]);
+            pp_pack_kernel<T><<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
             PSM_LAUNCH_CHECK(c);
             if (tuned)
-                pp_wmf_kernel<<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, c->dis_pp[v]);
+                pp_wmf_kernel<T><<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, dst, c->D, steps);
             else
-                pp_wmf_param_kernel<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_plut, lut_n, idx_mode,
-                                                                                              c->pp_radius, c->W, c->H, c->dis_pp[v]);
+                generic<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_plut, lut_n, idx_mode,
+                                                                                    c->pp_radius, c->W, c->H, dst);
             PSM_LAUNCH_CHECK(c);
         }
     }
     return stage_end(c, 5);
 }
 
-int psm_post_process(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+// psm_post_process[_u16]: the post-filter on the device, then both maps to the host
+template <typename T>
+static int post_process(psm_ctx* c, T* left, size_t left_step, T* right, size_t right_step)
 {
-    if (int rc = check_u8(c, "psm_post_process", "psm_post_process_u16")) return rc;
+    if (int rc = check_map_format<T>(c, "psm_post_process", "psm_post_process_u16")) return rc;
     if (int rc = psm_post_process_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis_pp[0], left, left_step)) return rc;
     if (int rc = copy_map_out(c, c->dis_pp[1], right, right_step)) return rc;
@@ -1317,14 +1301,22 @@ int psm_post_process(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right
     return PSM_OK;
 }
 
+extern "C" {
+
+int psm_post_process_device(psm_ctx* c)
+{
+    if (int rc = bind(c)) return rc;
+    return c->map_bytes == 2 ? post_process_maps<uint16_t>(c) : post_process_maps<uint8_t>(c);
+}
+
+int psm_post_process(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
+{
+    return post_process(c, left, left_step, right, right_step);
+}
+
 int psm_post_process_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
 {
-    if (int rc = check_u16(c, "psm_post_process_u16", "psm_post_process")) return rc;
-    if (int rc = psm_post_process_device(c)) return rc;
-    if (int rc = copy_map_out16(c, c->dis_pp[0], left, left_step)) return rc;
-    if (int rc = copy_map_out16(c, c->dis_pp[1], right, right_step)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    return post_process(c, left, left_step, right, right_step);
 }
 
 static int check_slice(psm_ctx* c, int view, int d)

@@ -14,6 +14,22 @@ constexpr int kBoxK = 8;        // GIF_R_WIN, reference include/ComFunc.h:49 (8x
 constexpr int kBoxAnchor = 4;   // cv::boxFilter default anchor = ksize/2
 constexpr float kGifEps = 0.0001f;  // GIF_EPS, include/ComFunc.h:50
 
+// The two disparity-map formats, by element type: uint8_t maps (psm_create, D <= 256) and uint16_t maps
+// (psm_create_u16, D <= 4096).  The post-filter packs a map value and the three 6-bit colours of its pixel into one u32,
+//   d << kDispShift | R6 << 2 * kColourBits | G6 << kColourBits | B6,
+// and its bisection gives the taps outside the window the disparity kSentinel, above every map value.
+template <typename T> struct MapFormat;
+template <> struct MapFormat<uint8_t> {
+    static constexpr int kMaxDisp = 256;
+    static constexpr int kDispShift = 24, kColourBits = 8;
+    static constexpr uint32_t kSentinel = 256u;
+};
+template <> struct MapFormat<uint16_t> {
+    static constexpr int kMaxDisp = 4096;   // a 12-bit disparity and 18 colour bits fill the packed u32
+    static constexpr int kDispShift = 18, kColourBits = 6;
+    static constexpr uint32_t kSentinel = 0xffffffffu;
+};
+
 __device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ float fsub(float a, float b) { return __fsub_rn(a, b); }

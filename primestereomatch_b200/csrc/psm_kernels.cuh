@@ -599,10 +599,11 @@ __global__ void cvf_naive_q_kernel(const float* __restrict__ ab, const float* __
 // ------------------------------------------------------------------------------------------
 // K4 WTA (DispSel.cpp:83-109): per pixel argmin over global d in [1, D), strict <, ties -> lowest d,
 // minCost starts at +inf, result 0 when nothing compares below +inf.  One thread = 4 pixels.
-// Emits the u8 map and/or the packed (cost,d) key used by the disparity-sharded reduction.
+// Emits the map (T = uint8_t or uint16_t) and/or the packed (cost,d) key used by the disparity-sharded reduction.
 // ------------------------------------------------------------------------------------------
+template <typename T>
 __global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin, int d_count,
-                                                  uint8_t* __restrict__ dis /* [H][W] or null */,
+                                                  T* __restrict__ dis /* [H][W] or null */,
                                                   unsigned long long* __restrict__ keys /* [H][W] or null */)
 {
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
@@ -626,7 +627,7 @@ __global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol,
     for (int j = 0; j < 4; ++j) {
         const int x = x4 + j;
         if (x < W) {
-            if (dis) dis[(size_t)y * W + x] = (uint8_t)md[j];
+            if (dis) dis[(size_t)y * W + x] = (T)md[j];
             if (keys) keys[(size_t)y * W + x] = ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j];
         }
     }
@@ -640,7 +641,7 @@ __global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol,
 //                        (peer device memory, plain st.global over NVLink) -- compute + scatter in one kernel;
 //                        its last CTA then raises this rank's ARRIVE flag in every peer's block;
 //   chunk_reduce_kernel: waits for the ARRIVE flags of all ranks (acquire loads on its own block), takes
-//                        the min over the nranks slots of its chunk, stores the winning disparity (u8)
+//                        the min over the nranks slots of its chunk, stores the winning disparity (u8 or u16)
 //                        into EVERY rank's result map -- reduce + gather in one kernel -- and its last CTA
 //                        raises this rank's DONE flag in every peer's block;
 //   p2p_wait_done_kernel: spins until all ranks' DONE flags carry this frame's sequence number; after it the local result
@@ -654,7 +655,7 @@ constexpr int kScatterRows = 4;   // image rows per CTA of wta_scatter_kernel
 
 struct P2pPeers {
     unsigned long long* keys[kMaxRanks];  // per rank: exchange block of this view  [nranks][chunk]
-    unsigned char* maps[kMaxRanks];       // per rank: result map of this view       [H*W]
+    unsigned char* maps[kMaxRanks];       // per rank: result map of this view       [H*W] of the map type
     unsigned* flags[kMaxRanks];           // per rank: flag words of this view: arrive[kMaxRanks], done[kMaxRanks]
     unsigned* counter;                    // device-local CTA counter of the launching rank (zero between launches)
     int nranks, rank;
@@ -740,6 +741,7 @@ __global__ void __launch_bounds__(256) wta_scatter_kernel(const float* __restric
     if (peers.seq) p2p_publish(peers, 0);   // ARRIVE
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256) chunk_reduce_kernel(P2pPeers peers, unsigned npix)
 {
     if (peers.seq) {   // wait until every rank's minima for this frame have landed in this rank's block
@@ -758,8 +760,8 @@ __global__ void __launch_bounds__(256) chunk_reduce_kernel(P2pPeers peers, unsig
             const unsigned long long v = __ldcg(mine + (size_t)r * peers.chunk + i);
             k = v < k ? v : k;
         }
-        const unsigned char d = (unsigned char)(k & 0xffu);
-        for (int r = 0; r < peers.nranks; ++r) peers.maps[r][pix] = d;  // every rank receives the final map
+        const T d = (T)k;
+        for (int r = 0; r < peers.nranks; ++r) reinterpret_cast<T*>(peers.maps[r])[pix] = d;  // every rank receives the final map
     }
     if (peers.seq) p2p_publish(peers, kMaxRanks);   // DONE
 }
@@ -773,9 +775,10 @@ __global__ void p2p_wait_done_kernel(const unsigned* flags /* this rank's flag w
     }
 }
 
-// Final step of the sharded WTA: min over ranks of the packed keys, low 8 bits -> u8 map.
+// Final step of the sharded WTA: min over ranks of the packed keys, low 8 or 16 bits -> the map.
+template <typename T>
 __global__ void keys_reduce_kernel(const unsigned long long* __restrict__ gathered, int nranks, size_t npix,
-                                   uint8_t* __restrict__ dis)
+                                   T* __restrict__ dis)
 {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= npix) return;
@@ -784,7 +787,7 @@ __global__ void keys_reduce_kernel(const unsigned long long* __restrict__ gather
         const unsigned long long v = gathered[(size_t)r * npix + i];
         k = v < k ? v : k;
     }
-    dis[i] = (uint8_t)(k & 0xffu);
+    dis[i] = (T)k;
 }
 
 }  // namespace psm

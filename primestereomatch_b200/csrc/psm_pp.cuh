@@ -16,10 +16,12 @@
 //
 // GPU mapping (nothing like the reference's serial column scan with necklace tables): one WARP per pixel,
 //   the 361 window taps dealt round-robin to the 32 lanes (12 rounds), each tap one 4-byte load of a packed
-//   u32 image (disparity << 24 | R6 << 16 | G6 << 8 | B6);
-//   the taps ((disparity, fixed-point weight) pairs) stay in registers, 12 per lane; the weighted median is found by eight
-//   bisection steps on the value, each a masked add per tap and one warp REDUX -- no shared memory, no atomics, integer
-//   sums (exact, order-independent, identical to a 256-bin histogram scan).
+//   u32 image, d << kDispShift | R6 << 2 * kColourBits | G6 << kColourBits | B6 (MapFormat, psm_common.cuh):
+//   d << 24 | R6 << 16 | G6 << 8 | B6 for u8 maps, d << 18 | R6 << 12 | G6 << 6 | B6 for u16 maps;
+//   the taps ((disparity, fixed-point weight) pairs) stay in registers, 12 per lane; the weighted median is found by
+//   bisection on the value, eight steps over [0, 255] on u8 maps and ceil(log2 D) steps over [0, D - 1] on u16 maps,
+//   each a masked add per tap and one warp REDUX -- no shared memory, no atomics, integer sums (exact,
+//   order-independent, identical to a histogram scan).
 #pragma once
 #include "psm_common.cuh"
 
@@ -32,10 +34,12 @@ constexpr int kPpLutN = 1344;                // the 2^-22 fixed-point weight is 
                                              // prefix of the table is ever non-zero; it lives in shared memory (random gathers: bank
                                              // conflicts cost a few cycles, L1 line wavefronts cost up to 32 per load)
 
-// guide planes (float, BGR planar) + u8 disparity map -> packed u32 image
+// guide planes (float, BGR planar) + disparity map -> packed u32 image
+template <typename T>
 __global__ void pp_pack_kernel(const float* __restrict__ I0, const float* __restrict__ I1, const float* __restrict__ I2, int Wp,
-                               const uint8_t* __restrict__ disp, int W, int H, uint32_t* __restrict__ packed)
+                               const T* __restrict__ disp, int W, int H, uint32_t* __restrict__ packed)
 {
+    using F = MapFormat<T>;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= W || y >= H) return;
@@ -47,12 +51,16 @@ __global__ void pp_pack_kernel(const float* __restrict__ I0, const float* __rest
         return (uint32_t)(q >> 2);           // JointWMF.h:546,559-561: 8 bit -> 6 bit
     };
     const uint32_t b = q6(I0[o]), g = q6(I1[o]), r = q6(I2[o]);
-    packed[(size_t)y * W + x] = ((uint32_t)disp[(size_t)y * W + x] << 24) | (r << 16) | (g << 8) | b;
+    packed[(size_t)y * W + x] =
+        ((uint32_t)disp[(size_t)y * W + x] << F::kDispShift) | (r << 2 * F::kColourBits) | (g << F::kColourBits) | b;
 }
 
+// max_disp and steps = ceil(log2 max_disp) bound the bisection on u16 maps; u8 maps always take eight steps over [0, 255]
+template <typename T>
 __global__ void __launch_bounds__(kPpWarps * 32) pp_wmf_kernel(const uint32_t* __restrict__ packed, const uint32_t* __restrict__ lut,
-                                                              int W, int H, uint8_t* __restrict__ out)
+                                                              int W, int H, T* __restrict__ out, int max_disp, int steps)
 {
+    using F = MapFormat<T>;
     __shared__ uint32_t slut[kPpLutN];
     for (int i = threadIdx.x; i < kPpLutN; i += blockDim.x) slut[i] = __ldg(lut + i);
     __syncthreads();
@@ -62,7 +70,7 @@ __global__ void __launch_bounds__(kPpWarps * 32) pp_wmf_kernel(const uint32_t* _
     for (long pix = (long)blockIdx.x * kPpWarps + warp; pix < npix; pix += (long)gridDim.x * kPpWarps) {
         const int y = (int)(pix / W), x = (int)(pix - (long)y * W);
         const uint32_t cp = __ldg(packed + pix);
-        const int pb = cp & 63, pg = (cp >> 8) & 63, pr = (cp >> 16) & 63;
+        const int pb = cp & 63, pg = (cp >> F::kColourBits) & 63, pr = (cp >> 2 * F::kColourBits) & 63;
         // the 361 window taps are dealt round-robin to the 32 lanes and stay in registers: (disparity, weight) x 12
         uint32_t dq[kRounds], wq[kRounds];
         uint32_t total = 0;
@@ -72,23 +80,27 @@ __global__ void __launch_bounds__(kPpWarps * 32) pp_wmf_kernel(const uint32_t* _
             const int dy = i / kSide, dx = i - dy * kSide;
             const int yy = y - kPpRadius + dy, xx = x - kPpRadius + dx;
             const bool ok = i < kTaps && yy >= 0 && yy < H && xx >= 0 && xx < W;
-            dq[r] = 256u;     // greater than every candidate value: never counted
+            dq[r] = F::kSentinel;     // greater than every candidate value: never counted
             wq[r] = 0u;
             if (ok) {
                 const uint32_t cq = __ldg(packed + (size_t)yy * W + xx);
-                const int d0 = pb - (int)(cq & 63), d1 = pg - (int)((cq >> 8) & 63), d2 = pr - (int)((cq >> 16) & 63);
+                const int d0 = pb - (int)(cq & 63), d1 = pg - (int)((cq >> F::kColourBits) & 63),
+                          d2 = pr - (int)((cq >> 2 * F::kColourBits) & 63);
                 const int dd = d0 * d0 + d1 * d1 + d2 * d2;
                 wq[r] = dd < kPpLutN ? slut[dd] : 0u;
-                dq[r] = cq >> 24;
+                dq[r] = cq >> F::kDispShift;
             }
             total += wq[r];
         }
         total = __reduce_add_sync(0xffffffffu, total);
-        // out = min { v : 2 * sum_{dq <= v} w >= total }: eight bisection steps, each one masked add per tap and one REDUX
-        // (integer sums: exact and order-independent, identical to a histogram scan)
-        int lo = 0, hi = 255;
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
+        // out = min { v : 2 * sum_{dq <= v} w >= total }: bisection steps, each one masked add per tap and one REDUX
+        // (integer sums: exact and order-independent, identical to a histogram scan).  u8 maps: eight fully unrolled
+        // steps over [0, 255]; u16 maps: `steps` rolled steps over [0, max_disp - 1]
+        constexpr bool kU8 = sizeof(T) == 1;
+        int lo = 0, hi = kU8 ? 255 : max_disp - 1;
+        const int nsteps = kU8 ? 8 : steps;
+#pragma unroll(kU8 ? 8 : 1)
+        for (int it = 0; it < nsteps; ++it) {
             const int mid = (lo + hi) >> 1;
             uint32_t s = 0;
 #pragma unroll
@@ -96,7 +108,7 @@ __global__ void __launch_bounds__(kPpWarps * 32) pp_wmf_kernel(const uint32_t* _
             s = __reduce_add_sync(0xffffffffu, s);
             if (2u * s >= total) hi = mid; else lo = mid + 1;
         }
-        if (lane == 0) out[pix] = (uint8_t)lo;
+        if (lane == 0) out[pix] = (T)lo;
     }
 }
 
