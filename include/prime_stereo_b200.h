@@ -207,8 +207,12 @@ int psm_cost_filter(psm_ctx* ctx);
 /* Stage 2, Fast-Guided-Filter variant (DispEst::CostFilter_FGF, what the reference's CPU branch runs today): every
  * slice is sub-sampled by `sub_sample_rate` (1, 2, 4 or 8; the reference's `s` key cycles 2, 4, 8, default 4),
  * guided-filtered there with a (2*(8/s)+1)^2 box and the coefficient means are bilinearly up-sampled.  In place,
- * asynchronous.  Results equal the CPU restatement orc_cost_filter_fgf (test infrastructure, oracle/) bit for bit, which is pinned against
- * OpenCV's own (non-IPP) cv::blur / cv::resize arithmetic (tests/golden/make_golden_fgf.py). */
+ * asynchronous.  Results equal the CPU restatement orc_cost_filter_fgf (test infrastructure, oracle/) bit for bit at any
+ * input, including wide-range, outlier and non-finite costs, which is pinned against OpenCV's own (non-IPP) cv::blur /
+ * cv::resize arithmetic (tests/golden/make_golden_fgf.py).  The K x K box is defined as the direct fp64 sum: from 0.0,
+ * the K taps of a row left to right, then the K row sums top to bottom, times 1/K^2 in double, one rounding.  That equals
+ * cv::blur wherever the fp64 sums are exact (values within 2^(29 - ceil(log2 K^2)) of each other in exponent); beyond
+ * that the direct order is this library's definition, and cv::blur, which slides part of its sums, may differ. */
 int psm_cost_filter_fgf(psm_ctx* ctx, int sub_sample_rate);
 
 /* Stage 3: WTA over d in [1, max_disp) for both views; copies the u8 maps to HOST memory

@@ -7,7 +7,10 @@
 // branch runs today (src/StereoMatch.cpp:214); it is NOT the full-resolution GIF of psm_cvf_stream.cuh.
 //
 // Numerics follow the CPU restatement orc_fgf_* (test infrastructure, oracle/) (pinned against cv2 with IPP off, tests/golden/
-// make_golden_fgf.py): box sums in fp64 (exact: <= 81 terms), * 1/(K*K) in double, one rounding; every float
+// make_golden_fgf.py): the K x K box is DEFINED as the direct fp64 sum, from 0.0, K taps left to right, then the K row
+// sums top to bottom, * 1/(K*K) in double, one rounding (orc_box_k).  That equals cv::blur wherever the fp64 sums are
+// exact (OpenCV slides part of its sums); beyond that, at wide-range, outlier or non-finite inputs, the direct order is
+// this project's definition, and the device performs the same fp64 operations in the same order at any input.  Every float
 // operation a separate IEEE op in source order; the diagonal variance terms (x - y + eps) in double with one
 // rounding (cv::addWeighted); true divisions; OpenCV's own INTER_NN / INTER_LINEAR index and weight formulas
 // (tables built on the host by the same float / double expressions, see psm_capi.cu).
@@ -44,17 +47,23 @@ __global__ void fgf_guide_kernel(const float* __restrict__ I /* 3 full-res plane
     if (x >= g.w2 || y >= g.h2) return;
     const int a = g.K / 2;
     const size_t n2 = (size_t)g.w2 * g.h2, o = (size_t)y * g.w2 + x;
+    // direct box sums in orc_box_k's order: per row, from 0.0, the taps left to right; then the row sums top to bottom
     double sm[3] = {0, 0, 0}, sp[6] = {0, 0, 0, 0, 0, 0};
     for (int dy = -a; dy <= a; ++dy) {
         const int yy = fgf_nn(reflect101(y + dy, g.h2), g.ify, g.H);
+        double rm[3] = {0, 0, 0}, rp[6] = {0, 0, 0, 0, 0, 0};
         for (int dx = -a; dx <= a; ++dx) {
             const int xx = fgf_nn(reflect101(x + dx, g.w2), g.ifx, g.W);
             const size_t q = (size_t)yy * g.Wp + xx;
             const float c0 = I[q], c1 = I[plane + q], c2 = I[2 * plane + q];
-            sm[0] += (double)c0; sm[1] += (double)c1; sm[2] += (double)c2;
-            sp[0] += (double)fmul(c0, c0); sp[1] += (double)fmul(c0, c1); sp[2] += (double)fmul(c0, c2);
-            sp[3] += (double)fmul(c1, c1); sp[4] += (double)fmul(c1, c2); sp[5] += (double)fmul(c2, c2);
+            rm[0] += (double)c0; rm[1] += (double)c1; rm[2] += (double)c2;
+            rp[0] += (double)fmul(c0, c0); rp[1] += (double)fmul(c0, c1); rp[2] += (double)fmul(c0, c2);
+            rp[3] += (double)fmul(c1, c1); rp[4] += (double)fmul(c1, c2); rp[5] += (double)fmul(c2, c2);
         }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) sm[k] += rm[k];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) sp[k] += rp[k];
     }
     const double scale = 1.0 / ((double)g.K * g.K);
     const float m0 = (float)(sm[0] * scale), m1 = (float)(sm[1] * scale), m2 = (float)(sm[2] * scale);
@@ -87,19 +96,35 @@ __global__ void fgf_guide_kernel(const float* __restrict__ I /* 3 full-res plane
 //   region R1 = tile + 2h halo (h = K/2): p and I*p at the NN sample points, widened once into shared memory (doubles)
 //   horizontal K-sums -> vertical K-sums -> box means on R2 = tile + h halo -> a (3), b there (floats, shared memory)
 //   horizontal / vertical K-sums of a, b -> their box means on the tile -> global memory (4 planes per slice)
-// Cells outside the low-res image hold the value of the BORDER_REFLECT_101 pixel; because reflect-101 is an even
-// symmetry and the fp64 sums are exact, the box around a halo cell equals the box around the pixel it mirrors, so the
-// second stage sees exactly cv::blur's border handling of the first stage's output.
+// Cells outside the low-res image hold the value of the BORDER_REFLECT_101 pixel.  The a, b cells of R2 outside the
+// image are computed as the a, b of the pixel they mirror (see the box sums below), so the second stage sees exactly the
+// direct box's border handling of the first stage's output.
 constexpr int kFgfTX = 32, kFgfTY = 16, kFgfThreads = 256;
 
 __host__ __device__ inline size_t fgf_smem_bytes(int K)
 {
     const int h = K / 2;
-    // row strides are made odd: the sliding sums run one thread per row, so consecutive lanes are one row stride apart
+    // the three regions with odd row strides; this bounds the box the call accepts (K <= 19 in an H100's 227 KB per block)
     const size_t r1 = (size_t)((kFgfTX + 4 * h) | 1) * (kFgfTY + 4 * h);    // inputs (4 planes of doubles)
     const size_t hs = (size_t)((kFgfTX + 2 * h) | 1) * (kFgfTY + 4 * h);    // horizontal sums (4 planes of doubles)
     const size_t r2 = (size_t)((kFgfTX + 2 * h) | 1) * (kFgfTY + 2 * h);    // a, b (4 planes of floats)
     return (r1 + hs) * 4 * sizeof(double) + r2 * 4 * sizeof(float);
+}
+
+// Direct fp64 box sums of the four planes (`pstride` apart) at two outputs at once: from 0.0, K taps `step` apart, in
+// order.  Eight independent chains, so that the dependent fp64 adds of one thread overlap.
+template <typename T>
+__device__ __forceinline__ void fgf_sum8(const T* a, const T* b, size_t pstride, int step, int K, double sa[4], double sb[4])
+{
+#pragma unroll
+    for (int k = 0; k < 4; ++k) sa[k] = sb[k] = 0.0;
+    for (int t = 0; t < K; ++t) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            sa[k] += (double)a[k * pstride + (size_t)t * step];
+            sb[k] += (double)b[k * pstride + (size_t)t * step];
+        }
+    }
 }
 
 __global__ void __launch_bounds__(kFgfThreads) fgf_lowres_kernel(const float* __restrict__ vol, size_t vplane, FgfGeom g,
@@ -113,6 +138,7 @@ __global__ void __launch_bounds__(kFgfThreads) fgf_lowres_kernel(const float* __
     constexpr int kTXs = kFgfTX | 1;                          // stage-2 row stride
     double* in = fsm;                                        // [4][H1][W1]
     double* hs = in + (size_t)4 * W1 * H1;                   // [4][H1][W2]  (stage 2 reuses it as [4][H2][kTXs])
+    // every sum below runs one thread per output, lanes along a row, so the strides give no bank conflicts either way
     float* ab = reinterpret_cast<float*>(hs + (size_t)4 * W2 * H1);   // [4][H2][W2]
     const int x0 = blockIdx.x * kFgfTX, y0 = blockIdx.y * kFgfTY, dl = blockIdx.z;
     const size_t n2 = (size_t)g.w2 * g.h2;
@@ -136,29 +162,42 @@ __global__ void __launch_bounds__(kFgfThreads) fgf_lowres_kernel(const float* __
         }
     }
     __syncthreads();
-    // Box sums as SLIDING fp64 sums (+ entering, - leaving): two shared-memory reads per output instead of K.  The sums
-    // are exact (<= 81 floats of bounded range), so the sliding form gives the same bits as the direct form.
-    // ---- stage 1, horizontal: one thread per (plane, row) slides along the W2 outputs
-    for (int task = threadIdx.x; task < 4 * H1; task += kFgfThreads) {
-        const double* src = in + (size_t)task * W1;      // task = plane * H1 + row
-        double* dst = hs + (size_t)task * W2;
-        double sacc = 0;
-        for (int d = 0; d < K; ++d) sacc += src[d];
-        dst[0] = sacc;
-        for (int x = 1; x < W2n; ++x) { sacc = (sacc + src[x + K - 1]) - src[x - 1]; dst[x] = sacc; }
+    // Box sums are DIRECT fp64 sums in orc_box_k's order: from 0.0, the K taps of a row left to right, then the K row sums
+    // top to bottom.  Every R2 cell gets the box of the real pixel it stands for, (reflect101(x), reflect101(y)): its taps
+    // are read around that pixel's own position in R1 (R1 cell j holds the value at reflect101(x0 - 2h + j), and
+    // reflect101 is idempotent), not around the halo cell, whose taps are the same values in mirrored order.  For every
+    // R2 cell a valid output reads, those taps lie inside R1; the others (beyond the image edge by more than h) are
+    // clamped into R1 and only feed outputs that are never stored.
+    // Each thread takes two outputs at a time and all four planes of each: eight independent chains of dependent adds.
+    // ---- stage 1, horizontal: row sums of every R1 row at the R2 columns
+    for (int i = threadIdx.x; i < H1 * W2n; i += 2 * kFgfThreads) {
+        const bool two = i + kFgfThreads < H1 * W2n;
+        const int j = two ? i + kFgfThreads : i;
+        const int ry0 = i / W2n, rx0 = i - ry0 * W2n, ry1 = j / W2n, rx1 = j - ry1 * W2n;
+        const int bx0 = min(max(reflect101(x0 - h + rx0, g.w2) - x0 + h, 0), W1n - K);   // R1 column of the first tap
+        const int bx1 = min(max(reflect101(x0 - h + rx1, g.w2) - x0 + h, 0), W1n - K);
+        double s0[4], s1[4];
+        fgf_sum8(in + ry0 * W1 + bx0, in + ry1 * W1 + bx1, (size_t)W1 * H1, 1, K, s0, s1);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            hs[((size_t)k * H1 + ry0) * W2 + rx0] = s0[k];
+            if (two) hs[((size_t)k * H1 + ry1) * W2 + rx1] = s1[k];
+        }
     }
     __syncthreads();
-    // ---- stage 1, vertical: one thread per (plane, column) slides down the H2 outputs -> box means (floats) into `ab`
-    for (int task = threadIdx.x; task < 4 * W2n; task += kFgfThreads) {
-        const int k = task / W2n, rx = task - k * W2n;
-        const double* src = hs + (size_t)k * H1 * W2 + rx;
-        float* dst = ab + (size_t)k * W2 * H2 + rx;
-        double sacc = 0;
-        for (int d = 0; d < K; ++d) sacc += src[(size_t)d * W2];
-        dst[0] = (float)(sacc * scale);
-        for (int y = 1; y < H2; ++y) {
-            sacc = (sacc + src[(size_t)(y + K - 1) * W2]) - src[(size_t)(y - 1) * W2];
-            dst[(size_t)y * W2] = (float)(sacc * scale);
+    // ---- stage 1, vertical: K row sums per R2 cell, top to bottom -> box means (floats) into `ab`
+    for (int i = threadIdx.x; i < H2 * W2n; i += 2 * kFgfThreads) {
+        const bool two = i + kFgfThreads < H2 * W2n;
+        const int j = two ? i + kFgfThreads : i;
+        const int ry0 = i / W2n, rx0 = i - ry0 * W2n, ry1 = j / W2n, rx1 = j - ry1 * W2n;
+        const int by0 = min(max(reflect101(y0 - h + ry0, g.h2) - y0 + h, 0), H1 - K);    // R1 row of the first tap
+        const int by1 = min(max(reflect101(y0 - h + ry1, g.h2) - y0 + h, 0), H1 - K);
+        double s0[4], s1[4];
+        fgf_sum8(hs + by0 * W2 + rx0, hs + by1 * W2 + rx1, (size_t)W2 * H1, W2, K, s0, s1);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            ab[((size_t)k * H2 + ry0) * W2 + rx0] = (float)(s0[k] * scale);
+            if (two) ab[((size_t)k * H2 + ry1) * W2 + rx1] = (float)(s1[k] * scale);
         }
     }
     __syncthreads();
@@ -182,35 +221,35 @@ __global__ void __launch_bounds__(kFgfThreads) fgf_lowres_kernel(const float* __
         }
     }
     __syncthreads();
-    // ---- stage 2, horizontal: (plane, row) tasks slide along the TX outputs of the tile
-    for (int task = threadIdx.x; task < 4 * H2; task += kFgfThreads) {
-        const float* src = ab + (size_t)task * W2;
-        double* dst = hs + (size_t)task * kTXs;
-        double sacc = 0;
-        for (int d = 0; d < K; ++d) sacc += (double)src[d];
-        dst[0] = sacc;
-        for (int x = 1; x < kFgfTX; ++x) { sacc = (sacc + (double)src[x + K - 1]) - (double)src[x - 1]; dst[x] = sacc; }
-    }
-    __syncthreads();
-    // ---- stage 2, vertical: (plane, column) tasks slide down the TY outputs -> means staged in `in` as floats [TY][TX][4]
-    float* stage = reinterpret_cast<float*>(in);
-    for (int task = threadIdx.x; task < 4 * kFgfTX; task += kFgfThreads) {
-        const int k = task / kFgfTX, tx = task - k * kFgfTX;
-        const double* src = hs + (size_t)k * H2 * kTXs + tx;
-        double sacc = 0;
-        for (int d = 0; d < K; ++d) sacc += src[(size_t)d * kTXs];
-        stage[(0 * kFgfTX + tx) * 4 + k] = (float)(sacc * scale);
-        for (int y = 1; y < kFgfTY; ++y) {
-            sacc = (sacc + src[(size_t)(y + K - 1) * kTXs]) - src[(size_t)(y - 1) * kTXs];
-            stage[(y * kFgfTX + tx) * 4 + k] = (float)(sacc * scale);
+    // ---- stage 2, horizontal: row sums of every R2 row at the tile's columns (output x reads R2 columns x - x0 .. + K-1)
+    for (int i = threadIdx.x; i < H2 * kFgfTX; i += 2 * kFgfThreads) {
+        const bool two = i + kFgfThreads < H2 * kFgfTX;
+        const int j = two ? i + kFgfThreads : i;
+        const int ry0 = i / kFgfTX, rx0 = i % kFgfTX, ry1 = j / kFgfTX, rx1 = j % kFgfTX;
+        double s0[4], s1[4];
+        fgf_sum8(ab + ry0 * W2 + rx0, ab + ry1 * W2 + rx1, (size_t)W2 * H2, 1, K, s0, s1);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            hs[((size_t)k * H2 + ry0) * kTXs + rx0] = s0[k];
+            if (two) hs[((size_t)k * H2 + ry1) * kTXs + rx1] = s1[k];
         }
     }
     __syncthreads();
-    // ---- (mean_a_r, mean_a_g, mean_a_b, mean_b) of the tile, interleaved per pixel, coalesced 128-bit stores (:188-191)
-    for (int ty = ty0; ty < kFgfTY; ty += kRowsPerPass) {
-        const int x = x0 + tx0, y = y0 + ty;
-        if (x >= g.w2 || y >= g.h2) continue;
-        reinterpret_cast<float4*>(mean)[(size_t)dl * n2 + (size_t)y * g.w2 + x] = reinterpret_cast<const float4*>(stage)[ty * kFgfTX + tx0];
+    // ---- stage 2, vertical -> (mean_a_r, mean_a_g, mean_a_b, mean_b) of the tile, interleaved per pixel, coalesced 128-bit
+    // stores (:188-191); the 32 x 16 outputs are exactly two per thread, rows ty0 and ty0 + 8
+    static_assert(kFgfTY == 2 * kRowsPerPass, "two output rows per thread");
+    {
+        double s0[4], s1[4];
+        fgf_sum8(hs + ty0 * kTXs + tx0, hs + (ty0 + kRowsPerPass) * kTXs + tx0, (size_t)kTXs * H2, kTXs, K, s0, s1);
+        const int x = x0 + tx0;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int y = y0 + ty0 + r * kRowsPerPass;
+            const double* sr = r ? s1 : s0;
+            if (x < g.w2 && y < g.h2)
+                reinterpret_cast<float4*>(mean)[(size_t)dl * n2 + (size_t)y * g.w2 + x] =
+                    make_float4((float)(sr[0] * scale), (float)(sr[1] * scale), (float)(sr[2] * scale), (float)(sr[3] * scale));
+        }
     }
 }
 

@@ -4,8 +4,10 @@ The reference fixes GIF_R_WIN = 8 and GIF_EPS = 0.0001f at compile time (include
 makes both run-time parameters.  This module restates, for any window K and eps, what the plain-C oracle
 (oracle/stereo_oracle.c) restates for (8, 1e-4f):
   * box(src, K)         cv::boxFilter(CV_32F, Size(K, K)), anchor K/2, BORDER_REFLECT_101, in OpenCV's own summation order
-                        (RowSum<float,double> then ColumnSum<double,float>; see orc_box8), so it equals cv2 even where
-                        fp64 sums are not exact;
+                        (RowSum<float,double>: direct sums up to K = 5, sliding above; then ColumnSum<double,float>,
+                        sliding; see orc_box8), so it equals cv2 even where fp64 sums are not exact;
+  * box_direct(src, K)  the Fast Guided Filter's box, DEFINED as the direct order (orc_box_k); it equals cv::blur wherever
+                        the fp64 sums are exact (see its docstring) and is this project's own definition beyond that;
   * cvf_preprocess      CVF::preprocess (CVF.cpp:44-70) with a K x K box;
   * guided_filter       GuidedFilter_cv (CVF.cpp:72-165), eps on the covariance diagonal, float operations in the reference's
                         order (numpy float32 arithmetic rounds every operation and never contracts to FMA);
@@ -37,12 +39,15 @@ def box(src, K):
     H, W = src.shape[-2:]
     a = K // 2
     scale = 1.0 / float(K * K)
-    # RowSum: padded row p[i] = src[reflect101(i - a)], s = p[0] + ... + p[K-1], then s += p[i+K] - p[i]
-    # (a 2-wide row sum is p[i] + p[i+1] in OpenCV, checked against cv2 by tests/test_oracle_window.py)
+    # RowSum: padded row p[i] = src[reflect101(i - a)], s = p[0] + ... + p[K-1], then s += p[i+K] - p[i]; rows up to 5
+    # wide OpenCV sums directly, p[i] + p[i+1] + ... + p[i+K-1] left to right (both checked against cv2 by
+    # tests/test_fgf_numerics.py on data where the two orders differ)
     cols = reflect101(np.arange(W + K - 1) - a, W)
     prow = src[..., cols].astype(np.float64)
-    if K == 2:
-        rs = prow[..., 0:W] + prow[..., 1:W + 1]
+    if K <= 5:
+        rs = prow[..., 0:W]
+        for i in range(1, K):
+            rs = rs + prow[..., i:i + W]
     else:
         rs = np.empty(src.shape, np.float64)
         acc = np.zeros(src.shape[:-1], np.float64)
@@ -125,7 +130,15 @@ def wta(vol):
 
 # ---- Fast Guided Filter (fastguidedfilter.cpp:121-198 with r, eps, s; the C restatement is orc_cost_filter_fgf) -----------
 def box_direct(src, K):
-    """cv::blur as restated by orc_box_k: fp64 row sums then fp64 column sums of reflected taps, one rounding."""
+    """The Fast Guided Filter's K x K box as orc_box_k defines it: per pixel, from 0.0, the K reflected taps of a row left
+    to right in fp64, then the K row sums top to bottom, * 1/(K*K) in double, one rounding.
+
+    cv::blur slides most of its fp64 sums (box above), so the two agree exactly when every fp64 sum either order forms
+    is exact.  That holds when all values are integer multiples of 2^q and below 2^Q in magnitude with
+    Q - q + ceil(log2(K*K)) <= 53: every partial sum is then a multiple of 2^q of magnitude at most 2^(q+53).  For
+    normal floats (a float in [2^e, 2^(e+1)) is a multiple of 2^(e-23)) this allows the exponents of the nonzero values
+    to span 29 - ceil(log2(K*K)) binary orders of magnitude: 20 at K = 17, 16 at K = 65.  Beyond that the direct order
+    is this project's definition, not cv::blur's."""
     src = np.asarray(src, F32)
     H, W = src.shape[-2:]
     a = K // 2
