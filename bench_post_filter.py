@@ -6,7 +6,7 @@ Configurations: (9, 25.5, 1, exp) is the default and runs the tuned kernel pair 
 two; radius 16 and 32, iv2 and 3 iterations are other settings.  Each configuration is timed in two alternating rounds.
 Per configuration and round: ms per call of psm_post_process_device (CUDA events around `steps` calls on the context's
 stream) and the median stage-5 time (psm_stage_ms, all passes of both views); in the first round the top 64 rows of both
-filtered maps are checked against the CPU restatement tests/pp_oracle.c run on rows [0, 64 + iterations * radius)
+filtered maps are checked against the CPU restatement oracle.post_process run on rows [0, 64 + iterations * radius)
 (exact: the clipped windows of those rows lie inside).  Quality: %BP (non-occluded, left map) of Cones and Teddy at
 D = 64 after post-processing, for a small grid of filter settings at the default matching cost and at
 (0.11, 0.21, 0.008), the metric of bench_gif_window.py.
@@ -48,7 +48,6 @@ def main():
     from bench_gif_window import bad_pixels_nonocc, read_png
     from primestereomatch_b200 import DispEst, capi, synth
     from oracle import oracle as O
-    import pp_oracle as P
     if not torch.cuda.is_available() or capi.lib().psm_device_count() < 1:
         raise SystemExit("bench_post_filter.py needs a CUDA device")
     W, H, D = 1920, 1080, 128
@@ -88,7 +87,7 @@ def main():
                     rows = BAND + cfg[2] * cfg[0]
                     ok = True
                     for img, dmap, got in ((l, ld, de.lDisMap), (r, rd, de.rDisMap)):
-                        want = P.post_process(img[:rows], dmap[:rows], *cfg)[:BAND]
+                        want = O.post_process(img[:rows], dmap[:rows], *cfg)[:BAND]
                         ok = ok and bool(np.array_equal(got[:BAND], want))
                     res["band_parity"] = ok
                 print(json.dumps({"progress": {"cfg": str(cfg), "ms_per_call": res["ms_per_call"][-1],

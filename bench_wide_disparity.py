@@ -8,7 +8,7 @@ Per configuration: `steps` timed frames after `warmup` (ingest -> CVC -> CVF -> 
 events around the whole loop on the context's stream -> ms per frame and frames per second; the median stage times
 (psm_stage_ms) of CVC, CVF, WTA and the post-filter at the default (radius 9) and at radius 16.
 Parity: before the line is printed, rows [0, 16) of both maps of every configuration are compared with the CPU oracle
-(oracle/ CVC + guided filter, tests/wide_oracle.c arg-min) run on rows [0, 32): the filtered costs of those rows depend on
+(oracle/ CVC, guided filter and u16 arg-min) run on rows [0, 32): the filtered costs of those rows depend on
 rows < 25 only.
 
 Usage: python bench_wide_disparity.py [--steps 10] [--warmup 2]
@@ -44,7 +44,6 @@ def main():
     from bench import device_info
     from primestereomatch_b200 import DispEst, capi, synth
     from oracle import oracle as O
-    import wide_oracle as WO
     if not torch.cuda.is_available() or capi.lib().psm_device_count() < 1:
         raise SystemExit("bench_wide_disparity.py needs a CUDA device")
     L = capi.lib()
@@ -100,7 +99,7 @@ def main():
         _, _, lraw, rraw = O.cost_const(lc, rc, D)
         lf, rf = O.cost_filter(lc, rc, lraw, rraw)
         del lraw, rraw
-        res["band_parity"] = bool(np.array_equal(ld, WO.wta16(lf)[:BAND]) and np.array_equal(rd, WO.wta16(rf)[:BAND]))
+        res["band_parity"] = bool(np.array_equal(ld, O.wta(lf, np.uint16)[:BAND]) and np.array_equal(rd, O.wta(rf, np.uint16)[:BAND]))
         del lf, rf
         results.append(res)
         print(json.dumps({"progress": res}), file=sys.stderr, flush=True)

@@ -14,7 +14,13 @@ _LIB = None
 
 _f32p = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
 _u8p = np.ctypeslib.ndpointer(dtype=np.uint8, flags="C_CONTIGUOUS")
+_u32p = np.ctypeslib.ndpointer(dtype=np.uint32, flags="C_CONTIGUOUS")
 _f64p = np.ctypeslib.ndpointer(dtype=np.float64, flags="C_CONTIGUOUS")
+
+# the post-filter's weight types (JointWMF.h:503-508 numbering, as psm_set_post_filter takes them)
+WEIGHTS = {"exp": 0, "iv1": 1, "iv2": 2, "off": 5}
+_PP_TABLE_MAX = 3 * 63 * 63 + 1
+_MAP_BYTES = {np.dtype(np.uint8): 1, np.dtype(np.uint16): 2}
 
 
 def build():
@@ -39,7 +45,7 @@ def lib():
         L.orc_cvf_preprocess.argtypes = [_f32p, C.c_int, C.c_int, _f32p, _f32p, _f32p]
         L.orc_guided_filter.argtypes = [_f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p,
                                         C.c_void_p, C.c_void_p]
-        L.orc_wta.argtypes = [_f32p, C.c_int, C.c_int, C.c_int, _u8p]
+        L.orc_wta.argtypes = [_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int]
         L.orc_cost_const.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                      _f32p, _f32p, _f32p, _f32p]
         L.orc_cost_filter.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -49,9 +55,12 @@ def lib():
                                    _f32p, _f32p, _u8p, _u8p, _f64p]
         L.orc_cost_filter_fgf.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p]
         L.orc_cost_filter_fgf.restype = C.c_int
-        L.orc_wmf.argtypes = [_u8p, _u8p, C.c_int, C.c_int, C.c_int, _u8p]
+        L.orc_pp_weight_table.argtypes = [C.c_float, C.c_int, _u32p]
+        L.orc_wmf.argtypes = [C.c_void_p, C.c_int, _u8p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int,
+                              C.c_void_p]
         L.orc_f32_to_u8x255.argtypes = [_f32p, _u8p, C.c_size_t]
-        for name in ("orc_cost_const", "orc_cost_filter", "orc_disp_select", "orc_pipeline"):
+        for name in ("orc_cost_const", "orc_cost_filter", "orc_disp_select", "orc_pipeline", "orc_pp_weight_table",
+                     "orc_wmf"):
             getattr(L, name).restype = C.c_int
         _LIB = L
     return _LIB
@@ -125,11 +134,19 @@ def guided_filter(rgb, mean, var, p, want_ab=False):
     return p
 
 
-def wta(vol):
+def _map_bytes(dtype):
+    try:
+        return _MAP_BYTES[np.dtype(dtype)]
+    except KeyError:
+        raise TypeError(f"disparity maps are uint8 or uint16, not {np.dtype(dtype)}") from None
+
+
+def wta(vol, dtype=np.uint8):
+    """vol[D, H, W] -> arg-min map over d in [1, D); uint8 keeps the low byte as the reference does, uint16 all of it"""
     vol = _c(vol)
     D, H, W = vol.shape
-    out = np.empty((H, W), np.uint8)
-    lib().orc_wta(vol, W, H, D, out)
+    out = np.empty((H, W), dtype)
+    lib().orc_wta(vol, W, H, D, out.ctypes.data_as(C.c_void_p), _map_bytes(dtype))
     return out
 
 
@@ -182,15 +199,32 @@ def pipeline(l, r, D, threads=8, gray_mode=0, keep_volumes=False):
     return out
 
 
-def post_process(img3_f32, disp, r=9):
-    """PP::processDM's live code for one view (src/PP.cpp:414-422), un-clustered restatement (see stereo_oracle.c)."""
+def to_u8x255(img3_f32):
+    """convertTo(CV_8UC3, 255) (src/PP.cpp:416-417): saturate_cast<uchar>(cvRound(v * 255)), half to even"""
     img3 = _c(img3_f32)
-    disp = _c(disp, np.uint8)
-    H, W = disp.shape
     img8 = np.empty(img3.shape, np.uint8)
     lib().orc_f32_to_u8x255(img3.reshape(-1), img8.reshape(-1), img3.size)
-    out = np.empty((H, W), np.uint8)
-    lib().orc_wmf(disp, img8, W, H, r, out)
+    return img8
+
+
+def weight_table(sigma=25.5, weight="exp"):
+    """the post-filter's 2^-22 fixed-point weight table at (sigma, weight), as uint32"""
+    t = np.zeros(_PP_TABLE_MAX, np.uint32)
+    n = lib().orc_pp_weight_table(sigma, WEIGHTS[weight], t)
+    return t[:n].copy()
+
+
+def post_process(img3_f32, disp, r=9, sigma=25.5, iterations=1, weight="exp", threads=8):
+    """One view of the post-filter, JointWMF::filter at (r, sigma, iterations, weight) as PP::processDM drives it
+    (src/PP.cpp:414-422, defaults: its live code), un-clustered restatement (see stereo_oracle.c).  img3_f32: float BGR
+    feature image in [0, 1]; disp: a uint8 or uint16 map -> the filtered map, of disp's dtype."""
+    img8 = to_u8x255(img3_f32)
+    disp = np.ascontiguousarray(disp)
+    H, W = disp.shape
+    out = np.empty((H, W), disp.dtype)
+    rc = lib().orc_wmf(disp.ctypes.data_as(C.c_void_p), _map_bytes(disp.dtype), img8, W, H, int(r), float(sigma),
+                       int(iterations), WEIGHTS[weight], int(threads), out.ctypes.data_as(C.c_void_p))
+    assert rc == 0
     return out
 
 

@@ -295,8 +295,10 @@ void orc_guided_filter(const float* rgb, const float* mean_I, const float* var_I
 
 /* ------------------------------------------------------------------ a12: WTA */
 
-/* DispSel.cpp:83-109: d from 1, strict <, minCost starts at (float)DBL_MAX = +inf */
-static void wta_rows(const float* vol, int W, int H, int D, uint8_t* disp, int y0, int y1)
+/* DispSel.cpp:83-109: d from 1, strict <, minCost starts at (float)DBL_MAX = +inf.  The arg-min is an int there; the
+ * reference stores it into a uchar (map_bytes 1), a 16-bit map (map_bytes 2) keeps it whole, so the u8 map is the low
+ * byte of the u16 one. */
+static void wta_rows(const float* vol, int W, int H, int D, void* disp, int map_bytes, int y0, int y1)
 {
     const size_t n = (size_t)W * H;
     for (int y = y0; y < y1; ++y) {
@@ -307,27 +309,37 @@ static void wta_rows(const float* vol, int W, int H, int D, uint8_t* disp, int y
                 const float c = vol[(size_t)d * n + (size_t)y * W + x];
                 if (c < minCost) { minCost = c; minDis = d; }
             }
-            disp[(size_t)y * W + x] = (uint8_t)minDis;
+            const size_t i = (size_t)y * W + x;
+            if (map_bytes == 2) ((uint16_t*)disp)[i] = (uint16_t)minDis;
+            else ((uint8_t*)disp)[i] = (uint8_t)minDis;
         }
     }
 }
 
-void orc_wta(const float* vol, int W, int H, int D, uint8_t* disp)
+void orc_wta(const float* vol, int W, int H, int D, void* disp, int map_bytes)
 {
-    wta_rows(vol, W, H, D, disp, 0, H);
+    wta_rows(vol, W, H, D, disp, map_bytes, 0, H);
 }
 
 /* ------------------------------------------------------------------ a7/a11: thread drivers */
 
 typedef struct {
-    int kind; /* 0 left cvc, 1 right cvc, 2 filter, 3 wta rows */
+    int kind; /* 0 left cvc, 1 right cvc, 2 filter, 3 wta rows, 4 weighted-median rows */
     const float *lImg, *rImg, *lGrd, *rGrd;
     const float *rgb, *mean, *var;
     const float* vol_in;
     float* slice;
-    uint8_t* disp;
+    void* disp;
+    int map_bytes;
+    const uint16_t* wmf_in;    /* kind 4: map, feature image, weight table, histogram size, output */
+    const uint8_t* img8;
+    const uint32_t* lut;
+    int r, wtype, nbins;
+    uint16_t* wmf_out;
     int W, H, D, d, y0, y1;
 } task_t;
+
+static void* wmf_rows(const task_t* t);
 
 static void* task_entry(void* arg)
 {
@@ -336,27 +348,55 @@ static void* task_entry(void* arg)
     case 0: orc_buildcv_left(t->lImg, t->rImg, t->lGrd, t->rGrd, t->W, t->H, t->d, t->slice); break;
     case 1: orc_buildcv_right(t->lImg, t->rImg, t->lGrd, t->rGrd, t->W, t->H, t->d, t->slice); break;
     case 2: orc_guided_filter(t->rgb, t->mean, t->var, t->W, t->H, t->slice, NULL, NULL); break;
-    case 3: wta_rows(t->vol_in, t->W, t->H, t->D, t->disp, t->y0, t->y1); break;
+    case 3: wta_rows(t->vol_in, t->W, t->H, t->D, t->disp, t->map_bytes, t->y0, t->y1); break;
+    case 4: return wmf_rows(t);
     }
     return NULL;
 }
 
 /* DispEst.cpp:235-251 batching: for level in 0..=n/threads, block = threads or n%threads,
- * create block pthreads (one per d), join them all, next level. */
+ * create block pthreads (one per d), join them all, next level.  -> 0, or -1 when a thread could not be created or a
+ * task failed */
 static int run_batched(task_t* tasks, int n, int threads)
 {
     if (threads < 1) threads = 1;
     pthread_t* th = (pthread_t*)malloc((size_t)n * sizeof(pthread_t));
-    for (int level = 0; level <= n / threads; ++level) {
+    if (!th) return -1;
+    int rc = 0;
+    for (int level = 0; level <= n / threads && rc == 0; ++level) {
         int block = (level < n / threads) ? threads : (n % threads);
-        for (int it = 0; it < block; ++it) {
-            int d = level * threads + it;
-            if (pthread_create(&th[d], NULL, task_entry, &tasks[d]) != 0) { free(th); return -1; }
+        int started = 0;
+        for (; started < block; ++started)
+            if (pthread_create(&th[level * threads + started], NULL, task_entry, &tasks[level * threads + started]) != 0) {
+                rc = -1;
+                break;
+            }
+        for (int it = 0; it < started; ++it) {
+            void* ret = NULL;
+            pthread_join(th[level * threads + it], &ret);
+            if (ret) rc = -1;
         }
-        for (int it = 0; it < block; ++it) pthread_join(th[level * threads + it], NULL);
     }
     free(th);
-    return 0;
+    return rc;
+}
+
+/* rows [0, H) split over `threads` pthreads, one copy of `proto` each (DispSel::CVSelect is "#pragma omp parallel for"
+ * over rows, DispSel.cpp:88) */
+static int run_rows(task_t proto, int H, int threads)
+{
+    if (threads < 1) threads = 1;
+    if (threads > H) threads = H;
+    task_t* tasks = (task_t*)malloc((size_t)threads * sizeof(task_t));
+    if (!tasks) return -1;
+    for (int t = 0; t < threads; ++t) {
+        tasks[t] = proto;
+        tasks[t].y0 = (int)((long)H * t / threads);
+        tasks[t].y1 = (int)((long)H * (t + 1) / threads);
+    }
+    int rc = run_batched(tasks, threads, threads);
+    free(tasks);
+    return rc;
 }
 
 /* DispEst.cpp:222-270 */
@@ -410,29 +450,19 @@ int orc_cost_filter(const float* lImg, const float* rImg, int W, int H, int D, i
     return rc;
 }
 
-/* DispEst.cpp:311-321; DispSel::CVSelect is "#pragma omp parallel for" over rows
- * (DispSel.cpp:88) -- rows are split over `threads` pthreads here. */
+/* DispEst.cpp:311-321, rows split over `threads` pthreads */
 static int wta_view(const float* vol, int W, int H, int D, uint8_t* dis, int threads)
 {
-    if (threads < 1) threads = 1;
-    if (threads > H) threads = H;
-    task_t* tasks = (task_t*)calloc((size_t)threads, sizeof(task_t));
-    for (int t = 0; t < threads; ++t) {
-        task_t k = {0};
-        k.kind = 3; k.vol_in = vol; k.W = W; k.H = H; k.D = D; k.disp = dis;
-        k.y0 = (int)((long)H * t / threads); k.y1 = (int)((long)H * (t + 1) / threads);
-        tasks[t] = k;
-    }
-    int rc = run_batched(tasks, threads, threads);
-    free(tasks);
-    return rc;
+    task_t k = {0};
+    k.kind = 3; k.vol_in = vol; k.W = W; k.H = H; k.D = D; k.disp = dis; k.map_bytes = 1;
+    return run_rows(k, H, threads);
 }
 
 int orc_disp_select(const float* lVol, const float* rVol, int W, int H, int D,
                     uint8_t* lDis, uint8_t* rDis)
 {
-    orc_wta(lVol, W, H, D, lDis);
-    orc_wta(rVol, W, H, D, rDis);
+    orc_wta(lVol, W, H, D, lDis, 1);
+    orc_wta(rVol, W, H, D, rDis, 1);
     return 0;
 }
 
@@ -468,53 +498,97 @@ int orc_pipeline(const float* lImg, const float* rImg, int W, int H, int D, int 
  * 6-bit colours, where every colour is its own cluster) -- with the definition of the output the reference's cut-point
  * search implements (JointWMF.h:257-316):  out = min { v : sum_{I_q <= v} w_q  >=  sum_{I_q > v} w_q }  over the
  * (2r+1)^2 window clipped at the image border (JointWMF.h:207-211, 322-325).
- * Weights: w = exp(-(d0^2+d1^2+d2^2) * divider), divider = 1/(2 s^2), s = 25.5/256*64 (JointWMF.h:620-641), evaluated
- * in float exactly like the reference and then held as 2^-22 fixed point so that the sums are exact integers,
- * independent of summation order (the reference's float sums depend on its necklace-table insertion history).
+ * Weights: JointWMF.h:620-648's float formulas (see orc_pp_weight_table) held as 2^-22 fixed point so that the sums are
+ * exact integers, independent of summation order (the reference's float sums depend on its necklace-table insertion
+ * history).  r, sigma, iter and weightType are JointWMF::filter's arguments; PP::processDM passes (9, 25.5, 1, exp).
  * -------------------------------------------------------------------------------------------------------------- */
-#define ORC_PP_MAXD2 (3 * 63 * 63)
-void orc_pp_weight_lut(uint32_t* lut /* ORC_PP_MAXD2 + 1 */)
+static float pp_weight(int type, float s, int k)
 {
-    const float nSigmaI = 25.5f / 256.0f * 64;
-    const float divider = (1.0f / (2 * nSigmaI * nSigmaI));
-    for (int d2 = 0; d2 <= ORC_PP_MAXD2; ++d2) {
-        const float w = expf(-(float)d2 * divider);
-        lut[d2] = (uint32_t)lrintf(w * 4194304.0f);
+    switch (type) {
+    case ORC_WMF_EXP: return expf(-(float)k * (1.0f / ((2 * s) * s)));
+    case ORC_WMF_IV1: return 1.0f / ((float)k + s);
+    case ORC_WMF_IV2: return 1.0f / ((float)k + s * s);
+    default: return 1.0f;
     }
 }
 
-/* img8: interleaved BGR u8 (the CV_8UC3 feature image), disp: u8 map, out: u8 map (may not alias disp) */
-void orc_wmf(const uint8_t* disp, const uint8_t* img8, int W, int H, int r, uint8_t* out)
+int orc_pp_weight_table(float sigma, int type, uint32_t* t)
 {
-    uint32_t* lut = (uint32_t*)malloc((ORC_PP_MAXD2 + 1) * sizeof(uint32_t));
-    orc_pp_weight_lut(lut);
-    for (int y = 0; y < H; ++y) {
+    const float s = sigma / 256.0f * 64;
+    const float w0 = pp_weight(type, s, 0);
+    const int n = type == ORC_WMF_IV1 ? 3 * 63 + 1 : (type == ORC_WMF_OFF ? 1 : ORC_PP_TABLE_MAX);
+    for (int k = 0; k < n; ++k) t[k] = (uint32_t)lrintf((pp_weight(type, s, k) / w0) * 4194304.0f);
+    return n;
+}
+
+/* one pass over rows [y0, y1): wmf_in -> wmf_out, a histogram over the map values [0, nbins) */
+static void* wmf_rows(const task_t* a)
+{
+    const int W = a->W, H = a->H, r = a->r;
+    uint64_t* hist = (uint64_t*)malloc((size_t)a->nbins * sizeof(uint64_t));
+    if (!hist) return (void*)1;
+    for (int y = a->y0; y < a->y1; ++y) {
         for (int x = 0; x < W; ++x) {
-            uint64_t hist[256];
-            memset(hist, 0, sizeof(hist));
-            const uint8_t* cp = img8 + ((size_t)y * W + x) * 3;
+            memset(hist, 0, (size_t)a->nbins * sizeof(uint64_t));
+            const uint8_t* cp = a->img8 + ((size_t)y * W + x) * 3;
             const int b = cp[0] >> 2, g = cp[1] >> 2, rr = cp[2] >> 2;
             uint64_t total = 0;
-            const int y0 = y - r < 0 ? 0 : y - r, y1 = y + r > H - 1 ? H - 1 : y + r;
-            const int x0 = x - r < 0 ? 0 : x - r, x1 = x + r > W - 1 ? W - 1 : x + r;
-            for (int yy = y0; yy <= y1; ++yy)
-                for (int xx = x0; xx <= x1; ++xx) {
-                    const uint8_t* cq = img8 + ((size_t)yy * W + xx) * 3;
+            const int ya = y - r < 0 ? 0 : y - r, yb = y + r > H - 1 ? H - 1 : y + r;
+            const int xa = x - r < 0 ? 0 : x - r, xb = x + r > W - 1 ? W - 1 : x + r;
+            for (int yy = ya; yy <= yb; ++yy)
+                for (int xx = xa; xx <= xb; ++xx) {
+                    const uint8_t* cq = a->img8 + ((size_t)yy * W + xx) * 3;
                     const int d0 = b - (cq[0] >> 2), d1 = g - (cq[1] >> 2), d2 = rr - (cq[2] >> 2);
-                    const uint32_t w = lut[d0 * d0 + d1 * d1 + d2 * d2];
-                    hist[disp[(size_t)yy * W + xx]] += w;
+                    const int k = a->wtype == ORC_WMF_IV1 ? abs(d0) + abs(d1) + abs(d2)
+                                : a->wtype == ORC_WMF_OFF ? 0 : d0 * d0 + d1 * d1 + d2 * d2;
+                    const uint32_t w = a->lut[k];
+                    hist[a->wmf_in[(size_t)yy * W + xx]] += w;
                     total += w;
                 }
             uint64_t cum = 0;
             int v = 0;
-            for (; v < 255; ++v) {
+            for (; v < a->nbins - 1; ++v) {
                 cum += hist[v];
                 if (2 * cum >= total) break;
             }
-            out[(size_t)y * W + x] = (uint8_t)v;
+            a->wmf_out[(size_t)y * W + x] = (uint16_t)v;
         }
     }
-    free(lut);
+    free(hist);
+    return NULL;
+}
+
+int orc_wmf(const void* disp, int map_bytes, const uint8_t* img8, int W, int H, int r, float sigma, int iterations,
+            int type, int threads, void* out)
+{
+    const size_t n = (size_t)W * H;
+    uint32_t* lut = (uint32_t*)malloc(ORC_PP_TABLE_MAX * sizeof(uint32_t));
+    uint16_t* cur = (uint16_t*)malloc(n * sizeof(uint16_t));
+    uint16_t* next = (uint16_t*)malloc(n * sizeof(uint16_t));
+    int rc = lut && cur && next ? 0 : -1;
+    if (rc == 0) {
+        orc_pp_weight_table(sigma, type, lut);
+        int maxv = 0;
+        for (size_t i = 0; i < n; ++i) {
+            cur[i] = map_bytes == 2 ? ((const uint16_t*)disp)[i] : ((const uint8_t*)disp)[i];
+            maxv = cur[i] > maxv ? cur[i] : maxv;
+        }
+        task_t k = {0};
+        k.kind = 4; k.img8 = img8; k.lut = lut; k.W = W; k.H = H; k.r = r; k.wtype = type;
+        k.nbins = maxv + 1;   /* the median is a value of the window, so no pass raises the maximum */
+        /* JointWMF.h:126-131: each iteration filters the previous output with the original feature image */
+        for (int it = 0; it < iterations && rc == 0; ++it) {
+            k.wmf_in = cur; k.wmf_out = next;
+            rc = run_rows(k, H, threads);
+            uint16_t* t = cur; cur = next; next = t;
+        }
+        for (size_t i = 0; i < n && rc == 0; ++i) {
+            if (map_bytes == 2) ((uint16_t*)out)[i] = cur[i];
+            else ((uint8_t*)out)[i] = (uint8_t)cur[i];
+        }
+    }
+    free(lut); free(cur); free(next);
+    return rc;
 }
 
 /* lImg.convertTo(lImg_8UC3, CV_8UC3, 255) (src/PP.cpp:416-417): saturate_cast<uchar>(cvRound(v * 255)) */

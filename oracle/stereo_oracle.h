@@ -17,7 +17,7 @@
  *
  * Layouts: images are interleaved 3-channel float (BGR order as cv::imread gives,
  * reference StereoMatch.cpp:557) with an element step; volumes are [d][y][x] float,
- * contiguous; disparity maps are u8 [y][x].
+ * contiguous; disparity maps are u8 [y][x] (u8 or u16 for orc_wta and orc_wmf, chosen by map_bytes).
  */
 #ifndef STEREO_ORACLE_H
 #define STEREO_ORACLE_H
@@ -69,8 +69,9 @@ void orc_cvf_preprocess(const float* img3, int W, int H, float* rgb, float* mean
 void orc_guided_filter(const float* rgb, const float* mean, const float* var, int W, int H,
                        float* p_inout, float* a_out, float* b_out);
 
-/* DispSel.cpp:83-109 */
-void orc_wta(const float* vol, int W, int H, int D, uint8_t* disp);
+/* DispSel.cpp:83-109: the arg-min over d in [1, D) (strict <, lowest d on ties, 0 when nothing is below +inf) into a
+ * u8 map (map_bytes 1, the reference's uchar store: the low byte) or a u16 map (map_bytes 2) */
+void orc_wta(const float* vol, int W, int H, int D, void* disp, int map_bytes);
 
 /* DispEst.cpp:222-270 CostConst_CPU: preprocess both, then left volume in batches of
  * `threads` pthreads (one per d), then right volume likewise.  lGrd/rGrd (H*W) are outputs. */
@@ -98,8 +99,22 @@ int orc_cost_filter_fgf(const float* lImg, const float* rImg, int W, int H, int 
 
 /* Post-processing (PP::processDM live code, src/PP.cpp:414-422 -> JointWMF::filter): see stereo_oracle.c.
  * PARITY UNPINNED for natural images (cv::kmeans feature clustering is RNG-seeded); this is the un-clustered filter. */
-void orc_pp_weight_lut(uint32_t* lut /* 3*63*63 + 1 entries, 2^-22 fixed point */);
-void orc_wmf(const uint8_t* disp, const uint8_t* img8_bgr, int W, int H, int r, uint8_t* out);
+enum { ORC_WMF_EXP = 0, ORC_WMF_IV1 = 1, ORC_WMF_IV2 = 2, ORC_WMF_OFF = 5 };   /* weightType, JointWMF.h:503-508 */
+#define ORC_PP_TABLE_MAX (3 * 63 * 63 + 1)   /* largest squared distance between two 6-bit colours, + 1 */
+
+/* The weight table of (sigma, type), 2^-22 fixed point: with s = sigma / 256.0f * 64 and w(k) in float with the
+ * operation order of JointWMF.h:620-648 (exp: expf(-(float)k * (1.0f / ((2*s)*s))), iv1: 1.0f / ((float)k + s),
+ * iv2: 1.0f / ((float)k + s*s), off: 1.0f), t[k] = lrintf((w(k) / w(0)) * 4194304.0f).  k is the squared distance of
+ * the 6-bit colours (exp, iv2), their L1 distance (iv1) or 0 (off).  t has room for ORC_PP_TABLE_MAX entries.
+ * -> the number of entries */
+int orc_pp_weight_table(float sigma, int type, uint32_t* t);
+/* JointWMF::filter(disp, img8, r, sigma, nI, 256, iterations, type) without the colour clustering:
+ * out(p) = min { v : 2 * sum_{q in window, I_q <= v} t[k(p,q)] >= sum_{q in window} t[k(p,q)] }, window clipped at the
+ * border, u64 sums; each iteration filters the previous output.  disp / out: u8 (map_bytes 1) or u16 (map_bytes 2) maps,
+ * may alias; img8: interleaved BGR u8 feature image; rows split over `threads` pthreads.  -> 0, or -1 (out of memory
+ * or no thread) */
+int orc_wmf(const void* disp, int map_bytes, const uint8_t* img8_bgr, int W, int H, int r, float sigma, int iterations,
+            int type, int threads, void* out);
 void orc_f32_to_u8x255(const float* src, uint8_t* dst, size_t n);
 
 #ifdef __cplusplus

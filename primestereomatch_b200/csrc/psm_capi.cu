@@ -56,9 +56,8 @@ struct psm_ctx {
     int fgf_s = 0;                          // sub-sampling rate the buffers / plan were built for
     uint8_t* dis_pp[2] = {nullptr, nullptr}; // post-processed maps (map_bytes per element)
     uint32_t* pp_packed = nullptr;          // packed (disparity, 6-bit colour) image of one view, lazy
-    uint32_t* pp_lut = nullptr;             // weight table indexed by squared colour distance, lazy
-    uint32_t* pp_plut = nullptr;            // weight table of the current post-filter setting (generic kernel), lazy
-    bool pp_plut_valid = false;             // pp_plut holds the table of (pp_sigma, pp_type)
+    uint32_t* pp_lut = nullptr;             // weight table of the current post-filter setting (kPpMaxD2 + 1 entries), lazy
+    bool pp_lut_valid = false;              // pp_lut holds the table of (pp_sigma, pp_type)
     bool have_maps = false;                 // disparity maps valid (a select / reduce stage ran)
     int* guide_flags = nullptr;             // [2] device flags: guide outside the integer-widening domain (see psm_cvf_stream.cuh)
     unsigned char* p2p_own = nullptr;       // own exchange block: keys [2 views][nranks][chunk] u64, maps [2 views][H*W] u8, flag words
@@ -115,6 +114,17 @@ int fail(psm_ctx* c, int code, const char* fmt, ...)
         (c)->launches++;                                                                           \
         PSM_CUDA((c), cudaGetLastError());                                                         \
     } while (0)
+
+// cudaMalloc into p while it is null; p stays null unless the allocation succeeds
+template <typename T>
+cudaError_t alloc_if_null(T*& p, size_t bytes)
+{
+    if (p) return cudaSuccess;
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, bytes);
+    if (e == cudaSuccess) p = static_cast<T*>(q);
+    return e;
+}
 
 int bind(psm_ctx* c)
 {
@@ -585,7 +595,7 @@ int psm_destroy(psm_ctx* c)
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaFree(c->ab);
     cudaFree(c->guide_flags);
-    cudaFree(c->pp_packed); cudaFree(c->pp_lut); cudaFree(c->pp_plut);
+    cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
     for (int v = 0; v < 2; ++v) cudaFree(c->dis_pp[v]);
     for (int s = 0; s < kNumStages; ++s) {
@@ -682,7 +692,7 @@ int psm_set_post_filter(psm_ctx* c, int radius, float sigma, int iterations, int
     if (iterations < 1 || iterations > 16) return fail(c, PSM_EINVAL, "post-filter iterations %d outside 1..16", iterations);
     if (weight_type != PSM_WMF_EXP && weight_type != PSM_WMF_IV1 && weight_type != PSM_WMF_IV2 && weight_type != PSM_WMF_OFF)
         return fail(c, PSM_EINVAL, "post-filter weight type %d is not exp (0), iv1 (1), iv2 (2) or off (5)", weight_type);
-    if (sigma != c->pp_sigma || weight_type != c->pp_type) c->pp_plut_valid = false;   // the table depends on both
+    if (sigma != c->pp_sigma || weight_type != c->pp_type) c->pp_lut_valid = false;   // the table depends on both
     c->pp_radius = radius;
     c->pp_sigma = sigma;
     c->pp_iter = iterations;
@@ -1196,7 +1206,8 @@ static int pp_weight_table_size(int type)
 
 // The post-filter's 2^-22 fixed-point weight table: JointWMF.h:620-648's float formulas on the 6-bit colour difference
 // (index: squared distance for exp / iv2, L1 distance for iv1, one entry for off), normalised by w(0) so that the centre
-// tap is always 2^22.  Built with -ffp-contract=off.  At (25.5, exp) equal to the default path's table.  -> entries
+// tap is always 2^22.  Built with -ffp-contract=off.  Both post-filter kernels read it: pp_wmf_kernel its first
+// kPpLutN entries, the generic kernels all of them.  -> entries
 static int pp_weight_table(float sigma, int type, uint32_t* t)
 {
     const float s = sigma / 256.0f * 64;
@@ -1227,37 +1238,26 @@ static int post_process_maps(psm_ctx* c)
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_post_process before psm_set_images");
     if (!c->have_maps && !(c->p2p_own && c->p2p_seq > 0)) return fail(c, PSM_ESTATE, "psm_post_process before a disparity-selection stage");
     const size_t npix = (size_t)c->W * c->H;
-    if (!c->pp_lut) {
-        // weight table: the reference's float expression (JointWMF.h:620-641, "exp" weights, sigma 25.5, 64 levels)
-        uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
-        if (!host) return fail(c, PSM_ENOMEM, "out of host memory");
-        const float nSigmaI = 25.5f / 256.0f * 64;
-        const float divider = (1.0f / (2 * nSigmaI * nSigmaI));
-        for (int d2 = 0; d2 <= kPpMaxD2; ++d2) host[d2] = (uint32_t)lrintf(expf(-(float)d2 * divider) * 4194304.0f);
-        cudaError_t e = cudaMalloc(&c->pp_lut, (kPpMaxD2 + 1) * sizeof(uint32_t));
-        if (e == cudaSuccess) e = cudaMemcpy(c->pp_lut, host, (kPpMaxD2 + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice);
-        delete[] host;
-        PSM_CUDA(c, e);
-        PSM_CUDA(c, cudaMalloc(&c->pp_packed, npix * sizeof(uint32_t)));
-        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->dis_pp[v], npix * c->map_bytes));
-    }
-    const bool tuned = c->pp_tuned();
-    const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
-    if (!tuned && !c->pp_plut_valid) {
-        if (!c->pp_plut) {
-            PSM_CUDA(c, cudaMalloc(&c->pp_plut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
-            PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        }
+    // Each buffer is allocated while its own pointer is null and the table is marked valid only once it is on the
+    // device, so a call that failed part-way leaves nothing a launch could trip over: the next call completes the set-up
+    // or fails in turn.
+    PSM_CUDA(c, alloc_if_null(c->pp_lut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
+    PSM_CUDA(c, alloc_if_null(c->pp_packed, npix * sizeof(uint32_t)));
+    for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->dis_pp[v], npix * c->map_bytes));
+    if (!c->pp_lut_valid) {
+        const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
+        PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
         if (!host) return fail(c, PSM_ENOMEM, "out of host memory");
         const int n = pp_weight_table(c->pp_sigma, c->pp_type, host);
         // stream-ordered: a previous frame's filter may still be reading the old table
-        cudaError_t e = cudaMemcpyAsync(c->pp_plut, host, n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
+        cudaError_t e = cudaMemcpyAsync(c->pp_lut, host, n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         delete[] host;
         PSM_CUDA(c, e);
-        c->pp_plut_valid = true;
+        c->pp_lut_valid = true;
     }
+    const bool tuned = c->pp_tuned();
     if (c->p2p_own && c->p2p_seq > 0)
         if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
@@ -1281,7 +1281,7 @@ static int post_process_maps(psm_ctx* c)
             if (tuned)
                 pp_wmf_kernel<T><<<nsm * 8, kPpWarps * 32, 0, c->stream>>>(c->pp_packed, c->pp_lut, c->W, c->H, dst, c->D, steps);
             else
-                generic<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_plut, lut_n, idx_mode,
+                generic<<<(unsigned)pgrid, kPpParamWarps * 32, psmem, c->stream>>>(c->pp_packed, c->pp_lut, lut_n, idx_mode,
                                                                                     c->pp_radius, c->W, c->H, dst);
             PSM_LAUNCH_CHECK(c);
         }

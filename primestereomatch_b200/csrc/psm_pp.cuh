@@ -9,10 +9,10 @@
 // JointWMF computes whenever the feature image has <= 256 distinct 6-bit colours): for every pixel p
 //   out(p) = min { v : sum_{q in window, I_q <= v} w(p,q)  >=  sum_{q in window, I_q > v} w(p,q) }
 // window = (2r+1)^2 clipped at the image border, w = exp(-|c_p - c_q|^2 / (2 s^2)) on the 6-bit colours
-// c = (B,G,R) >> 2, s = 25.5/256*64, held as 2^-22 fixed point (table indexed by the integer squared colour
-// distance, computed on the host with the reference's float expression).  The reference additionally clusters
-// the colours to 256 indices with cv::kmeans (RNG-seeded, un-vendored): parity for natural images is unpinned
-// by the reference itself; this kernel needs no clustering -- it evaluates the weights directly.
+// c = (B,G,R) >> 2, s = 25.5/256*64, held as 2^-22 fixed point: the context's one weight table, built on the host by
+// pp_weight_table (psm_capi.cu) from the reference's float expression; this kernel reads its first kPpLutN entries.  The
+// reference also clusters the colours to 256 indices with cv::kmeans (RNG-seeded, un-vendored): parity for natural
+// images is unpinned by the reference itself; this kernel needs no clustering -- it evaluates the weights directly.
 //
 // GPU mapping (nothing like the reference's serial column scan with necklace tables): one WARP per pixel,
 //   the 361 window taps dealt round-robin to the 32 lanes (12 rounds), each tap one 4-byte load of a packed

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Pin the post-filter restatement (tests/pp_oracle.c) to the reference's OWN include/JointWMF.h at a set of
-psm_set_post_filter settings, without needing the reference at test time.
+"""Pin the post-filter restatement (oracle.post_process, orc_wmf in oracle/stereo_oracle.c) to the reference's OWN
+include/JointWMF.h at a set of psm_set_post_filter settings, without needing the reference at test time.
 
 Needs a checkout of PRiMEStereoMatch (REF, default /root/reference) and a C++ compiler with OpenMP: ref_wmf_driver.cpp
 is compiled against REF/include (JointWMF.h unmodified) and oracle/shim with the flags of oracle/Makefile's _ref build,
@@ -31,7 +31,6 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 from conftest import read_png  # noqa: E402
 from oracle import oracle as O  # noqa: E402
-import pp_oracle as P  # noqa: E402
 
 REF = os.environ.get("REF", "/root/reference")
 
@@ -100,16 +99,16 @@ def main():
         L = ref_lib(tmp)
         for (r, sigma, it, weight) in SETTINGS:
             ent = {"key": key(r, sigma, it, weight), "radius": r, "sigma": float(sigma).hex(), "iterations": it,
-                   "weight": weight, "table_sha": P.table_sha(sigma, weight), "scenes": {}}
+                   "weight": weight, "table_sha": sha(O.weight_table(sigma, weight)), "scenes": {}}
             for name, views in inputs.items():
                 ent["scenes"][name] = {}
                 for view, (img, disp) in views.items():
                     H, W = disp.shape
                     want = np.empty((H, W), np.uint8)
                     n = C.c_int(0)
-                    assert L.ref_wmf(img, np.ascontiguousarray(disp), W, H, r, sigma, it, P.WEIGHTS[weight], want,
+                    assert L.ref_wmf(img, np.ascontiguousarray(disp), W, H, r, sigma, it, O.WEIGHTS[weight], want,
                                      C.byref(n)) == 0
-                    got = P.post_process(img, disp, r, sigma, it, weight)
+                    got = O.post_process(img, disp, r, sigma, it, weight)
                     ent["scenes"][name][view] = {"sha": sha(got), "ref_sha": sha(want), "differ": int((got != want).sum()),
                                                  "colours": n.value}
                     assert n.value <= 256

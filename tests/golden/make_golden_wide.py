@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Pin the 16-bit-map restatements (tests/wide_oracle.c) to the reference's OWN code, without needing the reference at
-test time.
+"""Pin the restatements on 16-bit maps (oracle.wta and oracle.post_process with uint16 maps) to the reference's OWN
+code, without needing the reference at test time.
 
 Needs a checkout of PRiMEStereoMatch (REF, default /root/reference):
   - oracle/_ref (oracle/Makefile target `ref`: src/DispSel.cpp compiled unmodified) for the selection;
@@ -8,11 +8,11 @@ Needs a checkout of PRiMEStereoMatch (REF, default /root/reference):
     oracle/shim with the flags of oracle/Makefile's _ref build, into a temporary directory.
 
 Records (committed as tests/golden/golden_wide.json):
-  wta:  seeded volumes (wide_oracle.argmin_volume) at D in {300, 511, 600, 1024}: the sha256 of DispSel::CVSelect's
-        uchar map, which must equal orc_wta16 & 0xff, and how many arg-mins exceed 255;
+  wta:  seeded volumes (wide_cases.argmin_volume) at D in {300, 511, 600, 1024}: the sha256 of DispSel::CVSelect's
+        uchar map, which must equal the low byte of the u16 orc_wta, and how many arg-mins exceed 255;
   wmf:  posterised Cones / Teddy (<= 256 six-bit colours, so the reference's colour clustering is exact), both views,
-        with wide maps (wide_oracle.widen of the D = 64 maps, values up to 511, max_disp 512): for each setting the sha256
-        of orc_wmf16, of JointWMF::filter on the map as CV_32F with nI = 512, and the number of pixels where they
+        with wide maps (wide_cases.widen of the D = 64 maps, values up to 511, max_disp 512): for each setting the sha256
+        of orc_wmf, of JointWMF::filter on the map as CV_32F with nI = 512, and the number of pixels where they
         differ (the reference's float cut-point search; 0 expected, as at these settings in golden_pp.json);
   loop: JointWMF::filter on the D = 64 maps as CV_32F (nI = 256) against the CV_8U path's hashes in golden_pp.json.
 """
@@ -34,7 +34,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 from conftest import read_png  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from oracle import ref as R  # noqa: E402
-import wide_oracle as WO  # noqa: E402
+from wide_cases import argmin_volume, widen  # noqa: E402
 
 REF = os.environ.get("REF", "/root/reference")
 
@@ -89,7 +89,7 @@ def ref_filter(L, img, disp, r, sigma, it, weight, nI):
     H, W = disp.shape
     out = np.empty((H, W), np.float32)
     n = C.c_int(0)
-    assert L.ref_wmf32f(img, np.ascontiguousarray(disp, np.float32), W, H, r, sigma, nI, it, WO.WEIGHTS[weight], out,
+    assert L.ref_wmf32f(img, np.ascontiguousarray(disp, np.float32), W, H, r, sigma, nI, it, O.WEIGHTS[weight], out,
                         C.byref(n)) == 0
     assert n.value <= 256
     assert np.array_equal(out, np.rint(out)), "the CV_32F path returned a value that is not one of the map's"
@@ -103,8 +103,8 @@ def main():
                                         "seed 7 left / 8 right), max_disp 512", "max_disp": WIDE_MAX_DISP, "settings": []},
            "loop": []}
     for D, W, H, seed in WTA_CASES:
-        vol, _ = WO.argmin_volume(W, H, D, seed)
-        mine = WO.wta16(vol)
+        vol, _ = argmin_volume(W, H, D, seed)
+        mine = O.wta(vol, np.uint16)
         ref8 = R.wta(vol)
         assert np.array_equal((mine & 0xFF).astype(np.uint8), ref8), f"D={D}: low byte differs from DispSel"
         out["wta"].append({"D": D, "W": W, "H": H, "seed": seed, "ref_sha": sha(ref8), "sha16": sha(mine),
@@ -116,8 +116,8 @@ def main():
         l8 = read_png(os.path.join(HERE, f"{s}_im2.png"))
         r8 = read_png(os.path.join(HERE, f"{s}_im6.png"))
         res = O.pipeline(O.u8_to_f32(l8), O.u8_to_f32(r8), 64, threads=8)
-        inputs[name] = {"l": (O.u8_to_f32(posterise(l8)), res["lDis"], WO.widen(res["lDis"], 7)),
-                        "r": (O.u8_to_f32(posterise(r8)), res["rDis"], WO.widen(res["rDis"], 8))}
+        inputs[name] = {"l": (O.u8_to_f32(posterise(l8)), res["lDis"], widen(res["lDis"], 7)),
+                        "r": (O.u8_to_f32(posterise(r8)), res["rDis"], widen(res["rDis"], 8))}
     with open(os.path.join(HERE, "golden_pp.json")) as f:
         gpp = {e["key"]: e for e in json.load(f)["settings"]}
     with tempfile.TemporaryDirectory() as tmp:
@@ -129,7 +129,7 @@ def main():
                 ent["scenes"][name] = {}
                 for view, (img, _, wide) in views.items():
                     want = ref_filter(L, img, wide, r, sigma, it, weight, WIDE_MAX_DISP).astype(np.uint16)
-                    got = WO.post_process16(img, wide, r, sigma, it, weight)
+                    got = O.post_process(img, wide, r, sigma, it, weight)
                     ent["scenes"][name][view] = {"sha": sha(got), "ref_sha": sha(want), "differ": int((got != want).sum()),
                                                  "max": int(got.max())}
             print(ent["key"], {k: [v["differ"] for v in s.values()] for k, s in ent["scenes"].items()}, flush=True)

@@ -1,4 +1,4 @@
-"""GPU: the post-filter at any psm_set_post_filter setting, bit-exact against the CPU restatement tests/pp_oracle.c
+"""GPU: the post-filter at any psm_set_post_filter setting, bit-exact against the CPU restatement oracle.post_process
 (pinned to the reference's JointWMF.h by golden_pp.json).  Every comparison goes through the C-ABI.
 
 Maps are injected through the C-ABI: after CostConst / CostFilter, one-hot cost slices (0 at the wanted disparity, 1
@@ -15,9 +15,10 @@ import pytest
 from conftest import GOLDEN, ROOT
 from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
-import pp_oracle as P
 
 pytestmark = pytest.mark.gpu
+
+DEFAULT = (9, 25.5, 1, "exp")
 
 with open(os.path.join(GOLDEN, "golden_pp.json")) as f:
     GOLD = json.load(f)["settings"]
@@ -64,8 +65,8 @@ def f32(img):
 def check(de, l, r, ld, rd, setting, what):
     r_, sigma, it, weight = setting
     gl, gr = post(de, setting)
-    assert_same(gl, P.post_process(f32(l), ld, r_, sigma, it, weight), f"{what} left")
-    assert_same(gr, P.post_process(f32(r), rd, r_, sigma, it, weight), f"{what} right")
+    assert_same(gl, O.post_process(f32(l), ld, r_, sigma, it, weight), f"{what} left")
+    assert_same(gr, O.post_process(f32(r), rd, r_, sigma, it, weight), f"{what} right")
 
 
 def random_case(W, H, D, seed, u8=False):
@@ -164,8 +165,8 @@ def test_1080p_radius_32_row_band():
         ld, rd = de.lDisMap.copy(), de.rDisMap.copy()
         gl, gr = post(de, (r_, 25.5, 1, "exp"))
     band = 64 + r_        # the clipped window of rows [0, 64) lies inside rows [0, 64 + r)
-    assert_same(gl[:64], P.post_process(l[:band], ld[:band], r_)[:64], "1080p left, top 64 rows")
-    assert_same(gr[:64], P.post_process(r[:band], rd[:band], r_)[:64], "1080p right, top 64 rows")
+    assert_same(gl[:64], O.post_process(l[:band], ld[:band], r_)[:64], "1080p left, top 64 rows")
+    assert_same(gr[:64], O.post_process(r[:band], rd[:band], r_)[:64], "1080p right, top 64 rows")
 
 
 def test_switching_settings_between_frames(full_scenes):
@@ -173,11 +174,11 @@ def test_switching_settings_between_frames(full_scenes):
     with DispEst(l, r, 64) as de:
         inject_maps(de, ld, rd)
         default = post(de, None)
-        assert_same(default[0], P.post_process(l, ld), "default before any setter")
+        assert_same(default[0], O.post_process(l, ld), "default before any setter")
         for setting in ((12, 25.5, 1, "exp"), (12, 60.0, 1, "exp"), (12, 60.0, 1, "iv1"), (4, 60.0, 2, "iv1"),
-                        (9, 25.5, 1, "exp"), (9, 25.5, 2, "exp"), (9, 25.5, 1, "off"), P.DEFAULT):
+                        (9, 25.5, 1, "exp"), (9, 25.5, 2, "exp"), (9, 25.5, 1, "off"), DEFAULT):
             check(de, l, r, ld, rd, setting, f"after switching to {setting}")
-        again = post(de, P.DEFAULT)
+        again = post(de, DEFAULT)
         assert_same(again[0], default[0], "back to the default")
         # a new frame with the same setting reuses the cached table
         assert de.setPostFilter(20, 5.0, 1, "iv2") == 0
@@ -245,8 +246,8 @@ def test_cpp_facade_set_post_filter(tmp_path, scenes, oracle_scene_results):
         rad, sig, it, w = int(setting[0]), float(setting[1]), int(setting[2]), setting[3]
         ld = np.fromfile(tmp_path / "l.u8", np.uint8).reshape(H, W)
         rd = np.fromfile(tmp_path / "r.u8", np.uint8).reshape(H, W)
-        assert_same(ld, P.post_process(l, ref["ld"], rad, sig, it, w), f"C++ facade left at {setting}")
-        assert_same(rd, P.post_process(r, ref["rd"], rad, sig, it, w), f"C++ facade right at {setting}")
+        assert_same(ld, O.post_process(l, ref["ld"], rad, sig, it, w), f"C++ facade left at {setting}")
+        assert_same(rd, O.post_process(r, ref["rd"], rad, sig, it, w), f"C++ facade right at {setting}")
     bad = subprocess.run([exe, str(W), str(H), "64", str(tmp_path / "l.f32"), str(tmp_path / "r.f32"),
                           str(tmp_path / "l.u8"), str(tmp_path / "r.u8"), "8", "0.0001", "0.9", "inf", "inf",
                           "9", "25.5", "1", "cos"], capture_output=True, text=True, timeout=300)

@@ -1,5 +1,5 @@
 """GPU: 16-bit disparity maps (psm_create_u16, max_disp up to 4096), bit for bit through the C-ABI against the CPU
-oracle (oracle/ for the volumes, tests/wide_oracle.c for the arg-min and the post-filter), the stored reference
+oracle (oracle/: the volumes, the arg-min and the post-filter on u16 maps), the stored reference
 results of golden_wide.json and the u8 contexts at D <= 256."""
 import ctypes as C
 import hashlib
@@ -14,7 +14,7 @@ from conftest import GOLDEN, ROOT
 from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
 from primestereomatch_b200.sharding import shard_range
-import wide_oracle as WO
+from wide_cases import argmin_volume, widen
 
 pytestmark = pytest.mark.gpu
 
@@ -56,7 +56,7 @@ def inject_maps(de, ld, rd):
 def oracle_maps(l, r, D):
     _, _, lraw, rraw = O.cost_const(l, r, D)
     lf, rf = O.cost_filter(l, r, lraw, rraw)
-    return lf, rf, WO.wta16(lf), WO.wta16(rf)
+    return lf, rf, O.wta(lf, np.uint16), O.wta(rf, np.uint16)
 
 
 # ---- 1. same maps as a u8 context at D <= 256 -------------------------------------------------------------------------
@@ -104,7 +104,7 @@ def test_default_map_bits_follow_maxdis():
 @pytest.mark.parametrize("case", GOLD["wta"], ids=lambda c: f"D{c['D']}")
 def test_selection_low_byte_is_the_stored_reference(case):
     D, W, H = case["D"], case["W"], case["H"]
-    vol, _ = WO.argmin_volume(W, H, D, case["seed"])
+    vol, _ = argmin_volume(W, H, D, case["seed"])
     l, r, _ = synth.stereo_pair_f32(W, H, 8)
     with DispEst(l, r, D) as de:
         de.CostConst_GPU(); de.CostFilter_GPU()
@@ -114,7 +114,7 @@ def test_selection_low_byte_is_the_stored_reference(case):
         assert sha((de.lDisMap & 0xFF).astype(np.uint8)) == case["ref_sha"]
         assert sha(de.lDisMap) == case["sha16"] and int(de.lDisMap.max()) > 255
         rv = np.concatenate([vol[:1], vol[:0:-1]])
-        assert_same(de.rDisMap, WO.wta16(rv), "right view")
+        assert_same(de.rDisMap, O.wta(rv, np.uint16), "right view")
 
 
 def band_crop(W, D):
@@ -161,7 +161,7 @@ def test_ragged_sizes(W, H, D):
         de.CostConst_GPU(); de.CostFilter_GPU(); de.DispSelect_GPU()
         assert_same(de.lDisMap, ld, f"{W}x{H}x{D} left"); assert_same(de.rDisMap, rd, f"{W}x{H}x{D} right")
         de.PostProcess_GPU()
-        assert_same(de.lDisMap, WO.post_process16(l, ld), f"{W}x{H}x{D} post-filtered left")
+        assert_same(de.lDisMap, O.post_process(l, ld), f"{W}x{H}x{D} post-filtered left")
 
 
 # ---- 4. with the other per-context settings ---------------------------------------------------------------------------
@@ -182,7 +182,7 @@ def test_settings_and_fgf(stage):
             assert_same(la[d], b.read_cost_slice(0, d), f"{stage} left slice {d}")
             assert_same(ra[d], b.read_cost_slice(1, d), f"{stage} right slice {d}")
         a.DispSelect_GPU()
-        assert_same(a.lDisMap, WO.wta16(la), f"{stage} left"); assert_same(a.rDisMap, WO.wta16(ra), f"{stage} right")
+        assert_same(a.lDisMap, O.wta(la, np.uint16), f"{stage} left"); assert_same(a.rDisMap, O.wta(ra, np.uint16), f"{stage} right")
         if stage == "fgf":
             _, _, lraw, rraw = O.cost_const(l, r, D)
             lf, _ = O.cost_filter_fgf(l, r, lraw, rraw, s=4)
@@ -195,7 +195,7 @@ def wide_scenes(scenes, oracle_scene_results):
     out = {}
     for name, (l8, r8, _, _) in scenes.items():
         res = oracle_scene_results[name]
-        out[name] = (O.u8_to_f32(posterise(l8)), O.u8_to_f32(posterise(r8)), WO.widen(res["ld"], 7), WO.widen(res["rd"], 8))
+        out[name] = (O.u8_to_f32(posterise(l8)), O.u8_to_f32(posterise(r8)), widen(res["ld"], 7), widen(res["rd"], 8))
     return out
 
 
@@ -221,8 +221,8 @@ def test_post_filter_every_radius_iterations_and_switching(wide_scenes):
                        [(9, 25.5, 16, "exp"), (6, 7.0, 16, "iv2"), (9, 25.5, 1, "off"), (12, 60.0, 2, "iv1"), (9, 25.5, 1, "exp")]:
             de.setPostFilter(*setting)
             de.DispSelect_GPU(); de.PostProcess_GPU()
-            assert_same(de.lDisMap, WO.post_process16(l, ld, *setting), f"left at {setting}")
-            assert_same(de.rDisMap, WO.post_process16(r, rd, *setting), f"right at {setting}")
+            assert_same(de.lDisMap, O.post_process(l, ld, *setting), f"left at {setting}")
+            assert_same(de.rDisMap, O.post_process(r, rd, *setting), f"right at {setting}")
 
 
 # ---- 6. sharded -------------------------------------------------------------------------------------------------------
@@ -394,4 +394,4 @@ def test_cpp_demo_at_d300(tmp_path):
     got_l = np.fromfile(tmp_path / "l.u16", np.uint16).reshape(H, W)
     got_r = np.fromfile(tmp_path / "r.u16", np.uint16).reshape(H, W)
     assert int(ld.max()) > 255
-    assert_same(got_l, WO.post_process16(l, ld), "C++ demo left"); assert_same(got_r, WO.post_process16(r, rd), "C++ demo right")
+    assert_same(got_l, O.post_process(l, ld), "C++ demo left"); assert_same(got_r, O.post_process(r, rd), "C++ demo right")

@@ -1,6 +1,6 @@
-"""CPU: the post-filter restatement at any psm_set_post_filter setting (tests/pp_oracle.c) against the reference's own
-JointWMF.h as recorded in tests/golden/golden_pp.json (make_golden_pp.py), against the existing restatement orc_wmf at
-the default, and against hand-checkable cases of the definition (DESIGN.md section 13)."""
+"""CPU: the post-filter restatement at any psm_set_post_filter setting (oracle.post_process, orc_wmf in
+oracle/stereo_oracle.c) against the reference's own JointWMF.h as recorded in tests/golden/golden_pp.json
+(make_golden_pp.py) and ref_outputs.json, and against hand-checkable cases of the definition (DESIGN.md section 13)."""
 import hashlib
 import json
 import os
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
-import pp_oracle as P
+from oracle import oracle as O
 
 
 def sha(a):
@@ -50,12 +50,12 @@ def test_golden_covers_the_settings():
 @pytest.mark.parametrize("ent", GOLD, ids=[e["key"] for e in GOLD])
 def test_restatement_matches_golden(ent, pp_inputs):
     r, sigma, it, weight = setting(ent)
-    assert P.table_sha(sigma, weight) == ent["table_sha"]
+    assert sha(O.weight_table(sigma, weight)) == ent["table_sha"]
     for name, views in pp_inputs.items():
         for view, (img, disp) in views.items():
             want = ent["scenes"][name][view]
             assert want["colours"] <= 256       # every colour is its own cluster: the reference's result is RNG-free
-            got = P.post_process(img, disp, r, sigma, it, weight)
+            got = O.post_process(img, disp, r, sigma, it, weight)
             assert sha(got) == want["sha"], f"{ent['key']} {name}/{view}"
             # the reference's float cut-point search agrees exactly, or differs by the count its float balances give
             assert (want["differ"] == 0) == (want["ref_sha"] == want["sha"])
@@ -74,31 +74,15 @@ def test_reference_agreement_counts():
             assert all(v["differ"] <= 25 for s in e["scenes"].values() for v in s.values()), e["key"]
 
 
-def test_default_equals_orc_wmf_and_reference(pp_inputs, oracle):
+def test_default_equals_reference(pp_inputs):
+    """The default call is PP::processDM's filter and gives the reference's own JointWMF results (ref_outputs.json)."""
     with open(os.path.join(GOLDEN, "ref_outputs.json")) as f:
         ref_pp = json.load(f)["pp"]
-    assert np.array_equal(P.weight_table(), np.asarray(_orc_table(oracle)))
     for name, views in pp_inputs.items():
         for view, (img, disp) in views.items():
-            got = P.post_process(img, disp)
-            assert np.array_equal(got, oracle.post_process(img, disp))
+            got = O.post_process(img, disp)
+            assert np.array_equal(got, O.post_process(img, disp, 9, 25.5, 1, "exp"))   # PP::processDM's arguments
             assert sha(got) == ref_pp[name][view]["sha"]
-
-
-def _orc_table(oracle):
-    import ctypes as C
-    t = np.zeros(3 * 63 * 63 + 1, np.uint32)
-    L = oracle.lib()
-    L.orc_pp_weight_lut.argtypes = [np.ctypeslib.ndpointer(dtype=np.uint32, flags="C_CONTIGUOUS")]
-    L.orc_pp_weight_lut.restype = None
-    L.orc_pp_weight_lut(t)
-    return t
-
-
-def test_default_on_natural_images_equals_orc_wmf(scenes, oracle, oracle_scene_results):
-    _, _, l, _ = scenes["Teddy"]
-    ld = oracle_scene_results["Teddy"]["ld"]
-    assert np.array_equal(P.post_process(l, ld), oracle.post_process(l, ld))
 
 
 def lower_median(disp, y, x, r):
@@ -112,7 +96,7 @@ def test_off_is_the_plain_lower_median_of_the_clipped_window(r):
     H, W = 23, 41
     img = rng.random((H, W, 3)).astype(np.float32)
     disp = rng.integers(0, 200, (H, W)).astype(np.uint8)
-    got = P.post_process(img, disp, r, 25.5, 1, "off")
+    got = O.post_process(img, disp, r, 25.5, 1, "off")
     for y in range(H):
         for x in range(W):
             assert got[y, x] == lower_median(disp, y, x, r), (y, x)
@@ -123,9 +107,9 @@ def test_two_iterations_equal_two_single_passes(weight):
     rng = np.random.default_rng(7)
     img = (rng.integers(0, 4, (40, 57, 3)) / 3.0).astype(np.float32)
     disp = rng.integers(0, 64, (40, 57)).astype(np.uint8)
-    once = P.post_process(img, disp, 5, 12.0, 1, weight)
-    twice = P.post_process(img, once, 5, 12.0, 1, weight)
-    assert np.array_equal(P.post_process(img, disp, 5, 12.0, 2, weight), twice)
+    once = O.post_process(img, disp, 5, 12.0, 1, weight)
+    twice = O.post_process(img, once, 5, 12.0, 1, weight)
+    assert np.array_equal(O.post_process(img, disp, 5, 12.0, 2, weight), twice)
     assert not np.array_equal(once, disp)
 
 
@@ -135,11 +119,11 @@ def test_radius_at_least_the_image_gives_whole_image_windows(weight):
     H, W = 9, 13
     img = rng.random((H, W, 3)).astype(np.float32)
     disp = rng.integers(0, 30, (H, W)).astype(np.uint8)
-    got = P.post_process(img, disp, 13, 25.5, 1, weight)
-    assert np.array_equal(got, P.post_process(img, disp, 32, 25.5, 1, weight))
+    got = O.post_process(img, disp, 13, 25.5, 1, weight)
+    assert np.array_equal(got, O.post_process(img, disp, 32, 25.5, 1, weight))
     # direct evaluation over every pixel of the image
-    c = (P.to_u8x255(img) >> 2).astype(np.int64).reshape(-1, 3)
-    t = P.weight_table(25.5, weight).astype(np.int64)
+    c = (O.to_u8x255(img) >> 2).astype(np.int64).reshape(-1, 3)
+    t = O.weight_table(25.5, weight).astype(np.int64)
     d = disp.reshape(-1).astype(np.int64)
     for p in range(H * W):
         diff = c - c[p]
@@ -154,7 +138,7 @@ def test_radius_at_least_the_image_gives_whole_image_windows(weight):
 @pytest.mark.parametrize("sigma", [2.0 ** -16, 2.0 ** 16])
 @pytest.mark.parametrize("weight", ["exp", "iv1", "iv2", "off"])
 def test_tables_at_the_sigma_ends_are_finite_with_unit_centre(sigma, weight):
-    t = P.weight_table(sigma, weight)
+    t = O.weight_table(sigma, weight)
     assert t[0] == 2 ** 22 and t.max() == 2 ** 22
     # the float weights behind the table: finite, w(0) > 0 and normal
     s = np.float32(sigma) / np.float32(256.0) * np.float32(64)
@@ -173,6 +157,6 @@ def test_tables_at_the_sigma_ends_are_finite_with_unit_centre(sigma, weight):
 
 def test_default_table_is_the_truncated_one():
     """exp at 25.5: the table is zero beyond d^2 = 1295, the prefix the tuned kernel keeps."""
-    t = P.weight_table()
+    t = O.weight_table()
     assert len(t) == 11908 and t[1295] > 0 and not t[1296:].any()
-    assert P.weight_table(2.0 ** 16, "iv2").min() > 0        # no truncation applies away from the default
+    assert O.weight_table(2.0 ** 16, "iv2").min() > 0        # no truncation applies away from the default

@@ -1,5 +1,6 @@
-"""CPU: the 16-bit-map restatements (tests/wide_oracle.c) against the reference's own code through golden_wide.json
-(written by tests/golden/make_golden_wide.py), and the streaming filter's work decomposition at up to 4096 slices."""
+"""CPU: the restatements on 16-bit maps (oracle.wta and oracle.post_process with uint16 maps) against the reference's own
+code through golden_wide.json (written by tests/golden/make_golden_wide.py), and the streaming filter's work
+decomposition at up to 4096 slices."""
 import hashlib
 import json
 import os
@@ -9,8 +10,8 @@ import pytest
 
 from conftest import GOLDEN
 from primestereomatch_b200 import capi
-import pp_oracle as P
-import wide_oracle as WO
+from oracle import oracle as O
+from wide_cases import argmin_volume, widen
 
 with open(os.path.join(GOLDEN, "golden_wide.json")) as f:
     GOLD = json.load(f)
@@ -28,8 +29,8 @@ def posterise(img8, masks=(0xE0, 0xE0, 0xC0)):
 
 @pytest.mark.parametrize("case", GOLD["wta"], ids=lambda c: f"D{c['D']}")
 def test_wta16_low_byte_is_the_reference_dispsel(case):
-    vol, want = WO.argmin_volume(case["W"], case["H"], case["D"], case["seed"])
-    got = WO.wta16(vol)
+    vol, want = argmin_volume(case["W"], case["H"], case["D"], case["seed"])
+    got = O.wta(vol, np.uint16)
     assert sha((got & 0xFF).astype(np.uint8)) == case["ref_sha"]
     assert sha(got) == case["sha16"]
     assert int((got > 255).sum()) == case["above_255"] > 0
@@ -42,10 +43,9 @@ def test_wta16_low_byte_is_the_reference_dispsel(case):
 def test_wta16_definition():
     rng = np.random.default_rng(0)
     vol = rng.integers(0, 5, (700, 6, 9)).astype(np.float32)               # many exact ties
-    got = WO.wta16(vol)
+    got = O.wta(vol, np.uint16)
     c = vol[1:].reshape(699, -1)
     assert np.array_equal(got.reshape(-1), 1 + np.argmin(c, axis=0))        # numpy's argmin: first minimum
-    assert np.array_equal(WO.wta16(vol[:64]).astype(np.uint8), __import__("oracle.oracle", fromlist=["wta"]).wta(vol[:64]))
 
 
 @pytest.fixture(scope="module")
@@ -53,8 +53,8 @@ def wide_inputs(scenes, oracle_scene_results, oracle):
     out = {}
     for name, (l8, r8, _, _) in scenes.items():
         res = oracle_scene_results[name]
-        out[name] = {"l": (oracle.u8_to_f32(posterise(l8)), res["ld"], WO.widen(res["ld"], 7)),
-                     "r": (oracle.u8_to_f32(posterise(r8)), res["rd"], WO.widen(res["rd"], 8))}
+        out[name] = {"l": (oracle.u8_to_f32(posterise(l8)), res["ld"], widen(res["ld"], 7)),
+                     "r": (oracle.u8_to_f32(posterise(r8)), res["rd"], widen(res["rd"], 8))}
     return out
 
 
@@ -65,7 +65,7 @@ def test_wmf16_against_jointwmf_cv32f(ent, wide_inputs):
         for view, (img, _, wide) in views.items():
             g = ent["scenes"][name][view]
             assert wide.max() > 255
-            got = WO.post_process16(img, wide, *setting)
+            got = O.post_process(img, wide, *setting)
             assert sha(got) == g["sha"], f"{name} {view}"
             assert int(got.max()) == g["max"] > 255
             # the reference's float cut-point search disagrees on a few near-tie pixels (DESIGN.md section 13); exact at
@@ -86,9 +86,12 @@ def test_cv32f_path_equals_cv8u_path_on_existing_goldens():
 
 @pytest.mark.parametrize("setting", [(9, 25.5, 1, "exp"), (4, 10.0, 2, "iv1"), (13, 3.0, 1, "iv2"), (2, 25.5, 3, "off")])
 def test_wmf16_equals_the_u8_restatement_on_u8_maps(setting, wide_inputs):
+    """The same map given as u8 and as u16 gives the same values."""
     img, d8, _ = wide_inputs["Teddy"]["l"]
     img, d8 = img[:90, :140], d8[:90, :140]
-    assert np.array_equal(WO.post_process16(img, d8, *setting), P.post_process(img, d8, *setting))
+    got8, got16 = O.post_process(img, d8, *setting), O.post_process(img, d8.astype(np.uint16), *setting)
+    assert got8.dtype == np.uint8 and got16.dtype == np.uint16
+    assert np.array_equal(got16, got8.astype(np.uint16)) and not np.array_equal(got8, d8)
 
 
 def test_wmf16_is_shift_and_scale_equivariant():
@@ -96,8 +99,8 @@ def test_wmf16_is_shift_and_scale_equivariant():
     rng = np.random.default_rng(4)
     img = rng.random((40, 50, 3)).astype(np.float32)
     d = rng.integers(0, 300, (40, 50)).astype(np.uint16)
-    base = WO.post_process16(img, d, 5, 25.5, 1, "exp")
-    assert np.array_equal(WO.post_process16(img, d * 13 + 5, 5, 25.5, 1, "exp"), base * 13 + 5)
+    base = O.post_process(img, d, 5, 25.5, 1, "exp")
+    assert np.array_equal(O.post_process(img, d * 13 + 5, 5, 25.5, 1, "exp"), base * 13 + 5)
 
 
 def stored_columns(plan, W, strip=112):
