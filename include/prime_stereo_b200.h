@@ -28,10 +28,18 @@
  * full-resolution guided filter) and src/DispSel.cpp bit for bit -- NOT the divergent OpenCL kernels (SURVEY.md section
  * 2.1), and NOT what the reference binary's CPU mode runs today: StereoMatch::compute calls CostFilter_FGF (the
  * sub-sampled Fast Guided Filter) because the CostFilter_CPU that would call GuidedFilter_cv is declared but never
- * defined; that branch is psm_cost_filter_fgf.  "Bit for bit" for the box filters means: fp64 sums of 64 floats are
- * exact -- and therefore independent of summation order -- unless a window spans more than 2^23 in magnitude; beyond that
- * OpenCV's order and this library's round differently in fp64 and the final float can differ in its last bit with
- * probability ~2^-28 per mean (never observed).  PSM_CVF_MIXED trades the bit-exact q for speed inside the tolerance
+ * defined; that branch is psm_cost_filter_fgf.  "Bit for bit" for the box filters: cv::boxFilter keeps running fp64
+ * sums along every row and down every column, so a rounding error, an inf or a NaN that enters one stays in it for the
+ * rest of the row or column.  The tuned kernels sum in other orders and equal the reference while every fp64 sum is
+ * exact.  Outside that domain, in OpenCV's order and bit for bit: every slice psm_write_cost_slice received with a
+ * negative, -0, inf, NaN or >= 2^63 cost, every slice of a view whose image holds a negative, -0, inf, NaN or >= 2^61
+ * value or whose solve terms are not finite, the guide of a view with a nonzero channel value outside [2^-12, 1], and
+ * everything in PSM_CVF_NAIVE.  That pass is slow (one thread per row, then per column) and needs 48 bytes of scratch
+ * per pixel, allocated on first use; u8 frames at the default window never take or allocate it.  Costs written
+ * directly into the device volumes (psm_device_ptr) are not inspected.  Finite, non-negative costs whose window sums
+ * are not exact (a magnitude range of more than ~2^29 in one row or column, such as a band of 1e15 above costs near
+ * 1e-3) keep the tuned order: there q differs from the reference by up to the fp64 rounding the running sums carry,
+ * which can be far more than one ulp of a small mean.  PSM_CVF_MIXED trades the bit-exact q for speed inside the tolerance
  * the task states (a, b bit-exact, |dq| <= 4e-6 on O(1) costs).  See DESIGN.md.
  *
  * Threading: one psm_ctx must not be used concurrently; it may be used from different
@@ -79,7 +87,7 @@ enum {
     PSM_CVF_MIXED = 1, /* the tolerance mode north_star allows for fp32: first box stage fp64 (a, b bit-exact), second
                           box stage fp32 with a fixed summation tree: q within ~3e-6 of EXACT, deterministic
                           (tests/mixed_model.py restates it on the CPU); same maps as EXACT on every tested frame */
-    PSM_CVF_NAIVE = 2  /* unfused two-pass direct 64-tap fp64 kernels: slow device-side cross-check */
+    PSM_CVF_NAIVE = 2  /* every slice in OpenCV's own summation order (psm_cvf_ref.cuh): slow device-side reference */
 };
 
 /* Diagnostic, needs no device: the work decomposition the streaming guided-filter kernel would use for a W x H x d_count

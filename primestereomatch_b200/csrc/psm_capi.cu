@@ -13,6 +13,7 @@
 
 #include "psm_cvf_stream.cuh"
 #include "psm_cvf_window.cuh"
+#include "psm_cvf_ref.cuh"
 #include "psm_pp.cuh"
 #include "psm_pp_param.cuh"
 #include "psm_fgf.cuh"
@@ -70,8 +71,12 @@ struct psm_ctx {
     int p2p_sync = 1;                       // 1: device-side ARRIVE/DONE flags; 0: the caller separates the kernels by its own barriers
     float* alloc[16] = {};                  // raw cudaMalloc pointers behind the halo-offset pointers above
     int nalloc = 0;
-    float* ab = nullptr;                    // naive-mode scratch [4][d_count][H][Wp], lazy
-    size_t ab_slices = 0;
+    int* slice_flags = nullptr;             // [2][d_count] device flags: slices the reference-order pass filters again
+    bool slices_flagged = false;            // some slice flag is set (psm_write_cost_slice found a special cost)
+    bool float_images = false;              // the current images came in as floats: the ingest flags may be set
+    double* ref_rs = nullptr;               // reference-order scratch (psm_cvf_ref.cuh): [4][H][W] row sums, lazy
+    float* ref_pl = nullptr;                // ... and [4][H][W] float planes
+    int ref_blocks = 0;                     // grid of the cooperative reference-order kernels
     cudaEvent_t ev0[kNumStages] = {}, ev1[kNumStages] = {};
     bool ev_valid[kNumStages] = {};
     int cvf_mode = PSM_CVF_EXACT, gray_mode = 0, timing = 1, cvf_variant = 0, cvf_target_rows = 0, cvf_extra_smem = 0, cvf_threads = 0, cvf_remap = 0, cvf_no_pack = 0, cvc_variant = 0, guide_seg_rows = 0, cvc_chunk = 0;
@@ -180,6 +185,7 @@ int ingest(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool 
         if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
     }
     c->have_images = true;
+    c->float_images = sizeof(T) != 1;   // u8 images lie in {0} U [1/255, 1]: they never raise an ingest flag
     c->guide_valid = false;
     c->have_cvc = false;
     c->filtered = false;
@@ -209,12 +215,66 @@ int upload_async(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep)
     return PSM_OK;
 }
 
+int launch_guide(psm_ctx* c);
+
+// the raw volumes were replaced or filtered: no slice is flagged any more
+int clear_slice_flags(psm_ctx* c)
+{
+    if (!c->slices_flagged) return PSM_OK;
+    PSM_CUDA(c, cudaMemsetAsync(c->slice_flags, 0, 2 * (size_t)c->d_count * sizeof(int), c->stream));
+    c->slices_flagged = false;
+    return PSM_OK;
+}
+
+// The cooperative reference-order kernels (psm_cvf_ref.cuh): scratch of one slice (48 bytes per pixel, allocated on the
+// first launch) and a grid that fits on the device at once.
+int launch_ref(psm_ctx* c, void* kernel, int mode, int one_view = 0, int one_d = 0)
+{
+    const size_t n = (size_t)c->W * c->H;
+    PSM_CUDA(c, alloc_if_null(c->ref_rs, 4 * n * sizeof(double)));
+    PSM_CUDA(c, alloc_if_null(c->ref_pl, 4 * n * sizeof(float)));
+    if (c->ref_blocks == 0) {
+        int nsm = 0, per_sm = 0;
+        PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
+        PSM_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cvf_ref_kernel, kRefThreads, 0));
+        int per_sm_g = 0;
+        PSM_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_g, guide_ref_kernel, kRefThreads, 0));
+        c->ref_blocks = nsm * std::min(2, std::min(per_sm, per_sm_g));
+    }
+    RefParams P;
+    for (int v = 0; v < 2; ++v) { P.vol_in[v] = c->vol[v]; P.vol_out[v] = c->vol_alt[v]; P.guide[v] = c->guide[v]; }
+    P.guide_flags = c->guide_flags;
+    P.slice_flags = c->slice_flags;
+    P.rs = c->ref_rs; P.pl = c->ref_pl;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->d_count;
+    P.K = c->gif_win; P.a = c->gif_win / 2;
+    P.scale = 1.0 / ((double)P.K * P.K);
+    P.eps = c->gif_eps;
+    P.mode = mode; P.one_view = one_view; P.one_d = one_d;
+    void* args[] = {&P};
+    PSM_CUDA(c, cudaLaunchCooperativeKernel(kernel, dim3(c->ref_blocks), dim3(kRefThreads), args, 0, c->stream));
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
 int ensure_guide(psm_ctx* c)
 {
     if (c->guide_valid) return PSM_OK;
+    if (int rc = launch_guide(c)) return rc;
+    // a view whose ingest found values outside {0} U [2^-12, 1] gets its guide again in OpenCV's order (the kernel
+    // leaves at once when no view is flagged; u8 images never are)
+    if (c->float_images)
+        if (int rc = launch_ref(c, (void*)guide_ref_kernel, kRefFlagged)) return rc;
+    c->guide_valid = true;
+    return PSM_OK;
+}
+
+int launch_guide(psm_ctx* c)
+{
     if (!c->gif_default()) {   // any other window / eps: the generic precompute (psm_cvf_window.cuh)
         WinGuideParams P;
         P.guide[0] = c->guide[0]; P.guide[1] = c->guide[1];
+        P.guide_flags = c->guide_flags;
         P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.K = c->gif_win; P.a = c->gif_win / 2;
         P.seg_rows = kWinGuideSegRows;
         P.scale = 1.0 / ((double)P.K * P.K);
@@ -222,7 +282,6 @@ int ensure_guide(psm_ctx* c)
         dim3 grd((c->W + 127) / 128, (c->H + P.seg_rows - 1) / P.seg_rows, 2);
         guide_window_kernel<<<grd, 128, 0, c->stream>>>(P);
         PSM_LAUNCH_CHECK(c);
-        c->guide_valid = true;
         return PSM_OK;
     }
     GuideParams P;
@@ -235,18 +294,9 @@ int ensure_guide(psm_ctx* c)
     const int tasks = 2 * P.nstrips * P.nseg;  // one warp each
     guide_kernel<<<(tasks + 3) / 4, 128, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
-    c->guide_valid = true;
     return PSM_OK;
 }
 
-int ensure_ab(psm_ctx* c, size_t slices)
-{
-    if (c->ab && c->ab_slices >= slices) return PSM_OK;
-    if (c->ab) { cudaFree(c->ab); c->ab = nullptr; c->ab_slices = 0; }
-    PSM_CUDA(c, cudaMalloc(&c->ab, 4 * slices * c->plane * sizeof(float)));
-    c->ab_slices = slices;
-    return PSM_OK;
-}
 
 // Row segmentation of the streaming kernel: segments are multiples of 8 rows, >= 16 rows, and the
 // last one keeps >= 8 rows so that only the first/last segment ever sees a reflected row.
@@ -534,6 +584,8 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
         PSM_CREATE_CUDA(cudaMemsetAsync(c->dis[v], 0, (size_t)c->W * c->H * map_bytes, c->stream));
     }
     PSM_CREATE_CUDA(cudaMalloc(&c->guide_flags, 2 * sizeof(int)));
+    PSM_CREATE_CUDA(cudaMalloc(&c->slice_flags, 2 * (size_t)c->d_count * sizeof(int)));
+    PSM_CREATE_CUDA(cudaMemsetAsync(c->slice_flags, 0, 2 * (size_t)c->d_count * sizeof(int), c->stream));
     PSM_CREATE_CUDA(cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
     PSM_CREATE_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->up_done, cudaEventDisableTiming));
@@ -593,7 +645,9 @@ int psm_destroy(psm_ctx* c)
     if (c->up_done) cudaEventDestroy(c->up_done);
     for (int k = 0; k < 2; ++k) if (c->ingest_done[k]) cudaEventDestroy(c->ingest_done[k]);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-    cudaFree(c->ab);
+    cudaFree(c->slice_flags);
+    cudaFree(c->ref_rs);
+    cudaFree(c->ref_pl);
     cudaFree(c->guide_flags);
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
@@ -807,6 +861,7 @@ int psm_cost_const(psm_ctx* c)
             for (int v = 0; v < 2; ++v)
                 if (int rc = pad_rows(c, c->vol[v], (size_t)c->d_count * c->H)) return rc;
     }
+    if (int rc = clear_slice_flags(c)) return rc;
     c->have_cvc = true;
     c->filtered = false;
     return stage_end(c, 1);
@@ -822,35 +877,20 @@ int psm_cost_filter(psm_ctx* c)
                     c->gif_win, (double)c->gif_eps);
     if (int rc = stage_begin(c, 2)) return rc;
     if (int rc = ensure_guide(c)) return rc;
-    if (!c->gif_default()) {
-        if (int rc = stage_begin(c, 4)) return rc;
-        if (int rc = launch_cvf_window(c)) return rc;
-        if (int rc = stage_end(c, 4)) return rc;
-        for (int v = 0; v < 2; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
-        c->have_cvc = false;
-        c->filtered = true;
-        return stage_end(c, 2);
-    }
-    const bool tiny = c->W < 16 || c->H < 16;
-    if (c->cvf_mode == PSM_CVF_NAIVE || tiny) {
-        if (int rc = ensure_ab(c, (size_t)c->d_count)) return rc;
-        if (int rc = stage_begin(c, 4)) return rc;
-        for (int v = 0; v < 2; ++v) {
-            dim3 blk(128), grd((c->W + 127) / 128, c->H, c->d_count);
-            cvf_naive_ab_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->guide[v], c->plane, c->W, c->H, c->Wp,
-                                                          c->d_count, c->ab);
-            PSM_LAUNCH_CHECK(c);
-            cvf_naive_q_kernel<<<grd, blk, 0, c->stream>>>(c->ab, c->guide[v], c->plane, c->W, c->H, c->Wp,
-                                                         c->d_count, c->vol_alt[v]);
-            PSM_LAUNCH_CHECK(c);
-        }
-        if (int rc = stage_end(c, 4)) return rc;
+    if (int rc = stage_begin(c, 4)) return rc;
+    // NAIVE and images below one strip: every slice in OpenCV's order.  Otherwise the tuned kernel, then, in OpenCV's
+    // order, the slices psm_write_cost_slice flagged and every slice of a view whose image is outside the integer domain
+    // or whose solve terms are not finite (psm_cvf_ref.cuh).  The second launch is needed only where a flag can be set:
+    // flagged slices, float images, a non-default window or eps.  u8 frames at the defaults run the tuned kernel alone.
+    if (c->gif_default() && (c->cvf_mode == PSM_CVF_NAIVE || c->W < 16 || c->H < 16)) {
+        if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAll)) return rc;
     } else {
-        if (int rc = stage_begin(c, 4)) return rc;
-        int rc = launch_cvf_stream(c);
-        if (rc) return rc;
-        if (int rc2 = stage_end(c, 4)) return rc2;
+        if (int rc = c->gif_default() ? launch_cvf_stream(c) : launch_cvf_window(c)) return rc;
+        if (c->slices_flagged || c->float_images || !c->gif_default())
+            if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefFlagged)) return rc;
     }
+    if (int rc = clear_slice_flags(c)) return rc;
+    if (int rc = stage_end(c, 4)) return rc;
     for (int v = 0; v < 2; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
     c->have_cvc = false;  // the volumes now hold filtered costs; filtering again needs a new CVC
     c->filtered = true;
@@ -1346,6 +1386,20 @@ int psm_write_cost_slice(psm_ctx* c, int view, int d, const float* src, size_t s
     PSM_CUDA(c, cudaMemcpy2DAsync(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->Wp * sizeof(float), src,
                                   src_step, c->W * sizeof(float), c->H, cudaMemcpyHostToDevice, c->stream));
     if (int rc = pad_rows(c, c->vol[view] + (size_t)(d - c->d_begin) * c->plane, (size_t)c->H)) return rc;
+    // A negative, -0, inf, NaN or >= 2^63 cost (bit patterns >= that of 2^63; the sign bit sorts last) makes the fp64 box
+    // sums order-dependent: flag the slice for the reference-order pass.  psm_cost_const never produces one from images
+    // without kGuideOutside, so this is the only other way such a cost enters a volume.
+    bool special = false;
+    for (int y = 0; y < c->H && !special; ++y) {
+        const uint32_t* row = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(src) + (size_t)y * src_step);
+        for (int x = 0; x < c->W; ++x) special |= row[x] >= 0x5f000000u;
+    }
+    if (special) {
+        static const int one = 1;
+        PSM_CUDA(c, cudaMemcpyAsync(c->slice_flags + (size_t)view * c->d_count + (d - c->d_begin), &one, sizeof(int),
+                                    cudaMemcpyHostToDevice, c->stream));
+        c->slices_flagged = true;
+    }
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     c->have_cvc = true;  // caller-provided raw costs may be filtered
     return PSM_OK;
@@ -1378,23 +1432,11 @@ int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
     if (!a3 || !b) return fail(c, PSM_EINVAL, "null output");
     if (!c->have_images) return fail(c, PSM_ESTATE, "no images set");
     if (int rc = ensure_guide(c)) return rc;
-    if (int rc = ensure_ab(c, 1)) return rc;
-    dim3 blk(128), grd((c->W + 127) / 128, c->H, 1);
-    if (!c->gif_default())
-        ab_window_kernel<<<grd, blk, 0, c->stream>>>(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->guide[view], c->plane,
-                                                     c->W, c->H, c->Wp, c->gif_win, c->gif_win / 2,
-                                                     1.0 / ((double)c->gif_win * c->gif_win), c->ab);
-    else
-        cvf_naive_ab_kernel<<<grd, blk, 0, c->stream>>>(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->guide[view],
-                                                      c->plane, c->W, c->H, c->Wp, 1, c->ab);
-    PSM_LAUNCH_CHECK(c);
-    const size_t wb = c->W * sizeof(float);
-    // scratch is laid out [4][ab_slices][plane]; only slice 0 of each plane group was written with nslices=1
-    for (int k = 0; k < 4; ++k) {
-        float* dst = k < 3 ? a3 + (size_t)k * c->W * c->H : b;
-        PSM_CUDA(c, cudaMemcpy2DAsync(dst, wb, c->ab + (size_t)k * c->plane, c->Wp * sizeof(float), wb, c->H,
-                                      cudaMemcpyDeviceToHost, c->stream));
-    }
+    // a, b in OpenCV's order (psm_cvf_ref.cuh), left in the scratch planes [4][H][W]
+    if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->d_begin)) return rc;
+    const size_t n = (size_t)c->W * c->H;
+    PSM_CUDA(c, cudaMemcpyAsync(a3, c->ref_pl, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    PSM_CUDA(c, cudaMemcpyAsync(b, c->ref_pl + 3 * n, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }

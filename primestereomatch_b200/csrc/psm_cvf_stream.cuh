@@ -6,10 +6,10 @@
 // passes per slice for the same result (SURVEY.md section 8a, row a9).
 //
 // Numerics
-//   * cv::boxFilter on CV_32F accumulates in double; an fp64 sum of 64 floats is exact unless the
-//     window spans > 2^23 in magnitude, so any summation order gives the same float after the one
-//     final rounding.  Box sums here are fp64 running column sums (+ newest row, - oldest row) and
-//     8-wide row sums, scaled and rounded once to float.
+//   * cv::boxFilter on CV_32F accumulates in double with running sums along whole rows and columns.
+//     Box sums here are fp64 running column sums per row segment (+ newest row, - oldest row) and
+//     8-wide row sums, scaled and rounded once to float: OpenCV's float while the fp64 sums are
+//     exact.  Outside that domain psm_cvf_ref.cuh filters the slice again in OpenCV's order.
 //   * every fp32 operation of a, b and q is a separate IEEE round-to-nearest op in the reference's
 //     order (CVF.cpp:87-163): __fmul_rn / __fadd_rn / __fsub_rn, which ptxas never contracts.
 //   * PSM_CVF_EXACT: all eight box sums in fp64 -> q bit-exact.

@@ -6,7 +6,6 @@
 // K (1..kWinMax) and eps at run time and compute the same quantities:
 //   guide_window_kernel : the 19-plane guide layout of guide_kernel (mean_I, adjugate of Sigma + eps I, 1/det, var_I)
 //   cvf_window_kernel   : the streaming guided filter, p read once and q written once per voxel, a and b never leave the SM
-//   ab_window_kernel    : a, b of one slice with direct K x K sums (psm_read_ab_slice)
 //
 // Numerics are those of psm_cvf_stream.cuh: every box sum in fp64 (exact, hence order-independent, unless a window spans
 // more than 2^(29 - ceil(log2 K^2)) in magnitude), scaled by 1/K^2 and rounded once; every f32 operation of a, b and q a
@@ -62,6 +61,7 @@ __device__ __forceinline__ void guide_solve_eps(const float m[9], float eps, flo
 
 struct WinGuideParams {
     float* guide[2];
+    int* guide_flags;   // [2]: kGuideNonFinite raised when a mean / adjugate / 1/det value is not finite
     int W, H, Wp, K, a, seg_rows;
     double scale;   // 1 / K^2
     float eps;
@@ -113,6 +113,12 @@ __global__ void __launch_bounds__(128) guide_window_kernel(const WinGuideParams 
             G[(size_t)(kGuideVar + k) * plane + o] = v[k];
         }
         G[(size_t)kGuideIdet * plane + o] = idet;
+        unsigned worst = __float_as_uint(idet) & 0x7fffffffu;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) worst = max(worst, __float_as_uint(M[k]) & 0x7fffffffu);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) worst = max(worst, __float_as_uint(m[k]) & 0x7fffffffu);
+        if (worst >= 0x7f800000u) atomicOr(P.guide_flags + view, kGuideNonFinite);
     }
 }
 
@@ -126,31 +132,6 @@ __device__ __forceinline__ GuidePix load_guide_pix(const float* __restrict__ g, 
     q.M12 = __ldg(g + (kGuideAdj + 4) * plane + o); q.M22 = __ldg(g + (kGuideAdj + 5) * plane + o);
     q.idet = __ldg(g + kGuideIdet * plane + o);
     return q;
-}
-
-// a, b of one slice, direct K x K fp64 sums per pixel (psm_read_ab_slice at non-default parameters)
-__global__ void ab_window_kernel(const float* __restrict__ p, const float* __restrict__ guide, size_t plane, int W, int H,
-                                 int Wp, int K, int a, double scale, float* __restrict__ ab /* [4][H][Wp] */)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
-    if (x >= W) return;
-    double s[4] = {0.0, 0.0, 0.0, 0.0};
-    for (int dy = -a; dy < K - a; ++dy) {
-        const size_t ro = (size_t)reflect101(y + dy, H) * Wp;
-        for (int dx = -a; dx < K - a; ++dx) {
-            const size_t o = ro + reflect101(x + dx, W);
-            const float pv = __ldg(p + o);
-            s[0] = __dadd_rn(s[0], (double)pv);
-            s[1] = __dadd_rn(s[1], (double)fmul(__ldg(guide + o), pv));
-            s[2] = __dadd_rn(s[2], (double)fmul(__ldg(guide + plane + o), pv));
-            s[3] = __dadd_rn(s[3], (double)fmul(__ldg(guide + 2 * plane + o), pv));
-        }
-    }
-    const size_t o = (size_t)y * Wp + x;
-    float a0, a1, a2, b;
-    gif_coeffs((float)__dmul_rn(s[0], scale), (float)__dmul_rn(s[1], scale), (float)__dmul_rn(s[2], scale),
-               (float)__dmul_rn(s[3], scale), load_guide_pix(guide, plane, o), a0, a1, a2, b);
-    ab[o] = a0; ab[plane + o] = a1; ab[2 * plane + o] = a2; ab[3 * plane + o] = b;
 }
 
 struct WinParams {

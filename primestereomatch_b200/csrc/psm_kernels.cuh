@@ -1,6 +1,6 @@
-// psm_kernels.cuh -- ingest, cost-volume construction (CVC), guide precompute, WTA and the
-// unfused "naive" CVF cross-check kernels.  The fused streaming CVF kernel is in
-// psm_cvf_stream.cuh.  Layout: every plane / volume row has pitch Wp floats and is stored with a
+// psm_kernels.cuh -- ingest, cost-volume construction (CVC), guide precompute and WTA.  The fused
+// streaming CVF kernel is in psm_cvf_stream.cuh, the reference-order guided filter (PSM_CVF_NAIVE)
+// in psm_cvf_ref.cuh.  Layout: every plane / volume row has pitch Wp floats and is stored with a
 // column halo: kPadLeft columns before column 0 and at least kPadRight after column W-1 (so a
 // pointer to (row, col 0) may be indexed from -kPadLeft .. W+kPadRight-1); pitch and halo are
 // multiples of 4 floats, so 4-column groups are 16-byte aligned.  The halos of the cost volumes
@@ -46,6 +46,11 @@ __global__ void pad_cols_kernel(float* __restrict__ base, size_t nrows, int W, i
 // Restates StereoMatch.cpp:193-197 (u8 * (1/255.0f)), CVF.cpp:47 (split) and CVC.cpp:41-46
 // (cvtColor RGB2GRAY on the BGR image, Sobel dx=1 ksize=1 with BORDER_REFLECT_101).
 // ------------------------------------------------------------------------------------------
+// guide_flags bits (per view): raised by ingest_kernel (kGuideOutside, kGuideInexact) and the guide precompute (kGuideNonFinite)
+constexpr int kGuideOutside = 1;     // a channel value is negative, -0, inf, NaN or >= 2^61: no integer widening
+constexpr int kGuideNonFinite = 2;   // a mean, adjugate or 1/det value is not finite
+constexpr int kGuideInexact = 4;     // a nonzero channel value lies outside [2^-12, 1]: the guide's box sums may be inexact
+
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(uint8_t v) { return fmul((float)v, 1 / 255.0f); }
 
@@ -73,9 +78,18 @@ __global__ void ingest_kernel(const T* __restrict__ src, size_t step_bytes, int 
     I1[o] = v1;
     I2[o] = v2;
     // the integer widening in guide_kernel / the CVF kernel assumes I >= +0, finite, and I * I finite (images are in
-    // [0,1] by contract, DispEst data contract SURVEY 8b); a negative, non-finite or >= 2^63 value raises the per-view
-    // flag and selects their conversion-pipe paths (bit patterns compare like the magnitudes; the sign bit sorts last)
-    if (max(max(__float_as_uint(v0), __float_as_uint(v1)), __float_as_uint(v2)) >= 0x5f000000u) atomicOr(guide_flag, 1);
+    // [0,1] by contract, DispEst data contract SURVEY 8b); a negative, non-finite or >= 2^61 value raises kGuideOutside
+    // and selects their conversion-pipe paths (bit patterns compare like the magnitudes; the sign bit sorts last).
+    // Below 2^61 every cost psm_cost_const builds is finite, >= +0 and < 2^63 (|l - r| < 2^61 per channel), so the
+    // slices of such a view need no reference-order pass of their own; with kGuideOutside the whole view takes it.
+    // The guide's box sums (I_c and the rounded products I_c I_c', CVF.cpp:49-62) are exact in any order when every
+    // nonzero value lies in [2^-12, 1]: a product is then 0 or at least 2^-24, a multiple of 2^-47, and a sum of at most
+    // 64 such values in [0, 64] needs at most 53 bits.  Any other nonzero value raises kGuideInexact and the guide is
+    // recomputed in OpenCV's order (psm_cvf_ref.cuh).  u8 images (0 or 1/255 .. 1) never raise it.
+    const unsigned u0 = __float_as_uint(v0), u1 = __float_as_uint(v1), u2 = __float_as_uint(v2);
+    if (max(max(u0, u1), u2) >= 0x5e000000u) atomicOr(guide_flag, kGuideOutside | kGuideInexact);
+    auto inexact = [](unsigned u) { return u != 0u && u - 0x39800000u > 0x3f800000u - 0x39800000u; };   // outside {0} U [2^-12, 1]
+    if (inexact(u0) || inexact(u1) || inexact(u2)) atomicOr(guide_flag, kGuideInexact);
     const float gr = gray_at(row, reflect101(x + 1, W), gray_mode);
     const float gl = gray_at(row, reflect101(x - 1, W), gray_mode);
     grd[o] = fsub(gr, gl);
@@ -348,27 +362,6 @@ __device__ __forceinline__ void cvc_body(const CvcParams& P, const Weigh& weigh)
 }
 
 // ------------------------------------------------------------------------------------------
-// Exact 8x8 box mean of a plane at one pixel: sum of 64 reflected taps in fp64, * 1/64, one
-// rounding to float == cv::boxFilter(CV_32F, Size(8,8)) (anchor (4,4), BORDER_REFLECT_101,
-// double accumulation).  Used by the guide precompute and the naive cross-check kernels.
-// ------------------------------------------------------------------------------------------
-template <typename F>
-__device__ __forceinline__ float box8_direct(F tap, int x, int y, int W, int H)
-{
-    double s = 0.0;
-#pragma unroll 1
-    for (int dy = -kBoxAnchor; dy < kBoxK - kBoxAnchor; ++dy) {
-        const int yy = reflect101(y + dy, H);
-        double rs = 0.0;
-#pragma unroll
-        for (int dx = -kBoxAnchor; dx < kBoxK - kBoxAnchor; ++dx)
-            rs = __dadd_rn(rs, (double)tap(reflect101(x + dx, W), yy));
-        s = __dadd_rn(s, rs);
-    }
-    return (float)__dmul_rn(s, 1.0 / 64.0);
-}
-
-// ------------------------------------------------------------------------------------------
 // K2 guide precompute (CVF::preprocess, CVF.cpp:44-70) + the d-independent part of the 3x3
 // solve of GuidedFilter_cv (CVF.cpp:117-126): the symmetric adjugate of (Sigma + eps I) and
 // 1/det.  One fused kernel: fp64 horizontal 8-sums of the 9 planes (I_c, I_c*I_c') per row,
@@ -435,7 +428,7 @@ constexpr int kGuideStripOut = 120;
 
 struct GuideParams {
     float* guide[2];
-    int* guide_flags;   // [2]: bit 1 raised when a mean / adjugate / 1/det value is not finite
+    int* guide_flags;   // [2]: kGuideNonFinite raised when a mean / adjugate / 1/det value is not finite
     int W, H, Wp, nstrips, nseg, seg_rows;
 };
 
@@ -517,7 +510,7 @@ __global__ void __launch_bounds__(128) guide_kernel(const GuideParams P)
                     for (int j = 0; j < 4; ++j) worst = max(worst, __float_as_uint(o[k][j]) & 0x7fffffffu);
                 }
             }
-            if (worst >= 0x7f800000u) atomicOr(P.guide_flags + view, 2);
+            if (worst >= 0x7f800000u) atomicOr(P.guide_flags + view, kGuideNonFinite);
         }
     }
 }
@@ -536,64 +529,6 @@ __device__ __forceinline__ void gif_coeffs(float mp, float mIp0, float mIp1, flo
     a1 = fmul(g.idet, fadd(fadd(fmul(c0, g.M01), fmul(c1, g.M11)), fmul(c2, g.M12)));
     a2 = fmul(g.idet, fadd(fadd(fmul(c0, g.M02), fmul(c1, g.M12)), fmul(c2, g.M22)));
     b = fsub(fsub(fsub(mp, fmul(a0, g.mI0)), fmul(a1, g.mI1)), fmul(a2, g.mI2));
-}
-
-// ------------------------------------------------------------------------------------------
-// Naive CVF (PSM_CVF_NAIVE): two unfused passes with direct 64-tap fp64 sums per voxel.
-// Slow by construction (256 loads per voxel per pass); exists as an independent device-side
-// implementation to cross-check the fused streaming kernel and for tiny images.
-// ------------------------------------------------------------------------------------------
-__global__ void cvf_naive_ab_kernel(const float* __restrict__ vol, const float* __restrict__ guide, size_t plane,
-                                    int W, int H, int Wp, int nslices,
-                                    float* __restrict__ ab /* [4][nslices][H][Wp] */)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    const int dl = blockIdx.z;
-    if (x >= W) return;
-    const float* p = vol + (size_t)dl * plane;
-    const float* I0 = guide;
-    const float* I1 = guide + plane;
-    const float* I2 = guide + 2 * plane;
-    const float mp = box8_direct([&](int xx, int yy) { return p[(size_t)yy * Wp + xx]; }, x, y, W, H);
-    const float m0 = box8_direct([&](int xx, int yy) { const size_t o = (size_t)yy * Wp + xx; return fmul(I0[o], p[o]); }, x, y, W, H);
-    const float m1 = box8_direct([&](int xx, int yy) { const size_t o = (size_t)yy * Wp + xx; return fmul(I1[o], p[o]); }, x, y, W, H);
-    const float m2 = box8_direct([&](int xx, int yy) { const size_t o = (size_t)yy * Wp + xx; return fmul(I2[o], p[o]); }, x, y, W, H);
-    const size_t o = (size_t)y * Wp + x;
-    GuidePix g;
-    g.mI0 = guide[(kGuideMean + 0) * plane + o]; g.mI1 = guide[(kGuideMean + 1) * plane + o]; g.mI2 = guide[(kGuideMean + 2) * plane + o];
-    g.M00 = guide[(kGuideAdj + 0) * plane + o]; g.M01 = guide[(kGuideAdj + 1) * plane + o]; g.M02 = guide[(kGuideAdj + 2) * plane + o];
-    g.M11 = guide[(kGuideAdj + 3) * plane + o]; g.M12 = guide[(kGuideAdj + 4) * plane + o]; g.M22 = guide[(kGuideAdj + 5) * plane + o];
-    g.idet = guide[kGuideIdet * plane + o];
-    float a0, a1, a2, b;
-    gif_coeffs(mp, m0, m1, m2, g, a0, a1, a2, b);
-    const size_t vs = (size_t)nslices * plane;
-    const size_t oo = (size_t)dl * plane + o;
-    ab[oo] = a0; ab[vs + oo] = a1; ab[2 * vs + oo] = a2; ab[3 * vs + oo] = b;
-}
-
-__global__ void cvf_naive_q_kernel(const float* __restrict__ ab, const float* __restrict__ guide, size_t plane,
-                                   int W, int H, int Wp, int nslices, float* __restrict__ vol_out)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    const int dl = blockIdx.z;
-    if (x >= W) return;
-    const size_t vs = (size_t)nslices * plane;
-    const float* a0 = ab + (size_t)dl * plane;
-    const float* a1 = a0 + vs;
-    const float* a2 = a1 + vs;
-    const float* b = a2 + vs;
-    auto tapper = [&](const float* pl) {
-        return box8_direct([&](int xx, int yy) { return pl[(size_t)yy * Wp + xx]; }, x, y, W, H);
-    };
-    const size_t o = (size_t)y * Wp + x;
-    // q = box(b); q += box(a_c) * I_c for c = 0,1,2   (CVF.cpp:157-163)
-    float q = tapper(b);
-    q = fadd(q, fmul(tapper(a0), guide[o]));
-    q = fadd(q, fmul(tapper(a1), guide[plane + o]));
-    q = fadd(q, fmul(tapper(a2), guide[2 * plane + o]));
-    vol_out[(size_t)dl * plane + o] = q;
 }
 
 // ------------------------------------------------------------------------------------------
