@@ -200,7 +200,8 @@ def pipeline(l, r, D, threads=8, gray_mode=0, keep_volumes=False):
 
 
 def to_u8x255(img3_f32):
-    """convertTo(CV_8UC3, 255) (src/PP.cpp:416-417): saturate_cast<uchar>(cvRound(v * 255)), half to even"""
+    """convertTo(CV_8UC3, 255) (src/PP.cpp:416-417): saturate_cast<uchar>(cvRound(v * 255)), half to even; 0 where the
+    float product is NaN or >= 2^31 (x86 cvRound's INT_MIN)"""
     img3 = _c(img3_f32)
     img8 = np.empty(img3.shape, np.uint8)
     lib().orc_f32_to_u8x255(img3.reshape(-1), img8.reshape(-1), img3.size)

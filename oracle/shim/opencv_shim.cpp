@@ -1,4 +1,4 @@
-// opencv_shim.cpp -- the five image primitives behind oracle/shim/opencv2/opencv.hpp.
+// opencv_shim.cpp -- the six image primitives behind oracle/shim/opencv2/opencv.hpp.
 // TEST INFRASTRUCTURE ONLY (part of oracle/_ref).  Each primitive forwards to the C restatement in
 // oracle/stereo_oracle.c, which is pinned against python cv2 (tests/test_oracle.py).
 #include <opencv2/opencv.hpp>
@@ -92,10 +92,9 @@ void Mat::convertTo(Mat& dst, int rtype, double alpha, double beta) const
         for (int x = 0; x < cols * cn; ++x) {
             if (sd == CV_8U && dd == CV_32S) { need(alpha == 1.0 && beta == 0.0, "convertTo scale"); out.ptr<int>(y)[x] = ptr<uchar>(y)[x]; }
             else if (sd == CV_32S && dd == CV_8U) { need(alpha == 1.0 && beta == 0.0, "convertTo scale"); int v = ptr<int>(y)[x]; out.ptr<uchar>(y)[x] = (uchar)(v < 0 ? 0 : (v > 255 ? 255 : v)); }
-            else if (sd == CV_32F && dd == CV_8U) {  // cv::saturate_cast<uchar>(cvRound(v*alpha+beta)), float arithmetic, round-half-even
-                const float v = ptr<float>(y)[x] * (float)alpha + (float)beta;
-                const long r = lrintf(v);
-                out.ptr<uchar>(y)[x] = (uchar)(r < 0 ? 0 : (r > 255 ? 255 : r));
+            else if (sd == CV_32F && dd == CV_8U) {  // cv::saturate_cast<uchar>(cvRound(v*alpha)): the C restatement
+                need(alpha == 255.0 && beta == 0.0, "convertTo 32F -> 8U scale other than 255");
+                orc_f32_to_u8x255(ptr<float>(y) + x, out.ptr<uchar>(y) + x, 1);
             } else need(false, "convertTo: unsupported depth pair");
         }
     dst = out;

@@ -591,12 +591,17 @@ int orc_wmf(const void* disp, int map_bytes, const uint8_t* img8, int W, int H, 
     return rc;
 }
 
-/* lImg.convertTo(lImg_8UC3, CV_8UC3, 255) (src/PP.cpp:416-417): saturate_cast<uchar>(cvRound(v * 255)) */
+/* lImg.convertTo(lImg_8UC3, CV_8UC3, 255) (src/PP.cpp:416-417): saturate_cast<uchar>(cvRound(v * 255)).  q = v * 255 is
+ * rounded to float; cvRound on x86 is cvtss2si, which returns INT_MIN when q is NaN or outside the int range, and that
+ * saturates to 0.  So: 0 if q is NaN or q >= 2^31 (+inf included), else clamp(rint(q), 0, 255), ties to even (pinned
+ * against cv2 by tests/golden/golden_image.json). */
 void orc_f32_to_u8x255(const float* src, uint8_t* dst, size_t n)
 {
     for (size_t i = 0; i < n; ++i) {
-        const long q = lrintf(src[i] * 255.0f);
-        dst[i] = (uint8_t)(q < 0 ? 0 : (q > 255 ? 255 : q));
+        const float q = src[i] * 255.0f;
+        if (!(q < 2147483648.0f)) { dst[i] = 0; continue; }   /* NaN, >= 2^31 */
+        const float r = rintf(q);
+        dst[i] = (uint8_t)(r < 0.0f ? 0 : (r > 255.0f ? 255 : (int)r));
     }
 }
 

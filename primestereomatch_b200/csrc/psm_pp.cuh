@@ -44,9 +44,11 @@ __global__ void pp_pack_kernel(const float* __restrict__ I0, const float* __rest
     const int y = blockIdx.y;
     if (x >= W || y >= H) return;
     const size_t o = (size_t)y * Wp + x;
-    // convertTo(CV_8UC3, 255): saturate_cast<uchar>(cvRound(v * 255.0f)), round half to even (PP.cpp:416-417)
+    // convertTo(CV_8UC3, 255): saturate_cast<uchar>(cvRound(v * 255.0f)), round half to even (PP.cpp:416-417).  cvRound
+    // on x86 returns INT_MIN for a NaN or a product >= 2^31, which saturates to 0 (__float2int_rn would give 255 there)
     auto q6 = [](float v) {
-        int q = __float2int_rn(fmul(v, 255.0f));
+        const float f = fmul(v, 255.0f);
+        int q = f < 2147483648.0f ? __float2int_rn(f) : 0;
         q = q < 0 ? 0 : (q > 255 ? 255 : q);
         return (uint32_t)(q >> 2);           // JointWMF.h:546,559-561: 8 bit -> 6 bit
     };
