@@ -21,6 +21,7 @@
  *                                                                 src/DispEst.cpp:323-328, src/DispSel_cl.cpp:123-134
  *   psm_post_process      <-> DispEst::PostProcess_GPU -> PP::processDM -> JointWMF::filter
  *                                                                 src/DispEst.cpp:338-344, src/PP.cpp:402-425
+ *   psm_set_lr_check      <-> PP::processDM's lrCheck + fillInv (commented out there)  src/PP.cpp:17-143, :405-406
  *   psm_read_cost_slice   <-> DispEst::printCV (cost-slice dump) src/DispEst.cpp:181-194
  *   psm_stage_ms          <-> cvc_time/cvf_time/dispsel_time     src/StereoMatch.cpp:209-241
  *
@@ -174,6 +175,31 @@ enum { PSM_WMF_EXP = 0, PSM_WMF_IV1 = 1, PSM_WMF_IV2 = 2, PSM_WMF_OFF = 5 };
  * on the context and rebuilt after a change of sigma or weight type.  See DESIGN.md section 13. */
 int psm_set_post_filter(psm_ctx* ctx, int radius, float sigma, int iterations, int weight_type);
 
+/* Left-right check modes of psm_set_lr_check */
+enum { PSM_LR_OFF = 0, PSM_LR_FILL_WMF = 1, PSM_LR_FILL = 2 };
+
+/* Left-right consistency check and occlusion fill (the reference's lrCheck and fillInv, src/PP.cpp:17-143, which
+ * PP::processDM has commented out at :405-406) for every later psm_post_process / _u16 / _device of this context:
+ *   PSM_LR_OFF (default): the post-filter alone, exactly as before (2 * 2 * iterations launches per call);
+ *   PSM_LR_FILL_WMF: processDM with lines 405-406 restored: check, fill, then the post-filter of psm_set_post_filter on
+ *                    the filled maps with the original feature image (1 + 4 * iterations launches);
+ *   PSM_LR_FILL: check and fill only; the filled maps are the result (one launch).
+ * Per row, on integer map values, W = width and mod the non-negative (Euclidean) remainder:
+ *   lValid[x] = l[x] == r[(x - l[x]) mod W] && l[x] >= 2      rValid[x] = r[x] == l[(x + r[x]) mod W] && r[x] >= 2
+ * both on the unmodified maps (disparities 0 and 1 are never valid; the gathers wrap around the row).  The reference
+ * writes (x - d + W) % W, a C remainder, which equals this wherever d <= x + W and reads out of bounds beyond (a map
+ * value above the width).  Then each view with its own mask: a valid pixel keeps its value, an invalid pixel x takes
+ * min(map[L], map[R]) of the nearest valid pixels L <= x <= R, or the one of them that exists; a row with no valid pixel
+ * is unchanged.  u16 maps use the same expressions.  The stage reads the maps of the last selection stage (or the
+ * exchange block's complete maps) and never writes them: the filled maps go to psm_device_ptr selectors 4 / 5, the masks
+ * to selectors 6 / 7.  Stage 5 of psm_stage_ms covers it.  Any other mode returns PSM_EINVAL and leaves the context
+ * unchanged.  Sharded contexts: every rank must set the same mode.  See DESIGN.md section 15. */
+int psm_set_lr_check(psm_ctx* ctx, int mode);
+
+/* The left-right check's mask of one view (0 / 1, W x H, row step in bytes >= W) to HOST memory; synchronises.
+ * PSM_ESTATE unless the last post-process call since the last selection stage ran the check. */
+int psm_read_valid_mask(psm_ctx* ctx, int view, uint8_t* dst, size_t dst_step);
+
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream. */
 int psm_set_stream(psm_ctx* ctx, void* cuda_stream);
@@ -310,11 +336,13 @@ int psm_read_ab_slice(psm_ctx* ctx, int view, int d, float* a3, float* b);
 
 /* Device pointers for zero-copy callers / benchmarks. what: 0 left volume, 1 right volume,
  * 2 left u8 map, 3 right u8 map, 4 / 5 post-processed left / right u8 map (uint16_t maps on a psm_create_u16 context,
- * pitch_elems = W).  pitch_elems receives the row pitch in elements. */
+ * pitch_elems = W), 6 / 7 left / right mask of the left-right check (uint8_t 0 / 1 on both map formats, pitch_elems = W;
+ * NULL until a post-process has run the check).  pitch_elems receives the row pitch in elements. */
 int psm_device_ptr(psm_ctx* ctx, int what, void** ptr, size_t* pitch_elems);
 
 /* Last measured stage durations in milliseconds (cudaEvent pairs on the context stream):
- * stage 0 ingest (H2D + planar/gradient), 1 CVC, 2 CVF (guide + filter), 3 WTA, 4 CVF filter kernel only, 5 post-process.
+ * stage 0 ingest (H2D + planar/gradient), 1 CVC, 2 CVF (guide + filter), 3 WTA, 4 CVF filter kernel only, 5 post-process
+ * (left-right check and fill included).
  * Synchronises on the stage's end event. */
 int psm_stage_ms(psm_ctx* ctx, int stage, float* ms);
 

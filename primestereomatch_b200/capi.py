@@ -21,7 +21,7 @@ SYMBOLS = [
     "psm_read_guide_plane", "psm_read_ab_slice", "psm_device_ptr", "psm_stage_ms",
     "psm_launch_count", "psm_sync", "psm_last_error", "psm_build_info", "psm_cvf_plan", "psm_set_guided_filter",
     "psm_set_matching_cost", "psm_set_post_filter", "psm_create_u16", "psm_disp_select_u16", "psm_disp_select_u16_async",
-    "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16",
+    "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -29,6 +29,7 @@ PSM_LEFT, PSM_RIGHT = 0, 1
 PSM_OPT_CVF_MODE, PSM_OPT_GRAY_MODE, PSM_OPT_TIMING, PSM_OPT_P2P_SYNC, PSM_OPT_VARIANT = 1, 2, 3, 4, 100
 PSM_CVF_EXACT, PSM_CVF_MIXED, PSM_CVF_NAIVE = 0, 1, 2
 PSM_WMF_EXP, PSM_WMF_IV1, PSM_WMF_IV2, PSM_WMF_OFF = 0, 1, 2, 5
+PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL = 0, 1, 2
 
 _lib = None
 
@@ -65,6 +66,8 @@ def lib():
     L.psm_set_guided_filter.argtypes = [vp, i, C.c_float]
     L.psm_set_matching_cost.argtypes = [vp, C.c_float, C.c_float, C.c_float]
     L.psm_set_post_filter.argtypes = [vp, i, C.c_float, i, i]
+    L.psm_set_lr_check.argtypes = [vp, i]
+    L.psm_read_valid_mask.argtypes = [vp, i, u8p, sz]
     L.psm_set_stream.argtypes = [vp, vp]
     L.psm_set_images.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_u8.argtypes = [vp, u8p, sz, u8p, sz]

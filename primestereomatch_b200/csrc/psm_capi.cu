@@ -17,6 +17,7 @@
 #include "psm_pp.cuh"
 #include "psm_pp_param.cuh"
 #include "psm_fgf.cuh"
+#include "psm_lr.cuh"
 
 #ifndef PSM_BUILD_FLAGS
 #define PSM_BUILD_FLAGS "unknown"
@@ -90,6 +91,9 @@ struct psm_ctx {
     float pp_sigma = 25.5f;
     int pp_iter = 1, pp_type = PSM_WMF_EXP;
     bool pp_tuned() const { return pp_radius == kPpRadius && pp_sigma == 25.5f && pp_type == PSM_WMF_EXP; }   // any pp_iter
+    int lr_mode = PSM_LR_OFF;               // left-right check and fill in front of the post-filter, psm_set_lr_check
+    uint8_t* lr_valid[2] = {nullptr, nullptr};  // the check's masks (W x H, 0/1), lazy
+    bool lr_masks_ok = false;               // lr_valid holds the masks of the current maps (psm_read_valid_mask)
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -651,7 +655,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->guide_flags);
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
-    for (int v = 0; v < 2; ++v) cudaFree(c->dis_pp[v]);
+    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); }
     for (int s = 0; s < kNumStages; ++s) {
         if (c->ev0[s]) cudaEventDestroy(c->ev0[s]);
         if (c->ev1[s]) cudaEventDestroy(c->ev1[s]);
@@ -751,6 +755,15 @@ int psm_set_post_filter(psm_ctx* c, int radius, float sigma, int iterations, int
     c->pp_sigma = sigma;
     c->pp_iter = iterations;
     c->pp_type = weight_type;
+    return PSM_OK;
+}
+
+int psm_set_lr_check(psm_ctx* c, int mode)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (mode != PSM_LR_OFF && mode != PSM_LR_FILL_WMF && mode != PSM_LR_FILL)
+        return fail(c, PSM_EINVAL, "left-right check mode %d is not off (0), fill + post-filter (1) or fill (2)", mode);
+    c->lr_mode = mode;
     return PSM_OK;
 }
 
@@ -1003,6 +1016,7 @@ static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const u
     if (int rc = bind(c)) return rc;
     if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
     const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
+    c->lr_masks_ok = false;
     const size_t npix = (size_t)c->W * c->H;
     for (int v = 0; v < 2; ++v) {
         keys_reduce_kernel<T><<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
@@ -1027,6 +1041,7 @@ int psm_disp_select_device(psm_ctx* c)
         return fail(c, PSM_ESTATE, "psm_disp_select on a sharded context: use psm_disp_select_keys + psm_disp_reduce_keys");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
+    c->lr_masks_ok = false;
     if (int rc = c->map_bytes == 2 ? select_maps<uint16_t>(c) : select_maps<uint8_t>(c)) return rc;
     c->have_maps = true;
     return stage_end(c, 3);
@@ -1165,6 +1180,7 @@ int psm_disp_select_keys_p2p(psm_ctx* c)
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys_p2p before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
     c->p2p_seq++;   // one sequence number per frame, identical on every rank (all ranks run the same frames)
+    c->lr_masks_ok = false;
     for (int v = 0; v < 2; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
@@ -1181,6 +1197,7 @@ int psm_disp_reduce_p2p(psm_ctx* c)
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "no exchange block");
     const unsigned npix = (unsigned)((size_t)c->W * c->H);
     const auto reduce = c->map_bytes == 2 ? chunk_reduce_kernel<uint16_t> : chunk_reduce_kernel<uint8_t>;
+    c->lr_masks_ok = false;
     for (int v = 0; v < 2; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
@@ -1275,16 +1292,22 @@ static int post_process_maps(psm_ctx* c)
     const auto generic = [] {
         if constexpr (sizeof(T) == 1) return pp_wmf_param_kernel; else return pp_wmf_param_two_level_kernel;
     }();
+    c->lr_masks_ok = false;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_post_process before psm_set_images");
     if (!c->have_maps && !(c->p2p_own && c->p2p_seq > 0)) return fail(c, PSM_ESTATE, "psm_post_process before a disparity-selection stage");
     const size_t npix = (size_t)c->W * c->H;
+    const bool lr = c->lr_mode != PSM_LR_OFF, wmf = c->lr_mode != PSM_LR_FILL;
     // Each buffer is allocated while its own pointer is null and the table is marked valid only once it is on the
     // device, so a call that failed part-way leaves nothing a launch could trip over: the next call completes the set-up
     // or fails in turn.
-    PSM_CUDA(c, alloc_if_null(c->pp_lut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
-    PSM_CUDA(c, alloc_if_null(c->pp_packed, npix * sizeof(uint32_t)));
+    if (wmf) {
+        PSM_CUDA(c, alloc_if_null(c->pp_lut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
+        PSM_CUDA(c, alloc_if_null(c->pp_packed, npix * sizeof(uint32_t)));
+    }
     for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->dis_pp[v], npix * c->map_bytes));
-    if (!c->pp_lut_valid) {
+    if (lr)
+        for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->lr_valid[v], npix));
+    if (wmf && !c->pp_lut_valid) {
         const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
         PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
@@ -1301,6 +1324,16 @@ static int post_process_maps(psm_ctx* c)
     if (c->p2p_own && c->p2p_seq > 0)
         if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
+    if (lr) {
+        // lrCheck + fillInv (PP.cpp:405-406): reads the selection maps, writes the filled maps into dis_pp
+        const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;
+        lr_check_fill_kernel<T><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
+            reinterpret_cast<const T*>(current_map(c, 0)), reinterpret_cast<const T*>(current_map(c, 1)), c->W,
+            reinterpret_cast<T*>(c->dis_pp[0]), reinterpret_cast<T*>(c->dis_pp[1]), c->lr_valid[0], c->lr_valid[1]);
+        PSM_LAUNCH_CHECK(c);
+        c->lr_masks_ok = true;
+        if (!wmf) return stage_end(c, 5);
+    }
     int nsm = 0;
     PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
     const int lut_n = pp_weight_table_size(c->pp_type);
@@ -1313,9 +1346,10 @@ static int post_process_maps(psm_ctx* c)
         const float* g = c->guide[v];
         T* dst = reinterpret_cast<T*>(c->dis_pp[v]);
         dim3 blk(256), grd((c->W + 255) / 256, c->H);
-        // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output
+        // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output (after
+        // the left-right fill, the first pass filters the filled map)
         for (int it = 0; it < c->pp_iter; ++it) {
-            const T* src = reinterpret_cast<const T*>(it == 0 ? current_map(c, v) : c->dis_pp[v]);
+            const T* src = reinterpret_cast<const T*>(it == 0 && !lr ? current_map(c, v) : c->dis_pp[v]);
             pp_pack_kernel<T><<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
             PSM_LAUNCH_CHECK(c);
             if (tuned)
@@ -1448,8 +1482,21 @@ int psm_device_ptr(psm_ctx* c, int what, void** ptr, size_t* pitch_elems)
     case 0: case 1: *ptr = c->vol[what]; if (pitch_elems) *pitch_elems = c->Wp; return PSM_OK;
     case 2: case 3: *ptr = c->dis[what - 2]; if (pitch_elems) *pitch_elems = c->W; return PSM_OK;
     case 4: case 5: *ptr = c->dis_pp[what - 4]; if (pitch_elems) *pitch_elems = c->W; return PSM_OK;
+    case 6: case 7: *ptr = c->lr_valid[what - 6]; if (pitch_elems) *pitch_elems = c->W; return PSM_OK;
     default: return fail(c, PSM_EINVAL, "bad selector %d", what);
     }
+}
+
+int psm_read_valid_mask(psm_ctx* c, int view, uint8_t* dst, size_t dst_step)
+{
+    if (int rc = bind(c)) return rc;
+    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
+    if (!dst || dst_step < (size_t)c->W) return fail(c, PSM_EINVAL, "bad dst/step");
+    if (!c->lr_masks_ok)
+        return fail(c, PSM_ESTATE, "no valid mask: the last post-process since the last selection stage did not run the left-right check");
+    PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->lr_valid[view], c->W, c->W, c->H, cudaMemcpyDeviceToHost, c->stream));
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
 }
 
 int psm_stage_ms(psm_ctx* c, int stage, float* ms)

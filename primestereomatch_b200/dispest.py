@@ -56,6 +56,9 @@ class DispEst:
         self.subsample_rate = 4
         self.lDisMap = np.zeros((self.hei, self.wid), mdt)  # DispEst.cpp:46-47
         self.rDisMap = np.zeros((self.hei, self.wid), mdt)
+        self.lValid = np.zeros((self.hei, self.wid), np.uint8)  # DispEst.cpp:48-49
+        self.rValid = np.zeros((self.hei, self.wid), np.uint8)
+        self.lr_mode = capi.PSM_LR_OFF
         self._lImg, self._rImg = l, r
         self._ctx = C.c_void_p()
         self._lib = None
@@ -132,6 +135,16 @@ class DispEst:
         capi.check(self._lib.psm_set_post_filter(self._ctx, int(radius), float(sigma), int(iterations), wt), self._ctx)
         return 0
 
+    def setLRCheck(self, mode):
+        """Left-right consistency check and occlusion fill (the reference's lrCheck / fillInv, commented out in
+        PP::processDM, src/PP.cpp:405-406) for every later PostProcess_GPU call: 0 off (default), 1 check + fill + the
+        post-filter (processDM with those lines restored), 2 check + fill only.  With mode 1 or 2 PostProcess_GPU also
+        fills lValid / rValid (0/1).  Raises PsmError on any other mode."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_lr_check(self._ctx, int(mode)), self._ctx)
+        self.lr_mode = int(mode)
+        return 0
+
     def set_option(self, key, value):
         capi.check(self._lib.psm_set_option(self._ctx, int(key), int(value)), self._ctx)
 
@@ -175,12 +188,16 @@ class DispEst:
         return 0
 
     def PostProcess_GPU(self):
-        """DispEst.cpp:338-344 -> PP::processDM (PP.cpp:402-425): joint weighted-median filter of both maps; the
-        reference runs it on the CPU even in GPU mode, here it is a device stage.  Results replace lDisMap / rDisMap."""
+        """DispEst.cpp:338-344 -> PP::processDM (PP.cpp:402-425): joint weighted-median filter of both maps (after the
+        left-right check and fill, or instead of the filter, as setLRCheck selects); the reference runs it on the CPU even
+        in GPU mode, here it is a device stage.  Results replace lDisMap / rDisMap."""
         self._need_gpu()
         pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
         capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
                       _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
+        if self.lr_mode != capi.PSM_LR_OFF:
+            for view, mask in ((capi.PSM_LEFT, self.lValid), (capi.PSM_RIGHT, self.rValid)):
+                capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)
         return 0
 
     def CostConst(self):

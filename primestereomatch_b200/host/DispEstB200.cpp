@@ -18,6 +18,8 @@ DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl)
     const bool wide = maxDis > 256;
     lDisMap = cv::Mat::zeros(hei, wid, wide ? CV_16UC1 : CV_8UC1);
     rDisMap = cv::Mat::zeros(hei, wid, wide ? CV_16UC1 : CV_8UC1);
+    lValid = cv::Mat::zeros(hei, wid, CV_8UC1);   // DispEst.cpp:48-49
+    rValid = cv::Mat::zeros(hei, wid, CV_8UC1);
     if (useOCL) {
         const int rc = wide ? psm_create_u16(&ctx, wid, hei, maxDis, 0, maxDis, 0) : psm_create(&ctx, wid, hei, maxDis, 0);
         if (rc != PSM_OK) {
@@ -68,6 +70,14 @@ int DispEst::setPostFilter(int radius, float sigma, int iterations, int weight_t
 {
     if (!ctx) return -1;
     return psm_set_post_filter(ctx, radius, sigma, iterations, weight_type);
+}
+
+int DispEst::setLRCheck(int mode)
+{
+    if (!ctx) return -1;
+    const int rc = psm_set_lr_check(ctx, mode);
+    if (rc == PSM_OK) lr_mode = mode;
+    return rc;
 }
 
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
@@ -123,11 +133,15 @@ int DispEst::DispSelect_GPU()
 }
 
 // reference src/DispEst.cpp:338-344 -> PP::processDM (src/PP.cpp:402-425): the joint weighted-median filter of
-// both maps.  The reference runs it on the CPU even in GPU mode; here it is a device stage (psm_pp.cuh).
+// both maps, after the left-right check and fill that setLRCheck enables (PP.cpp:405-406, psm_lr.cuh).  The reference
+// runs it on the CPU even in GPU mode; here it is a device stage (psm_pp.cuh).
 int DispEst::PostProcess_GPU()
 {
     if (!ctx) return -1;
-    if (lDisMap.type() == CV_16UC1)
-        return psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, rDisMap.ptr<uint16_t>(), rDisMap.step);
-    return psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, rDisMap.ptr<uint8_t>(), rDisMap.step);
+    const int rc = lDisMap.type() == CV_16UC1
+        ? psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, rDisMap.ptr<uint16_t>(), rDisMap.step)
+        : psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, rDisMap.ptr<uint8_t>(), rDisMap.step);
+    if (rc || lr_mode == PSM_LR_OFF) return rc;
+    if (int e = psm_read_valid_mask(ctx, PSM_LEFT, lValid.ptr<uint8_t>(), lValid.step)) return e;
+    return psm_read_valid_mask(ctx, PSM_RIGHT, rValid.ptr<uint8_t>(), rValid.step);
 }

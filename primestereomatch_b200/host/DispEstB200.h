@@ -81,6 +81,8 @@ public:
     cv::Mat lDisMap;  // CV_8UC1, raw disparity index (reference DispEst.h:28-29); CV_16UC1 when maxDis > 256 (psm_create_u16),
                       // whose low byte is the reference's uchar map
     cv::Mat rDisMap;
+    cv::Mat lValid;   // CV_8UC1 masks of the left-right check (reference DispEst.h:81-82), 0/1; PostProcess_GPU fills them
+    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF
 
     int setInputImages(cv::Mat l, cv::Mat r);
     int setThreads(unsigned int newThreads);
@@ -94,6 +96,10 @@ public:
     // Weighted-median post-filter (JointWMF::filter's r, sigma, iter, weightType: PSM_WMF_*) for every later PostProcess
     // call; see psm_set_post_filter.  INTEGRATION.md: setPostFilter(MED_SZ/2, 25.5f, 1, PSM_WMF_EXP).
     int setPostFilter(int radius, float sigma, int iterations, int weight_type);
+    // Left-right consistency check and occlusion fill in front of (PSM_LR_FILL_WMF) or instead of (PSM_LR_FILL) the
+    // post-filter for every later PostProcess call; see psm_set_lr_check.  INTEGRATION.md: a build that restores
+    // PP.cpp:405-406 calls setLRCheck(PSM_LR_FILL_WMF).
+    int setLRCheck(int mode);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
@@ -125,5 +131,6 @@ private:
     int hei, wid, maxDis, threads;
     bool useOCL;
     unsigned int subsample_rate = 4;
+    int lr_mode = PSM_LR_OFF;
     psm_ctx* ctx = nullptr;
 };

@@ -2,11 +2,12 @@
 // (reference src/StereoMatch.cpp:198-241): setInputImages -> CostConst_GPU -> CostFilter_GPU ->
 // DispSelect_GPU -> PostProcess_GPU.  Raw I/O so it needs no image library:
 //   dispest_demo W H D left.f32 right.f32 out_left.u8 out_right.u8 [window eps [alpha tau_color tau_grad
-//                [radius sigma iterations weight]]]
+//                [radius sigma iterations weight [lr_mode]]]]
 // The optional window / eps go to setGuidedFilter (default: the reference's 8 and 0.0001f), the optional alpha and
 // thresholds to setMatchingCost (default: 0.9 inf inf, i.e. no truncation), the optional post-filter radius, sigma,
-// iterations and weight (exp, iv1, iv2 or off) to setPostFilter (default: 9 25.5 1 exp).  D up to 4096: above 256
-// the maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.
+// iterations and weight (exp, iv1, iv2 or off) to setPostFilter (default: 9 25.5 1 exp), the optional left-right check
+// mode (0 off, 1 check + fill + post-filter, 2 check + fill) to setLRCheck (default 0).  D up to 4096: above 256 the
+// maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -25,9 +26,9 @@ static bool read_all(const char* path, void* dst, size_t n)
 
 int main(int argc, char** argv)
 {
-    if (argc != 8 && argc != 10 && argc != 13 && argc != 17) {
+    if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
         std::fprintf(stderr, "usage: %s W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
-                             " [radius sigma iterations exp|iv1|iv2|off]]]\n", argv[0]);
+                             " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
     const int W = std::atoi(argv[1]), H = std::atoi(argv[2]), D = std::atoi(argv[3]);
@@ -41,12 +42,13 @@ int main(int argc, char** argv)
     int rc = argc >= 10 ? SMDE->setGuidedFilter(std::atoi(argv[8]), (float)std::atof(argv[9])) : 0;
     if (!rc && argc >= 13)
         rc = SMDE->setMatchingCost((float)std::atof(argv[10]), (float)std::atof(argv[11]), (float)std::atof(argv[12]));
-    if (!rc && argc == 17) {
+    if (!rc && argc >= 17) {
         const char* w = argv[16];
         const int wt = !std::strcmp(w, "exp") ? PSM_WMF_EXP : !std::strcmp(w, "iv1") ? PSM_WMF_IV1
                      : !std::strcmp(w, "iv2") ? PSM_WMF_IV2 : !std::strcmp(w, "off") ? PSM_WMF_OFF : -1;
         rc = SMDE->setPostFilter(std::atoi(argv[13]), (float)std::atof(argv[14]), std::atoi(argv[15]), wt);
     }
+    if (!rc && argc == 18) rc = SMDE->setLRCheck(std::atoi(argv[17]));
     if (!rc) rc = SMDE->CostConst_GPU();
     if (!rc) rc = SMDE->CostFilter_GPU();
     if (!rc) rc = SMDE->DispSelect_GPU();
