@@ -5,7 +5,7 @@ Frame: the synthetic 1920 x 1080 x 128 stereo pair of bench.py (both views), dev
 the same values, the like-for-like comparison of the two; (0.11, 0.21, 0.008) and (0.5, inf, inf) are other settings.
 Each configuration is timed in two alternating rounds.  Per configuration and round: ms per frame (set images -> CVC ->
 CVF -> WTA, CUDA events) and the median CVC stage time (psm_stage_ms stage 1), plus the raw volumes of a top row band
-against the CPU restatement tests/cost_oracle.py.  Quality: %BP (non-occluded, left map) of Cones and Teddy at D = 64 for
+against the CPU oracle at that setting.  Quality: %BP (non-occluded, left map) of Cones and Teddy at D = 64 for
 a small grid of settings, from the GPU maps (the metric of bench_gif_window.py).
 
 Usage: python bench_cost_params.py [--steps 20] [--warmup 3] [--no-quality]
@@ -20,7 +20,6 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 INF = float("inf")
 CONFIGS = [(0.9, INF, INF), (0.9, 1e30, 1e30), (0.11, 0.21, 0.008), (0.5, INF, INF)]
@@ -40,7 +39,6 @@ def main():
     from bench_gif_window import bad_pixels_nonocc, read_png
     from primestereomatch_b200 import DispEst, capi, synth
     from oracle import oracle as O
-    import cost_oracle as CO
     if not torch.cuda.is_available() or capi.lib().psm_device_count() < 1:
         raise SystemExit("bench_cost_params.py needs a CUDA device")
     W, H, D = 1920, 1080, 128
@@ -85,7 +83,7 @@ def main():
                 res["cvc_ms"].append(round(float(np.median(kms)), 4))
                 if len(res["cvc_ms"]) == 1:   # raw volumes of the top row band against the CPU restatement
                     de.CostConst_GPU()
-                    lv, rv = CO.cost_volumes(l[:band], r[:band], D, *cost)
+                    lv, rv = O.cost_const(l[:band], r[:band], D, alpha=cost[0], tau_color=cost[1], tau_grad=cost[2])[2:]
                     for d in band_ds:
                         ok = (np.array_equal(de.read_cost_slice(0, d)[:band], lv[d])
                               and np.array_equal(de.read_cost_slice(1, d)[:band], rv[d]))

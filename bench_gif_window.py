@@ -21,7 +21,6 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 CONFIGS = [(8, 1e-4), (8, 2e-4), (12, 1e-4), (16, 1e-4), (24, 1e-4), (32, 1e-4)]
 HBM_GBS = 3350.0   # H100 SXM data sheet
@@ -58,7 +57,6 @@ def main():
     from bench import device_info
     from primestereomatch_b200 import DispEst, capi, synth
     from oracle import oracle as O
-    import window_oracle as WO
     if not torch.cuda.is_available() or capi.lib().psm_device_count() < 1:
         raise SystemExit("bench_gif_window.py needs a CUDA device")
     W, H, D = 1920, 1080, 128
@@ -96,13 +94,13 @@ def main():
             for _ in range(args.steps):   # kernel time of the filter alone (psm_stage_ms waits for each frame)
                 frame()
                 kms.append(de.stage_ms(4))
-            # maps of the top row band against the CPU restatement (oracle raw costs + any-window filter + WTA)
+            # maps of the top row band against the CPU oracle at this window (raw costs + filter + WTA)
             de.DispSelect_GPU()
             band = 32
             c1 = band + 2 * window + 8
             _, _, lraw, rraw = O.cost_const(np.ascontiguousarray(l[:c1]), np.ascontiguousarray(r[:c1]), D)
-            lf, rf = WO.cost_filter(l[:c1], r[:c1], lraw, rraw, window, eps)
-            parity = bool(np.array_equal(de.lDisMap[:band], WO.wta(lf)[:band]) and np.array_equal(de.rDisMap[:band], WO.wta(rf)[:band]))
+            lf, rf = O.cost_filter(l[:c1], r[:c1], lraw, rraw, window=window, eps=eps)
+            parity = bool(np.array_equal(de.lDisMap[:band], O.wta(lf)[:band]) and np.array_equal(de.rDisMap[:band], O.wta(rf)[:band]))
             kernel_ms = float(np.median(kms))
             results.append({"window": window, "eps": eps, "path": "tuned 8x8" if (window, eps) == (8, 1e-4) else "generic",
                             "ms_per_frame": round(ms_frame, 3), "cvf_kernel_ms": round(kernel_ms, 3),

@@ -21,6 +21,9 @@ _f64p = np.ctypeslib.ndpointer(dtype=np.float64, flags="C_CONTIGUOUS")
 WEIGHTS = {"exp": 0, "iv1": 1, "iv2": 2, "off": 5}
 _PP_TABLE_MAX = 3 * 63 * 63 + 1
 _MAP_BYTES = {np.dtype(np.uint8): 1, np.dtype(np.uint16): 2}
+# The reference's compile-time constants (ORC_GIF_R_WIN, ORC_GIF_EPS, ORC_ALPHA, no truncation) are the defaults of the
+# keyword arguments window, eps, alpha, tau_color and tau_grad below.
+INF = float("inf")
 
 
 def build():
@@ -41,26 +44,27 @@ def lib():
         L.orc_cvc_preprocess.argtypes = [_f32p, C.c_int, C.c_int, _f32p, C.c_int]
         for fn in (L.orc_buildcv_left, L.orc_buildcv_right):
             fn.argtypes = [_f32p, _f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, _f32p]
-        L.orc_box8.argtypes = [_f32p, C.c_int, C.c_int, _f32p]
-        L.orc_cvf_preprocess.argtypes = [_f32p, C.c_int, C.c_int, _f32p, _f32p, _f32p]
-        L.orc_guided_filter.argtypes = [_f32p, _f32p, _f32p, C.c_int, C.c_int, _f32p,
-                                        C.c_void_p, C.c_void_p]
+        for fn in (L.orc_box, L.orc_box_k):
+            fn.argtypes = [_f32p, C.c_int, C.c_int, C.c_int, _f32p]
+        L.orc_cvf_preprocess.argtypes = [_f32p, C.c_int, C.c_int, C.c_int, _f32p, _f32p, _f32p]
+        L.orc_guided_filter.argtypes = [_f32p, _f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_float, _f32p, _f32p, _f32p]
         L.orc_wta.argtypes = [_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int]
-        L.orc_cost_const.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                     _f32p, _f32p, _f32p, _f32p]
-        L.orc_cost_filter.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int,
+        L.orc_cost_const.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                     C.c_float, C.c_float, C.c_float, _f32p, _f32p, _f32p, _f32p]
+        L.orc_cost_filter.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                       _f32p, _f32p]
         L.orc_disp_select.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, _u8p, _u8p]
         L.orc_pipeline.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                   C.c_float, C.c_float, C.c_float, C.c_int, C.c_float,
                                    _f32p, _f32p, _u8p, _u8p, _f64p]
-        L.orc_cost_filter_fgf.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _f32p, _f32p]
-        L.orc_cost_filter_fgf.restype = C.c_int
+        L.orc_cost_filter_fgf.argtypes = [_f32p, _f32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                          _f32p, _f32p]
         L.orc_pp_weight_table.argtypes = [C.c_float, C.c_int, _u32p]
         L.orc_wmf.argtypes = [C.c_void_p, C.c_int, _u8p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int,
                               C.c_void_p]
         L.orc_f32_to_u8x255.argtypes = [_f32p, _u8p, C.c_size_t]
-        for name in ("orc_cost_const", "orc_cost_filter", "orc_disp_select", "orc_pipeline", "orc_pp_weight_table",
-                     "orc_wmf"):
+        for name in ("orc_cost_const", "orc_cost_filter", "orc_cost_filter_fgf", "orc_disp_select", "orc_pipeline",
+                     "orc_pp_weight_table", "orc_wmf"):
             getattr(L, name).restype = C.c_int
         _LIB = L
     return _LIB
@@ -101,37 +105,51 @@ def cvc_preprocess(img3, gray_mode=0):
     return out
 
 
-def box8(src):
+def box(src, K):
+    """cv::boxFilter(src, -1, (K, K)) of one plane, in OpenCV's order of fp64 operations (orc_box)"""
     src = _c(src)
     H, W = src.shape
     out = np.empty((H, W), np.float32)
-    lib().orc_box8(src, W, H, out)
+    lib().orc_box(src, W, H, K, out)
     return out
 
 
-def cvf_preprocess(img3):
+def box8(src):
+    return box(src, 8)
+
+
+def box_direct(src, K):
+    """the Fast Guided Filter's K x K box of one plane: direct fp64 sums (orc_box_k; stereo_oracle.h says when it equals
+    box)"""
+    src = _c(src)
+    H, W = src.shape
+    out = np.empty((H, W), np.float32)
+    lib().orc_box_k(src, W, H, K, out)
+    return out
+
+
+def cvf_preprocess(img3, *, window=8):
     """-> rgb[3,H,W], mean[3,H,W], var[6,H,W]"""
     img3 = _c(img3)
     H, W, _ = img3.shape
     rgb = np.empty((3, H, W), np.float32)
     mean = np.empty((3, H, W), np.float32)
     var = np.empty((6, H, W), np.float32)
-    lib().orc_cvf_preprocess(img3, W, H, rgb, mean, var)
+    lib().orc_cvf_preprocess(img3, W, H, window, rgb, mean, var)
     return rgb, mean, var
 
 
-def guided_filter(rgb, mean, var, p, want_ab=False):
-    """-> q  (or (q, a[3,H,W], b[H,W]) with want_ab)"""
-    p = _c(p).copy()
-    H, W = p.shape
-    if want_ab:
-        a = np.empty((3, H, W), np.float32)
-        b = np.empty((H, W), np.float32)
-        lib().orc_guided_filter(_c(rgb), _c(mean), _c(var), W, H, p,
-                                a.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p))
-        return p, a, b
-    lib().orc_guided_filter(_c(rgb), _c(mean), _c(var), W, H, p, None, None)
-    return p
+def guided_filter(rgb, mean, var, p, want_ab=False, *, window=8, eps=1e-4):
+    """GuidedFilter_cv of one slice p[H,W] or of every slice of a volume p[D,H,W]
+    -> q  (or (q, a[3,H,W], b[H,W]) with want_ab; a[D,3,H,W], b[D,H,W] for a volume)"""
+    rgb, mean, var = _c(rgb), _c(mean), _c(var)
+    q = _c(p).copy()
+    H, W = q.shape[-2:]
+    a = np.empty(q.shape[:-2] + (3, H, W), np.float32)
+    b = np.empty(q.shape, np.float32)
+    for qs, as_, bs in zip(q.reshape(-1, H, W), a.reshape(-1, 3, H, W), b.reshape(-1, H, W)):
+        lib().orc_guided_filter(rgb, mean, var, W, H, window, eps, qs, as_, bs)
+    return (q, a, b) if want_ab else q
 
 
 def _map_bytes(dtype):
@@ -150,25 +168,27 @@ def wta(vol, dtype=np.uint8):
     return out
 
 
-def cost_const(l, r, D, threads=8, gray_mode=0):
-    """-> lGrd, rGrd, lVol[D,H,W], rVol[D,H,W]  (raw cost volumes)"""
+def cost_const(l, r, D, threads=8, gray_mode=0, *, alpha=0.9, tau_color=INF, tau_grad=INF, d_begin=0, d_count=None):
+    """-> lGrd, rGrd, lVol, rVol  (raw cost volumes [d_count,H,W] of the disparities [d_begin, d_begin + d_count), all
+    of [0, D) by default)"""
     l, r = _c(l), _c(r)
     H, W, _ = l.shape
+    d_count = D - d_begin if d_count is None else d_count
     lg = np.empty((H, W), np.float32)
     rg = np.empty((H, W), np.float32)
-    lv = np.empty((D, H, W), np.float32)
-    rv = np.empty((D, H, W), np.float32)
-    rc = lib().orc_cost_const(l, r, W, H, D, threads, gray_mode, lg, rg, lv, rv)
+    lv = np.empty((d_count, H, W), np.float32)
+    rv = np.empty((d_count, H, W), np.float32)
+    rc = lib().orc_cost_const(l, r, W, H, d_begin, d_count, threads, gray_mode, alpha, tau_color, tau_grad, lg, rg, lv, rv)
     assert rc == 0
     return lg, rg, lv, rv
 
 
-def cost_filter(l, r, lv, rv, threads=8):
+def cost_filter(l, r, lv, rv, threads=8, *, window=8, eps=1e-4):
     """filters copies of the volumes -> lVolF, rVolF"""
     l, r = _c(l), _c(r)
     lv, rv = _c(lv).copy(), _c(rv).copy()
     D, H, W = lv.shape
-    rc = lib().orc_cost_filter(l, r, W, H, D, threads, lv, rv)
+    rc = lib().orc_cost_filter(l, r, W, H, D, threads, window, eps, lv, rv)
     assert rc == 0
     return lv, rv
 
@@ -182,7 +202,8 @@ def disp_select(lv, rv):
     return ld, rd
 
 
-def pipeline(l, r, D, threads=8, gray_mode=0, keep_volumes=False):
+def pipeline(l, r, D, threads=8, gray_mode=0, keep_volumes=False, *, alpha=0.9, tau_color=INF, tau_grad=INF, window=8,
+             eps=1e-4):
     """Full CVC->CVF->WTA.  -> dict(lDis, rDis, times_ms=[cvc,cvf,wta], [lVol, rVol])"""
     l, r = _c(l), _c(r)
     H, W, _ = l.shape
@@ -191,7 +212,7 @@ def pipeline(l, r, D, threads=8, gray_mode=0, keep_volumes=False):
     ld = np.empty((H, W), np.uint8)
     rd = np.empty((H, W), np.uint8)
     t = np.zeros(3, np.float64)
-    rc = lib().orc_pipeline(l, r, W, H, D, threads, gray_mode, lv, rv, ld, rd, t)
+    rc = lib().orc_pipeline(l, r, W, H, D, threads, gray_mode, alpha, tau_color, tau_grad, window, eps, lv, rv, ld, rd, t)
     assert rc == 0
     out = {"lDis": ld, "rDis": rd, "times_ms": t.tolist()}
     if keep_volumes:
@@ -229,11 +250,11 @@ def post_process(img3_f32, disp, r=9, sigma=25.5, iterations=1, weight="exp", th
     return out
 
 
-def cost_filter_fgf(l, r, lv, rv, s=4, threads=8):
-    """DispEst::CostFilter_FGF (Fast Guided Filter, sub-sampling rate s) on copies of the volumes -> lVolF, rVolF"""
+def cost_filter_fgf(l, r, lv, rv, s=4, threads=8, *, window=8, eps=1e-4):
+    """DispEst::CostFilter_FGF (FastGuidedFilter(img, window, eps, s)) on copies of the volumes -> lVolF, rVolF"""
     l, r = _c(l), _c(r)
     lv, rv = _c(lv).copy(), _c(rv).copy()
     D, H, W = lv.shape
-    rc = lib().orc_cost_filter_fgf(l, r, W, H, D, threads, s, lv, rv)
+    rc = lib().orc_cost_filter_fgf(l, r, W, H, D, threads, s, window, eps, lv, rv)
     assert rc == 0
     return lv, rv

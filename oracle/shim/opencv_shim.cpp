@@ -182,14 +182,14 @@ void boxFilter(const Mat& src, Mat& dst, int ddepth, Size ksize)
     need(src.type() == CV_32FC1 && ddepth == -1 && ksize.width == ORC_GIF_R_WIN && ksize.height == ORC_GIF_R_WIN,
          "boxFilter(CV_32FC1, -1, Size(8,8))");
     const int rows = src.rows, cols = src.cols;
-    if (src.step == (size_t)cols * sizeof(float)) {   // packed rows: filter straight into the destination (orc_box8 allows src == dst)
+    if (src.step == (size_t)cols * sizeof(float)) {   // packed rows: filter straight into the destination (orc_box allows src == dst)
         const Mat keep = src;                          // dst may be the same header as src
         dst.create(rows, cols, CV_32FC1);
-        orc_box8(keep.ptr<float>(0), cols, rows, dst.ptr<float>(0));
+        orc_box(keep.ptr<float>(0), cols, rows, ksize.width, dst.ptr<float>(0));
         return;
     }
     std::vector<float> in = packed(src), out(in.size());
-    orc_box8(in.data(), cols, rows, out.data());
+    orc_box(in.data(), cols, rows, ksize.width, out.data());
     unpack(out, dst, rows, cols);
 }
 

@@ -95,28 +95,38 @@ void orc_cvc_preprocess(const float* img3, int W, int H, float* grdx, int gray_m
 
 /* ------------------------------------------------------------------ a3/a4: myCostGrd */
 
+/* CVC.cpp:24-27 / 36-39 with the truncation the reference leaves commented out restored: a NaN difference is not above
+ * any threshold and stays NaN, +inf truncates nothing; every float operation is rounded separately. */
+static inline float cost_weigh(float clrDiff, float grdDiff, float alpha, float tau_color, float tau_grad)
+{
+    if (clrDiff > tau_color) clrDiff = tau_color;
+    if (grdDiff > tau_grad) grdDiff = tau_grad;
+    return alpha * clrDiff + (1 - alpha) * grdDiff;
+}
+
 /* CVC.cpp:18-27: all-float arithmetic (math.h in C++ gives fabs(float) -> float). */
-static inline float cost_grd4(const float* lC, const float* rC, const float* lG, const float* rG)
+static inline float cost_grd4(const float* lC, const float* rC, const float* lG, const float* rG,
+                              float alpha, float tau_color, float tau_grad)
 {
     float clrDiff = fabsf(lC[0] - rC[0]) + fabsf(lC[1] - rC[1]) + fabsf(lC[2] - rC[2]);
     float grdDiff = fabsf(*lG - *rG);
-    return 0.9f * clrDiff + (1 - 0.9f) * grdDiff; /* ALPHA_32F 0.9f, CVC.h:22 */
+    return cost_weigh(clrDiff, grdDiff, alpha, tau_color, tau_grad);
 }
 
 /* CVC.cpp:30-39: BC_32F is the double literal 1.0 (CVC.h:12), so the differences, fabs and
  * the three-term sum are evaluated in double and rounded to float once per assignment. */
-static inline float cost_grd2(const float* lC, const float* lG)
+static inline float cost_grd2(const float* lC, const float* lG, float alpha, float tau_color, float tau_grad)
 {
     float clrDiff = (float)(fabs((double)lC[0] - 1.0) + fabs((double)lC[1] - 1.0) + fabs((double)lC[2] - 1.0));
     float grdDiff = (float)fabs((double)*lG - 1.0);
-    return 0.9f * clrDiff + (1 - 0.9f) * grdDiff;
+    return cost_weigh(clrDiff, grdDiff, alpha, tau_color, tau_grad);
 }
 
 /* ------------------------------------------------------------------ a5/a6: buildCV */
 
 /* CVC.cpp:122-149 */
-void orc_buildcv_left(const float* lImg, const float* rImg, const float* lGrd, const float* rGrd,
-                      int W, int H, int d, float* cost)
+static void buildcv_left(const float* lImg, const float* rImg, const float* lGrd, const float* rGrd,
+                         int W, int H, int d, float alpha, float tau_color, float tau_grad, float* cost)
 {
     for (int y = 0; y < H; ++y) {
         const float* lData = lImg + (size_t)y * W * 3;
@@ -125,15 +135,15 @@ void orc_buildcv_left(const float* lImg, const float* rImg, const float* lGrd, c
         const float* rGData = rGrd + (size_t)y * W;
         float* c = cost + (size_t)y * W;
         for (int x = d; x < W; ++x)
-            c[x] = cost_grd4(lData + 3 * x, rData + 3 * (x - d), lGData + x, rGData + x - d);
+            c[x] = cost_grd4(lData + 3 * x, rData + 3 * (x - d), lGData + x, rGData + x - d, alpha, tau_color, tau_grad);
         for (int x = 0; x < d && x < W; ++x)
-            c[x] = cost_grd2(lData + 3 * x, lGData + x);
+            c[x] = cost_grd2(lData + 3 * x, lGData + x, alpha, tau_color, tau_grad);
     }
 }
 
 /* CVC.cpp:151-179 */
-void orc_buildcv_right(const float* lImg, const float* rImg, const float* lGrd, const float* rGrd,
-                       int W, int H, int d, float* cost)
+static void buildcv_right(const float* lImg, const float* rImg, const float* lGrd, const float* rGrd,
+                          int W, int H, int d, float alpha, float tau_color, float tau_grad, float* cost)
 {
     int border = W - d;
     if (border < 0) border = 0;
@@ -144,22 +154,41 @@ void orc_buildcv_right(const float* lImg, const float* rImg, const float* lGrd, 
         const float* rGData = rGrd + (size_t)y * W;
         float* c = cost + (size_t)y * W;
         for (int x = 0; x < border; ++x)
-            c[x] = cost_grd4(lData + 3 * x, rData + 3 * (x + d), lGData + x, rGData + x + d);
+            c[x] = cost_grd4(lData + 3 * x, rData + 3 * (x + d), lGData + x, rGData + x + d, alpha, tau_color, tau_grad);
         for (int x = border; x < W; ++x)
-            c[x] = cost_grd2(lData + 3 * x, lGData + x);
+            c[x] = cost_grd2(lData + 3 * x, lGData + x, alpha, tau_color, tau_grad);
     }
 }
 
-/* ------------------------------------------------------------------ a10: cv::boxFilter 8x8 */
-
-/* OpenCV box filter for CV_32F, normalize=true, ksize 8x8, default anchor (4,4),
- * BORDER_REFLECT_101.  Restates modules/imgproc/src/box_filter.simd.hpp:
- *   RowSum<float,double>:   s = sum of first 8 (double); then s += (double)S[i+8] - (double)S[i]
- *   ColumnSum<double,float>: s0 = SUM + newest; dst = (float)(s0 * (1.0/64)); SUM = s0 - oldest
- * Rows are padded 4 left / 3 right, the column pass sees rows y-4 .. y+3 (reflected). */
-void orc_box8(const float* src, int W, int H, float* dst)
+/* the reference's own entry points: its signatures, its constants */
+void orc_buildcv_left(const float* lImg, const float* rImg, const float* lGrd, const float* rGrd,
+                      int W, int H, int d, float* cost)
 {
-    const int K = ORC_GIF_R_WIN, AL = 4;
+    buildcv_left(lImg, rImg, lGrd, rGrd, W, H, d, ORC_ALPHA, INFINITY, INFINITY, cost);
+}
+
+void orc_buildcv_right(const float* lImg, const float* rImg, const float* lGrd, const float* rGrd,
+                       int W, int H, int d, float* cost)
+{
+    buildcv_right(lImg, rImg, lGrd, rGrd, W, H, d, ORC_ALPHA, INFINITY, INFINITY, cost);
+}
+
+/* ------------------------------------------------------------------ a10: cv::boxFilter K x K */
+
+/* OpenCV box filter for CV_32F, normalize=true, ksize K x K, default anchor (K/2, K/2), BORDER_REFLECT_101 with any
+ * overshoot (images smaller than the window).  Restates modules/imgproc/src/box_filter.simd.hpp:
+ *   K == 1:                 a copy
+ *   RowSum<float,double>:   K <= 5: S[i] + S[i+1] + ... + S[i+K-1], left to right;
+ *                           above:  s = sum of the first K (double); then s += (double)S[i+K] - (double)S[i]
+ *   ColumnSum<double,float>: s0 = SUM + newest; dst = (float)(s0 * (1.0/(K*K))); SUM = s0 - oldest
+ * Rows are padded K/2 left / K-1-K/2 right, the column pass sees rows y-K/2 .. y+K-1-K/2 (reflected). */
+void orc_box(const float* src, int W, int H, int K, float* dst)
+{
+    if (K == 1) {
+        if (dst != src) memcpy(dst, src, (size_t)W * H * sizeof(float));
+        return;
+    }
+    const int AL = K / 2;
     const double scale = 1.0 / (double)(K * K);
     const int PW = W + K - 1;
     float* prow = (float*)malloc((size_t)PW * sizeof(float));
@@ -170,6 +199,14 @@ void orc_box8(const float* src, int W, int H, float* dst)
         const float* s = src + (size_t)y * W;
         for (int i = 0; i < PW; ++i) prow[i] = s[reflect101(i - AL, W)];
         double* D = rs + (size_t)y * W;
+        if (K <= 5) {
+            for (int i = 0; i < W; ++i) {
+                double acc = (double)prow[i];
+                for (int j = 1; j < K; ++j) acc += (double)prow[i + j];
+                D[i] = acc;
+            }
+            continue;
+        }
         double acc = 0;
         for (int i = 0; i < K; ++i) acc += (double)prow[i];
         D[0] = acc;
@@ -178,7 +215,7 @@ void orc_box8(const float* src, int W, int H, float* dst)
             D[i + 1] = acc;
         }
     }
-    /* column pass; padded row index r = y' + 4 maps to source row reflect101(y', H) */
+    /* column pass; padded row index r = y' + AL maps to source row reflect101(y', H) */
     for (int r = 0; r < K - 1; ++r) {
         const double* Sp = rs + (size_t)reflect101(r - AL, H) * W;
         for (int i = 0; i < W; ++i) SUM[i] += Sp[i];
@@ -187,8 +224,8 @@ void orc_box8(const float* src, int W, int H, float* dst)
     float* tmp = NULL;
     if (src == dst) { tmp = (float*)malloc((size_t)W * H * sizeof(float)); out = tmp; }
     for (int y = 0; y < H; ++y) {
-        const double* Sp = rs + (size_t)reflect101(y + K - 1 - AL, H) * W; /* newest: y+3 */
-        const double* Sm = rs + (size_t)reflect101(y - AL, H) * W;         /* oldest: y-4 */
+        const double* Sp = rs + (size_t)reflect101(y + K - 1 - AL, H) * W; /* newest */
+        const double* Sm = rs + (size_t)reflect101(y - AL, H) * W;         /* oldest */
         float* D = out + (size_t)y * W;
         for (int i = 0; i < W; ++i) {
             double s0 = SUM[i] + Sp[i];
@@ -203,20 +240,20 @@ void orc_box8(const float* src, int W, int H, float* dst)
 /* ------------------------------------------------------------------ a8: CVF::preprocess */
 
 /* CVF.cpp:44-70 */
-void orc_cvf_preprocess(const float* img3, int W, int H, float* rgb, float* mean, float* var)
+void orc_cvf_preprocess(const float* img3, int W, int H, int window, float* rgb, float* mean, float* var)
 {
     const size_t n = (size_t)W * H;
     for (size_t i = 0; i < n; ++i)                 /* split(), CVF.cpp:47 */
         for (int c = 0; c < 3; ++c) rgb[c * n + i] = img3[3 * i + c];
     for (int c = 0; c < 3; ++c)                    /* CVF.cpp:49-51 */
-        orc_box8(rgb + c * n, W, H, mean + c * n);
+        orc_box(rgb + c * n, W, H, window, mean + c * n);
     float* tmp = (float*)malloc(n * sizeof(float));
     int varIdx = 0;
     for (int c = 0; c < 3; ++c) {                  /* CVF.cpp:60-69 */
         for (int cp = c; cp < 3; ++cp) {
             float* v = var + (size_t)varIdx * n;
             for (size_t i = 0; i < n; ++i) tmp[i] = rgb[c * n + i] * rgb[cp * n + i];
-            orc_box8(tmp, W, H, v);
+            orc_box(tmp, W, H, window, v);
             for (size_t i = 0; i < n; ++i) tmp[i] = mean[c * n + i] * mean[cp * n + i];
             for (size_t i = 0; i < n; ++i) v[i] -= tmp[i];
             ++varIdx;
@@ -228,7 +265,7 @@ void orc_cvf_preprocess(const float* img3, int W, int H, float* rgb, float* mean
 /* ------------------------------------------------------------------ a9: GuidedFilter_cv */
 
 /* CVF.cpp:72-165 */
-void orc_guided_filter(const float* rgb, const float* mean_I, const float* var_I, int W, int H,
+void orc_guided_filter(const float* rgb, const float* mean_I, const float* var_I, int W, int H, int window, float eps,
                        float* p, float* a_out, float* b_out)
 {
     const size_t n = (size_t)W * H;
@@ -238,10 +275,10 @@ void orc_guided_filter(const float* rgb, const float* mean_I, const float* var_I
     float* a = (float*)malloc(3 * n * sizeof(float));
     float* q = (float*)malloc(n * sizeof(float));
 
-    orc_box8(p, W, H, mean_p);                                   /* CVF.cpp:81-82 */
+    orc_box(p, W, H, window, mean_p);                                  /* CVF.cpp:81-82 */
     for (int c = 0; c < 3; ++c) {                                /* CVF.cpp:86-89 */
         for (size_t i = 0; i < n; ++i) tmp[i] = rgb[c * n + i] * p[i];
-        orc_box8(tmp, W, H, mean_Ip + c * n);
+        orc_box(tmp, W, H, window, mean_Ip + c * n);
     }
     for (int c = 0; c < 3; ++c) {                                /* CVF.cpp:92-95 */
         for (size_t i = 0; i < n; ++i) tmp[i] = mean_I[c * n + i] * mean_p[i];
@@ -250,15 +287,15 @@ void orc_guided_filter(const float* rgb, const float* mean_I, const float* var_I
     const float* cov = mean_Ip;
     for (size_t i = 0; i < n; ++i) {                             /* CVF.cpp:102-149 */
         float c0 = cov[i], c1 = cov[n + i], c2 = cov[2 * n + i];
-        float a11 = var_I[i] + ORC_GIF_EPS;
+        float a11 = var_I[i] + eps;
         float a12 = var_I[n + i];
         float a13 = var_I[2 * n + i];
         float a21 = var_I[n + i];
-        float a22 = var_I[3 * n + i] + ORC_GIF_EPS;
+        float a22 = var_I[3 * n + i] + eps;
         float a23 = var_I[4 * n + i];
         float a31 = var_I[2 * n + i];
         float a32 = var_I[4 * n + i];
-        float a33 = var_I[5 * n + i] + ORC_GIF_EPS;
+        float a33 = var_I[5 * n + i] + eps;
         float DET = a11 * (a33 * a22 - a32 * a23) -
                     a21 * (a33 * a12 - a32 * a13) +
                     a31 * (a23 * a12 - a22 * a13);
@@ -283,9 +320,9 @@ void orc_guided_filter(const float* rgb, const float* mean_I, const float* var_I
     if (a_out) memcpy(a_out, a, 3 * n * sizeof(float));
     if (b_out) memcpy(b_out, mean_p, n * sizeof(float));
 
-    orc_box8(mean_p, W, H, q);                                   /* CVF.cpp:157-158 */
+    orc_box(mean_p, W, H, window, q);                                 /* CVF.cpp:157-158 */
     for (int c = 0; c < 3; ++c) {                                /* CVF.cpp:159-163 */
-        orc_box8(a + c * n, W, H, tmp);
+        orc_box(a + c * n, W, H, window, tmp);
         for (size_t i = 0; i < n; ++i) tmp[i] = tmp[i] * rgb[c * n + i];
         for (size_t i = 0; i < n; ++i) q[i] += tmp[i];
     }
@@ -336,6 +373,9 @@ typedef struct {
     const uint32_t* lut;
     int r, wtype, nbins;
     uint16_t* wmf_out;
+    float alpha, tau_color, tau_grad;   /* kinds 0, 1 */
+    int window;                         /* kind 2 */
+    float eps;
     int W, H, D, d, y0, y1;
 } task_t;
 
@@ -345,9 +385,9 @@ static void* task_entry(void* arg)
 {
     task_t* t = (task_t*)arg;
     switch (t->kind) {
-    case 0: orc_buildcv_left(t->lImg, t->rImg, t->lGrd, t->rGrd, t->W, t->H, t->d, t->slice); break;
-    case 1: orc_buildcv_right(t->lImg, t->rImg, t->lGrd, t->rGrd, t->W, t->H, t->d, t->slice); break;
-    case 2: orc_guided_filter(t->rgb, t->mean, t->var, t->W, t->H, t->slice, NULL, NULL); break;
+    case 0: buildcv_left(t->lImg, t->rImg, t->lGrd, t->rGrd, t->W, t->H, t->d, t->alpha, t->tau_color, t->tau_grad, t->slice); break;
+    case 1: buildcv_right(t->lImg, t->rImg, t->lGrd, t->rGrd, t->W, t->H, t->d, t->alpha, t->tau_color, t->tau_grad, t->slice); break;
+    case 2: orc_guided_filter(t->rgb, t->mean, t->var, t->W, t->H, t->window, t->eps, t->slice, NULL, NULL); break;
     case 3: wta_rows(t->vol_in, t->W, t->H, t->D, t->disp, t->map_bytes, t->y0, t->y1); break;
     case 4: return wmf_rows(t);
     }
@@ -399,35 +439,37 @@ static int run_rows(task_t proto, int H, int threads)
     return rc;
 }
 
-/* DispEst.cpp:222-270 */
-int orc_cost_const(const float* lImg, const float* rImg, int W, int H, int D, int threads,
-                   int gray_mode, float* lGrd, float* rGrd, float* lVol, float* rVol)
+/* DispEst.cpp:222-270, the slices of the disparities [d_begin, d_begin + d_count) */
+int orc_cost_const(const float* lImg, const float* rImg, int W, int H, int d_begin, int d_count, int threads,
+                   int gray_mode, float alpha, float tau_color, float tau_grad,
+                   float* lGrd, float* rGrd, float* lVol, float* rVol)
 {
     const size_t n = (size_t)W * H;
     orc_cvc_preprocess(lImg, W, H, lGrd, gray_mode);   /* DispEst.cpp:232 */
     orc_cvc_preprocess(rImg, W, H, rGrd, gray_mode);   /* DispEst.cpp:233 */
-    task_t* tasks = (task_t*)calloc((size_t)D, sizeof(task_t));
-    for (int d = 0; d < D; ++d) {                      /* DispEst.cpp:243 */
+    task_t* tasks = (task_t*)calloc((size_t)d_count, sizeof(task_t));
+    for (int i = 0; i < d_count; ++i) {                /* DispEst.cpp:243 */
         task_t t = {0};
         t.kind = 0; t.lImg = lImg; t.rImg = rImg; t.lGrd = lGrd; t.rGrd = rGrd;
-        t.W = W; t.H = H; t.d = d; t.slice = lVol + (size_t)d * n;
-        tasks[d] = t;
+        t.alpha = alpha; t.tau_color = tau_color; t.tau_grad = tau_grad;
+        t.W = W; t.H = H; t.d = d_begin + i; t.slice = lVol + (size_t)i * n;
+        tasks[i] = t;
     }
-    int rc = run_batched(tasks, D, threads);
-    for (int d = 0; d < D && rc == 0; ++d) {           /* DispEst.cpp:260: swapped arguments */
-        task_t t = {0};
+    int rc = run_batched(tasks, d_count, threads);
+    for (int i = 0; i < d_count && rc == 0; ++i) {     /* DispEst.cpp:260: swapped arguments */
+        task_t t = tasks[i];
         t.kind = 1; t.lImg = rImg; t.rImg = lImg; t.lGrd = rGrd; t.rGrd = lGrd;
-        t.W = W; t.H = H; t.d = d; t.slice = rVol + (size_t)d * n;
-        tasks[d] = t;
+        t.slice = rVol + (size_t)i * n;
+        tasks[i] = t;
     }
-    if (rc == 0) rc = run_batched(tasks, D, threads);
+    if (rc == 0) rc = run_batched(tasks, d_count, threads);
     free(tasks);
     return rc;
 }
 
 /* Reconstructed CostFilter_CPU (declared DispEst.h:42, never defined): CVF::preprocess per
  * view (CVF.cpp:44) then one filterCV_thread per d (CVF.cpp:28-41) in CostConst_CPU batches. */
-int orc_cost_filter(const float* lImg, const float* rImg, int W, int H, int D, int threads,
+int orc_cost_filter(const float* lImg, const float* rImg, int W, int H, int D, int threads, int window, float eps,
                     float* lVol, float* rVol)
 {
     const size_t n = (size_t)W * H;
@@ -436,11 +478,11 @@ int orc_cost_filter(const float* lImg, const float* rImg, int W, int H, int D, i
     task_t* tasks = (task_t*)calloc((size_t)D, sizeof(task_t));
     int rc = 0;
     for (int view = 0; view < 2 && rc == 0; ++view) {
-        orc_cvf_preprocess(view == 0 ? lImg : rImg, W, H, rgb, mean, var);
+        orc_cvf_preprocess(view == 0 ? lImg : rImg, W, H, window, rgb, mean, var);
         float* vol = view == 0 ? lVol : rVol;
         for (int d = 0; d < D; ++d) {
             task_t t = {0};
-            t.kind = 2; t.rgb = rgb; t.mean = mean; t.var = var;
+            t.kind = 2; t.rgb = rgb; t.mean = mean; t.var = var; t.window = window; t.eps = eps;
             t.W = W; t.H = H; t.d = d; t.slice = vol + (size_t)d * n;
             tasks[d] = t;
         }
@@ -467,16 +509,16 @@ int orc_disp_select(const float* lVol, const float* rVol, int W, int H, int D,
 }
 
 int orc_pipeline(const float* lImg, const float* rImg, int W, int H, int D, int threads,
-                 int gray_mode, float* lVol, float* rVol, uint8_t* lDis, uint8_t* rDis,
-                 double* times_ms)
+                 int gray_mode, float alpha, float tau_color, float tau_grad, int window, float eps,
+                 float* lVol, float* rVol, uint8_t* lDis, uint8_t* rDis, double* times_ms)
 {
     const size_t n = (size_t)W * H;
     float* lGrd = (float*)malloc(n * sizeof(float));
     float* rGrd = (float*)malloc(n * sizeof(float));
     double t0 = now_ms();
-    int rc = orc_cost_const(lImg, rImg, W, H, D, threads, gray_mode, lGrd, rGrd, lVol, rVol);
+    int rc = orc_cost_const(lImg, rImg, W, H, 0, D, threads, gray_mode, alpha, tau_color, tau_grad, lGrd, rGrd, lVol, rVol);
     double t1 = now_ms();
-    if (rc == 0) rc = orc_cost_filter(lImg, rImg, W, H, D, threads, lVol, rVol);
+    if (rc == 0) rc = orc_cost_filter(lImg, rImg, W, H, D, threads, window, eps, lVol, rVol);
     double t2 = now_ms();
     if (rc == 0) rc = wta_view(lVol, W, H, D, lDis, threads);
     if (rc == 0) rc = wta_view(rVol, W, H, D, rDis, threads);
@@ -608,8 +650,8 @@ void orc_f32_to_u8x255(const float* src, uint8_t* dst, size_t n)
 
 /* ------------------------------------------------------------------------------------------------------------
  * Fast Guided Filter branch: FastGuidedFilterColor (src/fastguidedfilter.cpp:121-198) as driven by
- * DispEst::CostFilter_FGF (src/DispEst.cpp:281-296): FastGuidedFilter(img, GIF_R_WIN, GIF_EPS, s) -> box size
- * K = 2*(8/s)+1 on the s-times sub-sampled planes (:206-208).
+ * DispEst::CostFilter_FGF (src/DispEst.cpp:281-296): FastGuidedFilter(img, window, eps, s) -> box size
+ * K = 2*(window/s)+1 on the s-times sub-sampled planes (:206-208).
  * OpenCV primitives restated from OpenCV's own implementation and pinned against cv2 4.13 (IPP off) by
  * tests/golden/make_golden_fgf.py: cv::blur == normalised K x K box, anchor K/2, BORDER_REFLECT_101, double
  * accumulation, * (1.0/(K*K)) in double, one rounding; cv::resize INTER_NN: x -> min(floor(x * (1/(w2/W))), W-1);
@@ -657,10 +699,10 @@ static void fgf_free(fgf_guide* g)
     free(g->xs); free(g->ys); free(g->lx0); free(g->lx1); free(g->ly0); free(g->ly1); free(g->fx); free(g->fy);
 }
 
-static void fgf_build(fgf_guide* g, const float* img3, int W, int H, int s, float eps)
+static void fgf_build(fgf_guide* g, const float* img3, int W, int H, int s, int window, float eps)
 {
     memset(g, 0, sizeof(*g));
-    g->W = W; g->H = H; g->s = s; g->w2 = W / s; g->h2 = H / s; g->K = 2 * (ORC_GIF_R_WIN / s) + 1;
+    g->W = W; g->H = H; g->s = s; g->w2 = W / s; g->h2 = H / s; g->K = 2 * (window / s) + 1;
     const int w2 = g->w2, h2 = g->h2, K = g->K;
     const size_t n = (size_t)W * H, n2 = (size_t)w2 * h2;
     g->xs = (int*)malloc(w2 * sizeof(int)); g->ys = (int*)malloc(h2 * sizeof(int));
@@ -769,7 +811,8 @@ typedef struct { const fgf_guide* g; float* slice; } fgf_task;
 static void* fgf_thread(void* arg) { fgf_task* k = (fgf_task*)arg; fgf_filter(k->g, k->slice); return NULL; }
 
 /* DispEst::CostFilter_FGF (DispEst.cpp:281-296; OpenMP over d there, `threads` pthreads here), volumes filtered in place */
-int orc_cost_filter_fgf(const float* lImg, const float* rImg, int W, int H, int D, int threads, int s, float* lVol, float* rVol)
+int orc_cost_filter_fgf(const float* lImg, const float* rImg, int W, int H, int D, int threads, int s, int window, float eps,
+                        float* lVol, float* rVol)
 {
     if (s < 1 || W / s < 1 || H / s < 1) return -1;
     const float* imgs[2] = {lImg, rImg};
@@ -777,7 +820,7 @@ int orc_cost_filter_fgf(const float* lImg, const float* rImg, int W, int H, int 
     if (threads < 1) threads = 1;
     for (int v = 0; v < 2; ++v) {
         fgf_guide g;
-        fgf_build(&g, imgs[v], W, H, s, ORC_GIF_EPS);
+        fgf_build(&g, imgs[v], W, H, s, window, eps);
         pthread_t* th = (pthread_t*)malloc((size_t)D * sizeof(pthread_t));
         fgf_task* tk = (fgf_task*)malloc((size_t)D * sizeof(fgf_task));
         for (int d0 = 0; d0 < D; d0 += threads) {

@@ -8,7 +8,7 @@
 // column sums at every row segment and take each row sum from one window; cvf_window_kernel likewise).  Both orders give
 // the same float while every fp64 sum is exact; where one is not, only this order reproduces the reference.
 //
-// The kernels below repeat the order of orc_box8 / window_oracle.box operation for operation: one thread per row slides
+// The kernels below repeat the order of the CPU oracle's orc_box operation for operation: one thread per row slides
 // along it, then one thread per column slides down it.  They are cooperative launches (grid-wide barriers between the
 // passes) over scratch of one slice ([4][H][W] fp64 row sums, [4][H][W] float planes):
 //   guide_ref_kernel : CVF::preprocess (CVF.cpp:44-70) + the solve terms of guide_solve_eps, for every view whose ingest

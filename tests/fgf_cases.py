@@ -4,8 +4,6 @@ guide pair with a near-black background.  Special voxels sit on the NN sample po
 only full-resolution pixels the low-resolution stages read), near the start of a 32 x 16 low-resolution tile row."""
 import numpy as np
 
-import window_oracle as WO
-
 F32 = np.float32
 COST_KINDS = ("wide12", "wide40", "outlier", "posinf", "neginf", "nan", "mixed", "ties")
 SPECIAL = {"outlier": 1e30, "posinf": np.inf, "neginf": -np.inf, "nan": np.nan}
@@ -13,7 +11,9 @@ SPECIAL = {"outlier": 1e30, "posinf": np.inf, "neginf": -np.inf, "nan": np.nan}
 
 def sample_points(W, H, s):
     """-> (xs, ys): the full-resolution column / row that low-resolution column / row i samples (cv::resize INTER_NN)"""
-    xs, ys = WO._fgf_plan(W, H, s)[:2]
+    w2, h2 = W // s, H // s
+    xs = np.minimum(np.floor(np.arange(w2) * (1.0 / (w2 / W))).astype(np.int64), W - 1)
+    ys = np.minimum(np.floor(np.arange(h2) * (1.0 / (h2 / H))).astype(np.int64), H - 1)
     return xs, ys
 
 

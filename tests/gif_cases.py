@@ -111,22 +111,26 @@ _F = 2.0 ** -24     # fp32 unit roundoff
 
 def _sum_error(x, K=8):
     """Per pixel: the largest rounding error that the fp64 box sum of the plane x (K x K, reflected, anchor K/2) can carry
-    in either order.  OpenCV (orc_box8): one running sum per row (2 roundings per step, W + K steps) whose magnitude is at
+    in either order.  OpenCV (orc_box): one running sum per row (2 roundings per step, W + K steps) whose magnitude is at
     most the largest K-wide row window of |x| it has passed (columns <= x), then one running sum per column (2 (H + K)
     roundings) of magnitude at most the largest box of |x| it has passed (centres <= y).  The tuned kernels: running column
     sums of single columns within a row segment (the 8 columns x - 4 .. x + 3, each at most such a box) and 8-wide row sums
     of those.  The error is the sum of the two."""
     from scipy.ndimage import maximum_filter1d
-    import window_oracle as WO
     a = np.abs(np.asarray(x, np.float64))
     h, w = a.shape
     k0 = K // 2
-    rows = sum(a[:, WO.reflect101(np.arange(w) + dx, w)] for dx in range(-k0, K - k0))        # row windows of |x|
-    boxes = sum(rows[WO.reflect101(np.arange(h) + dy, h), :] for dy in range(-k0, K - k0))    # box windows of |x|
+
+    def window_sums(t, axis):
+        """sums over the K reflected taps -k0 .. K-1-k0 along an axis (numpy's "reflect" is BORDER_REFLECT_101)"""
+        pad = np.pad(t, [(k0, K - 1 - k0) if ax == axis else (0, 0) for ax in range(2)], mode="reflect")
+        return sum(np.take(pad, np.arange(t.shape[axis]) + i, axis=axis) for i in range(K))
+
+    rows = window_sums(a, 1)                                                                   # row windows of |x|
+    boxes = window_sums(rows, 0)                                                               # box windows of |x|
     row_err = 2 * (w + K) * _U * np.maximum.accumulate(rows, axis=1)
     col_m = maximum_filter1d(np.maximum.accumulate(boxes, axis=0), size=K + 1, axis=1, mode="nearest")
-    return (sum(row_err[WO.reflect101(np.arange(h) + dy, h), :] for dy in range(-k0, K - k0))
-            + (K + 1) * 2 * (h + K) * _U * col_m + 2 * K * _U * boxes), boxes
+    return window_sums(row_err, 0) + (K + 1) * 2 * (h + K) * _U * col_m + 2 * K * _U * boxes, boxes
 
 
 def carried_error_bound(img, p, K=8, eps=1e-4):
@@ -138,19 +142,19 @@ def carried_error_bound(img, p, K=8, eps=1e-4):
     of a plane x differs by at most that carried error / K^2, plus one float rounding.  The difference is carried through cov, a, b (CVF.cpp:92-155) with this voxel's own mean_I, adjugate and
     1/det, through the second box (whose inputs a, b now differ as well) and q = box(b) + sum_c box(a_c) I_c; every float
     operation on the way adds at most 2^-24 of the magnitudes involved.  Non-finite voxels of the reference get inf."""
-    import window_oracle as WO
+    from oracle import oracle as O
     img = np.asarray(img, np.float32)
     p = np.asarray(p, np.float32)
     with np.errstate(all="ignore"):
-        rgb, mean, var = WO.cvf_preprocess(img, K)
-        q, a, b = WO.guided_filter(rgb, mean, var, p, K, eps, want_ab=True)
+        rgb, mean, var = O.cvf_preprocess(img, window=K)
+        q, a, b = O.guided_filter(rgb, mean, var, p, want_ab=True, window=K, eps=eps)
         f64 = lambda t: np.asarray(t, np.float64)
         I, mI, v = f64(rgb), f64(mean), f64(var)
         a, b, q = f64(a), f64(b), f64(q)
 
         def mean_err(x, dx=None):
             """|box mean of x computed two ways| where the inputs themselves may differ by dx"""
-            m = np.abs(f64(WO.box(np.asarray(x, np.float32), K)))
+            m = np.abs(f64(O.box(np.asarray(x, np.float32), K)))
             xa = np.abs(f64(x)) if dx is None else np.abs(f64(x)) + dx
             e = _sum_error(xa, K)[0] / (K * K)
             if dx is not None:

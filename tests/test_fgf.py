@@ -35,15 +35,10 @@ def test_port_matches_cv2_driven_golden(s, scenes, oracle, oracle_scene_results,
 def test_port_primitives_against_live_cv2(oracle):
     """The two OpenCV primitives the FGF branch adds (K x K blur, INTER_LINEAR up-sampling) against the cv2 in this image."""
     cv2 = pytest.importorskip("cv2")
-    import ctypes as C
     rng = np.random.default_rng(5)
     for (H, W, K) in ((67, 120, 5), (40, 33, 9), (21, 19, 3)):
         p = (rng.standard_normal((H, W)) * 3).astype(np.float32)
-        out = np.empty_like(p)
-        oracle.lib().orc_box_k.argtypes = [np.ctypeslib.ndpointer(np.float32, flags="C"), C.c_int, C.c_int, C.c_int,
-                                           np.ctypeslib.ndpointer(np.float32, flags="C")]
-        oracle.lib().orc_box_k(p, W, H, K, out)
-        assert np.array_equal(out, cv2.blur(p, (K, K)))
+        assert np.array_equal(oracle.box_direct(p, K), cv2.blur(p, (K, K)))
 
 
 @pytest.mark.gpu

@@ -4,17 +4,15 @@ tests/golden/golden_gif.json holds sha256 values of CVF::preprocess, GuidedFilte
 with real cv2.boxFilter (tests/golden/make_golden_gif.py, IPP off), on every cost kind and image kind of gif_cases:
 non-finite and 1e30 costs, a 1e15 band, wide-range, signed-zero and tied costs, a near-black float guide, its 8-bit
 version and a guide with NaN / inf pixels -- inputs where OpenCV's running fp64 sums give other floats than any other
-summation order.  The C oracle (orc_cvf_preprocess, orc_guided_filter, orc_wta) and the numpy restatement
-(window_oracle at window 8) must reproduce every value, NaN at the same places whatever the payload.  The device is
-compared with these references, so they are what ties it to OpenCV."""
+summation order.  The C oracle (orc_cvf_preprocess, orc_guided_filter, orc_wta) must reproduce every value, slice by
+slice and on whole volumes, NaN at the same places whatever the payload.  The device is compared with it, so this is what
+ties it to OpenCV."""
 import importlib.util
 import json
 import os
 
 import numpy as np
 import pytest
-
-import window_oracle as WO
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = os.path.join(HERE, "golden")
@@ -69,16 +67,16 @@ def test_c_oracle_equals_opencv(case, cases, golden_gif, gen, oracle):
 
 
 @pytest.mark.parametrize("case", CASES)
-def test_window_oracle_at_window_8_equals_opencv(case, cases, golden_gif, gen):
+def test_c_oracle_on_whole_volumes_equals_opencv(case, cases, golden_gif, gen, oracle):
+    """the volume at once, window and eps given explicitly, as the device tests call the oracle"""
     img, vol = cases[case]
     g = golden_gif["cases"][case]
-    with np.errstate(all="ignore"):
-        rgb, mean, var = WO.cvf_preprocess(img, 8)
-        q = WO.guided_filter(rgb, mean, var, vol, 8, 1e-4)
-    assert gen.sha(mean) == g["mean"], f"{case}: window_oracle.cvf_preprocess mean"
-    assert gen.sha(var) == g["var"], f"{case}: window_oracle.cvf_preprocess var"
-    assert [gen.sha(s) for s in q] == g["slices"], f"{case}: window_oracle.guided_filter"
-    assert gen.sha(WO.wta(q)) == g["wta"], f"{case}: window_oracle.wta"
+    rgb, mean, var = oracle.cvf_preprocess(img, window=8)
+    q = oracle.guided_filter(rgb, mean, var, vol, window=8, eps=1e-4)
+    assert gen.sha(mean) == g["mean"], f"{case}: orc_cvf_preprocess mean"
+    assert gen.sha(var) == g["var"], f"{case}: orc_cvf_preprocess var"
+    assert [gen.sha(s) for s in q] == g["slices"], f"{case}: orc_guided_filter"
+    assert gen.sha(oracle.wta(q)) == g["wta"], f"{case}: orc_wta"
 
 
 def test_generator_reproduces_the_golden_byte_for_byte(gen):
@@ -86,14 +84,14 @@ def test_generator_reproduces_the_golden_byte_for_byte(gen):
         assert gen.golden_text() == f.read()
 
 
-def test_orders_differ_on_these_inputs(cases):
+def test_orders_differ_on_these_inputs(cases, oracle):
     """the cases are ones where the summation order matters: direct window sums give other means than OpenCV's"""
     img, vol = cases["cost_band"]
     p = vol[1]
-    assert np.count_nonzero(WO.box(p, 8) != WO.box_direct(p, 8)) > 1000
+    assert np.count_nonzero(oracle.box(p, 8) != oracle.box_direct(p, 8)) > 1000
     img, _ = cases["image_dark_f32"]
     prod = img[..., 0] * img[..., 1]
-    assert np.count_nonzero(WO.box(prod, 8) != WO.box_direct(prod, 8)) > 100
+    assert np.count_nonzero(oracle.box(prod, 8) != oracle.box_direct(prod, 8)) > 100
 
 
 # ---- the carried-error bound the device test asserts on inexact sums is not vacuous ------------------------------------

@@ -1,6 +1,6 @@
 """GPU: the matching cost at run-time alpha and truncation thresholds (psm_set_matching_cost), bit-exact against the
-any-setting CPU restatement tests/cost_oracle.py (which reproduces the existing goldens at the defaults and the
-cv2-driven golden_cost.json at the other settings).  Every comparison goes through the C-ABI."""
+C oracle at that setting (which reproduces the existing goldens at the defaults and the cv2-driven golden_cost.json at
+the other settings).  Every comparison goes through the C-ABI."""
 import ctypes as C
 import json
 import os
@@ -10,10 +10,9 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, ROOT, read_png
+from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi
-import cost_oracle as CO
 import mixed_model as MM
-import window_oracle as WO
 
 pytestmark = pytest.mark.gpu
 
@@ -51,8 +50,13 @@ def run(l, r, D, cost, d_begin=0, d_count=None, window=None, filt=True):
     return out
 
 
+def raw_volumes(l, r, D, cost, **shard):
+    alpha, tau_color, tau_grad = cost
+    return O.cost_const(l, r, D, alpha=alpha, tau_color=tau_color, tau_grad=tau_grad, **shard)[2:]
+
+
 def check_raw(l, r, D, cost, got, what, d_begin=0, d_count=None):
-    lraw, rraw = CO.cost_volumes(l, r, D, *(cost or CO.DEFAULT), d_begin=d_begin, d_count=d_count)
+    lraw, rraw = raw_volumes(l, r, D, cost or (0.9, INF, INF), d_begin=d_begin, d_count=d_count)
     assert_same(got["lraw"], lraw, f"{what} left raw volume")
     assert_same(got["rraw"], rraw, f"{what} right raw volume")
     return lraw, rraw
@@ -83,11 +87,11 @@ def test_raw_volumes_on_crops(scene, cost, crops):
     l, r = crops[scene]
     got = run(l, r, 24, cost)
     lraw, rraw = check_raw(l, r, 24, cost, got, f"{scene} crop {cost}")
-    lf, rf = WO.cost_filter(l, r, lraw, rraw)
+    lf, rf = O.cost_filter(l, r, lraw, rraw)
     assert_same(got["lf"], lf, f"{scene} crop {cost} left filtered")
     assert_same(got["rf"], rf, f"{scene} crop {cost} right filtered")
-    assert_same(got["ld"], WO.wta(lf), f"{scene} crop {cost} left map")
-    assert_same(got["rd"], WO.wta(rf), f"{scene} crop {cost} right map")
+    assert_same(got["ld"], O.wta(lf), f"{scene} crop {cost} left map")
+    assert_same(got["rd"], O.wta(rf), f"{scene} crop {cost} right map")
 
 
 @pytest.mark.parametrize("W,H,D", [(1, 1, 3), (2, 3, 4), (5, 40, 5), (17, 23, 7), (31, 9, 40), (32, 6, 33), (33, 5, 40),
@@ -99,7 +103,7 @@ def test_ragged_sizes(W, H, D):
     cost = (0.3, 0.12, 0.01)
     got = run(l, r, D, cost)
     lraw, rraw = check_raw(l, r, D, cost, got, f"{W}x{H}x{D}")
-    lf, rf = WO.cost_filter(l, r, lraw, rraw)   # W < 32: the mirrored halo comes from the separate pass
+    lf, rf = O.cost_filter(l, r, lraw, rraw)   # W < 32: the mirrored halo comes from the separate pass
     assert_same(got["lf"], lf, f"{W}x{H}x{D} left filtered")
     assert_same(got["rf"], rf, f"{W}x{H}x{D} right filtered")
 
@@ -125,9 +129,9 @@ def test_full_scene_maps_and_bad_pixels_at_best_setting(scene, scenes):
     _, _, l, r = scenes[scene]
     got = run(l, r, 64, BEST)
     lraw, rraw = check_raw(l, r, 64, BEST, got, f"{scene} {BEST}")
-    lf, rf = WO.cost_filter(l, r, lraw, rraw)
-    assert_same(got["ld"], WO.wta(lf), f"{scene} left map")
-    assert_same(got["rd"], WO.wta(rf), f"{scene} right map")
+    lf, rf = O.cost_filter(l, r, lraw, rraw)
+    assert_same(got["ld"], O.wta(lf), f"{scene} left map")
+    assert_same(got["rd"], O.wta(rf), f"{scene} right map")
     s = scene.lower()
     gt, occl = read_png(os.path.join(GOLDEN, f"{s}_disp2.png"), True), read_png(os.path.join(GOLDEN, f"{s}_occl.png"), True)
     assert abs(bad_pixels_nonocc(got["ld"], gt, occl) - g["bp_nonocc_left"]) < 1e-3
@@ -156,15 +160,15 @@ def test_with_window_16(crops):
     l, r = crops["Teddy"]
     got = run(l, r, 24, BEST, window=(16, 1e-4))
     lraw, rraw = check_raw(l, r, 24, BEST, got, "window 16")
-    lf, rf = WO.cost_filter(l, r, lraw, rraw, 16, 1e-4)
+    lf, rf = O.cost_filter(l, r, lraw, rraw, window=16, eps=1e-4)
     assert_same(got["lf"], lf, "window 16 left filtered")
     assert_same(got["rf"], rf, "window 16 right filtered")
 
 
 def test_with_fgf(scenes):
     _, _, l, r = scenes["Teddy"]
-    lraw, rraw = CO.cost_volumes(l, r, 64, *BEST)
-    lf, rf = WO.cost_filter_fgf(l, r, lraw, rraw, 8, 1e-4, 4)
+    lraw, rraw = raw_volumes(l, r, 64, BEST)
+    lf, rf = O.cost_filter_fgf(l, r, lraw, rraw, 4, window=8, eps=1e-4)
     with DispEst(l, r, 64) as de:
         de.setMatchingCost(*BEST)
         de.setSubsampleRate(4)
@@ -177,7 +181,7 @@ def test_with_fgf(scenes):
 @pytest.mark.parametrize("mode", [capi.PSM_CVF_MIXED, capi.PSM_CVF_NAIVE])
 def test_with_mixed_and_naive_modes(mode, crops, oracle):
     l, r = crops["Cones"]
-    lraw, rraw = CO.cost_volumes(l, r, 24, *BEST)
+    lraw, rraw = raw_volumes(l, r, 24, BEST)
     with DispEst(l, r, 24) as de:
         de.setMatchingCost(*BEST)
         de.set_option(capi.PSM_OPT_CVF_MODE, mode)
@@ -188,7 +192,7 @@ def test_with_mixed_and_naive_modes(mode, crops, oracle):
         assert_same(lf, MM.cost_filter_mixed(oracle, l, lraw), "MIXED left vs its CPU model")
         assert_same(rf, MM.cost_filter_mixed(oracle, r, rraw), "MIXED right vs its CPU model")
     else:
-        wl, wr = WO.cost_filter(l, r, lraw, rraw)
+        wl, wr = O.cost_filter(l, r, lraw, rraw)
         assert_same(lf, wl, "NAIVE left")
         assert_same(rf, wr, "NAIVE right")
 
@@ -198,8 +202,8 @@ def test_sharded_keys_match_unsharded(crops):
     l, r = crops["Cones"]
     H, W, _ = l.shape
     D = 24
-    lraw, rraw = CO.cost_volumes(l, r, D, *BEST)
-    lf, rf = WO.cost_filter(l, r, lraw, rraw)
+    lraw, rraw = raw_volumes(l, r, D, BEST)
+    lf, rf = O.cost_filter(l, r, lraw, rraw)
     L = capi.lib()
     keys = torch.empty((2, 2, H * W), dtype=torch.int64, device="cuda")
     shards = [DispEst(l, r, D, d_begin=0, d_count=11), DispEst(l, r, D, d_begin=11, d_count=13)]
@@ -214,8 +218,8 @@ def test_sharded_keys_match_unsharded(crops):
         de = shards[0]
         capi.check(L.psm_disp_reduce_keys(de.handle, keys[0].data_ptr(), keys[1].data_ptr(), 2,
                                           ld.ctypes.data_as(C.c_void_p), W, rd.ctypes.data_as(C.c_void_p), W), de.handle)
-        assert_same(ld, WO.wta(lf), "sharded left map")
-        assert_same(rd, WO.wta(rf), "sharded right map")
+        assert_same(ld, O.wta(lf), "sharded left map")
+        assert_same(rd, O.wta(rf), "sharded right map")
     finally:
         for de in shards:
             de.close()
@@ -242,11 +246,11 @@ def test_switching_settings_between_frames(scenes, oracle_scene_results):
                 assert_same(de.lDisMap, ref["ld"], "back to defaults: left map")
                 assert_same(de.rDisMap, ref["rd"], "back to defaults: right map")
             else:
-                lraw, rraw = CO.cost_volumes(l, r, 64, *cost)
+                lraw, rraw = raw_volumes(l, r, 64, cost)
                 assert_same(raw, lraw, f"{cost} left raw volume")
-                lf, rf = WO.cost_filter(l, r, lraw, rraw)
-                assert_same(de.lDisMap, WO.wta(lf), f"{cost} left map")
-                assert_same(de.rDisMap, WO.wta(rf), f"{cost} right map")
+                lf, rf = O.cost_filter(l, r, lraw, rraw)
+                assert_same(de.lDisMap, O.wta(lf), f"{cost} left map")
+                assert_same(de.rDisMap, O.wta(rf), f"{cost} right map")
 
 
 def test_default_launch_count_unchanged(crops):
@@ -273,7 +277,7 @@ def test_errors_leave_context_unchanged(crops):
                 de.setMatchingCost(*cost)
         assert L.psm_set_matching_cost(None, 0.5, 0.1, 0.1) == capi.PSM_EINVAL
         de.CostConst_GPU()
-        lraw, rraw = CO.cost_volumes(l, r, 24, *BEST)
+        lraw, rraw = raw_volumes(l, r, 24, BEST)
         assert_same(de.read_cost_volume(0), lraw, "after rejected calls: the best setting still in force (left)")
         assert_same(de.read_cost_volume(1), rraw, "after rejected calls: right")
 
@@ -289,7 +293,7 @@ def test_cpp_facade_set_matching_cost(tmp_path, scenes, oracle):
                           str(tmp_path / "l.u8"), str(tmp_path / "r.u8"), "8", "0.0001", "0.11", "0.21", "0.008"],
                          capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stderr
-    lraw, rraw = CO.cost_volumes(l, r, 64, *BEST)
-    lf, _ = WO.cost_filter(l, r, lraw, rraw)
+    lraw, rraw = raw_volumes(l, r, 64, BEST)
+    lf, _ = O.cost_filter(l, r, lraw, rraw)
     ld = np.fromfile(tmp_path / "l.u8", np.uint8).reshape(H, W)
-    assert_same(ld, oracle.post_process(l, WO.wta(lf)), "C++ facade lDisMap at the best setting (after PostProcess_GPU)")
+    assert_same(ld, oracle.post_process(l, O.wta(lf)), "C++ facade lDisMap at the best setting (after PostProcess_GPU)")

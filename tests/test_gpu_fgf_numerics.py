@@ -1,5 +1,5 @@
-"""GPU: the Fast Guided Filter (psm_cost_filter_fgf) bit for bit against the C port orc_cost_filter_fgf (window 8,
-eps 1e-4) and the any-window restatement window_oracle.fgf_filter_volume, where the fp64 box sums are not exact: costs
+"""GPU: the Fast Guided Filter (psm_cost_filter_fgf) bit for bit against the C oracle's orc_cost_filter_fgf at the
+context's window and eps, where the fp64 box sums are not exact: costs
 over wide ranges, a 1e30 outlier, +inf / -inf / NaN voxels, mixed signs and -0.0, exact ties between slices, a guide with
 a near-black background (float and 8-bit), low-resolution sizes at and around the 32 x 16 tile edges and below half the
 box, the largest box the kernel accepts, a sharded context and a 16-bit-map context at D > 256.  Filtered volumes are
@@ -11,7 +11,6 @@ from primestereomatch_b200 import DispEst, capi
 from oracle import oracle as O
 import fgf_cases as FC
 from fgf_cases import assert_same
-import window_oracle as WO
 
 pytestmark = pytest.mark.gpu
 
@@ -19,23 +18,9 @@ F32 = np.float32
 RATES = [1, 2, 4, 8]
 
 
-def wta(vol, dtype=np.uint8):
-    """DispSel.cpp:83-109: argmin over d >= 1, strict <, ties to the lowest d, 0 when nothing is below +inf"""
-    best = np.full(vol.shape[1:], np.inf, F32)
-    dis = np.zeros(vol.shape[1:], dtype)
-    for d in range(1, vol.shape[0]):
-        m = vol[d] < best
-        best = np.where(m, vol[d], best)
-        dis[m] = d
-    return dis
-
-
 def reference(l, r, lraw, rraw, s, window=8, eps=1e-4):
     """filtered copies of both raw volumes; float guide images"""
-    if (window, eps) == (8, 1e-4):
-        return O.cost_filter_fgf(l, r, lraw, rraw, s=s)
-    with np.errstate(all="ignore"):
-        return WO.cost_filter_fgf(l, r, lraw, rraw, window, eps, s)
+    return O.cost_filter_fgf(l, r, lraw, rraw, s, window=window, eps=eps)
 
 
 def run(l, r, D, s, writes=(), window=None, eps=1e-4, d_begin=0, map_bits=None):
@@ -65,8 +50,8 @@ def check(got, lf, rf, what, d_begin=0, map_dtype=np.uint8):
     assert_same(got["lf"], lf[d_begin:], f"{what} left volume")
     assert_same(got["rf"], rf[d_begin:], f"{what} right volume")
     if "ld" in got:
-        assert_same(got["ld"], wta(lf, map_dtype), f"{what} left map")
-        assert_same(got["rd"], wta(rf, map_dtype), f"{what} right map")
+        assert_same(got["ld"], O.wta(lf, map_dtype), f"{what} left map")
+        assert_same(got["rd"], O.wta(rf, map_dtype), f"{what} right map")
 
 
 # ---- costs outside the bounded case ------------------------------------------------------------------------------------

@@ -20,7 +20,6 @@ from oracle import oracle as O
 import gif_cases as GC
 from gif_cases import assert_same, differ
 import mixed_model as MM
-import window_oracle as WO
 
 pytestmark = pytest.mark.gpu
 
@@ -28,28 +27,13 @@ F32 = np.float32
 D = 5
 
 
-def wta(vol, dtype=np.uint8):
-    best = np.full(vol.shape[1:], np.inf, F32)
-    dis = np.zeros(vol.shape[1:], dtype)
-    for d in range(1, vol.shape[0]):
-        m = vol[d] < best
-        best = np.where(m, vol[d], best)
-        dis[m] = d
-    return dis
-
-
 def reference(img, vol, window=8, eps=1e-4, want_ab=False):
     """filtered copy of one view's raw volume (and a, b of every slice)"""
-    with np.errstate(all="ignore"):
-        if (window, eps) == (8, 1e-4):
-            rgb, mean, var = O.cvf_preprocess(img)
-            res = [O.guided_filter(rgb, mean, var, vol[d], want_ab=want_ab) for d in range(vol.shape[0])]
-        else:
-            rgb, mean, var = WO.cvf_preprocess(img, window)
-            res = [WO.guided_filter(rgb, mean, var, vol[d], window, eps, want_ab=want_ab) for d in range(vol.shape[0])]
+    rgb, mean, var = O.cvf_preprocess(img, window=window)
+    res = O.guided_filter(rgb, mean, var, vol, want_ab=want_ab, window=window, eps=eps)
     if want_ab:
-        return np.stack([r[0] for r in res]), [(r[1], r[2]) for r in res]
-    return np.stack(res)
+        return res[0], list(zip(res[1], res[2]))
+    return res
 
 
 def run(imgs, Dn, writes=(), mode=None, variant=None, options=(), window=None, eps=1e-4, d_begin=0, map_bits=None,
@@ -86,8 +70,8 @@ def check(got, lf, rf, what, d_begin=0, map_dtype=np.uint8):
     assert_same(got["lf"], lf[d_begin:], f"{what} left volume")
     assert_same(got["rf"], rf[d_begin:], f"{what} right volume")
     if "ld" in got:
-        assert_same(got["ld"], wta(lf, map_dtype), f"{what} left map")
-        assert_same(got["rd"], wta(rf, map_dtype), f"{what} right map")
+        assert_same(got["ld"], O.wta(lf, map_dtype), f"{what} left map")
+        assert_same(got["rd"], O.wta(rf, map_dtype), f"{what} right map")
 
 
 @pytest.fixture(scope="module")
@@ -229,7 +213,7 @@ def check_bounded(got, imgs, raws, lf, rf, what):
         assert not far.any(), (f"{what} view {v}: {int(far.sum())} voxels beyond the carried-error bound, first at "
                                f"{np.argwhere(far)[0].tolist()}")
     for v, (m, vol) in enumerate(((got["ld"], lf), (got["rd"], rf))):
-        print(f"{what} view {v}: {int(np.count_nonzero(m != wta(vol)))} of {m.size} map pixels differ")
+        print(f"{what} view {v}: {int(np.count_nonzero(m != O.wta(vol)))} of {m.size} map pixels differ")
 
 
 @pytest.mark.parametrize("plan", PLANS[:4], ids=[p[0] for p in PLANS[:4]])

@@ -18,10 +18,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import cost_oracle as CO
 import gif_cases as GC
 import image_cases as IC
-import window_oracle as WO
 from gif_cases import assert_same, differ
 from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi
@@ -86,7 +84,7 @@ def test_cost_kernel_at_other_settings(kind, size, setting):
     l, r = frame(kind, size)
     W, H, D = dims(size)
     with np.errstate(all="ignore"):
-        lv, rv = CO.cost_volumes(l, r, D, *setting)
+        lv, rv = O.cost_const(l, r, D, alpha=setting[0], tau_color=setting[1], tau_grad=setting[2])[2:]
     with DispEst(l, r, D) as de:
         de.setMatchingCost(*setting)
         assert de.CostConst_GPU() == 0
@@ -190,8 +188,8 @@ def test_flagged_generic_window(kind, window):
         _, _, lraw, rraw = O.cost_const(l, r, D)
         want = []
         for img, raw in ((l, lraw), (r, rraw)):
-            rgb, mean, var = WO.cvf_preprocess(img, window)
-            want.append(WO.guided_filter(rgb, mean, var, raw, window, eps))
+            rgb, mean, var = O.cvf_preprocess(img, window=window)
+            want.append(O.guided_filter(rgb, mean, var, raw, window=window, eps=eps))
     with DispEst(l, r, D) as de:
         de.setGuidedFilter(window, eps)
         assert de.CostConst_GPU() == 0 and de.CostFilter_GPU() == 0

@@ -1,5 +1,5 @@
-"""GPU: the guided filter at run-time window / epsilon (psm_set_guided_filter), bit-exact against the any-window CPU
-restatement tests/window_oracle.py (which reproduces the existing goldens at (8, 1e-4f) and cv2 at the other windows)."""
+"""GPU: the guided filter at run-time window / epsilon (psm_set_guided_filter), bit-exact against the C oracle at that
+window and epsilon (which reproduces the existing goldens at (8, 1e-4f) and cv2 at the other windows)."""
 import ctypes as C
 import os
 import subprocess
@@ -8,8 +8,8 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
+from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
-import window_oracle as WO
 
 pytestmark = pytest.mark.gpu
 
@@ -46,16 +46,16 @@ def run(l, r, D, window, eps, raw=None, guide=False, d_begin=0, d_count=None):
 
 
 def check_against_oracle(l, r, lraw, rraw, window, eps, got, what):
-    lf, rf = WO.cost_filter(l, r, lraw, rraw, window, eps)
+    lf, rf = O.cost_filter(l, r, lraw, rraw, window=window, eps=eps)
     if "mean" in got:
-        _, mean, var = WO.cvf_preprocess(l, window)
+        _, mean, var = O.cvf_preprocess(l, window=window)
         assert_same(got["mean"], mean, f"{what} mean_I")
         assert_same(got["var"], var, f"{what} var_I")
     assert_same(got["lf"], lf, f"{what} left filtered volume")
     assert_same(got["rf"], rf, f"{what} right filtered volume")
     if "ld" in got:
-        assert_same(got["ld"], WO.wta(lf), f"{what} left map")
-        assert_same(got["rd"], WO.wta(rf), f"{what} right map")
+        assert_same(got["ld"], O.wta(lf), f"{what} left map")
+        assert_same(got["rd"], O.wta(rf), f"{what} right map")
 
 
 @pytest.fixture(scope="module")
@@ -101,13 +101,13 @@ def test_ragged_sizes(W, H, D, window, oracle):
 @pytest.mark.parametrize("window,eps", [(5, 1e-4), (16, 1e-2), (32, 1e-3)])
 def test_read_ab_slice(window, eps, crops):
     l, r, lraw, _ = crops["Teddy"]
-    rgb, mean, var = WO.cvf_preprocess(l, window)
+    rgb, mean, var = O.cvf_preprocess(l, window=window)
     with DispEst(l, r, 24) as de:
         de.setGuidedFilter(window, eps)
         de.CostConst_GPU()
         for d in (1, 13):
             a, b = de.read_ab_slice(0, d)
-            _, wa, wb = WO.guided_filter(rgb, mean, var, lraw[d], window, eps, want_ab=True)
+            _, wa, wb = O.guided_filter(rgb, mean, var, lraw[d], want_ab=True, window=window, eps=eps)
             assert_same(a, wa, f"a d={d}")
             assert_same(b, wb, f"b d={d}")
 
@@ -130,7 +130,7 @@ def test_sharded_keys_match_unsharded(crops):
     l, r, lraw, rraw = crops["Cones"]
     H, W, _ = l.shape
     D, window, eps = 24, 12, 1e-3
-    lf, rf = WO.cost_filter(l, r, lraw, rraw, window, eps)
+    lf, rf = O.cost_filter(l, r, lraw, rraw, window=window, eps=eps)
     L = capi.lib()
     keys = torch.empty((2, 2, H * W), dtype=torch.int64, device="cuda")
     shards = [DispEst(l, r, D, d_begin=0, d_count=10), DispEst(l, r, D, d_begin=10, d_count=14)]
@@ -145,8 +145,8 @@ def test_sharded_keys_match_unsharded(crops):
         de = shards[0]
         capi.check(L.psm_disp_reduce_keys(de.handle, keys[0].data_ptr(), keys[1].data_ptr(), 2,
                                           ld.ctypes.data_as(C.c_void_p), W, rd.ctypes.data_as(C.c_void_p), W), de.handle)
-        assert_same(ld, WO.wta(lf), "sharded left map")
-        assert_same(rd, WO.wta(rf), "sharded right map")
+        assert_same(ld, O.wta(lf), "sharded left map")
+        assert_same(rd, O.wta(rf), "sharded right map")
     finally:
         for de in shards:
             de.close()
@@ -156,7 +156,7 @@ def test_sharded_keys_match_unsharded(crops):
 def test_fgf_window16(s, scenes, oracle_scene_results):
     _, _, l, r = scenes["Teddy"]
     ref = oracle_scene_results["Teddy"]
-    lf, rf = WO.cost_filter_fgf(l, r, ref["lraw"], ref["rraw"], 16, 1e-4, s)
+    lf, rf = O.cost_filter_fgf(l, r, ref["lraw"], ref["rraw"], s, window=16, eps=1e-4)
     with DispEst(l, r, 64) as de:
         de.setGuidedFilter(16, 1e-4)
         de.setSubsampleRate(s)
@@ -199,9 +199,9 @@ def test_switching_parameters_between_frames(scenes, oracle_scene_results):
                 assert_same(de.lDisMap, ref["ld"], "back to defaults: left map")
                 assert_same(de.rDisMap, ref["rd"], "back to defaults: right map")
             else:
-                lf, _ = WO.cost_filter(l, r, ref["lraw"], ref["rraw"], window, eps)
+                lf, _ = O.cost_filter(l, r, ref["lraw"], ref["rraw"], window=window, eps=eps)
                 assert_same(de.read_cost_volume(0), lf, f"window {window} left volume")
-                assert_same(de.lDisMap, WO.wta(lf), f"window {window} left map")
+                assert_same(de.lDisMap, O.wta(lf), f"window {window} left map")
 
 
 def test_full_hd_window16_row_band(oracle):
@@ -217,9 +217,9 @@ def test_full_hd_window16_row_band(oracle):
         de.CostFilter_GPU()
         got = {v: {d: de.read_cost_slice(v, d) for d in ds} for v in (0, 1)}
     for v, img in ((0, l), (1, r)):
-        rgb, mean, var = WO.cvf_preprocess(img, window)
+        rgb, mean, var = O.cvf_preprocess(img, window=window)
         for d in ds:
-            q = WO.guided_filter(rgb, mean, var, raw[v][d], window, eps)
+            q = O.guided_filter(rgb, mean, var, raw[v][d], window=window, eps=eps)
             for ys in (slice(0, 40), slice(500, 540), slice(1050, 1080)):
                 assert_same(got[v][d][ys], q[ys], f"view {v} d {d} rows {ys}")
 
@@ -235,7 +235,7 @@ def test_errors_leave_context_unchanged(crops):
                 de.setGuidedFilter(window, eps)
         de.CostConst_GPU()
         de.CostFilter_GPU()
-        lf, _ = WO.cost_filter(l, r, lraw, rraw, 9, 1e-3)
+        lf, _ = O.cost_filter(l, r, lraw, rraw, window=9, eps=1e-3)
         assert_same(de.read_cost_volume(0), lf, "after rejected calls: (9, 1e-3) still in force")
         for mode in (capi.PSM_CVF_MIXED, capi.PSM_CVF_NAIVE):
             de.set_option(capi.PSM_OPT_CVF_MODE, mode)
@@ -257,6 +257,6 @@ def test_cpp_facade_set_guided_filter(tmp_path, scenes, oracle_scene_results, or
     out = subprocess.run([exe, str(W), str(H), "64", str(tmp_path / "l.f32"), str(tmp_path / "r.f32"),
                           str(tmp_path / "l.u8"), str(tmp_path / "r.u8"), "12", "0.001"], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stderr
-    lf, _ = WO.cost_filter(l, r, ref["lraw"], ref["rraw"], 12, 1e-3)
+    lf, _ = O.cost_filter(l, r, ref["lraw"], ref["rraw"], window=12, eps=1e-3)
     ld = np.fromfile(tmp_path / "l.u8", np.uint8).reshape(H, W)
-    assert_same(ld, oracle.post_process(l, WO.wta(lf)), "C++ facade lDisMap at window 12 (after PostProcess_GPU)")
+    assert_same(ld, oracle.post_process(l, O.wta(lf)), "C++ facade lDisMap at window 12 (after PostProcess_GPU)")
