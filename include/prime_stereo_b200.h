@@ -46,6 +46,14 @@
  * Threading: one psm_ctx must not be used concurrently; it may be used from different
  * host threads over its life (every call binds its CUDA device first), matching how the
  * reference constructs DispEst on the HCI thread and runs stages on the worker thread.
+ *
+ * Host synchronisation: the calls documented as asynchronous only enqueue work once their first use is behind them.
+ * On first use, or on the first call after a setting change, these may wait for the device (allocations, cudaFree,
+ * blocking uploads): psm_set_images_async / _u8_async (the second staging set), psm_cost_filter and psm_read_ab_slice
+ * (the scratch of the reference-order pass: float frames, a non-default guided filter, PSM_CVF_NAIVE, flagged slices),
+ * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
+ * (its buffers and, after a change of sigma or weight type, the weight table).  Run them once before a latency-critical
+ * loop.  psm_set_stream always waits for the stream it leaves.
  */
 #ifndef PRIME_STEREO_B200_H
 #define PRIME_STEREO_B200_H
@@ -129,6 +137,8 @@ int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp,
 int psm_create_u16(psm_ctx** out, int width, int height, int max_disp,
                    int d_begin, int d_count, int device);
 
+/* Waits for the context's work on the stream it is bound to (psm_set_stream), on its own stream and on its copy stream,
+ * then frees everything: a caller's stream bound with psm_set_stream must still exist when this is called. */
 int psm_destroy(psm_ctx* ctx);
 
 int psm_set_option(psm_ctx* ctx, int key, int value);
@@ -201,30 +211,39 @@ int psm_set_lr_check(psm_ctx* ctx, int mode);
 int psm_read_valid_mask(psm_ctx* ctx, int view, uint8_t* dst, size_t dst_step);
 
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
- * context's own stream.  Lets a caller time with its own events on that stream. */
+ * context's own stream.  Lets a caller time with its own events on that stream.  Waits for the work already enqueued
+ * on the stream the context was using.  The stream must outlive the context, or be replaced before psm_destroy. */
 int psm_set_stream(psm_ctx* ctx, void* cuda_stream);
 
 /* Inputs: interleaved 3-channel float images (cv::Mat CV_32FC3, BGR, values in [0,1]) in HOST
  * memory, row steps in BYTES.  Copies H2D and builds planar channels + x-gradients
- * (CVC::preprocess, src/CVC.cpp:41-46) on the device. */
+ * (CVC::preprocess, src/CVC.cpp:41-46) on the device.
+ * The buffers may be reused as soon as the call returns, page-locked or not: the copy runs on the context's copy
+ * stream into a device staging set, once the last ingest from that set has read it (and after a pending
+ * psm_set_images_async upload), and the call waits for it; the ingest kernels follow on the context's stream.  It does
+ * not wait for the rest of the context's stream. */
 int psm_set_images(psm_ctx* ctx, const float* left, size_t left_step,
                    const float* right, size_t right_step);
 
 /* Same, 8-bit interleaved BGR input; the convertTo(CV_32F, 1/255.0f) of
- * src/StereoMatch.cpp:193-197 is done on the device (4x less H2D traffic). */
+ * src/StereoMatch.cpp:193-197 is done on the device (4x less H2D traffic).  Buffers reusable on return. */
 int psm_set_images_u8(psm_ctx* ctx, const uint8_t* left, size_t left_step,
                       const uint8_t* right, size_t right_step);
 
-/* Same as psm_set_images but the interleaved float images already live in DEVICE memory. */
+/* Same as psm_set_images but the interleaved float images already live in DEVICE memory.  Asynchronous: the images are
+ * read by the ingest kernels on the context's stream, so the caller orders the work that produces them, and any later
+ * overwrite of them, against that stream (psm_set_stream, or events). */
 int psm_set_images_device(psm_ctx* ctx, const float* d_left, size_t left_step,
                           const float* d_right, size_t right_step);
 
 /* Pipelined upload (extension; the reference's DispEst is synchronous per frame): start the H2D copy
  * of the NEXT frame on the context's copy stream into a second staging set while the current frame
  * is still being computed, then make it the current frame.  Host buffers must be page-locked for the
- * copy to overlap and must stay valid until psm_set_images_commit has returned.
+ * copy to overlap and must stay valid until psm_set_images_commit has returned; they may be reused after that.
  *   psm_set_images_async(k+1) ... stages of frame k ... psm_set_images_commit()  ->  frame k+1 is current
- * commit = compute stream waits for the upload, then the same ingest kernels as psm_set_images. */
+ * The copy waits until frame k-1's ingest has read the staging set it overwrites.  commit = the compute stream waits for
+ * the upload, then the same ingest kernels as psm_set_images, then the host waits for the copy (in the two-deep pipeline
+ * the frames already enqueued keep the device busy meanwhile). */
 int psm_set_images_async(psm_ctx* ctx, const float* left, size_t left_step,
                          const float* right, size_t right_step);
 int psm_set_images_u8_async(psm_ctx* ctx, const uint8_t* left, size_t left_step,

@@ -43,8 +43,9 @@ struct psm_ctx {
     float* vol_alt[2] = {nullptr, nullptr}; // the other half of the ping-pong
     void* stage_in[2] = {nullptr, nullptr}; // device staging for the interleaved upload (the set the synchronous calls use)
     void* stage_alt[2] = {nullptr, nullptr};// second staging set: psm_set_images_async uploads frame k+1 while frame k is in flight
-    cudaStream_t copy_stream = nullptr;     // H2D stream of the asynchronous upload
+    cudaStream_t copy_stream = nullptr;     // H2D stream of every host upload
     cudaEvent_t up_done = nullptr;          // async upload finished (recorded on copy_stream)
+    cudaEvent_t host_copied = nullptr;      // H2D of a synchronous host upload finished (recorded on copy_stream)
     cudaEvent_t ingest_done[2] = {nullptr, nullptr};  // ingest kernels consumed staging set k (recorded on the compute stream)
     bool ingest_done_valid[2] = {false, false};
     int stage_cur = 0;                      // staging set holding the current frame: 0 = stage_in, 1 = stage_alt
@@ -170,23 +171,37 @@ int ingest(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool 
     const T* src[2] = {l, r};
     const size_t step[2] = {lstep, rstep};
     const size_t row_bytes = (size_t)c->W * 3 * sizeof(T);
+    for (int v = 0; v < 2; ++v)
+        if (!src[v] || step[v] < row_bytes) return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
+    const int set = c->stage_cur;
+    if (!from_device) {
+        // Host frames go through the current staging set on the copy stream, once the last ingest from that set has
+        // read it, so that the copy does not queue behind the compute stream's backlog; the compute stream waits for
+        // it, and the call returns once it has read the caller's buffers (from page-locked memory the copy would
+        // otherwise still be reading them after the return).
+        if (c->ingest_done_valid[set]) PSM_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ingest_done[set], 0));
+        for (int v = 0; v < 2; ++v)
+            PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v], step[v], row_bytes, c->H,
+                                          cudaMemcpyHostToDevice, c->copy_stream));
+        PSM_CUDA(c, cudaEventRecord(c->host_copied, c->copy_stream));
+        PSM_CUDA(c, cudaStreamWaitEvent(c->stream, c->host_copied, 0));
+    }
     PSM_CUDA(c, cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
     for (int v = 0; v < 2; ++v) {
-        if (!src[v] || step[v] < row_bytes) return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
-        const T* dsrc = src[v];
-        size_t dstep = step[v];
-        if (!from_device) {
-            PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, c->stage_cur, v), row_bytes, src[v], step[v], row_bytes, c->H,
-                                          cudaMemcpyHostToDevice, c->stream));
-            dsrc = static_cast<const T*>(stage_buf(c, c->stage_cur, v));
-            dstep = row_bytes;
-        }
+        const T* dsrc = from_device ? src[v] : static_cast<const T*>(stage_buf(c, set, v));
+        const size_t dstep = from_device ? step[v] : row_bytes;
         float* g = c->guide[v];
         dim3 blk(128), grd((c->W + 3 + 127) / 128, c->H);
         ingest_kernel<T><<<grd, blk, 0, c->stream>>>(dsrc, dstep, c->W, c->H, c->Wp, g, g + c->plane,
                                                       g + 2 * c->plane, c->grd[v], c->gray_mode, c->guide_flags + v);
         PSM_LAUNCH_CHECK(c);
         if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
+    }
+    if (!from_device) {
+        // the next upload into this set waits for these kernels (psm_set_images_commit records its own ingests)
+        PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
+        c->ingest_done_valid[set] = true;
+        PSM_CUDA(c, cudaEventSynchronize(c->host_copied));
     }
     c->have_images = true;
     c->float_images = sizeof(T) != 1;   // u8 images lie in {0} U [1/255, 1]: they never raise an ingest flag
@@ -593,6 +608,7 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
     PSM_CREATE_CUDA(cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
     PSM_CREATE_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->up_done, cudaEventDisableTiming));
+    PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->host_copied, cudaEventDisableTiming));
     for (int k = 0; k < 2; ++k) PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->ingest_done[k], cudaEventDisableTiming));
     for (int s = 0; s < kNumStages; ++s) {
         PSM_CREATE_CUDA(cudaEventCreate(&c->ev0[s]));
@@ -639,14 +655,18 @@ int psm_destroy(psm_ctx* c)
 {
     if (!c) return PSM_OK;
     cudaSetDevice(c->device);
+    // every stream that may still run work on the buffers below: the caller's (psm_set_stream), the context's own one
+    // (work enqueued before a psm_set_stream) and the copy stream
+    if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->own_stream) cudaStreamSynchronize(c->own_stream);
+    if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
     for (int i = 0; i < c->p2p_nimported; ++i) cudaIpcCloseMemHandle(c->p2p_imported[i]);
     cudaFree(c->p2p_own);
     cudaFree(c->p2p_counter);
     for (int i = 0; i < c->nalloc; ++i) cudaFree(c->alloc[i]);
-    if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
     for (int v = 0; v < 2; ++v) { cudaFree(c->stage_in[v]); cudaFree(c->stage_alt[v]); cudaFree(c->dis[v]); }
     if (c->up_done) cudaEventDestroy(c->up_done);
+    if (c->host_copied) cudaEventDestroy(c->host_copied);
     for (int k = 0; k < 2; ++k) if (c->ingest_done[k]) cudaEventDestroy(c->ingest_done[k]);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaFree(c->slice_flags);
@@ -829,7 +849,11 @@ int psm_set_images_commit(psm_ctx* c)
     if (rc) return rc;
     PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
     c->ingest_done_valid[set] = true;
-    return stage_end(c, 0);
+    if ((rc = stage_end(c, 0))) return rc;
+    // the caller may reuse its host buffers once this returns: wait for the copy that reads them (it may still be
+    // waiting for the frame before last to leave this staging set); the ingest kernels are already queued behind it
+    PSM_CUDA(c, cudaEventSynchronize(c->up_done));
+    return PSM_OK;
 }
 
 int psm_cost_const(psm_ctx* c)
