@@ -137,6 +137,33 @@ int psm_create_sharded(psm_ctx** out, int width, int height, int max_disp,
 int psm_create_u16(psm_ctx** out, int width, int height, int max_disp,
                    int d_begin, int d_count, int device);
 
+/* Blocked context: owns the global slices [d_begin, d_begin + d_count) of a max_disp-deep problem like psm_create_u16,
+ * but holds only `block_slices` of them at a time (1 <= block_slices <= d_count), so its device memory depends on the
+ * block size instead of on d_count.  map_bits 8 (max_disp <= 256, the u8 map calls) or 16 (max_disp <= 4096, the _u16
+ * calls).  Geometry, block size and map bits are validated before any CUDA call (PSM_EINVAL); allocation failure
+ * returns PSM_ENOMEM.  Every map equals the one an unblocked context with the same arguments gives, bit for bit.
+ * Device memory, with Wp = psm's row pitch (W rounded up to 4, plus 44 columns of halo, rounded up to 32 floats; at
+ * least 160) and B = block_slices:
+ *     4 * B * H * Wp * 4 bytes    the four volumes (two views, raw and filtered)
+ *   + 16 * H * W                  two running-key planes (uint64)
+ *   + about 2 * 20 * H * Wp * 4 + 2 * H * W * (3 * 4 + map_bits / 8)   guide planes, staging, maps
+ * plus what the stages allocate on first use (post-filter; reference-order scratch: 48 bytes per pixel; FGF: 16 * B
+ * bytes of coefficient means per low-resolution pixel).  At 1920 x 1080 (Wp = 1984) one slice of volume is 32.7 MiB: B = 128 takes about 4.3 GiB.
+ * Stages on a blocked context:
+ *   - psm_cost_const builds the raw costs of the first block (stage 1 times it);
+ *   - psm_cost_filter / psm_cost_filter_fgf compute the guide once, then filter every block (building its raw costs
+ *     first, for every block after the first) and fold its winner-take-all into the running keys.  Stage 2 covers the
+ *     whole walk; stage 4 is not recorded (psm_stage_ms(4) returns PSM_ESTATE);
+ *   - psm_disp_select* reduce the running keys to the maps (stage 3); psm_disp_select_keys copies them to the caller's
+ *     buffers, so blocked shards feed psm_disp_reduce_keys as unblocked ones do.  Post-filter and left-right check as usual;
+ *   - PSM_EINVAL, with the reason in psm_last_error: psm_write_cost_slice, psm_disp_select_keys_p2p, and
+ *     psm_read_cost_slice / psm_read_ab_slice of a slice that is not resident (the first block after psm_cost_const,
+ *     filtered costs of the last block after a filter stage);
+ *   - psm_device_ptr selectors 0 / 1 return the resident block (slice d at offset d - its first slice).
+ * See DESIGN.md section 16. */
+int psm_create_blocked(psm_ctx** out, int width, int height, int max_disp,
+                       int d_begin, int d_count, int block_slices, int map_bits, int device);
+
 /* Waits for the context's work on the stream it is bound to (psm_set_stream), on its own stream and on its copy stream,
  * then frees everything: a caller's stream bound with psm_set_stream must still exist when this is called. */
 int psm_destroy(psm_ctx* ctx);

@@ -95,6 +95,12 @@ struct psm_ctx {
     int lr_mode = PSM_LR_OFF;               // left-right check and fill in front of the post-filter, psm_set_lr_check
     uint8_t* lr_valid[2] = {nullptr, nullptr};  // the check's masks (W x H, 0/1), lazy
     bool lr_masks_ok = false;               // lr_valid holds the masks of the current maps (psm_read_valid_mask)
+    // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
+    // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
+    int blk_slices = 0;
+    int res_begin = 0, res_count = 0;       // blocked: the global slices resident in the volumes
+    unsigned long long* run_keys[2] = {nullptr, nullptr};  // blocked: running (cost, d) keys per view, [H][W]
+    int vol_slices() const { return blk_slices ? blk_slices : d_count; }   // slices the volumes and per-slice scratch hold
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -500,6 +506,89 @@ int launch_cvf_window(psm_ctx* c)
     return PSM_OK;
 }
 
+// K1: both raw volumes of the context's slice range
+int launch_cvc(psm_ctx* c)
+{
+    CvcParams2 P2;
+    for (int v = 0; v < 2; ++v) {
+        CvcParams& P = P2.v[v];
+        const float* gs = c->guide[v];
+        const float* go = c->guide[1 - v];
+        for (int k = 0; k < 3; ++k) { P.self[k] = gs + k * c->plane; P.other[k] = go + k * c->plane; }
+        P.self[3] = c->grd[v];
+        P.other[3] = c->grd[1 - v];
+        P.vol = c->vol[v];
+        P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count;
+        P.fold_halo = c->W >= 32 ? 1 : 0;
+    }
+    // option 108 (tuning): slices per CTA (0 = all owned slices in one CTA, the shipped decomposition)
+    P2.chunk = (c->cvc_chunk > 0 && c->cvc_chunk < c->d_count) ? c->cvc_chunk : 0;
+    const int nchunks = P2.chunk ? (c->d_count + P2.chunk - 1) / P2.chunk : 1;
+    dim3 blk(128), grd((((c->W + 3) / 4) + 127) / 128, c->H, 2 * nchunks);
+    // option 106 (tuning): 0 shipped = interior fast path + scalar window loads; 2 = no fast path (the round-1 loop);
+    // 1 / 3 = fast path + grouped 128-bit window loads for the border warps without / with a register cap (DESIGN.md section 10)
+    // Any matching cost other than the default runs the parameterised build of the shipped variant, all owned slices
+    // per CTA: options 106 and 108 do not apply to it.
+    if (!c->cost_default()) {
+        grd.z = 2;
+        cvc_cost_kernel<<<grd, blk, 0, c->stream>>>(P2, c->cost);
+    } else {
+        switch (c->cvc_variant) {
+        case 1: cvc_both_kernel<4, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+        case 2: cvc_both_kernel<7, 2><<<grd, blk, 0, c->stream>>>(P2); break;
+        case 3: cvc_both_kernel<5, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+        default: cvc_both_kernel<7, 0><<<grd, blk, 0, c->stream>>>(P2); break;
+        }
+    }
+    PSM_LAUNCH_CHECK(c);
+    if (!P2.v[0].fold_halo)  // narrow images: separate halo pass (general reflection)
+        for (int v = 0; v < 2; ++v)
+            if (int rc = pad_rows(c, c->vol[v], (size_t)c->d_count * c->H)) return rc;
+    return PSM_OK;
+}
+
+// A blocked context runs the launchers above, which take their slice range from the context, on one block: for the
+// scope's life the context's range is the block's, and its volumes hold that block.
+struct BlockScope {
+    psm_ctx* c;
+    int begin, count;
+    BlockScope(psm_ctx* ctx, int b, int n) : c(ctx), begin(ctx->d_begin), count(ctx->d_count)
+    {
+        c->d_begin = b; c->d_count = n;
+        c->res_begin = b; c->res_count = n;
+    }
+    ~BlockScope() { c->d_begin = begin; c->d_count = count; }
+};
+
+// the filtered block in the volumes -> the running keys (stored by the first block, min-folded by the others)
+int launch_fold(psm_ctx* c, bool first)
+{
+    FoldParams P;
+    for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count; P.first = first ? 1 : 0;
+    dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, 2);
+    wta_fold_kernel<<<grd, blk, 0, c->stream>>>(P);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
+// A blocked context's filter stage: every block of [d_begin, d_begin + d_count) in turn gets its raw costs (the first
+// block's are psm_cost_const's), `filter` (which leaves the filtered block in c->vol) and the fold into the running keys.
+template <class Filter>
+int run_blocks(psm_ctx* c, Filter filter)
+{
+    const int end = c->d_begin + c->d_count;
+    for (int b = c->d_begin; b < end; b += c->blk_slices) {
+        const bool first = b == c->d_begin;
+        BlockScope scope(c, b, std::min(c->blk_slices, end - b));
+        if (!first)
+            if (int rc = launch_cvc(c)) return rc;
+        if (int rc = filter()) return rc;
+        if (int rc = launch_fold(c, first)) return rc;
+    }
+    return PSM_OK;
+}
+
 // device map -> host rows of W elements of the context's map format
 int copy_map_out(psm_ctx* c, const uint8_t* dsrc, void* dst, size_t step)
 {
@@ -554,7 +643,8 @@ int psm_cvf_plan(int width, int height, int d_count, int sm_count, int no_pack, 
 }  // extern "C"
 
 // geometry already validated by the caller; map_bytes 1 (u8 maps) or 2 (u16 maps)
-static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device, int map_bytes)
+static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device, int map_bytes,
+                      int block_slices = 0)
 {
     int ndev = psm_device_count();
     if (device < 0 || device >= ndev) return fail(nullptr, PSM_ECUDA, "CUDA device %d not available (%d devices)", device, ndev);
@@ -564,6 +654,7 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
     c->d_begin = d_begin; c->d_count = d_count; c->device = device;
     c->plane = (size_t)c->H * c->Wp;
     c->map_bytes = map_bytes;
+    c->blk_slices = block_slices;
     auto bail = [&](int code) {
         snprintf(g_create_error, sizeof(g_create_error), "%s", c->err);
         psm_destroy(c);
@@ -592,7 +683,7 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
         *out = raw + kPadLeft;
         return e;
     };
-    const size_t vol_rows = (size_t)d_count * c->H;
+    const size_t vol_rows = (size_t)c->vol_slices() * c->H;
     for (int v = 0; v < 2; ++v) {
         PSM_CREATE_CUDA(halo_alloc(&c->guide[v], (size_t)kGuidePlanes * c->H));
         PSM_CREATE_CUDA(halo_alloc(&c->grd[v], (size_t)c->H));
@@ -601,10 +692,11 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
         PSM_CREATE_CUDA(cudaMalloc(&c->stage_in[v], (size_t)c->W * c->H * 3 * sizeof(float)));
         PSM_CREATE_CUDA(cudaMalloc(&c->dis[v], (size_t)c->W * c->H * map_bytes));
         PSM_CREATE_CUDA(cudaMemsetAsync(c->dis[v], 0, (size_t)c->W * c->H * map_bytes, c->stream));
+        if (block_slices) PSM_CREATE_CUDA(cudaMalloc(&c->run_keys[v], (size_t)c->W * c->H * sizeof(unsigned long long)));
     }
     PSM_CREATE_CUDA(cudaMalloc(&c->guide_flags, 2 * sizeof(int)));
-    PSM_CREATE_CUDA(cudaMalloc(&c->slice_flags, 2 * (size_t)c->d_count * sizeof(int)));
-    PSM_CREATE_CUDA(cudaMemsetAsync(c->slice_flags, 0, 2 * (size_t)c->d_count * sizeof(int), c->stream));
+    PSM_CREATE_CUDA(cudaMalloc(&c->slice_flags, 2 * (size_t)c->vol_slices() * sizeof(int)));
+    PSM_CREATE_CUDA(cudaMemsetAsync(c->slice_flags, 0, 2 * (size_t)c->vol_slices() * sizeof(int), c->stream));
     PSM_CREATE_CUDA(cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
     PSM_CREATE_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->up_done, cudaEventDisableTiming));
@@ -646,6 +738,23 @@ int psm_create_u16(psm_ctx** out, int width, int height, int max_disp, int d_beg
     return create_ctx(out, width, height, max_disp, d_begin, d_count, device, 2);
 }
 
+int psm_create_blocked(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int block_slices,
+                       int map_bits, int device)
+{
+    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
+    *out = nullptr;
+    if (map_bits != 8 && map_bits != 16) return fail(nullptr, PSM_EINVAL, "map_bits must be 8 or 16 (got %d)", map_bits);
+    const int dmax = map_bits == 8 ? MapFormat<uint8_t>::kMaxDisp : MapFormat<uint16_t>::kMaxDisp;
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > dmax)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d with %d-bit maps)", width, height,
+                    max_disp, dmax, map_bits);
+    if (d_begin < 0 || d_count < 1 || d_begin + d_count > max_disp)
+        return fail(nullptr, PSM_EINVAL, "bad shard [%d,%d) of %d", d_begin, d_begin + d_count, max_disp);
+    if (block_slices < 1 || block_slices > d_count)
+        return fail(nullptr, PSM_EINVAL, "block_slices %d outside 1..%d (the context's d_count)", block_slices, d_count);
+    return create_ctx(out, width, height, max_disp, d_begin, d_count, device, map_bits / 8, block_slices);
+}
+
 int psm_create(psm_ctx** out, int width, int height, int max_disp, int device)
 {
     return psm_create_sharded(out, width, height, max_disp, 0, max_disp, device);
@@ -675,7 +784,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->guide_flags);
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
-    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); }
+    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]); }
     for (int s = 0; s < kNumStages; ++s) {
         if (c->ev0[s]) cudaEventDestroy(c->ev0[s]);
         if (c->ev1[s]) cudaEventDestroy(c->ev1[s]);
@@ -861,43 +970,14 @@ int psm_cost_const(psm_ctx* c)
     if (int rc = bind(c)) return rc;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_cost_const before psm_set_images");
     if (int rc = stage_begin(c, 1)) return rc;
-    CvcParams2 P2;
-    for (int v = 0; v < 2; ++v) {
-        CvcParams& P = P2.v[v];
-        const float* gs = c->guide[v];
-        const float* go = c->guide[1 - v];
-        for (int k = 0; k < 3; ++k) { P.self[k] = gs + k * c->plane; P.other[k] = go + k * c->plane; }
-        P.self[3] = c->grd[v];
-        P.other[3] = c->grd[1 - v];
-        P.vol = c->vol[v];
-        P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count;
-        P.fold_halo = c->W >= 32 ? 1 : 0;
+    int rc;
+    if (c->blk_slices) {   // the first block; the filter stages build the others
+        BlockScope scope(c, c->d_begin, c->blk_slices);
+        rc = launch_cvc(c);
+    } else {
+        rc = launch_cvc(c);
     }
-    {
-        // option 108 (tuning): slices per CTA (0 = all owned slices in one CTA, the shipped decomposition)
-        P2.chunk = (c->cvc_chunk > 0 && c->cvc_chunk < c->d_count) ? c->cvc_chunk : 0;
-        const int nchunks = P2.chunk ? (c->d_count + P2.chunk - 1) / P2.chunk : 1;
-        dim3 blk(128), grd((((c->W + 3) / 4) + 127) / 128, c->H, 2 * nchunks);
-        // option 106 (tuning): 0 shipped = interior fast path + scalar window loads; 2 = no fast path (the round-1 loop);
-        // 1 / 3 = fast path + grouped 128-bit window loads for the border warps without / with a register cap (DESIGN.md section 10)
-        // Any matching cost other than the default runs the parameterised build of the shipped variant, all owned slices
-        // per CTA: options 106 and 108 do not apply to it.
-        if (!c->cost_default()) {
-            grd.z = 2;
-            cvc_cost_kernel<<<grd, blk, 0, c->stream>>>(P2, c->cost);
-        } else {
-            switch (c->cvc_variant) {
-            case 1: cvc_both_kernel<4, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-            case 2: cvc_both_kernel<7, 2><<<grd, blk, 0, c->stream>>>(P2); break;
-            case 3: cvc_both_kernel<5, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-            default: cvc_both_kernel<7, 0><<<grd, blk, 0, c->stream>>>(P2); break;
-            }
-        }
-        PSM_LAUNCH_CHECK(c);
-        if (!P2.v[0].fold_halo)  // narrow images: separate halo pass (general reflection)
-            for (int v = 0; v < 2; ++v)
-                if (int rc = pad_rows(c, c->vol[v], (size_t)c->d_count * c->H)) return rc;
-    }
+    if (rc) return rc;
     if (int rc = clear_slice_flags(c)) return rc;
     c->have_cvc = true;
     c->filtered = false;
@@ -914,21 +994,29 @@ int psm_cost_filter(psm_ctx* c)
                     c->gif_win, (double)c->gif_eps);
     if (int rc = stage_begin(c, 2)) return rc;
     if (int rc = ensure_guide(c)) return rc;
-    if (int rc = stage_begin(c, 4)) return rc;
     // NAIVE and images below one strip: every slice in OpenCV's order.  Otherwise the tuned kernel, then, in OpenCV's
     // order, the slices psm_write_cost_slice flagged and every slice of a view whose image is outside the integer domain
     // or whose solve terms are not finite (psm_cvf_ref.cuh).  The second launch is needed only where a flag can be set:
     // flagged slices, float images, a non-default window or eps.  u8 frames at the defaults run the tuned kernel alone.
-    if (c->gif_default() && (c->cvf_mode == PSM_CVF_NAIVE || c->W < 16 || c->H < 16)) {
-        if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAll)) return rc;
+    const auto filter = [c]() -> int {
+        if (c->gif_default() && (c->cvf_mode == PSM_CVF_NAIVE || c->W < 16 || c->H < 16)) {
+            if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAll)) return rc;
+        } else {
+            if (int rc = c->gif_default() ? launch_cvf_stream(c) : launch_cvf_window(c)) return rc;
+            if (c->slices_flagged || c->float_images || !c->gif_default())
+                if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefFlagged)) return rc;
+        }
+        if (int rc = clear_slice_flags(c)) return rc;
+        for (int v = 0; v < 2; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
+        return PSM_OK;
+    };
+    if (c->blk_slices) {   // stage 4 is not recorded: its kernels interleave with every block's CVC and fold
+        if (int rc = run_blocks(c, filter)) return rc;
     } else {
-        if (int rc = c->gif_default() ? launch_cvf_stream(c) : launch_cvf_window(c)) return rc;
-        if (c->slices_flagged || c->float_images || !c->gif_default())
-            if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefFlagged)) return rc;
+        if (int rc = stage_begin(c, 4)) return rc;
+        if (int rc = filter()) return rc;
+        if (int rc = stage_end(c, 4)) return rc;
     }
-    if (int rc = clear_slice_flags(c)) return rc;
-    if (int rc = stage_end(c, 4)) return rc;
-    for (int v = 0; v < 2; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
     c->have_cvc = false;  // the volumes now hold filtered costs; filtering again needs a new CVC
     c->filtered = true;
     return stage_end(c, 2);
@@ -957,7 +1045,7 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
         cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
         c->fgf_lo[0] = c->fgf_lo[1] = c->fgf_mean = nullptr; c->fgf_plan = nullptr; c->fgf_s = 0;
         for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->fgf_lo[v], 12 * n2 * sizeof(float)));
-        PSM_CUDA(c, cudaMalloc(&c->fgf_mean, (size_t)4 * c->d_count * n2 * sizeof(float)));
+        PSM_CUDA(c, cudaMalloc(&c->fgf_mean, (size_t)4 * c->vol_slices() * n2 * sizeof(float)));
         PSM_CUDA(c, cudaMalloc(&c->fgf_plan, (size_t)(c->W + c->H) * sizeof(FgfTap)));
         // cv::resize INTER_LINEAR coordinates (OpenCV's own implementation; same expressions as the CPU restatement fgf_build in oracle/)
         FgfTap* hp = new (std::nothrow) FgfTap[c->W + c->H];
@@ -983,12 +1071,15 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
     FgfPlan pl;
     pl.x = static_cast<const FgfTap*>(c->fgf_plan);
     pl.y = pl.x + c->W;
-    if (int rc = stage_begin(c, 2)) return rc;
-    if (int rc = stage_begin(c, 4)) return rc;
-    for (int v = 0; v < 2; ++v) {
+    // the low-resolution guide of view v, then the filter of view v's resident slices
+    const auto guide = [&](int v) -> int {
         dim3 blk(128), g2((g.w2 + 127) / 128, g.h2);
         fgf_guide_kernel<<<g2, blk, 0, c->stream>>>(c->guide[v], c->plane, g, c->gif_eps, c->fgf_lo[v]);
         PSM_LAUNCH_CHECK(c);
+        return PSM_OK;
+    };
+    const auto slices = [&](int v) -> int {
+        dim3 blk(128);
         dim3 g3((g.w2 + kFgfTX - 1) / kFgfTX, (g.h2 + kFgfTY - 1) / kFgfTY, c->d_count);
         const size_t fsmem = fgf_smem_bytes(g.K);
         PSM_CUDA(c, cudaFuncSetAttribute(fgf_lowres_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
@@ -997,8 +1088,25 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
         dim3 g5((((c->W + 3) / 4) + 127) / 128, c->H, c->d_count);
         fgf_up_kernel<<<g5, blk, 0, c->stream>>>(c->vol[v], c->plane, c->guide[v], c->plane, g, pl, c->fgf_mean);
         PSM_LAUNCH_CHECK(c);
+        return PSM_OK;
+    };
+    if (int rc = stage_begin(c, 2)) return rc;
+    if (c->blk_slices) {   // both guides once, then every block; stage 4 is not recorded
+        for (int v = 0; v < 2; ++v)
+            if (int rc = guide(v)) return rc;
+        if (int rc = run_blocks(c, [&]() -> int {
+                for (int v = 0; v < 2; ++v)
+                    if (int rc = slices(v)) return rc;
+                return PSM_OK;
+            })) return rc;
+    } else {
+        if (int rc = stage_begin(c, 4)) return rc;
+        for (int v = 0; v < 2; ++v) {
+            if (int rc = guide(v)) return rc;
+            if (int rc = slices(v)) return rc;
+        }
+        if (int rc = stage_end(c, 4)) return rc;
     }
-    if (int rc = stage_end(c, 4)) return rc;
     c->have_cvc = false;
     c->filtered = true;
     return stage_end(c, 2);
@@ -1010,6 +1118,15 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
 template <typename T>
 static int select_maps(psm_ctx* c)
 {
+    if (c->blk_slices) {   // a blocked context's selection is in its running keys: reduce them as one rank's
+        const size_t npix = (size_t)c->W * c->H;
+        for (int v = 0; v < 2; ++v) {
+            keys_reduce_kernel<T><<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(c->run_keys[v], 1, npix,
+                                                                                         reinterpret_cast<T*>(c->dis[v]));
+            PSM_LAUNCH_CHECK(c);
+        }
+        return PSM_OK;
+    }
     for (int v = 0; v < 2; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
         wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
@@ -1098,6 +1215,12 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
     uint64_t* keys[2] = {d_keys_left, d_keys_right};
+    if (c->blk_slices) {   // the running keys are this context's minima already
+        for (int v = 0; v < 2; ++v)
+            PSM_CUDA(c, cudaMemcpyAsync(keys[v], c->run_keys[v], (size_t)c->W * c->H * sizeof(uint64_t),
+                                        cudaMemcpyDeviceToDevice, c->stream));
+        return stage_end(c, 3);
+    }
     for (int v = 0; v < 2; ++v) {   // keys only, on either map format
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
         wta_kernel<uint8_t><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, nullptr,
@@ -1200,6 +1323,9 @@ static void p2p_fill(const psm_ctx* c, int view, P2pPeers& peers)
 int psm_disp_select_keys_p2p(psm_ctx* c)
 {
     if (int rc = bind(c)) return rc;
+    if (c->blk_slices)
+        return fail(c, PSM_EINVAL, "psm_disp_select_keys_p2p on a blocked context: the fused exchange scans whole volumes, a "
+                    "blocked context holds one block; use psm_disp_select_keys + psm_disp_reduce_keys");
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "psm_p2p_create_buffer / psm_p2p_set_peers first");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys_p2p before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
@@ -1422,15 +1548,21 @@ static int check_slice(psm_ctx* c, int view, int d)
     if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
     if (d < c->d_begin || d >= c->d_begin + c->d_count)
         return fail(c, PSM_EINVAL, "slice %d not owned by this context [%d,%d)", d, c->d_begin, c->d_begin + c->d_count);
+    if (c->blk_slices && (d < c->res_begin || d >= c->res_begin + c->res_count))
+        return fail(c, PSM_EINVAL, "slice %d is not resident: this blocked context holds slices [%d,%d) only (the first block "
+                    "after psm_cost_const, the last after a filter stage)", d, c->res_begin, c->res_begin + c->res_count);
     return PSM_OK;
 }
+
+// the offset of a checked slice in the volumes
+static size_t slice_offset(const psm_ctx* c, int d) { return (size_t)(d - (c->blk_slices ? c->res_begin : c->d_begin)) * c->plane; }
 
 int psm_read_cost_slice(psm_ctx* c, int view, int d, float* dst, size_t dst_step)
 {
     if (int rc = bind(c)) return rc;
     if (int rc = check_slice(c, view, d)) return rc;
     if (!dst || dst_step < (size_t)c->W * sizeof(float)) return fail(c, PSM_EINVAL, "bad dst/step");
-    PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->vol[view] + (size_t)(d - c->d_begin) * c->plane,
+    PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->vol[view] + slice_offset(c, d),
                                   c->Wp * sizeof(float), c->W * sizeof(float), c->H, cudaMemcpyDeviceToHost, c->stream));
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
@@ -1439,6 +1571,9 @@ int psm_read_cost_slice(psm_ctx* c, int view, int d, float* dst, size_t dst_step
 int psm_write_cost_slice(psm_ctx* c, int view, int d, const float* src, size_t src_step)
 {
     if (int rc = bind(c)) return rc;
+    if (c->blk_slices)
+        return fail(c, PSM_EINVAL, "psm_write_cost_slice on a blocked context: the filter stages rebuild every block after the "
+                    "first from the images, so a written slice would not be filtered");
     if (int rc = check_slice(c, view, d)) return rc;
     if (!src || src_step < (size_t)c->W * sizeof(float)) return fail(c, PSM_EINVAL, "bad src/step");
     PSM_CUDA(c, cudaMemcpy2DAsync(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->Wp * sizeof(float), src,
@@ -1491,7 +1626,14 @@ int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
     if (!c->have_images) return fail(c, PSM_ESTATE, "no images set");
     if (int rc = ensure_guide(c)) return rc;
     // a, b in OpenCV's order (psm_cvf_ref.cuh), left in the scratch planes [4][H][W]
-    if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->d_begin)) return rc;
+    int rc;
+    if (c->blk_slices) {
+        BlockScope scope(c, c->res_begin, c->res_count);
+        rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->res_begin);
+    } else {
+        rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->d_begin);
+    }
+    if (rc) return rc;
     const size_t n = (size_t)c->W * c->H;
     PSM_CUDA(c, cudaMemcpyAsync(a3, c->ref_pl, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     PSM_CUDA(c, cudaMemcpyAsync(b, c->ref_pl + 3 * n, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));

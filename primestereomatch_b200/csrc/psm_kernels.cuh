@@ -568,6 +568,51 @@ __global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol,
     }
 }
 
+// WTA of one block of slices of a blocked context (psm_create_blocked), both views in one launch (blockIdx.z = view):
+// the wta_kernel scan over the block's d_count slices starting at global d_begin, then its packed (cost, d) key is
+// stored (first block) or folded into the running key by min.  The min over keys of consecutive blocks is the
+// selection over their union: the strict <, the lowest-d tie-break and +inf / NaN costs behave as in one scan.
+struct FoldParams {
+    const float* vol[2];             // the block's filtered volumes [d_count][H][Wp]
+    unsigned long long* keys[2];     // running keys [H][W]
+    int W, H, Wp, d_begin, d_count, first;
+};
+
+__global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
+{
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y, view = blockIdx.z;
+    if (x4 >= P.W) return;
+    const size_t plane = (size_t)P.H * P.Wp;
+    // views selected, not indexed: a parameter array indexed by a run-time value is copied to the stack
+    const float* p = (view ? P.vol[1] : P.vol[0]) + (size_t)y * P.Wp + x4;
+    float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+    int md[4] = {0, 0, 0, 0};
+    int dl = (P.d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (DispSel.cpp:96)
+#pragma unroll 8
+    for (; dl < P.d_count; ++dl) {
+        const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
+        const int d = P.d_begin + dl;
+        if (c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
+        if (c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
+        if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
+        if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
+    }
+    unsigned long long* k = (view ? P.keys[1] : P.keys[0]) + (size_t)y * P.W;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int x = x4 + j;
+        if (x < P.W) {
+            unsigned long long v = ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j];
+            if (!P.first) {
+                const unsigned long long old = k[x];
+                v = old < v ? old : v;
+            }
+            k[x] = v;
+        }
+    }
+}
+
 // Sharded WTA fused with its exchange (reduce-scatter + all-gather of a min-reduction, hand-rolled
 // over NVLink peer memory).  Pixels are partitioned into `nranks` chunks; rank r is the reducer of
 // chunk r.

@@ -36,9 +36,13 @@ class DispEst:
     map_bits : None (8-bit maps for d <= 256, 16-bit above), 8 or 16 (16-bit maps at any d, d <= 4096).  With 16 bits
     lDisMap / rDisMap are uint16 (CV_16UC1) and the context comes from psm_create_u16; their low byte is the
     reference's uchar map.
+    block_slices : None (the volumes hold every owned slice) or the number of slices a blocked context
+    (psm_create_blocked) holds at once: the filter stages walk the owned range in blocks of that many, so device memory
+    depends on it instead of on d.  The maps are the same either way; read_cost_volume is not available.
     """
 
-    def __init__(self, l, r, d, t=MAX_CPU_THREADS, ocl=True, device=0, d_begin=0, d_count=None, map_bits=None):
+    def __init__(self, l, r, d, t=MAX_CPU_THREADS, ocl=True, device=0, d_begin=0, d_count=None, map_bits=None,
+                 block_slices=None):
         l, r = np.asarray(l), np.asarray(r)
         if l.dtype != r.dtype or l.shape != r.shape:
             # reference: "DE: Error - Left & Right images are of different types." then exit(1)
@@ -66,9 +70,14 @@ class DispEst:
             L = capi.lib()
             self._lib = L
             dc = self.maxDis - d_begin if d_count is None else d_count
-            create = L.psm_create_u16 if self.map_bits == 16 else L.psm_create_sharded
-            capi.check(create(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc), int(device)))
+            if block_slices is not None:
+                capi.check(L.psm_create_blocked(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc),
+                                                int(block_slices), self.map_bits, int(device)))
+            else:
+                create = L.psm_create_u16 if self.map_bits == 16 else L.psm_create_sharded
+                capi.check(create(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc), int(device)))
         self.d_begin, self.d_count = d_begin, (self.maxDis - d_begin if d_count is None else d_count)
+        self.block_slices = block_slices
 
     # -- lifetime ---------------------------------------------------------------------------
     def close(self):
@@ -212,6 +221,9 @@ class DispEst:
         return out
 
     def read_cost_volume(self, view):
+        if self.block_slices is not None:
+            raise RuntimeError("read_cost_volume on a blocked context: it holds one block of slices at a time "
+                               "(read_cost_slice reads a slice of the resident block)")
         return np.stack([self.read_cost_slice(view, d) for d in range(self.d_begin, self.d_begin + self.d_count)])
 
     def write_cost_slice(self, view, d, src):

@@ -74,8 +74,9 @@ inline int b200devicepoll() { return psm_device_count(); }
 
 class DispEst {
 public:
-    // reference src/DispEst.cpp:10-143.  `ocl` == use the GPU path.
-    DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl);
+    // reference src/DispEst.cpp:10-143.  `ocl` == use the GPU path.  block_slices > 0: a blocked context
+    // (psm_create_blocked) that holds that many disparity slices at a time, for ranges the device cannot hold whole.
+    DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices = 0);
     ~DispEst(void);
 
     cv::Mat lDisMap;  // CV_8UC1, raw disparity index (reference DispEst.h:28-29); CV_16UC1 when maxDis > 256 (psm_create_u16),
