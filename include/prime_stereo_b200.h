@@ -164,6 +164,42 @@ int psm_create_u16(psm_ctx** out, int width, int height, int max_disp,
 int psm_create_blocked(psm_ctx** out, int width, int height, int max_disp,
                        int d_begin, int d_count, int block_slices, int map_bits, int device);
 
+/* Multi-device context: one context over n_devices shards in this process, shard k on CUDA device devices[k] owning the
+ * contiguous slices sharding.py's shard_range gives (max_disp / n_devices each, the last shard takes the remainder).
+ * Devices may repeat: several shards on one device is a legal configuration.  block_slices 0 gives unblocked shards,
+ * otherwise every shard is blocked (psm_create_blocked) with min(block_slices, its slice count).  map_bits 8
+ * (max_disp <= 256, the u8 map calls) or 16 (max_disp <= 4096, the _u16 calls).  Every map equals the one a single-device
+ * context of the same geometry gives, bit for bit.
+ *   - PSM_EINVAL before any CUDA call: bad geometry or map bits, n_devices outside 1..min(8, max_disp), a null `devices`,
+ *     a negative device id or block_slices < 0.  Then PSM_EINVAL for a device id at or above the device count, or for a
+ *     pair of distinct devices without peer access (the message names the pair).  Peer access is enabled between every
+ *     pair of distinct devices ("already enabled" is success) and never disabled: it is process-wide.  Allocation
+ *     failure returns PSM_ENOMEM and frees what was built.
+ *   - Every setter, psm_set_option (except PSM_OPT_P2P_SYNC), psm_cost_const, psm_cost_filter and psm_cost_filter_fgf
+ *     go to every shard; a setter value one shard rejects leaves the context unchanged.
+ *   - psm_set_images / _u8: the first shard uploads the frame once, as a single-device context does (host buffers are
+ *     reusable on return); every other shard receives it from the first shard's device memory, device to device, and
+ *     ingests it itself.  psm_set_images_device takes images resident on the first device, ordered against the work the
+ *     context enqueues as for a single-device context (psm_sync, or the caller's own synchronisation).
+ *   - psm_disp_select* and _u16: every shard scatters its minima (blocked shards: their running keys) into the
+ *     reducers' exchange blocks, then every shard reduces its pixel chunk into every shard's maps; the kernels are
+ *     ordered by CUDA events across the shards' streams and never wait on a flag.  The first shard's maps are the
+ *     context's: psm_device_ptr selectors 2 / 3 (complete once psm_sync returns after psm_disp_select_device), the
+ *     post-process (psm_post_process, _u16, _device, psm_read_valid_mask, selectors 4-7) runs on the first shard.
+ *   - psm_read_cost_slice, psm_read_ab_slice and psm_write_cost_slice (unblocked shards only) go to the shard that owns
+ *     global slice d; psm_read_guide_plane reads the first shard's planes.
+ *   - psm_stage_ms: stages 0-2 and 4 are the longest of the shards' own times (stage 0 of the other shards covers the
+ *     device-to-device copy; stage 4 is not recorded on blocked shards); stage 3 is timed on the first shard's stream
+ *     from before its scatter to its maps being complete, so it includes the waits for the other shards; stage 5 is the
+ *     first shard's.  psm_launch_count is the sum over the shards, psm_sync waits for every shard.
+ *   - PSM_EINVAL, with the reason in psm_last_error: psm_set_stream (a stream belongs to one device), the asynchronous
+ *     upload pair psm_set_images_async / _u8_async / _commit, psm_device_ptr selectors 0 / 1 (the volumes are split),
+ *     psm_disp_select_keys, psm_disp_reduce_keys*, every psm_p2p_* / psm_ipc_* / *_p2p call, PSM_OPT_P2P_SYNC.
+ * Device memory per shard: the shard's context (psm_create_u16 or psm_create_blocked of its slices) plus its exchange
+ * block, about 16 * H * W + 2 * H * W * map_bits / 8 bytes.  See DESIGN.md section 17. */
+int psm_create_multi(psm_ctx** out, int width, int height, int max_disp,
+                     const int* devices, int n_devices, int block_slices, int map_bits);
+
 /* Waits for the context's work on the stream it is bound to (psm_set_stream), on its own stream and on its copy stream,
  * then frees everything: a caller's stream bound with psm_set_stream must still exist when this is called. */
 int psm_destroy(psm_ctx* ctx);

@@ -22,7 +22,7 @@ SYMBOLS = [
     "psm_launch_count", "psm_sync", "psm_last_error", "psm_build_info", "psm_cvf_plan", "psm_set_guided_filter",
     "psm_set_matching_cost", "psm_set_post_filter", "psm_create_u16", "psm_disp_select_u16", "psm_disp_select_u16_async",
     "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
-    "psm_create_blocked",
+    "psm_create_blocked", "psm_create_multi",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -58,6 +58,7 @@ def lib():
     L.psm_create_sharded.argtypes = [C.POINTER(vp), i, i, i, i, i, i]
     L.psm_create_u16.argtypes = [C.POINTER(vp), i, i, i, i, i, i]
     L.psm_create_blocked.argtypes = [C.POINTER(vp), i, i, i, i, i, i, i, i]
+    L.psm_create_multi.argtypes = [C.POINTER(vp), i, i, i, C.POINTER(C.c_int), i, i, i]
     L.psm_disp_select_u16.argtypes = [vp, vp, sz, vp, sz]
     L.psm_disp_select_u16_async.argtypes = [vp, vp, sz, vp, sz]
     L.psm_disp_reduce_keys_u16.argtypes = [vp, vp, vp, i, vp, sz, vp, sz]

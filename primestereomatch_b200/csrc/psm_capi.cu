@@ -101,6 +101,15 @@ struct psm_ctx {
     int res_begin = 0, res_count = 0;       // blocked: the global slices resident in the volumes
     unsigned long long* run_keys[2] = {nullptr, nullptr};  // blocked: running (cost, d) keys per view, [H][W]
     int vol_slices() const { return blk_slices ? blk_slices : d_count; }   // slices the volumes and per-slice scratch hold
+    // psm_create_multi: the context drives nshards shard contexts (shard k on its own device, owning the slices
+    // shard_range(D, nshards, k)) through the fused exchange, ordered by these events; every other context has none
+    int nshards = 0;
+    psm_ctx* shard[kMaxRanks] = {};
+    cudaEvent_t ev_scattered[kMaxRanks] = {};  // shard k's scatter of the current frame (on its stream)
+    cudaEvent_t ev_reduced[kMaxRanks] = {};    // shard k's reduce of the last frame (on its stream)
+    bool reduced_valid = false;
+    cudaEvent_t ev_copied[kMaxRanks] = {};     // shard k (k >= 1) has read the frame it receives from the first shard
+    cudaEvent_t ev_images = nullptr;           // psm_set_images_device: the caller's images as the first shard's stream sees them
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -611,6 +620,87 @@ int check_map_format(psm_ctx* c, const char* u8_call, const char* u16_call)
     return fail(c, PSM_EINVAL, "%s on a context with 8-bit maps (psm_create / psm_create_sharded): use %s", u16_call, u8_call);
 }
 
+// ---- multi-device contexts (psm_create_multi) ----
+// The context aliases the first shard's stream and complete maps (the maps in its exchange block), so the map calls that
+// copy out or sync run unchanged on it; every other call is forwarded to the shards, or rejected.
+
+bool is_multi(const psm_ctx* c) { return c && c->nshards; }
+
+// a call on shard k failed: its error becomes the multi-device context's
+int relay(psm_ctx* c, int k, int rc)
+{
+    if (rc) {
+        char text[512];
+        snprintf(text, sizeof(text), "%s", c->shard[k]->err);
+        fail(c, rc, "shard %d (device %d): %s", k, c->shard[k]->device, text);
+    }
+    return rc;
+}
+
+// the same call on every shard in turn, up to the first failure.  The setters judge the value alone, the same way on
+// every shard, so a value that one shard rejects is rejected by the first one, before any shard has changed.
+template <class F>
+int forward(psm_ctx* c, F f)
+{
+    for (int k = 0; k < c->nshards; ++k)
+        if (int rc = f(c->shard[k])) return relay(c, k, rc);
+    return PSM_OK;
+}
+
+int reject_multi(psm_ctx* c, const char* call, const char* why)
+{
+    return fail(c, PSM_EINVAL, "%s on a multi-device context (psm_create_multi): %s", call, why);
+}
+
+// psm_set_images[_u8|_device] on a multi-device context.  The first shard ingests the frame as a single-device context
+// does (a host frame: one upload into its staging set).  Every other shard receives the frame device to device into its
+// own staging set and runs its own ingest kernels; its stage 0 covers the copy.  The staging sets' readers and writers:
+//   - shard k's copy starts once the source holds the frame (the first shard's staging set after its upload, or the
+//     caller's device images at the first shard's ingest) and once shard k's last ingest has read shard k's staging set;
+//   - the source's next writer follows every copy: the first shard's copy stream (its next upload) for a host frame, the
+//     first shard's stream (which the caller orders its overwrites against) for device images;
+//   - shard k's ingest kernels follow its copy, and its next copy follows them (ingest_done).
+template <typename T>
+int multi_set_images(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool from_device)
+{
+    psm_ctx* s0 = c->shard[0];
+    int rc = bind(s0);
+    if (!rc) rc = stage_begin(s0, 0);
+    if (!rc) rc = ingest<T>(s0, l, lstep, r, rstep, from_device);
+    if (!rc) rc = stage_end(s0, 0);
+    if (rc) return relay(c, 0, rc);
+    const size_t row = (size_t)c->W * 3 * sizeof(T);
+    const void* src[2] = {l, r};
+    size_t step[2] = {lstep, rstep};
+    cudaEvent_t ready = s0->host_copied;
+    cudaStream_t next_writer = s0->copy_stream;
+    if (from_device) {
+        PSM_CUDA(c, cudaEventRecord(c->ev_images, s0->stream));
+        ready = c->ev_images;
+        next_writer = s0->stream;
+    } else {
+        for (int v = 0; v < 2; ++v) { src[v] = stage_buf(s0, s0->stage_cur, v); step[v] = row; }
+    }
+    for (int k = 1; k < c->nshards; ++k) {
+        psm_ctx* s = c->shard[k];
+        if ((rc = bind(s))) return relay(c, k, rc);
+        if (s->ingest_done_valid[0]) PSM_CUDA(c, cudaStreamWaitEvent(s->copy_stream, s->ingest_done[0], 0));
+        PSM_CUDA(c, cudaStreamWaitEvent(s->copy_stream, ready, 0));
+        if (s->timing) PSM_CUDA(c, cudaEventRecord(s->ev0[0], s->copy_stream));
+        for (int v = 0; v < 2; ++v)   // a peer copy between distinct devices
+            PSM_CUDA(c, cudaMemcpy2DAsync(s->stage_in[v], row, src[v], step[v], row, c->H, cudaMemcpyDefault, s->copy_stream));
+        PSM_CUDA(c, cudaEventRecord(c->ev_copied[k], s->copy_stream));
+        PSM_CUDA(c, cudaStreamWaitEvent(next_writer, c->ev_copied[k], 0));
+        PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_copied[k], 0));
+        rc = ingest<T>(s, static_cast<const T*>(s->stage_in[0]), row, static_cast<const T*>(s->stage_in[1]), row, true);
+        if (rc) return relay(c, k, rc);
+        PSM_CUDA(c, cudaEventRecord(s->ingest_done[0], s->stream));
+        s->ingest_done_valid[0] = true;
+        if ((rc = stage_end(s, 0))) return relay(c, k, rc);
+    }
+    return PSM_OK;
+}
+
 }  // namespace
 
 // ----------------------------------------------------------------------------------------------
@@ -760,9 +850,115 @@ int psm_create(psm_ctx** out, int width, int height, int max_disp, int device)
     return psm_create_sharded(out, width, height, max_disp, 0, max_disp, device);
 }
 
+static size_t p2p_keys_bytes(const psm_ctx* c, int nranks);   // the exchange block's layout (below)
+
+int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const int* devices, int n_devices, int block_slices,
+                     int map_bits)
+{
+    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
+    *out = nullptr;
+    if (map_bits != 8 && map_bits != 16) return fail(nullptr, PSM_EINVAL, "map_bits must be 8 or 16 (got %d)", map_bits);
+    const int dmax = map_bits == 8 ? MapFormat<uint8_t>::kMaxDisp : MapFormat<uint16_t>::kMaxDisp;
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > dmax)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d with %d-bit maps)", width, height,
+                    max_disp, dmax, map_bits);
+    if (n_devices < 1 || n_devices > kMaxRanks || n_devices > max_disp)
+        return fail(nullptr, PSM_EINVAL, "n_devices %d outside 1..%d (at most %d shards, each owning at least one of the %d slices)",
+                    n_devices, std::min(kMaxRanks, max_disp), kMaxRanks, max_disp);
+    if (!devices) return fail(nullptr, PSM_EINVAL, "devices is null");
+    if (block_slices < 0) return fail(nullptr, PSM_EINVAL, "block_slices %d is negative (0 = unblocked shards)", block_slices);
+    for (int k = 0; k < n_devices; ++k)
+        if (devices[k] < 0) return fail(nullptr, PSM_EINVAL, "devices[%d] = %d is negative", k, devices[k]);
+    const int ndev = psm_device_count();
+    for (int k = 0; k < n_devices; ++k)
+        if (devices[k] >= ndev)
+            return fail(nullptr, PSM_EINVAL, "devices[%d] = %d: CUDA device not available (%d devices)", k, devices[k], ndev);
+    // Shards on distinct devices store into each other's memory: every such pair needs peer access both ways.  Peer
+    // access is process-wide and another context may rely on it, so it is enabled here and never disabled.
+    for (int i = 0; i < n_devices; ++i)
+        for (int j = 0; j < n_devices; ++j) {
+            const int a = devices[i], b = devices[j];
+            if (a == b) continue;
+            int ok = 0;
+            cudaError_t e = cudaDeviceCanAccessPeer(&ok, a, b);
+            if (e != cudaSuccess) return fail(nullptr, PSM_ECUDA, "cudaDeviceCanAccessPeer(%d, %d) failed: %s", a, b, cudaGetErrorString(e));
+            if (!ok) return fail(nullptr, PSM_EINVAL, "device %d cannot access the memory of device %d (no peer access)", a, b);
+            if ((e = cudaSetDevice(a)) == cudaSuccess) e = cudaDeviceEnablePeerAccess(b, 0);
+            if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); e = cudaSuccess; }
+            if (e != cudaSuccess) return fail(nullptr, PSM_ECUDA, "enabling peer access %d -> %d failed: %s", a, b, cudaGetErrorString(e));
+        }
+    psm_ctx* c = new (std::nothrow) psm_ctx();
+    if (!c) return fail(nullptr, PSM_ENOMEM, "out of host memory");
+    c->W = width; c->H = height; c->Wp = pitch_for_width(width); c->D = max_disp;
+    c->d_begin = 0; c->d_count = max_disp; c->device = devices[0];
+    c->map_bytes = map_bits / 8;
+    auto bail = [&](int code) {
+        snprintf(g_create_error, sizeof(g_create_error), "%s", c->err);
+        psm_destroy(c);
+        return code;
+    };
+    // the split of sharding.py's shard_range: contiguous slices, the last shard takes the remainder
+    const int base = max_disp / n_devices;
+    for (int k = 0; k < n_devices; ++k) {
+        const int d_begin = k * base, d_count = k < n_devices - 1 ? base : max_disp - d_begin;
+        if (int rc = create_ctx(&c->shard[k], width, height, max_disp, d_begin, d_count, devices[k], c->map_bytes,
+                                block_slices ? std::min(block_slices, d_count) : 0)) {
+            snprintf(c->err, sizeof(c->err), "shard %d (device %d): %.400s", k, devices[k], g_create_error);
+            return bail(rc);
+        }
+        c->nshards = k + 1;
+        c->shard[k]->p2p_sync = 0;   // the shards' exchange kernels never spin on a flag: events order them
+    }
+    // every shard's exchange block, its peers' blocks as raw pointers (one process, no IPC), and the ordering events
+    void* blocks[kMaxRanks] = {};
+    for (int k = 0; k < n_devices; ++k) {
+        if (int rc = psm_p2p_create_buffer(c->shard[k], n_devices, &blocks[k])) {
+            const bool oom = cudaGetLastError() == cudaErrorMemoryAllocation;
+            relay(c, k, rc);
+            return bail(oom ? PSM_ENOMEM : rc);
+        }
+    }
+    for (int k = 0; k < n_devices; ++k) {
+        if (int rc = psm_p2p_set_peers(c->shard[k], blocks, n_devices, k)) { relay(c, k, rc); return bail(rc); }
+        cudaError_t e = cudaSetDevice(devices[k]);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_scattered[k], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_reduced[k], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied[k], cudaEventDisableTiming);
+        if (e == cudaSuccess && k == 0) e = cudaEventCreateWithFlags(&c->ev_images, cudaEventDisableTiming);
+        if (e != cudaSuccess) { fail(c, PSM_ECUDA, "event creation on device %d failed: %s", devices[k], cudaGetErrorString(e)); return bail(PSM_ECUDA); }
+    }
+    // the first shard's stream and complete maps stand for the context's (see is_multi)
+    psm_ctx* s0 = c->shard[0];
+    c->stream = s0->stream;
+    for (int v = 0; v < 2; ++v)
+        c->dis[v] = static_cast<uint8_t*>(blocks[0]) + p2p_keys_bytes(s0, n_devices) + (size_t)v * width * height * c->map_bytes;
+    *out = c;
+    return PSM_OK;
+}
+
 int psm_destroy(psm_ctx* c)
 {
     if (!c) return PSM_OK;
+    if (c->nshards) {
+        // every shard's work first: a shard's kernels store into the other shards' exchange blocks, and its copies read
+        // the first shard's staging set
+        for (int k = 0; k < c->nshards; ++k) {
+            cudaSetDevice(c->shard[k]->device);
+            cudaStreamSynchronize(c->shard[k]->stream);
+            cudaStreamSynchronize(c->shard[k]->copy_stream);
+        }
+        for (int k = 0; k < c->nshards; ++k) {
+            cudaSetDevice(c->shard[k]->device);
+            if (c->ev_scattered[k]) cudaEventDestroy(c->ev_scattered[k]);
+            if (c->ev_reduced[k]) cudaEventDestroy(c->ev_reduced[k]);
+            if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]);
+            if (k == 0 && c->ev_images) cudaEventDestroy(c->ev_images);
+            psm_destroy(c->shard[k]);
+        }
+        cudaGetLastError();
+        delete c;
+        return PSM_OK;
+    }
     cudaSetDevice(c->device);
     // every stream that may still run work on the buffers below: the caller's (psm_set_stream), the context's own one
     // (work enqueued before a psm_set_stream) and the copy stream
@@ -798,6 +994,11 @@ int psm_destroy(psm_ctx* c)
 int psm_set_option(psm_ctx* c, int key, int value)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) {
+        if (key == PSM_OPT_P2P_SYNC)
+            return reject_multi(c, "PSM_OPT_P2P_SYNC", "its shards' exchange is ordered by events, never by flags");
+        return forward(c, [&](psm_ctx* s) { return psm_set_option(s, key, value); });
+    }
     switch (key) {
     case PSM_OPT_CVF_MODE:
         if (value != PSM_CVF_EXACT && value != PSM_CVF_MIXED && value != PSM_CVF_NAIVE)
@@ -853,6 +1054,7 @@ int psm_set_option(psm_ctx* c, int key, int value)
 int psm_set_guided_filter(psm_ctx* c, int window, float eps)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_guided_filter(s, window, eps); });
     if (window < 1 || window > kWinMax) return fail(c, PSM_EINVAL, "guided-filter window %d outside 1..%d", window, kWinMax);
     if (!(eps > 0.0f) || !std::isfinite(eps)) return fail(c, PSM_EINVAL, "guided-filter eps %g is not a finite value > 0", (double)eps);
     if (window != c->gif_win || eps != c->gif_eps) c->guide_valid = false;   // mean_I, var_I and the solve depend on both
@@ -864,6 +1066,7 @@ int psm_set_guided_filter(psm_ctx* c, int window, float eps)
 int psm_set_matching_cost(psm_ctx* c, float alpha, float tau_color, float tau_grad)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_matching_cost(s, alpha, tau_color, tau_grad); });
     if (!(alpha >= 0.0f && alpha <= 1.0f)) return fail(c, PSM_EINVAL, "matching-cost alpha %g is not in [0, 1]", (double)alpha);
     if (!(tau_color >= 0.0f)) return fail(c, PSM_EINVAL, "colour threshold %g is not >= 0 or +inf", (double)tau_color);
     if (!(tau_grad >= 0.0f)) return fail(c, PSM_EINVAL, "gradient threshold %g is not >= 0 or +inf", (double)tau_grad);
@@ -874,6 +1077,7 @@ int psm_set_matching_cost(psm_ctx* c, float alpha, float tau_color, float tau_gr
 int psm_set_post_filter(psm_ctx* c, int radius, float sigma, int iterations, int weight_type)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_post_filter(s, radius, sigma, iterations, weight_type); });
     if (radius < 1 || radius > kPpParamMaxRadius) return fail(c, PSM_EINVAL, "post-filter radius %d outside 1..%d", radius, kPpParamMaxRadius);
     if (!(sigma >= 0x1p-16f && sigma <= 0x1p16f)) return fail(c, PSM_EINVAL, "post-filter sigma %g outside [2^-16, 2^16]", (double)sigma);
     if (iterations < 1 || iterations > 16) return fail(c, PSM_EINVAL, "post-filter iterations %d outside 1..16", iterations);
@@ -890,6 +1094,7 @@ int psm_set_post_filter(psm_ctx* c, int radius, float sigma, int iterations, int
 int psm_set_lr_check(psm_ctx* c, int mode)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_lr_check(s, mode); });
     if (mode != PSM_LR_OFF && mode != PSM_LR_FILL_WMF && mode != PSM_LR_FILL)
         return fail(c, PSM_EINVAL, "left-right check mode %d is not off (0), fill + post-filter (1) or fill (2)", mode);
     c->lr_mode = mode;
@@ -898,6 +1103,7 @@ int psm_set_lr_check(psm_ctx* c, int mode)
 
 int psm_set_stream(psm_ctx* c, void* cuda_stream)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_set_stream", "a stream belongs to one device, the context spans several");
     if (int rc = bind(c)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     c->stream = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : c->own_stream;
@@ -906,6 +1112,7 @@ int psm_set_stream(psm_ctx* c, void* cuda_stream)
 
 int psm_set_images(psm_ctx* c, const float* left, size_t left_step, const float* right, size_t right_step)
 {
+    if (is_multi(c)) return multi_set_images<float>(c, left, left_step, right, right_step, false);
     if (int rc = bind(c)) return rc;
     if (int rc = stage_begin(c, 0)) return rc;
     if (int rc = ingest<float>(c, left, left_step, right, right_step, false)) return rc;
@@ -914,6 +1121,7 @@ int psm_set_images(psm_ctx* c, const float* left, size_t left_step, const float*
 
 int psm_set_images_u8(psm_ctx* c, const uint8_t* left, size_t left_step, const uint8_t* right, size_t right_step)
 {
+    if (is_multi(c)) return multi_set_images<uint8_t>(c, left, left_step, right, right_step, false);
     if (int rc = bind(c)) return rc;
     if (int rc = stage_begin(c, 0)) return rc;
     if (int rc = ingest<uint8_t>(c, left, left_step, right, right_step, false)) return rc;
@@ -922,6 +1130,7 @@ int psm_set_images_u8(psm_ctx* c, const uint8_t* left, size_t left_step, const u
 
 int psm_set_images_device(psm_ctx* c, const float* d_left, size_t left_step, const float* d_right, size_t right_step)
 {
+    if (is_multi(c)) return multi_set_images<float>(c, d_left, left_step, d_right, right_step, true);
     if (int rc = bind(c)) return rc;
     if (int rc = stage_begin(c, 0)) return rc;
     if (int rc = ingest<float>(c, d_left, left_step, d_right, right_step, true)) return rc;
@@ -930,18 +1139,21 @@ int psm_set_images_device(psm_ctx* c, const float* d_left, size_t left_step, con
 
 int psm_set_images_async(psm_ctx* c, const float* left, size_t left_step, const float* right, size_t right_step)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_set_images_async", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
     if (int rc = bind(c)) return rc;
     return upload_async<float>(c, left, left_step, right, right_step);
 }
 
 int psm_set_images_u8_async(psm_ctx* c, const uint8_t* left, size_t left_step, const uint8_t* right, size_t right_step)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_set_images_u8_async", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
     if (int rc = bind(c)) return rc;
     return upload_async<uint8_t>(c, left, left_step, right, right_step);
 }
 
 int psm_set_images_commit(psm_ctx* c)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_set_images_commit", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
     if (int rc = bind(c)) return rc;
     if (!c->up_pending) return fail(c, PSM_ESTATE, "psm_set_images_commit without a pending psm_set_images_async");
     const int set = c->stage_cur ^ 1;
@@ -967,6 +1179,7 @@ int psm_set_images_commit(psm_ctx* c)
 
 int psm_cost_const(psm_ctx* c)
 {
+    if (is_multi(c)) return forward(c, [](psm_ctx* s) { return psm_cost_const(s); });
     if (int rc = bind(c)) return rc;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_cost_const before psm_set_images");
     if (int rc = stage_begin(c, 1)) return rc;
@@ -986,6 +1199,7 @@ int psm_cost_const(psm_ctx* c)
 
 int psm_cost_filter(psm_ctx* c)
 {
+    if (is_multi(c)) return forward(c, [](psm_ctx* s) { return psm_cost_filter(s); });
     if (int rc = bind(c)) return rc;
     if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter before psm_cost_const");
     if (!c->gif_default() && c->cvf_mode != PSM_CVF_EXACT)
@@ -1025,6 +1239,7 @@ int psm_cost_filter(psm_ctx* c)
 // DispEst::CostFilter_FGF (reference src/DispEst.cpp:281-296): Fast Guided Filter with sub-sampling rate s
 int psm_cost_filter_fgf(psm_ctx* c, int s)
 {
+    if (is_multi(c)) return forward(c, [s](psm_ctx* sh) { return psm_cost_filter_fgf(sh, s); });
     if (int rc = bind(c)) return rc;
     if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter_fgf before psm_cost_const");
     if (s != 1 && s != 2 && s != 4 && s != 8) return fail(c, PSM_EINVAL, "sub-sampling rate must be 1, 2, 4 or 8 (got %d)", s);
@@ -1153,6 +1368,7 @@ template <typename T>
 static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const uint64_t* d_gathered_right, int nranks,
                             T* left, size_t left_step, T* right, size_t right_step)
 {
+    if (is_multi(c)) return reject_multi(c, sizeof(T) == 1 ? "psm_disp_reduce_keys" : "psm_disp_reduce_keys_u16", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = check_map_format<T>(c, "psm_disp_reduce_keys", "psm_disp_reduce_keys_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
@@ -1175,8 +1391,11 @@ static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const u
 
 extern "C" {
 
+static int multi_select(psm_ctx* c);   // below
+
 int psm_disp_select_device(psm_ctx* c)
 {
+    if (is_multi(c)) return multi_select(c);
     if (int rc = bind(c)) return rc;
     if (c->d_begin != 0 || c->d_count != c->D)
         return fail(c, PSM_ESTATE, "psm_disp_select on a sharded context: use psm_disp_select_keys + psm_disp_reduce_keys");
@@ -1210,6 +1429,7 @@ int psm_disp_select_u16_async(psm_ctx* c, uint16_t* left, size_t left_step, uint
 
 int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_right)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_disp_select_keys", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (!d_keys_left || !d_keys_right) return fail(c, PSM_EINVAL, "null key buffer");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
@@ -1251,6 +1471,7 @@ static size_t p2p_flags_bytes() { return (size_t)2 * 2 * kMaxRanks * sizeof(unsi
 
 int psm_p2p_create_buffer(psm_ctx* c, int nranks, void** d_buffer)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_p2p_create_buffer", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (nranks < 1 || nranks > kMaxRanks || !d_buffer) return fail(c, PSM_EINVAL, "bad nranks %d (1..%d)", nranks, kMaxRanks);
     if (c->p2p_own) { cudaFree(c->p2p_own); c->p2p_own = nullptr; }
@@ -1273,6 +1494,7 @@ int psm_p2p_create_buffer(psm_ctx* c, int nranks, void** d_buffer)
 
 int psm_ipc_export(psm_ctx* c, void* d_ptr, unsigned char handle_out[64])
 {
+    if (is_multi(c)) return reject_multi(c, "psm_ipc_export", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     cudaIpcMemHandle_t h;
@@ -1283,6 +1505,7 @@ int psm_ipc_export(psm_ctx* c, void* d_ptr, unsigned char handle_out[64])
 
 int psm_ipc_import(psm_ctx* c, const unsigned char handle[64], void** d_ptr)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_ipc_import", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (c->p2p_nimported >= kMaxRanks) return fail(c, PSM_EINVAL, "too many imported buffers");
     cudaIpcMemHandle_t h;
@@ -1294,6 +1517,7 @@ int psm_ipc_import(psm_ctx* c, const unsigned char handle[64], void** d_ptr)
 
 int psm_p2p_set_peers(psm_ctx* c, void* const* d_buffers, int nranks, int rank)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_p2p_set_peers", "the context already spans the whole disparity range; use psm_disp_select*");
     if (!c || !d_buffers) return fail(c, PSM_EINVAL, "null argument");
     if (nranks != c->p2p_nranks || rank < 0 || rank >= nranks) return fail(c, PSM_EINVAL, "bad peers (nranks %d, rank %d)", nranks, rank);
     for (int r = 0; r < nranks; ++r) {
@@ -1320,8 +1544,28 @@ static void p2p_fill(const psm_ctx* c, int view, P2pPeers& peers)
     }
 }
 
+// the scatter of the fused exchange over this context's slices: wta_scatter_kernel over the filtered volumes, or, for a
+// blocked shard of a multi-device context, keys_scatter_kernel over its running keys
+static int p2p_scatter(psm_ctx* c)
+{
+    c->p2p_seq++;   // one sequence number per frame, identical on every rank (all ranks run the same frames)
+    c->lr_masks_ok = false;
+    for (int v = 0; v < 2; ++v) {
+        P2pPeers peers;
+        p2p_fill(c, v, peers);
+        dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, (c->H + kScatterRows - 1) / kScatterRows);
+        if (c->blk_slices)
+            keys_scatter_kernel<<<grd, blk, 0, c->stream>>>(c->run_keys[v], c->W, c->H, peers);
+        else
+            wta_scatter_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, peers);
+        PSM_LAUNCH_CHECK(c);
+    }
+    return PSM_OK;
+}
+
 int psm_disp_select_keys_p2p(psm_ctx* c)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_disp_select_keys_p2p", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (c->blk_slices)
         return fail(c, PSM_EINVAL, "psm_disp_select_keys_p2p on a blocked context: the fused exchange scans whole volumes, a "
@@ -1329,20 +1573,13 @@ int psm_disp_select_keys_p2p(psm_ctx* c)
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "psm_p2p_create_buffer / psm_p2p_set_peers first");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys_p2p before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
-    c->p2p_seq++;   // one sequence number per frame, identical on every rank (all ranks run the same frames)
-    c->lr_masks_ok = false;
-    for (int v = 0; v < 2; ++v) {
-        P2pPeers peers;
-        p2p_fill(c, v, peers);
-        dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, (c->H + kScatterRows - 1) / kScatterRows);
-        wta_scatter_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, peers);
-        PSM_LAUNCH_CHECK(c);
-    }
+    if (int rc = p2p_scatter(c)) return rc;
     return stage_end(c, 3);
 }
 
 int psm_disp_reduce_p2p(psm_ctx* c)
 {
+    if (is_multi(c)) return reject_multi(c, "psm_disp_reduce_p2p", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "no exchange block");
     const unsigned npix = (unsigned)((size_t)c->W * c->H);
@@ -1370,11 +1607,53 @@ static int p2p_wait_done(psm_ctx* c)
     return PSM_OK;
 }
 
+// Selection on a multi-device context: the fused exchange's two kernels on every shard, which never wait on a flag
+// (PSM_OPT_P2P_SYNC = 0), ordered by events across the shards' streams instead.  The hazards, for frame f:
+//   1. every shard's scatter overwrites key slots that every shard's reduce of frame f - 1 read: it waits for them;
+//   2. every shard's reduce reads the slots of every shard's scatter of frame f: it waits for them;
+//   3. whatever reads the first shard's complete maps after the select (D2H, post-filter, left-right check, psm_sync in
+//      front of a psm_device_ptr user) runs on the first shard's stream, which waits for every shard's reduce;
+//   4. every reduce writes the first shard's maps, which what the first shard enqueued before this select (a previous
+//      post-filter, an asynchronous D2H) may still read: the wait of 2 on the first shard's scatter, queued behind
+//      that work, covers it.
+// No kernel waits for another queued behind it, so shards on one device are as safe as shards on several.
+static int multi_select(psm_ctx* c)
+{
+    const int n = c->nshards;
+    for (int k = 0; k < n; ++k)
+        if (!c->shard[k]->filtered) return fail(c, PSM_ESTATE, "psm_disp_select before psm_cost_filter (shard %d)", k);
+    for (int k = 0; k < n; ++k) {
+        psm_ctx* s = c->shard[k];
+        if (int rc = bind(s)) return relay(c, k, rc);
+        if (c->reduced_valid)
+            for (int j = 0; j < n; ++j)
+                if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_reduced[j], 0));   // 1
+        if (k == 0)
+            if (int rc = stage_begin(s, 3)) return relay(c, k, rc);
+        if (int rc = p2p_scatter(s)) return relay(c, k, rc);
+        PSM_CUDA(c, cudaEventRecord(c->ev_scattered[k], s->stream));
+    }
+    for (int k = 0; k < n; ++k) {
+        psm_ctx* s = c->shard[k];
+        if (int rc = bind(s)) return relay(c, k, rc);
+        for (int j = 0; j < n; ++j)
+            if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_scattered[j], 0));   // 2, and 4
+        if (int rc = psm_disp_reduce_p2p(s)) return relay(c, k, rc);
+        PSM_CUDA(c, cudaEventRecord(c->ev_reduced[k], s->stream));
+    }
+    c->reduced_valid = true;
+    psm_ctx* s0 = c->shard[0];
+    if (int rc = bind(s0)) return relay(c, 0, rc);
+    for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_reduced[j], 0));   // 3
+    return relay(c, 0, stage_end(s0, 3));
+}
+
 }  // extern "C"
 
 template <typename T>
 static int disp_fetch_p2p(psm_ctx* c, T* left, size_t left_step, T* right, size_t right_step)
 {
+    if (is_multi(c)) return reject_multi(c, sizeof(T) == 1 ? "psm_disp_fetch_p2p" : "psm_disp_fetch_p2p_u16", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = check_map_format<T>(c, "psm_disp_fetch_p2p", "psm_disp_fetch_p2p_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
@@ -1529,6 +1808,12 @@ extern "C" {
 
 int psm_post_process_device(psm_ctx* c)
 {
+    if (is_multi(c)) {   // on the first shard, which holds the complete maps; its outputs stand for the context's
+        psm_ctx* s0 = c->shard[0];
+        if (int rc = psm_post_process_device(s0)) return relay(c, 0, rc);
+        for (int v = 0; v < 2; ++v) { c->dis_pp[v] = s0->dis_pp[v]; c->lr_valid[v] = s0->lr_valid[v]; }
+        return PSM_OK;
+    }
     if (int rc = bind(c)) return rc;
     return c->map_bytes == 2 ? post_process_maps<uint16_t>(c) : post_process_maps<uint8_t>(c);
 }
@@ -1554,11 +1839,25 @@ static int check_slice(psm_ctx* c, int view, int d)
     return PSM_OK;
 }
 
+}  // extern "C"
+
+// a per-slice call on a multi-device context: routed to the shard that owns global slice d
+template <class F>
+static int route_slice(psm_ctx* c, int d, F f)
+{
+    for (int k = 0; k < c->nshards; ++k)
+        if (d >= c->shard[k]->d_begin && d < c->shard[k]->d_begin + c->shard[k]->d_count) return relay(c, k, f(c->shard[k]));
+    return fail(c, PSM_EINVAL, "slice %d outside [0,%d)", d, c->D);
+}
+
+extern "C" {
+
 // the offset of a checked slice in the volumes
 static size_t slice_offset(const psm_ctx* c, int d) { return (size_t)(d - (c->blk_slices ? c->res_begin : c->d_begin)) * c->plane; }
 
 int psm_read_cost_slice(psm_ctx* c, int view, int d, float* dst, size_t dst_step)
 {
+    if (is_multi(c)) return route_slice(c, d, [&](psm_ctx* s) { return psm_read_cost_slice(s, view, d, dst, dst_step); });
     if (int rc = bind(c)) return rc;
     if (int rc = check_slice(c, view, d)) return rc;
     if (!dst || dst_step < (size_t)c->W * sizeof(float)) return fail(c, PSM_EINVAL, "bad dst/step");
@@ -1570,6 +1869,7 @@ int psm_read_cost_slice(psm_ctx* c, int view, int d, float* dst, size_t dst_step
 
 int psm_write_cost_slice(psm_ctx* c, int view, int d, const float* src, size_t src_step)
 {
+    if (is_multi(c)) return route_slice(c, d, [&](psm_ctx* s) { return psm_write_cost_slice(s, view, d, src, src_step); });
     if (int rc = bind(c)) return rc;
     if (c->blk_slices)
         return fail(c, PSM_EINVAL, "psm_write_cost_slice on a blocked context: the filter stages rebuild every block after the "
@@ -1600,6 +1900,7 @@ int psm_write_cost_slice(psm_ctx* c, int view, int d, const float* src, size_t s
 
 int psm_read_guide_plane(psm_ctx* c, int view, int plane_id, float* dst, size_t dst_step)
 {
+    if (is_multi(c)) return relay(c, 0, psm_read_guide_plane(c->shard[0], view, plane_id, dst, dst_step));
     if (int rc = bind(c)) return rc;
     if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
     if (!c->have_images) return fail(c, PSM_ESTATE, "no images set");
@@ -1620,6 +1921,7 @@ int psm_read_guide_plane(psm_ctx* c, int view, int plane_id, float* dst, size_t 
 
 int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
 {
+    if (is_multi(c)) return route_slice(c, d, [&](psm_ctx* s) { return psm_read_ab_slice(s, view, d, a3, b); });
     if (int rc = bind(c)) return rc;
     if (int rc = check_slice(c, view, d)) return rc;
     if (!a3 || !b) return fail(c, PSM_EINVAL, "null output");
@@ -1644,6 +1946,8 @@ int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
 int psm_device_ptr(psm_ctx* c, int what, void** ptr, size_t* pitch_elems)
 {
     if (!c || !ptr) return fail(c, PSM_EINVAL, "null argument");
+    if (c->nshards && (what == 0 || what == 1))
+        return reject_multi(c, "psm_device_ptr selectors 0 / 1", "the volumes are split across the shards");
     switch (what) {
     case 0: case 1: *ptr = c->vol[what]; if (pitch_elems) *pitch_elems = c->Wp; return PSM_OK;
     case 2: case 3: *ptr = c->dis[what - 2]; if (pitch_elems) *pitch_elems = c->W; return PSM_OK;
@@ -1655,6 +1959,7 @@ int psm_device_ptr(psm_ctx* c, int what, void** ptr, size_t* pitch_elems)
 
 int psm_read_valid_mask(psm_ctx* c, int view, uint8_t* dst, size_t dst_step)
 {
+    if (is_multi(c)) return relay(c, 0, psm_read_valid_mask(c->shard[0], view, dst, dst_step));
     if (int rc = bind(c)) return rc;
     if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
     if (!dst || dst_step < (size_t)c->W) return fail(c, PSM_EINVAL, "bad dst/step");
@@ -1667,6 +1972,18 @@ int psm_read_valid_mask(psm_ctx* c, int view, uint8_t* dst, size_t dst_step)
 
 int psm_stage_ms(psm_ctx* c, int stage, float* ms)
 {
+    if (is_multi(c)) {
+        // stages 3 (timed across the shards) and 5 (the post-process) run on the first shard; the others are the
+        // longest of the shards' own times
+        if (stage == 3 || stage == 5) return relay(c, 0, psm_stage_ms(c->shard[0], stage, ms));
+        float worst = 0.0f, t = 0.0f;
+        for (int k = 0; k < c->nshards; ++k) {
+            if (int rc = psm_stage_ms(c->shard[k], stage, &t)) return relay(c, k, rc);
+            worst = std::max(worst, t);
+        }
+        *ms = worst;
+        return PSM_OK;
+    }
     if (int rc = bind(c)) return rc;
     if (stage < 0 || stage >= kNumStages || !ms) return fail(c, PSM_EINVAL, "bad stage %d", stage);
     if (!c->ev_valid[stage]) return fail(c, PSM_ESTATE, "stage %d has not been timed", stage);
@@ -1679,11 +1996,13 @@ int psm_launch_count(psm_ctx* c, uint64_t* n)
 {
     if (!c || !n) return fail(c, PSM_EINVAL, "null argument");
     *n = c->launches;
+    for (int k = 0; k < c->nshards; ++k) *n += c->shard[k]->launches;
     return PSM_OK;
 }
 
 int psm_sync(psm_ctx* c)
 {
+    if (is_multi(c)) return forward(c, [](psm_ctx* s) { return psm_sync(s); });
     if (int rc = bind(c)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;

@@ -624,6 +624,8 @@ __global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
 //                        the min over the nranks slots of its chunk, stores the winning disparity (u8 or u16)
 //                        into EVERY rank's result map -- reduce + gather in one kernel -- and its last CTA
 //                        raises this rank's DONE flag in every peer's block;
+//   keys_scatter_kernel: the scatter of a blocked shard of a multi-device context, whose minima are already folded
+//                        into its running keys; same staged store (p2p_store_row) and ARRIVE flag as wta_scatter_kernel;
 //   p2p_wait_done_kernel: spins until all ranks' DONE flags carry this frame's sequence number; after it the local result
 //                        maps are complete.  Launched only in front of a consumer of the maps (D2H fetch, post-filter);
 //                        the NEXT frame's scatter kernel does the same wait itself before it overwrites the key slots.
@@ -668,10 +670,51 @@ __device__ __forceinline__ void p2p_publish(const P2pPeers& peers, int flag_offs
     }
 }
 
+// called by every thread of a scatter kernel before its peer stores: the key slots it writes were read by the reducers
+// of the PREVIOUS frame, so wait for their DONE flags
+__device__ __forceinline__ void p2p_wait_reducers(const P2pPeers& peers)
+{
+    if (peers.seq > 1) {
+        if (threadIdx.x < (unsigned)peers.nranks) {
+            const unsigned* f = peers.flags[peers.rank] + kMaxRanks + threadIdx.x;
+            while ((int)(ld_acquire_sys(f) - (peers.seq - 1)) < 0) __nanosleep(64);
+        }
+        __syncthreads();
+    }
+}
+
+// The scatter kernels' store of one row: lane `lane` holds the keys key(0..3) of columns x4 .. x4 + 3, x4 = xw + 4 * lane,
+// and every pixel's key goes to slot [this rank][pixel-in-chunk] of its reducer's exchange block (peer or own memory).
+// The warp's 128 keys are staged in `stage` (128 shared slots of the warp) and sent out lane-contiguously: every store
+// instruction then writes 32 consecutive keys (256 contiguous bytes, whole 32-byte sectors) to one peer, instead of
+// 32 lanes x 8 bytes at a 32-byte stride (partial sectors over NVLink).  Every lane of the warp takes part, also those
+// whose columns lie past the image.
+template <class Key>
+__device__ __forceinline__ void p2p_store_row(unsigned long long* stage, const P2pPeers& peers, int W, int y, int xw, int lane,
+                                              Key key)
+{
+    __syncwarp();   // the previous row's staged keys have been sent
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+        stage[4 * lane + j] = key(j);
+    __syncwarp();
+#pragma unroll
+    for (int s4 = 0; s4 < 4; ++s4) {
+        const int idx = 32 * s4 + lane;
+        const int x = xw + idx;
+        if (x < W) {
+            const unsigned pix = (unsigned)y * (unsigned)W + (unsigned)x;
+            const unsigned owner = pix / peers.chunk;
+            peers.keys[owner][(size_t)peers.rank * peers.chunk + (pix - owner * peers.chunk)] = stage[idx];
+        }
+    }
+}
+
 __global__ void __launch_bounds__(256) wta_scatter_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin, int d_count,
                                                           P2pPeers peers)
 {
-    if (peers.seq > 1) {   // the key slots written below were read by the reducers of the PREVIOUS frame: wait for their DONE flags
+    // p2p_wait_reducers, spelled out: the call schedules this kernel's instructions differently
+    if (peers.seq > 1) {
         if (threadIdx.x < (unsigned)peers.nranks) {
             const unsigned* f = peers.flags[peers.rank] + kMaxRanks + threadIdx.x;
             while ((int)(ld_acquire_sys(f) - (peers.seq - 1)) < 0) __nanosleep(64);
@@ -681,9 +724,6 @@ __global__ void __launch_bounds__(256) wta_scatter_kernel(const float* __restric
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const bool active = x4 < W;  // inactive lanes still take part in the staged store below
     const size_t plane = (size_t)H * Wp;
-    // Stage the warp's 128 keys in shared memory and send them out lane-contiguously: every store
-    // instruction then writes 32 consecutive keys (256 contiguous bytes, whole 32-byte sectors) to
-    // one peer, instead of 32 lanes x 8 bytes at a 32-byte stride (partial sectors over NVLink).
     __shared__ unsigned long long stage[8][128];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // a CTA handles kScatterRows consecutive rows: four times fewer CTAs have to fence and count in p2p_publish
@@ -701,22 +741,26 @@ __global__ void __launch_bounds__(256) wta_scatter_kernel(const float* __restric
             if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
             if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
         }
-        __syncwarp();   // the previous row's staged keys have been sent
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-            stage[warp][4 * lane + j] = ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j];
-        __syncwarp();
-        const int xw = x4 - 4 * lane;  // first column of this warp
-#pragma unroll
-        for (int s4 = 0; s4 < 4; ++s4) {
-            const int idx = 32 * s4 + lane;
-            const int x = xw + idx;
-            if (x < W) {
-                const unsigned pix = (unsigned)y * (unsigned)W + (unsigned)x;
-                const unsigned owner = pix / peers.chunk;
-                peers.keys[owner][(size_t)peers.rank * peers.chunk + (pix - owner * peers.chunk)] = stage[warp][idx];  // peer (or own) memory
-            }
-        }
+        p2p_store_row(stage[warp], peers, W, y, x4 - 4 * lane, lane,
+                      [&](int j) { return ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j]; });
+    }
+    if (peers.seq) p2p_publish(peers, 0);   // ARRIVE
+}
+
+// The scatter of a blocked shard of a multi-device context (psm_create_multi): its selection is already folded into the
+// running keys (wta_fold_kernel), so each pixel's running key goes to its reducer's slot, with wta_scatter_kernel's
+// grid, staged store and ARRIVE flag.
+__global__ void __launch_bounds__(256) keys_scatter_kernel(const unsigned long long* __restrict__ keys /* [H][W] */, int W, int H,
+                                                           P2pPeers peers)
+{
+    p2p_wait_reducers(peers);
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    __shared__ unsigned long long stage[8][128];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int y = blockIdx.y * kScatterRows; y < min(H, (int)(blockIdx.y + 1) * kScatterRows); ++y) {
+        const unsigned long long* k = keys + (size_t)y * W + x4;
+        p2p_store_row(stage[warp], peers, W, y, x4 - 4 * lane, lane,
+                      [&](int j) { return x4 + j < W ? __ldg(k + j) : 0ull; });
     }
     if (peers.seq) p2p_publish(peers, 0);   // ARRIVE
 }

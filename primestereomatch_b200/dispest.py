@@ -39,10 +39,13 @@ class DispEst:
     block_slices : None (the volumes hold every owned slice) or the number of slices a blocked context
     (psm_create_blocked) holds at once: the filter stages walk the owned range in blocks of that many, so device memory
     depends on it instead of on d.  The maps are the same either way; read_cost_volume is not available.
+    devices : None (one device, `device`) or a list of CUDA device ids: a multi-device context (psm_create_multi) whose
+    shard k runs on devices[k] and owns the k-th contiguous part of [0, d); ids may repeat.  The maps equal a
+    single-device context's.  Not combinable with d_begin / d_count; block_slices blocks every shard.
     """
 
     def __init__(self, l, r, d, t=MAX_CPU_THREADS, ocl=True, device=0, d_begin=0, d_count=None, map_bits=None,
-                 block_slices=None):
+                 block_slices=None, devices=None):
         l, r = np.asarray(l), np.asarray(r)
         if l.dtype != r.dtype or l.shape != r.shape:
             # reference: "DE: Error - Left & Right images are of different types." then exit(1)
@@ -63,6 +66,8 @@ class DispEst:
         self.lValid = np.zeros((self.hei, self.wid), np.uint8)  # DispEst.cpp:48-49
         self.rValid = np.zeros((self.hei, self.wid), np.uint8)
         self.lr_mode = capi.PSM_LR_OFF
+        if devices is not None and (d_begin != 0 or d_count is not None):
+            raise ValueError("devices (a multi-device context over the whole range) excludes d_begin / d_count")
         self._lImg, self._rImg = l, r
         self._ctx = C.c_void_p()
         self._lib = None
@@ -70,14 +75,20 @@ class DispEst:
             L = capi.lib()
             self._lib = L
             dc = self.maxDis - d_begin if d_count is None else d_count
-            if block_slices is not None:
+            if devices is not None:
+                devs = [int(x) for x in devices]
+                arr = (C.c_int * max(1, len(devs)))(*devs)
+                capi.check(L.psm_create_multi(C.byref(self._ctx), self.wid, self.hei, self.maxDis, arr, len(devs),
+                                              int(block_slices or 0), self.map_bits))
+            elif block_slices is not None:
                 capi.check(L.psm_create_blocked(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc),
                                                 int(block_slices), self.map_bits, int(device)))
             else:
                 create = L.psm_create_u16 if self.map_bits == 16 else L.psm_create_sharded
                 capi.check(create(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc), int(device)))
         self.d_begin, self.d_count = d_begin, (self.maxDis - d_begin if d_count is None else d_count)
-        self.block_slices = block_slices
+        self.block_slices = None if devices is not None and not block_slices else block_slices   # 0: unblocked shards
+        self.devices = None if devices is None else list(devices)
 
     # -- lifetime ---------------------------------------------------------------------------
     def close(self):

@@ -5,7 +5,7 @@
 
 // reference src/DispEst.cpp:10-143: type check (exit(1) on mismatch), output maps, and -- instead of
 // the OpenCL context / queue / 12 cl_mem buffers / three run-time compiled programs -- one psm_ctx.
-DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices)
+DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices, std::vector<int> devices)
     : lImg(l), rImg(r), maxDis(d), threads(t), useOCL(ocl)
 {
     hei = lImg.rows;
@@ -21,8 +21,12 @@ DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_s
     lValid = cv::Mat::zeros(hei, wid, CV_8UC1);   // DispEst.cpp:48-49
     rValid = cv::Mat::zeros(hei, wid, CV_8UC1);
     if (useOCL) {
-        const int rc = block_slices > 0 ? psm_create_blocked(&ctx, wid, hei, maxDis, 0, maxDis, block_slices, wide ? 16 : 8, 0)
-                     : wide ? psm_create_u16(&ctx, wid, hei, maxDis, 0, maxDis, 0) : psm_create(&ctx, wid, hei, maxDis, 0);
+        const int dev = devices.empty() ? 0 : devices[0];
+        const int rc = devices.size() >= 2
+                           ? psm_create_multi(&ctx, wid, hei, maxDis, devices.data(), (int)devices.size(), block_slices > 0 ? block_slices : 0,
+                                              wide ? 16 : 8)
+                     : block_slices > 0 ? psm_create_blocked(&ctx, wid, hei, maxDis, 0, maxDis, block_slices, wide ? 16 : 8, dev)
+                     : wide ? psm_create_u16(&ctx, wid, hei, maxDis, 0, maxDis, dev) : psm_create(&ctx, wid, hei, maxDis, dev);
         if (rc != PSM_OK) {
             // reference logs OpenCL set-up failures and carries on (DispEst.cpp:69-79); so do we, with
             // the GPU stages then returning an error code instead of computing anything on the CPU

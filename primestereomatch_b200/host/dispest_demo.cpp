@@ -8,7 +8,8 @@
 // iterations and weight (exp, iv1, iv2 or off) to setPostFilter (default: 9 25.5 1 exp), the optional left-right check
 // mode (0 off, 1 check + fill + post-filter, 2 check + fill) to setLRCheck (default 0).  D up to 4096: above 256 the
 // maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.  A leading
-// `--block-slices N` runs a blocked context (psm_create_blocked) that holds N disparity slices at a time.
+// `--block-slices N` runs a blocked context (psm_create_blocked) that holds N disparity slices at a time, a leading
+// `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -28,14 +29,24 @@ static bool read_all(const char* path, void* dst, size_t n)
 int main(int argc, char** argv)
 {
     int block_slices = 0;
-    if (argc >= 3 && !std::strcmp(argv[1], "--block-slices")) {
-        block_slices = std::atoi(argv[2]);
+    std::vector<int> devices;
+    while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices"))) {
+        if (!std::strcmp(argv[1], "--block-slices")) {
+            block_slices = std::atoi(argv[2]);
+        } else {
+            for (const char* p = argv[2]; *p;) {
+                char* end = nullptr;
+                devices.push_back((int)std::strtol(p, &end, 10));
+                if (end == p) { std::fprintf(stderr, "bad device list %s\n", argv[2]); return 2; }
+                p = *end == ',' ? end + 1 : end;
+            }
+        }
         argv[2] = argv[0];
         argv += 2;
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--block-slices N] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--block-slices N] [--devices i,j,...] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -43,7 +54,7 @@ int main(int argc, char** argv)
     if (b200devicepoll() == 0) { std::fprintf(stderr, "no CUDA device\n"); return 3; }
     cv::Mat l(H, W, CV_32FC3), r(H, W, CV_32FC3);
     if (!read_all(argv[4], l.data, l.step * H) || !read_all(argv[5], r.data, r.step * H)) { std::fprintf(stderr, "bad input\n"); return 2; }
-    DispEst* SMDE = new DispEst(l, r, D, MAX_CPU_THREADS, true, block_slices);
+    DispEst* SMDE = new DispEst(l, r, D, MAX_CPU_THREADS, true, block_slices, devices);
     SMDE->setInputImages(l, r);
     SMDE->setThreads(MAX_CPU_THREADS);
     SMDE->setSubsampleRate(4);
