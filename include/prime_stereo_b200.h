@@ -84,13 +84,39 @@ enum {
     PSM_OPT_GRAY_MODE = 2, /* 0: fma(c2,.114,fma(c0,.299,c1*.587)) (OpenCV SIMD/IPP builds, default)
                               1: (c0*.299+c1*.587)+c2*.114 (non-FMA OpenCV builds) */
     PSM_OPT_TIMING = 3,    /* 1: record cudaEvents around each stage (default 1) */
-    PSM_OPT_P2P_SYNC = 4   /* fused multi-GPU exchange: 1 (default) = the kernels synchronise across ranks by
+    PSM_OPT_P2P_SYNC = 4,  /* fused multi-GPU exchange: 1 (default) = the kernels synchronise across ranks by
                               device-side flags in the exchange blocks (no library collective, no host barrier);
                               0 = the caller separates select / reduce / fetch by its own cross-rank barriers */
+    PSM_OPT_VIEWS = 5      /* PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT: which disparity maps a frame computes; see
+                              "Left-only frames" below */
     /* keys 100..106 are kernel tuning knobs used by bench.py experiments (variant, rows per segment, extra
        shared memory, threads per CTA, block remap, packed remainder strips off, CVC build); they never
        change results */
 };
+/* Values of PSM_OPT_VIEWS */
+enum { PSM_VIEWS_LEFT = 1, PSM_VIEWS_BOTH = 2 };
+
+/* Left-only frames (PSM_OPT_VIEWS = PSM_VIEWS_LEFT), for callers that consume the left map alone: about half of a
+ * frame's device work computes the right view, which only the right map and the left-right check use.
+ *   - Any value other than PSM_VIEWS_LEFT / PSM_VIEWS_BOTH returns PSM_EINVAL and changes nothing.  Changing the value
+ *     keeps the current images and resets the frame's stages: the next stage must be psm_cost_const (every other stage
+ *     returns PSM_ESTATE until then), and the earlier maps, masks, volumes and right-view guide are stale.
+ *   - Ingest (psm_set_images*) is unchanged: both images are uploaded and ingested, because the left costs read the
+ *     right image and its gradient (the right view's ingest planes 0-2 and 12 stay readable).
+ *   - psm_cost_const builds the left raw volume; psm_cost_filter / psm_cost_filter_fgf compute the left guide and
+ *     filter the left volume (every mode, window and rate; blocked contexts fold the left running keys only).
+ *   - Selection writes the left map (and the left keys) only.  The right map pointer of psm_disp_select*,
+ *     psm_disp_fetch_p2p* and psm_post_process* and the right key / gathered-key pointers of psm_disp_select_keys and
+ *     psm_disp_reduce_keys* must be NULL: a non-NULL one returns PSM_EINVAL.  The fused exchange moves and reduces the
+ *     left keys only; every rank must use the same setting.  Multi-device contexts forward the option to every shard.
+ *   - psm_post_process* filters the left map only.  With a left-right check mode (psm_set_lr_check 1 or 2) it returns
+ *     PSM_ESTATE: the check needs both maps.  psm_set_lr_check itself may be called at any time.
+ *   - PSM_ESTATE: psm_read_cost_slice, psm_read_ab_slice and psm_read_guide_plane planes 3-11 of the right view, and
+ *     psm_read_valid_mask.
+ *   - Nothing else is written: the right volume, the right map, the right post-filtered map and the right mask keep
+ *     their contents.  psm_device_ptr returns the same addresses, and no device memory is freed or allocated.
+ *     psm_stage_ms reports the left view's work, psm_launch_count the kernels that ran. */
+
 enum {
     PSM_CVF_EXACT = 0, /* streaming fused kernel, every box sum accumulated in fp64: bit-exact q */
     PSM_CVF_MIXED = 1, /* the tolerance mode north_star allows for fp32: first box stage fp64 (a, b bit-exact), second

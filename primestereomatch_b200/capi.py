@@ -28,6 +28,8 @@ SYMBOLS = [
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
 PSM_LEFT, PSM_RIGHT = 0, 1
 PSM_OPT_CVF_MODE, PSM_OPT_GRAY_MODE, PSM_OPT_TIMING, PSM_OPT_P2P_SYNC, PSM_OPT_VARIANT = 1, 2, 3, 4, 100
+PSM_OPT_VIEWS = 5
+PSM_VIEWS_LEFT, PSM_VIEWS_BOTH = 1, 2
 PSM_CVF_EXACT, PSM_CVF_MIXED, PSM_CVF_NAIVE = 0, 1, 2
 PSM_WMF_EXP, PSM_WMF_IV1, PSM_WMF_IV2, PSM_WMF_OFF = 0, 1, 2, 5
 PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL = 0, 1, 2

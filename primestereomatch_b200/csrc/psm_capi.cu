@@ -110,6 +110,12 @@ struct psm_ctx {
     bool reduced_valid = false;
     cudaEvent_t ev_copied[kMaxRanks] = {};     // shard k (k >= 1) has read the frame it receives from the first shard
     cudaEvent_t ev_images = nullptr;           // psm_set_images_device: the caller's images as the first shard's stream sees them
+    // PSM_OPT_VIEWS: 2 (both views) or 1 (the left view alone: the right view's guide, volume, selection and post-filter
+    // are skipped).  views_reset: the value changed since the last psm_cost_const, so the volumes, maps and masks are stale.
+    int views = 2;
+    bool views_reset = false;
+    unsigned p2p_seq_right = 0;                // frames whose exchange included the right view (p2p_seq counts every frame)
+    bool p2p_right_current = false;            // the last frame's exchange included the right view
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -155,6 +161,35 @@ int bind(psm_ctx* c)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
     PSM_CUDA(c, cudaSetDevice(c->device));
+    return PSM_OK;
+}
+
+// a call that would read or return right-view data: PSM_ESTATE on a left-only context, and after a PSM_OPT_VIEWS change
+// until psm_cost_const has built the current frame's volumes again
+int check_right_view(psm_ctx* c, const char* call)
+{
+    if (c->views == 1)
+        return fail(c, PSM_ESTATE, "%s of the right view on a left-only context (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): the right "
+                    "view is not computed; set PSM_VIEWS_BOTH", call);
+    if (c->views_reset)
+        return fail(c, PSM_ESTATE, "%s of the right view after a PSM_OPT_VIEWS change: call psm_cost_const first", call);
+    return PSM_OK;
+}
+
+// a right-view output of a selection / map call: must be NULL on a left-only context, and is required otherwise
+int check_right_arg(psm_ctx* c, const void* right, const char* call)
+{
+    if (c->views == 1 && right)
+        return fail(c, PSM_EINVAL, "%s: the right map / key buffer must be NULL on a left-only context "
+                    "(PSM_OPT_VIEWS = PSM_VIEWS_LEFT)", call);
+    return PSM_OK;
+}
+
+// a stage that needs the stage state PSM_OPT_VIEWS reset
+int check_views_reset(psm_ctx* c, const char* call)
+{
+    if (c->views_reset)
+        return fail(c, PSM_ESTATE, "%s after a PSM_OPT_VIEWS change: the next stage must be psm_cost_const", call);
     return PSM_OK;
 }
 
@@ -285,6 +320,7 @@ int launch_ref(psm_ctx* c, void* kernel, int mode, int one_view = 0, int one_d =
     P.scale = 1.0 / ((double)P.K * P.K);
     P.eps = c->gif_eps;
     P.mode = mode; P.one_view = one_view; P.one_d = one_d;
+    P.nviews = c->views;
     void* args[] = {&P};
     PSM_CUDA(c, cudaLaunchCooperativeKernel(kernel, dim3(c->ref_blocks), dim3(kRefThreads), args, 0, c->stream));
     PSM_LAUNCH_CHECK(c);
@@ -313,7 +349,7 @@ int launch_guide(psm_ctx* c)
         P.seg_rows = kWinGuideSegRows;
         P.scale = 1.0 / ((double)P.K * P.K);
         P.eps = c->gif_eps;
-        dim3 grd((c->W + 127) / 128, (c->H + P.seg_rows - 1) / P.seg_rows, 2);
+        dim3 grd((c->W + 127) / 128, (c->H + P.seg_rows - 1) / P.seg_rows, c->views);
         guide_window_kernel<<<grd, 128, 0, c->stream>>>(P);
         PSM_LAUNCH_CHECK(c);
         return PSM_OK;
@@ -325,8 +361,11 @@ int launch_guide(psm_ctx* c)
     P.nstrips = (c->W + kGuideStripOut - 1) / kGuideStripOut;
     P.seg_rows = c->guide_seg_rows > 0 ? c->guide_seg_rows : kGuideSegRows;   // option 107 (tuning)
     P.nseg = (c->H + P.seg_rows - 1) / P.seg_rows;
-    const int tasks = 2 * P.nstrips * P.nseg;  // one warp each
-    guide_kernel<<<(tasks + 3) / 4, 128, 0, c->stream>>>(P);
+    const int tasks = c->views * P.nstrips * P.nseg;  // one warp each
+    if (c->views == 2)
+        guide_kernel<<<(tasks + 3) / 4, 128, 0, c->stream>>>(P);
+    else   // one warp per CTA: a spare warp of the last CTA would take a right-view task
+        guide_kernel<<<tasks, 32, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
@@ -357,7 +396,8 @@ struct CvfPlan {
     unsigned grid;
 };
 
-CvfPlan plan_cvf(int W, int H, int d_count, int nsm, int threads_override, int target_rows, bool allow_pack)
+// nviews: 2, or 1 for a left-only context (the grid holds the left view's CTAs alone)
+CvfPlan plan_cvf(int W, int H, int d_count, int nsm, int threads_override, int target_rows, bool allow_pack, int nviews)
 {
     CvfPlan q{};
     q.nstrips = (W + kStripOut - 1) / kStripOut;
@@ -386,7 +426,7 @@ CvfPlan plan_cvf(int W, int H, int d_count, int nsm, int threads_override, int t
         for (int want = 1; want <= 12; ++want) {
             int ns = 1, rows = H;
             plan_segments(H, (H + want - 1) / want, &ns, &rows);
-            const long ctas = 2L * ns * (q.nstrips * q.ndgroups + q.pack_ndg);
+            const long ctas = (long)nviews * ns * (q.nstrips * q.ndgroups + q.pack_ndg);
             const long waves = (ctas + slots - 1) / slots;
             // the last wave rarely runs full length: count it in proportion to its fill, but never below half a wave
             const long rem_ctas = ctas - (waves - 1) * slots;
@@ -400,8 +440,8 @@ CvfPlan plan_cvf(int W, int H, int d_count, int nsm, int threads_override, int t
     }
     q.nseg = best_ns; q.seg_rows = best_rows;
     if (target_rows > 0) plan_segments(H, target_rows, &q.nseg, &q.seg_rows);
-    q.pack_first = 2 * q.nseg * q.nstrips * q.ndgroups;
-    q.grid = (unsigned)q.pack_first + 2u * q.nseg * q.pack_ndg;
+    q.pack_first = nviews * q.nseg * q.nstrips * q.ndgroups;
+    q.grid = (unsigned)q.pack_first + (unsigned)nviews * q.nseg * q.pack_ndg;
     return q;
 }
 
@@ -416,7 +456,7 @@ int launch_cvf_stream(psm_ctx* c)
     int nsm = 0;
     PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
     const CvfPlan plan = plan_cvf(c->W, c->H, c->d_count, nsm, c->cvf_threads, c->cvf_target_rows,
-                                  !c->cvf_no_pack && !plain_variant && !c->cvf_remap);
+                                  !c->cvf_no_pack && !plain_variant && !c->cvf_remap, c->views);
     const int nthreads = plan.nthreads;
     P.nstrips = plan.nstrips; P.ndgroups = plan.ndgroups; P.nseg = plan.nseg; P.seg_rows = plan.seg_rows;
     P.pack_gl = plan.pack_gl; P.pack_x0 = plan.pack_x0; P.pack_ndg = plan.pack_ndg; P.pack_first = plan.pack_first;
@@ -501,7 +541,7 @@ int launch_cvf_window(psm_ctx* c)
     int nsm = 0, smem_max = 0;
     PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
     PSM_CUDA(c, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
-    const long base = 2L * P.Dloc * P.nstrips;
+    const long base = (long)c->views * P.Dloc * P.nstrips;
     int nseg = 1;
     while (base * nseg < 4L * nsm && c->H / (nseg + 1) >= 4 * P.K) ++nseg;
     P.seg_rows = (c->H + nseg - 1) / nseg;
@@ -533,25 +573,33 @@ int launch_cvc(psm_ctx* c)
     // option 108 (tuning): slices per CTA (0 = all owned slices in one CTA, the shipped decomposition)
     P2.chunk = (c->cvc_chunk > 0 && c->cvc_chunk < c->d_count) ? c->cvc_chunk : 0;
     const int nchunks = P2.chunk ? (c->d_count + P2.chunk - 1) / P2.chunk : 1;
-    dim3 blk(128), grd((((c->W + 3) / 4) + 127) / 128, c->H, 2 * nchunks);
+    dim3 blk(128), grd((((c->W + 3) / 4) + 127) / 128, c->H, c->views * nchunks);
     // option 106 (tuning): 0 shipped = interior fast path + scalar window loads; 2 = no fast path (the round-1 loop);
     // 1 / 3 = fast path + grouped 128-bit window loads for the border warps without / with a register cap (DESIGN.md section 10)
     // Any matching cost other than the default runs the parameterised build of the shipped variant, all owned slices
-    // per CTA: options 106 and 108 do not apply to it.
+    // per CTA: options 106 and 108 do not apply to it.  A left-only context runs the one-view builds.
     if (!c->cost_default()) {
-        grd.z = 2;
-        cvc_cost_kernel<<<grd, blk, 0, c->stream>>>(P2, c->cost);
-    } else {
+        grd.z = c->views;
+        if (c->views == 2) cvc_cost_kernel<<<grd, blk, 0, c->stream>>>(P2, c->cost);
+        else cvc_cost_kernel<1><<<grd, blk, 0, c->stream>>>(P2, c->cost);
+    } else if (c->views == 2) {
         switch (c->cvc_variant) {
         case 1: cvc_both_kernel<4, 1><<<grd, blk, 0, c->stream>>>(P2); break;
         case 2: cvc_both_kernel<7, 2><<<grd, blk, 0, c->stream>>>(P2); break;
         case 3: cvc_both_kernel<5, 1><<<grd, blk, 0, c->stream>>>(P2); break;
         default: cvc_both_kernel<7, 0><<<grd, blk, 0, c->stream>>>(P2); break;
         }
+    } else {
+        switch (c->cvc_variant) {
+        case 1: cvc_both_kernel<4, 1, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+        case 2: cvc_both_kernel<7, 2, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+        case 3: cvc_both_kernel<5, 1, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+        default: cvc_both_kernel<7, 0, 1><<<grd, blk, 0, c->stream>>>(P2); break;
+        }
     }
     PSM_LAUNCH_CHECK(c);
     if (!P2.v[0].fold_halo)  // narrow images: separate halo pass (general reflection)
-        for (int v = 0; v < 2; ++v)
+        for (int v = 0; v < c->views; ++v)
             if (int rc = pad_rows(c, c->vol[v], (size_t)c->d_count * c->H)) return rc;
     return PSM_OK;
 }
@@ -575,7 +623,7 @@ int launch_fold(psm_ctx* c, bool first)
     FoldParams P;
     for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count; P.first = first ? 1 : 0;
-    dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, 2);
+    dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, c->views);
     wta_fold_kernel<<<grd, blk, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
@@ -724,7 +772,7 @@ const char* psm_last_error(psm_ctx* ctx) { return ctx ? ctx->err : g_create_erro
 int psm_cvf_plan(int width, int height, int d_count, int sm_count, int no_pack, int* out, int n)
 {
     if (width < 1 || height < 1 || d_count < 1 || sm_count < 1 || !out || n < 10) return PSM_EINVAL;
-    const CvfPlan q = plan_cvf(width, height, d_count, sm_count, 0, 0, !no_pack);
+    const CvfPlan q = plan_cvf(width, height, d_count, sm_count, 0, 0, !no_pack, 2);
     const int v[10] = {q.nthreads, q.nstrips, q.ndgroups, q.nseg, q.seg_rows, q.pack_gl, q.pack_x0, q.pack_ndg, q.pack_first, (int)q.grid};
     for (int i = 0; i < 10; ++i) out[i] = v[i];
     return PSM_OK;
@@ -997,9 +1045,26 @@ int psm_set_option(psm_ctx* c, int key, int value)
     if (c->nshards) {
         if (key == PSM_OPT_P2P_SYNC)
             return reject_multi(c, "PSM_OPT_P2P_SYNC", "its shards' exchange is ordered by events, never by flags");
-        return forward(c, [&](psm_ctx* s) { return psm_set_option(s, key, value); });
+        if (int rc = forward(c, [&](psm_ctx* s) { return psm_set_option(s, key, value); })) return rc;
+        if (key == PSM_OPT_VIEWS) c->views = value;   // the map calls check the right-view arguments on the context itself
+        return PSM_OK;
     }
     switch (key) {
+    case PSM_OPT_VIEWS:
+        if (value != PSM_VIEWS_LEFT && value != PSM_VIEWS_BOTH)
+            return fail(c, PSM_EINVAL, "PSM_OPT_VIEWS must be PSM_VIEWS_LEFT (1) or PSM_VIEWS_BOTH (2) (got %d)", value);
+        if (value != c->views) {
+            // the frame's stages start again from psm_cost_const on the current images; nothing computed for the other
+            // setting (volumes, maps, masks, the guide of the right view) can be read or selected from
+            c->views = value;
+            c->views_reset = true;
+            c->guide_valid = false;
+            c->have_cvc = false;
+            c->filtered = false;
+            c->have_maps = false;
+            c->lr_masks_ok = false;
+        }
+        return PSM_OK;
     case PSM_OPT_CVF_MODE:
         if (value != PSM_CVF_EXACT && value != PSM_CVF_MIXED && value != PSM_CVF_NAIVE)
             return fail(c, PSM_EINVAL, "unknown CVF mode %d", value);
@@ -1194,6 +1259,7 @@ int psm_cost_const(psm_ctx* c)
     if (int rc = clear_slice_flags(c)) return rc;
     c->have_cvc = true;
     c->filtered = false;
+    c->views_reset = false;
     return stage_end(c, 1);
 }
 
@@ -1201,6 +1267,7 @@ int psm_cost_filter(psm_ctx* c)
 {
     if (is_multi(c)) return forward(c, [](psm_ctx* s) { return psm_cost_filter(s); });
     if (int rc = bind(c)) return rc;
+    if (int rc = check_views_reset(c, "psm_cost_filter")) return rc;
     if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter before psm_cost_const");
     if (!c->gif_default() && c->cvf_mode != PSM_CVF_EXACT)
         return fail(c, PSM_EINVAL, "CVF mode %s exists only for the default guided filter (window 8, eps 1e-4); "
@@ -1221,7 +1288,8 @@ int psm_cost_filter(psm_ctx* c)
                 if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefFlagged)) return rc;
         }
         if (int rc = clear_slice_flags(c)) return rc;
-        for (int v = 0; v < 2; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
+        // the right view's pair is not swapped on a left-only context: its volume buffers keep their roles
+        for (int v = 0; v < c->views; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
         return PSM_OK;
     };
     if (c->blk_slices) {   // stage 4 is not recorded: its kernels interleave with every block's CVC and fold
@@ -1241,6 +1309,7 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
 {
     if (is_multi(c)) return forward(c, [s](psm_ctx* sh) { return psm_cost_filter_fgf(sh, s); });
     if (int rc = bind(c)) return rc;
+    if (int rc = check_views_reset(c, "psm_cost_filter_fgf")) return rc;
     if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter_fgf before psm_cost_const");
     if (s != 1 && s != 2 && s != 4 && s != 8) return fail(c, PSM_EINVAL, "sub-sampling rate must be 1, 2, 4 or 8 (got %d)", s);
     if (c->W / s < 1 || c->H / s < 1) return fail(c, PSM_EINVAL, "image smaller than the sub-sampling rate");
@@ -1306,17 +1375,17 @@ int psm_cost_filter_fgf(psm_ctx* c, int s)
         return PSM_OK;
     };
     if (int rc = stage_begin(c, 2)) return rc;
-    if (c->blk_slices) {   // both guides once, then every block; stage 4 is not recorded
-        for (int v = 0; v < 2; ++v)
+    if (c->blk_slices) {   // the guides once, then every block; stage 4 is not recorded
+        for (int v = 0; v < c->views; ++v)
             if (int rc = guide(v)) return rc;
         if (int rc = run_blocks(c, [&]() -> int {
-                for (int v = 0; v < 2; ++v)
+                for (int v = 0; v < c->views; ++v)
                     if (int rc = slices(v)) return rc;
                 return PSM_OK;
             })) return rc;
     } else {
         if (int rc = stage_begin(c, 4)) return rc;
-        for (int v = 0; v < 2; ++v) {
+        for (int v = 0; v < c->views; ++v) {
             if (int rc = guide(v)) return rc;
             if (int rc = slices(v)) return rc;
         }
@@ -1335,14 +1404,14 @@ static int select_maps(psm_ctx* c)
 {
     if (c->blk_slices) {   // a blocked context's selection is in its running keys: reduce them as one rank's
         const size_t npix = (size_t)c->W * c->H;
-        for (int v = 0; v < 2; ++v) {
+        for (int v = 0; v < c->views; ++v) {
             keys_reduce_kernel<T><<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(c->run_keys[v], 1, npix,
                                                                                          reinterpret_cast<T*>(c->dis[v]));
             PSM_LAUNCH_CHECK(c);
         }
         return PSM_OK;
     }
-    for (int v = 0; v < 2; ++v) {
+    for (int v = 0; v < c->views; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
         wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
                                                   reinterpret_cast<T*>(c->dis[v]), nullptr);
@@ -1357,9 +1426,11 @@ static int disp_select(psm_ctx* c, T* left, size_t left_step, T* right, size_t r
 {
     if (int rc = sync ? check_map_format<T>(c, "psm_disp_select", "psm_disp_select_u16")
                       : check_map_format<T>(c, "psm_disp_select_async", "psm_disp_select_u16_async")) return rc;
+    if (int rc = check_right_arg(c, right, "psm_disp_select")) return rc;
     if (int rc = psm_disp_select_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
-    if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
+    if (c->views == 2)
+        if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
     if (sync) PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }
@@ -1371,19 +1442,23 @@ static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const u
     if (is_multi(c)) return reject_multi(c, sizeof(T) == 1 ? "psm_disp_reduce_keys" : "psm_disp_reduce_keys_u16", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = check_map_format<T>(c, "psm_disp_reduce_keys", "psm_disp_reduce_keys_u16")) return rc;
     if (int rc = bind(c)) return rc;
-    if (!d_gathered_left || !d_gathered_right || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
+    if (int rc = check_views_reset(c, "psm_disp_reduce_keys")) return rc;
+    if (int rc = check_right_arg(c, d_gathered_right, "psm_disp_reduce_keys")) return rc;
+    if (int rc = check_right_arg(c, right, "psm_disp_reduce_keys")) return rc;
+    if (!d_gathered_left || (c->views == 2 && !d_gathered_right) || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
     const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
     c->lr_masks_ok = false;
     const size_t npix = (size_t)c->W * c->H;
-    for (int v = 0; v < 2; ++v) {
+    for (int v = 0; v < c->views; ++v) {
         keys_reduce_kernel<T><<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
             reinterpret_cast<const unsigned long long*>(g[v]), nranks, npix, reinterpret_cast<T*>(c->dis[v]));
         PSM_LAUNCH_CHECK(c);
     }
     c->have_maps = true;
-    if (left && right) {
+    if (left && (right || c->views == 1)) {
         if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
-        if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
+        if (c->views == 2)
+            if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
     }
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
@@ -1431,17 +1506,18 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
 {
     if (is_multi(c)) return reject_multi(c, "psm_disp_select_keys", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
-    if (!d_keys_left || !d_keys_right) return fail(c, PSM_EINVAL, "null key buffer");
+    if (int rc = check_right_arg(c, d_keys_right, "psm_disp_select_keys")) return rc;
+    if (!d_keys_left || (c->views == 2 && !d_keys_right)) return fail(c, PSM_EINVAL, "null key buffer");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
     uint64_t* keys[2] = {d_keys_left, d_keys_right};
     if (c->blk_slices) {   // the running keys are this context's minima already
-        for (int v = 0; v < 2; ++v)
+        for (int v = 0; v < c->views; ++v)
             PSM_CUDA(c, cudaMemcpyAsync(keys[v], c->run_keys[v], (size_t)c->W * c->H * sizeof(uint64_t),
                                         cudaMemcpyDeviceToDevice, c->stream));
         return stage_end(c, 3);
     }
-    for (int v = 0; v < 2; ++v) {   // keys only, on either map format
+    for (int v = 0; v < c->views; ++v) {   // keys only, on either map format
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
         wta_kernel<uint8_t><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, nullptr,
                                                         reinterpret_cast<unsigned long long*>(keys[v]));
@@ -1487,6 +1563,8 @@ int psm_p2p_create_buffer(psm_ctx* c, int nranks, void** d_buffer)
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     c->p2p_nranks = nranks;
     c->p2p_seq = 0;
+    c->p2p_seq_right = 0;
+    c->p2p_right_current = false;
     c->p2p_waited_seq = 0;
     *d_buffer = c->p2p_own;
     return PSM_OK;
@@ -1535,7 +1613,8 @@ static void p2p_fill(const psm_ctx* c, int view, P2pPeers& peers)
     const size_t kb = p2p_keys_bytes(c, c->p2p_nranks), mb = p2p_maps_bytes(c);
     peers.nranks = c->p2p_nranks; peers.rank = c->p2p_rank; peers.chunk = (unsigned)chunk;
     peers.counter = c->p2p_counter;
-    peers.seq = c->p2p_sync ? c->p2p_seq : 0u;
+    // each view's flags carry the number of the last frame that exchanged that view
+    peers.seq = c->p2p_sync ? (view ? c->p2p_seq_right : c->p2p_seq) : 0u;
     for (int r = 0; r < kMaxRanks; ++r) {
         unsigned char* base = r < c->p2p_nranks ? c->p2p_peer[r] : nullptr;
         peers.keys[r] = base ? reinterpret_cast<unsigned long long*>(base) + (size_t)view * c->p2p_nranks * chunk : nullptr;
@@ -1548,9 +1627,11 @@ static void p2p_fill(const psm_ctx* c, int view, P2pPeers& peers)
 // blocked shard of a multi-device context, keys_scatter_kernel over its running keys
 static int p2p_scatter(psm_ctx* c)
 {
-    c->p2p_seq++;   // one sequence number per frame, identical on every rank (all ranks run the same frames)
+    c->p2p_seq++;   // one sequence number per frame, identical on every rank (all ranks run the same frames and views)
+    if (c->views == 2) c->p2p_seq_right++;
+    c->p2p_right_current = c->views == 2;
     c->lr_masks_ok = false;
-    for (int v = 0; v < 2; ++v) {
+    for (int v = 0; v < c->views; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, (c->H + kScatterRows - 1) / kScatterRows);
@@ -1582,15 +1663,25 @@ int psm_disp_reduce_p2p(psm_ctx* c)
     if (is_multi(c)) return reject_multi(c, "psm_disp_reduce_p2p", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "no exchange block");
+    if (int rc = check_views_reset(c, "psm_disp_reduce_p2p")) return rc;
     const unsigned npix = (unsigned)((size_t)c->W * c->H);
     const auto reduce = c->map_bytes == 2 ? chunk_reduce_kernel<uint16_t> : chunk_reduce_kernel<uint8_t>;
     c->lr_masks_ok = false;
-    for (int v = 0; v < 2; ++v) {
+    for (int v = 0; v < c->views; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
         reduce<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
         PSM_LAUNCH_CHECK(c);
     }
+    return PSM_OK;
+}
+
+// the exchange block's right map is from an earlier frame than its left map (the last exchanged frame was left-only)
+static int check_p2p_right_map(psm_ctx* c, const char* call)
+{
+    if (c->views == 2 && c->p2p_seq > 0 && !c->p2p_right_current)
+        return fail(c, PSM_ESTATE, "%s: the exchanged right map is from a frame before the last left-only one; run a "
+                    "selection stage with PSM_VIEWS_BOTH first", call);
     return PSM_OK;
 }
 
@@ -1601,8 +1692,16 @@ static int p2p_wait_done(psm_ctx* c)
     if (!c->p2p_sync || c->p2p_waited_seq == c->p2p_seq) return PSM_OK;
     P2pPeers peers;
     p2p_fill(c, 0, peers);
-    p2p_wait_done_kernel<<<1, 32, 0, c->stream>>>(peers.flags[c->p2p_rank], c->p2p_nranks, c->p2p_seq);
-    PSM_LAUNCH_CHECK(c);
+    if (c->views == 2 && c->p2p_seq_right == c->p2p_seq) {
+        p2p_wait_done_kernel<<<1, 32, 0, c->stream>>>(peers.flags[c->p2p_rank], c->p2p_nranks, c->p2p_seq);
+        PSM_LAUNCH_CHECK(c);
+    } else {   // the views' flags carry different frame numbers: one wait per view, nranks threads (the first view's words)
+        for (int v = 0; v < c->views; ++v) {
+            p2p_wait_done_kernel<<<1, c->p2p_nranks, 0, c->stream>>>(peers.flags[c->p2p_rank] + (size_t)v * 2 * kMaxRanks,
+                                                                     c->p2p_nranks, v ? c->p2p_seq_right : c->p2p_seq);
+            PSM_LAUNCH_CHECK(c);
+        }
+    }
     c->p2p_waited_seq = c->p2p_seq;
     return PSM_OK;
 }
@@ -1657,10 +1756,14 @@ static int disp_fetch_p2p(psm_ctx* c, T* left, size_t left_step, T* right, size_
     if (int rc = check_map_format<T>(c, "psm_disp_fetch_p2p", "psm_disp_fetch_p2p_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
+    if (int rc = check_views_reset(c, "psm_disp_fetch_p2p")) return rc;
+    if (int rc = check_right_arg(c, right, "psm_disp_fetch_p2p")) return rc;
+    if (int rc = check_p2p_right_map(c, "psm_disp_fetch_p2p")) return rc;
     if (int rc = p2p_wait_done(c)) return rc;
     const unsigned char* maps = c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks);
     if (int rc = copy_map_out(c, maps, left, left_step)) return rc;
-    if (int rc = copy_map_out(c, maps + (size_t)c->W * c->H * sizeof(T), right, right_step)) return rc;
+    if (c->views == 2)
+        if (int rc = copy_map_out(c, maps + (size_t)c->W * c->H * sizeof(T), right, right_step)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }
@@ -1723,9 +1826,16 @@ static int post_process_maps(psm_ctx* c)
     }();
     c->lr_masks_ok = false;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_post_process before psm_set_images");
+    if (int rc = check_views_reset(c, "psm_post_process")) return rc;
     if (!c->have_maps && !(c->p2p_own && c->p2p_seq > 0)) return fail(c, PSM_ESTATE, "psm_post_process before a disparity-selection stage");
+    if (c->p2p_own && c->p2p_seq > 0)
+        if (int rc = check_p2p_right_map(c, "psm_post_process")) return rc;
     const size_t npix = (size_t)c->W * c->H;
     const bool lr = c->lr_mode != PSM_LR_OFF, wmf = c->lr_mode != PSM_LR_FILL;
+    if (lr && c->views == 1)
+        return fail(c, PSM_ESTATE, "psm_post_process: the left-right check (psm_set_lr_check mode %d) needs both maps, and "
+                    "this context computes the left view alone (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): set PSM_LR_OFF or "
+                    "PSM_VIEWS_BOTH", c->lr_mode);
     // Each buffer is allocated while its own pointer is null and the table is marked valid only once it is on the
     // device, so a call that failed part-way leaves nothing a launch could trip over: the next call completes the set-up
     // or fails in turn.
@@ -1771,7 +1881,7 @@ static int post_process_maps(psm_ctx* c)
     const long pgrid = std::min<long>((long)nsm * 8, ((long)npix + kPpParamWarps - 1) / kPpParamWarps);
     int steps = 0;
     while ((1 << steps) < c->D) ++steps;   // u16 maps: ceil(log2 max_disp) bisection steps over [0, max_disp - 1]
-    for (int v = 0; v < 2; ++v) {
+    for (int v = 0; v < c->views; ++v) {
         const float* g = c->guide[v];
         T* dst = reinterpret_cast<T*>(c->dis_pp[v]);
         dim3 blk(256), grd((c->W + 255) / 256, c->H);
@@ -1797,9 +1907,11 @@ template <typename T>
 static int post_process(psm_ctx* c, T* left, size_t left_step, T* right, size_t right_step)
 {
     if (int rc = check_map_format<T>(c, "psm_post_process", "psm_post_process_u16")) return rc;
+    if (int rc = check_right_arg(c, right, "psm_post_process")) return rc;
     if (int rc = psm_post_process_device(c)) return rc;
     if (int rc = copy_map_out(c, c->dis_pp[0], left, left_step)) return rc;
-    if (int rc = copy_map_out(c, c->dis_pp[1], right, right_step)) return rc;
+    if (c->views == 2)
+        if (int rc = copy_map_out(c, c->dis_pp[1], right, right_step)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }
@@ -1860,6 +1972,8 @@ int psm_read_cost_slice(psm_ctx* c, int view, int d, float* dst, size_t dst_step
     if (is_multi(c)) return route_slice(c, d, [&](psm_ctx* s) { return psm_read_cost_slice(s, view, d, dst, dst_step); });
     if (int rc = bind(c)) return rc;
     if (int rc = check_slice(c, view, d)) return rc;
+    if (view == PSM_RIGHT)
+        if (int rc = check_right_view(c, "psm_read_cost_slice")) return rc;
     if (!dst || dst_step < (size_t)c->W * sizeof(float)) return fail(c, PSM_EINVAL, "bad dst/step");
     PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->vol[view] + slice_offset(c, d),
                                   c->Wp * sizeof(float), c->W * sizeof(float), c->H, cudaMemcpyDeviceToHost, c->stream));
@@ -1911,8 +2025,10 @@ int psm_read_guide_plane(psm_ctx* c, int view, int plane_id, float* dst, size_t 
     else if (plane_id >= 6 && plane_id <= 11) src = c->guide[view] + (size_t)(kGuideVar + plane_id - 6) * c->plane;
     else if (plane_id == 12) src = c->grd[view];
     else return fail(c, PSM_EINVAL, "bad plane id %d", plane_id);
-    if (plane_id >= 3 && plane_id <= 11)
+    if (plane_id >= 3 && plane_id <= 11) {
+        if (view == PSM_RIGHT && c->views == 1) return check_right_view(c, "psm_read_guide_plane (planes 3-11)");
         if (int rc = ensure_guide(c)) return rc;
+    }
     PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, src, c->Wp * sizeof(float), c->W * sizeof(float), c->H,
                                   cudaMemcpyDeviceToHost, c->stream));
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1924,6 +2040,8 @@ int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
     if (is_multi(c)) return route_slice(c, d, [&](psm_ctx* s) { return psm_read_ab_slice(s, view, d, a3, b); });
     if (int rc = bind(c)) return rc;
     if (int rc = check_slice(c, view, d)) return rc;
+    if (view == PSM_RIGHT)
+        if (int rc = check_right_view(c, "psm_read_ab_slice")) return rc;
     if (!a3 || !b) return fail(c, PSM_EINVAL, "null output");
     if (!c->have_images) return fail(c, PSM_ESTATE, "no images set");
     if (int rc = ensure_guide(c)) return rc;
@@ -1963,6 +2081,9 @@ int psm_read_valid_mask(psm_ctx* c, int view, uint8_t* dst, size_t dst_step)
     if (int rc = bind(c)) return rc;
     if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
     if (!dst || dst_step < (size_t)c->W) return fail(c, PSM_EINVAL, "bad dst/step");
+    if (c->views == 1)   // the left-right check never runs on a left-only context
+        return fail(c, PSM_ESTATE, "psm_read_valid_mask on a left-only context (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): the "
+                    "left-right check needs both maps; set PSM_VIEWS_BOTH");
     if (!c->lr_masks_ok)
         return fail(c, PSM_ESTATE, "no valid mask: the last post-process since the last selection stage did not run the left-right check");
     PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->lr_valid[view], c->W, c->W, c->H, cudaMemcpyDeviceToHost, c->stream));

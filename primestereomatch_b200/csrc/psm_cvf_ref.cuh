@@ -51,6 +51,7 @@ struct RefParams {
     double scale;         // 1 / K^2
     float eps;
     int mode, one_view, one_d;
+    int nviews;           // 2, or 1: the left view alone (PSM_VIEWS_LEFT)
 };
 
 // Row pass: rs[q][y][x] = the K-wide row sum of quantity q at (x, y), RowSum<float, double>'s order.  One thread per row.
@@ -130,7 +131,7 @@ __device__ __forceinline__ void ref_cols(const double* __restrict__ rs, int W, i
 __global__ void __launch_bounds__(kRefThreads) guide_ref_kernel(const RefParams P)
 {
     const bool todo0 = (P.guide_flags[0] & (kGuideOutside | kGuideInexact)) != 0;
-    const bool todo1 = (P.guide_flags[1] & (kGuideOutside | kGuideInexact)) != 0;
+    const bool todo1 = P.nviews > 1 && (P.guide_flags[1] & (kGuideOutside | kGuideInexact)) != 0;
     if (!todo0 && !todo1) return;   // the same for every block
     cg::grid_group grid = cg::this_grid();
     const int W = P.W, H = P.H, Wp = P.Wp;
@@ -224,10 +225,10 @@ __device__ __forceinline__ void ref_filter_slice(const RefParams& P, cg::grid_gr
 __global__ void __launch_bounds__(kRefThreads) cvf_ref_kernel(const RefParams P)
 {
     const int views_all = ((P.guide_flags[0] & (kGuideOutside | kGuideNonFinite)) ? 1 : 0) |
-                          ((P.guide_flags[1] & (kGuideOutside | kGuideNonFinite)) ? 2 : 0);
+                          (P.nviews > 1 && (P.guide_flags[1] & (kGuideOutside | kGuideNonFinite)) ? 2 : 0);
     if (P.mode == kRefFlagged) {
         int any = views_all;
-        for (int i = threadIdx.x; i < 2 * P.Dloc; i += blockDim.x) any |= P.slice_flags[i];
+        for (int i = threadIdx.x; i < P.nviews * P.Dloc; i += blockDim.x) any |= P.slice_flags[i];
         if (!__syncthreads_or(any)) return;   // the same for every block
     }
     cg::grid_group grid = cg::this_grid();
@@ -235,7 +236,7 @@ __global__ void __launch_bounds__(kRefThreads) cvf_ref_kernel(const RefParams P)
         ref_filter_slice(P, grid, P.one_view, P.one_d, true);
         return;
     }
-    for (int view = 0; view < 2; ++view)
+    for (int view = 0; view < P.nviews; ++view)
         for (int dl = 0; dl < P.Dloc; ++dl)
             if (P.mode == kRefAll || ((views_all >> view) & 1) || P.slice_flags[view * P.Dloc + dl])
                 ref_filter_slice(P, grid, view, dl, false);

@@ -165,11 +165,12 @@ __device__ __forceinline__ void cvc_body(const CvcParams& P, const Weigh& weigh)
 // blockIdx.z = chunk * 2 + view: with chunk > 0 (P2.chunk slices per CTA instead of all owned slices) the grid walks the volume
 // chunk by chunk -- z is the slowest block index -- so that at any moment the GPU writes a few neighbouring slices instead of one
 // 2 KB run in each of 128 slices 8 MB apart (DRAM page locality of the 2.1 GB store stream; DESIGN.md section 10).
+// NVIEWS = 1 (PSM_VIEWS_LEFT) builds the left volume alone: blockIdx.z = chunk.
 struct CvcParams2 { CvcParams v[2]; int chunk; };
-template <int MINB, int GROUPED>
+template <int MINB, int GROUPED, int NVIEWS = 2>
 __global__ void __launch_bounds__(128, MINB) cvc_both_kernel(const CvcParams2 P2)
 {
-    const int view = blockIdx.z & 1, chunk = blockIdx.z >> 1;
+    const int view = NVIEWS == 2 ? blockIdx.z & 1 : 0, chunk = NVIEWS == 2 ? blockIdx.z >> 1 : blockIdx.z;
     CvcParams P = P2.v[view];
     if (P2.chunk > 0) {
         const int first = chunk * P2.chunk;
@@ -182,10 +183,12 @@ __global__ void __launch_bounds__(128, MINB) cvc_both_kernel(const CvcParams2 P2
 }
 
 // The same K1 at any psm_set_matching_cost setting other than the default: the shipped decomposition (interior fast path,
-// scalar window loads, all owned slices per CTA; tuning options 106 and 108 do not apply), grid z = view.
+// scalar window loads, all owned slices per CTA; tuning options 106 and 108 do not apply), grid z = view (NVIEWS = 1: the
+// left volume alone).
+template <int NVIEWS = 2>
 __global__ void __launch_bounds__(128, 7) cvc_cost_kernel(const CvcParams2 P2, const CvcCost K)
 {
-    const int view = blockIdx.z & 1;
+    const int view = NVIEWS == 2 ? blockIdx.z & 1 : 0;
     const CvcParams P = P2.v[view];
     const CostParam weigh(K);
     if (view == 0) cvc_body<-1, 0>(P, weigh);

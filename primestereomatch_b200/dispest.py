@@ -165,6 +165,27 @@ class DispEst:
         self.lr_mode = int(mode)
         return 0
 
+    _VIEWS = {"left": capi.PSM_VIEWS_LEFT, "both": capi.PSM_VIEWS_BOTH}
+
+    def setViews(self, views):
+        """Which disparity maps the later frames compute (PSM_OPT_VIEWS): "both" (default) or "left".  "left" skips every
+        right-view stage after ingest; DispSelect_GPU and PostProcess_GPU then fill lDisMap alone, rDisMap is None, and
+        setLRCheck modes 1 and 2 make PostProcess_GPU raise.  Changing it restarts the frame at CostConst_GPU.  Raises
+        ValueError on any other value."""
+        if not isinstance(views, str) or views not in self._VIEWS:
+            raise ValueError(f'setViews takes "left" or "both" (got {views!r})')
+        self._need_gpu()
+        capi.check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_VIEWS, self._VIEWS[views]), self._ctx)
+        if views == "left":
+            self.rDisMap = None
+        elif self.rDisMap is None:
+            self.rDisMap = np.zeros_like(self.lDisMap)
+        return 0
+
+    @staticmethod
+    def _map_arg(m):
+        return (None, 0) if m is None else (_ptr(m), m.strides[0])
+
     def set_option(self, key, value):
         capi.check(self._lib.psm_set_option(self._ctx, int(key), int(value)), self._ctx)
 
@@ -203,8 +224,7 @@ class DispEst:
         """DispEst.cpp:323-328: WTA, results land in lDisMap / rDisMap."""
         self._need_gpu()
         sel = self._lib.psm_disp_select_u16 if self.map_bits == 16 else self._lib.psm_disp_select
-        capi.check(sel(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
-                       _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
+        capi.check(sel(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
         return 0
 
     def PostProcess_GPU(self):
@@ -213,8 +233,7 @@ class DispEst:
         in GPU mode, here it is a device stage.  Results replace lDisMap / rDisMap."""
         self._need_gpu()
         pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
-        capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0],
-                      _ptr(self.rDisMap), self.rDisMap.strides[0]), self._ctx)
+        capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
         if self.lr_mode != capi.PSM_LR_OFF:
             for view, mask in ((capi.PSM_LEFT, self.lValid), (capi.PSM_RIGHT, self.rValid)):
                 capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)

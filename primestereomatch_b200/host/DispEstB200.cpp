@@ -85,6 +85,14 @@ int DispEst::setLRCheck(int mode)
     return rc;
 }
 
+int DispEst::setViews(int v)
+{
+    if (!ctx) return -1;
+    const int rc = psm_set_option(ctx, PSM_OPT_VIEWS, v);
+    if (rc == PSM_OK) views = v;
+    return rc;
+}
+
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
 {
@@ -132,9 +140,10 @@ int DispEst::CostFilter_GPU()
 int DispEst::DispSelect_GPU()
 {
     if (!ctx) return -1;
+    const bool both = views == PSM_VIEWS_BOTH;   // a left-only context takes no right map
     if (lDisMap.type() == CV_16UC1)
-        return psm_disp_select_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, rDisMap.ptr<uint16_t>(), rDisMap.step);
-    return psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, rDisMap.ptr<uint8_t>(), rDisMap.step);
+        return psm_disp_select_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step);
+    return psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
 }
 
 // reference src/DispEst.cpp:338-344 -> PP::processDM (src/PP.cpp:402-425): the joint weighted-median filter of
@@ -143,9 +152,10 @@ int DispEst::DispSelect_GPU()
 int DispEst::PostProcess_GPU()
 {
     if (!ctx) return -1;
+    const bool both = views == PSM_VIEWS_BOTH;
     const int rc = lDisMap.type() == CV_16UC1
-        ? psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, rDisMap.ptr<uint16_t>(), rDisMap.step)
-        : psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, rDisMap.ptr<uint8_t>(), rDisMap.step);
+        ? psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step)
+        : psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
     if (rc || lr_mode == PSM_LR_OFF) return rc;
     if (int e = psm_read_valid_mask(ctx, PSM_LEFT, lValid.ptr<uint8_t>(), lValid.step)) return e;
     return psm_read_valid_mask(ctx, PSM_RIGHT, rValid.ptr<uint8_t>(), rValid.step);

@@ -104,6 +104,10 @@ public:
     // post-filter for every later PostProcess call; see psm_set_lr_check.  INTEGRATION.md: a build that restores
     // PP.cpp:405-406 calls setLRCheck(PSM_LR_FILL_WMF).
     int setLRCheck(int mode);
+    // PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT (PSM_OPT_VIEWS): with PSM_VIEWS_LEFT the later frames compute the left
+    // map alone; DispSelect_GPU and PostProcess_GPU then leave rDisMap (and rValid) untouched.  The next stage after a
+    // change must be CostConst_GPU.
+    int setViews(int views);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
@@ -136,5 +140,6 @@ private:
     bool useOCL;
     unsigned int subsample_rate = 4;
     int lr_mode = PSM_LR_OFF;
+    int views = PSM_VIEWS_BOTH;
     psm_ctx* ctx = nullptr;
 };

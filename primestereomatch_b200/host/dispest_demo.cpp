@@ -9,7 +9,8 @@
 // mode (0 off, 1 check + fill + post-filter, 2 check + fill) to setLRCheck (default 0).  D up to 4096: above 256 the
 // maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.  A leading
 // `--block-slices N` runs a blocked context (psm_create_blocked) that holds N disparity slices at a time, a leading
-// `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat).
+// `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat).  A leading
+// `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -30,6 +31,12 @@ int main(int argc, char** argv)
 {
     int block_slices = 0;
     std::vector<int> devices;
+    const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
+    if (left_only) {
+        argv[1] = argv[0];
+        ++argv;
+        --argc;
+    }
     while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices"))) {
         if (!std::strcmp(argv[1], "--block-slices")) {
             block_slices = std::atoi(argv[2]);
@@ -46,7 +53,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--block-slices N] [--devices i,j,...] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -58,7 +65,8 @@ int main(int argc, char** argv)
     SMDE->setInputImages(l, r);
     SMDE->setThreads(MAX_CPU_THREADS);
     SMDE->setSubsampleRate(4);
-    int rc = argc >= 10 ? SMDE->setGuidedFilter(std::atoi(argv[8]), (float)std::atof(argv[9])) : 0;
+    int rc = left_only ? SMDE->setViews(PSM_VIEWS_LEFT) : 0;
+    if (!rc && argc >= 10) rc = SMDE->setGuidedFilter(std::atoi(argv[8]), (float)std::atof(argv[9]));
     if (!rc && argc >= 13)
         rc = SMDE->setMatchingCost((float)std::atof(argv[10]), (float)std::atof(argv[11]), (float)std::atof(argv[12]));
     if (!rc && argc >= 17) {
@@ -76,7 +84,7 @@ int main(int argc, char** argv)
     std::printf("CVC %.3f ms  CVF %.3f ms  DispSel %.3f ms  PP %.3f ms\n", SMDE->stage_ms(1), SMDE->stage_ms(2), SMDE->stage_ms(3), SMDE->stage_ms(5));
     const size_t bytes = SMDE->lDisMap.step * H;   // dense rows: W * 1 or W * 2 bytes
     FILE* f = std::fopen(argv[6], "wb"); std::fwrite(SMDE->lDisMap.data, 1, bytes, f); std::fclose(f);
-    f = std::fopen(argv[7], "wb"); std::fwrite(SMDE->rDisMap.data, 1, bytes, f); std::fclose(f);
+    if (!left_only) { f = std::fopen(argv[7], "wb"); std::fwrite(SMDE->rDisMap.data, 1, bytes, f); std::fclose(f); }
     delete SMDE;
     return 0;
 }
