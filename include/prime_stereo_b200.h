@@ -304,6 +304,18 @@ int psm_read_valid_mask(psm_ctx* ctx, int view, uint8_t* dst, size_t dst_step);
  * on the stream the context was using.  The stream must outlive the context, or be replaced before psm_destroy. */
 int psm_set_stream(psm_ctx* ctx, void* cuda_stream);
 
+/* Ordering against a caller's stream (cudaStream_t passed as void*, NULL = the legacy default stream, on the context's
+ * first device) with CUDA events only: neither call waits on the host, and both work on every kind of context.
+ *   psm_wait_stream:   the context's later work waits for all work enqueued on the stream so far (e.g. the kernel
+ *                      that wrote the frame psm_set_images_device_planes is about to read);
+ *   psm_signal_stream: later work on the stream waits for all work the context has enqueued so far (e.g. a consumer of
+ *                      the maps of psm_copy_maps_device, or the overwrite or free of the input frames).
+ * "The context" is its compute and copy streams, on every shard of a multi-device context, including the
+ * device-to-device copies that broadcast a frame.  The binding of psm_set_stream is unchanged.  PSM_EINVAL for a null
+ * context. */
+int psm_wait_stream(psm_ctx* ctx, void* cuda_stream);
+int psm_signal_stream(psm_ctx* ctx, void* cuda_stream);
+
 /* Inputs: interleaved 3-channel float images (cv::Mat CV_32FC3, BGR, values in [0,1]) in HOST
  * memory, row steps in BYTES.  Copies H2D and builds planar channels + x-gradients
  * (CVC::preprocess, src/CVC.cpp:41-46) on the device.
@@ -324,6 +336,29 @@ int psm_set_images_u8(psm_ctx* ctx, const uint8_t* left, size_t left_step,
  * overwrite of them, against that stream (psm_set_stream, or events). */
 int psm_set_images_device(psm_ctx* ctx, const float* d_left, size_t left_step,
                           const float* d_right, size_t right_step);
+
+/* Sample types of psm_set_images_device_planes */
+enum { PSM_PIX_U8 = 1, PSM_PIX_F32 = 2 };
+
+/* Device frames in any 8-bit or float pixel layout (NVDEC / nvJPEG output, a tensor another model produced), read in
+ * place: no staging copy, no host wait.  left[c] / right[c] point at channel c of pixel (0, 0) in B, G, R order; sample
+ * (x, y) of channel c is at left[c] + y * row_step + x * col_step (bytes), in device memory of the context's (first)
+ * device.  elem = 1 (PSM_PIX_U8) or 4 (PSM_PIX_F32) bytes; plane = the byte offset between channel planes:
+ *   HWC BGR   p + 0, p + 1, p + 2 (times elem)   col_step 3 * elem
+ *   HWC RGB   p + 2, p + 1, p + 0 (times elem)   col_step 3 * elem
+ *   CHW RGB   p + 2 * plane, p + plane, p        col_step elem       (torchvision's decode_jpeg)
+ *   BGRA      p + 0, p + 1, p + 2 (times elem)   col_step 4 * elem
+ * The planes, gradients and guide flags equal those psm_set_images / _u8 build from the same sample values (u8 samples
+ * scaled by 1/255.0f as convertTo does), so every later result is the same bit for bit; float frames take the same
+ * flagged or unflagged filter route.  One ingest_planes_kernel launch and one halo pass per view; stage 0 times it.
+ *   - PSM_EINVAL before any CUDA call: a null array or channel pointer, an unknown pix_type, col_step < elem,
+ *     row_step < (W - 1) * col_step + elem, and for float samples a pointer or step that is not a multiple of 4.
+ *   - Asynchronous like psm_set_images_device: the kernels read the frames on the context's stream.  Order their
+ *     producer before the call with psm_wait_stream, and their next overwrite or free after it with psm_signal_stream.
+ *   - Multi-device contexts: the frames are read on the first device only; every other shard receives the first shard's
+ *     ingested planes device to device, ordered by events (DESIGN.md section 19). */
+int psm_set_images_device_planes(psm_ctx* ctx, int pix_type, const void* const left[3], const void* const right[3],
+                                 size_t row_step, size_t col_step);
 
 /* Pipelined upload (extension; the reference's DispEst is synchronous per frame): start the H2D copy
  * of the NEXT frame on the context's copy stream into a second staging set while the current frame
@@ -390,6 +425,16 @@ int psm_post_process(psm_ctx* ctx, uint8_t* left, size_t left_step, uint8_t* rig
 int psm_post_process_device(psm_ctx* ctx);
 /* Stage 4 on a u16 context: as psm_post_process with uint16_t maps (row steps in bytes). */
 int psm_post_process_u16(psm_ctx* ctx, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step);
+
+/* Both maps into caller DEVICE buffers (row steps in bytes, at least W * map bytes), device to device on the context's
+ * stream, asynchronous, in the context's map format (uint8_t, or uint16_t on a 16-bit context).  which = 0: the maps of
+ * the last selection stage (psm_device_ptr selectors 2 / 3; a fused-exchange context's complete maps, as
+ * psm_disp_fetch_p2p copies them); which = 1: the post-processed maps (selectors 4 / 5).  A multi-device context copies
+ * the first shard's.  d_right must be NULL on a left-only context and is required otherwise.
+ *   - PSM_EINVAL before any CUDA call: which not 0 / 1, a null pointer or a step below a row.
+ *   - PSM_ESTATE: no selection (which = 0) or post-process (which = 1) since the context was created or PSM_OPT_VIEWS
+ *     last changed, and under the exchanged-map rules of psm_disp_fetch_p2p. */
+int psm_copy_maps_device(psm_ctx* ctx, int which, void* d_left, size_t left_step, void* d_right, size_t right_step);
 
 /* Sharded stage 3a: per-pixel packed minima over this context's slices, written to DEVICE
  * buffers of H*W uint64 each:  key = (order_preserving_u32(cost) << 32) | global_d.

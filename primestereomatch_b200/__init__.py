@@ -7,3 +7,11 @@ from .dispest import DispEst, device_count, MAX_CPU_THREADS, OCV_DE, OCL_DE  # n
 from . import capi, synth  # noqa: F401
 
 __all__ = ["DispEst", "device_count", "capi", "synth"]
+
+
+def __getattr__(name):
+    # TorchStereo imports torch: only on first use, so the numpy facade never pays for it
+    if name == "TorchStereo":
+        from .torch_stereo import TorchStereo
+        return TorchStereo
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -22,7 +22,8 @@ SYMBOLS = [
     "psm_launch_count", "psm_sync", "psm_last_error", "psm_build_info", "psm_cvf_plan", "psm_set_guided_filter",
     "psm_set_matching_cost", "psm_set_post_filter", "psm_create_u16", "psm_disp_select_u16", "psm_disp_select_u16_async",
     "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
-    "psm_create_blocked", "psm_create_multi",
+    "psm_create_blocked", "psm_create_multi", "psm_set_images_device_planes", "psm_wait_stream", "psm_signal_stream",
+    "psm_copy_maps_device",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -33,6 +34,7 @@ PSM_VIEWS_LEFT, PSM_VIEWS_BOTH = 1, 2
 PSM_CVF_EXACT, PSM_CVF_MIXED, PSM_CVF_NAIVE = 0, 1, 2
 PSM_WMF_EXP, PSM_WMF_IV1, PSM_WMF_IV2, PSM_WMF_OFF = 0, 1, 2, 5
 PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL = 0, 1, 2
+PSM_PIX_U8, PSM_PIX_F32 = 1, 2
 
 _lib = None
 
@@ -77,6 +79,10 @@ def lib():
     L.psm_set_images.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_u8.argtypes = [vp, u8p, sz, u8p, sz]
     L.psm_set_images_device.argtypes = [vp, fp, sz, fp, sz]
+    L.psm_set_images_device_planes.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), sz, sz]
+    L.psm_wait_stream.argtypes = [vp, vp]
+    L.psm_signal_stream.argtypes = [vp, vp]
+    L.psm_copy_maps_device.argtypes = [vp, i, vp, sz, vp, sz]
     L.psm_set_images_async.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_u8_async.argtypes = [vp, u8p, sz, u8p, sz]
     L.psm_set_images_commit.argtypes = [vp]

@@ -116,6 +116,9 @@ struct psm_ctx {
     bool views_reset = false;
     unsigned p2p_seq_right = 0;                // frames whose exchange included the right view (p2p_seq counts every frame)
     bool p2p_right_current = false;            // the last frame's exchange included the right view
+    bool have_pp = false;                      // dis_pp holds the maps of a post-process since the last PSM_OPT_VIEWS change
+    cudaEvent_t ev_user = nullptr;             // psm_wait_stream: the caller's stream, recorded
+    cudaEvent_t ev_signal[2] = {nullptr, nullptr};  // psm_signal_stream: the compute and the copy stream, recorded
     uint64_t launches = 0;
     char err[512] = "";
 };
@@ -215,6 +218,16 @@ int pad_rows(psm_ctx* c, float* base, size_t nrows)
 
 void* stage_buf(psm_ctx* c, int set, int view) { return set ? c->stage_alt[view] : c->stage_in[view]; }
 
+// a new frame's planes are (being) written: every stage after ingest starts again
+void images_ingested(psm_ctx* c, bool float_images)
+{
+    c->have_images = true;
+    c->float_images = float_images;   // u8 images lie in {0} U [1/255, 1]: they never raise an ingest flag
+    c->guide_valid = false;
+    c->have_cvc = false;
+    c->filtered = false;
+}
+
 template <typename T>
 int ingest(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool from_device)
 {
@@ -253,11 +266,60 @@ int ingest(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool 
         c->ingest_done_valid[set] = true;
         PSM_CUDA(c, cudaEventSynchronize(c->host_copied));
     }
-    c->have_images = true;
-    c->float_images = sizeof(T) != 1;   // u8 images lie in {0} U [1/255, 1]: they never raise an ingest flag
-    c->guide_valid = false;
-    c->have_cvc = false;
-    c->filtered = false;
+    images_ingested(c, sizeof(T) != 1);
+    return PSM_OK;
+}
+
+// psm_set_images_device_planes: the caller's two frames and their layout -> src, or PSM_EINVAL before any CUDA call
+int check_planes(psm_ctx* c, int pix_type, const void* const left[3], const void* const right[3], size_t row_step,
+                 size_t col_step, PlanesSrc src[2])
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (pix_type != PSM_PIX_U8 && pix_type != PSM_PIX_F32)
+        return fail(c, PSM_EINVAL, "unknown pixel type %d (PSM_PIX_U8 = 1, PSM_PIX_F32 = 2)", pix_type);
+    const size_t elem = pix_type == PSM_PIX_U8 ? 1 : sizeof(float);
+    const void* const* ch[2] = {left, right};
+    for (int v = 0; v < 2; ++v) {
+        if (!ch[v]) return fail(c, PSM_EINVAL, "null channel pointer array for view %d", v);
+        for (int k = 0; k < 3; ++k) {
+            if (!ch[v][k]) return fail(c, PSM_EINVAL, "null pointer for channel %d of view %d", k, v);
+            if ((uintptr_t)ch[v][k] % elem)
+                return fail(c, PSM_EINVAL, "channel %d of view %d is not aligned to the %zu bytes of a float sample", k, v, elem);
+            src[v].ch[k] = static_cast<const char*>(ch[v][k]);
+        }
+        src[v].row_step = row_step;
+        src[v].col_step = col_step;
+    }
+    if (col_step < elem) return fail(c, PSM_EINVAL, "col_step %zu is below the %zu bytes of one sample", col_step, elem);
+    const size_t span = (size_t)(c->W - 1);
+    if ((span && col_step > (SIZE_MAX - elem) / span) || row_step < span * col_step + elem)
+        return fail(c, PSM_EINVAL, "row_step %zu is below the (W - 1) * col_step + %zu bytes a row of W = %d spans", row_step,
+                    elem, c->W);
+    if (row_step % elem || col_step % elem)
+        return fail(c, PSM_EINVAL, "row_step %zu / col_step %zu are not multiples of the %zu bytes of a float sample",
+                    row_step, col_step, elem);
+    return PSM_OK;
+}
+
+// the caller's frame, read in place by ingest_planes_kernel on the context's stream (one launch and pad_rows per view)
+int ingest_planes(psm_ctx* c, bool u8, const PlanesSrc src[2])
+{
+    PSM_CUDA(c, cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
+    for (int v = 0; v < 2; ++v) {
+        float* g = c->guide[v];
+        dim3 blk(128), grd((c->W + 3 + 127) / 128, c->H);
+        if (u8)
+            ingest_planes_kernel<uint8_t><<<grd, blk, 0, c->stream>>>(src[v], c->W, c->H, c->Wp, g, g + c->plane,
+                                                                       g + 2 * c->plane, c->grd[v], c->gray_mode,
+                                                                       c->guide_flags + v);
+        else
+            ingest_planes_kernel<float><<<grd, blk, 0, c->stream>>>(src[v], c->W, c->H, c->Wp, g, g + c->plane,
+                                                                     g + 2 * c->plane, c->grd[v], c->gray_mode,
+                                                                     c->guide_flags + v);
+        PSM_LAUNCH_CHECK(c);
+        if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
+    }
+    images_ingested(c, !u8);
     return PSM_OK;
 }
 
@@ -749,6 +811,51 @@ int multi_set_images(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rs
     return PSM_OK;
 }
 
+// psm_set_images_device_planes on a multi-device context.  The first shard ingests the caller's frame; every other
+// shard copies what that ingest wrote (the three channel planes with their mirrored halos, the gradient planes and the
+// ingest flags, byte for byte) device to device on its own stream, so the caller's buffers are read on the first device
+// only and every shard holds the planes its own ingest would have written.  The broadcast's readers and writers:
+//   - shard k's copy follows the first shard's ingest (ev_images) and, on its own stream, shard k's earlier work, which
+//     reads the planes the copy overwrites;
+//   - the first shard's later work (its next ingest, and the guide precompute, which adds to the flags) follows every
+//     copy (ev_copied), and so does whatever orders itself after the first shard's stream (psm_signal_stream).
+int multi_set_planes(psm_ctx* c, bool u8, const PlanesSrc src[2])
+{
+    psm_ctx* s0 = c->shard[0];
+    int rc = bind(s0);
+    if (!rc) rc = stage_begin(s0, 0);
+    if (!rc) rc = ingest_planes(s0, u8, src);
+    if (!rc) rc = stage_end(s0, 0);
+    if (rc) return relay(c, 0, rc);
+    PSM_CUDA(c, cudaEventRecord(c->ev_images, s0->stream));
+    for (int k = 1; k < c->nshards; ++k) {
+        psm_ctx* s = c->shard[k];
+        if ((rc = bind(s))) return relay(c, k, rc);
+        PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_images, 0));
+        if ((rc = stage_begin(s, 0))) return relay(c, k, rc);
+        for (int v = 0; v < 2; ++v) {   // from the first row's left halo: 3 channel planes, then the gradient plane
+            PSM_CUDA(c, cudaMemcpyAsync(s->guide[v] - kPadLeft, s0->guide[v] - kPadLeft, 3 * s0->plane * sizeof(float),
+                                        cudaMemcpyDefault, s->stream));
+            PSM_CUDA(c, cudaMemcpyAsync(s->grd[v] - kPadLeft, s0->grd[v] - kPadLeft, s0->plane * sizeof(float),
+                                        cudaMemcpyDefault, s->stream));
+        }
+        PSM_CUDA(c, cudaMemcpyAsync(s->guide_flags, s0->guide_flags, 2 * sizeof(int), cudaMemcpyDefault, s->stream));
+        PSM_CUDA(c, cudaEventRecord(c->ev_copied[k], s->stream));
+        PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_copied[k], 0));
+        images_ingested(s, !u8);
+        if ((rc = stage_end(s, 0))) return relay(c, k, rc);
+    }
+    return PSM_OK;
+}
+
+// the contexts whose streams carry a context's work: the shards of a multi-device context, or the context itself
+int ctx_parts(psm_ctx* c, psm_ctx** parts)
+{
+    if (!is_multi(c)) { parts[0] = c; return 1; }
+    for (int k = 0; k < c->nshards; ++k) parts[k] = c->shard[k];
+    return c->nshards;
+}
+
 }  // namespace
 
 // ----------------------------------------------------------------------------------------------
@@ -840,6 +947,8 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
     PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->up_done, cudaEventDisableTiming));
     PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->host_copied, cudaEventDisableTiming));
     for (int k = 0; k < 2; ++k) PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->ingest_done[k], cudaEventDisableTiming));
+    PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->ev_user, cudaEventDisableTiming));
+    for (int k = 0; k < 2; ++k) PSM_CREATE_CUDA(cudaEventCreateWithFlags(&c->ev_signal[k], cudaEventDisableTiming));
     for (int s = 0; s < kNumStages; ++s) {
         PSM_CREATE_CUDA(cudaEventCreate(&c->ev0[s]));
         PSM_CREATE_CUDA(cudaEventCreate(&c->ev1[s]));
@@ -1021,6 +1130,8 @@ int psm_destroy(psm_ctx* c)
     if (c->up_done) cudaEventDestroy(c->up_done);
     if (c->host_copied) cudaEventDestroy(c->host_copied);
     for (int k = 0; k < 2; ++k) if (c->ingest_done[k]) cudaEventDestroy(c->ingest_done[k]);
+    if (c->ev_user) cudaEventDestroy(c->ev_user);
+    for (int k = 0; k < 2; ++k) if (c->ev_signal[k]) cudaEventDestroy(c->ev_signal[k]);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaFree(c->slice_flags);
     cudaFree(c->ref_rs);
@@ -1062,6 +1173,7 @@ int psm_set_option(psm_ctx* c, int key, int value)
             c->have_cvc = false;
             c->filtered = false;
             c->have_maps = false;
+            c->have_pp = false;
             c->lr_masks_ok = false;
         }
         return PSM_OK;
@@ -1200,6 +1312,55 @@ int psm_set_images_device(psm_ctx* c, const float* d_left, size_t left_step, con
     if (int rc = stage_begin(c, 0)) return rc;
     if (int rc = ingest<float>(c, d_left, left_step, d_right, right_step, true)) return rc;
     return stage_end(c, 0);
+}
+
+int psm_set_images_device_planes(psm_ctx* c, int pix_type, const void* const left[3], const void* const right[3],
+                                 size_t row_step, size_t col_step)
+{
+    PlanesSrc src[2];
+    if (int rc = check_planes(c, pix_type, left, right, row_step, col_step, src)) return rc;
+    const bool u8 = pix_type == PSM_PIX_U8;
+    if (is_multi(c)) return multi_set_planes(c, u8, src);
+    if (int rc = bind(c)) return rc;
+    if (int rc = stage_begin(c, 0)) return rc;
+    if (int rc = ingest_planes(c, u8, src)) return rc;
+    return stage_end(c, 0);
+}
+
+// Events only: the caller's stream is recorded once (on the context's first device) and every stream of the context
+// waits for that record.
+int psm_wait_stream(psm_ctx* c, void* cuda_stream)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    psm_ctx* parts[kMaxRanks];
+    const int n = ctx_parts(c, parts);
+    if (int rc = bind(parts[0])) return rc;
+    PSM_CUDA(c, cudaEventRecord(parts[0]->ev_user, static_cast<cudaStream_t>(cuda_stream)));
+    for (int k = 0; k < n; ++k) {
+        if (int rc = bind(parts[k])) return rc;
+        PSM_CUDA(c, cudaStreamWaitEvent(parts[k]->stream, parts[0]->ev_user, 0));
+        PSM_CUDA(c, cudaStreamWaitEvent(parts[k]->copy_stream, parts[0]->ev_user, 0));
+    }
+    return PSM_OK;
+}
+
+// Events only: every stream of the context is recorded and the caller's stream waits for each record.
+int psm_signal_stream(psm_ctx* c, void* cuda_stream)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    psm_ctx* parts[kMaxRanks];
+    const int n = ctx_parts(c, parts);
+    const cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
+    for (int k = 0; k < n; ++k) {
+        psm_ctx* p = parts[k];
+        if (int rc = bind(p)) return rc;
+        PSM_CUDA(c, cudaEventRecord(p->ev_signal[0], p->stream));
+        PSM_CUDA(c, cudaEventRecord(p->ev_signal[1], p->copy_stream));
+    }
+    if (int rc = bind(parts[0])) return rc;   // the caller's stream lives on the first device
+    for (int k = 0; k < n; ++k)
+        for (int e = 0; e < 2; ++e) PSM_CUDA(c, cudaStreamWaitEvent(s, parts[k]->ev_signal[e], 0));
+    return PSM_OK;
 }
 
 int psm_set_images_async(psm_ctx* c, const float* left, size_t left_step, const float* right, size_t right_step)
@@ -1927,7 +2088,9 @@ int psm_post_process_device(psm_ctx* c)
         return PSM_OK;
     }
     if (int rc = bind(c)) return rc;
-    return c->map_bytes == 2 ? post_process_maps<uint16_t>(c) : post_process_maps<uint8_t>(c);
+    const int rc = c->map_bytes == 2 ? post_process_maps<uint16_t>(c) : post_process_maps<uint8_t>(c);
+    if (!rc) c->have_pp = true;
+    return rc;
 }
 
 int psm_post_process(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step)
@@ -1938,6 +2101,41 @@ int psm_post_process(psm_ctx* c, uint8_t* left, size_t left_step, uint8_t* right
 int psm_post_process_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step)
 {
     return post_process(c, left, left_step, right, right_step);
+}
+
+int psm_copy_maps_device(psm_ctx* c, int which, void* d_left, size_t left_step, void* d_right, size_t right_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (which != 0 && which != 1)
+        return fail(c, PSM_EINVAL, "psm_copy_maps_device: which %d is neither 0 (selection maps) nor 1 (post-processed maps)", which);
+    const size_t row = (size_t)c->W * c->map_bytes;
+    if (!d_left || left_step < row)
+        return fail(c, PSM_EINVAL, "psm_copy_maps_device: bad left map pointer/step (a row of %d-bit maps is %zu bytes)",
+                    8 * c->map_bytes, row);
+    if (int rc = check_right_arg(c, d_right, "psm_copy_maps_device")) return rc;
+    if (c->views == 2 && (!d_right || right_step < row))
+        return fail(c, PSM_EINVAL, "psm_copy_maps_device: bad right map pointer/step (a row of %d-bit maps is %zu bytes)",
+                    8 * c->map_bytes, row);
+    // a multi-device context's maps are the first shard's (its exchange block, and its post-filter's outputs)
+    if (is_multi(c)) return relay(c, 0, psm_copy_maps_device(c->shard[0], which, d_left, left_step, d_right, right_step));
+    if (int rc = bind(c)) return rc;
+    if (int rc = check_views_reset(c, "psm_copy_maps_device")) return rc;
+    const bool exchanged = c->p2p_own && c->p2p_seq > 0;
+    if (which == 0) {
+        if (!c->have_maps && !exchanged) return fail(c, PSM_ESTATE, "psm_copy_maps_device before a disparity-selection stage");
+        if (exchanged) {   // the rules of psm_disp_fetch_p2p
+            if (int rc = check_p2p_right_map(c, "psm_copy_maps_device")) return rc;
+            if (int rc = p2p_wait_done(c)) return rc;
+        }
+    } else if (!c->have_pp) {
+        return fail(c, PSM_ESTATE, "psm_copy_maps_device of the post-processed maps before a post-process");
+    }
+    void* dst[2] = {d_left, d_right};
+    const size_t step[2] = {left_step, right_step};
+    for (int v = 0; v < c->views; ++v)
+        PSM_CUDA(c, cudaMemcpy2DAsync(dst[v], step[v], which ? c->dis_pp[v] : current_map(c, v), row, row, c->H,
+                                      cudaMemcpyDefault, c->stream));
+    return PSM_OK;
 }
 
 static int check_slice(psm_ctx* c, int view, int d)

@@ -54,12 +54,26 @@ constexpr int kGuideInexact = 4;     // a nonzero channel value lies outside [2^
 __device__ __forceinline__ float to_f32(float v) { return v; }
 __device__ __forceinline__ float to_f32(uint8_t v) { return fmul((float)v, 1 / 255.0f); }
 
+// gray of one pixel's channels c0, c1, c2 (B, G, R) in either PSM_OPT_GRAY_MODE
+__device__ __forceinline__ float gray_of(float c0, float c1, float c2, int gray_mode)
+{
+    if (gray_mode == 0) return __fmaf_rn(c2, 0.114f, __fmaf_rn(c0, 0.299f, fmul(c1, 0.587f)));
+    return fadd(fadd(fmul(c0, 0.299f), fmul(c1, 0.587f)), fmul(c2, 0.114f));
+}
+
 template <typename T>
 __device__ __forceinline__ float gray_at(const T* __restrict__ row, int x, int gray_mode)
 {
-    const float c0 = to_f32(row[3 * x]), c1 = to_f32(row[3 * x + 1]), c2 = to_f32(row[3 * x + 2]);
-    if (gray_mode == 0) return __fmaf_rn(c2, 0.114f, __fmaf_rn(c0, 0.299f, fmul(c1, 0.587f)));
-    return fadd(fadd(fmul(c0, 0.299f), fmul(c1, 0.587f)), fmul(c2, 0.114f));
+    return gray_of(to_f32(row[3 * x]), to_f32(row[3 * x + 1]), to_f32(row[3 * x + 2]), gray_mode);
+}
+
+// the guide flags one pixel's channel values raise (see ingest_kernel)
+__device__ __forceinline__ void ingest_flags(float v0, float v1, float v2, int* __restrict__ guide_flag)
+{
+    const unsigned u0 = __float_as_uint(v0), u1 = __float_as_uint(v1), u2 = __float_as_uint(v2);
+    if (max(max(u0, u1), u2) >= 0x5e000000u) atomicOr(guide_flag, kGuideOutside | kGuideInexact);
+    auto inexact = [](unsigned u) { return u != 0u && u - 0x39800000u > 0x3f800000u - 0x39800000u; };   // outside {0} U [2^-12, 1]
+    if (inexact(u0) || inexact(u1) || inexact(u2)) atomicOr(guide_flag, kGuideInexact);
 }
 
 template <typename T>
@@ -86,12 +100,43 @@ __global__ void ingest_kernel(const T* __restrict__ src, size_t step_bytes, int 
     // nonzero value lies in [2^-12, 1]: a product is then 0 or at least 2^-24, a multiple of 2^-47, and a sum of at most
     // 64 such values in [0, 64] needs at most 53 bits.  Any other nonzero value raises kGuideInexact and the guide is
     // recomputed in OpenCV's order (psm_cvf_ref.cuh).  u8 images (0 or 1/255 .. 1) never raise it.
-    const unsigned u0 = __float_as_uint(v0), u1 = __float_as_uint(v1), u2 = __float_as_uint(v2);
-    if (max(max(u0, u1), u2) >= 0x5e000000u) atomicOr(guide_flag, kGuideOutside | kGuideInexact);
-    auto inexact = [](unsigned u) { return u != 0u && u - 0x39800000u > 0x3f800000u - 0x39800000u; };   // outside {0} U [2^-12, 1]
-    if (inexact(u0) || inexact(u1) || inexact(u2)) atomicOr(guide_flag, kGuideInexact);
+    ingest_flags(v0, v1, v2, guide_flag);
     const float gr = gray_at(row, reflect101(x + 1, W), gray_mode);
     const float gl = gray_at(row, reflect101(x - 1, W), gray_mode);
+    grd[o] = fsub(gr, gl);
+}
+
+// A frame given as three channel pointers (B, G, R) and byte steps (psm_set_images_device_planes): sample (x, y) of
+// channel c at ch[c] + y * row_step + x * col_step.  HWC BGR / RGB, BGRA and planar CHW frames all fit.
+struct PlanesSrc {
+    const char* ch[3];
+    size_t row_step, col_step;
+};
+
+// What ingest_kernel<T> writes for an interleaved frame holding the same sample values, from any PlanesSrc layout:
+// the three planes, the flags and the gradient of the gray image, the same operations in the same order.
+template <typename T>
+__global__ void ingest_planes_kernel(PlanesSrc src, int W, int H, int Wp,
+                                     float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
+                                     float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y;
+    if (x >= ((W + 3) & ~3) || y >= H) return;
+    const size_t o = (size_t)y * Wp + x;
+    if (x >= W) { I0[o] = 0.f; I1[o] = 0.f; I2[o] = 0.f; grd[o] = 0.f; return; }
+    const size_t row = (size_t)y * src.row_step;
+    auto sample = [&](int c, int xx) {
+        return to_f32(*reinterpret_cast<const T*>(src.ch[c] + row + (size_t)xx * src.col_step));
+    };
+    const float v0 = sample(0, x), v1 = sample(1, x), v2 = sample(2, x);
+    I0[o] = v0;
+    I1[o] = v1;
+    I2[o] = v2;
+    ingest_flags(v0, v1, v2, guide_flag);
+    const int xr = reflect101(x + 1, W), xl = reflect101(x - 1, W);
+    const float gr = gray_of(sample(0, xr), sample(1, xr), sample(2, xr), gray_mode);
+    const float gl = gray_of(sample(0, xl), sample(1, xl), sample(2, xl), gray_mode);
     grd[o] = fsub(gr, gl);
 }
 

@@ -28,6 +28,35 @@ def _ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def resolve_map_bits(max_disp, map_bits):
+    """map_bits None -> 8-bit maps for max_disp <= 256, 16-bit above; 8 and 16 stay.  Raises ValueError otherwise."""
+    if map_bits not in (None, 8, 16):
+        raise ValueError(f"map_bits must be None, 8 or 16 (got {map_bits!r})")
+    return map_bits if map_bits is not None else (16 if max_disp > 256 else 8)
+
+
+def create_context(width, height, max_disp, map_bits, *, device=0, d_begin=0, d_count=None, block_slices=None,
+                   devices=None):
+    """The context DispEst and TorchStereo run on, as a c_void_p handle (psm_destroy frees it): a multi-device context
+    over `devices` (psm_create_multi, block_slices blocks every shard), a blocked context (psm_create_blocked), or one of
+    [d_begin, d_begin + d_count) on `device` with map_bits-bit maps (psm_create_u16 / psm_create_sharded)."""
+    L = capi.lib()
+    ctx = C.c_void_p()
+    dc = max_disp - d_begin if d_count is None else d_count
+    if devices is not None:
+        devs = [int(x) for x in devices]
+        arr = (C.c_int * max(1, len(devs)))(*devs)
+        capi.check(L.psm_create_multi(C.byref(ctx), width, height, max_disp, arr, len(devs), int(block_slices or 0),
+                                      map_bits))
+    elif block_slices is not None:
+        capi.check(L.psm_create_blocked(C.byref(ctx), width, height, max_disp, int(d_begin), int(dc), int(block_slices),
+                                        map_bits, int(device)))
+    else:
+        create = L.psm_create_u16 if map_bits == 16 else L.psm_create_sharded
+        capi.check(create(C.byref(ctx), width, height, max_disp, int(d_begin), int(dc), int(device)))
+    return ctx
+
+
 class DispEst:
     """DispEst(l, r, d, t, ocl) -- reference src/DispEst.cpp:10-143.
 
@@ -54,9 +83,7 @@ class DispEst:
             raise ValueError("DispEst expects HxWx3 float32 or uint8 images")
         self.hei, self.wid = int(l.shape[0]), int(l.shape[1])
         self.maxDis = int(d)
-        if map_bits not in (None, 8, 16):
-            raise ValueError(f"map_bits must be None, 8 or 16 (got {map_bits!r})")
-        self.map_bits = map_bits if map_bits is not None else (16 if self.maxDis > 256 else 8)
+        self.map_bits = resolve_map_bits(self.maxDis, map_bits)
         mdt = np.uint16 if self.map_bits == 16 else np.uint8
         self.threads = int(t)
         self.useOCL = bool(ocl)
@@ -72,20 +99,9 @@ class DispEst:
         self._ctx = C.c_void_p()
         self._lib = None
         if self.useOCL:
-            L = capi.lib()
-            self._lib = L
-            dc = self.maxDis - d_begin if d_count is None else d_count
-            if devices is not None:
-                devs = [int(x) for x in devices]
-                arr = (C.c_int * max(1, len(devs)))(*devs)
-                capi.check(L.psm_create_multi(C.byref(self._ctx), self.wid, self.hei, self.maxDis, arr, len(devs),
-                                              int(block_slices or 0), self.map_bits))
-            elif block_slices is not None:
-                capi.check(L.psm_create_blocked(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc),
-                                                int(block_slices), self.map_bits, int(device)))
-            else:
-                create = L.psm_create_u16 if self.map_bits == 16 else L.psm_create_sharded
-                capi.check(create(C.byref(self._ctx), self.wid, self.hei, self.maxDis, int(d_begin), int(dc), int(device)))
+            self._lib = capi.lib()
+            self._ctx = create_context(self.wid, self.hei, self.maxDis, self.map_bits, device=device, d_begin=d_begin,
+                                       d_count=d_count, block_slices=block_slices, devices=devices)
         self.d_begin, self.d_count = d_begin, (self.maxDis - d_begin if d_count is None else d_count)
         self.block_slices = None if devices is not None and not block_slices else block_slices   # 0: unblocked shards
         self.devices = None if devices is None else list(devices)

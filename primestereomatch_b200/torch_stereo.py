@@ -1,0 +1,187 @@
+"""PyTorch interface: stereo frames that are already CUDA tensors in, disparity maps as CUDA tensors out.
+
+`TorchStereo` runs the same contexts as `DispEst` (one device, blocked, or several devices) on frames in GPU memory --
+NVDEC / nvJPEG output, `torchvision.io.decode_jpeg(..., device="cuda")`, another model's tensor -- in any of the layouts
+`psm_set_images_device_planes` reads in place: HWC BGR / RGB, BGRA / RGBA and planar CHW, 8-bit or float, any row
+stride.  `match` orders itself against torch's current stream with events (psm_wait_stream / psm_signal_stream) and
+never waits on the host, so the frames and maps stay in the caller's stream order.  The maps equal, bit for bit, those of
+the host upload of the same pixels.  Importing this module imports torch; the package imports it only on first use.
+"""
+import ctypes as C
+
+import torch
+
+from . import capi
+from .dispest import DispEst, create_context, resolve_map_bits
+
+_PIX = {torch.uint8: capi.PSM_PIX_U8, torch.float32: capi.PSM_PIX_F32}
+_ORDER = {"bgr": (0, 1, 2), "rgb": (2, 1, 0)}   # the tensor channel that holds B, G and R
+
+
+def frame_layout(t, height, width, channels="bgr"):
+    """The psm_set_images_device_planes arguments of a frame tensor, or of each frame of a batch.
+
+    t: uint8 or float32, shaped (H, W, C) with C = 3 or 4 (the fourth channel, alpha, is not read), (3, H, W), or either
+    with a leading batch dimension; (H, W, C) is taken when both fit.  channels: "bgr" or "rgb", the order of the first
+    three channels.  -> (pix_type, [(B, G, R) byte addresses] per frame, row_step, col_step, batched).  Raises TypeError
+    or ValueError on anything the layout cannot express (a column stride of 0, rows that overlap, other shapes); the
+    tensor's device is not looked at."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"expected a torch.Tensor (got {type(t).__name__})")
+    if t.dtype not in _PIX:
+        raise TypeError(f"frames must be uint8 or float32 tensors (got {t.dtype})")
+    if channels not in _ORDER:
+        raise ValueError(f'channels must be "bgr" or "rgb" (got {channels!r})')
+    if t.dim() not in (3, 4):
+        raise ValueError(f"frames must be (H, W, C), (3, H, W) or batches of them (got shape {tuple(t.shape)})")
+    shape, strides = tuple(t.shape[-3:]), tuple(t.stride()[-3:])
+    if shape[:2] == (height, width) and shape[2] in (3, 4):
+        sr, sc, sch = strides
+    elif shape == (3, height, width):
+        sch, sr, sc = strides
+    else:
+        raise ValueError(f"frames must be ({height}, {width}, 3 or 4) or (3, {height}, {width}), optionally with a leading "
+                         f"batch dimension (got shape {tuple(t.shape)})")
+    elem = t.element_size()
+    row_step, col_step = sr * elem, sc * elem
+    if sc < 1:
+        raise ValueError(f"the column stride is {sc} elements: pixels of a row must not share samples")
+    if row_step < (width - 1) * col_step + elem:
+        raise ValueError(f"the row stride ({sr} elements) is shorter than a row ({width} pixels {sc} elements apart)")
+    batched = t.dim() == 4
+    n, bstride = (t.shape[0], t.stride(0) * elem) if batched else (1, 0)
+    if n < 1:
+        raise ValueError("empty batch")
+    base = t.data_ptr()
+    order = _ORDER[channels]
+    frames = [tuple(base + b * bstride + order[c] * sch * elem for c in range(3)) for b in range(n)]
+    return _PIX[t.dtype], frames, row_step, col_step, batched
+
+
+class TorchStereo:
+    """TorchStereo(width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None)
+
+    The context `DispEst` creates for the same arguments: `device` (an index, "cuda:k" or torch.device; None = the
+    current device), `map_bits` (None: 8-bit maps up to max_disp 256, 16-bit above), `block_slices` (a blocked context),
+    `devices` (a multi-device context whose frames and maps live on devices[0]).  The setters pass their values straight
+    to the C-ABI, which rejects bad ones with PsmError."""
+
+    def __init__(self, width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None):
+        self.width, self.height, self.max_disp = int(width), int(height), int(max_disp)
+        self.map_bits = resolve_map_bits(self.max_disp, map_bits)
+        if devices is not None:
+            index = int(devices[0]) if len(devices) else 0
+        else:
+            dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device or "cuda")
+            index = dev.index if dev.index is not None else torch.cuda.current_device()
+        self.device = torch.device("cuda", index)
+        self.subsample_rate = 4
+        self.views = capi.PSM_VIEWS_BOTH
+        self._lib = capi.lib()
+        self._ctx = C.c_void_p()
+        self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
+                                   block_slices=block_slices, devices=devices)
+
+    # -- lifetime ---------------------------------------------------------------------------
+    def close(self):
+        if self._ctx:
+            self._lib.psm_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    @property
+    def handle(self):
+        return self._ctx
+
+    # -- settings (the C-ABI judges every value) ---------------------------------------------
+    def _check(self, rc):
+        capi.check(rc, self._ctx)
+
+    def setGuidedFilter(self, window, eps):
+        self._check(self._lib.psm_set_guided_filter(self._ctx, int(window), float(eps)))
+
+    def setMatchingCost(self, alpha, tau_color, tau_grad):
+        self._check(self._lib.psm_set_matching_cost(self._ctx, float(alpha), float(tau_color), float(tau_grad)))
+
+    def setPostFilter(self, radius, sigma=25.5, iterations=1, weight="exp"):
+        wt = DispEst._WMF_WEIGHTS.get(weight, -1) if isinstance(weight, str) else -1
+        self._check(self._lib.psm_set_post_filter(self._ctx, int(radius), float(sigma), int(iterations), wt))
+
+    def setLRCheck(self, mode):
+        self._check(self._lib.psm_set_lr_check(self._ctx, int(mode)))
+
+    def setViews(self, views):
+        value = DispEst._VIEWS.get(views, -1) if isinstance(views, str) else -1
+        self._check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_VIEWS, value))
+        self.views = value
+
+    def setSubsampleRate(self, rate):
+        """The Fast Guided Filter's sub-sampling rate for match(..., fgf=True); psm_cost_filter_fgf judges it."""
+        self.subsample_rate = int(rate)
+
+    # -- frames -------------------------------------------------------------------------------
+    def _layout(self, left, right, channels):
+        """Both frames' layout, checked in full before any device work."""
+        pix, lf, row_step, col_step, batched = frame_layout(left, self.height, self.width, channels)
+        other = frame_layout(right, self.height, self.width, channels)
+        if left.shape != right.shape or left.dtype != right.dtype or (pix, row_step, col_step) != (other[0], other[2], other[3]):
+            raise ValueError("left and right must have the same shape, dtype and strides")
+        for name, t in (("left", left), ("right", right)):
+            if t.device != self.device:
+                raise ValueError(f"{name} is on {t.device}: frames must be CUDA tensors on the context's device {self.device}")
+        return pix, lf, other[1], row_step, col_step, batched
+
+    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False):
+        """Disparity maps of one frame pair or a batch -> (lmap, rmap): new uint8 / uint16 tensors of shape (H, W) or
+        (B, H, W) on the context's device; rmap is None on a left-only context.
+
+        After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
+        (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
+        with post_process=True, and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
+        host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
+        pix, lf, rf, row_step, col_step, batched = self._layout(left, right, channels)
+        L, ctx = self._lib, self._ctx
+        H, W = self.height, self.width
+        mdt = torch.uint16 if self.map_bits == 16 else torch.uint8
+        shape = (len(lf), H, W) if batched else (H, W)
+        stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        lmap = torch.empty(shape, dtype=mdt, device=self.device)
+        rmap = torch.empty(shape, dtype=mdt, device=self.device) if self.views == capi.PSM_VIEWS_BOTH else None
+        row = W * lmap.element_size()
+        self._check(L.psm_wait_stream(ctx, stream))
+        for b in range(len(lf)):
+            lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
+            self._check(L.psm_set_images_device_planes(ctx, pix, lp, rp, row_step, col_step))
+            self._check(L.psm_cost_const(ctx))
+            self._check(L.psm_cost_filter_fgf(ctx, self.subsample_rate) if fgf else L.psm_cost_filter(ctx))
+            self._check(L.psm_disp_select_device(ctx))
+            if post_process:
+                self._check(L.psm_post_process_device(ctx))
+            lm = lmap[b] if batched else lmap
+            rm = None if rmap is None else (rmap[b] if batched else rmap)
+            self._check(L.psm_copy_maps_device(ctx, 1 if post_process else 0, lm.data_ptr(), row,
+                                               None if rm is None else rm.data_ptr(), row))
+        self._check(L.psm_signal_stream(ctx, stream))
+        return lmap, rmap
+
+    # -- measurement helpers ------------------------------------------------------------------
+    def stage_ms(self, stage):
+        ms = C.c_float()
+        self._check(self._lib.psm_stage_ms(self._ctx, stage, C.byref(ms)))
+        return ms.value
+
+    def launch_count(self):
+        n = C.c_uint64()
+        self._check(self._lib.psm_launch_count(self._ctx, C.byref(n)))
+        return n.value
