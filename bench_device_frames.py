@@ -12,9 +12,10 @@ stream synchronised).  Every round runs one frame of each arm in turn, so drift 
 frames/s is 1000 over the median frame time, and stage 0 (ingest) the median of psm_stage_ms(0).  Workloads:
 1920 x 1080 at D = 128 and 450 x 375 at D = 64 on the synthetic pair of bench.py (synth.stereo_pair_u8).  Before the line
 is printed every arm's maps must equal arm a's.  "ingest_kernels_ms" times the ingest alone (stage 0, median over
---steps calls on one context with nothing else queued): ingest_kernel on interleaved device frames (f32 through
+--steps calls on one context with nothing else queued), by entry point: interleaved frames (f32 through
 psm_set_images_device, u8 through psm_set_images_u8_async after its upload has finished, then psm_set_images_commit)
-against ingest_planes_kernel on the same pixels as HWC BGR u8 / f32 and CHW RGB u8 tensors.  The GPU name and power limit are read in the same run.
+and psm_set_images_device_planes on the same pixels as HWC BGR u8 / f32 and CHW RGB u8 tensors.  The GPU name and power
+limit are read in the same run.
 
 Usage: python bench_device_frames.py [--steps 50] [--warmup 5]
 """
@@ -53,9 +54,9 @@ def ingest_only(L, capi, torch, de, pinned, hwc, chw, W, steps):
         capi.check(L.psm_set_images_commit(h), h)
 
     paths = {
-        "ingest_kernel_f32": lambda: capi.check(L.psm_set_images_device(h, f32[0].data_ptr(), W * 12, f32[1].data_ptr(),
-                                                                        W * 12), h),
-        "ingest_kernel_u8": commit_u8,
+        "device_f32": lambda: capi.check(L.psm_set_images_device(h, f32[0].data_ptr(), W * 12, f32[1].data_ptr(),
+                                                                 W * 12), h),
+        "async_commit_u8": commit_u8,
         "planes_hwc_bgr_u8": planes(hwc, "bgr"),
         "planes_hwc_bgr_f32": planes(f32, "bgr"),
         "planes_chw_rgb_u8": planes(chw, "rgb"),

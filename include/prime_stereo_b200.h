@@ -333,7 +333,8 @@ int psm_set_images_u8(psm_ctx* ctx, const uint8_t* left, size_t left_step,
 
 /* Same as psm_set_images but the interleaved float images already live in DEVICE memory.  Asynchronous: the images are
  * read by the ingest kernels on the context's stream, so the caller orders the work that produces them, and any later
- * overwrite of them, against that stream (psm_set_stream, or events). */
+ * overwrite of them, against that stream (psm_set_stream, or events).  The pointers and steps must be multiples of 4
+ * bytes (PSM_EINVAL before any CUDA call otherwise). */
 int psm_set_images_device(psm_ctx* ctx, const float* d_left, size_t left_step,
                           const float* d_right, size_t right_step);
 
@@ -350,7 +351,7 @@ enum { PSM_PIX_U8 = 1, PSM_PIX_F32 = 2 };
  *   BGRA      p + 0, p + 1, p + 2 (times elem)   col_step 4 * elem
  * The planes, gradients and guide flags equal those psm_set_images / _u8 build from the same sample values (u8 samples
  * scaled by 1/255.0f as convertTo does), so every later result is the same bit for bit; float frames take the same
- * flagged or unflagged filter route.  One ingest_planes_kernel launch and one halo pass per view; stage 0 times it.
+ * flagged or unflagged filter route.  One ingest_kernel launch and one halo pass per view; stage 0 times it.
  *   - PSM_EINVAL before any CUDA call: a null array or channel pointer, an unknown pix_type, col_step < elem,
  *     row_step < (W - 1) * col_step + elem, and for float samples a pointer or step that is not a multiple of 4.
  *   - Asynchronous like psm_set_images_device: the kernels read the frames on the context's stream.  Order their

@@ -49,7 +49,7 @@ struct psm_ctx {
     cudaEvent_t ingest_done[2] = {nullptr, nullptr};  // ingest kernels consumed staging set k (recorded on the compute stream)
     bool ingest_done_valid[2] = {false, false};
     int stage_cur = 0;                      // staging set holding the current frame: 0 = stage_in, 1 = stage_alt
-    int up_pending = 0;                     // 0 none, 1 f32 upload pending, 2 u8 upload pending
+    int up_pending = 0;                     // pixel type (PSM_PIX_*) of the pending asynchronous upload, 0 none
     uint8_t* dis[2] = {nullptr, nullptr};    // disparity maps: u8, or u16 (map_bytes = 2, psm_create_u16) behind the same pointer
     int map_bytes = 1;                       // bytes per disparity-map element
     // Fast Guided Filter branch (lazy): low-res guide planes per view, low-res coefficient scratch, up-sampling plan
@@ -228,45 +228,67 @@ void images_ingested(psm_ctx* c, bool float_images)
     c->filtered = false;
 }
 
-template <typename T>
-int ingest(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool from_device)
+size_t pix_bytes(int pix) { return pix == PSM_PIX_U8 ? 1 : sizeof(float); }
+
+// the frame's planes, gradients and ingest flags: one ingest_kernel launch and one pad_rows per view on the context's stream
+int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
 {
-    const T* src[2] = {l, r};
-    const size_t step[2] = {lstep, rstep};
-    const size_t row_bytes = (size_t)c->W * 3 * sizeof(T);
-    for (int v = 0; v < 2; ++v)
-        if (!src[v] || step[v] < row_bytes) return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
-    const int set = c->stage_cur;
-    if (!from_device) {
-        // Host frames go through the current staging set on the copy stream, once the last ingest from that set has
-        // read it, so that the copy does not queue behind the compute stream's backlog; the compute stream waits for
-        // it, and the call returns once it has read the caller's buffers (from page-locked memory the copy would
-        // otherwise still be reading them after the return).
-        if (c->ingest_done_valid[set]) PSM_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ingest_done[set], 0));
-        for (int v = 0; v < 2; ++v)
-            PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v], step[v], row_bytes, c->H,
-                                          cudaMemcpyHostToDevice, c->copy_stream));
-        PSM_CUDA(c, cudaEventRecord(c->host_copied, c->copy_stream));
-        PSM_CUDA(c, cudaStreamWaitEvent(c->stream, c->host_copied, 0));
-    }
     PSM_CUDA(c, cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
+    const auto kernel = pix == PSM_PIX_U8 ? ingest_kernel<uint8_t> : ingest_kernel<float>;
     for (int v = 0; v < 2; ++v) {
-        const T* dsrc = from_device ? src[v] : static_cast<const T*>(stage_buf(c, set, v));
-        const size_t dstep = from_device ? step[v] : row_bytes;
         float* g = c->guide[v];
         dim3 blk(128), grd((c->W + 3 + 127) / 128, c->H);
-        ingest_kernel<T><<<grd, blk, 0, c->stream>>>(dsrc, dstep, c->W, c->H, c->Wp, g, g + c->plane,
-                                                      g + 2 * c->plane, c->grd[v], c->gray_mode, c->guide_flags + v);
+        kernel<<<grd, blk, 0, c->stream>>>(src[v], c->W, c->H, c->Wp, g, g + c->plane, g + 2 * c->plane, c->grd[v],
+                                           c->gray_mode, c->guide_flags + v);
         PSM_LAUNCH_CHECK(c);
         if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
     }
-    if (!from_device) {
-        // the next upload into this set waits for these kernels (psm_set_images_commit records its own ingests)
-        PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
-        c->ingest_done_valid[set] = true;
-        PSM_CUDA(c, cudaEventSynchronize(c->host_copied));
+    images_ingested(c, pix != PSM_PIX_U8);
+    return PSM_OK;
+}
+
+// Copy a checked interleaved host frame into staging set `set` on the copy stream and record `done` there.  The copy
+// starts once the last ingest from that set has read it, so that it does not queue behind the compute stream's backlog.
+int upload(psm_ctx* c, int set, int pix, const PlanesSrc src[2], cudaEvent_t done)
+{
+    const size_t row_bytes = (size_t)c->W * 3 * pix_bytes(pix);
+    if (c->ingest_done_valid[set]) PSM_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ingest_done[set], 0));
+    for (int v = 0; v < 2; ++v)
+        PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v].ch[0], src[v].row_step, row_bytes, c->H,
+                                      cudaMemcpyHostToDevice, c->copy_stream));
+    PSM_CUDA(c, cudaEventRecord(done, c->copy_stream));
+    return PSM_OK;
+}
+
+// ingest staging set `set` once the copy that filled it (`copied`) is done; the next copy into the set waits for this
+int ingest_staged(psm_ctx* c, int set, int pix, cudaEvent_t copied)
+{
+    PSM_CUDA(c, cudaStreamWaitEvent(c->stream, copied, 0));
+    const size_t elem = pix_bytes(pix), row_bytes = (size_t)c->W * 3 * elem;
+    const PlanesSrc src[2] = {interleaved_src(stage_buf(c, set, 0), elem, row_bytes),
+                              interleaved_src(stage_buf(c, set, 1), elem, row_bytes)};
+    if (int rc = ingest(c, pix, src)) return rc;
+    PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
+    c->ingest_done_valid[set] = true;
+    return PSM_OK;
+}
+
+// psm_set_images[_u8|_device][_async]: two interleaved BGR frames -> src, or PSM_EINVAL before any CUDA call.  The
+// kernel reads a device frame in place with loads of whole samples, so its pointers and steps are multiples of a sample.
+int check_interleaved(psm_ctx* c, int pix, bool device, const void* l, size_t lstep, const void* r, size_t rstep,
+                      PlanesSrc src[2])
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    const void* p[2] = {l, r};
+    const size_t step[2] = {lstep, rstep};
+    const size_t elem = pix_bytes(pix);
+    for (int v = 0; v < 2; ++v) {
+        if (!p[v] || step[v] < (size_t)c->W * 3 * elem) return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
+        if (device && ((uintptr_t)p[v] % elem || step[v] % elem))
+            return fail(c, PSM_EINVAL, "pointer or step %zu of view %d is not a multiple of the %zu bytes of a float sample",
+                        step[v], v, elem);
+        src[v] = interleaved_src(p[v], elem, step[v]);
     }
-    images_ingested(c, sizeof(T) != 1);
     return PSM_OK;
 }
 
@@ -277,7 +299,7 @@ int check_planes(psm_ctx* c, int pix_type, const void* const left[3], const void
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
     if (pix_type != PSM_PIX_U8 && pix_type != PSM_PIX_F32)
         return fail(c, PSM_EINVAL, "unknown pixel type %d (PSM_PIX_U8 = 1, PSM_PIX_F32 = 2)", pix_type);
-    const size_t elem = pix_type == PSM_PIX_U8 ? 1 : sizeof(float);
+    const size_t elem = pix_bytes(pix_type);
     const void* const* ch[2] = {left, right};
     for (int v = 0; v < 2; ++v) {
         if (!ch[v]) return fail(c, PSM_EINVAL, "null channel pointer array for view %d", v);
@@ -301,49 +323,24 @@ int check_planes(psm_ctx* c, int pix_type, const void* const left[3], const void
     return PSM_OK;
 }
 
-// the caller's frame, read in place by ingest_planes_kernel on the context's stream (one launch and pad_rows per view)
-int ingest_planes(psm_ctx* c, bool u8, const PlanesSrc src[2])
-{
-    PSM_CUDA(c, cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
-    for (int v = 0; v < 2; ++v) {
-        float* g = c->guide[v];
-        dim3 blk(128), grd((c->W + 3 + 127) / 128, c->H);
-        if (u8)
-            ingest_planes_kernel<uint8_t><<<grd, blk, 0, c->stream>>>(src[v], c->W, c->H, c->Wp, g, g + c->plane,
-                                                                       g + 2 * c->plane, c->grd[v], c->gray_mode,
-                                                                       c->guide_flags + v);
-        else
-            ingest_planes_kernel<float><<<grd, blk, 0, c->stream>>>(src[v], c->W, c->H, c->Wp, g, g + c->plane,
-                                                                     g + 2 * c->plane, c->grd[v], c->gray_mode,
-                                                                     c->guide_flags + v);
-        PSM_LAUNCH_CHECK(c);
-        if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
-    }
-    images_ingested(c, !u8);
-    return PSM_OK;
-}
+// how a checked frame reaches the context: host buffers through a staging set, or device memory read in place
+enum class Frame { host, device, planes };
 
-// asynchronous upload of the NEXT frame into the staging set that is not in use (copy stream)
-template <typename T>
-int upload_async(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep)
+// stage 0 of one context.  A host frame is copied into the current staging set and ingested from there; the call returns
+// once the copy has read the caller's buffers (from page-locked memory it would otherwise still be reading them after the
+// return).  A device frame is ingested in place.
+int set_images_one(psm_ctx* c, Frame kind, int pix, const PlanesSrc src[2])
 {
-    const T* src[2] = {l, r};
-    const size_t step[2] = {lstep, rstep};
-    const size_t row_bytes = (size_t)c->W * 3 * sizeof(T);
-    if (c->up_pending) return fail(c, PSM_ESTATE, "an asynchronous upload is already pending: call psm_set_images_commit first");
-    const int set = c->stage_cur ^ 1;
-    if (!c->stage_alt[0]) {  // allocated on first use: synchronous callers never pay for the second set
-        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->stage_alt[v], (size_t)c->W * c->H * 3 * sizeof(float)));
+    if (int rc = bind(c)) return rc;
+    if (int rc = stage_begin(c, 0)) return rc;
+    if (kind == Frame::host) {
+        if (int rc = upload(c, c->stage_cur, pix, src, c->host_copied)) return rc;
+        if (int rc = ingest_staged(c, c->stage_cur, pix, c->host_copied)) return rc;
+        PSM_CUDA(c, cudaEventSynchronize(c->host_copied));
+    } else if (int rc = ingest(c, pix, src)) {
+        return rc;
     }
-    if (c->ingest_done_valid[set]) PSM_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ingest_done[set], 0));
-    for (int v = 0; v < 2; ++v) {
-        if (!src[v] || step[v] < row_bytes) return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
-        PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v], step[v], row_bytes, c->H,
-                                      cudaMemcpyHostToDevice, c->copy_stream));
-    }
-    PSM_CUDA(c, cudaEventRecord(c->up_done, c->copy_stream));
-    c->up_pending = sizeof(T) == 1 ? 2 : 1;
-    return PSM_OK;
+    return stage_end(c, 0);
 }
 
 int launch_guide(psm_ctx* c);
@@ -762,75 +759,61 @@ int reject_multi(psm_ctx* c, const char* call, const char* why)
     return fail(c, PSM_EINVAL, "%s on a multi-device context (psm_create_multi): %s", call, why);
 }
 
-// psm_set_images[_u8|_device] on a multi-device context.  The first shard ingests the frame as a single-device context
-// does (a host frame: one upload into its staging set).  Every other shard receives the frame device to device into its
-// own staging set and runs its own ingest kernels; its stage 0 covers the copy.  The staging sets' readers and writers:
+// psm_set_images[_u8|_device] on a multi-device context, after the first shard's stage 0.  Every other shard receives
+// the frame device to device into its own staging set and runs its own ingest kernels; its stage 0 covers the copy.
+// The staging sets' readers and writers:
 //   - shard k's copy starts once the source holds the frame (the first shard's staging set after its upload, or the
 //     caller's device images at the first shard's ingest) and once shard k's last ingest has read shard k's staging set;
 //   - the source's next writer follows every copy: the first shard's copy stream (its next upload) for a host frame, the
 //     first shard's stream (which the caller orders its overwrites against) for device images;
 //   - shard k's ingest kernels follow its copy, and its next copy follows them (ingest_done).
-template <typename T>
-int multi_set_images(psm_ctx* c, const T* l, size_t lstep, const T* r, size_t rstep, bool from_device)
+int multi_send_frame(psm_ctx* c, Frame kind, int pix, const PlanesSrc src[2])
 {
     psm_ctx* s0 = c->shard[0];
-    int rc = bind(s0);
-    if (!rc) rc = stage_begin(s0, 0);
-    if (!rc) rc = ingest<T>(s0, l, lstep, r, rstep, from_device);
-    if (!rc) rc = stage_end(s0, 0);
-    if (rc) return relay(c, 0, rc);
-    const size_t row = (size_t)c->W * 3 * sizeof(T);
-    const void* src[2] = {l, r};
-    size_t step[2] = {lstep, rstep};
+    const size_t row = (size_t)c->W * 3 * pix_bytes(pix);
+    const void* from[2] = {src[0].ch[0], src[1].ch[0]};
+    size_t step[2] = {src[0].row_step, src[1].row_step};
     cudaEvent_t ready = s0->host_copied;
     cudaStream_t next_writer = s0->copy_stream;
-    if (from_device) {
+    if (kind == Frame::device) {
         PSM_CUDA(c, cudaEventRecord(c->ev_images, s0->stream));
         ready = c->ev_images;
         next_writer = s0->stream;
     } else {
-        for (int v = 0; v < 2; ++v) { src[v] = stage_buf(s0, s0->stage_cur, v); step[v] = row; }
+        for (int v = 0; v < 2; ++v) { from[v] = stage_buf(s0, s0->stage_cur, v); step[v] = row; }
     }
     for (int k = 1; k < c->nshards; ++k) {
         psm_ctx* s = c->shard[k];
-        if ((rc = bind(s))) return relay(c, k, rc);
+        int rc = bind(s);
+        if (rc) return relay(c, k, rc);
         if (s->ingest_done_valid[0]) PSM_CUDA(c, cudaStreamWaitEvent(s->copy_stream, s->ingest_done[0], 0));
         PSM_CUDA(c, cudaStreamWaitEvent(s->copy_stream, ready, 0));
         if (s->timing) PSM_CUDA(c, cudaEventRecord(s->ev0[0], s->copy_stream));
         for (int v = 0; v < 2; ++v)   // a peer copy between distinct devices
-            PSM_CUDA(c, cudaMemcpy2DAsync(s->stage_in[v], row, src[v], step[v], row, c->H, cudaMemcpyDefault, s->copy_stream));
+            PSM_CUDA(c, cudaMemcpy2DAsync(s->stage_in[v], row, from[v], step[v], row, c->H, cudaMemcpyDefault, s->copy_stream));
         PSM_CUDA(c, cudaEventRecord(c->ev_copied[k], s->copy_stream));
         PSM_CUDA(c, cudaStreamWaitEvent(next_writer, c->ev_copied[k], 0));
-        PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_copied[k], 0));
-        rc = ingest<T>(s, static_cast<const T*>(s->stage_in[0]), row, static_cast<const T*>(s->stage_in[1]), row, true);
-        if (rc) return relay(c, k, rc);
-        PSM_CUDA(c, cudaEventRecord(s->ingest_done[0], s->stream));
-        s->ingest_done_valid[0] = true;
-        if ((rc = stage_end(s, 0))) return relay(c, k, rc);
+        if ((rc = ingest_staged(s, 0, pix, c->ev_copied[k])) || (rc = stage_end(s, 0))) return relay(c, k, rc);
     }
     return PSM_OK;
 }
 
-// psm_set_images_device_planes on a multi-device context.  The first shard ingests the caller's frame; every other
-// shard copies what that ingest wrote (the three channel planes with their mirrored halos, the gradient planes and the
-// ingest flags, byte for byte) device to device on its own stream, so the caller's buffers are read on the first device
-// only and every shard holds the planes its own ingest would have written.  The broadcast's readers and writers:
+// psm_set_images_device_planes on a multi-device context, after the first shard's stage 0.  Every other shard copies what
+// the first shard's ingest wrote (the three channel planes with their mirrored halos, the gradient planes and the ingest
+// flags, byte for byte) device to device on its own stream, so the caller's buffers are read on the first device only and
+// every shard holds the planes its own ingest would have written.  The broadcast's readers and writers:
 //   - shard k's copy follows the first shard's ingest (ev_images) and, on its own stream, shard k's earlier work, which
 //     reads the planes the copy overwrites;
 //   - the first shard's later work (its next ingest, and the guide precompute, which adds to the flags) follows every
 //     copy (ev_copied), and so does whatever orders itself after the first shard's stream (psm_signal_stream).
-int multi_set_planes(psm_ctx* c, bool u8, const PlanesSrc src[2])
+int multi_send_planes(psm_ctx* c, int pix)
 {
     psm_ctx* s0 = c->shard[0];
-    int rc = bind(s0);
-    if (!rc) rc = stage_begin(s0, 0);
-    if (!rc) rc = ingest_planes(s0, u8, src);
-    if (!rc) rc = stage_end(s0, 0);
-    if (rc) return relay(c, 0, rc);
     PSM_CUDA(c, cudaEventRecord(c->ev_images, s0->stream));
     for (int k = 1; k < c->nshards; ++k) {
         psm_ctx* s = c->shard[k];
-        if ((rc = bind(s))) return relay(c, k, rc);
+        int rc = bind(s);
+        if (rc) return relay(c, k, rc);
         PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_images, 0));
         if ((rc = stage_begin(s, 0))) return relay(c, k, rc);
         for (int v = 0; v < 2; ++v) {   // from the first row's left halo: 3 channel planes, then the gradient plane
@@ -842,9 +825,34 @@ int multi_set_planes(psm_ctx* c, bool u8, const PlanesSrc src[2])
         PSM_CUDA(c, cudaMemcpyAsync(s->guide_flags, s0->guide_flags, 2 * sizeof(int), cudaMemcpyDefault, s->stream));
         PSM_CUDA(c, cudaEventRecord(c->ev_copied[k], s->stream));
         PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_copied[k], 0));
-        images_ingested(s, !u8);
+        images_ingested(s, pix != PSM_PIX_U8);
         if ((rc = stage_end(s, 0))) return relay(c, k, rc);
     }
+    return PSM_OK;
+}
+
+// the body of every synchronous psm_set_images* call once its frame is checked.  A multi-device context runs stage 0 on
+// its first shard and sends the other shards the frame, or the planes the first shard ingested.
+int set_images(psm_ctx* c, Frame kind, int pix, const PlanesSrc src[2])
+{
+    if (!is_multi(c)) return set_images_one(c, kind, pix, src);
+    if (int rc = set_images_one(c->shard[0], kind, pix, src)) return relay(c, 0, rc);
+    return kind == Frame::planes ? multi_send_planes(c, pix) : multi_send_frame(c, kind, pix, src);
+}
+
+// psm_set_images[_u8]_async: the frame is uploaded into the staging set that is not in use, on the copy stream
+int set_images_async(psm_ctx* c, int pix, const void* l, size_t lstep, const void* r, size_t rstep, const char* call)
+{
+    if (is_multi(c)) return reject_multi(c, call, "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
+    if (int rc = bind(c)) return rc;
+    if (c->up_pending) return fail(c, PSM_ESTATE, "an asynchronous upload is already pending: call psm_set_images_commit first");
+    PlanesSrc src[2];
+    if (int rc = check_interleaved(c, pix, false, l, lstep, r, rstep, src)) return rc;
+    if (!c->stage_alt[0]) {  // allocated on first use: synchronous callers never pay for the second set
+        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->stage_alt[v], (size_t)c->W * c->H * 3 * sizeof(float)));
+    }
+    if (int rc = upload(c, c->stage_cur ^ 1, pix, src, c->up_done)) return rc;
+    c->up_pending = pix;
     return PSM_OK;
 }
 
@@ -1289,29 +1297,23 @@ int psm_set_stream(psm_ctx* c, void* cuda_stream)
 
 int psm_set_images(psm_ctx* c, const float* left, size_t left_step, const float* right, size_t right_step)
 {
-    if (is_multi(c)) return multi_set_images<float>(c, left, left_step, right, right_step, false);
-    if (int rc = bind(c)) return rc;
-    if (int rc = stage_begin(c, 0)) return rc;
-    if (int rc = ingest<float>(c, left, left_step, right, right_step, false)) return rc;
-    return stage_end(c, 0);
+    PlanesSrc src[2];
+    if (int rc = check_interleaved(c, PSM_PIX_F32, false, left, left_step, right, right_step, src)) return rc;
+    return set_images(c, Frame::host, PSM_PIX_F32, src);
 }
 
 int psm_set_images_u8(psm_ctx* c, const uint8_t* left, size_t left_step, const uint8_t* right, size_t right_step)
 {
-    if (is_multi(c)) return multi_set_images<uint8_t>(c, left, left_step, right, right_step, false);
-    if (int rc = bind(c)) return rc;
-    if (int rc = stage_begin(c, 0)) return rc;
-    if (int rc = ingest<uint8_t>(c, left, left_step, right, right_step, false)) return rc;
-    return stage_end(c, 0);
+    PlanesSrc src[2];
+    if (int rc = check_interleaved(c, PSM_PIX_U8, false, left, left_step, right, right_step, src)) return rc;
+    return set_images(c, Frame::host, PSM_PIX_U8, src);
 }
 
 int psm_set_images_device(psm_ctx* c, const float* d_left, size_t left_step, const float* d_right, size_t right_step)
 {
-    if (is_multi(c)) return multi_set_images<float>(c, d_left, left_step, d_right, right_step, true);
-    if (int rc = bind(c)) return rc;
-    if (int rc = stage_begin(c, 0)) return rc;
-    if (int rc = ingest<float>(c, d_left, left_step, d_right, right_step, true)) return rc;
-    return stage_end(c, 0);
+    PlanesSrc src[2];
+    if (int rc = check_interleaved(c, PSM_PIX_F32, true, d_left, left_step, d_right, right_step, src)) return rc;
+    return set_images(c, Frame::device, PSM_PIX_F32, src);
 }
 
 int psm_set_images_device_planes(psm_ctx* c, int pix_type, const void* const left[3], const void* const right[3],
@@ -1319,12 +1321,7 @@ int psm_set_images_device_planes(psm_ctx* c, int pix_type, const void* const lef
 {
     PlanesSrc src[2];
     if (int rc = check_planes(c, pix_type, left, right, row_step, col_step, src)) return rc;
-    const bool u8 = pix_type == PSM_PIX_U8;
-    if (is_multi(c)) return multi_set_planes(c, u8, src);
-    if (int rc = bind(c)) return rc;
-    if (int rc = stage_begin(c, 0)) return rc;
-    if (int rc = ingest_planes(c, u8, src)) return rc;
-    return stage_end(c, 0);
+    return set_images(c, Frame::planes, pix_type, src);
 }
 
 // Events only: the caller's stream is recorded once (on the context's first device) and every stream of the context
@@ -1365,16 +1362,12 @@ int psm_signal_stream(psm_ctx* c, void* cuda_stream)
 
 int psm_set_images_async(psm_ctx* c, const float* left, size_t left_step, const float* right, size_t right_step)
 {
-    if (is_multi(c)) return reject_multi(c, "psm_set_images_async", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
-    if (int rc = bind(c)) return rc;
-    return upload_async<float>(c, left, left_step, right, right_step);
+    return set_images_async(c, PSM_PIX_F32, left, left_step, right, right_step, "psm_set_images_async");
 }
 
 int psm_set_images_u8_async(psm_ctx* c, const uint8_t* left, size_t left_step, const uint8_t* right, size_t right_step)
 {
-    if (is_multi(c)) return reject_multi(c, "psm_set_images_u8_async", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
-    if (int rc = bind(c)) return rc;
-    return upload_async<uint8_t>(c, left, left_step, right, right_step);
+    return set_images_async(c, PSM_PIX_U8, left, left_step, right, right_step, "psm_set_images_u8_async");
 }
 
 int psm_set_images_commit(psm_ctx* c)
@@ -1382,21 +1375,12 @@ int psm_set_images_commit(psm_ctx* c)
     if (is_multi(c)) return reject_multi(c, "psm_set_images_commit", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
     if (int rc = bind(c)) return rc;
     if (!c->up_pending) return fail(c, PSM_ESTATE, "psm_set_images_commit without a pending psm_set_images_async");
-    const int set = c->stage_cur ^ 1;
-    const bool u8 = c->up_pending == 2;
+    const int set = c->stage_cur ^ 1, pix = c->up_pending;
     if (int rc = stage_begin(c, 0)) return rc;
-    PSM_CUDA(c, cudaStreamWaitEvent(c->stream, c->up_done, 0));
     c->stage_cur = set;
     c->up_pending = 0;
-    int rc;
-    if (u8) rc = ingest<uint8_t>(c, static_cast<const uint8_t*>(stage_buf(c, set, 0)), (size_t)c->W * 3,
-                                 static_cast<const uint8_t*>(stage_buf(c, set, 1)), (size_t)c->W * 3, true);
-    else rc = ingest<float>(c, static_cast<const float*>(stage_buf(c, set, 0)), (size_t)c->W * 3 * sizeof(float),
-                            static_cast<const float*>(stage_buf(c, set, 1)), (size_t)c->W * 3 * sizeof(float), true);
-    if (rc) return rc;
-    PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
-    c->ingest_done_valid[set] = true;
-    if ((rc = stage_end(c, 0))) return rc;
+    if (int rc = ingest_staged(c, set, pix, c->up_done)) return rc;
+    if (int rc = stage_end(c, 0)) return rc;
     // the caller may reuse its host buffers once this returns: wait for the copy that reads them (it may still be
     // waiting for the frame before last to leave this staging set); the ingest kernels are already queued behind it
     PSM_CUDA(c, cudaEventSynchronize(c->up_done));

@@ -42,7 +42,7 @@ __global__ void pad_cols_kernel(float* __restrict__ base, size_t nrows, int W, i
 }
 
 // ------------------------------------------------------------------------------------------
-// Ingest: interleaved BGR (float or u8) -> 3 planar channels + x-gradient of the gray image.
+// Ingest: a BGR frame (float or u8) in any PlanesSrc layout -> 3 planar channels + x-gradient of the gray image.
 // Restates StereoMatch.cpp:193-197 (u8 * (1/255.0f)), CVF.cpp:47 (split) and CVC.cpp:41-46
 // (cvtColor RGB2GRAY on the BGR image, Sobel dx=1 ksize=1 with BORDER_REFLECT_101).
 // ------------------------------------------------------------------------------------------
@@ -61,12 +61,6 @@ __device__ __forceinline__ float gray_of(float c0, float c1, float c2, int gray_
     return fadd(fadd(fmul(c0, 0.299f), fmul(c1, 0.587f)), fmul(c2, 0.114f));
 }
 
-template <typename T>
-__device__ __forceinline__ float gray_at(const T* __restrict__ row, int x, int gray_mode)
-{
-    return gray_of(to_f32(row[3 * x]), to_f32(row[3 * x + 1]), to_f32(row[3 * x + 2]), gray_mode);
-}
-
 // the guide flags one pixel's channel values raise (see ingest_kernel)
 __device__ __forceinline__ void ingest_flags(float v0, float v1, float v2, int* __restrict__ guide_flag)
 {
@@ -76,49 +70,24 @@ __device__ __forceinline__ void ingest_flags(float v0, float v1, float v2, int* 
     if (inexact(u0) || inexact(u1) || inexact(u2)) atomicOr(guide_flag, kGuideInexact);
 }
 
-template <typename T>
-__global__ void ingest_kernel(const T* __restrict__ src, size_t step_bytes, int W, int H, int Wp,
-                              float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
-                              float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    if (x >= ((W + 3) & ~3) || y >= H) return;
-    const size_t o = (size_t)y * Wp + x;
-    if (x >= W) { I0[o] = 0.f; I1[o] = 0.f; I2[o] = 0.f; grd[o] = 0.f; return; }
-    const T* row = reinterpret_cast<const T*>(reinterpret_cast<const char*>(src) + (size_t)y * step_bytes);
-    const float v0 = to_f32(row[3 * x]), v1 = to_f32(row[3 * x + 1]), v2 = to_f32(row[3 * x + 2]);
-    I0[o] = v0;
-    I1[o] = v1;
-    I2[o] = v2;
-    // the integer widening in guide_kernel / the CVF kernel assumes I >= +0, finite, and I * I finite (images are in
-    // [0,1] by contract, DispEst data contract SURVEY 8b); a negative, non-finite or >= 2^61 value raises kGuideOutside
-    // and selects their conversion-pipe paths (bit patterns compare like the magnitudes; the sign bit sorts last).
-    // Below 2^61 every cost psm_cost_const builds is finite, >= +0 and < 2^63 (|l - r| < 2^61 per channel), so the
-    // slices of such a view need no reference-order pass of their own; with kGuideOutside the whole view takes it.
-    // The guide's box sums (I_c and the rounded products I_c I_c', CVF.cpp:49-62) are exact in any order when every
-    // nonzero value lies in [2^-12, 1]: a product is then 0 or at least 2^-24, a multiple of 2^-47, and a sum of at most
-    // 64 such values in [0, 64] needs at most 53 bits.  Any other nonzero value raises kGuideInexact and the guide is
-    // recomputed in OpenCV's order (psm_cvf_ref.cuh).  u8 images (0 or 1/255 .. 1) never raise it.
-    ingest_flags(v0, v1, v2, guide_flag);
-    const float gr = gray_at(row, reflect101(x + 1, W), gray_mode);
-    const float gl = gray_at(row, reflect101(x - 1, W), gray_mode);
-    grd[o] = fsub(gr, gl);
-}
-
-// A frame given as three channel pointers (B, G, R) and byte steps (psm_set_images_device_planes): sample (x, y) of
-// channel c at ch[c] + y * row_step + x * col_step.  HWC BGR / RGB, BGRA and planar CHW frames all fit.
+// A frame given as three channel pointers (B, G, R) and byte steps: sample (x, y) of channel c at
+// ch[c] + y * row_step + x * col_step.  HWC BGR / RGB, BGRA and planar CHW frames all fit.
 struct PlanesSrc {
     const char* ch[3];
     size_t row_step, col_step;
 };
 
-// What ingest_kernel<T> writes for an interleaved frame holding the same sample values, from any PlanesSrc layout:
-// the three planes, the flags and the gradient of the gray image, the same operations in the same order.
+// the PlanesSrc of an interleaved BGR frame of `elem`-byte samples whose rows lie `step` bytes apart
+inline PlanesSrc interleaved_src(const void* p, size_t elem, size_t step)
+{
+    const char* b = static_cast<const char*>(p);
+    return PlanesSrc{{b, b + elem, b + 2 * elem}, step, 3 * elem};
+}
+
 template <typename T>
-__global__ void ingest_planes_kernel(PlanesSrc src, int W, int H, int Wp,
-                                     float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
-                                     float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
+__global__ void ingest_kernel(PlanesSrc src, int W, int H, int Wp,
+                              float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
+                              float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
@@ -133,6 +102,15 @@ __global__ void ingest_planes_kernel(PlanesSrc src, int W, int H, int Wp,
     I0[o] = v0;
     I1[o] = v1;
     I2[o] = v2;
+    // the integer widening in guide_kernel / the CVF kernel assumes I >= +0, finite, and I * I finite (images are in
+    // [0,1] by contract, DispEst data contract SURVEY 8b); a negative, non-finite or >= 2^61 value raises kGuideOutside
+    // and selects their conversion-pipe paths (bit patterns compare like the magnitudes; the sign bit sorts last).
+    // Below 2^61 every cost psm_cost_const builds is finite, >= +0 and < 2^63 (|l - r| < 2^61 per channel), so the
+    // slices of such a view need no reference-order pass of their own; with kGuideOutside the whole view takes it.
+    // The guide's box sums (I_c and the rounded products I_c I_c', CVF.cpp:49-62) are exact in any order when every
+    // nonzero value lies in [2^-12, 1]: a product is then 0 or at least 2^-24, a multiple of 2^-47, and a sum of at most
+    // 64 such values in [0, 64] needs at most 53 bits.  Any other nonzero value raises kGuideInexact and the guide is
+    // recomputed in OpenCV's order (psm_cvf_ref.cuh).  u8 images (0 or 1/255 .. 1) never raise it.
     ingest_flags(v0, v1, v2, guide_flag);
     const int xr = reflect101(x + 1, W), xl = reflect101(x - 1, W);
     const float gr = gray_of(sample(0, xr), sample(1, xr), sample(2, xr), gray_mode);

@@ -410,7 +410,7 @@ def test_launch_counts(kw, scenes):
         n3 = launches(de)
         shards = len(kw.get("devices", [0]))
         assert n1 - n0 == 4 * shards and n2 - n1 == 4 * shards     # unchanged: ingest + halo pass per view and shard
-        assert n3 - n2 == 4                                          # one ingest_planes_kernel + halo pass per view
+        assert n3 - n2 == 4                                          # one ingest_kernel + halo pass per view
         de.sync()
 
 
@@ -444,6 +444,13 @@ def test_rejected_arguments_change_nothing(scenes):
         for pix, lp, rp, row, col, text in cases:
             assert L.psm_set_images_device_planes(h, pix, lp, rp, row, col) == capi.PSM_EINVAL, text
             assert text.encode() in L.psm_last_error(h), (text, L.psm_last_error(h))
+        for lp, step in [(f + 2, 12 * W), (f, 12 * W + 2)]:   # interleaved float frames: the same 4-byte rule
+            assert L.psm_set_images_device(h, lp, step, f, 12 * W) == capi.PSM_EINVAL, (lp - f, step)
+            assert b"not a multiple of the 4 bytes" in L.psm_last_error(h), L.psm_last_error(h)
+        hf = np.zeros((H, W, 3), np.float32)
+        assert L.psm_set_images_async(h, hf.ctypes.data, 12 * W, None, 12 * W) == capi.PSM_EINVAL
+        assert b"view 1" in L.psm_last_error(h), L.psm_last_error(h)
+        assert L.psm_set_images_commit(h) == capi.PSM_ESTATE   # nothing was uploaded
         assert L.psm_cost_const(h) == capi.PSM_ESTATE      # no frame was taken
         m = torch.zeros(H, W, dtype=torch.uint8, device="cuda")
         for args, code in [((2, m.data_ptr(), W, m.data_ptr(), W), capi.PSM_EINVAL),
