@@ -394,12 +394,15 @@ int psm_cost_filter(psm_ctx* ctx);
 int psm_cost_filter_fgf(psm_ctx* ctx, int sub_sample_rate);
 
 /* Stage 3: WTA over d in [1, max_disp) for both views; copies the u8 maps to HOST memory
- * (row steps in bytes) and synchronises (DispSelect_GPU).  Only valid on an unsharded context. */
+ * (row steps in bytes) and synchronises (DispSelect_GPU).  Only valid on an unsharded context.
+ * The destinations are checked before the selection runs: a null left map, or a step below a row, returns PSM_EINVAL
+ * with nothing enqueued and the context unchanged; on a two-view context the same holds for the right map. */
 int psm_disp_select(psm_ctx* ctx, uint8_t* left, size_t left_step,
                     uint8_t* right, size_t right_step);
 
 /* Stage 3 with the D2H copies enqueued but NOT synchronised: the host maps are valid after psm_sync
- * (or any later synchronising call).  Page-locked host memory keeps the call asynchronous. */
+ * (or any later synchronising call).  Page-locked host memory keeps the call asynchronous.  Destinations are checked
+ * before the selection runs, as in psm_disp_select. */
 int psm_disp_select_async(psm_ctx* ctx, uint8_t* left, size_t left_step,
                           uint8_t* right, size_t right_step);
 
@@ -407,7 +410,7 @@ int psm_disp_select_async(psm_ctx* ctx, uint8_t* left, size_t left_step,
 int psm_disp_select_device(psm_ctx* ctx);
 
 /* Stage 3 on a u16 context (psm_create_u16): as psm_disp_select / psm_disp_select_async with uint16_t maps over
- * d in [1, max_disp); row steps in bytes (at least 2 * W). */
+ * d in [1, max_disp); row steps in bytes (at least 2 * W), checked before the selection runs. */
 int psm_disp_select_u16(psm_ctx* ctx, uint16_t* left, size_t left_step,
                         uint16_t* right, size_t right_step);
 int psm_disp_select_u16_async(psm_ctx* ctx, uint16_t* left, size_t left_step,
@@ -417,14 +420,16 @@ int psm_disp_select_u16_async(psm_ctx* ctx, uint16_t* left, size_t left_step,
  * "exp" colour weights on the 6-bit-quantised left / right image, JointWMF defaults), on the device; the
  * reference runs this stage on the CPU even in GPU mode (src/DispEst.cpp:338-344).  Input: the maps of the last
  * selection stage (for a sharded context with the fused exchange: the complete maps of psm_disp_reduce_p2p);
- * output: filtered u8 maps copied to HOST memory (row steps in bytes), synchronises.
+ * output: filtered u8 maps copied to HOST memory (row steps in bytes), synchronises.  The destinations are checked before
+ * the post-filter runs: a null left map, or a step below a row (the right map's too on a two-view context), returns
+ * PSM_EINVAL with nothing enqueued and the context unchanged.
  * Parity: equals the reference's JointWMF whenever the feature image has <= 256 distinct 6-bit colours; beyond
  * that the reference clusters colours with an RNG-seeded cv::kmeans (an approximation by its own documentation,
  * JointWMF.h:70-72) while this stage evaluates the un-clustered weights -- see DESIGN.md. */
 int psm_post_process(psm_ctx* ctx, uint8_t* left, size_t left_step, uint8_t* right, size_t right_step);
 /* Same without the D2H copy (maps stay on the device: psm_device_ptr selectors 4, 5). Asynchronous. */
 int psm_post_process_device(psm_ctx* ctx);
-/* Stage 4 on a u16 context: as psm_post_process with uint16_t maps (row steps in bytes). */
+/* Stage 4 on a u16 context: as psm_post_process with uint16_t maps (row steps in bytes, checked before the post-filter). */
 int psm_post_process_u16(psm_ctx* ctx, uint16_t* left, size_t left_step, uint16_t* right, size_t right_step);
 
 /* Both maps into caller DEVICE buffers (row steps in bytes, at least W * map bytes), device to device on the context's
@@ -443,7 +448,9 @@ int psm_copy_maps_device(psm_ctx* ctx, int which, void* d_left, size_t left_step
 int psm_disp_select_keys(psm_ctx* ctx, uint64_t* d_keys_left, uint64_t* d_keys_right);
 
 /* Sharded stage 3b: reduce `nranks` gathered key planes (DEVICE, [nranks][H*W] per view) to the
- * final u8 maps in HOST memory and synchronise. */
+ * final u8 maps in HOST memory and synchronise.  A null left map (or a null right map on a two-view context) keeps the
+ * maps on the device.  Otherwise a step below a row returns PSM_EINVAL before the reduction runs, with nothing enqueued
+ * and the context unchanged. */
 int psm_disp_reduce_keys(psm_ctx* ctx, const uint64_t* d_gathered_left,
                          const uint64_t* d_gathered_right, int nranks,
                          uint8_t* left, size_t left_step, uint8_t* right, size_t right_step);
@@ -459,7 +466,9 @@ int psm_disp_reduce_keys_u16(psm_ctx* ctx, const uint64_t* d_gathered_left,
  *                              straight into the exchange block of the rank that reduces that pixel;
  *   psm_disp_reduce_p2p      : this rank reduces its pixel chunk over all ranks' minima and stores the
  *                              winning disparity into EVERY rank's result map;
- *   psm_disp_fetch_p2p       : copy this rank's (complete) result maps to host memory and synchronise.
+ *   psm_disp_fetch_p2p       : copy this rank's (complete) result maps to host memory and synchronise; a null left
+ *                              map or a step below a row (the right map's too on a two-view context) returns
+ *                              PSM_EINVAL before the DONE wait is enqueued, with the context unchanged.
  * The three kernels order themselves across ranks through ARRIVE / DONE flag words in the exchange blocks
  * (release stores over NVLink, acquire loads; PSM_OPT_P2P_SYNC = 1, default): select -> reduce -> fetch can be
  * enqueued back to back on every rank without any library collective or host barrier, provided every rank runs

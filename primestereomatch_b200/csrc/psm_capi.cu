@@ -63,7 +63,7 @@ struct psm_ctx {
     bool pp_lut_valid = false;              // pp_lut holds the table of (pp_sigma, pp_type)
     bool have_maps = false;                 // disparity maps valid (a select / reduce stage ran)
     int* guide_flags = nullptr;             // [2] device flags: guide outside the integer-widening domain (see psm_cvf_stream.cuh)
-    unsigned char* p2p_own = nullptr;       // own exchange block: keys [2 views][nranks][chunk] u64, maps [2 views][H*W] u8, flag words
+    unsigned char* p2p_own = nullptr;       // own exchange block (P2pLayout): keys, maps and flag words of both views
     unsigned char* p2p_peer[kMaxRanks] = {};// every rank's exchange block as mapped here
     void* p2p_imported[kMaxRanks] = {};     // IPC mappings to close at destroy
     int p2p_nimported = 0, p2p_nranks = 0, p2p_rank = 0;
@@ -705,16 +705,50 @@ int run_blocks(psm_ctx* c, Filter filter)
     return PSM_OK;
 }
 
-// device map -> host rows of W elements of the context's map format
-int copy_map_out(psm_ctx* c, const uint8_t* dsrc, void* dst, size_t step)
+// The destinations of a map call `call`: rows of W elements of the map format, the right map's on a two-view context only.
+// Checked before the call's first launch: a bad one returns PSM_EINVAL with nothing enqueued and no state changed.
+int check_map_dst(psm_ctx* c, const char* call, const void* left, size_t left_step, const void* right, size_t right_step)
 {
+    if (int rc = check_right_arg(c, right, call)) return rc;
     const size_t row = (size_t)c->W * c->map_bytes;
-    if (!dst || step < row)
+    if (!left || left_step < row || (c->views == 2 && (!right || right_step < row)))
         return c->map_bytes == 1 ? fail(c, PSM_EINVAL, "bad disparity map pointer/step")
                                  : fail(c, PSM_EINVAL, "bad disparity map pointer/step (u16 maps need a step of at least %zu bytes)", row);
-    PSM_CUDA(c, cudaMemcpy2DAsync(dst, step, dsrc, row, row, c->H, cudaMemcpyDeviceToHost, c->stream));
     return PSM_OK;
 }
+
+// device maps src[view] -> the checked destinations, on the context's stream; then waits for the copies if `sync`
+int copy_maps_out(psm_ctx* c, const uint8_t* const src[2], void* left, size_t left_step, void* right, size_t right_step,
+                  cudaMemcpyKind kind, bool sync)
+{
+    const size_t row = (size_t)c->W * c->map_bytes;
+    PSM_CUDA(c, cudaMemcpy2DAsync(left, left_step, src[0], row, row, c->H, kind, c->stream));
+    if (c->views == 2) PSM_CUDA(c, cudaMemcpy2DAsync(right, right_step, src[1], row, row, c->H, kind, c->stream));
+    if (sync) PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
+}
+
+// The exchange block of one rank (psm_p2p_create_buffer), as byte offsets: keys [2 views][nranks][chunk] u64, maps
+// [2 views][H*W] of the map format rounded up to 256 bytes, flag words [2 views][2 * kMaxRanks] u32 (ARRIVE, DONE per rank).
+struct P2pLayout {
+    size_t chunk, keys_view, maps_at, map_view, flags_at, bytes;
+    unsigned long long* keys(unsigned char* base, int v) const { return reinterpret_cast<unsigned long long*>(base + v * keys_view); }
+    unsigned char* maps(unsigned char* base, int v) const { return base + maps_at + v * map_view; }
+    unsigned* flags(unsigned char* base, int v) const { return reinterpret_cast<unsigned*>(base + flags_at) + v * 2 * kMaxRanks; }
+};
+
+P2pLayout p2p_layout(const psm_ctx* c, int nranks)
+{
+    const size_t npix = (size_t)c->W * c->H, chunk = (npix + nranks - 1) / nranks, keys_view = nranks * chunk * sizeof(uint64_t);
+    const size_t map_view = npix * c->map_bytes, flags_at = 2 * keys_view + ((2 * map_view + 255) & ~(size_t)255);
+    return {chunk, keys_view, 2 * keys_view, map_view, flags_at, flags_at + 2 * 2 * kMaxRanks * sizeof(unsigned)};
+}
+
+// the current maps are the exchange block's: from the first exchanged frame on, also after a later local selection
+bool exchanged(const psm_ctx* c) { return c->p2p_own && c->p2p_seq > 0; }
+
+// a selection stage wrote new maps (`own`: the context's own, not an exchange block's): the left-right masks are stale
+void selection_ran(psm_ctx* c, bool own) { c->lr_masks_ok = false; c->have_maps = c->have_maps || own; }
 
 // a map call for maps of type T, named u8_call / u16_call in its two formats, on a context of the other format:
 // PSM_EINVAL naming the right call
@@ -1015,8 +1049,6 @@ int psm_create(psm_ctx** out, int width, int height, int max_disp, int device)
     return psm_create_sharded(out, width, height, max_disp, 0, max_disp, device);
 }
 
-static size_t p2p_keys_bytes(const psm_ctx* c, int nranks);   // the exchange block's layout (below)
-
 int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const int* devices, int n_devices, int block_slices,
                      int map_bits)
 {
@@ -1095,8 +1127,7 @@ int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const i
     // the first shard's stream and complete maps stand for the context's (see is_multi)
     psm_ctx* s0 = c->shard[0];
     c->stream = s0->stream;
-    for (int v = 0; v < 2; ++v)
-        c->dis[v] = static_cast<uint8_t*>(blocks[0]) + p2p_keys_bytes(s0, n_devices) + (size_t)v * width * height * c->map_bytes;
+    for (int v = 0; v < 2; ++v) c->dis[v] = p2p_layout(c, n_devices).maps(static_cast<unsigned char*>(blocks[0]), v);
     *out = c;
     return PSM_OK;
 }
@@ -1571,13 +1602,9 @@ static int disp_select(psm_ctx* c, T* left, size_t left_step, T* right, size_t r
 {
     if (int rc = sync ? check_map_format<T>(c, "psm_disp_select", "psm_disp_select_u16")
                       : check_map_format<T>(c, "psm_disp_select_async", "psm_disp_select_u16_async")) return rc;
-    if (int rc = check_right_arg(c, right, "psm_disp_select")) return rc;
+    if (int rc = check_map_dst(c, "psm_disp_select", left, left_step, right, right_step)) return rc;
     if (int rc = psm_disp_select_device(c)) return rc;
-    if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
-    if (c->views == 2)
-        if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
-    if (sync) PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    return copy_maps_out(c, c->dis, left, left_step, right, right_step, cudaMemcpyDeviceToHost, sync);
 }
 
 template <typename T>
@@ -1590,21 +1617,18 @@ static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const u
     if (int rc = check_views_reset(c, "psm_disp_reduce_keys")) return rc;
     if (int rc = check_right_arg(c, d_gathered_right, "psm_disp_reduce_keys")) return rc;
     if (int rc = check_right_arg(c, right, "psm_disp_reduce_keys")) return rc;
+    const bool to_host = left && (right || c->views == 1);   // a null map pointer: the maps stay on the device
+    if (int rc = to_host ? check_map_dst(c, "psm_disp_reduce_keys", left, left_step, right, right_step) : PSM_OK) return rc;
     if (!d_gathered_left || (c->views == 2 && !d_gathered_right) || nranks < 1) return fail(c, PSM_EINVAL, "bad gathered keys");
     const uint64_t* g[2] = {d_gathered_left, d_gathered_right};
-    c->lr_masks_ok = false;
     const size_t npix = (size_t)c->W * c->H;
     for (int v = 0; v < c->views; ++v) {
         keys_reduce_kernel<T><<<(unsigned)((npix + 255) / 256), 256, 0, c->stream>>>(
             reinterpret_cast<const unsigned long long*>(g[v]), nranks, npix, reinterpret_cast<T*>(c->dis[v]));
         PSM_LAUNCH_CHECK(c);
     }
-    c->have_maps = true;
-    if (left && (right || c->views == 1)) {
-        if (int rc = copy_map_out(c, c->dis[0], left, left_step)) return rc;
-        if (c->views == 2)
-            if (int rc = copy_map_out(c, c->dis[1], right, right_step)) return rc;
-    }
+    selection_ran(c, true);
+    if (to_host) return copy_maps_out(c, c->dis, left, left_step, right, right_step, cudaMemcpyDeviceToHost, true);
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }
@@ -1621,9 +1645,8 @@ int psm_disp_select_device(psm_ctx* c)
         return fail(c, PSM_ESTATE, "psm_disp_select on a sharded context: use psm_disp_select_keys + psm_disp_reduce_keys");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
-    c->lr_masks_ok = false;
     if (int rc = c->map_bytes == 2 ? select_maps<uint16_t>(c) : select_maps<uint8_t>(c)) return rc;
-    c->have_maps = true;
+    selection_ran(c, true);
     return stage_end(c, 3);
 }
 
@@ -1683,13 +1706,6 @@ int psm_disp_reduce_keys_u16(psm_ctx* c, const uint64_t* d_gathered_left, const 
     return disp_reduce_keys(c, d_gathered_left, d_gathered_right, nranks, left, left_step, right, right_step);
 }
 
-// Exchange block of one rank: [2 views][nranks][chunk] uint64 keys, [2 views][H*W] result maps (u8, or u16 on a u16 context),
-// [2 views][2 * kMaxRanks] u32 flag words (ARRIVE per rank, DONE per rank), each part 256-byte aligned.
-static size_t p2p_chunk(const psm_ctx* c, int nranks) { return ((size_t)c->W * c->H + nranks - 1) / nranks; }
-static size_t p2p_keys_bytes(const psm_ctx* c, int nranks) { return (size_t)2 * nranks * p2p_chunk(c, nranks) * sizeof(unsigned long long); }
-static size_t p2p_maps_bytes(const psm_ctx* c) { return (((size_t)2 * c->W * c->H * c->map_bytes) + 255) & ~(size_t)255; }
-static size_t p2p_flags_bytes() { return (size_t)2 * 2 * kMaxRanks * sizeof(unsigned); }
-
 int psm_p2p_create_buffer(psm_ctx* c, int nranks, void** d_buffer)
 {
     if (is_multi(c)) return reject_multi(c, "psm_p2p_create_buffer", "the context already spans the whole disparity range; use psm_disp_select*");
@@ -1699,10 +1715,10 @@ int psm_p2p_create_buffer(psm_ctx* c, int nranks, void** d_buffer)
     for (int i = 0; i < c->p2p_nimported; ++i) cudaIpcCloseMemHandle(c->p2p_imported[i]);   // peers of a previous exchange set-up
     c->p2p_nimported = 0;
     for (int r = 0; r < kMaxRanks; ++r) c->p2p_peer[r] = nullptr;
-    const size_t kb = p2p_keys_bytes(c, nranks), mb = p2p_maps_bytes(c), fb = p2p_flags_bytes();
-    PSM_CUDA(c, cudaMalloc(&c->p2p_own, kb + mb + fb));
-    PSM_CUDA(c, cudaMemsetAsync(c->p2p_own, 0xff, kb + mb, c->stream));
-    PSM_CUDA(c, cudaMemsetAsync(c->p2p_own + kb + mb, 0, fb, c->stream));
+    const P2pLayout L = p2p_layout(c, nranks);
+    PSM_CUDA(c, cudaMalloc(&c->p2p_own, L.bytes));
+    PSM_CUDA(c, cudaMemsetAsync(c->p2p_own, 0xff, L.flags_at, c->stream));   // keys and maps
+    PSM_CUDA(c, cudaMemsetAsync(c->p2p_own + L.flags_at, 0, L.bytes - L.flags_at, c->stream));
     if (!c->p2p_counter) PSM_CUDA(c, cudaMalloc(&c->p2p_counter, sizeof(unsigned)));
     PSM_CUDA(c, cudaMemsetAsync(c->p2p_counter, 0, sizeof(unsigned), c->stream));
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -1753,18 +1769,16 @@ int psm_p2p_set_peers(psm_ctx* c, void* const* d_buffers, int nranks, int rank)
 
 static void p2p_fill(const psm_ctx* c, int view, P2pPeers& peers)
 {
-    const size_t chunk = p2p_chunk(c, c->p2p_nranks);
-    const size_t npix = (size_t)c->W * c->H;
-    const size_t kb = p2p_keys_bytes(c, c->p2p_nranks), mb = p2p_maps_bytes(c);
-    peers.nranks = c->p2p_nranks; peers.rank = c->p2p_rank; peers.chunk = (unsigned)chunk;
+    const P2pLayout L = p2p_layout(c, c->p2p_nranks);
+    peers.nranks = c->p2p_nranks; peers.rank = c->p2p_rank; peers.chunk = (unsigned)L.chunk;
     peers.counter = c->p2p_counter;
     // each view's flags carry the number of the last frame that exchanged that view
     peers.seq = c->p2p_sync ? (view ? c->p2p_seq_right : c->p2p_seq) : 0u;
     for (int r = 0; r < kMaxRanks; ++r) {
         unsigned char* base = r < c->p2p_nranks ? c->p2p_peer[r] : nullptr;
-        peers.keys[r] = base ? reinterpret_cast<unsigned long long*>(base) + (size_t)view * c->p2p_nranks * chunk : nullptr;
-        peers.maps[r] = base ? base + kb + (size_t)view * npix * c->map_bytes : nullptr;
-        peers.flags[r] = base ? reinterpret_cast<unsigned*>(base + kb + mb) + (size_t)view * 2 * kMaxRanks : nullptr;
+        peers.keys[r] = base ? L.keys(base, view) : nullptr;
+        peers.maps[r] = base ? L.maps(base, view) : nullptr;
+        peers.flags[r] = base ? L.flags(base, view) : nullptr;
     }
 }
 
@@ -1775,7 +1789,6 @@ static int p2p_scatter(psm_ctx* c)
     c->p2p_seq++;   // one sequence number per frame, identical on every rank (all ranks run the same frames and views)
     if (c->views == 2) c->p2p_seq_right++;
     c->p2p_right_current = c->views == 2;
-    c->lr_masks_ok = false;
     for (int v = 0; v < c->views; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
@@ -1786,6 +1799,7 @@ static int p2p_scatter(psm_ctx* c)
             wta_scatter_kernel<<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, peers);
         PSM_LAUNCH_CHECK(c);
     }
+    selection_ran(c, false);
     return PSM_OK;
 }
 
@@ -1811,13 +1825,13 @@ int psm_disp_reduce_p2p(psm_ctx* c)
     if (int rc = check_views_reset(c, "psm_disp_reduce_p2p")) return rc;
     const unsigned npix = (unsigned)((size_t)c->W * c->H);
     const auto reduce = c->map_bytes == 2 ? chunk_reduce_kernel<uint16_t> : chunk_reduce_kernel<uint8_t>;
-    c->lr_masks_ok = false;
     for (int v = 0; v < c->views; ++v) {
         P2pPeers peers;
         p2p_fill(c, v, peers);
         reduce<<<(peers.chunk + 255) / 256, 256, 0, c->stream>>>(peers, npix);
         PSM_LAUNCH_CHECK(c);
     }
+    selection_ran(c, false);
     return PSM_OK;
 }
 
@@ -1830,20 +1844,20 @@ static int check_p2p_right_map(psm_ctx* c, const char* call)
     return PSM_OK;
 }
 
-// the local result maps are complete once every rank's DONE flag carries this frame's number: enqueue the wait in front
+// the exchanged maps are complete once every rank's DONE flag carries this frame's number: enqueue the wait in front
 // of a consumer of the maps (once per frame)
 static int p2p_wait_done(psm_ctx* c)
 {
-    if (!c->p2p_sync || c->p2p_waited_seq == c->p2p_seq) return PSM_OK;
-    P2pPeers peers;
-    p2p_fill(c, 0, peers);
+    if (!exchanged(c) || !c->p2p_sync || c->p2p_waited_seq == c->p2p_seq) return PSM_OK;
+    const P2pLayout L = p2p_layout(c, c->p2p_nranks);
+    unsigned char* own = c->p2p_peer[c->p2p_rank];
     if (c->views == 2 && c->p2p_seq_right == c->p2p_seq) {
-        p2p_wait_done_kernel<<<1, 32, 0, c->stream>>>(peers.flags[c->p2p_rank], c->p2p_nranks, c->p2p_seq);
+        p2p_wait_done_kernel<<<1, 32, 0, c->stream>>>(L.flags(own, 0), c->p2p_nranks, c->p2p_seq);
         PSM_LAUNCH_CHECK(c);
     } else {   // the views' flags carry different frame numbers: one wait per view, nranks threads (the first view's words)
         for (int v = 0; v < c->views; ++v) {
-            p2p_wait_done_kernel<<<1, c->p2p_nranks, 0, c->stream>>>(peers.flags[c->p2p_rank] + (size_t)v * 2 * kMaxRanks,
-                                                                     c->p2p_nranks, v ? c->p2p_seq_right : c->p2p_seq);
+            p2p_wait_done_kernel<<<1, c->p2p_nranks, 0, c->stream>>>(L.flags(own, v), c->p2p_nranks,
+                                                                     v ? c->p2p_seq_right : c->p2p_seq);
             PSM_LAUNCH_CHECK(c);
         }
     }
@@ -1902,15 +1916,12 @@ static int disp_fetch_p2p(psm_ctx* c, T* left, size_t left_step, T* right, size_
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
     if (int rc = check_views_reset(c, "psm_disp_fetch_p2p")) return rc;
-    if (int rc = check_right_arg(c, right, "psm_disp_fetch_p2p")) return rc;
+    if (int rc = check_map_dst(c, "psm_disp_fetch_p2p", left, left_step, right, right_step)) return rc;
     if (int rc = check_p2p_right_map(c, "psm_disp_fetch_p2p")) return rc;
     if (int rc = p2p_wait_done(c)) return rc;
-    const unsigned char* maps = c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks);
-    if (int rc = copy_map_out(c, maps, left, left_step)) return rc;
-    if (c->views == 2)
-        if (int rc = copy_map_out(c, maps + (size_t)c->W * c->H * sizeof(T), right, right_step)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    const P2pLayout L = p2p_layout(c, c->p2p_nranks);
+    const uint8_t* maps[2] = {L.maps(c->p2p_own, 0), L.maps(c->p2p_own, 1)};
+    return copy_maps_out(c, maps, left, left_step, right, right_step, cudaMemcpyDeviceToHost, true);
 }
 
 extern "C" {
@@ -1926,11 +1937,18 @@ int psm_disp_fetch_p2p_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_
 }
 
 // ---- post-processing (PP::processDM) ----------------------------------------------------------------
-static const uint8_t* current_map(const psm_ctx* c, int v)
+// the maps of the last selection stage for psm_post_process* and psm_copy_maps_device, under the exchanged-map rules of
+// psm_disp_fetch_p2p; the caller enqueues p2p_wait_done before it reads them
+static int selection_maps(psm_ctx* c, const char* call, const uint8_t* maps[2])
 {
-    if (c->p2p_own && c->p2p_seq > 0)   // sharded: the complete maps live in the exchange block
-        return c->p2p_own + p2p_keys_bytes(c, c->p2p_nranks) + (size_t)v * c->W * c->H * c->map_bytes;
-    return c->dis[v];
+    if (!exchanged(c)) {
+        if (!c->have_maps) return fail(c, PSM_ESTATE, "%s before a disparity-selection stage", call);
+        maps[0] = c->dis[0]; maps[1] = c->dis[1];
+        return PSM_OK;
+    }
+    const P2pLayout L = p2p_layout(c, c->p2p_nranks);
+    maps[0] = L.maps(c->p2p_own, 0); maps[1] = L.maps(c->p2p_own, 1);
+    return check_p2p_right_map(c, call);
 }
 
 static int pp_weight_table_size(int type)
@@ -1972,9 +1990,8 @@ static int post_process_maps(psm_ctx* c)
     c->lr_masks_ok = false;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_post_process before psm_set_images");
     if (int rc = check_views_reset(c, "psm_post_process")) return rc;
-    if (!c->have_maps && !(c->p2p_own && c->p2p_seq > 0)) return fail(c, PSM_ESTATE, "psm_post_process before a disparity-selection stage");
-    if (c->p2p_own && c->p2p_seq > 0)
-        if (int rc = check_p2p_right_map(c, "psm_post_process")) return rc;
+    const uint8_t* maps[2];
+    if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
     const bool lr = c->lr_mode != PSM_LR_OFF, wmf = c->lr_mode != PSM_LR_FILL;
     if (lr && c->views == 1)
@@ -2005,14 +2022,13 @@ static int post_process_maps(psm_ctx* c)
         c->pp_lut_valid = true;
     }
     const bool tuned = c->pp_tuned();
-    if (c->p2p_own && c->p2p_seq > 0)
-        if (int rc = p2p_wait_done(c)) return rc;
+    if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
     if (lr) {
         // lrCheck + fillInv (PP.cpp:405-406): reads the selection maps, writes the filled maps into dis_pp
         const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;
         lr_check_fill_kernel<T><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
-            reinterpret_cast<const T*>(current_map(c, 0)), reinterpret_cast<const T*>(current_map(c, 1)), c->W,
+            reinterpret_cast<const T*>(maps[0]), reinterpret_cast<const T*>(maps[1]), c->W,
             reinterpret_cast<T*>(c->dis_pp[0]), reinterpret_cast<T*>(c->dis_pp[1]), c->lr_valid[0], c->lr_valid[1]);
         PSM_LAUNCH_CHECK(c);
         c->lr_masks_ok = true;
@@ -2033,7 +2049,7 @@ static int post_process_maps(psm_ctx* c)
         // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output (after
         // the left-right fill, the first pass filters the filled map)
         for (int it = 0; it < c->pp_iter; ++it) {
-            const T* src = reinterpret_cast<const T*>(it == 0 && !lr ? current_map(c, v) : c->dis_pp[v]);
+            const T* src = reinterpret_cast<const T*>(it == 0 && !lr ? maps[v] : c->dis_pp[v]);
             pp_pack_kernel<T><<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
             PSM_LAUNCH_CHECK(c);
             if (tuned)
@@ -2052,13 +2068,9 @@ template <typename T>
 static int post_process(psm_ctx* c, T* left, size_t left_step, T* right, size_t right_step)
 {
     if (int rc = check_map_format<T>(c, "psm_post_process", "psm_post_process_u16")) return rc;
-    if (int rc = check_right_arg(c, right, "psm_post_process")) return rc;
+    if (int rc = check_map_dst(c, "psm_post_process", left, left_step, right, right_step)) return rc;
     if (int rc = psm_post_process_device(c)) return rc;
-    if (int rc = copy_map_out(c, c->dis_pp[0], left, left_step)) return rc;
-    if (c->views == 2)
-        if (int rc = copy_map_out(c, c->dis_pp[1], right, right_step)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    return copy_maps_out(c, c->dis_pp, left, left_step, right, right_step, cudaMemcpyDeviceToHost, true);
 }
 
 extern "C" {
@@ -2092,34 +2104,19 @@ int psm_copy_maps_device(psm_ctx* c, int which, void* d_left, size_t left_step, 
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
     if (which != 0 && which != 1)
         return fail(c, PSM_EINVAL, "psm_copy_maps_device: which %d is neither 0 (selection maps) nor 1 (post-processed maps)", which);
-    const size_t row = (size_t)c->W * c->map_bytes;
-    if (!d_left || left_step < row)
-        return fail(c, PSM_EINVAL, "psm_copy_maps_device: bad left map pointer/step (a row of %d-bit maps is %zu bytes)",
-                    8 * c->map_bytes, row);
-    if (int rc = check_right_arg(c, d_right, "psm_copy_maps_device")) return rc;
-    if (c->views == 2 && (!d_right || right_step < row))
-        return fail(c, PSM_EINVAL, "psm_copy_maps_device: bad right map pointer/step (a row of %d-bit maps is %zu bytes)",
-                    8 * c->map_bytes, row);
+    if (int rc = check_map_dst(c, "psm_copy_maps_device", d_left, left_step, d_right, right_step)) return rc;
     // a multi-device context's maps are the first shard's (its exchange block, and its post-filter's outputs)
     if (is_multi(c)) return relay(c, 0, psm_copy_maps_device(c->shard[0], which, d_left, left_step, d_right, right_step));
     if (int rc = bind(c)) return rc;
     if (int rc = check_views_reset(c, "psm_copy_maps_device")) return rc;
-    const bool exchanged = c->p2p_own && c->p2p_seq > 0;
+    const uint8_t* maps[2] = {c->dis_pp[0], c->dis_pp[1]};
     if (which == 0) {
-        if (!c->have_maps && !exchanged) return fail(c, PSM_ESTATE, "psm_copy_maps_device before a disparity-selection stage");
-        if (exchanged) {   // the rules of psm_disp_fetch_p2p
-            if (int rc = check_p2p_right_map(c, "psm_copy_maps_device")) return rc;
-            if (int rc = p2p_wait_done(c)) return rc;
-        }
+        if (int rc = selection_maps(c, "psm_copy_maps_device", maps)) return rc;
+        if (int rc = p2p_wait_done(c)) return rc;
     } else if (!c->have_pp) {
         return fail(c, PSM_ESTATE, "psm_copy_maps_device of the post-processed maps before a post-process");
     }
-    void* dst[2] = {d_left, d_right};
-    const size_t step[2] = {left_step, right_step};
-    for (int v = 0; v < c->views; ++v)
-        PSM_CUDA(c, cudaMemcpy2DAsync(dst[v], step[v], which ? c->dis_pp[v] : current_map(c, v), row, row, c->H,
-                                      cudaMemcpyDefault, c->stream));
-    return PSM_OK;
+    return copy_maps_out(c, maps, d_left, left_step, d_right, right_step, cudaMemcpyDefault, false);
 }
 
 static int check_slice(psm_ctx* c, int view, int d)

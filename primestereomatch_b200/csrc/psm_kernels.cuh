@@ -559,9 +559,32 @@ __device__ __forceinline__ void gif_coeffs(float mp, float mIp0, float mIp1, flo
 
 // ------------------------------------------------------------------------------------------
 // K4 WTA (DispSel.cpp:83-109): per pixel argmin over global d in [1, D), strict <, ties -> lowest d,
-// minCost starts at +inf, result 0 when nothing compares below +inf.  One thread = 4 pixels.
-// Emits the map (T = uint8_t or uint16_t) and/or the packed (cost,d) key used by the disparity-sharded reduction.
+// minCost starts at +inf, result 0 when nothing compares below +inf.  One thread = 4 pixels.  wta_scan4 is the scan of
+// every selection kernel, wta_key the packed (cost, d) key in which every shard, block and rank exchanges its minima.
 // ------------------------------------------------------------------------------------------
+// the scan of slices [d_begin, d_begin + d_count), slice dl at p + dl * plane, into the caller's mc / md (set to +inf / 0;
+// returning them in a struct instead changes the kernels' SASS); an inactive lane scans nothing
+__device__ __forceinline__ void wta_scan4(const float* p, size_t plane, int d_begin, int d_count, bool active, float (&mc)[4],
+                                          int (&md)[4])
+{
+    int dl = (d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (DispSel.cpp:96)
+#pragma unroll 8
+    for (; active && dl < d_count; ++dl) {
+        const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
+        const int d = d_begin + dl;
+        if (c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
+        if (c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
+        if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
+        if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
+    }
+}
+
+__device__ __forceinline__ unsigned long long wta_key(float cost, int d)
+{
+    return ((unsigned long long)float_order_key(cost) << 32) | (unsigned)d;
+}
+
+// the scan of one volume: the map (T = uint8_t or uint16_t) and/or the keys used by the disparity-sharded reduction
 template <typename T>
 __global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin, int d_count,
                                                   T* __restrict__ dis /* [H][W] or null */,
@@ -574,29 +597,20 @@ __global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol,
     const float* p = vol + (size_t)y * Wp + x4;
     float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
     int md[4] = {0, 0, 0, 0};
-    int dl = (d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (DispSel.cpp:96)
-#pragma unroll 8
-    for (; dl < d_count; ++dl) {
-        const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
-        const int d = d_begin + dl;
-        if (c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
-        if (c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
-        if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
-        if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
-    }
+    wta_scan4(p, plane, d_begin, d_count, true, mc, md);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const int x = x4 + j;
         if (x < W) {
             if (dis) dis[(size_t)y * W + x] = (T)md[j];
-            if (keys) keys[(size_t)y * W + x] = ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j];
+            if (keys) keys[(size_t)y * W + x] = wta_key(mc[j], md[j]);
         }
     }
 }
 
 // WTA of one block of slices of a blocked context (psm_create_blocked), both views in one launch (blockIdx.z = view):
-// the wta_kernel scan over the block's d_count slices starting at global d_begin, then its packed (cost, d) key is
-// stored (first block) or folded into the running key by min.  The min over keys of consecutive blocks is the
+// wta_scan4 over the block's d_count slices starting at global d_begin, then its wta_key is stored (first block) or
+// folded into the running key by min.  The min over keys of consecutive blocks is the
 // selection over their union: the strict <, the lowest-d tie-break and +inf / NaN costs behave as in one scan.
 struct FoldParams {
     const float* vol[2];             // the block's filtered volumes [d_count][H][Wp]
@@ -614,22 +628,13 @@ __global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
     const float* p = (view ? P.vol[1] : P.vol[0]) + (size_t)y * P.Wp + x4;
     float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
     int md[4] = {0, 0, 0, 0};
-    int dl = (P.d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (DispSel.cpp:96)
-#pragma unroll 8
-    for (; dl < P.d_count; ++dl) {
-        const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
-        const int d = P.d_begin + dl;
-        if (c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
-        if (c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
-        if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
-        if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
-    }
+    wta_scan4(p, plane, P.d_begin, P.d_count, true, mc, md);
     unsigned long long* k = (view ? P.keys[1] : P.keys[0]) + (size_t)y * P.W;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const int x = x4 + j;
         if (x < P.W) {
-            unsigned long long v = ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j];
+            unsigned long long v = wta_key(mc[j], md[j]);
             if (!P.first) {
                 const unsigned long long old = k[x];
                 v = old < v ? old : v;
@@ -642,7 +647,7 @@ __global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
 // Sharded WTA fused with its exchange (reduce-scatter + all-gather of a min-reduction, hand-rolled
 // over NVLink peer memory).  Pixels are partitioned into `nranks` chunks; rank r is the reducer of
 // chunk r.
-//   wta_scatter_kernel : the WTA scan of wta_kernel, then the packed (cost,d) minimum of every pixel
+//   wta_scatter_kernel : wta_scan4 over the filtered volume, then the wta_key minimum of every pixel
 //                        is stored into its reducer's exchange block, slot [this rank][pixel-in-chunk]
 //                        (peer device memory, plain st.global over NVLink) -- compute + scatter in one kernel;
 //                        its last CTA then raises this rank's ARRIVE flag in every peer's block;
@@ -757,18 +762,9 @@ __global__ void __launch_bounds__(256) wta_scatter_kernel(const float* __restric
         const float* p = vol + (size_t)y * Wp + (active ? x4 : 0);
         float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
         int md[4] = {0, 0, 0, 0};
-        int dl = (d_begin == 0) ? 1 : 0;
-#pragma unroll 8
-        for (; active && dl < d_count; ++dl) {
-            const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
-            const int d = d_begin + dl;
-            if (c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
-            if (c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
-            if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
-            if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
-        }
+        wta_scan4(p, plane, d_begin, d_count, active, mc, md);
         p2p_store_row(stage[warp], peers, W, y, x4 - 4 * lane, lane,
-                      [&](int j) { return ((unsigned long long)float_order_key(mc[j]) << 32) | (unsigned)md[j]; });
+                      [&](int j) { return wta_key(mc[j], md[j]); });
     }
     if (peers.seq) p2p_publish(peers, 0);   // ARRIVE
 }
