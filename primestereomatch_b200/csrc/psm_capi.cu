@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstring>
 #include <new>
+#include <type_traits>
 
 #include <cmath>
 
@@ -73,7 +74,7 @@ struct psm_ctx {
     int p2p_sync = 1;                       // 1: device-side ARRIVE/DONE flags; 0: the caller separates the kernels by its own barriers
     float* alloc[16] = {};                  // raw cudaMalloc pointers behind the halo-offset pointers above
     int nalloc = 0;
-    int* slice_flags = nullptr;             // [2][d_count] device flags: slices the reference-order pass filters again
+    int* slice_flags = nullptr;             // [2][res.count] device flags: slices the reference-order pass filters again
     bool slices_flagged = false;            // some slice flag is set (psm_write_cost_slice found a special cost)
     bool float_images = false;              // the current images came in as floats: the ingest flags may be set
     double* ref_rs = nullptr;               // reference-order scratch (psm_cvf_ref.cuh): [4][H][W] row sums, lazy
@@ -98,7 +99,10 @@ struct psm_ctx {
     // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
     // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
     int blk_slices = 0;
-    int res_begin = 0, res_count = 0;       // blocked: the global slices resident in the volumes
+    // The global slices [begin, begin + count) the volumes and the per-slice scratch hold, which every launcher works on:
+    // the owned range on an unblocked context; on a blocked one nothing before psm_cost_const, then its first block,
+    // each block in turn during a filter stage's walk and the last block after it.
+    struct Slices { int begin, count; } res = {0, 0};
     unsigned long long* run_keys[2] = {nullptr, nullptr};  // blocked: running (cost, d) keys per view, [H][W]
     int vol_slices() const { return blk_slices ? blk_slices : d_count; }   // slices the volumes and per-slice scratch hold
     // psm_create_multi: the context drives nshards shard contexts (shard k on its own device, owning the slices
@@ -349,7 +353,7 @@ int launch_guide(psm_ctx* c);
 int clear_slice_flags(psm_ctx* c)
 {
     if (!c->slices_flagged) return PSM_OK;
-    PSM_CUDA(c, cudaMemsetAsync(c->slice_flags, 0, 2 * (size_t)c->d_count * sizeof(int), c->stream));
+    PSM_CUDA(c, cudaMemsetAsync(c->slice_flags, 0, 2 * (size_t)c->vol_slices() * sizeof(int), c->stream));
     c->slices_flagged = false;
     return PSM_OK;
 }
@@ -374,7 +378,7 @@ int launch_ref(psm_ctx* c, void* kernel, int mode, int one_view = 0, int one_d =
     P.guide_flags = c->guide_flags;
     P.slice_flags = c->slice_flags;
     P.rs = c->ref_rs; P.pl = c->ref_pl;
-    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->d_count;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->res.count;
     P.K = c->gif_win; P.a = c->gif_win / 2;
     P.scale = 1.0 / ((double)P.K * P.K);
     P.eps = c->gif_eps;
@@ -429,6 +433,85 @@ int launch_guide(psm_ctx* c)
     return PSM_OK;
 }
 
+// FastGuidedFilter(img, r = GIF_R_WIN, eps = GIF_EPS, s) (DispEst.cpp:283-284) at rate s: box K = 2 * (r / s) + 1 at low
+// resolution
+FgfGeom fgf_geom(const psm_ctx* c, int s)
+{
+    FgfGeom g;
+    g.W = c->W; g.H = c->H; g.Wp = c->Wp; g.s = s; g.w2 = c->W / s; g.h2 = c->H / s; g.K = 2 * (c->gif_win / s) + 1;
+    g.ifx = 1.0 / ((double)g.w2 / g.W); g.ify = 1.0 / ((double)g.h2 / g.H);
+    return g;
+}
+
+// The Fast Guided Filter at rate s: PSM_EINVAL for a rate it does not take; otherwise the low-resolution buffers and the
+// INTER_LINEAR plan, (re)built when the rate changes
+int ensure_fgf(psm_ctx* c, int s)
+{
+    if (s != 1 && s != 2 && s != 4 && s != 8) return fail(c, PSM_EINVAL, "sub-sampling rate must be 1, 2, 4 or 8 (got %d)", s);
+    if (c->W / s < 1 || c->H / s < 1) return fail(c, PSM_EINVAL, "image smaller than the sub-sampling rate");
+    const FgfGeom g = fgf_geom(c, s);
+    int smem_max = 0;
+    PSM_CUDA(c, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    if (fgf_smem_bytes(g.K) > (size_t)smem_max)
+        return fail(c, PSM_EINVAL, "Fast Guided Filter box %d (window %d, rate %d) needs %zu bytes of shared memory, more than "
+                    "the %d a block may have", g.K, c->gif_win, s, fgf_smem_bytes(g.K), smem_max);
+    if (c->fgf_s == s) return PSM_OK;
+    const size_t n2 = (size_t)g.w2 * g.h2;
+    cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
+    c->fgf_lo[0] = c->fgf_lo[1] = c->fgf_mean = nullptr; c->fgf_plan = nullptr; c->fgf_s = 0;
+    for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->fgf_lo[v], 12 * n2 * sizeof(float)));
+    PSM_CUDA(c, cudaMalloc(&c->fgf_mean, (size_t)4 * c->vol_slices() * n2 * sizeof(float)));
+    PSM_CUDA(c, cudaMalloc(&c->fgf_plan, (size_t)(c->W + c->H) * sizeof(FgfTap)));
+    // cv::resize INTER_LINEAR coordinates (OpenCV's own implementation; same expressions as the CPU restatement fgf_build in oracle/)
+    FgfTap* hp = new (std::nothrow) FgfTap[c->W + c->H];
+    if (!hp) return fail(c, PSM_ENOMEM, "out of host memory");
+    { const double sc = (double)g.w2 / g.W;
+      for (int x = 0; x < c->W; ++x) {
+          float f = (float)((x + 0.5) * sc - 0.5); int i = (int)floorf(f); f -= (float)i;
+          if (i < 0) { f = 0.f; i = 0; }
+          if (i >= g.w2 - 1) { f = 0.f; i = g.w2 - 1; }
+          hp[x].i0 = i; hp[x].i1 = i + 1 < g.w2 ? i + 1 : g.w2 - 1; hp[x].f = f; hp[x].pad = 0.f; } }
+    { const double sc = (double)g.h2 / g.H;
+      for (int y = 0; y < c->H; ++y) {
+          float f = (float)((y + 0.5) * sc - 0.5); int i = (int)floorf(f); f -= (float)i;
+          FgfTap& t = hp[c->W + y];
+          t.i0 = i < 0 ? 0 : (i > g.h2 - 1 ? g.h2 - 1 : i);
+          t.i1 = i + 1 < 0 ? 0 : (i + 1 > g.h2 - 1 ? g.h2 - 1 : i + 1);
+          t.f = f; t.pad = 0.f; } }
+    cudaError_t e = cudaMemcpy(c->fgf_plan, hp, (size_t)(c->W + c->H) * sizeof(FgfTap), cudaMemcpyHostToDevice);
+    delete[] hp;
+    PSM_CUDA(c, e);
+    c->fgf_s = s;
+    return PSM_OK;
+}
+
+// The Fast Guided Filter at rate s, view by view: the view's low-resolution guide if `guide`, then the filter of its
+// resident slices if `slices`
+int fgf_views(psm_ctx* c, int s, bool guide, bool slices)
+{
+    const FgfGeom g = fgf_geom(c, s);
+    FgfPlan pl;
+    pl.x = static_cast<const FgfTap*>(c->fgf_plan);
+    pl.y = pl.x + c->W;
+    for (int v = 0; v < c->views; ++v) {
+        if (guide) {
+            dim3 blk(128), g2((g.w2 + 127) / 128, g.h2);
+            fgf_guide_kernel<<<g2, blk, 0, c->stream>>>(c->guide[v], c->plane, g, c->gif_eps, c->fgf_lo[v]);
+            PSM_LAUNCH_CHECK(c);
+        }
+        if (!slices) continue;
+        dim3 blk(128);
+        dim3 g3((g.w2 + kFgfTX - 1) / kFgfTX, (g.h2 + kFgfTY - 1) / kFgfTY, c->res.count);
+        const size_t fsmem = fgf_smem_bytes(g.K);
+        PSM_CUDA(c, cudaFuncSetAttribute(fgf_lowres_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+        fgf_lowres_kernel<<<g3, kFgfThreads, fsmem, c->stream>>>(c->vol[v], c->plane, g, c->fgf_lo[v], c->fgf_mean);
+        PSM_LAUNCH_CHECK(c);
+        dim3 g5((((c->W + 3) / 4) + 127) / 128, c->H, c->res.count);
+        fgf_up_kernel<<<g5, blk, 0, c->stream>>>(c->vol[v], c->plane, c->guide[v], c->plane, g, pl, c->fgf_mean);
+        PSM_LAUNCH_CHECK(c);
+    }
+    return PSM_OK;
+}
 
 // Row segmentation of the streaming kernel: segments are multiples of 8 rows, >= 16 rows, and the
 // last one keeps >= 8 rows so that only the first/last segment ever sees a reflected row.
@@ -508,13 +591,13 @@ int launch_cvf_stream(psm_ctx* c)
 {
     CvfParams P;
     for (int v = 0; v < 2; ++v) { P.vol_in[v] = c->vol[v]; P.vol_out[v] = c->vol_alt[v]; P.guide[v] = c->guide[v]; }
-    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->d_count;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->res.count;
     // the packed remainder needs no CTA-level staging (variant 9 stages the guide rows of one strip); variants 1 and 2
     // keep the plain decomposition of the round-1 kernel; option 105 = 1 disables it
     const bool plain_variant = c->cvf_variant == 9 || c->cvf_variant == 2 || (c->cvf_mode != PSM_CVF_MIXED && c->cvf_variant == 1);
     int nsm = 0;
     PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
-    const CvfPlan plan = plan_cvf(c->W, c->H, c->d_count, nsm, c->cvf_threads, c->cvf_target_rows,
+    const CvfPlan plan = plan_cvf(c->W, c->H, c->res.count, nsm, c->cvf_threads, c->cvf_target_rows,
                                   !c->cvf_no_pack && !plain_variant && !c->cvf_remap, c->views);
     const int nthreads = plan.nthreads;
     P.nstrips = plan.nstrips; P.ndgroups = plan.ndgroups; P.nseg = plan.nseg; P.seg_rows = plan.seg_rows;
@@ -591,7 +674,7 @@ int launch_cvf_window(psm_ctx* c)
 {
     WinParams P;
     for (int v = 0; v < 2; ++v) { P.vol_in[v] = c->vol[v]; P.vol_out[v] = c->vol_alt[v]; P.guide[v] = c->guide[v]; }
-    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->d_count;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.Dloc = c->res.count;
     P.K = c->gif_win; P.a = c->gif_win / 2;
     P.scale = 1.0 / ((double)P.K * P.K);
     P.tw = kWinThreads - 2 * P.K + 2;
@@ -614,7 +697,7 @@ int launch_cvf_window(psm_ctx* c)
     return PSM_OK;
 }
 
-// K1: both raw volumes of the context's slice range
+// K1: both raw volumes of the resident slices
 int launch_cvc(psm_ctx* c)
 {
     CvcParams2 P2;
@@ -626,83 +709,59 @@ int launch_cvc(psm_ctx* c)
         P.self[3] = c->grd[v];
         P.other[3] = c->grd[1 - v];
         P.vol = c->vol[v];
-        P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count;
+        P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->res.begin; P.d_count = c->res.count;
         P.fold_halo = c->W >= 32 ? 1 : 0;
     }
-    // option 108 (tuning): slices per CTA (0 = all owned slices in one CTA, the shipped decomposition)
-    P2.chunk = (c->cvc_chunk > 0 && c->cvc_chunk < c->d_count) ? c->cvc_chunk : 0;
-    const int nchunks = P2.chunk ? (c->d_count + P2.chunk - 1) / P2.chunk : 1;
+    // option 108 (tuning): slices per CTA (0 = all resident slices in one CTA, the shipped decomposition)
+    P2.chunk = (c->cvc_chunk > 0 && c->cvc_chunk < c->res.count) ? c->cvc_chunk : 0;
+    const int nchunks = P2.chunk ? (c->res.count + P2.chunk - 1) / P2.chunk : 1;
     dim3 blk(128), grd((((c->W + 3) / 4) + 127) / 128, c->H, c->views * nchunks);
     // option 106 (tuning): 0 shipped = interior fast path + scalar window loads; 2 = no fast path (the round-1 loop);
     // 1 / 3 = fast path + grouped 128-bit window loads for the border warps without / with a register cap (DESIGN.md section 10)
-    // Any matching cost other than the default runs the parameterised build of the shipped variant, all owned slices
+    const auto both = [&](auto nviews) {
+        constexpr int NV = decltype(nviews)::value;
+        switch (c->cvc_variant) {
+        case 1: cvc_both_kernel<4, 1, NV><<<grd, blk, 0, c->stream>>>(P2); break;
+        case 2: cvc_both_kernel<7, 2, NV><<<grd, blk, 0, c->stream>>>(P2); break;
+        case 3: cvc_both_kernel<5, 1, NV><<<grd, blk, 0, c->stream>>>(P2); break;
+        default: cvc_both_kernel<7, 0, NV><<<grd, blk, 0, c->stream>>>(P2); break;
+        }
+    };
+    // Any matching cost other than the default runs the parameterised build of the shipped variant, all resident slices
     // per CTA: options 106 and 108 do not apply to it.  A left-only context runs the one-view builds.
     if (!c->cost_default()) {
         grd.z = c->views;
         if (c->views == 2) cvc_cost_kernel<<<grd, blk, 0, c->stream>>>(P2, c->cost);
         else cvc_cost_kernel<1><<<grd, blk, 0, c->stream>>>(P2, c->cost);
     } else if (c->views == 2) {
-        switch (c->cvc_variant) {
-        case 1: cvc_both_kernel<4, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        case 2: cvc_both_kernel<7, 2><<<grd, blk, 0, c->stream>>>(P2); break;
-        case 3: cvc_both_kernel<5, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        default: cvc_both_kernel<7, 0><<<grd, blk, 0, c->stream>>>(P2); break;
-        }
+        both(std::integral_constant<int, 2>());
     } else {
-        switch (c->cvc_variant) {
-        case 1: cvc_both_kernel<4, 1, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        case 2: cvc_both_kernel<7, 2, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        case 3: cvc_both_kernel<5, 1, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        default: cvc_both_kernel<7, 0, 1><<<grd, blk, 0, c->stream>>>(P2); break;
-        }
+        both(std::integral_constant<int, 1>());
     }
     PSM_LAUNCH_CHECK(c);
     if (!P2.v[0].fold_halo)  // narrow images: separate halo pass (general reflection)
         for (int v = 0; v < c->views; ++v)
-            if (int rc = pad_rows(c, c->vol[v], (size_t)c->d_count * c->H)) return rc;
+            if (int rc = pad_rows(c, c->vol[v], (size_t)c->res.count * c->H)) return rc;
     return PSM_OK;
 }
-
-// A blocked context runs the launchers above, which take their slice range from the context, on one block: for the
-// scope's life the context's range is the block's, and its volumes hold that block.
-struct BlockScope {
-    psm_ctx* c;
-    int begin, count;
-    BlockScope(psm_ctx* ctx, int b, int n) : c(ctx), begin(ctx->d_begin), count(ctx->d_count)
-    {
-        c->d_begin = b; c->d_count = n;
-        c->res_begin = b; c->res_count = n;
-    }
-    ~BlockScope() { c->d_begin = begin; c->d_count = count; }
-};
 
 // the filtered block in the volumes -> the running keys (stored by the first block, min-folded by the others)
 int launch_fold(psm_ctx* c, bool first)
 {
     FoldParams P;
     for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
-    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count; P.first = first ? 1 : 0;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->res.begin; P.d_count = c->res.count; P.first = first ? 1 : 0;
     dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, c->views);
     wta_fold_kernel<<<grd, blk, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
 
-// A blocked context's filter stage: every block of [d_begin, d_begin + d_count) in turn gets its raw costs (the first
-// block's are psm_cost_const's), `filter` (which leaves the filtered block in c->vol) and the fold into the running keys.
-template <class Filter>
-int run_blocks(psm_ctx* c, Filter filter)
+// The slices the volumes hold while the context's stages work from global slice `b` on: up to vol_slices() of the owned
+// range, so the owned range itself on an unblocked context and the block starting at b on a blocked one.
+psm_ctx::Slices block_at(const psm_ctx* c, int b)
 {
-    const int end = c->d_begin + c->d_count;
-    for (int b = c->d_begin; b < end; b += c->blk_slices) {
-        const bool first = b == c->d_begin;
-        BlockScope scope(c, b, std::min(c->blk_slices, end - b));
-        if (!first)
-            if (int rc = launch_cvc(c)) return rc;
-        if (int rc = filter()) return rc;
-        if (int rc = launch_fold(c, first)) return rc;
-    }
-    return PSM_OK;
+    return {b, std::min(c->vol_slices(), c->d_begin + c->d_count - b)};
 }
 
 // The destinations of a map call `call`: rows of W elements of the map format, the right map's on a two-view context only.
@@ -898,6 +957,70 @@ int ctx_parts(psm_ctx* c, psm_ctx** parts)
     return c->nshards;
 }
 
+// psm_cost_filter: the MIXED and NAIVE modes exist for the default guided filter alone
+int check_cvf_mode(psm_ctx* c)
+{
+    if (!c->gif_default() && c->cvf_mode != PSM_CVF_EXACT)
+        return fail(c, PSM_EINVAL, "CVF mode %s exists only for the default guided filter (window 8, eps 1e-4); "
+                    "this context has window %d, eps %g: use PSM_CVF_EXACT", c->cvf_mode == PSM_CVF_MIXED ? "MIXED" : "NAIVE",
+                    c->gif_win, (double)c->gif_eps);
+    return PSM_OK;
+}
+
+// psm_cost_filter on the resident slices.  NAIVE and images below one strip: every slice in OpenCV's order.  Otherwise
+// the tuned kernel, then, in OpenCV's order, the slices psm_write_cost_slice flagged and every slice of a view whose image
+// is outside the integer domain or whose solve terms are not finite (psm_cvf_ref.cuh).  The second launch is needed only
+// where a flag can be set: flagged slices, float images, a non-default window or eps.  u8 frames at the defaults run the
+// tuned kernel alone.
+int cvf_block(psm_ctx* c)
+{
+    if (c->gif_default() && (c->cvf_mode == PSM_CVF_NAIVE || c->W < 16 || c->H < 16)) {
+        if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAll)) return rc;
+    } else {
+        if (int rc = c->gif_default() ? launch_cvf_stream(c) : launch_cvf_window(c)) return rc;
+        if (c->slices_flagged || c->float_images || !c->gif_default())
+            if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefFlagged)) return rc;
+    }
+    if (int rc = clear_slice_flags(c)) return rc;
+    // the right view's pair is not swapped on a left-only context: its volume buffers keep their roles
+    for (int v = 0; v < c->views; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
+    return PSM_OK;
+}
+
+// The filter stage of entry point `call`.  `prepare` checks the entry point's own arguments and sets up its buffers; then
+// stage 2 runs `guide` once and `filter`, which leaves the resident slices filtered in c->vol, on the range.  An unblocked
+// context filters every slice it owns in one pass, timed as stage 4.  A blocked context walks its range block by block:
+// the block's raw costs (psm_cost_const built the first block's), `filter`, and the fold into the running keys.  It
+// records no stage 4, whose kernels would interleave with every block's CVC and fold.
+template <class Prepare, class Guide, class Filter>
+int filter_stage(psm_ctx* c, const char* call, Prepare prepare, Guide guide, Filter filter)
+{
+    if (is_multi(c)) return forward(c, [&](psm_ctx* s) { return filter_stage(s, call, prepare, guide, filter); });
+    if (int rc = bind(c)) return rc;
+    if (int rc = check_views_reset(c, call)) return rc;
+    if (!c->have_cvc) return fail(c, PSM_ESTATE, "%s before psm_cost_const", call);
+    if (int rc = prepare(c)) return rc;
+    if (int rc = stage_begin(c, 2)) return rc;
+    if (int rc = guide(c)) return rc;
+    if (!c->blk_slices) {
+        if (int rc = stage_begin(c, 4)) return rc;
+        if (int rc = filter(c)) return rc;
+        if (int rc = stage_end(c, 4)) return rc;
+    } else {
+        for (int b = c->d_begin; b < c->d_begin + c->d_count; b += c->blk_slices) {
+            const bool first = b == c->d_begin;
+            c->res = block_at(c, b);
+            if (!first)
+                if (int rc = launch_cvc(c)) return rc;
+            if (int rc = filter(c)) return rc;
+            if (int rc = launch_fold(c, first)) return rc;
+        }
+    }
+    c->have_cvc = false;  // the volumes now hold filtered costs; filtering again needs a new CVC
+    c->filtered = true;
+    return stage_end(c, 2);
+}
+
 }  // namespace
 
 // ----------------------------------------------------------------------------------------------
@@ -942,6 +1065,7 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
     c->plane = (size_t)c->H * c->Wp;
     c->map_bytes = map_bytes;
     c->blk_slices = block_slices;
+    if (!block_slices) c->res = {d_begin, d_count};
     auto bail = [&](int code) {
         snprintf(g_create_error, sizeof(g_create_error), "%s", c->err);
         psm_destroy(c);
@@ -1424,14 +1548,8 @@ int psm_cost_const(psm_ctx* c)
     if (int rc = bind(c)) return rc;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_cost_const before psm_set_images");
     if (int rc = stage_begin(c, 1)) return rc;
-    int rc;
-    if (c->blk_slices) {   // the first block; the filter stages build the others
-        BlockScope scope(c, c->d_begin, c->blk_slices);
-        rc = launch_cvc(c);
-    } else {
-        rc = launch_cvc(c);
-    }
-    if (rc) return rc;
+    c->res = block_at(c, c->d_begin);   // a blocked context's first block; the filter stages build the others
+    if (int rc = launch_cvc(c)) return rc;
     if (int rc = clear_slice_flags(c)) return rc;
     c->have_cvc = true;
     c->filtered = false;
@@ -1441,135 +1559,17 @@ int psm_cost_const(psm_ctx* c)
 
 int psm_cost_filter(psm_ctx* c)
 {
-    if (is_multi(c)) return forward(c, [](psm_ctx* s) { return psm_cost_filter(s); });
-    if (int rc = bind(c)) return rc;
-    if (int rc = check_views_reset(c, "psm_cost_filter")) return rc;
-    if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter before psm_cost_const");
-    if (!c->gif_default() && c->cvf_mode != PSM_CVF_EXACT)
-        return fail(c, PSM_EINVAL, "CVF mode %s exists only for the default guided filter (window 8, eps 1e-4); "
-                    "this context has window %d, eps %g: use PSM_CVF_EXACT", c->cvf_mode == PSM_CVF_MIXED ? "MIXED" : "NAIVE",
-                    c->gif_win, (double)c->gif_eps);
-    if (int rc = stage_begin(c, 2)) return rc;
-    if (int rc = ensure_guide(c)) return rc;
-    // NAIVE and images below one strip: every slice in OpenCV's order.  Otherwise the tuned kernel, then, in OpenCV's
-    // order, the slices psm_write_cost_slice flagged and every slice of a view whose image is outside the integer domain
-    // or whose solve terms are not finite (psm_cvf_ref.cuh).  The second launch is needed only where a flag can be set:
-    // flagged slices, float images, a non-default window or eps.  u8 frames at the defaults run the tuned kernel alone.
-    const auto filter = [c]() -> int {
-        if (c->gif_default() && (c->cvf_mode == PSM_CVF_NAIVE || c->W < 16 || c->H < 16)) {
-            if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAll)) return rc;
-        } else {
-            if (int rc = c->gif_default() ? launch_cvf_stream(c) : launch_cvf_window(c)) return rc;
-            if (c->slices_flagged || c->float_images || !c->gif_default())
-                if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefFlagged)) return rc;
-        }
-        if (int rc = clear_slice_flags(c)) return rc;
-        // the right view's pair is not swapped on a left-only context: its volume buffers keep their roles
-        for (int v = 0; v < c->views; ++v) { float* t = c->vol[v]; c->vol[v] = c->vol_alt[v]; c->vol_alt[v] = t; }
-        return PSM_OK;
-    };
-    if (c->blk_slices) {   // stage 4 is not recorded: its kernels interleave with every block's CVC and fold
-        if (int rc = run_blocks(c, filter)) return rc;
-    } else {
-        if (int rc = stage_begin(c, 4)) return rc;
-        if (int rc = filter()) return rc;
-        if (int rc = stage_end(c, 4)) return rc;
-    }
-    c->have_cvc = false;  // the volumes now hold filtered costs; filtering again needs a new CVC
-    c->filtered = true;
-    return stage_end(c, 2);
+    return filter_stage(c, "psm_cost_filter", check_cvf_mode, ensure_guide, cvf_block);
 }
 
-// DispEst::CostFilter_FGF (reference src/DispEst.cpp:281-296): Fast Guided Filter with sub-sampling rate s
+// DispEst::CostFilter_FGF (reference src/DispEst.cpp:281-296): Fast Guided Filter with sub-sampling rate s.  An unblocked
+// context computes each view's low-resolution guide just before that view's slices; a blocked one computes both guides
+// before its walk.
 int psm_cost_filter_fgf(psm_ctx* c, int s)
 {
-    if (is_multi(c)) return forward(c, [s](psm_ctx* sh) { return psm_cost_filter_fgf(sh, s); });
-    if (int rc = bind(c)) return rc;
-    if (int rc = check_views_reset(c, "psm_cost_filter_fgf")) return rc;
-    if (!c->have_cvc) return fail(c, PSM_ESTATE, "psm_cost_filter_fgf before psm_cost_const");
-    if (s != 1 && s != 2 && s != 4 && s != 8) return fail(c, PSM_EINVAL, "sub-sampling rate must be 1, 2, 4 or 8 (got %d)", s);
-    if (c->W / s < 1 || c->H / s < 1) return fail(c, PSM_EINVAL, "image smaller than the sub-sampling rate");
-    FgfGeom g;
-    // FastGuidedFilter(img, r = GIF_R_WIN, eps = GIF_EPS, s) (DispEst.cpp:283-284): box K = 2 * (r / s) + 1 at low resolution
-    g.W = c->W; g.H = c->H; g.Wp = c->Wp; g.s = s; g.w2 = c->W / s; g.h2 = c->H / s; g.K = 2 * (c->gif_win / s) + 1;
-    {
-        int smem_max = 0;
-        PSM_CUDA(c, cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
-        if (fgf_smem_bytes(g.K) > (size_t)smem_max)
-            return fail(c, PSM_EINVAL, "Fast Guided Filter box %d (window %d, rate %d) needs %zu bytes of shared memory, more than "
-                        "the %d a block may have", g.K, c->gif_win, s, fgf_smem_bytes(g.K), smem_max);
-    }
-    g.ifx = 1.0 / ((double)g.w2 / g.W); g.ify = 1.0 / ((double)g.h2 / g.H);
-    const size_t n2 = (size_t)g.w2 * g.h2;
-    if (c->fgf_s != s) {   // (re)build buffers and the INTER_LINEAR plan for this rate
-        cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
-        c->fgf_lo[0] = c->fgf_lo[1] = c->fgf_mean = nullptr; c->fgf_plan = nullptr; c->fgf_s = 0;
-        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->fgf_lo[v], 12 * n2 * sizeof(float)));
-        PSM_CUDA(c, cudaMalloc(&c->fgf_mean, (size_t)4 * c->vol_slices() * n2 * sizeof(float)));
-        PSM_CUDA(c, cudaMalloc(&c->fgf_plan, (size_t)(c->W + c->H) * sizeof(FgfTap)));
-        // cv::resize INTER_LINEAR coordinates (OpenCV's own implementation; same expressions as the CPU restatement fgf_build in oracle/)
-        FgfTap* hp = new (std::nothrow) FgfTap[c->W + c->H];
-        if (!hp) return fail(c, PSM_ENOMEM, "out of host memory");
-        { const double sc = (double)g.w2 / g.W;
-          for (int x = 0; x < c->W; ++x) {
-              float f = (float)((x + 0.5) * sc - 0.5); int i = (int)floorf(f); f -= (float)i;
-              if (i < 0) { f = 0.f; i = 0; }
-              if (i >= g.w2 - 1) { f = 0.f; i = g.w2 - 1; }
-              hp[x].i0 = i; hp[x].i1 = i + 1 < g.w2 ? i + 1 : g.w2 - 1; hp[x].f = f; hp[x].pad = 0.f; } }
-        { const double sc = (double)g.h2 / g.H;
-          for (int y = 0; y < c->H; ++y) {
-              float f = (float)((y + 0.5) * sc - 0.5); int i = (int)floorf(f); f -= (float)i;
-              FgfTap& t = hp[c->W + y];
-              t.i0 = i < 0 ? 0 : (i > g.h2 - 1 ? g.h2 - 1 : i);
-              t.i1 = i + 1 < 0 ? 0 : (i + 1 > g.h2 - 1 ? g.h2 - 1 : i + 1);
-              t.f = f; t.pad = 0.f; } }
-        cudaError_t e = cudaMemcpy(c->fgf_plan, hp, (size_t)(c->W + c->H) * sizeof(FgfTap), cudaMemcpyHostToDevice);
-        delete[] hp;
-        PSM_CUDA(c, e);
-        c->fgf_s = s;
-    }
-    FgfPlan pl;
-    pl.x = static_cast<const FgfTap*>(c->fgf_plan);
-    pl.y = pl.x + c->W;
-    // the low-resolution guide of view v, then the filter of view v's resident slices
-    const auto guide = [&](int v) -> int {
-        dim3 blk(128), g2((g.w2 + 127) / 128, g.h2);
-        fgf_guide_kernel<<<g2, blk, 0, c->stream>>>(c->guide[v], c->plane, g, c->gif_eps, c->fgf_lo[v]);
-        PSM_LAUNCH_CHECK(c);
-        return PSM_OK;
-    };
-    const auto slices = [&](int v) -> int {
-        dim3 blk(128);
-        dim3 g3((g.w2 + kFgfTX - 1) / kFgfTX, (g.h2 + kFgfTY - 1) / kFgfTY, c->d_count);
-        const size_t fsmem = fgf_smem_bytes(g.K);
-        PSM_CUDA(c, cudaFuncSetAttribute(fgf_lowres_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-        fgf_lowres_kernel<<<g3, kFgfThreads, fsmem, c->stream>>>(c->vol[v], c->plane, g, c->fgf_lo[v], c->fgf_mean);
-        PSM_LAUNCH_CHECK(c);
-        dim3 g5((((c->W + 3) / 4) + 127) / 128, c->H, c->d_count);
-        fgf_up_kernel<<<g5, blk, 0, c->stream>>>(c->vol[v], c->plane, c->guide[v], c->plane, g, pl, c->fgf_mean);
-        PSM_LAUNCH_CHECK(c);
-        return PSM_OK;
-    };
-    if (int rc = stage_begin(c, 2)) return rc;
-    if (c->blk_slices) {   // the guides once, then every block; stage 4 is not recorded
-        for (int v = 0; v < c->views; ++v)
-            if (int rc = guide(v)) return rc;
-        if (int rc = run_blocks(c, [&]() -> int {
-                for (int v = 0; v < c->views; ++v)
-                    if (int rc = slices(v)) return rc;
-                return PSM_OK;
-            })) return rc;
-    } else {
-        if (int rc = stage_begin(c, 4)) return rc;
-        for (int v = 0; v < c->views; ++v) {
-            if (int rc = guide(v)) return rc;
-            if (int rc = slices(v)) return rc;
-        }
-        if (int rc = stage_end(c, 4)) return rc;
-    }
-    c->have_cvc = false;
-    c->filtered = true;
-    return stage_end(c, 2);
+    return filter_stage(c, "psm_cost_filter_fgf", [s](psm_ctx* c) { return ensure_fgf(c, s); },
+                        [s](psm_ctx* c) { return fgf_views(c, s, c->blk_slices != 0, false); },
+                        [s](psm_ctx* c) { return fgf_views(c, s, c->blk_slices == 0, true); });
 }
 
 }  // extern "C"
@@ -2124,9 +2124,9 @@ static int check_slice(psm_ctx* c, int view, int d)
     if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
     if (d < c->d_begin || d >= c->d_begin + c->d_count)
         return fail(c, PSM_EINVAL, "slice %d not owned by this context [%d,%d)", d, c->d_begin, c->d_begin + c->d_count);
-    if (c->blk_slices && (d < c->res_begin || d >= c->res_begin + c->res_count))
+    if (d < c->res.begin || d >= c->res.begin + c->res.count)
         return fail(c, PSM_EINVAL, "slice %d is not resident: this blocked context holds slices [%d,%d) only (the first block "
-                    "after psm_cost_const, the last after a filter stage)", d, c->res_begin, c->res_begin + c->res_count);
+                    "after psm_cost_const, the last after a filter stage)", d, c->res.begin, c->res.begin + c->res.count);
     return PSM_OK;
 }
 
@@ -2144,7 +2144,7 @@ static int route_slice(psm_ctx* c, int d, F f)
 extern "C" {
 
 // the offset of a checked slice in the volumes
-static size_t slice_offset(const psm_ctx* c, int d) { return (size_t)(d - (c->blk_slices ? c->res_begin : c->d_begin)) * c->plane; }
+static size_t slice_offset(const psm_ctx* c, int d) { return (size_t)(d - c->res.begin) * c->plane; }
 
 int psm_read_cost_slice(psm_ctx* c, int view, int d, float* dst, size_t dst_step)
 {
@@ -2169,9 +2169,9 @@ int psm_write_cost_slice(psm_ctx* c, int view, int d, const float* src, size_t s
                     "first from the images, so a written slice would not be filtered");
     if (int rc = check_slice(c, view, d)) return rc;
     if (!src || src_step < (size_t)c->W * sizeof(float)) return fail(c, PSM_EINVAL, "bad src/step");
-    PSM_CUDA(c, cudaMemcpy2DAsync(c->vol[view] + (size_t)(d - c->d_begin) * c->plane, c->Wp * sizeof(float), src,
-                                  src_step, c->W * sizeof(float), c->H, cudaMemcpyHostToDevice, c->stream));
-    if (int rc = pad_rows(c, c->vol[view] + (size_t)(d - c->d_begin) * c->plane, (size_t)c->H)) return rc;
+    PSM_CUDA(c, cudaMemcpy2DAsync(c->vol[view] + slice_offset(c, d), c->Wp * sizeof(float), src, src_step,
+                                  c->W * sizeof(float), c->H, cudaMemcpyHostToDevice, c->stream));
+    if (int rc = pad_rows(c, c->vol[view] + slice_offset(c, d), (size_t)c->H)) return rc;
     // A negative, -0, inf, NaN or >= 2^63 cost (bit patterns >= that of 2^63; the sign bit sorts last) makes the fp64 box
     // sums order-dependent: flag the slice for the reference-order pass.  psm_cost_const never produces one from images
     // without kGuideOutside, so this is the only other way such a cost enters a volume.
@@ -2182,7 +2182,7 @@ int psm_write_cost_slice(psm_ctx* c, int view, int d, const float* src, size_t s
     }
     if (special) {
         static const int one = 1;
-        PSM_CUDA(c, cudaMemcpyAsync(c->slice_flags + (size_t)view * c->d_count + (d - c->d_begin), &one, sizeof(int),
+        PSM_CUDA(c, cudaMemcpyAsync(c->slice_flags + (size_t)view * c->res.count + (d - c->res.begin), &one, sizeof(int),
                                     cudaMemcpyHostToDevice, c->stream));
         c->slices_flagged = true;
     }
@@ -2225,14 +2225,7 @@ int psm_read_ab_slice(psm_ctx* c, int view, int d, float* a3, float* b)
     if (!c->have_images) return fail(c, PSM_ESTATE, "no images set");
     if (int rc = ensure_guide(c)) return rc;
     // a, b in OpenCV's order (psm_cvf_ref.cuh), left in the scratch planes [4][H][W]
-    int rc;
-    if (c->blk_slices) {
-        BlockScope scope(c, c->res_begin, c->res_count);
-        rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->res_begin);
-    } else {
-        rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->d_begin);
-    }
-    if (rc) return rc;
+    if (int rc = launch_ref(c, (void*)cvf_ref_kernel, kRefAbOnly, view, d - c->res.begin)) return rc;
     const size_t n = (size_t)c->W * c->H;
     PSM_CUDA(c, cudaMemcpyAsync(a3, c->ref_pl, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     PSM_CUDA(c, cudaMemcpyAsync(b, c->ref_pl + 3 * n, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));

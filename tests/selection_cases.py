@@ -6,7 +6,7 @@ for disparity shards, wta_fold_kernel's running keys of a blocked context, the k
 exchange.  The min over keys of disjoint slice ranges is claimed to be the winner-take-all over their union (strict <,
 lowest d on ties, +inf and NaN never win, global d = 0 never a candidate).  This module restates the key
 (psm_common.cuh::float_order_key), the one-scan key of a range of slices, the fold over a partition of the range, and
-the partitions the library makes: blocks of a blocked context (run_blocks) and shards (sharding.shard_range)."""
+the partitions the library makes: blocks of a blocked context (block_at) and shards (sharding.shard_range)."""
 import numpy as np
 
 from primestereomatch_b200.sharding import shard_range

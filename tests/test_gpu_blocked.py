@@ -176,6 +176,38 @@ def test_full_hd_at_d2560():
 
 
 # ---- 7. errors and state ----------------------------------------------------------------------------------------------
+def _check_resident(de, full, lo, hi):
+    """de's slice reads accept exactly the slices [lo, hi) and return full's there; every other slice is not resident
+    where de owns it and not owned elsewhere"""
+    for d in range(de.d_begin - 1, de.d_begin + de.d_count + 1):
+        for view in (0, 1):
+            if lo <= d < hi:
+                assert_same(de.read_cost_slice(view, d), full.read_cost_slice(view, d), f"view {view} slice {d}")
+                (a, b), (a0, b0) = de.read_ab_slice(view, d), full.read_ab_slice(view, d)
+                assert_same(a, a0, f"a of view {view} slice {d}"); assert_same(b, b0, f"b of view {view} slice {d}")
+                continue
+            why = "not resident" if de.d_begin <= d < de.d_begin + de.d_count else "not owned"
+            for read in (de.read_cost_slice, de.read_ab_slice):
+                with pytest.raises(capi.PsmError) as e:
+                    read(view, d)
+                assert e.value.code == capi.PSM_EINVAL and why in str(e.value), (view, d, str(e.value))
+
+
+def _walk(de, full, B, fgf):
+    """one frame's CVC and filter stage through a blocked context and an unblocked one of the same range: the first block
+    is resident after CVC and the last after the filter; stage 4 is not recorded on the blocked context"""
+    L, ms = capi.lib(), C.c_float()
+    end = de.d_begin + de.d_count
+    last = de.d_begin + (de.d_count - 1) // B * B
+    full.CostConst_GPU(); de.CostConst_GPU()
+    _check_resident(de, full, de.d_begin, min(de.d_begin + B, end))
+    assert L.psm_stage_ms(de.handle, 4, C.byref(ms)) == capi.PSM_ESTATE
+    for ctx in (full, de):
+        (ctx.CostFilter_FGF_GPU if fgf else ctx.CostFilter_GPU)()
+    _check_resident(de, full, last, end)
+    assert L.psm_stage_ms(de.handle, 4, C.byref(ms)) == capi.PSM_ESTATE
+
+
 def test_errors_and_state():
     L = capi.lib()
     W, H, D, B = 64, 24, 40, 16
@@ -192,57 +224,79 @@ def test_errors_and_state():
     with DispEst(l, r, D) as full, DispEst(l, r, D, block_slices=B) as de:
         h = de.handle
         # stages out of order
-        assert L.psm_cost_filter(h) == capi.PSM_ESTATE
+        assert L.psm_cost_filter(h) == capi.PSM_ESTATE and b"psm_cost_filter before" in L.psm_last_error(h)
+        assert L.psm_cost_filter_fgf(h, 4) == capi.PSM_ESTATE and b"psm_cost_filter_fgf before" in L.psm_last_error(h)
         assert L.psm_disp_select(h, ptr(u8), W, ptr(u8), W) == capi.PSM_ESTATE
-        assert L.psm_read_cost_slice(h, 0, 1, ptr(sl), 4 * W) == capi.PSM_EINVAL   # nothing resident yet
-        full.CostConst_GPU(); de.CostConst_GPU()
-        # raw costs of the first block are resident; the next block is not
-        for d in (0, 5, B - 1):
-            assert_same(de.read_cost_slice(0, d), full.read_cost_slice(0, d), f"raw slice {d}")
-        a, b = de.read_ab_slice(1, 3)
-        a0, b0 = full.read_ab_slice(1, 3)
-        assert_same(a, a0, "a of slice 3"); assert_same(b, b0, "b of slice 3")
-        for fn in (lambda: de.read_cost_slice(0, B), lambda: de.read_ab_slice(0, D - 1)):
-            with pytest.raises(capi.PsmError) as e:
-                fn()
-            assert e.value.code == capi.PSM_EINVAL and "not resident" in str(e.value)
+        _check_resident(de, full, 0, 0)   # nothing resident yet
+        # the last block (40 = 16 + 16 + 8) holds filtered costs; psm_device_ptr 0 / 1 point at it
+        _walk(de, full, B, fgf=False)
         with pytest.raises(capi.PsmError) as e:
             de.write_cost_slice(0, 1, sl)
         assert e.value.code == capi.PSM_EINVAL and "blocked" in str(e.value)
         with pytest.raises(RuntimeError):
             de.read_cost_volume(0)
-        full.CostFilter_GPU(); de.CostFilter_GPU()
-        # the last block (40 = 16 + 16 + 8) holds filtered costs; psm_device_ptr 0 / 1 point at it
-        for d in (32, D - 1):
-            assert_same(de.read_cost_slice(1, d), full.read_cost_slice(1, d), f"filtered slice {d}")
-        with pytest.raises(capi.PsmError):
-            de.read_cost_slice(1, 31)
         p, pitch = C.c_void_p(), C.c_size_t()
         capi.check(L.psm_device_ptr(h, 0, C.byref(p), C.byref(pitch)), h)
         assert p.value and pitch.value >= W
         assert L.psm_disp_select_keys_p2p(h) == capi.PSM_EINVAL and b"blocked" in L.psm_last_error(h)
         # stage 4 is not recorded on a blocked context; stages 1 and 2 are
-        ms = C.c_float()
-        assert L.psm_stage_ms(h, 4, C.byref(ms)) == capi.PSM_ESTATE
         assert de.stage_ms(1) > 0 and de.stage_ms(2) > 0 and full.stage_ms(4) > 0
         full.DispSelect_GPU(); de.DispSelect_GPU()
         assert_same(de.lDisMap, full.lDisMap, "left"); assert_same(de.rDisMap, full.rDisMap, "right")
         assert de.stage_ms(3) > 0
+        _walk(de, full, B, fgf=True)
+        full.DispSelect_GPU(); de.DispSelect_GPU()
+        assert_same(de.lDisMap, full.lDisMap, "FGF left"); assert_same(de.rDisMap, full.rDisMap, "FGF right")
+    # a shard off its block grid: blocks [7,15) .. [31,39), then [39,40)
+    with DispEst(l, r, D, d_begin=7, d_count=33) as full, DispEst(l, r, D, d_begin=7, d_count=33, block_slices=8) as de:
+        _check_resident(de, full, 7, 7)
+        for fgf in (False, True):
+            _walk(de, full, 8, fgf)
+
+
+# Filter-stage launches (unblocked, at B = 16) on 200 x 40 x 50, whose blocks are 16 + 16 + 16 + 2 slices.  A blocked stage
+# launches its guide kernels once, then per block its filter, the block's CVC after the first block and one fold:
+# guide + 4 x filter + 3 + 4.
+FILTER_LAUNCHES = {
+    "exact": (2, 12),      # guide, streaming filter
+    "mixed": (2, 12),
+    "naive": (2, 12),      # guide, every slice in the reference order
+    "window5": (3, 16),    # generic-window guide; generic-window filter, then the reference-order pass
+    "window16": (3, 16),
+    "cost": (2, 12),
+    # per view: low-resolution guide, low-resolution filter, up-sampling; blocked: both guides, then 4 x 2 views x 2
+    "fgf1": (6, 25), "fgf2": (6, 25), "fgf4": (6, 25), "fgf8": (6, 25),
+    "negative": (4, 17),   # float frames: guide and its reference-order pass; filter and the reference-order pass
+    "above1": (4, 17),
+    "left": (2, 12),       # left-only: the one-view guide and filter
+}
 
 
 def test_launch_counts():
-    """unblocked contexts launch what they did before the blocked path existed; a blocked filter stage launches the guide
-    once, then per block its CVC (after the first), its filter and one fold"""
+    """unblocked contexts launch what they did before the blocked path existed; a blocked filter stage launches its guide
+    once, then per block its CVC (after the first), its filter and one fold.  Every filter path and a left-only context
+    is run; the mismatches of all of them are reported together."""
     W, H, D, B = 200, 40, 50, 16
-    l8, r8, _ = synth.stereo_pair_u8(W, H, D, seed=4)
-    nblocks = -(-D // B)
-    for block, cvc, cvf, sel in ((None, 1, 2, 2), (B, 1, 1 + nblocks + (nblocks - 1) + nblocks, 2)):
-        with DispEst(l8, r8, D, block_slices=block) as de:
-            c = []
-            for stage in (de.CostConst_GPU, de.CostFilter_GPU, de.DispSelect_GPU):
-                n = de.launch_count(); stage(); c.append(de.launch_count() - n)
-            # ingest (2 views x ingest + halo) is part of CostConst_GPU
-            assert c == [4 + cvc, cvf, sel], (block, c)
+    u8 = synth.stereo_pair_u8(W, H, D, seed=4)[:2]
+    bad = []
+    for path, counts in FILTER_LAUNCHES.items():
+        l, r = IC.frame(path, W, H, D) if path in ("negative", "above1") else u8
+        kw = dict(setup=lambda de: de.setViews("left")) if path == "left" else PATHS[path]
+        views = 1 if path == "left" else 2
+        for block, cvf in zip((None, B), counts):
+            with DispEst(l, r, D, block_slices=block) as de:
+                if "setup" in kw:
+                    kw["setup"](de)
+                if "fgf" in kw:
+                    de.setSubsampleRate(kw["fgf"])
+                c = []
+                for stage in (de.CostConst_GPU, de.CostFilter_FGF_GPU if "fgf" in kw else de.CostFilter_GPU,
+                              de.DispSelect_GPU):
+                    n = de.launch_count(); stage(); c.append(de.launch_count() - n)
+                # CostConst_GPU: ingest (2 views x ingest + halo) and one CVC launch; selection: one kernel per view
+                if c != [5, cvf, views]:
+                    bad.append((path, block, c, [5, cvf, views]))
+    assert not bad, bad
 
 
 # ---- 8. the C++ facade ------------------------------------------------------------------------------------------------
