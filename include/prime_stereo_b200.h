@@ -52,7 +52,8 @@
  * blocking uploads): psm_set_images_async / _u8_async (the second staging set), psm_cost_filter and psm_read_ab_slice
  * (the scratch of the reference-order pass: float frames, a non-default guided filter, PSM_CVF_NAIVE, flagged slices),
  * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
- * (its buffers and, after a change of sigma or weight type, the weight table).  Run them once before a latency-critical
+ * (its buffers and, after a change of sigma or weight type, the weight table), psm_set_option(PSM_OPT_COSTS, 1) (the
+ * cost planes).  Run them once before a latency-critical
  * loop.  psm_set_stream always waits for the stream it leaves.
  */
 #ifndef PRIME_STEREO_B200_H
@@ -87,8 +88,10 @@ enum {
     PSM_OPT_P2P_SYNC = 4,  /* fused multi-GPU exchange: 1 (default) = the kernels synchronise across ranks by
                               device-side flags in the exchange blocks (no library collective, no host barrier);
                               0 = the caller separates select / reduce / fetch by its own cross-rank barriers */
-    PSM_OPT_VIEWS = 5      /* PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT: which disparity maps a frame computes; see
+    PSM_OPT_VIEWS = 5,     /* PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT: which disparity maps a frame computes; see
                               "Left-only frames" below */
+    PSM_OPT_COSTS = 6      /* 0 (default) or 1: the selection stages also keep the filtered costs beside each winner;
+                              see psm_copy_costs_device */
     /* keys 100..106 are kernel tuning knobs used by bench.py experiments (variant, rows per segment, extra
        shared memory, threads per CTA, block remap, packed remainder strips off, CVC build); they never
        change results */
@@ -441,6 +444,37 @@ int psm_post_process_u16(psm_ctx* ctx, uint16_t* left, size_t left_step, uint16_
  *   - PSM_ESTATE: no selection (which = 0) or post-process (which = 1) since the context was created or PSM_OPT_VIEWS
  *     last changed, and under the exchanged-map rules of psm_disp_fetch_p2p. */
 int psm_copy_maps_device(psm_ctx* ctx, int which, void* d_left, size_t left_step, void* d_right, size_t right_step);
+
+/* The filtered costs at and beside each pixel's winning disparity (PSM_OPT_COSTS = 1), for sub-pixel refinement,
+ * confidence masks or a cost threshold in the caller.  Per computed view, three float planes of H x W: plane k holds
+ * q(x, y, m + k - 1), where m is the map of the last selection stage and q the filtered volume it scanned (the exact
+ * filter in any mode, window or order, PSM_CVF_MIXED's q, or the Fast Guided Filter's q).  Every value is the volume's,
+ * bit for bit (-0, +-inf and NaN payloads included).  An index outside [0, D) gives the quiet NaN 0x7FC00000, so a pixel
+ * with no winner (map 0: every cost NaN or +inf) gets (NaN, q(0), q(1)).  The post-filter and the left-right check do not
+ * change them: they belong to the selection maps.  Only a selection stage writes them, so on every kind of context they
+ * stay the last selection's through the next frame's psm_set_images*, psm_cost_const and filter stage.
+ *   - PSM_OPT_COSTS takes 0 or 1, anything else returns PSM_EINVAL and changes nothing.  Turning it on allocates the
+ *     planes: 12 * H * W bytes per view, plus 16 * H * W on a blocked context, which tracks its winners' neighbours
+ *     during the walk (a multi-device context: the result planes on the first shard only, the tracking planes on every
+ *     blocked shard, 20 * H * W on a shard that owns no slice 0).  A failed allocation changes no setting, on any shard.
+ *     A change resets the frame's stages as PSM_OPT_VIEWS does: the next stage must be psm_cost_const.  Turning it on
+ *     returns PSM_EINVAL on a context that owns part of the range (psm_create_sharded, or psm_create_u16 /
+ *     psm_create_blocked with d_count < max_disp); 0, the default, is accepted there.  A multi-device context passes it
+ *     to every shard, since it spans [0, max_disp).
+ *   - The work: after selection, one kernel per view writes the costs, from the volume on an unblocked context and from
+ *     the tracking planes on a blocked one (whose block folds track them, in the same launches); on multi-device
+ *     contexts every shard writes the entries it owns into the first shard's planes after the reduce.  Stage 3
+ *     (psm_stage_ms) covers these kernels; psm_launch_count counts them.  With the option off nothing of this runs.
+ *   - psm_disp_select_keys does not write the costs, and neither do the fused-exchange calls.
+ * psm_copy_costs_device writes view v's planes to caller DEVICE memory on the context's stream, asynchronously: plane k
+ * starts at dst + k * H * row_step (a contiguous (3, H, W) float32 tensor: row_step = 4 * W).  d_right must be NULL on a
+ * left-only context and is required otherwise.  psm_read_costs writes one view's planes to HOST memory, same layout,
+ * and synchronises.  A multi-device context copies the first shard's planes.
+ *   - PSM_EINVAL before any CUDA call: a null pointer, a row_step below 4 * W, a bad view.
+ *   - PSM_ESTATE: the last selection stage (psm_disp_select*) since the context was created or PSM_OPT_VIEWS /
+ *     PSM_OPT_COSTS last changed did not run with PSM_OPT_COSTS = 1; a right-view read on a left-only context. */
+int psm_copy_costs_device(psm_ctx* ctx, float* d_left, float* d_right, size_t row_step);
+int psm_read_costs(psm_ctx* ctx, int view, float* dst, size_t row_step);
 
 /* Sharded stage 3a: per-pixel packed minima over this context's slices, written to DEVICE
  * buffers of H*W uint64 each:  key = (order_preserving_u32(cost) << 32) | global_d.

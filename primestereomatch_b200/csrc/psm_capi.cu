@@ -113,11 +113,23 @@ struct psm_ctx {
     cudaEvent_t ev_reduced[kMaxRanks] = {};    // shard k's reduce of the last frame (on its stream)
     bool reduced_valid = false;
     cudaEvent_t ev_copied[kMaxRanks] = {};     // shard k (k >= 1) has read the frame it receives from the first shard
+    cudaEvent_t ev_gathered[kMaxRanks] = {};   // PSM_OPT_COSTS: shard k's cost entries of the current frame (on its stream)
     cudaEvent_t ev_images = nullptr;           // psm_set_images_device: the caller's images as the first shard's stream sees them
     // PSM_OPT_VIEWS: 2 (both views) or 1 (the left view alone: the right view's guide, volume, selection and post-filter
-    // are skipped).  views_reset: the value changed since the last psm_cost_const, so the volumes, maps and masks are stale.
+    // are skipped).  stages_reset: PSM_OPT_VIEWS or PSM_OPT_COSTS changed since the last psm_cost_const, so the volumes,
+    // maps, masks and costs are stale.
     int views = 2;
-    bool views_reset = false;
+    bool stages_reset = false;
+    // PSM_OPT_COSTS: 1 = the selection stages also write the filtered costs beside each winner into win_cost[view]
+    // (kCostOut planes; a multi-device context's shards write the first shard's, the others have none), and a blocked
+    // walk tracks them in track[view] (track_planes()).  Both are allocated when the option is turned on.
+    // have_costs: the last selection stage since the last reset wrote them.
+    int costs = 0;
+    float* win_cost[2] = {nullptr, nullptr};
+    float* track[2] = {nullptr, nullptr};
+    bool have_costs = false;
+    // kCostFirst only where a neighbour shard below reads it
+    int track_planes() const { return d_begin > 0 ? kCostFirst + 1 : kCostLast + 1; }
     unsigned p2p_seq_right = 0;                // frames whose exchange included the right view (p2p_seq counts every frame)
     bool p2p_right_current = false;            // the last frame's exchange included the right view
     bool have_pp = false;                      // dis_pp holds the maps of a post-process since the last PSM_OPT_VIEWS change
@@ -171,15 +183,15 @@ int bind(psm_ctx* c)
     return PSM_OK;
 }
 
-// a call that would read or return right-view data: PSM_ESTATE on a left-only context, and after a PSM_OPT_VIEWS change
+// a call that would read or return right-view data: PSM_ESTATE on a left-only context, and after a PSM_OPT_VIEWS or PSM_OPT_COSTS change
 // until psm_cost_const has built the current frame's volumes again
 int check_right_view(psm_ctx* c, const char* call)
 {
     if (c->views == 1)
         return fail(c, PSM_ESTATE, "%s of the right view on a left-only context (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): the right "
                     "view is not computed; set PSM_VIEWS_BOTH", call);
-    if (c->views_reset)
-        return fail(c, PSM_ESTATE, "%s of the right view after a PSM_OPT_VIEWS change: call psm_cost_const first", call);
+    if (c->stages_reset)
+        return fail(c, PSM_ESTATE, "%s of the right view after a PSM_OPT_VIEWS or PSM_OPT_COSTS change: call psm_cost_const first", call);
     return PSM_OK;
 }
 
@@ -193,10 +205,10 @@ int check_right_arg(psm_ctx* c, const void* right, const char* call)
 }
 
 // a stage that needs the stage state PSM_OPT_VIEWS reset
-int check_views_reset(psm_ctx* c, const char* call)
+int check_stages_reset(psm_ctx* c, const char* call)
 {
-    if (c->views_reset)
-        return fail(c, PSM_ESTATE, "%s after a PSM_OPT_VIEWS change: the next stage must be psm_cost_const", call);
+    if (c->stages_reset)
+        return fail(c, PSM_ESTATE, "%s after a PSM_OPT_VIEWS or PSM_OPT_COSTS change: the next stage must be psm_cost_const", call);
     return PSM_OK;
 }
 
@@ -745,14 +757,39 @@ int launch_cvc(psm_ctx* c)
     return PSM_OK;
 }
 
-// the filtered block in the volumes -> the running keys (stored by the first block, min-folded by the others)
+// the result planes and the tracking planes of view v (PSM_OPT_COSTS)
+CostPlanes cost_planes(const psm_ctx* c, int v) { return {c->win_cost[v], (size_t)c->W * c->H}; }
+CostPlanes track_planes(const psm_ctx* c, int v) { return {c->track[v], (size_t)c->W * c->H}; }
+
+// the filtered block in the volumes -> the running keys (stored by the first block, min-folded by the others), and with
+// PSM_OPT_COSTS the costs beside the running winners
 int launch_fold(psm_ctx* c, bool first)
 {
     FoldParams P;
     for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->res.begin; P.d_count = c->res.count; P.first = first ? 1 : 0;
     dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, c->views);
-    wta_fold_kernel<<<grd, blk, 0, c->stream>>>(P);
+    if (c->costs)
+        wta_fold_costs_kernel<<<grd, blk, 0, c->stream>>>(
+            FoldCostParams{P, {track_planes(c, 0), track_planes(c, 1)}, c->track_planes() > kCostFirst});
+    else
+        wta_fold_kernel<<<grd, blk, 0, c->stream>>>(P);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
+// The cost entries context c owns (cost_write_kernel) from `map` (the complete selection map of view v) into dst: from
+// its resident volume on an unblocked context, from its tracking planes on a blocked one
+int launch_cost_write(psm_ctx* c, int v, const void* map, CostPlanes dst)
+{
+    CostWriteParams P;
+    P.map = map; P.vol = c->vol[v]; P.src = track_planes(c, v); P.dst = dst;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.D = c->D; P.d_begin = c->d_begin; P.d_count = c->d_count;
+    dim3 blk(256), grd((c->W + 255) / 256, c->H);
+    if (c->map_bytes == 2)
+        (c->blk_slices ? cost_write_kernel<uint16_t, true> : cost_write_kernel<uint16_t, false>)<<<grd, blk, 0, c->stream>>>(P);
+    else
+        (c->blk_slices ? cost_write_kernel<uint8_t, true> : cost_write_kernel<uint8_t, false>)<<<grd, blk, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
@@ -807,7 +844,13 @@ P2pLayout p2p_layout(const psm_ctx* c, int nranks)
 bool exchanged(const psm_ctx* c) { return c->p2p_own && c->p2p_seq > 0; }
 
 // a selection stage wrote new maps (`own`: the context's own, not an exchange block's): the left-right masks are stale
-void selection_ran(psm_ctx* c, bool own) { c->lr_masks_ok = false; c->have_maps = c->have_maps || own; }
+// and so are the costs, until the stage writes them too
+void selection_ran(psm_ctx* c, bool own)
+{
+    c->lr_masks_ok = false;
+    c->have_maps = c->have_maps || own;
+    c->have_costs = false;
+}
 
 // a map call for maps of type T, named u8_call / u16_call in its two formats, on a context of the other format:
 // PSM_EINVAL naming the right call
@@ -997,7 +1040,7 @@ int filter_stage(psm_ctx* c, const char* call, Prepare prepare, Guide guide, Fil
 {
     if (is_multi(c)) return forward(c, [&](psm_ctx* s) { return filter_stage(s, call, prepare, guide, filter); });
     if (int rc = bind(c)) return rc;
-    if (int rc = check_views_reset(c, call)) return rc;
+    if (int rc = check_stages_reset(c, call)) return rc;
     if (!c->have_cvc) return fail(c, PSM_ESTATE, "%s before psm_cost_const", call);
     if (int rc = prepare(c)) return rc;
     if (int rc = stage_begin(c, 2)) return rc;
@@ -1245,6 +1288,7 @@ int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const i
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_scattered[k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_reduced[k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied[k], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_gathered[k], cudaEventDisableTiming);
         if (e == cudaSuccess && k == 0) e = cudaEventCreateWithFlags(&c->ev_images, cudaEventDisableTiming);
         if (e != cudaSuccess) { fail(c, PSM_ECUDA, "event creation on device %d failed: %s", devices[k], cudaGetErrorString(e)); return bail(PSM_ECUDA); }
     }
@@ -1272,6 +1316,7 @@ int psm_destroy(psm_ctx* c)
             if (c->ev_scattered[k]) cudaEventDestroy(c->ev_scattered[k]);
             if (c->ev_reduced[k]) cudaEventDestroy(c->ev_reduced[k]);
             if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]);
+            if (c->ev_gathered[k]) cudaEventDestroy(c->ev_gathered[k]);
             if (k == 0 && c->ev_images) cudaEventDestroy(c->ev_images);
             psm_destroy(c->shard[k]);
         }
@@ -1302,7 +1347,8 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->guide_flags);
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
-    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]); }
+    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]); cudaFree(c->win_cost[v]);
+                                   cudaFree(c->track[v]); }
     for (int s = 0; s < kNumStages; ++s) {
         if (c->ev0[s]) cudaEventDestroy(c->ev0[s]);
         if (c->ev1[s]) cudaEventDestroy(c->ev1[s]);
@@ -1313,12 +1359,68 @@ int psm_destroy(psm_ctx* c)
     return PSM_OK;
 }
 
+}  // extern "C"
+
+// PSM_OPT_VIEWS or PSM_OPT_COSTS changed: the frame's stages start again from psm_cost_const on the current images; nothing
+// computed for the other setting (volumes, maps, masks, costs, the guide of the right view) can be read or selected from
+static void reset_stages(psm_ctx* c)
+{
+    c->stages_reset = true;
+    c->guide_valid = false;
+    c->have_cvc = false;
+    c->filtered = false;
+    c->have_maps = false;
+    c->have_pp = false;
+    c->lr_masks_ok = false;
+    c->have_costs = false;
+}
+
+// PSM_OPT_COSTS = 1 on one context, a multi-device context's shards included: the planes it reads or writes, the result
+// planes where `result` (a single-device context, the first shard) and the tracking planes on a blocked context.  Only
+// allocates: a failure leaves the setting as it was.
+static int alloc_costs(psm_ctx* c, bool result)
+{
+    if (int rc = bind(c)) return rc;
+    const size_t plane = (size_t)c->W * c->H * sizeof(float);
+    for (int v = 0; v < 2; ++v) {
+        if (result) PSM_CUDA(c, alloc_if_null(c->win_cost[v], kCostOut * plane));
+        if (c->blk_slices) PSM_CUDA(c, alloc_if_null(c->track[v], c->track_planes() * plane));
+    }
+    return PSM_OK;
+}
+
+// PSM_OPT_COSTS = value, its planes allocated: a blocked context's walk tracks the costs, so a change restarts the frame
+static void apply_costs(psm_ctx* c, int value)
+{
+    if (value != c->costs) {
+        reset_stages(c);
+        c->costs = value;
+    }
+}
+
+static int check_costs_value(psm_ctx* c, int value)
+{
+    if (value != 0 && value != 1) return fail(c, PSM_EINVAL, "PSM_OPT_COSTS must be 0 or 1 (got %d)", value);
+    return PSM_OK;
+}
+
+extern "C" {
+
 int psm_set_option(psm_ctx* c, int key, int value)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
     if (c->nshards) {
         if (key == PSM_OPT_P2P_SYNC)
             return reject_multi(c, "PSM_OPT_P2P_SYNC", "its shards' exchange is ordered by events, never by flags");
+        if (key == PSM_OPT_COSTS) {   // the shards own part of the range, the context as a whole spans [0, D)
+            if (int rc = check_costs_value(c, value)) return rc;
+            // every shard's planes first, then the setting on all of them: a failed allocation changes no shard's setting
+            for (int k = 0; value && k < c->nshards; ++k)
+                if (int rc = alloc_costs(c->shard[k], k == 0)) return relay(c, k, rc);
+            for (int k = 0; k < c->nshards; ++k) apply_costs(c->shard[k], value);
+            c->costs = value;
+            return PSM_OK;
+        }
         if (int rc = forward(c, [&](psm_ctx* s) { return psm_set_option(s, key, value); })) return rc;
         if (key == PSM_OPT_VIEWS) c->views = value;   // the map calls check the right-view arguments on the context itself
         return PSM_OK;
@@ -1328,17 +1430,18 @@ int psm_set_option(psm_ctx* c, int key, int value)
         if (value != PSM_VIEWS_LEFT && value != PSM_VIEWS_BOTH)
             return fail(c, PSM_EINVAL, "PSM_OPT_VIEWS must be PSM_VIEWS_LEFT (1) or PSM_VIEWS_BOTH (2) (got %d)", value);
         if (value != c->views) {
-            // the frame's stages start again from psm_cost_const on the current images; nothing computed for the other
-            // setting (volumes, maps, masks, the guide of the right view) can be read or selected from
             c->views = value;
-            c->views_reset = true;
-            c->guide_valid = false;
-            c->have_cvc = false;
-            c->filtered = false;
-            c->have_maps = false;
-            c->have_pp = false;
-            c->lr_masks_ok = false;
+            reset_stages(c);
         }
+        return PSM_OK;
+    case PSM_OPT_COSTS:
+        if (int rc = check_costs_value(c, value)) return rc;
+        if (value && (c->d_begin != 0 || c->d_count != c->D))
+            return fail(c, PSM_EINVAL, "PSM_OPT_COSTS on a context that owns slices [%d,%d) of %d: the costs beside a winner "
+                        "may lie on another context; use a context over the whole range (psm_create, psm_create_u16 / "
+                        "psm_create_blocked over [0, max_disp), or psm_create_multi)", c->d_begin, c->d_begin + c->d_count, c->D);
+        if (int rc = value ? alloc_costs(c, true) : PSM_OK) return rc;
+        apply_costs(c, value);
         return PSM_OK;
     case PSM_OPT_CVF_MODE:
         if (value != PSM_CVF_EXACT && value != PSM_CVF_MIXED && value != PSM_CVF_NAIVE)
@@ -1553,7 +1656,7 @@ int psm_cost_const(psm_ctx* c)
     if (int rc = clear_slice_flags(c)) return rc;
     c->have_cvc = true;
     c->filtered = false;
-    c->views_reset = false;
+    c->stages_reset = false;
     return stage_end(c, 1);
 }
 
@@ -1614,7 +1717,7 @@ static int disp_reduce_keys(psm_ctx* c, const uint64_t* d_gathered_left, const u
     if (is_multi(c)) return reject_multi(c, sizeof(T) == 1 ? "psm_disp_reduce_keys" : "psm_disp_reduce_keys_u16", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = check_map_format<T>(c, "psm_disp_reduce_keys", "psm_disp_reduce_keys_u16")) return rc;
     if (int rc = bind(c)) return rc;
-    if (int rc = check_views_reset(c, "psm_disp_reduce_keys")) return rc;
+    if (int rc = check_stages_reset(c, "psm_disp_reduce_keys")) return rc;
     if (int rc = check_right_arg(c, d_gathered_right, "psm_disp_reduce_keys")) return rc;
     if (int rc = check_right_arg(c, right, "psm_disp_reduce_keys")) return rc;
     const bool to_host = left && (right || c->views == 1);   // a null map pointer: the maps stay on the device
@@ -1647,6 +1750,11 @@ int psm_disp_select_device(psm_ctx* c)
     if (int rc = stage_begin(c, 3)) return rc;
     if (int rc = c->map_bytes == 2 ? select_maps<uint16_t>(c) : select_maps<uint8_t>(c)) return rc;
     selection_ran(c, true);
+    if (c->costs) {   // from the volume, or from a blocked context's tracking planes, which its next walk rewrites
+        for (int v = 0; v < c->views; ++v)
+            if (int rc = launch_cost_write(c, v, c->dis[v], cost_planes(c, v))) return rc;
+        c->have_costs = true;
+    }
     return stage_end(c, 3);
 }
 
@@ -1678,6 +1786,7 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
     if (!d_keys_left || (c->views == 2 && !d_keys_right)) return fail(c, PSM_EINVAL, "null key buffer");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
+    c->have_costs = false;   // keys carry no costs beside the winner
     uint64_t* keys[2] = {d_keys_left, d_keys_right};
     if (c->blk_slices) {   // the running keys are this context's minima already
         for (int v = 0; v < c->views; ++v)
@@ -1822,7 +1931,7 @@ int psm_disp_reduce_p2p(psm_ctx* c)
     if (is_multi(c)) return reject_multi(c, "psm_disp_reduce_p2p", "the context already spans the whole disparity range; use psm_disp_select*");
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own || !c->p2p_peer[0]) return fail(c, PSM_ESTATE, "no exchange block");
-    if (int rc = check_views_reset(c, "psm_disp_reduce_p2p")) return rc;
+    if (int rc = check_stages_reset(c, "psm_disp_reduce_p2p")) return rc;
     const unsigned npix = (unsigned)((size_t)c->W * c->H);
     const auto reduce = c->map_bytes == 2 ? chunk_reduce_kernel<uint16_t> : chunk_reduce_kernel<uint8_t>;
     for (int v = 0; v < c->views; ++v) {
@@ -1874,6 +1983,18 @@ static int p2p_wait_done(psm_ctx* c)
 //   4. every reduce writes the first shard's maps, which what the first shard enqueued before this select (a previous
 //      post-filter, an asynchronous D2H) may still read: the wait of 2 on the first shard's scatter, queued behind
 //      that work, covers it.
+// With PSM_OPT_COSTS, every shard then writes the cost entries it owns into the first shard's cost planes:
+//   5. shard k's gather reads its copy of the complete maps, which every shard's reduce writes: it waits for them;
+//   6. the first shard's stream, which carries every reader of the costs (psm_copy_costs_device, psm_read_costs), waits
+//      for every gather;
+//   7. the gathers overwrite cost planes that a copy-out of the previous frame on the first shard's stream may still
+//      read: each gather follows its shard's reduce, which waits for the first shard's scatter (2), queued behind that
+//      copy-out;
+//   8. a gather reads its shard's map, which the next frame's reduces overwrite: they wait for that shard's next
+//      scatter (2), queued behind the gather; and the volumes or tracking planes it reads are rewritten only by later
+//      stages on its own stream.
+// The first shard's result planes are written by these gathers alone, never by a filter stage (its tracking planes are
+// separate), so they hold frame f's costs until the next select, as on a single-device context.
 // No kernel waits for another queued behind it, so shards on one device are as safe as shards on several.
 static int multi_select(psm_ctx* c)
 {
@@ -1901,8 +2022,24 @@ static int multi_select(psm_ctx* c)
     }
     c->reduced_valid = true;
     psm_ctx* s0 = c->shard[0];
+    if (c->costs) {
+        for (int k = 0; k < n; ++k) {
+            psm_ctx* s = c->shard[k];
+            if (int rc = bind(s)) return relay(c, k, rc);
+            for (int j = 0; j < n; ++j)
+                if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_reduced[j], 0));   // 5
+            const P2pLayout L = p2p_layout(s, s->p2p_nranks);
+            for (int v = 0; v < s->views; ++v)   // peer stores between distinct devices
+                if (int rc = launch_cost_write(s, v, L.maps(s->p2p_own, v), cost_planes(s0, v))) return relay(c, k, rc);
+            PSM_CUDA(c, cudaEventRecord(c->ev_gathered[k], s->stream));
+        }
+    }
     if (int rc = bind(s0)) return relay(c, 0, rc);
     for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_reduced[j], 0));   // 3
+    if (c->costs) {
+        for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_gathered[j], 0));   // 6
+        s0->have_costs = true;
+    }
     return relay(c, 0, stage_end(s0, 3));
 }
 
@@ -1915,7 +2052,7 @@ static int disp_fetch_p2p(psm_ctx* c, T* left, size_t left_step, T* right, size_
     if (int rc = check_map_format<T>(c, "psm_disp_fetch_p2p", "psm_disp_fetch_p2p_u16")) return rc;
     if (int rc = bind(c)) return rc;
     if (!c->p2p_own) return fail(c, PSM_ESTATE, "no exchange block");
-    if (int rc = check_views_reset(c, "psm_disp_fetch_p2p")) return rc;
+    if (int rc = check_stages_reset(c, "psm_disp_fetch_p2p")) return rc;
     if (int rc = check_map_dst(c, "psm_disp_fetch_p2p", left, left_step, right, right_step)) return rc;
     if (int rc = check_p2p_right_map(c, "psm_disp_fetch_p2p")) return rc;
     if (int rc = p2p_wait_done(c)) return rc;
@@ -1989,7 +2126,7 @@ static int post_process_maps(psm_ctx* c)
     }();
     c->lr_masks_ok = false;
     if (!c->have_images) return fail(c, PSM_ESTATE, "psm_post_process before psm_set_images");
-    if (int rc = check_views_reset(c, "psm_post_process")) return rc;
+    if (int rc = check_stages_reset(c, "psm_post_process")) return rc;
     const uint8_t* maps[2];
     if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
@@ -2108,7 +2245,7 @@ int psm_copy_maps_device(psm_ctx* c, int which, void* d_left, size_t left_step, 
     // a multi-device context's maps are the first shard's (its exchange block, and its post-filter's outputs)
     if (is_multi(c)) return relay(c, 0, psm_copy_maps_device(c->shard[0], which, d_left, left_step, d_right, right_step));
     if (int rc = bind(c)) return rc;
-    if (int rc = check_views_reset(c, "psm_copy_maps_device")) return rc;
+    if (int rc = check_stages_reset(c, "psm_copy_maps_device")) return rc;
     const uint8_t* maps[2] = {c->dis_pp[0], c->dis_pp[1]};
     if (which == 0) {
         if (int rc = selection_maps(c, "psm_copy_maps_device", maps)) return rc;
@@ -2117,6 +2254,58 @@ int psm_copy_maps_device(psm_ctx* c, int which, void* d_left, size_t left_step, 
         return fail(c, PSM_ESTATE, "psm_copy_maps_device of the post-processed maps before a post-process");
     }
     return copy_maps_out(c, maps, d_left, left_step, d_right, right_step, cudaMemcpyDefault, false);
+}
+
+// the costs of the last selection stage for psm_copy_costs_device and psm_read_costs
+static int check_costs_ready(psm_ctx* c, const char* call)
+{
+    if (int rc = check_stages_reset(c, call)) return rc;
+    if (!c->have_costs)
+        return fail(c, PSM_ESTATE, "%s: no costs; the last selection stage since the context was created or the last "
+                    "PSM_OPT_VIEWS / PSM_OPT_COSTS change did not write them (psm_disp_select* with PSM_OPT_COSTS = 1)", call);
+    return PSM_OK;
+}
+
+// view v's kCostOut planes -> dst (plane k at dst + k * H * row_step) on the context's stream: one copy of 3H rows
+static int copy_costs_out(psm_ctx* c, int v, float* dst, size_t row_step, cudaMemcpyKind kind)
+{
+    const size_t row = (size_t)c->W * sizeof(float);
+    PSM_CUDA(c, cudaMemcpy2DAsync(dst, row_step, c->win_cost[v], row, row, (size_t)kCostOut * c->H, kind, c->stream));
+    return PSM_OK;
+}
+
+int psm_copy_costs_device(psm_ctx* c, float* d_left, float* d_right, size_t row_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (int rc = check_right_arg(c, d_right, "psm_copy_costs_device")) return rc;
+    const size_t row = (size_t)c->W * sizeof(float);
+    if (!d_left || (c->views == 2 && !d_right) || row_step < row)
+        return fail(c, PSM_EINVAL, "psm_copy_costs_device: bad cost plane pointer/step (row_step must be at least %zu bytes)", row);
+    // a multi-device context's costs are the first shard's
+    if (is_multi(c)) return relay(c, 0, psm_copy_costs_device(c->shard[0], d_left, d_right, row_step));
+    if (int rc = bind(c)) return rc;
+    if (int rc = check_costs_ready(c, "psm_copy_costs_device")) return rc;
+    float* dst[2] = {d_left, d_right};
+    for (int v = 0; v < c->views; ++v)
+        if (int rc = copy_costs_out(c, v, dst[v], row_step, cudaMemcpyDefault)) return rc;
+    return PSM_OK;
+}
+
+int psm_read_costs(psm_ctx* c, int view, float* dst, size_t row_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
+    const size_t row = (size_t)c->W * sizeof(float);
+    if (!dst || row_step < row)
+        return fail(c, PSM_EINVAL, "psm_read_costs: bad cost plane pointer/step (row_step must be at least %zu bytes)", row);
+    if (is_multi(c)) return relay(c, 0, psm_read_costs(c->shard[0], view, dst, row_step));
+    if (int rc = bind(c)) return rc;
+    if (view == PSM_RIGHT)
+        if (int rc = check_right_view(c, "psm_read_costs")) return rc;
+    if (int rc = check_costs_ready(c, "psm_read_costs")) return rc;
+    if (int rc = copy_costs_out(c, view, dst, row_step, cudaMemcpyDeviceToHost)) return rc;
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
 }
 
 static int check_slice(psm_ctx* c, int view, int d)

@@ -644,6 +644,141 @@ __global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// The filtered costs beside each winner (PSM_OPT_COSTS): q(m - 1), q(m), q(m + 1) of the volume selection scanned, at the
+// selection map's m, copied bit for bit.  An index outside [0, D) gives kCostNaN; a pixel without a winner (m = 0) gets
+// (kCostNaN, q(0), q(1)).
+// ------------------------------------------------------------------------------------------
+// Planes of H * W floats (row pitch W), per view.  The result: kCostOut planes holding q(m - 1), q(m), q(m + 1); the
+// selection stages write them and nothing else does, so they stay the last selection's until the next one.  A blocked
+// context's tracking planes, which its walk rewrites block by block: planes 0..2 hold the running winner's costs, then
+// kCostLast the cost at the last slice of the block walked last and, on a shard that owns no slice 0, kCostFirst the cost
+// at its first owned slice (read by the shard below it at their seam).
+constexpr int kCostOut = 3, kCostLast = 3, kCostFirst = 4;
+constexpr unsigned kCostNaNBits = 0x7fc00000u;   // the canonical quiet NaN of an index outside [0, D)
+
+struct CostPlanes {
+    float* base;
+    size_t npix;   // H * W
+    __host__ __device__ float* plane(int k) const { return base + (size_t)k * npix; }
+};
+
+// wta_scan4 over slices [d_begin, d_begin + d_count), tracking the costs beside the running minimum: on a new minimum at
+// d, lo = the previous slice's cost (`prev`, seeded with the cost before the range) and hi waits for slice d + 1.  Slice
+// 0 is scanned but is never a candidate: the no-winner state (md = 0) takes ce = q(0) and, from the md == d - 1 rule,
+// hi = q(1).  `first` and `prev` end as the range's first and last costs.
+__device__ __forceinline__ void wta_scan4_costs(const float* p, size_t plane, int d_begin, int d_count, float (&mc)[4],
+                                                int (&md)[4], float (&lo)[4], float (&ce)[4], float (&hi)[4],
+                                                float (&prev)[4], float (&first)[4])
+{
+    const float nan = __uint_as_float(kCostNaNBits);
+    for (int dl = 0; dl < d_count; ++dl) {
+        const float4 c4 = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
+        const float c[4] = {c4.x, c4.y, c4.z, c4.w};
+        const int d = d_begin + dl;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (md[j] == d - 1) hi[j] = c[j];
+            if (d == 0) ce[j] = c[j];
+            else if (c[j] < mc[j]) { mc[j] = c[j]; md[j] = d; lo[j] = prev[j]; ce[j] = c[j]; hi[j] = nan; }
+            prev[j] = c[j];
+            if (dl == 0) first[j] = c[j];
+        }
+    }
+}
+
+// wta_fold_kernel with the costs tracked in track[view] (the tracking planes).  Planes 0..2 hold the running winner's
+// (lo, ce, hi).  A block whose key is below the running key (the fold's own comparison) replaces them; its lo at its
+// first slice is the previous block's last cost (kCostLast).  A running winner on the previous block's last slice takes
+// hi from this block's first slice.  The first block starts from the no-winner state and, if write_first, records
+// kCostFirst.
+struct FoldCostParams {
+    FoldParams f;
+    CostPlanes track[2];
+    int write_first;
+};
+
+__global__ void __launch_bounds__(256) wta_fold_costs_kernel(const FoldCostParams P)
+{
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y, view = blockIdx.z;
+    if (x4 >= P.f.W) return;
+    const size_t plane = (size_t)P.f.H * P.f.Wp;
+    const float* p = (view ? P.f.vol[1] : P.f.vol[0]) + (size_t)y * P.f.Wp + x4;
+    unsigned long long* k = (view ? P.f.keys[1] : P.f.keys[0]) + (size_t)y * P.f.W;
+    const CostPlanes t = view ? P.track[1] : P.track[0];
+    const size_t row = (size_t)y * P.f.W;
+    const float nan = __uint_as_float(kCostNaNBits);
+    float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+    int md[4] = {0, 0, 0, 0};
+    float lo[4] = {nan, nan, nan, nan}, ce[4] = {nan, nan, nan, nan}, hi[4] = {nan, nan, nan, nan};
+    float prev[4] = {nan, nan, nan, nan}, first[4];
+    if (!P.f.first)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (x4 + j < P.f.W) prev[j] = t.plane(kCostLast)[row + x4 + j];
+    wta_scan4_costs(p, plane, P.f.d_begin, P.f.d_count, mc, md, lo, ce, hi, prev, first);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int x = x4 + j;
+        if (x >= P.f.W) continue;
+        const size_t i = row + x;
+        const unsigned long long v = wta_key(mc[j], md[j]);
+        t.plane(kCostLast)[i] = prev[j];
+        bool win = true;
+        if (P.f.first) {
+            if (P.write_first) t.plane(kCostFirst)[i] = first[j];
+        } else {
+            const unsigned long long old = k[x];
+            win = v < old;
+            if (!win && (int)(unsigned)old == P.f.d_begin - 1) t.plane(2)[i] = first[j];
+        }
+        if (win) {
+            k[x] = v;
+            t.plane(0)[i] = lo[j]; t.plane(1)[i] = ce[j]; t.plane(2)[i] = hi[j];
+        }
+    }
+}
+
+// The costs of the entries a context owns, from the complete selection map (T) into dst, which may be a peer's planes.
+// Entry k of pixel i is q(d), d = m + k - 1.  Its one writer: the owner of slice d, [d_begin, d_begin + d_count), for d
+// in [0, D), and the owner of m (kCostNaN) otherwise.  kTracked = false reads q(d) from the resident volume (an
+// unblocked context); kTracked = true from the tracking planes of a blocked one: planes 0..2 for its own winners, and
+// at its seams kCostFirst (m just below its range) or kCostLast (m just above).
+struct CostWriteParams {
+    const void* map;      // [H][W] of T
+    const float* vol;     // kTracked = false: the filtered volume of slices [d_begin, d_begin + d_count), [d][H][Wp]
+    CostPlanes src;       // kTracked = true: the tracking planes
+    CostPlanes dst;
+    int W, H, Wp, D, d_begin, d_count;
+};
+
+template <typename T, bool kTracked>
+__global__ void __launch_bounds__(256) cost_write_kernel(const CostWriteParams P)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= P.W) return;
+    const size_t i = (size_t)y * P.W + x;
+    const int m = static_cast<const T*>(P.map)[i];
+    const auto owned = [&](int d) { return d >= P.d_begin && d < P.d_begin + P.d_count; };
+#pragma unroll
+    for (int k = 0; k < kCostOut; ++k) {
+        const int d = m + k - 1;
+        float q;
+        if (d < 0 || d >= P.D) {
+            if (!owned(m)) continue;
+            q = __uint_as_float(kCostNaNBits);
+        } else if (!owned(d)) {
+            continue;
+        } else if (!kTracked) {
+            q = P.vol[(size_t)(d - P.d_begin) * P.H * P.Wp + (size_t)y * P.Wp + x];
+        } else {
+            q = P.src.plane(owned(m) ? k : (k == 2 ? kCostFirst : kCostLast))[i];
+        }
+        P.dst.plane(k)[i] = q;
+    }
+}
+
 // Sharded WTA fused with its exchange (reduce-scatter + all-gather of a min-reduction, hand-rolled
 // over NVLink peer memory).  Pixels are partitioned into `nranks` chunks; rank r is the reducer of
 // chunk r.

@@ -93,6 +93,8 @@ class DispEst:
         self.lValid = np.zeros((self.hei, self.wid), np.uint8)  # DispEst.cpp:48-49
         self.rValid = np.zeros((self.hei, self.wid), np.uint8)
         self.lr_mode = capi.PSM_LR_OFF
+        self.cost_output = False
+        self.lCosts = self.rCosts = None   # setCostOutput(True): DispSelect_GPU's (3, H, W) float32 costs
         if devices is not None and (d_begin != 0 or d_count is not None):
             raise ValueError("devices (a multi-device context over the whole range) excludes d_begin / d_count")
         self._lImg, self._rImg = l, r
@@ -198,6 +200,25 @@ class DispEst:
             self.rDisMap = np.zeros_like(self.lDisMap)
         return 0
 
+    def setCostOutput(self, on):
+        """Whether DispSelect_GPU also fills lCosts / rCosts (PSM_OPT_COSTS): numpy float32 (3, H, W) whose plane k holds
+        the filtered cost at disparity m + k - 1, m the selection map, bit for bit as the filter left it; the quiet NaN
+        0x7FC00000 where m + k - 1 lies outside [0, maxDis).  rCosts is None on left-only frames.  Changing it restarts
+        the frame at CostConst_GPU.  Raises TypeError unless on is a bool, PsmError on a context that owns part of the
+        disparity range (d_begin / d_count)."""
+        if not isinstance(on, bool):
+            raise TypeError(f"setCostOutput takes True or False (got {on!r})")
+        self._need_gpu()
+        capi.check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_COSTS, int(on)), self._ctx)
+        self.cost_output = on
+        self.lCosts = self.rCosts = None
+        return 0
+
+    def _read_costs(self, view):
+        out = np.empty((3, self.hei, self.wid), np.float32)
+        capi.check(self._lib.psm_read_costs(self._ctx, view, _ptr(out), out.strides[1]), self._ctx)
+        return out
+
     @staticmethod
     def _map_arg(m):
         return (None, 0) if m is None else (_ptr(m), m.strides[0])
@@ -241,6 +262,9 @@ class DispEst:
         self._need_gpu()
         sel = self._lib.psm_disp_select_u16 if self.map_bits == 16 else self._lib.psm_disp_select
         capi.check(sel(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
+        if self.cost_output:
+            self.lCosts = self._read_costs(capi.PSM_LEFT)
+            self.rCosts = None if self.rDisMap is None else self._read_costs(capi.PSM_RIGHT)
         return 0
 
     def PostProcess_GPU(self):

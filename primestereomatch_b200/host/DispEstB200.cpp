@@ -2,6 +2,7 @@
 #include "DispEstB200.h"
 
 #include <cassert>
+#include <cstring>
 
 // reference src/DispEst.cpp:10-143: type check (exit(1) on mismatch), output maps, and -- instead of
 // the OpenCL context / queue / 12 cl_mem buffers / three run-time compiled programs -- one psm_ctx.
@@ -93,6 +94,26 @@ int DispEst::setViews(int v)
     return rc;
 }
 
+int DispEst::setCostOutput(bool on)
+{
+    if (!ctx) return -1;
+    const int rc = psm_set_option(ctx, PSM_OPT_COSTS, on ? 1 : 0);
+    if (rc == PSM_OK) cost_output = on;
+    return rc;
+}
+
+// one view's three cost planes (psm_read_costs, contiguous) -> three CV_32FC1 matrices
+int DispEst::read_costs(int view, cv::Mat* planes)
+{
+    cv::Mat all(3 * hei, wid, CV_32FC1);
+    if (int rc = psm_read_costs(ctx, view, all.ptr<float>(), all.step)) return rc;
+    for (int k = 0; k < 3; ++k) {
+        planes[k] = cv::Mat(hei, wid, CV_32FC1);
+        for (int y = 0; y < hei; ++y) std::memcpy(planes[k].ptr<float>(y), all.ptr<float>(k * hei + y), (size_t)wid * sizeof(float));
+    }
+    return 0;
+}
+
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
 {
@@ -141,9 +162,12 @@ int DispEst::DispSelect_GPU()
 {
     if (!ctx) return -1;
     const bool both = views == PSM_VIEWS_BOTH;   // a left-only context takes no right map
-    if (lDisMap.type() == CV_16UC1)
-        return psm_disp_select_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step);
-    return psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
+    const int rc = lDisMap.type() == CV_16UC1
+        ? psm_disp_select_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step)
+        : psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
+    if (rc || !cost_output) return rc;
+    if (int e = read_costs(PSM_LEFT, lCosts)) return e;
+    return both ? read_costs(PSM_RIGHT, rCosts) : 0;
 }
 
 // reference src/DispEst.cpp:338-344 -> PP::processDM (src/PP.cpp:402-425): the joint weighted-median filter of

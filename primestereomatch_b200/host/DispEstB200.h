@@ -87,6 +87,8 @@ public:
     cv::Mat rDisMap;
     cv::Mat lValid;   // CV_8UC1 masks of the left-right check (reference DispEst.h:81-82), 0/1; PostProcess_GPU fills them
     cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF
+    cv::Mat lCosts[3];  // setCostOutput(true): CV_32FC1 filtered costs at disparity m - 1, m, m + 1 of the selection map's
+    cv::Mat rCosts[3];  // m (psm_read_costs); DispSelect_GPU fills them, rCosts not on a left-only context
 
     int setInputImages(cv::Mat l, cv::Mat r);
     int setThreads(unsigned int newThreads);
@@ -108,6 +110,9 @@ public:
     // map alone; DispSelect_GPU and PostProcess_GPU then leave rDisMap (and rValid) untouched.  The next stage after a
     // change must be CostConst_GPU.
     int setViews(int views);
+    // PSM_OPT_COSTS: with true, DispSelect_GPU also fills lCosts / rCosts.  The next stage after a change must be
+    // CostConst_GPU.  Fails on a context that owns part of the disparity range.
+    int setCostOutput(bool on);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
@@ -141,5 +146,7 @@ private:
     unsigned int subsample_rate = 4;
     int lr_mode = PSM_LR_OFF;
     int views = PSM_VIEWS_BOTH;
+    bool cost_output = false;
+    int read_costs(int view, cv::Mat* planes);
     psm_ctx* ctx = nullptr;
 };

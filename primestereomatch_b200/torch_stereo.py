@@ -77,6 +77,7 @@ class TorchStereo:
         self.device = torch.device("cuda", index)
         self.subsample_rate = 4
         self.views = capi.PSM_VIEWS_BOTH
+        self.costs = False   # PSM_OPT_COSTS as match() last set it
         self._lib = capi.lib()
         self._ctx = C.c_void_p()
         self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
@@ -142,14 +143,21 @@ class TorchStereo:
                 raise ValueError(f"{name} is on {t.device}: frames must be CUDA tensors on the context's device {self.device}")
         return pix, lf, other[1], row_step, col_step, batched
 
-    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False):
+    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False, costs=False):
         """Disparity maps of one frame pair or a batch -> (lmap, rmap): new uint8 / uint16 tensors of shape (H, W) or
         (B, H, W) on the context's device; rmap is None on a left-only context.
+
+        costs=True -> (lmap, rmap, lcosts, rcosts): also the filtered costs beside each winner of the selection maps
+        (PSM_OPT_COSTS, psm_copy_costs_device), new float32 tensors (3, H, W) or (B, 3, H, W) whose plane k holds the cost
+        at disparity m + k - 1, bit for bit (the quiet NaN 0x7FC00000 outside [0, max_disp)); rcosts is None on a
+        left-only context.  The option is set when costs differs from the last call's, which restarts the frame.
 
         After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
         with post_process=True, and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
         host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
+        if not isinstance(costs, bool):
+            raise TypeError(f"costs must be True or False (got {costs!r})")
         pix, lf, rf, row_step, col_step, batched = self._layout(left, right, channels)
         L, ctx = self._lib, self._ctx
         H, W = self.height, self.width
@@ -159,6 +167,12 @@ class TorchStereo:
         lmap = torch.empty(shape, dtype=mdt, device=self.device)
         rmap = torch.empty(shape, dtype=mdt, device=self.device) if self.views == capi.PSM_VIEWS_BOTH else None
         row = W * lmap.element_size()
+        if costs != self.costs:
+            self._check(L.psm_set_option(ctx, capi.PSM_OPT_COSTS, int(costs)))
+            self.costs = costs
+        cshape = (len(lf), 3, H, W) if batched else (3, H, W)
+        lcost = torch.empty(cshape, dtype=torch.float32, device=self.device) if costs else None
+        rcost = torch.empty(cshape, dtype=torch.float32, device=self.device) if costs and rmap is not None else None
         self._check(L.psm_wait_stream(ctx, stream))
         for b in range(len(lf)):
             lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
@@ -172,8 +186,12 @@ class TorchStereo:
             rm = None if rmap is None else (rmap[b] if batched else rmap)
             self._check(L.psm_copy_maps_device(ctx, 1 if post_process else 0, lm.data_ptr(), row,
                                                None if rm is None else rm.data_ptr(), row))
+            if costs:
+                lc = lcost[b] if batched else lcost
+                rc = None if rcost is None else (rcost[b] if batched else rcost)
+                self._check(L.psm_copy_costs_device(ctx, lc.data_ptr(), None if rc is None else rc.data_ptr(), W * 4))
         self._check(L.psm_signal_stream(ctx, stream))
-        return lmap, rmap
+        return (lmap, rmap, lcost, rcost) if costs else (lmap, rmap)
 
     # -- measurement helpers ------------------------------------------------------------------
     def stage_ms(self, stage):
