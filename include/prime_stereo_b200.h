@@ -53,7 +53,8 @@
  * (the scratch of the reference-order pass: float frames, a non-default guided filter, PSM_CVF_NAIVE, flagged slices),
  * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
  * (its buffers and, after a change of sigma or weight type, the weight table), psm_set_option(PSM_OPT_COSTS, 1) (the
- * cost planes).  Run them once before a latency-critical
+ * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots).  Run them once before a
+ * latency-critical
  * loop.  psm_set_stream always waits for the stream it leaves.
  */
 #ifndef PRIME_STEREO_B200_H
@@ -90,8 +91,10 @@ enum {
                               0 = the caller separates select / reduce / fetch by its own cross-rank barriers */
     PSM_OPT_VIEWS = 5,     /* PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT: which disparity maps a frame computes; see
                               "Left-only frames" below */
-    PSM_OPT_COSTS = 6      /* 0 (default) or 1: the selection stages also keep the filtered costs beside each winner;
+    PSM_OPT_COSTS = 6,     /* 0 (default) or 1: the selection stages also keep the filtered costs beside each winner;
                               see psm_copy_costs_device */
+    PSM_OPT_RUNNER_UP = 7  /* 0 (default) or 1: the selection stages also keep each pixel's runner-up disparity away
+                              from the winner and its filtered cost; see psm_copy_runner_up_device */
     /* keys 100..106 are kernel tuning knobs used by bench.py experiments (variant, rows per segment, extra
        shared memory, threads per CTA, block remap, packed remainder strips off, CVC build); they never
        change results */
@@ -475,6 +478,38 @@ int psm_copy_maps_device(psm_ctx* ctx, int which, void* d_left, size_t left_step
  *     PSM_OPT_COSTS last changed did not run with PSM_OPT_COSTS = 1; a right-view read on a left-only context. */
 int psm_copy_costs_device(psm_ctx* ctx, float* d_left, float* d_right, size_t row_step);
 int psm_read_costs(psm_ctx* ctx, int view, float* dst, size_t row_step);
+
+/* Each pixel's runner-up away from its winner (PSM_OPT_RUNNER_UP = 1), for the confidence tests a caller builds on it
+ * (a uniqueness ratio as OpenCV's StereoBM / StereoSGBM uniquenessRatio, the peak ratio, the maximum margin).  The
+ * reference has no confidence output; this is not part of its pipeline.  Take the filtered volume q the last selection
+ * stage scanned (any filter path) and its map m.  The candidates are the arg-min's: d in [1, D) whose cost compares below
+ * +inf (NaN and +inf never are, -0 ties with +0), lowest cost first and the lowest d first on ties.  The runner-up r is
+ * the first candidate with |d - m| >= 2, and 0 when there is none (m = 0, D <= 3, or every cost away from m is +inf or
+ * NaN).  Per computed view, two float planes of H x W: plane 0 holds r (an exact integer), plane 1 q(r), bit for bit
+ * (the quiet NaN 0x7FC00000 where r = 0).  The exclusion width is 1 and fixed.  With PSM_OPT_COSTS the plain second
+ * minimum is the first of q(m - 1) (m - 1 >= 1), q(m + 1) (m + 1 < D) and q(r) in that order.  The post-filter and the
+ * left-right check do not change the planes; only a selection stage writes them, so on every kind of context they stay
+ * the last selection's through the next frame's psm_set_images*, psm_cost_const and filter stage.
+ *   - PSM_OPT_RUNNER_UP takes 0 or 1, anything else returns PSM_EINVAL and changes nothing.  Turning it on allocates
+ *     8 * H * W bytes per view of result planes; a blocked context also keeps the running list's entries beside its
+ *     running keys (28 * H * W bytes per view: four costs and three disparities), and a multi-device context keeps the
+ *     result planes and one slot per shard on the first shard (12 * H * W bytes per shard and view) and the lists on
+ *     every blocked shard.  A failed allocation changes no setting, on any shard.  A change resets the frame's stages as
+ *     PSM_OPT_VIEWS does: the next stage must be psm_cost_const.  Turning it on returns PSM_EINVAL on a context that owns
+ *     part of the range; 0, the default, is accepted there.  It may be on together with PSM_OPT_COSTS.
+ *   - The work, all in stage 3 (psm_stage_ms) except the fold: an unblocked context selects the map and the runner-up in
+ *     one kernel per view, in place of the plain selection (no extra launch); a blocked context's block folds keep the
+ *     lists in the launches they make anyway, and one kernel per view picks the runner-up after selection; on a
+ *     multi-device context every shard picks its candidate after the reduce (one kernel per view, a list scan of its
+ *     slices when unblocked) into its slot on the first shard, which reduces the slots (one kernel per view).
+ *     psm_launch_count counts them.  With the option off nothing of this runs.
+ *   - psm_disp_select_keys does not write the runner-up, and neither do the fused-exchange calls.
+ * psm_copy_runner_up_device writes view v's planes to caller DEVICE memory on the context's stream, asynchronously: plane
+ * k starts at dst + k * H * row_step (a contiguous (2, H, W) float32 tensor: row_step = 4 * W).  psm_read_runner_up writes
+ * one view's planes to HOST memory, same layout, and synchronises.  Arguments, left-only contexts and states as for
+ * psm_copy_costs_device / psm_read_costs, with PSM_OPT_RUNNER_UP in place of PSM_OPT_COSTS. */
+int psm_copy_runner_up_device(psm_ctx* ctx, float* d_left, float* d_right, size_t row_step);
+int psm_read_runner_up(psm_ctx* ctx, int view, float* dst, size_t row_step);
 
 /* Sharded stage 3a: per-pixel packed minima over this context's slices, written to DEVICE
  * buffers of H*W uint64 each:  key = (order_preserving_u32(cost) << 32) | global_d.

@@ -23,7 +23,7 @@ SYMBOLS = [
     "psm_set_matching_cost", "psm_set_post_filter", "psm_create_u16", "psm_disp_select_u16", "psm_disp_select_u16_async",
     "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
     "psm_create_blocked", "psm_create_multi", "psm_set_images_device_planes", "psm_wait_stream", "psm_signal_stream",
-    "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs",
+    "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs", "psm_copy_runner_up_device", "psm_read_runner_up",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -31,6 +31,7 @@ PSM_LEFT, PSM_RIGHT = 0, 1
 PSM_OPT_CVF_MODE, PSM_OPT_GRAY_MODE, PSM_OPT_TIMING, PSM_OPT_P2P_SYNC, PSM_OPT_VARIANT = 1, 2, 3, 4, 100
 PSM_OPT_VIEWS = 5
 PSM_OPT_COSTS = 6
+PSM_OPT_RUNNER_UP = 7
 PSM_VIEWS_LEFT, PSM_VIEWS_BOTH = 1, 2
 PSM_CVF_EXACT, PSM_CVF_MIXED, PSM_CVF_NAIVE = 0, 1, 2
 PSM_WMF_EXP, PSM_WMF_IV1, PSM_WMF_IV2, PSM_WMF_OFF = 0, 1, 2, 5
@@ -86,6 +87,8 @@ def lib():
     L.psm_copy_maps_device.argtypes = [vp, i, vp, sz, vp, sz]
     L.psm_copy_costs_device.argtypes = [vp, fp, fp, sz]
     L.psm_read_costs.argtypes = [vp, i, fp, sz]
+    L.psm_copy_runner_up_device.argtypes = [vp, fp, fp, sz]
+    L.psm_read_runner_up.argtypes = [vp, i, fp, sz]
     L.psm_set_images_async.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_u8_async.argtypes = [vp, u8p, sz, u8p, sz]
     L.psm_set_images_commit.argtypes = [vp]

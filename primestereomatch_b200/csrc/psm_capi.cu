@@ -114,10 +114,11 @@ struct psm_ctx {
     bool reduced_valid = false;
     cudaEvent_t ev_copied[kMaxRanks] = {};     // shard k (k >= 1) has read the frame it receives from the first shard
     cudaEvent_t ev_gathered[kMaxRanks] = {};   // PSM_OPT_COSTS: shard k's cost entries of the current frame (on its stream)
+    cudaEvent_t ev_picked[kMaxRanks] = {};     // PSM_OPT_RUNNER_UP: shard k's runner-up pick of the current frame (on its stream)
     cudaEvent_t ev_images = nullptr;           // psm_set_images_device: the caller's images as the first shard's stream sees them
     // PSM_OPT_VIEWS: 2 (both views) or 1 (the left view alone: the right view's guide, volume, selection and post-filter
-    // are skipped).  stages_reset: PSM_OPT_VIEWS or PSM_OPT_COSTS changed since the last psm_cost_const, so the volumes,
-    // maps, masks and costs are stale.
+    // are skipped).  stages_reset: PSM_OPT_VIEWS, PSM_OPT_COSTS or PSM_OPT_RUNNER_UP changed since the last psm_cost_const,
+    // so the volumes, maps, masks, costs and runner-up are stale.
     int views = 2;
     bool stages_reset = false;
     // PSM_OPT_COSTS: 1 = the selection stages also write the filtered costs beside each winner into win_cost[view]
@@ -130,6 +131,15 @@ struct psm_ctx {
     bool have_costs = false;
     // kCostFirst only where a neighbour shard below reads it
     int track_planes() const { return d_begin > 0 ? kCostFirst + 1 : kCostLast + 1; }
+    // PSM_OPT_RUNNER_UP: 1 = the selection stages also write the runner-up into ru_out[view] (kRunnerUpOut planes; a
+    // multi-device context's first shard reduces its shards' picks from ru_slots[view] into its own, the others have
+    // neither), and a blocked walk keeps the running list in ru_list[view] (kListPlanes).  All are allocated when the
+    // option is turned on.  have_runner_up: the last selection stage since the last reset wrote ru_out.
+    int runner_up = 0;
+    float* ru_out[2] = {nullptr, nullptr};
+    float* ru_list[2] = {nullptr, nullptr};
+    unsigned char* ru_slots[2] = {nullptr, nullptr};
+    bool have_runner_up = false;
     unsigned p2p_seq_right = 0;                // frames whose exchange included the right view (p2p_seq counts every frame)
     bool p2p_right_current = false;            // the last frame's exchange included the right view
     bool have_pp = false;                      // dis_pp holds the maps of a post-process since the last PSM_OPT_VIEWS change
@@ -183,7 +193,8 @@ int bind(psm_ctx* c)
     return PSM_OK;
 }
 
-// a call that would read or return right-view data: PSM_ESTATE on a left-only context, and after a PSM_OPT_VIEWS or PSM_OPT_COSTS change
+// a call that would read or return right-view data: PSM_ESTATE on a left-only context, and after a PSM_OPT_VIEWS,
+// PSM_OPT_COSTS or PSM_OPT_RUNNER_UP change
 // until psm_cost_const has built the current frame's volumes again
 int check_right_view(psm_ctx* c, const char* call)
 {
@@ -191,7 +202,8 @@ int check_right_view(psm_ctx* c, const char* call)
         return fail(c, PSM_ESTATE, "%s of the right view on a left-only context (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): the right "
                     "view is not computed; set PSM_VIEWS_BOTH", call);
     if (c->stages_reset)
-        return fail(c, PSM_ESTATE, "%s of the right view after a PSM_OPT_VIEWS or PSM_OPT_COSTS change: call psm_cost_const first", call);
+        return fail(c, PSM_ESTATE, "%s of the right view after a PSM_OPT_VIEWS, PSM_OPT_COSTS or PSM_OPT_RUNNER_UP change: "
+                    "call psm_cost_const first", call);
     return PSM_OK;
 }
 
@@ -204,11 +216,12 @@ int check_right_arg(psm_ctx* c, const void* right, const char* call)
     return PSM_OK;
 }
 
-// a stage that needs the stage state PSM_OPT_VIEWS reset
+// a stage that needs the stage state a PSM_OPT_VIEWS, PSM_OPT_COSTS or PSM_OPT_RUNNER_UP change reset
 int check_stages_reset(psm_ctx* c, const char* call)
 {
     if (c->stages_reset)
-        return fail(c, PSM_ESTATE, "%s after a PSM_OPT_VIEWS or PSM_OPT_COSTS change: the next stage must be psm_cost_const", call);
+        return fail(c, PSM_ESTATE, "%s after a PSM_OPT_VIEWS, PSM_OPT_COSTS or PSM_OPT_RUNNER_UP change: the next stage must "
+                    "be psm_cost_const", call);
     return PSM_OK;
 }
 
@@ -760,16 +773,25 @@ int launch_cvc(psm_ctx* c)
 // the result planes and the tracking planes of view v (PSM_OPT_COSTS)
 CostPlanes cost_planes(const psm_ctx* c, int v) { return {c->win_cost[v], (size_t)c->W * c->H}; }
 CostPlanes track_planes(const psm_ctx* c, int v) { return {c->track[v], (size_t)c->W * c->H}; }
+// the result planes, the running list and (on the first shard of a multi-device context of nslots shards) the slots of
+// view v (PSM_OPT_RUNNER_UP)
+CostPlanes runner_up_planes(const psm_ctx* c, int v) { return {c->ru_out[v], (size_t)c->W * c->H}; }
+CostPlanes list_planes(const psm_ctx* c, int v) { return {c->ru_list[v], (size_t)c->W * c->H}; }
+RunnerUpSlots runner_up_slots(const psm_ctx* c, int v, int nslots) { return {c->ru_slots[v], (size_t)c->W * c->H, nslots}; }
 
-// the filtered block in the volumes -> the running keys (stored by the first block, min-folded by the others), and with
-// PSM_OPT_COSTS the costs beside the running winners
+// the filtered block in the volumes -> the running keys (stored by the first block, min-folded by the others), with
+// PSM_OPT_COSTS the costs beside the running winners, and with PSM_OPT_RUNNER_UP the running lists
 int launch_fold(psm_ctx* c, bool first)
 {
     FoldParams P;
     for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->res.begin; P.d_count = c->res.count; P.first = first ? 1 : 0;
     dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, c->views);
-    if (c->costs)
+    if (c->runner_up)
+        (c->costs ? wta_fold_list_kernel<true> : wta_fold_list_kernel<false>)<<<grd, blk, 0, c->stream>>>(
+            FoldListParams{P, {list_planes(c, 0), list_planes(c, 1)}, {track_planes(c, 0), track_planes(c, 1)},
+                           c->track_planes() > kCostFirst});
+    else if (c->costs)
         wta_fold_costs_kernel<<<grd, blk, 0, c->stream>>>(
             FoldCostParams{P, {track_planes(c, 0), track_planes(c, 1)}, c->track_planes() > kCostFirst});
     else
@@ -790,6 +812,24 @@ int launch_cost_write(psm_ctx* c, int v, const void* map, CostPlanes dst)
         (c->blk_slices ? cost_write_kernel<uint16_t, true> : cost_write_kernel<uint16_t, false>)<<<grd, blk, 0, c->stream>>>(P);
     else
         (c->blk_slices ? cost_write_kernel<uint8_t, true> : cost_write_kernel<uint8_t, false>)<<<grd, blk, 0, c->stream>>>(P);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
+// The runner-up of the slices context c owns (runner_up_write_kernel), from `map` (the complete selection map of view v):
+// from a list scan of its resident volume on an unblocked context, from its running lists on a blocked one.  Into its
+// own result planes, or, where slots.base is set, into slot `slot` of the first shard's.
+int launch_runner_up_write(psm_ctx* c, int v, const void* map, RunnerUpSlots slots, int slot)
+{
+    RunnerUpWriteParams P;
+    P.map = map; P.vol = c->vol[v]; P.keys = c->run_keys[v]; P.list = list_planes(c, v); P.dst = runner_up_planes(c, v);
+    P.slots = slots; P.slot = slot;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count;
+    dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
+    if (c->map_bytes == 2)
+        (c->blk_slices ? runner_up_write_kernel<uint16_t, true> : runner_up_write_kernel<uint16_t, false>)<<<grd, blk, 0, c->stream>>>(P);
+    else
+        (c->blk_slices ? runner_up_write_kernel<uint8_t, true> : runner_up_write_kernel<uint8_t, false>)<<<grd, blk, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
@@ -844,12 +884,13 @@ P2pLayout p2p_layout(const psm_ctx* c, int nranks)
 bool exchanged(const psm_ctx* c) { return c->p2p_own && c->p2p_seq > 0; }
 
 // a selection stage wrote new maps (`own`: the context's own, not an exchange block's): the left-right masks are stale
-// and so are the costs, until the stage writes them too
+// and so are the costs and the runner-up, until the stage writes them too
 void selection_ran(psm_ctx* c, bool own)
 {
     c->lr_masks_ok = false;
     c->have_maps = c->have_maps || own;
     c->have_costs = false;
+    c->have_runner_up = false;
 }
 
 // a map call for maps of type T, named u8_call / u16_call in its two formats, on a context of the other format:
@@ -1289,6 +1330,7 @@ int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const i
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_reduced[k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied[k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_gathered[k], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_picked[k], cudaEventDisableTiming);
         if (e == cudaSuccess && k == 0) e = cudaEventCreateWithFlags(&c->ev_images, cudaEventDisableTiming);
         if (e != cudaSuccess) { fail(c, PSM_ECUDA, "event creation on device %d failed: %s", devices[k], cudaGetErrorString(e)); return bail(PSM_ECUDA); }
     }
@@ -1317,6 +1359,7 @@ int psm_destroy(psm_ctx* c)
             if (c->ev_reduced[k]) cudaEventDestroy(c->ev_reduced[k]);
             if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]);
             if (c->ev_gathered[k]) cudaEventDestroy(c->ev_gathered[k]);
+            if (c->ev_picked[k]) cudaEventDestroy(c->ev_picked[k]);
             if (k == 0 && c->ev_images) cudaEventDestroy(c->ev_images);
             psm_destroy(c->shard[k]);
         }
@@ -1348,7 +1391,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
     for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]); cudaFree(c->win_cost[v]);
-                                   cudaFree(c->track[v]); }
+                                   cudaFree(c->track[v]); cudaFree(c->ru_out[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]); }
     for (int s = 0; s < kNumStages; ++s) {
         if (c->ev0[s]) cudaEventDestroy(c->ev0[s]);
         if (c->ev1[s]) cudaEventDestroy(c->ev1[s]);
@@ -1361,8 +1404,9 @@ int psm_destroy(psm_ctx* c)
 
 }  // extern "C"
 
-// PSM_OPT_VIEWS or PSM_OPT_COSTS changed: the frame's stages start again from psm_cost_const on the current images; nothing
-// computed for the other setting (volumes, maps, masks, costs, the guide of the right view) can be read or selected from
+// PSM_OPT_VIEWS, PSM_OPT_COSTS or PSM_OPT_RUNNER_UP changed: the frame's stages start again from psm_cost_const on the
+// current images; nothing computed for the other setting (volumes, maps, masks, costs, runner-up, the guide of the right
+// view) can be read or selected from
 static void reset_stages(psm_ctx* c)
 {
     c->stages_reset = true;
@@ -1373,6 +1417,7 @@ static void reset_stages(psm_ctx* c)
     c->have_pp = false;
     c->lr_masks_ok = false;
     c->have_costs = false;
+    c->have_runner_up = false;
 }
 
 // PSM_OPT_COSTS = 1 on one context, a multi-device context's shards included: the planes it reads or writes, the result
@@ -1404,6 +1449,37 @@ static int check_costs_value(psm_ctx* c, int value)
     return PSM_OK;
 }
 
+// PSM_OPT_RUNNER_UP = 1 on one context, a multi-device context's shards included: the planes it reads or writes, the
+// result planes where `result` (a single-device context, the first shard), the slots of `nslots` shards (the first shard
+// of a multi-device context) and the running lists on a blocked context.  Only allocates: a failure leaves the setting
+// as it was.
+static int alloc_runner_up(psm_ctx* c, bool result, int nslots)
+{
+    if (int rc = bind(c)) return rc;
+    const size_t npix = (size_t)c->W * c->H, plane = npix * sizeof(float);
+    for (int v = 0; v < 2; ++v) {
+        if (result) PSM_CUDA(c, alloc_if_null(c->ru_out[v], kRunnerUpOut * plane));
+        if (nslots) PSM_CUDA(c, alloc_if_null(c->ru_slots[v], RunnerUpSlots::bytes(npix, nslots)));
+        if (c->blk_slices) PSM_CUDA(c, alloc_if_null(c->ru_list[v], kListPlanes * plane));
+    }
+    return PSM_OK;
+}
+
+// PSM_OPT_RUNNER_UP = value, its planes allocated: a blocked context's walk keeps the lists, so a change restarts the frame
+static void apply_runner_up(psm_ctx* c, int value)
+{
+    if (value != c->runner_up) {
+        reset_stages(c);
+        c->runner_up = value;
+    }
+}
+
+static int check_runner_up_value(psm_ctx* c, int value)
+{
+    if (value != 0 && value != 1) return fail(c, PSM_EINVAL, "PSM_OPT_RUNNER_UP must be 0 or 1 (got %d)", value);
+    return PSM_OK;
+}
+
 extern "C" {
 
 int psm_set_option(psm_ctx* c, int key, int value)
@@ -1419,6 +1495,14 @@ int psm_set_option(psm_ctx* c, int key, int value)
                 if (int rc = alloc_costs(c->shard[k], k == 0)) return relay(c, k, rc);
             for (int k = 0; k < c->nshards; ++k) apply_costs(c->shard[k], value);
             c->costs = value;
+            return PSM_OK;
+        }
+        if (key == PSM_OPT_RUNNER_UP) {   // as PSM_OPT_COSTS; the first shard also holds every shard's slot
+            if (int rc = check_runner_up_value(c, value)) return rc;
+            for (int k = 0; value && k < c->nshards; ++k)
+                if (int rc = alloc_runner_up(c->shard[k], k == 0, k == 0 ? c->nshards : 0)) return relay(c, k, rc);
+            for (int k = 0; k < c->nshards; ++k) apply_runner_up(c->shard[k], value);
+            c->runner_up = value;
             return PSM_OK;
         }
         if (int rc = forward(c, [&](psm_ctx* s) { return psm_set_option(s, key, value); })) return rc;
@@ -1442,6 +1526,16 @@ int psm_set_option(psm_ctx* c, int key, int value)
                         "psm_create_blocked over [0, max_disp), or psm_create_multi)", c->d_begin, c->d_begin + c->d_count, c->D);
         if (int rc = value ? alloc_costs(c, true) : PSM_OK) return rc;
         apply_costs(c, value);
+        return PSM_OK;
+    case PSM_OPT_RUNNER_UP:
+        if (int rc = check_runner_up_value(c, value)) return rc;
+        if (value && (c->d_begin != 0 || c->d_count != c->D))
+            return fail(c, PSM_EINVAL, "PSM_OPT_RUNNER_UP on a context that owns slices [%d,%d) of %d: the runner-up and "
+                        "the winner may lie on different contexts; use a context over the whole range (psm_create, "
+                        "psm_create_u16 / psm_create_blocked over [0, max_disp), or psm_create_multi)", c->d_begin,
+                        c->d_begin + c->d_count, c->D);
+        if (int rc = value ? alloc_runner_up(c, true, 0) : PSM_OK) return rc;
+        apply_runner_up(c, value);
         return PSM_OK;
     case PSM_OPT_CVF_MODE:
         if (value != PSM_CVF_EXACT && value != PSM_CVF_MIXED && value != PSM_CVF_NAIVE)
@@ -1692,8 +1786,12 @@ static int select_maps(psm_ctx* c)
     }
     for (int v = 0; v < c->views; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
-                                                  reinterpret_cast<T*>(c->dis[v]), nullptr);
+        if (c->runner_up)   // the map and the runner-up in one read of the volume
+            wta_runner_up_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
+                                                                reinterpret_cast<T*>(c->dis[v]), runner_up_planes(c, v));
+        else
+            wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
+                                                      reinterpret_cast<T*>(c->dis[v]), nullptr);
         PSM_LAUNCH_CHECK(c);
     }
     return PSM_OK;
@@ -1755,6 +1853,11 @@ int psm_disp_select_device(psm_ctx* c)
             if (int rc = launch_cost_write(c, v, c->dis[v], cost_planes(c, v))) return rc;
         c->have_costs = true;
     }
+    if (c->runner_up) {   // select_maps wrote it on an unblocked context; a blocked one picks it from its running lists
+        for (int v = 0; c->blk_slices && v < c->views; ++v)
+            if (int rc = launch_runner_up_write(c, v, c->dis[v], RunnerUpSlots{}, 0)) return rc;
+        c->have_runner_up = true;
+    }
     return stage_end(c, 3);
 }
 
@@ -1786,7 +1889,8 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
     if (!d_keys_left || (c->views == 2 && !d_keys_right)) return fail(c, PSM_EINVAL, "null key buffer");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
-    c->have_costs = false;   // keys carry no costs beside the winner
+    c->have_costs = false;   // keys carry no costs beside the winner, and no runner-up
+    c->have_runner_up = false;
     uint64_t* keys[2] = {d_keys_left, d_keys_right};
     if (c->blk_slices) {   // the running keys are this context's minima already
         for (int v = 0; v < c->views; ++v)
@@ -1995,6 +2099,19 @@ static int p2p_wait_done(psm_ctx* c)
 //      stages on its own stream.
 // The first shard's result planes are written by these gathers alone, never by a filter stage (its tracking planes are
 // separate), so they hold frame f's costs until the next select, as on a single-device context.
+// With PSM_OPT_RUNNER_UP, every shard then writes its pick into its own slot on the first shard, and the first shard
+// reduces the slots into its result planes:
+//   9. shard k's pick reads its copy of the complete maps, which every shard's reduce writes: it waits for them;
+//  10. the first shard's slot reduce reads every shard's slot: it waits for every pick.  Its stream carries every reader
+//      of the result planes (psm_copy_runner_up_device, psm_read_runner_up), queued behind the reduce;
+//  11. the picks overwrite slots that the first shard's slot reduce of frame f - 1 read: each pick follows its shard's
+//      reduce, which waits for the first shard's scatter (2), queued behind that slot reduce;
+//  12. a pick reads its shard's map, which the next frame's reduces overwrite: they wait for that shard's next scatter
+//      (2), queued behind the pick; and the volume or running lists it reads are rewritten only by later stages on its
+//      own stream.
+// Every slot has one writer and the reduce takes the first slot of the lowest key, so the result does not depend on the
+// order in which the picks land.  The result planes are written by the slot reduce alone, so they hold frame f's
+// runner-up until the next select.
 // No kernel waits for another queued behind it, so shards on one device are as safe as shards on several.
 static int multi_select(psm_ctx* c)
 {
@@ -2034,11 +2151,34 @@ static int multi_select(psm_ctx* c)
             PSM_CUDA(c, cudaEventRecord(c->ev_gathered[k], s->stream));
         }
     }
+    if (c->runner_up) {
+        for (int k = 0; k < n; ++k) {
+            psm_ctx* s = c->shard[k];
+            if (int rc = bind(s)) return relay(c, k, rc);
+            for (int j = 0; j < n; ++j)
+                if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_reduced[j], 0));   // 9
+            const P2pLayout L = p2p_layout(s, s->p2p_nranks);
+            for (int v = 0; v < s->views; ++v)   // peer stores between distinct devices
+                if (int rc = launch_runner_up_write(s, v, L.maps(s->p2p_own, v), runner_up_slots(s0, v, n), k))
+                    return relay(c, k, rc);
+            PSM_CUDA(c, cudaEventRecord(c->ev_picked[k], s->stream));
+        }
+    }
     if (int rc = bind(s0)) return relay(c, 0, rc);
     for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_reduced[j], 0));   // 3
     if (c->costs) {
         for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_gathered[j], 0));   // 6
         s0->have_costs = true;
+    }
+    if (c->runner_up) {
+        for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_picked[j], 0));   // 10
+        const size_t npix = (size_t)s0->W * s0->H;
+        for (int v = 0; v < s0->views; ++v) {
+            runner_up_reduce_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, s0->stream>>>(runner_up_slots(s0, v, n),
+                                                                                           runner_up_planes(s0, v));
+            PSM_LAUNCH_CHECK(s0);
+        }
+        s0->have_runner_up = true;
     }
     return relay(c, 0, stage_end(s0, 3));
 }
@@ -2266,12 +2406,19 @@ static int check_costs_ready(psm_ctx* c, const char* call)
     return PSM_OK;
 }
 
-// view v's kCostOut planes -> dst (plane k at dst + k * H * row_step) on the context's stream: one copy of 3H rows
-static int copy_costs_out(psm_ctx* c, int v, float* dst, size_t row_step, cudaMemcpyKind kind)
+// nplanes planes of H x W floats at src -> dst (plane k at dst + k * H * row_step) on the context's stream: one copy of
+// nplanes * H rows
+static int copy_planes_out(psm_ctx* c, const float* src, int nplanes, float* dst, size_t row_step, cudaMemcpyKind kind)
 {
     const size_t row = (size_t)c->W * sizeof(float);
-    PSM_CUDA(c, cudaMemcpy2DAsync(dst, row_step, c->win_cost[v], row, row, (size_t)kCostOut * c->H, kind, c->stream));
+    PSM_CUDA(c, cudaMemcpy2DAsync(dst, row_step, src, row, row, (size_t)nplanes * c->H, kind, c->stream));
     return PSM_OK;
+}
+
+// view v's kCostOut planes -> dst
+static int copy_costs_out(psm_ctx* c, int v, float* dst, size_t row_step, cudaMemcpyKind kind)
+{
+    return copy_planes_out(c, c->win_cost[v], kCostOut, dst, row_step, kind);
 }
 
 int psm_copy_costs_device(psm_ctx* c, float* d_left, float* d_right, size_t row_step)
@@ -2304,6 +2451,53 @@ int psm_read_costs(psm_ctx* c, int view, float* dst, size_t row_step)
         if (int rc = check_right_view(c, "psm_read_costs")) return rc;
     if (int rc = check_costs_ready(c, "psm_read_costs")) return rc;
     if (int rc = copy_costs_out(c, view, dst, row_step, cudaMemcpyDeviceToHost)) return rc;
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
+}
+
+// the runner-up of the last selection stage for psm_copy_runner_up_device and psm_read_runner_up
+static int check_runner_up_ready(psm_ctx* c, const char* call)
+{
+    if (int rc = check_stages_reset(c, call)) return rc;
+    if (!c->have_runner_up)
+        return fail(c, PSM_ESTATE, "%s: no runner-up; the last selection stage since the context was created or the last "
+                    "PSM_OPT_VIEWS / PSM_OPT_COSTS / PSM_OPT_RUNNER_UP change did not write it (psm_disp_select* with "
+                    "PSM_OPT_RUNNER_UP = 1)", call);
+    return PSM_OK;
+}
+
+int psm_copy_runner_up_device(psm_ctx* c, float* d_left, float* d_right, size_t row_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (int rc = check_right_arg(c, d_right, "psm_copy_runner_up_device")) return rc;
+    const size_t row = (size_t)c->W * sizeof(float);
+    if (!d_left || (c->views == 2 && !d_right) || row_step < row)
+        return fail(c, PSM_EINVAL, "psm_copy_runner_up_device: bad runner-up plane pointer/step (row_step must be at "
+                    "least %zu bytes)", row);
+    // a multi-device context's runner-up is the first shard's
+    if (is_multi(c)) return relay(c, 0, psm_copy_runner_up_device(c->shard[0], d_left, d_right, row_step));
+    if (int rc = bind(c)) return rc;
+    if (int rc = check_runner_up_ready(c, "psm_copy_runner_up_device")) return rc;
+    float* dst[2] = {d_left, d_right};
+    for (int v = 0; v < c->views; ++v)
+        if (int rc = copy_planes_out(c, c->ru_out[v], kRunnerUpOut, dst[v], row_step, cudaMemcpyDefault)) return rc;
+    return PSM_OK;
+}
+
+int psm_read_runner_up(psm_ctx* c, int view, float* dst, size_t row_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
+    const size_t row = (size_t)c->W * sizeof(float);
+    if (!dst || row_step < row)
+        return fail(c, PSM_EINVAL, "psm_read_runner_up: bad runner-up plane pointer/step (row_step must be at least %zu "
+                    "bytes)", row);
+    if (is_multi(c)) return relay(c, 0, psm_read_runner_up(c->shard[0], view, dst, row_step));
+    if (int rc = bind(c)) return rc;
+    if (view == PSM_RIGHT)
+        if (int rc = check_right_view(c, "psm_read_runner_up")) return rc;
+    if (int rc = check_runner_up_ready(c, "psm_read_runner_up")) return rc;
+    if (int rc = copy_planes_out(c, c->ru_out[view], kRunnerUpOut, dst, row_step, cudaMemcpyDeviceToHost)) return rc;
     PSM_CUDA(c, cudaStreamSynchronize(c->stream));
     return PSM_OK;
 }

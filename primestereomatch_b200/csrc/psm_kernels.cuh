@@ -661,6 +661,26 @@ struct CostPlanes {
     float* base;
     size_t npix;   // H * W
     __host__ __device__ float* plane(int k) const { return base + (size_t)k * npix; }
+    __host__ __device__ unsigned* uplane(int k) const { return reinterpret_cast<unsigned*>(plane(k)); }
+};
+
+// The runner-up (PSM_OPT_RUNNER_UP), in planes of the same shape.  The result: kRunnerUpOut planes, r as a float and
+// q(r) bit for bit (kCostNaN where r = 0); only the selection stages write them.  A blocked context's running list
+// (kListPlanes, beside the head's key in its running keys): planes kListCost + e hold the cost bits of entries e = 0..3,
+// planes kListD + e - 1 the d of entries e = 1..3.  A multi-device context's slots on the first shard (RunnerUpSlots):
+// per shard and pixel, the candidate's key and its cost bits.
+constexpr int kRunnerUpOut = 2, kListLen = 4, kListCost = 0, kListD = 4, kListPlanes = 7;
+
+struct RunnerUpSlots {
+    unsigned char* base;   // [nslots][npix] keys, then [nslots][npix] cost bits
+    size_t npix;
+    int nslots;
+    static size_t bytes(size_t npix, int nslots) { return (size_t)nslots * npix * (sizeof(unsigned long long) + sizeof(float)); }
+    __host__ __device__ unsigned long long* key(int k) const { return reinterpret_cast<unsigned long long*>(base) + (size_t)k * npix; }
+    __host__ __device__ float* cost(int k) const
+    {
+        return reinterpret_cast<float*>(base + (size_t)nslots * npix * sizeof(unsigned long long)) + (size_t)k * npix;
+    }
 };
 
 // wta_scan4 over slices [d_begin, d_begin + d_count), tracking the costs beside the running minimum: on a new minimum at
@@ -685,6 +705,19 @@ __device__ __forceinline__ void wta_scan4_costs(const float* p, size_t plane, in
             if (dl == 0) first[j] = c[j];
         }
     }
+}
+
+// one pixel's step of wta_scan4_costs at slice d, the dl-th of the range, for the list scan (list_scan4) that tracks the
+// costs in the same read.  wta_scan4_costs keeps its own copy of these lines: calling this from it changes the SASS of
+// wta_fold_costs_kernel.
+__device__ __forceinline__ void costs_step(float c, int d, int dl, float nan, float& mc, int& md, float& lo, float& ce,
+                                           float& hi, float& prev, float& first)
+{
+    if (md == d - 1) hi = c;
+    if (d == 0) ce = c;
+    else if (c < mc) { mc = c; md = d; lo = prev; ce = c; hi = nan; }
+    prev = c;
+    if (dl == 0) first = c;
 }
 
 // wta_fold_kernel with the costs tracked in track[view] (the tracking planes).  Planes 0..2 hold the running winner's
@@ -777,6 +810,255 @@ __global__ void __launch_bounds__(256) cost_write_kernel(const CostWriteParams P
         }
         P.dst.plane(k)[i] = q;
     }
+}
+
+// ------------------------------------------------------------------------------------------
+// The runner-up away from the winner (PSM_OPT_RUNNER_UP).  The candidates are the arg-min's: d in [1, D) whose cost
+// compares below +inf, in the order of wta_key (the cost, -0 equal to +0, then the lowest d).  The runner-up r of a pixel
+// with map m is the first candidate with |d - m| >= 2, 0 when there is none; the result planes hold (float)r and q(r)
+// bit for bit (kCostNaN where r = 0).
+// Every path keeps, per pixel, the list of its four lowest candidates, lowest first, empty entries (+inf, 0) behind them.
+// Four are enough: at most three entries lie in {m - 1, m, m + 1}, so the first entry outside them is the lowest
+// candidate outside them.  The list is mergeable: the four lowest of a union of disjoint slice ranges are the four
+// lowest of the ranges' lists.  So a blocked walk folds each block's list into a running one, and the shards of a
+// multi-device context each pick from their own list and the first shard takes the lowest key of the picks.
+// ------------------------------------------------------------------------------------------
+// c at slice d into a sorted list whose entries all come from slices below d or cost less: the strict < puts it behind
+// every entry of equal cost, as the arg-min's lowest-d rule does, and a +inf or NaN cost never enters
+__device__ __forceinline__ void list_insert(float (&lc)[kListLen], int (&ld)[kListLen], float c, int d)
+{
+    const bool b0 = c < lc[0], b1 = c < lc[1], b2 = c < lc[2], b3 = c < lc[3];
+    lc[3] = b2 ? lc[2] : (b3 ? c : lc[3]);  ld[3] = b2 ? ld[2] : (b3 ? d : ld[3]);
+    lc[2] = b1 ? lc[1] : (b2 ? c : lc[2]);  ld[2] = b1 ? ld[1] : (b2 ? d : ld[2]);
+    lc[1] = b0 ? lc[0] : (b1 ? c : lc[1]);  ld[1] = b0 ? ld[0] : (b1 ? d : ld[1]);
+    lc[0] = b0 ? c : lc[0];                 ld[0] = b0 ? d : ld[0];
+}
+
+__device__ __forceinline__ void list_clear(float (&lc)[4][kListLen], int (&ld)[4][kListLen])
+{
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int e = 0; e < kListLen; ++e) { lc[j][e] = INFINITY; ld[j][e] = 0; }
+}
+
+// wta_scan4_costs's state of four pixels, for a list scan that also tracks the costs beside the winner
+struct CostTrack4 {
+    float mc[4];
+    int md[4];
+    float lo[4], ce[4], hi[4], prev[4], first[4];
+};
+
+// The lists of four pixels over slices [d_begin, d_begin + d_count), as wta_scan4 reads them (slice dl at p + dl * plane).
+// The head of each list is wta_scan4's (mc, md).  kCosts: t also takes wta_scan4_costs's steps, in the same read.
+template <bool kCosts>
+__device__ __forceinline__ void list_scan4(const float* p, size_t plane, int d_begin, int d_count, float (&lc)[4][kListLen],
+                                           int (&ld)[4][kListLen], CostTrack4* t)
+{
+    const float nan = __uint_as_float(kCostNaNBits);
+    int dl = (!kCosts && d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (the costs scan still reads it)
+#pragma unroll 8
+    for (; dl < d_count; ++dl) {
+        const float4 c4 = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
+        const float c[4] = {c4.x, c4.y, c4.z, c4.w};
+        const int d = d_begin + dl;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if constexpr (kCosts)
+                costs_step(c[j], d, dl, nan, t->mc[j], t->md[j], t->lo[j], t->ce[j], t->hi[j], t->prev[j], t->first[j]);
+            if (!kCosts || d != 0) list_insert(lc[j], ld[j], c[j], d);
+        }
+    }
+}
+
+// the runner-up of a pixel with map m from its list: (r, q(r)), or (0, kCostNaN)
+__device__ __forceinline__ void runner_up_pick(const float (&lc)[kListLen], const int (&ld)[kListLen], int m, int& r, float& q)
+{
+    r = 0;
+    q = __uint_as_float(kCostNaNBits);
+#pragma unroll
+    for (int e = kListLen - 1; e >= 0; --e)
+        if (ld[e] != 0 && abs(ld[e] - m) >= 2) { r = ld[e]; q = lc[e]; }
+}
+
+// The selection of an unblocked single-device context with the runner-up: wta_kernel's map (the lists' heads) and the
+// result planes, in one read of the volume.
+template <typename T>
+__global__ void __launch_bounds__(256) wta_runner_up_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin,
+                                                            int d_count, T* __restrict__ dis, const CostPlanes dst)
+{
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y;
+    if (x4 >= W) return;
+    float lc[4][kListLen];
+    int ld[4][kListLen];
+    list_clear(lc, ld);
+    list_scan4<false>(vol + (size_t)y * Wp + x4, (size_t)H * Wp, d_begin, d_count, lc, ld, nullptr);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int x = x4 + j;
+        if (x >= W) continue;
+        const size_t i = (size_t)y * W + x;
+        int r;
+        float q;
+        runner_up_pick(lc[j], ld[j], ld[j][0], r, q);
+        dis[i] = (T)ld[j][0];
+        dst.plane(0)[i] = (float)r;
+        dst.plane(1)[i] = q;
+    }
+}
+
+// wta_fold_kernel with the running list in list[view] (the head's key stays in the running keys): the block's list
+// folds into it, entry by entry, and only a list that changes is written back.  kCosts: wta_fold_costs_kernel's
+// tracking too, from the same read, with its own key comparison.
+struct FoldListParams {
+    FoldParams f;
+    CostPlanes list[2];
+    CostPlanes track[2];   // kCosts
+    int write_first;       // kCosts
+};
+
+template <bool kCosts>
+__global__ void __launch_bounds__(256) wta_fold_list_kernel(const FoldListParams P)
+{
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y, view = blockIdx.z;
+    if (x4 >= P.f.W) return;
+    const size_t plane = (size_t)P.f.H * P.f.Wp;
+    const float* p = (view ? P.f.vol[1] : P.f.vol[0]) + (size_t)y * P.f.Wp + x4;
+    unsigned long long* k = (view ? P.f.keys[1] : P.f.keys[0]) + (size_t)y * P.f.W;
+    const CostPlanes L = view ? P.list[1] : P.list[0];
+    const size_t row = (size_t)y * P.f.W;
+    float lc[4][kListLen];
+    int ld[4][kListLen];
+    list_clear(lc, ld);
+    CostTrack4 t;
+    if constexpr (kCosts) {
+        const CostPlanes tr = view ? P.track[1] : P.track[0];
+        const float nan = __uint_as_float(kCostNaNBits);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            t.mc[j] = INFINITY; t.md[j] = 0; t.lo[j] = t.ce[j] = t.hi[j] = t.prev[j] = nan;
+            if (!P.f.first && x4 + j < P.f.W) t.prev[j] = tr.plane(kCostLast)[row + x4 + j];
+        }
+    }
+    list_scan4<kCosts>(p, plane, P.f.d_begin, P.f.d_count, lc, ld, &t);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int x = x4 + j;
+        if (x >= P.f.W) continue;
+        const size_t i = row + x;
+        const unsigned long long old = P.f.first ? 0ull : k[x];
+        if constexpr (kCosts) {   // wta_fold_costs_kernel's epilogue, but the key is written below
+            const CostPlanes tr = view ? P.track[1] : P.track[0];
+            tr.plane(kCostLast)[i] = t.prev[j];
+            bool win = true;
+            if (P.f.first) {
+                if (P.write_first) tr.plane(kCostFirst)[i] = t.first[j];
+            } else {
+                win = wta_key(t.mc[j], t.md[j]) < old;
+                if (!win && (int)(unsigned)old == P.f.d_begin - 1) tr.plane(2)[i] = t.first[j];
+            }
+            if (win) { tr.plane(0)[i] = t.lo[j]; tr.plane(1)[i] = t.ce[j]; tr.plane(2)[i] = t.hi[j]; }
+        }
+        float rc[kListLen];
+        int rd[kListLen];
+        if (P.f.first) {
+#pragma unroll
+            for (int e = 0; e < kListLen; ++e) { rc[e] = lc[j][e]; rd[e] = ld[j][e]; }
+        } else {
+            rc[3] = L.plane(kListCost + 3)[i];
+            if (!(lc[j][0] < rc[3])) continue;   // no entry of the block enters the running list
+            rd[0] = (int)(unsigned)old;
+            rc[0] = L.plane(kListCost)[i];
+#pragma unroll
+            for (int e = 1; e < kListLen; ++e) {
+                if (e < 3) rc[e] = L.plane(kListCost + e)[i];
+                rd[e] = (int)L.uplane(kListD + e - 1)[i];
+            }
+#pragma unroll
+            for (int e = 0; e < kListLen; ++e) list_insert(rc, rd, lc[j][e], ld[j][e]);
+        }
+        k[x] = wta_key(rc[0], rd[0]);
+#pragma unroll
+        for (int e = 0; e < kListLen; ++e) {
+            L.plane(kListCost + e)[i] = rc[e];
+            if (e > 0) L.uplane(kListD + e - 1)[i] = (unsigned)rd[e];
+        }
+    }
+}
+
+// The runner-up of the slices a context owns, from the complete selection map (T): from a list scan of its resident
+// volume (kTracked = false: an unblocked shard) or from its running list (kTracked = true: a blocked context).  Into the
+// result planes, or, where slots.base is set (a shard of a multi-device context), into slot `slot` of the first shard's
+// slots as (key, cost bits), wta_key(+inf, 0) and kCostNaN where it has none.
+struct RunnerUpWriteParams {
+    const void* map;                    // [H][W] of T
+    const float* vol;                   // kTracked = false: the filtered volume of slices [d_begin, d_begin + d_count)
+    const unsigned long long* keys;     // kTracked = true: the running keys (the lists' heads) ...
+    CostPlanes list;                    // ... and the running lists
+    CostPlanes dst;
+    RunnerUpSlots slots;
+    int slot, W, H, Wp, d_begin, d_count;
+};
+
+template <typename T, bool kTracked>
+__global__ void __launch_bounds__(256) runner_up_write_kernel(const RunnerUpWriteParams P)
+{
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y;
+    if (x4 >= P.W) return;
+    const size_t row = (size_t)y * P.W;
+    float lc[4][kListLen];
+    int ld[4][kListLen];
+    list_clear(lc, ld);
+    if constexpr (!kTracked) {
+        list_scan4<false>(P.vol + (size_t)y * P.Wp + x4, (size_t)P.H * P.Wp, P.d_begin, P.d_count, lc, ld, nullptr);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (x4 + j >= P.W) continue;
+            const size_t i = row + x4 + j;
+            ld[j][0] = (int)(unsigned)P.keys[i];
+#pragma unroll
+            for (int e = 0; e < kListLen; ++e) {
+                lc[j][e] = P.list.plane(kListCost + e)[i];
+                if (e > 0) ld[j][e] = (int)P.list.uplane(kListD + e - 1)[i];
+            }
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int x = x4 + j;
+        if (x >= P.W) continue;
+        const size_t i = row + x;
+        int r;
+        float q;
+        runner_up_pick(lc[j], ld[j], static_cast<const T*>(P.map)[i], r, q);
+        if (P.slots.base) {
+            P.slots.key(P.slot)[i] = r ? wta_key(q, r) : wta_key(INFINITY, 0);
+            P.slots.cost(P.slot)[i] = q;
+        } else {
+            P.dst.plane(0)[i] = (float)r;
+            P.dst.plane(1)[i] = q;
+        }
+    }
+}
+
+// The first shard's runner-up: the lowest key of the shards' picks (the first slot on equal keys, which only empty
+// picks share) and its cost bits
+__global__ void __launch_bounds__(256) runner_up_reduce_kernel(const RunnerUpSlots S, const CostPlanes dst)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= S.npix) return;
+    unsigned long long k = S.key(0)[i];
+    int best = 0;
+    for (int s = 1; s < S.nslots; ++s) {
+        const unsigned long long v = S.key(s)[i];
+        if (v < k) { k = v; best = s; }
+    }
+    dst.plane(0)[i] = (float)(unsigned)k;
+    dst.plane(1)[i] = S.cost(best)[i];
 }
 
 // Sharded WTA fused with its exchange (reduce-scatter + all-gather of a min-reduction, hand-rolled

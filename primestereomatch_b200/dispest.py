@@ -95,6 +95,8 @@ class DispEst:
         self.lr_mode = capi.PSM_LR_OFF
         self.cost_output = False
         self.lCosts = self.rCosts = None   # setCostOutput(True): DispSelect_GPU's (3, H, W) float32 costs
+        self.runner_up_output = False
+        self.lRunnerUp = self.rRunnerUp = None   # setRunnerUpOutput(True): DispSelect_GPU's (2, H, W) float32 runner-up
         if devices is not None and (d_begin != 0 or d_count is not None):
             raise ValueError("devices (a multi-device context over the whole range) excludes d_begin / d_count")
         self._lImg, self._rImg = l, r
@@ -219,6 +221,25 @@ class DispEst:
         capi.check(self._lib.psm_read_costs(self._ctx, view, _ptr(out), out.strides[1]), self._ctx)
         return out
 
+    def setRunnerUpOutput(self, on):
+        """Whether DispSelect_GPU also fills lRunnerUp / rRunnerUp (PSM_OPT_RUNNER_UP): numpy float32 (2, H, W), plane 0
+        the runner-up r (the lowest-cost disparity d >= 1 with |d - m| >= 2, m the selection map; 0 where none exists),
+        plane 1 its filtered cost bit for bit (the quiet NaN 0x7FC00000 where r = 0).  rRunnerUp is None on left-only
+        frames.  Changing it restarts the frame at CostConst_GPU.  Raises TypeError unless on is a bool, PsmError on a
+        context that owns part of the disparity range (d_begin / d_count)."""
+        if not isinstance(on, bool):
+            raise TypeError(f"setRunnerUpOutput takes True or False (got {on!r})")
+        self._need_gpu()
+        capi.check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_RUNNER_UP, int(on)), self._ctx)
+        self.runner_up_output = on
+        self.lRunnerUp = self.rRunnerUp = None
+        return 0
+
+    def _read_runner_up(self, view):
+        out = np.empty((2, self.hei, self.wid), np.float32)
+        capi.check(self._lib.psm_read_runner_up(self._ctx, view, _ptr(out), out.strides[1]), self._ctx)
+        return out
+
     @staticmethod
     def _map_arg(m):
         return (None, 0) if m is None else (_ptr(m), m.strides[0])
@@ -265,6 +286,9 @@ class DispEst:
         if self.cost_output:
             self.lCosts = self._read_costs(capi.PSM_LEFT)
             self.rCosts = None if self.rDisMap is None else self._read_costs(capi.PSM_RIGHT)
+        if self.runner_up_output:
+            self.lRunnerUp = self._read_runner_up(capi.PSM_LEFT)
+            self.rRunnerUp = None if self.rDisMap is None else self._read_runner_up(capi.PSM_RIGHT)
         return 0
 
     def PostProcess_GPU(self):

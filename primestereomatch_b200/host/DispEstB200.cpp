@@ -102,17 +102,28 @@ int DispEst::setCostOutput(bool on)
     return rc;
 }
 
-// one view's three cost planes (psm_read_costs, contiguous) -> three CV_32FC1 matrices
-int DispEst::read_costs(int view, cv::Mat* planes)
+int DispEst::setRunnerUpOutput(bool on)
 {
-    cv::Mat all(3 * hei, wid, CV_32FC1);
-    if (int rc = psm_read_costs(ctx, view, all.ptr<float>(), all.step)) return rc;
-    for (int k = 0; k < 3; ++k) {
+    if (!ctx) return -1;
+    const int rc = psm_set_option(ctx, PSM_OPT_RUNNER_UP, on ? 1 : 0);
+    if (rc == PSM_OK) runner_up_output = on;
+    return rc;
+}
+
+// one view's n planes (read: psm_read_costs or psm_read_runner_up, contiguous) -> n CV_32FC1 matrices
+int DispEst::read_planes(int view, int n, int (*read)(psm_ctx*, int, float*, size_t), cv::Mat* planes)
+{
+    cv::Mat all(n * hei, wid, CV_32FC1);
+    if (int rc = read(ctx, view, all.ptr<float>(), all.step)) return rc;
+    for (int k = 0; k < n; ++k) {
         planes[k] = cv::Mat(hei, wid, CV_32FC1);
         for (int y = 0; y < hei; ++y) std::memcpy(planes[k].ptr<float>(y), all.ptr<float>(k * hei + y), (size_t)wid * sizeof(float));
     }
     return 0;
 }
+
+// one view's three cost planes -> three CV_32FC1 matrices
+int DispEst::read_costs(int view, cv::Mat* planes) { return read_planes(view, 3, psm_read_costs, planes); }
 
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
@@ -165,9 +176,18 @@ int DispEst::DispSelect_GPU()
     const int rc = lDisMap.type() == CV_16UC1
         ? psm_disp_select_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step)
         : psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
-    if (rc || !cost_output) return rc;
-    if (int e = read_costs(PSM_LEFT, lCosts)) return e;
-    return both ? read_costs(PSM_RIGHT, rCosts) : 0;
+    if (rc) return rc;
+    if (cost_output) {
+        if (int e = read_costs(PSM_LEFT, lCosts)) return e;
+        if (both)
+            if (int e = read_costs(PSM_RIGHT, rCosts)) return e;
+    }
+    if (runner_up_output) {
+        if (int e = read_planes(PSM_LEFT, 2, psm_read_runner_up, lRunnerUp)) return e;
+        if (both)
+            if (int e = read_planes(PSM_RIGHT, 2, psm_read_runner_up, rRunnerUp)) return e;
+    }
+    return 0;
 }
 
 // reference src/DispEst.cpp:338-344 -> PP::processDM (src/PP.cpp:402-425): the joint weighted-median filter of

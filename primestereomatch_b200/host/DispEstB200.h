@@ -89,6 +89,8 @@ public:
     cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF
     cv::Mat lCosts[3];  // setCostOutput(true): CV_32FC1 filtered costs at disparity m - 1, m, m + 1 of the selection map's
     cv::Mat rCosts[3];  // m (psm_read_costs); DispSelect_GPU fills them, rCosts not on a left-only context
+    cv::Mat lRunnerUp[2];  // setRunnerUpOutput(true): CV_32FC1 runner-up disparity r (0 where none exists) and its
+    cv::Mat rRunnerUp[2];  // filtered cost (psm_read_runner_up); DispSelect_GPU fills them, rRunnerUp not when left-only
 
     int setInputImages(cv::Mat l, cv::Mat r);
     int setThreads(unsigned int newThreads);
@@ -113,6 +115,9 @@ public:
     // PSM_OPT_COSTS: with true, DispSelect_GPU also fills lCosts / rCosts.  The next stage after a change must be
     // CostConst_GPU.  Fails on a context that owns part of the disparity range.
     int setCostOutput(bool on);
+    // PSM_OPT_RUNNER_UP: with true, DispSelect_GPU also fills lRunnerUp / rRunnerUp.  The next stage after a change must
+    // be CostConst_GPU.  Fails on a context that owns part of the disparity range.
+    int setRunnerUpOutput(bool on);
     int printCV(void);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
@@ -147,6 +152,8 @@ private:
     int lr_mode = PSM_LR_OFF;
     int views = PSM_VIEWS_BOTH;
     bool cost_output = false;
+    bool runner_up_output = false;
     int read_costs(int view, cv::Mat* planes);
+    int read_planes(int view, int n, int (*read)(psm_ctx*, int, float*, size_t), cv::Mat* planes);
     psm_ctx* ctx = nullptr;
 };

@@ -78,6 +78,7 @@ class TorchStereo:
         self.subsample_rate = 4
         self.views = capi.PSM_VIEWS_BOTH
         self.costs = False   # PSM_OPT_COSTS as match() last set it
+        self.runner_up = False   # PSM_OPT_RUNNER_UP as match() last set it
         self._lib = capi.lib()
         self._ctx = C.c_void_p()
         self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
@@ -143,7 +144,7 @@ class TorchStereo:
                 raise ValueError(f"{name} is on {t.device}: frames must be CUDA tensors on the context's device {self.device}")
         return pix, lf, other[1], row_step, col_step, batched
 
-    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False, costs=False):
+    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False, costs=False, runner_up=False):
         """Disparity maps of one frame pair or a batch -> (lmap, rmap): new uint8 / uint16 tensors of shape (H, W) or
         (B, H, W) on the context's device; rmap is None on a left-only context.
 
@@ -152,12 +153,19 @@ class TorchStereo:
         at disparity m + k - 1, bit for bit (the quiet NaN 0x7FC00000 outside [0, max_disp)); rcosts is None on a
         left-only context.  The option is set when costs differs from the last call's, which restarts the frame.
 
+        runner_up=True -> also (lrunner, rrunner), appended after any costs: each pixel's runner-up away from the winner
+        (PSM_OPT_RUNNER_UP, psm_copy_runner_up_device), new float32 tensors (2, H, W) or (B, 2, H, W): plane 0 the
+        disparity r (0 where none exists), plane 1 its filtered cost bit for bit (the quiet NaN 0x7FC00000 where r = 0);
+        rrunner is None on a left-only context.  The option is set when runner_up differs from the last call's.
+
         After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
         with post_process=True, and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
         host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
         if not isinstance(costs, bool):
             raise TypeError(f"costs must be True or False (got {costs!r})")
+        if not isinstance(runner_up, bool):
+            raise TypeError(f"runner_up must be True or False (got {runner_up!r})")
         pix, lf, rf, row_step, col_step, batched = self._layout(left, right, channels)
         L, ctx = self._lib, self._ctx
         H, W = self.height, self.width
@@ -173,6 +181,12 @@ class TorchStereo:
         cshape = (len(lf), 3, H, W) if batched else (3, H, W)
         lcost = torch.empty(cshape, dtype=torch.float32, device=self.device) if costs else None
         rcost = torch.empty(cshape, dtype=torch.float32, device=self.device) if costs and rmap is not None else None
+        if runner_up != self.runner_up:
+            self._check(L.psm_set_option(ctx, capi.PSM_OPT_RUNNER_UP, int(runner_up)))
+            self.runner_up = runner_up
+        rshape = (len(lf), 2, H, W) if batched else (2, H, W)
+        lrun = torch.empty(rshape, dtype=torch.float32, device=self.device) if runner_up else None
+        rrun = torch.empty(rshape, dtype=torch.float32, device=self.device) if runner_up and rmap is not None else None
         self._check(L.psm_wait_stream(ctx, stream))
         for b in range(len(lf)):
             lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
@@ -190,8 +204,12 @@ class TorchStereo:
                 lc = lcost[b] if batched else lcost
                 rc = None if rcost is None else (rcost[b] if batched else rcost)
                 self._check(L.psm_copy_costs_device(ctx, lc.data_ptr(), None if rc is None else rc.data_ptr(), W * 4))
+            if runner_up:
+                lu = lrun[b] if batched else lrun
+                ru = None if rrun is None else (rrun[b] if batched else rrun)
+                self._check(L.psm_copy_runner_up_device(ctx, lu.data_ptr(), None if ru is None else ru.data_ptr(), W * 4))
         self._check(L.psm_signal_stream(ctx, stream))
-        return (lmap, rmap, lcost, rcost) if costs else (lmap, rmap)
+        return (lmap, rmap) + ((lcost, rcost) if costs else ()) + ((lrun, rrun) if runner_up else ())
 
     # -- measurement helpers ------------------------------------------------------------------
     def stage_ms(self, stage):
