@@ -232,6 +232,32 @@ int psm_create_blocked(psm_ctx** out, int width, int height, int max_disp,
 int psm_create_multi(psm_ctx** out, int width, int height, int max_disp,
                      const int* devices, int n_devices, int block_slices, int map_bits);
 
+/* Range context: solves the problem over disparities [min_disp, max_disp), 0 <= min_disp < max_disp, and holds its
+ * n = max_disp - min_disp slices (or blocks of them), so memory and time follow n rather than max_disp.  A rig that never
+ * sees anything beyond a known depth (a bin, a conveyor, a wall) has no disparity below some minimum; this is OpenCV's
+ * minDisparity of StereoBM / StereoSGBM.
+ *   - What it creates: n_devices == 1 with block_slices == 0 an unblocked context on devices[0], with block_slices > 0 a
+ *     blocked one (psm_create_blocked) holding min(block_slices, n) slices; n_devices >= 2 a multi-device context
+ *     (psm_create_multi) whose shards split [min_disp, max_disp) as psm_create_multi splits [0, max_disp).  min_disp = 0
+ *     gives exactly the context psm_create_u16 (psm_create_sharded for 8-bit maps) / psm_create_blocked /
+ *     psm_create_multi give over [0, max_disp).
+ *   - PSM_EINVAL before any CUDA call: W or H below 1, min_disp < 0, max_disp < 2, min_disp >= max_disp, map_bits other
+ *     than 8 (max_disp <= 256) or 16 (max_disp <= 4096), n_devices outside 1..min(8, n), block_slices < 0, a null
+ *     `devices` or a negative device id.  Then the device and peer-access errors of psm_create_multi.
+ *   - Slices: slice d of the range is built and filtered exactly as on a [0, max_disp) context, in every filter path; its
+ *     raw and filtered costs are bit-identical to that context's slice d.
+ *   - Selection: the candidates are d in [max(1, min_disp), max_disp) in the arg-min's order (strict <, lowest d on ties,
+ *     NaN and +inf never win).  Maps hold the absolute disparity; 0 still means "no winner".
+ *   - PSM_OPT_COSTS: entry k is q(m + k - 1), the quiet NaN 0x7FC00000 for an index outside [min_disp, max_disp).
+ *     PSM_OPT_RUNNER_UP: the first candidate with |d - m| >= 2, 0 with a NaN cost when there is none.  Both are allowed.
+ *   - The left-right check and the post-filter work on the absolute maps unchanged; the post-filter's value range is
+ *     max_disp.
+ *   - psm_read_cost_slice / psm_write_cost_slice / psm_read_ab_slice take a global d in the range (PSM_EINVAL outside
+ *     it); on an unblocked context psm_device_ptr selectors 0 / 1 hold slice d at offset d - min_disp.
+ * Every other call behaves as on the context of the same kind over [0, max_disp).  See DESIGN.md section 22. */
+int psm_create_range(psm_ctx** out, int width, int height, int min_disp, int max_disp,
+                     const int* devices, int n_devices, int block_slices, int map_bits);
+
 /* Waits for the context's work on the stream it is bound to (psm_set_stream), on its own stream and on its copy stream,
  * then frees everything: a caller's stream bound with psm_set_stream must still exist when this is called. */
 int psm_destroy(psm_ctx* ctx);

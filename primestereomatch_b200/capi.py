@@ -24,6 +24,7 @@ SYMBOLS = [
     "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
     "psm_create_blocked", "psm_create_multi", "psm_set_images_device_planes", "psm_wait_stream", "psm_signal_stream",
     "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs", "psm_copy_runner_up_device", "psm_read_runner_up",
+    "psm_create_range",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -65,6 +66,7 @@ def lib():
     L.psm_create_u16.argtypes = [C.POINTER(vp), i, i, i, i, i, i]
     L.psm_create_blocked.argtypes = [C.POINTER(vp), i, i, i, i, i, i, i, i]
     L.psm_create_multi.argtypes = [C.POINTER(vp), i, i, i, C.POINTER(C.c_int), i, i, i]
+    L.psm_create_range.argtypes = [C.POINTER(vp), i, i, i, i, C.POINTER(C.c_int), i, i, i]
     L.psm_disp_select_u16.argtypes = [vp, vp, sz, vp, sz]
     L.psm_disp_select_u16_async.argtypes = [vp, vp, sz, vp, sz]
     L.psm_disp_reduce_keys_u16.argtypes = [vp, vp, vp, i, vp, sz, vp, sz]

@@ -36,6 +36,11 @@ thread_local char g_create_error[512] = "";  // per host thread: psm_last_error(
 
 struct psm_ctx {
     int W = 0, H = 0, Wp = 0, D = 0, d_begin = 0, d_count = 0, device = 0;
+    // The problem's range is [d_lo, D): 0 on every context but those of psm_create_range (and their shards).  The context
+    // owns [d_begin, d_begin + d_count) of it.
+    int d_lo = 0;
+    // the context owns the whole problem range: selection, PSM_OPT_COSTS and PSM_OPT_RUNNER_UP need no other context
+    bool owns_problem() const { return d_begin == d_lo && d_count == D - d_lo; }
     size_t plane = 0;  // H * Wp
     cudaStream_t own_stream = nullptr, stream = nullptr;
     float* guide[2] = {nullptr, nullptr};   // kGuidePlanes planes per view
@@ -130,7 +135,7 @@ struct psm_ctx {
     float* track[2] = {nullptr, nullptr};
     bool have_costs = false;
     // kCostFirst only where a neighbour shard below reads it
-    int track_planes() const { return d_begin > 0 ? kCostFirst + 1 : kCostLast + 1; }
+    int track_planes() const { return d_begin > d_lo ? kCostFirst + 1 : kCostLast + 1; }
     // PSM_OPT_RUNNER_UP: 1 = the selection stages also write the runner-up into ru_out[view] (kRunnerUpOut planes; a
     // multi-device context's first shard reduces its shards' picks from ru_slots[view] into its own, the others have
     // neither), and a blocked walk keeps the running list in ru_list[view] (kListPlanes).  All are allocated when the
@@ -806,7 +811,7 @@ int launch_cost_write(psm_ctx* c, int v, const void* map, CostPlanes dst)
 {
     CostWriteParams P;
     P.map = map; P.vol = c->vol[v]; P.src = track_planes(c, v); P.dst = dst;
-    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.D = c->D; P.d_begin = c->d_begin; P.d_count = c->d_count;
+    P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.D = c->D; P.d_lo = c->d_lo; P.d_begin = c->d_begin; P.d_count = c->d_count;
     dim3 blk(256), grd((c->W + 255) / 256, c->H);
     if (c->map_bytes == 2)
         (c->blk_slices ? cost_write_kernel<uint16_t, true> : cost_write_kernel<uint16_t, false>)<<<grd, blk, 0, c->stream>>>(P);
@@ -1138,14 +1143,14 @@ int psm_cvf_plan(int width, int height, int d_count, int sm_count, int no_pack, 
 
 // geometry already validated by the caller; map_bytes 1 (u8 maps) or 2 (u16 maps)
 static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_begin, int d_count, int device, int map_bytes,
-                      int block_slices = 0)
+                      int block_slices = 0, int d_lo = 0)
 {
     int ndev = psm_device_count();
     if (device < 0 || device >= ndev) return fail(nullptr, PSM_ECUDA, "CUDA device %d not available (%d devices)", device, ndev);
     psm_ctx* c = new (std::nothrow) psm_ctx();
     if (!c) return fail(nullptr, PSM_ENOMEM, "out of host memory");
     c->W = width; c->H = height; c->Wp = pitch_for_width(width); c->D = max_disp;
-    c->d_begin = d_begin; c->d_count = d_count; c->device = device;
+    c->d_begin = d_begin; c->d_count = d_count; c->device = device; c->d_lo = d_lo;
     c->plane = (size_t)c->H * c->Wp;
     c->map_bytes = map_bytes;
     c->blk_slices = block_slices;
@@ -1257,23 +1262,13 @@ int psm_create(psm_ctx** out, int width, int height, int max_disp, int device)
     return psm_create_sharded(out, width, height, max_disp, 0, max_disp, device);
 }
 
-int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const int* devices, int n_devices, int block_slices,
-                     int map_bits)
+}  // extern "C"
+
+// The multi-device context over the problem range [d_lo, max_disp), its arguments checked up to the devices' existence:
+// shard k owns the k-th part of sharding.py's shard_range split of the range.
+static int create_multi(psm_ctx** out, int width, int height, int d_lo, int max_disp, const int* devices, int n_devices,
+                        int block_slices, int map_bits)
 {
-    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
-    *out = nullptr;
-    if (map_bits != 8 && map_bits != 16) return fail(nullptr, PSM_EINVAL, "map_bits must be 8 or 16 (got %d)", map_bits);
-    const int dmax = map_bits == 8 ? MapFormat<uint8_t>::kMaxDisp : MapFormat<uint16_t>::kMaxDisp;
-    if (width < 1 || height < 1 || max_disp < 2 || max_disp > dmax)
-        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d with %d-bit maps)", width, height,
-                    max_disp, dmax, map_bits);
-    if (n_devices < 1 || n_devices > kMaxRanks || n_devices > max_disp)
-        return fail(nullptr, PSM_EINVAL, "n_devices %d outside 1..%d (at most %d shards, each owning at least one of the %d slices)",
-                    n_devices, std::min(kMaxRanks, max_disp), kMaxRanks, max_disp);
-    if (!devices) return fail(nullptr, PSM_EINVAL, "devices is null");
-    if (block_slices < 0) return fail(nullptr, PSM_EINVAL, "block_slices %d is negative (0 = unblocked shards)", block_slices);
-    for (int k = 0; k < n_devices; ++k)
-        if (devices[k] < 0) return fail(nullptr, PSM_EINVAL, "devices[%d] = %d is negative", k, devices[k]);
     const int ndev = psm_device_count();
     for (int k = 0; k < n_devices; ++k)
         if (devices[k] >= ndev)
@@ -1295,7 +1290,7 @@ int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const i
     psm_ctx* c = new (std::nothrow) psm_ctx();
     if (!c) return fail(nullptr, PSM_ENOMEM, "out of host memory");
     c->W = width; c->H = height; c->Wp = pitch_for_width(width); c->D = max_disp;
-    c->d_begin = 0; c->d_count = max_disp; c->device = devices[0];
+    c->d_begin = d_lo; c->d_count = max_disp - d_lo; c->d_lo = d_lo; c->device = devices[0];
     c->map_bytes = map_bits / 8;
     auto bail = [&](int code) {
         snprintf(g_create_error, sizeof(g_create_error), "%s", c->err);
@@ -1303,11 +1298,11 @@ int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const i
         return code;
     };
     // the split of sharding.py's shard_range: contiguous slices, the last shard takes the remainder
-    const int base = max_disp / n_devices;
+    const int base = c->d_count / n_devices;
     for (int k = 0; k < n_devices; ++k) {
-        const int d_begin = k * base, d_count = k < n_devices - 1 ? base : max_disp - d_begin;
+        const int d_begin = d_lo + k * base, d_count = k < n_devices - 1 ? base : max_disp - d_begin;
         if (int rc = create_ctx(&c->shard[k], width, height, max_disp, d_begin, d_count, devices[k], c->map_bytes,
-                                block_slices ? std::min(block_slices, d_count) : 0)) {
+                                block_slices ? std::min(block_slices, d_count) : 0, d_lo)) {
             snprintf(c->err, sizeof(c->err), "shard %d (device %d): %.400s", k, devices[k], g_create_error);
             return bail(rc);
         }
@@ -1340,6 +1335,58 @@ int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const i
     for (int v = 0; v < 2; ++v) c->dis[v] = p2p_layout(c, n_devices).maps(static_cast<unsigned char*>(blocks[0]), v);
     *out = c;
     return PSM_OK;
+}
+
+extern "C" {
+
+int psm_create_multi(psm_ctx** out, int width, int height, int max_disp, const int* devices, int n_devices, int block_slices,
+                     int map_bits)
+{
+    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
+    *out = nullptr;
+    if (map_bits != 8 && map_bits != 16) return fail(nullptr, PSM_EINVAL, "map_bits must be 8 or 16 (got %d)", map_bits);
+    const int dmax = map_bits == 8 ? MapFormat<uint8_t>::kMaxDisp : MapFormat<uint16_t>::kMaxDisp;
+    if (width < 1 || height < 1 || max_disp < 2 || max_disp > dmax)
+        return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d D=%d (need W,H>=1, 2<=D<=%d with %d-bit maps)", width, height,
+                    max_disp, dmax, map_bits);
+    if (n_devices < 1 || n_devices > kMaxRanks || n_devices > max_disp)
+        return fail(nullptr, PSM_EINVAL, "n_devices %d outside 1..%d (at most %d shards, each owning at least one of the %d slices)",
+                    n_devices, std::min(kMaxRanks, max_disp), kMaxRanks, max_disp);
+    if (!devices) return fail(nullptr, PSM_EINVAL, "devices is null");
+    if (block_slices < 0) return fail(nullptr, PSM_EINVAL, "block_slices %d is negative (0 = unblocked shards)", block_slices);
+    for (int k = 0; k < n_devices; ++k)
+        if (devices[k] < 0) return fail(nullptr, PSM_EINVAL, "devices[%d] = %d is negative", k, devices[k]);
+    return create_multi(out, width, height, 0, max_disp, devices, n_devices, block_slices, map_bits);
+}
+
+int psm_create_range(psm_ctx** out, int width, int height, int min_disp, int max_disp, const int* devices, int n_devices,
+                     int block_slices, int map_bits)
+{
+    if (!out) return fail(nullptr, PSM_EINVAL, "out is null");
+    *out = nullptr;
+    if (width < 1 || height < 1) return fail(nullptr, PSM_EINVAL, "bad geometry W=%d H=%d (need W,H>=1)", width, height);
+    if (min_disp < 0) return fail(nullptr, PSM_EINVAL, "min_disp %d is negative", min_disp);
+    if (max_disp < 2) return fail(nullptr, PSM_EINVAL, "max_disp %d is below 2", max_disp);
+    if (min_disp >= max_disp)
+        return fail(nullptr, PSM_EINVAL, "min_disp %d is not below max_disp %d: the range [min_disp, max_disp) is empty",
+                    min_disp, max_disp);
+    if (map_bits != 8 && map_bits != 16) return fail(nullptr, PSM_EINVAL, "map_bits must be 8 or 16 (got %d)", map_bits);
+    const int dmax = map_bits == 8 ? MapFormat<uint8_t>::kMaxDisp : MapFormat<uint16_t>::kMaxDisp;
+    if (max_disp > dmax)
+        return fail(nullptr, PSM_EINVAL, "max_disp %d above %d: %d-bit maps hold disparities up to %d", max_disp, dmax,
+                    map_bits, dmax - 1);
+    const int n = max_disp - min_disp;
+    if (n_devices < 1 || n_devices > kMaxRanks || n_devices > n)
+        return fail(nullptr, PSM_EINVAL, "n_devices %d outside 1..%d (at most %d shards, each owning at least one of the %d "
+                    "slices)", n_devices, std::min(kMaxRanks, n), kMaxRanks, n);
+    if (block_slices < 0) return fail(nullptr, PSM_EINVAL, "block_slices %d is negative (0 = unblocked)", block_slices);
+    if (!devices) return fail(nullptr, PSM_EINVAL, "devices is null");
+    for (int k = 0; k < n_devices; ++k)
+        if (devices[k] < 0) return fail(nullptr, PSM_EINVAL, "devices[%d] = %d is negative", k, devices[k]);
+    if (n_devices == 1)
+        return create_ctx(out, width, height, max_disp, min_disp, n, devices[0], map_bits / 8, std::min(block_slices, n),
+                          min_disp);
+    return create_multi(out, width, height, min_disp, max_disp, devices, n_devices, block_slices, map_bits);
 }
 
 int psm_destroy(psm_ctx* c)
@@ -1520,19 +1567,20 @@ int psm_set_option(psm_ctx* c, int key, int value)
         return PSM_OK;
     case PSM_OPT_COSTS:
         if (int rc = check_costs_value(c, value)) return rc;
-        if (value && (c->d_begin != 0 || c->d_count != c->D))
+        if (value && !c->owns_problem())
             return fail(c, PSM_EINVAL, "PSM_OPT_COSTS on a context that owns slices [%d,%d) of %d: the costs beside a winner "
                         "may lie on another context; use a context over the whole range (psm_create, psm_create_u16 / "
-                        "psm_create_blocked over [0, max_disp), or psm_create_multi)", c->d_begin, c->d_begin + c->d_count, c->D);
+                        "psm_create_blocked over [0, max_disp), psm_create_multi or psm_create_range)", c->d_begin,
+                        c->d_begin + c->d_count, c->D);
         if (int rc = value ? alloc_costs(c, true) : PSM_OK) return rc;
         apply_costs(c, value);
         return PSM_OK;
     case PSM_OPT_RUNNER_UP:
         if (int rc = check_runner_up_value(c, value)) return rc;
-        if (value && (c->d_begin != 0 || c->d_count != c->D))
+        if (value && !c->owns_problem())
             return fail(c, PSM_EINVAL, "PSM_OPT_RUNNER_UP on a context that owns slices [%d,%d) of %d: the runner-up and "
                         "the winner may lie on different contexts; use a context over the whole range (psm_create, "
-                        "psm_create_u16 / psm_create_blocked over [0, max_disp), or psm_create_multi)", c->d_begin,
+                        "psm_create_u16 / psm_create_blocked over [0, max_disp), psm_create_multi or psm_create_range)", c->d_begin,
                         c->d_begin + c->d_count, c->D);
         if (int rc = value ? alloc_runner_up(c, true, 0) : PSM_OK) return rc;
         apply_runner_up(c, value);
@@ -1842,7 +1890,7 @@ int psm_disp_select_device(psm_ctx* c)
 {
     if (is_multi(c)) return multi_select(c);
     if (int rc = bind(c)) return rc;
-    if (c->d_begin != 0 || c->d_count != c->D)
+    if (!c->owns_problem())
         return fail(c, PSM_ESTATE, "psm_disp_select on a sharded context: use psm_disp_select_keys + psm_disp_reduce_keys");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
@@ -2521,7 +2569,7 @@ static int route_slice(psm_ctx* c, int d, F f)
 {
     for (int k = 0; k < c->nshards; ++k)
         if (d >= c->shard[k]->d_begin && d < c->shard[k]->d_begin + c->shard[k]->d_count) return relay(c, k, f(c->shard[k]));
-    return fail(c, PSM_EINVAL, "slice %d outside [0,%d)", d, c->D);
+    return fail(c, PSM_EINVAL, "slice %d outside [%d,%d)", d, c->d_lo, c->D);
 }
 
 extern "C" {

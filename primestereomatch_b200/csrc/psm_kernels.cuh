@@ -646,14 +646,14 @@ __global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
 
 // ------------------------------------------------------------------------------------------
 // The filtered costs beside each winner (PSM_OPT_COSTS): q(m - 1), q(m), q(m + 1) of the volume selection scanned, at the
-// selection map's m, copied bit for bit.  An index outside [0, D) gives kCostNaN; a pixel without a winner (m = 0) gets
-// (kCostNaN, q(0), q(1)).
+// selection map's m, copied bit for bit.  An index outside the problem's range [d_lo, D) gives kCostNaN; a pixel without a
+// winner (m = 0) gets (kCostNaN, q(0), q(1)) where d_lo = 0, and kCostNaN for each index below d_lo otherwise.
 // ------------------------------------------------------------------------------------------
 // Planes of H * W floats (row pitch W), per view.  The result: kCostOut planes holding q(m - 1), q(m), q(m + 1); the
 // selection stages write them and nothing else does, so they stay the last selection's until the next one.  A blocked
 // context's tracking planes, which its walk rewrites block by block: planes 0..2 hold the running winner's costs, then
-// kCostLast the cost at the last slice of the block walked last and, on a shard that owns no slice 0, kCostFirst the cost
-// at its first owned slice (read by the shard below it at their seam).
+// kCostLast the cost at the last slice of the block walked last and, on a shard that does not own the problem's first
+// slice d_lo, kCostFirst the cost at its first owned slice (read by the shard below it at their seam).
 constexpr int kCostOut = 3, kCostLast = 3, kCostFirst = 4;
 constexpr unsigned kCostNaNBits = 0x7fc00000u;   // the canonical quiet NaN of an index outside [0, D)
 
@@ -775,15 +775,16 @@ __global__ void __launch_bounds__(256) wta_fold_costs_kernel(const FoldCostParam
 
 // The costs of the entries a context owns, from the complete selection map (T) into dst, which may be a peer's planes.
 // Entry k of pixel i is q(d), d = m + k - 1.  Its one writer: the owner of slice d, [d_begin, d_begin + d_count), for d
-// in [0, D), and the owner of m (kCostNaN) otherwise.  kTracked = false reads q(d) from the resident volume (an
-// unblocked context); kTracked = true from the tracking planes of a blocked one: planes 0..2 for its own winners, and
-// at its seams kCostFirst (m just below its range) or kCostLast (m just above).
+// in the problem's range [d_lo, D), and otherwise (kCostNaN) the owner of m, or of d_lo where m lies below the range (the
+// no-winner map 0 of a range starting above 0).  kTracked = false reads q(d) from the resident volume (an unblocked
+// context); kTracked = true from the tracking planes of a blocked one: planes 0..2 for its own winners, and at its seams
+// kCostFirst (m just below its range) or kCostLast (m just above).
 struct CostWriteParams {
     const void* map;      // [H][W] of T
     const float* vol;     // kTracked = false: the filtered volume of slices [d_begin, d_begin + d_count), [d][H][Wp]
     CostPlanes src;       // kTracked = true: the tracking planes
     CostPlanes dst;
-    int W, H, Wp, D, d_begin, d_count;
+    int W, H, Wp, D, d_lo, d_begin, d_count;
 };
 
 template <typename T, bool kTracked>
@@ -793,20 +794,21 @@ __global__ void __launch_bounds__(256) cost_write_kernel(const CostWriteParams P
     if (x >= P.W) return;
     const size_t i = (size_t)y * P.W + x;
     const int m = static_cast<const T*>(P.map)[i];
+    const int mo = m < P.d_lo ? P.d_lo : m;   // the slice whose owner holds m's state: its planes 0..2 on a blocked one
     const auto owned = [&](int d) { return d >= P.d_begin && d < P.d_begin + P.d_count; };
 #pragma unroll
     for (int k = 0; k < kCostOut; ++k) {
         const int d = m + k - 1;
         float q;
-        if (d < 0 || d >= P.D) {
-            if (!owned(m)) continue;
+        if (d < P.d_lo || d >= P.D) {
+            if (!owned(mo)) continue;
             q = __uint_as_float(kCostNaNBits);
         } else if (!owned(d)) {
             continue;
         } else if (!kTracked) {
             q = P.vol[(size_t)(d - P.d_begin) * P.H * P.Wp + (size_t)y * P.Wp + x];
         } else {
-            q = P.src.plane(owned(m) ? k : (k == 2 ? kCostFirst : kCostLast))[i];
+            q = P.src.plane(owned(mo) ? k : (k == 2 ? kCostFirst : kCostLast))[i];
         }
         P.dst.plane(k)[i] = q;
     }

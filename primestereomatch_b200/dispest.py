@@ -36,14 +36,23 @@ def resolve_map_bits(max_disp, map_bits):
 
 
 def create_context(width, height, max_disp, map_bits, *, device=0, d_begin=0, d_count=None, block_slices=None,
-                   devices=None):
+                   devices=None, min_disp=0):
     """The context DispEst and TorchStereo run on, as a c_void_p handle (psm_destroy frees it): a multi-device context
     over `devices` (psm_create_multi, block_slices blocks every shard), a blocked context (psm_create_blocked), or one of
-    [d_begin, d_begin + d_count) on `device` with map_bits-bit maps (psm_create_u16 / psm_create_sharded)."""
+    [d_begin, d_begin + d_count) on `device` with map_bits-bit maps (psm_create_u16 / psm_create_sharded).  min_disp > 0:
+    a range context over [min_disp, max_disp) of the same kind (psm_create_range); it is not a shard, so d_begin /
+    d_count raise ValueError with it."""
     L = capi.lib()
     ctx = C.c_void_p()
     dc = max_disp - d_begin if d_count is None else d_count
-    if devices is not None:
+    if min_disp:
+        if d_begin != 0 or d_count is not None:
+            raise ValueError("min_disp (a range context over [min_disp, max_disp)) excludes d_begin / d_count")
+        devs = [int(device)] if devices is None else [int(x) for x in devices]
+        arr = (C.c_int * max(1, len(devs)))(*devs)
+        capi.check(L.psm_create_range(C.byref(ctx), width, height, int(min_disp), max_disp, arr, len(devs),
+                                      int(block_slices or 0), map_bits))
+    elif devices is not None:
         devs = [int(x) for x in devices]
         arr = (C.c_int * max(1, len(devs)))(*devs)
         capi.check(L.psm_create_multi(C.byref(ctx), width, height, max_disp, arr, len(devs), int(block_slices or 0),
@@ -71,10 +80,13 @@ class DispEst:
     devices : None (one device, `device`) or a list of CUDA device ids: a multi-device context (psm_create_multi) whose
     shard k runs on devices[k] and owns the k-th contiguous part of [0, d); ids may repeat.  The maps equal a
     single-device context's.  Not combinable with d_begin / d_count; block_slices blocks every shard.
+    min_disp : 0 (default) or the first disparity of a range context over [min_disp, d) (psm_create_range), of the kind
+    the other arguments select: it holds d - min_disp slices, its maps hold absolute disparities and its costs and
+    runner-up are NaN / 0 outside the range.  Not combinable with d_begin / d_count (ValueError).
     """
 
     def __init__(self, l, r, d, t=MAX_CPU_THREADS, ocl=True, device=0, d_begin=0, d_count=None, map_bits=None,
-                 block_slices=None, devices=None):
+                 block_slices=None, devices=None, min_disp=0):
         l, r = np.asarray(l), np.asarray(r)
         if l.dtype != r.dtype or l.shape != r.shape:
             # reference: "DE: Error - Left & Right images are of different types." then exit(1)
@@ -99,13 +111,18 @@ class DispEst:
         self.lRunnerUp = self.rRunnerUp = None   # setRunnerUpOutput(True): DispSelect_GPU's (2, H, W) float32 runner-up
         if devices is not None and (d_begin != 0 or d_count is not None):
             raise ValueError("devices (a multi-device context over the whole range) excludes d_begin / d_count")
+        if min_disp and (d_begin != 0 or d_count is not None):
+            raise ValueError("min_disp (a range context over [min_disp, max_disp)) excludes d_begin / d_count")
+        self.min_disp = int(min_disp)
         self._lImg, self._rImg = l, r
         self._ctx = C.c_void_p()
         self._lib = None
         if self.useOCL:
             self._lib = capi.lib()
             self._ctx = create_context(self.wid, self.hei, self.maxDis, self.map_bits, device=device, d_begin=d_begin,
-                                       d_count=d_count, block_slices=block_slices, devices=devices)
+                                       d_count=d_count, block_slices=block_slices, devices=devices, min_disp=min_disp)
+        if self.min_disp:
+            d_begin = self.min_disp
         self.d_begin, self.d_count = d_begin, (self.maxDis - d_begin if d_count is None else d_count)
         self.block_slices = None if devices is not None and not block_slices else block_slices   # 0: unblocked shards
         self.devices = None if devices is None else list(devices)

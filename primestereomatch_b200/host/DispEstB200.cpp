@@ -6,7 +6,7 @@
 
 // reference src/DispEst.cpp:10-143: type check (exit(1) on mismatch), output maps, and -- instead of
 // the OpenCL context / queue / 12 cl_mem buffers / three run-time compiled programs -- one psm_ctx.
-DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices, std::vector<int> devices)
+DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices, std::vector<int> devices, int min_disp)
     : lImg(l), rImg(r), maxDis(d), threads(t), useOCL(ocl)
 {
     hei = lImg.rows;
@@ -23,7 +23,11 @@ DispEst::DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_s
     rValid = cv::Mat::zeros(hei, wid, CV_8UC1);
     if (useOCL) {
         const int dev = devices.empty() ? 0 : devices[0];
-        const int rc = devices.size() >= 2
+        if (devices.empty()) devices.push_back(dev);
+        const int rc = min_disp > 0
+                           ? psm_create_range(&ctx, wid, hei, min_disp, maxDis, devices.data(), (int)devices.size(),
+                                              block_slices > 0 ? block_slices : 0, wide ? 16 : 8)
+                     : devices.size() >= 2
                            ? psm_create_multi(&ctx, wid, hei, maxDis, devices.data(), (int)devices.size(), block_slices > 0 ? block_slices : 0,
                                               wide ? 16 : 8)
                      : block_slices > 0 ? psm_create_blocked(&ctx, wid, hei, maxDis, 0, maxDis, block_slices, wide ? 16 : 8, dev)

@@ -78,8 +78,10 @@ public:
     // reference src/DispEst.cpp:10-143.  `ocl` == use the GPU path.  block_slices > 0: a blocked context
     // (psm_create_blocked) that holds that many disparity slices at a time, for ranges the device cannot hold whole.
     // devices: empty = device 0; one id = that device; two or more = a multi-device context (psm_create_multi) whose
-    // shard k runs on devices[k] (ids may repeat), each shard blocked by block_slices when it is > 0.
-    DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices = 0, std::vector<int> devices = {});
+    // shard k runs on devices[k] (ids may repeat), each shard blocked by block_slices when it is > 0.  min_disp > 0: the
+    // same kind of context over disparities [min_disp, d) alone (psm_create_range); the maps hold absolute disparities.
+    DispEst(cv::Mat l, cv::Mat r, const int d, int t, bool ocl, int block_slices = 0, std::vector<int> devices = {},
+            int min_disp = 0);
     ~DispEst(void);
 
     cv::Mat lDisMap;  // CV_8UC1, raw disparity index (reference DispEst.h:28-29); CV_16UC1 when maxDis > 256 (psm_create_u16),

@@ -9,7 +9,8 @@
 // mode (0 off, 1 check + fill + post-filter, 2 check + fill) to setLRCheck (default 0).  D up to 4096: above 256 the
 // maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.  A leading
 // `--block-slices N` runs a blocked context (psm_create_blocked) that holds N disparity slices at a time, a leading
-// `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat).  A leading
+// `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat), a leading
+// `--min-disp N` a context over disparities [N, D) alone (psm_create_range; the maps hold absolute disparities).  A leading
 // `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.
 #include <cstdio>
 #include <cstdlib>
@@ -29,7 +30,7 @@ static bool read_all(const char* path, void* dst, size_t n)
 
 int main(int argc, char** argv)
 {
-    int block_slices = 0;
+    int block_slices = 0, min_disp = 0;
     std::vector<int> devices;
     const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
     if (left_only) {
@@ -37,9 +38,12 @@ int main(int argc, char** argv)
         ++argv;
         --argc;
     }
-    while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices"))) {
+    while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices") ||
+                         !std::strcmp(argv[1], "--min-disp"))) {
         if (!std::strcmp(argv[1], "--block-slices")) {
             block_slices = std::atoi(argv[2]);
+        } else if (!std::strcmp(argv[1], "--min-disp")) {
+            min_disp = std::atoi(argv[2]);
         } else {
             for (const char* p = argv[2]; *p;) {
                 char* end = nullptr;
@@ -53,7 +57,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -61,7 +65,7 @@ int main(int argc, char** argv)
     if (b200devicepoll() == 0) { std::fprintf(stderr, "no CUDA device\n"); return 3; }
     cv::Mat l(H, W, CV_32FC3), r(H, W, CV_32FC3);
     if (!read_all(argv[4], l.data, l.step * H) || !read_all(argv[5], r.data, r.step * H)) { std::fprintf(stderr, "bad input\n"); return 2; }
-    DispEst* SMDE = new DispEst(l, r, D, MAX_CPU_THREADS, true, block_slices, devices);
+    DispEst* SMDE = new DispEst(l, r, D, MAX_CPU_THREADS, true, block_slices, devices, min_disp);
     SMDE->setInputImages(l, r);
     SMDE->setThreads(MAX_CPU_THREADS);
     SMDE->setSubsampleRate(4);

@@ -12,13 +12,14 @@ import ctypes as C
 from . import capi
 
 
-def shard_range(max_disp, world, rank):
-    """Contiguous slices [d_begin, d_begin + d_count) of rank `rank`; the last rank takes the remainder.
-    Every rank owns at least one slice (world <= max_disp)."""
-    if not (0 <= rank < world) or world > max_disp:
-        raise ValueError(f"bad shard request rank={rank} world={world} D={max_disp}")
-    base = max_disp // world
-    d_begin = rank * base
+def shard_range(max_disp, world, rank, min_disp=0):
+    """Contiguous slices [d_begin, d_begin + d_count) of rank `rank` in [min_disp, max_disp); the last rank takes the
+    remainder.  Every rank owns at least one slice (world <= max_disp - min_disp)."""
+    n = max_disp - min_disp
+    if not (0 <= rank < world) or not (0 <= min_disp < max_disp) or world > n:
+        raise ValueError(f"bad shard request rank={rank} world={world} range=[{min_disp},{max_disp})")
+    base = n // world
+    d_begin = min_disp + rank * base
     d_count = base if rank < world - 1 else max_disp - d_begin
     return d_begin, d_count
 

@@ -59,15 +59,17 @@ def frame_layout(t, height, width, channels="bgr"):
 
 
 class TorchStereo:
-    """TorchStereo(width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None)
+    """TorchStereo(width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None, min_disp=0)
 
     The context `DispEst` creates for the same arguments: `device` (an index, "cuda:k" or torch.device; None = the
     current device), `map_bits` (None: 8-bit maps up to max_disp 256, 16-bit above), `block_slices` (a blocked context),
-    `devices` (a multi-device context whose frames and maps live on devices[0]).  The setters pass their values straight
-    to the C-ABI, which rejects bad ones with PsmError."""
+    `devices` (a multi-device context whose frames and maps live on devices[0]), `min_disp` (a range context over
+    [min_disp, max_disp), psm_create_range).  The setters pass their values straight to the C-ABI, which rejects bad ones
+    with PsmError."""
 
-    def __init__(self, width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None):
+    def __init__(self, width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None, min_disp=0):
         self.width, self.height, self.max_disp = int(width), int(height), int(max_disp)
+        self.min_disp = int(min_disp)
         self.map_bits = resolve_map_bits(self.max_disp, map_bits)
         if devices is not None:
             index = int(devices[0]) if len(devices) else 0
@@ -82,7 +84,7 @@ class TorchStereo:
         self._lib = capi.lib()
         self._ctx = C.c_void_p()
         self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
-                                   block_slices=block_slices, devices=devices)
+                                   block_slices=block_slices, devices=devices, min_disp=self.min_disp)
 
     # -- lifetime ---------------------------------------------------------------------------
     def close(self):
@@ -150,7 +152,7 @@ class TorchStereo:
 
         costs=True -> (lmap, rmap, lcosts, rcosts): also the filtered costs beside each winner of the selection maps
         (PSM_OPT_COSTS, psm_copy_costs_device), new float32 tensors (3, H, W) or (B, 3, H, W) whose plane k holds the cost
-        at disparity m + k - 1, bit for bit (the quiet NaN 0x7FC00000 outside [0, max_disp)); rcosts is None on a
+        at disparity m + k - 1, bit for bit (the quiet NaN 0x7FC00000 outside [min_disp, max_disp)); rcosts is None on a
         left-only context.  The option is set when costs differs from the last call's, which restarts the frame.
 
         runner_up=True -> also (lrunner, rrunner), appended after any costs: each pixel's runner-up away from the winner
