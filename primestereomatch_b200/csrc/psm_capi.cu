@@ -32,6 +32,20 @@ constexpr int kNumStages = 6;  // ingest, cvc, cvf, wta, cvf-filter-kernel, post
 
 thread_local char g_create_error[512] = "";  // per host thread: psm_last_error(NULL) reports the calling thread's last failed creation
 
+// The per-pixel outputs a selection stage writes beside the maps when their option is on, and the facts every host path
+// of an output reads from here: its option, the noun of its messages and its result planes per view.
+enum SelOut { kOutCosts, kOutRunnerUp, kNumOuts };
+struct SelOutInfo {
+    int key;
+    const char* option;
+    const char* noun;
+    int planes;
+};
+constexpr SelOutInfo kSelOut[kNumOuts] = {
+    {PSM_OPT_COSTS, "PSM_OPT_COSTS", "costs", kCostOut},
+    {PSM_OPT_RUNNER_UP, "PSM_OPT_RUNNER_UP", "runner-up", kRunnerUpOut},
+};
+
 }  // namespace
 
 struct psm_ctx {
@@ -118,33 +132,30 @@ struct psm_ctx {
     cudaEvent_t ev_reduced[kMaxRanks] = {};    // shard k's reduce of the last frame (on its stream)
     bool reduced_valid = false;
     cudaEvent_t ev_copied[kMaxRanks] = {};     // shard k (k >= 1) has read the frame it receives from the first shard
-    cudaEvent_t ev_gathered[kMaxRanks] = {};   // PSM_OPT_COSTS: shard k's cost entries of the current frame (on its stream)
-    cudaEvent_t ev_picked[kMaxRanks] = {};     // PSM_OPT_RUNNER_UP: shard k's runner-up pick of the current frame (on its stream)
+    cudaEvent_t ev_written[kMaxRanks] = {};    // shard k's writes of the enabled outputs of the current frame (on its stream)
     cudaEvent_t ev_images = nullptr;           // psm_set_images_device: the caller's images as the first shard's stream sees them
     // PSM_OPT_VIEWS: 2 (both views) or 1 (the left view alone: the right view's guide, volume, selection and post-filter
     // are skipped).  stages_reset: PSM_OPT_VIEWS, PSM_OPT_COSTS or PSM_OPT_RUNNER_UP changed since the last psm_cost_const,
     // so the volumes, maps, masks, costs and runner-up are stale.
     int views = 2;
     bool stages_reset = false;
-    // PSM_OPT_COSTS: 1 = the selection stages also write the filtered costs beside each winner into win_cost[view]
-    // (kCostOut planes; a multi-device context's shards write the first shard's, the others have none), and a blocked
-    // walk tracks them in track[view] (track_planes()).  Both are allocated when the option is turned on.
-    // have_costs: the last selection stage since the last reset wrote them.
-    int costs = 0;
-    float* win_cost[2] = {nullptr, nullptr};
+    // One per output (kSelOut): on = 1 while the selection stages also write it into planes[view] (its result planes; a
+    // multi-device context's shards write the first shard's, the others have none), allocated when the option is turned
+    // on.  have: the last selection stage since the last reset wrote them.
+    struct OutState {
+        int on = 0;
+        bool have = false;
+        float* planes[2] = {nullptr, nullptr};
+    } outs[kNumOuts];
+    bool outs_on() const { return std::any_of(outs, outs + kNumOuts, [](const OutState& o) { return o.on; }); }
+    // PSM_OPT_COSTS: a blocked walk tracks the costs in track[view] (track_planes(); kCostFirst only where a neighbour
+    // shard below reads it)
     float* track[2] = {nullptr, nullptr};
-    bool have_costs = false;
-    // kCostFirst only where a neighbour shard below reads it
     int track_planes() const { return d_begin > d_lo ? kCostFirst + 1 : kCostLast + 1; }
-    // PSM_OPT_RUNNER_UP: 1 = the selection stages also write the runner-up into ru_out[view] (kRunnerUpOut planes; a
-    // multi-device context's first shard reduces its shards' picks from ru_slots[view] into its own, the others have
-    // neither), and a blocked walk keeps the running list in ru_list[view] (kListPlanes).  All are allocated when the
-    // option is turned on.  have_runner_up: the last selection stage since the last reset wrote ru_out.
-    int runner_up = 0;
-    float* ru_out[2] = {nullptr, nullptr};
+    // PSM_OPT_RUNNER_UP: a blocked walk keeps the running list in ru_list[view] (kListPlanes), and a multi-device
+    // context's first shard reduces its shards' picks from ru_slots[view]
     float* ru_list[2] = {nullptr, nullptr};
     unsigned char* ru_slots[2] = {nullptr, nullptr};
-    bool have_runner_up = false;
     unsigned p2p_seq_right = 0;                // frames whose exchange included the right view (p2p_seq counts every frame)
     bool p2p_right_current = false;            // the last frame's exchange included the right view
     bool have_pp = false;                      // dis_pp holds the maps of a post-process since the last PSM_OPT_VIEWS change
@@ -775,12 +786,10 @@ int launch_cvc(psm_ctx* c)
     return PSM_OK;
 }
 
-// the result planes and the tracking planes of view v (PSM_OPT_COSTS)
-CostPlanes cost_planes(const psm_ctx* c, int v) { return {c->win_cost[v], (size_t)c->W * c->H}; }
+// of view v: the result planes of output o, the costs' tracking planes, the runner-up's running list and (on the first
+// shard of a multi-device context of nslots shards) its slots
+CostPlanes out_planes(const psm_ctx* c, int o, int v) { return {c->outs[o].planes[v], (size_t)c->W * c->H}; }
 CostPlanes track_planes(const psm_ctx* c, int v) { return {c->track[v], (size_t)c->W * c->H}; }
-// the result planes, the running list and (on the first shard of a multi-device context of nslots shards) the slots of
-// view v (PSM_OPT_RUNNER_UP)
-CostPlanes runner_up_planes(const psm_ctx* c, int v) { return {c->ru_out[v], (size_t)c->W * c->H}; }
 CostPlanes list_planes(const psm_ctx* c, int v) { return {c->ru_list[v], (size_t)c->W * c->H}; }
 RunnerUpSlots runner_up_slots(const psm_ctx* c, int v, int nslots) { return {c->ru_slots[v], (size_t)c->W * c->H, nslots}; }
 
@@ -792,11 +801,11 @@ int launch_fold(psm_ctx* c, bool first)
     for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->res.begin; P.d_count = c->res.count; P.first = first ? 1 : 0;
     dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, c->views);
-    if (c->runner_up)
-        (c->costs ? wta_fold_list_kernel<true> : wta_fold_list_kernel<false>)<<<grd, blk, 0, c->stream>>>(
+    if (c->outs[kOutRunnerUp].on)
+        (c->outs[kOutCosts].on ? wta_fold_list_kernel<true> : wta_fold_list_kernel<false>)<<<grd, blk, 0, c->stream>>>(
             FoldListParams{P, {list_planes(c, 0), list_planes(c, 1)}, {track_planes(c, 0), track_planes(c, 1)},
                            c->track_planes() > kCostFirst});
-    else if (c->costs)
+    else if (c->outs[kOutCosts].on)
         wta_fold_costs_kernel<<<grd, blk, 0, c->stream>>>(
             FoldCostParams{P, {track_planes(c, 0), track_planes(c, 1)}, c->track_planes() > kCostFirst});
     else
@@ -827,8 +836,8 @@ int launch_cost_write(psm_ctx* c, int v, const void* map, CostPlanes dst)
 int launch_runner_up_write(psm_ctx* c, int v, const void* map, RunnerUpSlots slots, int slot)
 {
     RunnerUpWriteParams P;
-    P.map = map; P.vol = c->vol[v]; P.keys = c->run_keys[v]; P.list = list_planes(c, v); P.dst = runner_up_planes(c, v);
-    P.slots = slots; P.slot = slot;
+    P.map = map; P.vol = c->vol[v]; P.keys = c->run_keys[v]; P.list = list_planes(c, v);
+    P.dst = out_planes(c, kOutRunnerUp, v); P.slots = slots; P.slot = slot;
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->d_begin; P.d_count = c->d_count;
     dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
     if (c->map_bytes == 2)
@@ -837,6 +846,16 @@ int launch_runner_up_write(psm_ctx* c, int v, const void* map, RunnerUpSlots slo
         (c->blk_slices ? runner_up_write_kernel<uint8_t, true> : runner_up_write_kernel<uint8_t, false>)<<<grd, blk, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
+}
+
+// Output o of view v once `map` (its complete selection map) is written: context c's writer of the entries it owns.  On a
+// single-device context (n = 0) into its own result planes; on shard k of a multi-device context of n shards into the
+// first shard s0's result planes (the costs) or into its slot there (the runner-up, which s0 then reduces).
+int launch_out_write(psm_ctx* c, int o, int v, const void* map, psm_ctx* s0, int k, int n)
+{
+    if (o == kOutCosts) return launch_cost_write(c, v, map, out_planes(s0, kOutCosts, v));
+    if (!n && !c->blk_slices) return PSM_OK;   // an unblocked context's selection kernel wrote it beside the map
+    return launch_runner_up_write(c, v, map, n ? runner_up_slots(s0, v, n) : RunnerUpSlots{}, k);
 }
 
 // The slices the volumes hold while the context's stages work from global slice `b` on: up to vol_slices() of the owned
@@ -894,8 +913,7 @@ void selection_ran(psm_ctx* c, bool own)
 {
     c->lr_masks_ok = false;
     c->have_maps = c->have_maps || own;
-    c->have_costs = false;
-    c->have_runner_up = false;
+    for (psm_ctx::OutState& o : c->outs) o.have = false;
 }
 
 // a map call for maps of type T, named u8_call / u16_call in its two formats, on a context of the other format:
@@ -1324,8 +1342,7 @@ static int create_multi(psm_ctx** out, int width, int height, int d_lo, int max_
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_scattered[k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_reduced[k], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied[k], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_gathered[k], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_picked[k], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_written[k], cudaEventDisableTiming);
         if (e == cudaSuccess && k == 0) e = cudaEventCreateWithFlags(&c->ev_images, cudaEventDisableTiming);
         if (e != cudaSuccess) { fail(c, PSM_ECUDA, "event creation on device %d failed: %s", devices[k], cudaGetErrorString(e)); return bail(PSM_ECUDA); }
     }
@@ -1405,8 +1422,7 @@ int psm_destroy(psm_ctx* c)
             if (c->ev_scattered[k]) cudaEventDestroy(c->ev_scattered[k]);
             if (c->ev_reduced[k]) cudaEventDestroy(c->ev_reduced[k]);
             if (c->ev_copied[k]) cudaEventDestroy(c->ev_copied[k]);
-            if (c->ev_gathered[k]) cudaEventDestroy(c->ev_gathered[k]);
-            if (c->ev_picked[k]) cudaEventDestroy(c->ev_picked[k]);
+            if (c->ev_written[k]) cudaEventDestroy(c->ev_written[k]);
             if (k == 0 && c->ev_images) cudaEventDestroy(c->ev_images);
             psm_destroy(c->shard[k]);
         }
@@ -1437,8 +1453,9 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->guide_flags);
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
-    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]); cudaFree(c->win_cost[v]);
-                                   cudaFree(c->track[v]); cudaFree(c->ru_out[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]); }
+    for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]);
+                                   cudaFree(c->track[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]);
+                                   for (psm_ctx::OutState& o : c->outs) cudaFree(o.planes[v]); }
     for (int s = 0; s < kNumStages; ++s) {
         if (c->ev0[s]) cudaEventDestroy(c->ev0[s]);
         if (c->ev1[s]) cudaEventDestroy(c->ev1[s]);
@@ -1463,67 +1480,50 @@ static void reset_stages(psm_ctx* c)
     c->have_maps = false;
     c->have_pp = false;
     c->lr_masks_ok = false;
-    c->have_costs = false;
-    c->have_runner_up = false;
+    for (psm_ctx::OutState& o : c->outs) o.have = false;
 }
 
-// PSM_OPT_COSTS = 1 on one context, a multi-device context's shards included: the planes it reads or writes, the result
-// planes where `result` (a single-device context, the first shard) and the tracking planes on a blocked context.  Only
-// allocates: a failure leaves the setting as it was.
-static int alloc_costs(psm_ctx* c, bool result)
+// the output whose option is `key`, or -1
+static int out_of_key(int key)
 {
-    if (int rc = bind(c)) return rc;
-    const size_t plane = (size_t)c->W * c->H * sizeof(float);
-    for (int v = 0; v < 2; ++v) {
-        if (result) PSM_CUDA(c, alloc_if_null(c->win_cost[v], kCostOut * plane));
-        if (c->blk_slices) PSM_CUDA(c, alloc_if_null(c->track[v], c->track_planes() * plane));
-    }
-    return PSM_OK;
+    for (int o = 0; o < kNumOuts; ++o)
+        if (kSelOut[o].key == key) return o;
+    return -1;
 }
 
-// PSM_OPT_COSTS = value, its planes allocated: a blocked context's walk tracks the costs, so a change restarts the frame
-static void apply_costs(psm_ctx* c, int value)
-{
-    if (value != c->costs) {
-        reset_stages(c);
-        c->costs = value;
-    }
-}
-
-static int check_costs_value(psm_ctx* c, int value)
-{
-    if (value != 0 && value != 1) return fail(c, PSM_EINVAL, "PSM_OPT_COSTS must be 0 or 1 (got %d)", value);
-    return PSM_OK;
-}
-
-// PSM_OPT_RUNNER_UP = 1 on one context, a multi-device context's shards included: the planes it reads or writes, the
-// result planes where `result` (a single-device context, the first shard), the slots of `nslots` shards (the first shard
-// of a multi-device context) and the running lists on a blocked context.  Only allocates: a failure leaves the setting
-// as it was.
-static int alloc_runner_up(psm_ctx* c, bool result, int nslots)
+// output o = 1 on one context, a multi-device context's shards included: the planes it reads or writes.  The result
+// planes where `result` (a single-device context, the first shard), then the output's own scratch: the costs' tracking
+// planes on a blocked context; the runner-up's running lists on a blocked context and the slots of `nslots` shards (the
+// first shard of a multi-device context).  Only allocates: a failure leaves the setting as it was.
+static int alloc_out(psm_ctx* c, int o, bool result, int nslots)
 {
     if (int rc = bind(c)) return rc;
     const size_t npix = (size_t)c->W * c->H, plane = npix * sizeof(float);
     for (int v = 0; v < 2; ++v) {
-        if (result) PSM_CUDA(c, alloc_if_null(c->ru_out[v], kRunnerUpOut * plane));
-        if (nslots) PSM_CUDA(c, alloc_if_null(c->ru_slots[v], RunnerUpSlots::bytes(npix, nslots)));
-        if (c->blk_slices) PSM_CUDA(c, alloc_if_null(c->ru_list[v], kListPlanes * plane));
+        if (result) PSM_CUDA(c, alloc_if_null(c->outs[o].planes[v], kSelOut[o].planes * plane));
+        if (o == kOutCosts) {
+            if (c->blk_slices) PSM_CUDA(c, alloc_if_null(c->track[v], c->track_planes() * plane));
+        } else {
+            if (nslots) PSM_CUDA(c, alloc_if_null(c->ru_slots[v], RunnerUpSlots::bytes(npix, nslots)));
+            if (c->blk_slices) PSM_CUDA(c, alloc_if_null(c->ru_list[v], kListPlanes * plane));
+        }
     }
     return PSM_OK;
 }
 
-// PSM_OPT_RUNNER_UP = value, its planes allocated: a blocked context's walk keeps the lists, so a change restarts the frame
-static void apply_runner_up(psm_ctx* c, int value)
+// output o = value, its planes allocated: a blocked context's walk keeps the output's running state, so a change
+// restarts the frame
+static void apply_out(psm_ctx* c, int o, int value)
 {
-    if (value != c->runner_up) {
+    if (value != c->outs[o].on) {
         reset_stages(c);
-        c->runner_up = value;
+        c->outs[o].on = value;
     }
 }
 
-static int check_runner_up_value(psm_ctx* c, int value)
+static int check_out_value(psm_ctx* c, int o, int value)
 {
-    if (value != 0 && value != 1) return fail(c, PSM_EINVAL, "PSM_OPT_RUNNER_UP must be 0 or 1 (got %d)", value);
+    if (value != 0 && value != 1) return fail(c, PSM_EINVAL, "%s must be 0 or 1 (got %d)", kSelOut[o].option, value);
     return PSM_OK;
 }
 
@@ -1532,28 +1532,33 @@ extern "C" {
 int psm_set_option(psm_ctx* c, int key, int value)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    const int o = out_of_key(key);
     if (c->nshards) {
         if (key == PSM_OPT_P2P_SYNC)
             return reject_multi(c, "PSM_OPT_P2P_SYNC", "its shards' exchange is ordered by events, never by flags");
-        if (key == PSM_OPT_COSTS) {   // the shards own part of the range, the context as a whole spans [0, D)
-            if (int rc = check_costs_value(c, value)) return rc;
-            // every shard's planes first, then the setting on all of them: a failed allocation changes no shard's setting
+        if (o >= 0) {   // the shards own part of the range, the context as a whole spans it
+            if (int rc = check_out_value(c, o, value)) return rc;
+            // every shard's planes first (the first shard's hold the results and every shard's slot), then the setting
+            // on all of them: a failed allocation changes no shard's setting
             for (int k = 0; value && k < c->nshards; ++k)
-                if (int rc = alloc_costs(c->shard[k], k == 0)) return relay(c, k, rc);
-            for (int k = 0; k < c->nshards; ++k) apply_costs(c->shard[k], value);
-            c->costs = value;
-            return PSM_OK;
-        }
-        if (key == PSM_OPT_RUNNER_UP) {   // as PSM_OPT_COSTS; the first shard also holds every shard's slot
-            if (int rc = check_runner_up_value(c, value)) return rc;
-            for (int k = 0; value && k < c->nshards; ++k)
-                if (int rc = alloc_runner_up(c->shard[k], k == 0, k == 0 ? c->nshards : 0)) return relay(c, k, rc);
-            for (int k = 0; k < c->nshards; ++k) apply_runner_up(c->shard[k], value);
-            c->runner_up = value;
+                if (int rc = alloc_out(c->shard[k], o, k == 0, k == 0 ? c->nshards : 0)) return relay(c, k, rc);
+            for (int k = 0; k < c->nshards; ++k) apply_out(c->shard[k], o, value);
+            c->outs[o].on = value;
             return PSM_OK;
         }
         if (int rc = forward(c, [&](psm_ctx* s) { return psm_set_option(s, key, value); })) return rc;
         if (key == PSM_OPT_VIEWS) c->views = value;   // the map calls check the right-view arguments on the context itself
+        return PSM_OK;
+    }
+    if (o >= 0) {
+        if (int rc = check_out_value(c, o, value)) return rc;
+        if (value && !c->owns_problem())
+            return fail(c, PSM_EINVAL, "%s on a context that owns slices [%d,%d) of %d: the %s may depend on slices "
+                        "another context owns; use a context over the whole range (psm_create, psm_create_u16 / "
+                        "psm_create_blocked over [0, max_disp), psm_create_multi or psm_create_range)", kSelOut[o].option,
+                        c->d_begin, c->d_begin + c->d_count, c->D, kSelOut[o].noun);
+        if (int rc = value ? alloc_out(c, o, true, 0) : PSM_OK) return rc;
+        apply_out(c, o, value);
         return PSM_OK;
     }
     switch (key) {
@@ -1564,26 +1569,6 @@ int psm_set_option(psm_ctx* c, int key, int value)
             c->views = value;
             reset_stages(c);
         }
-        return PSM_OK;
-    case PSM_OPT_COSTS:
-        if (int rc = check_costs_value(c, value)) return rc;
-        if (value && !c->owns_problem())
-            return fail(c, PSM_EINVAL, "PSM_OPT_COSTS on a context that owns slices [%d,%d) of %d: the costs beside a winner "
-                        "may lie on another context; use a context over the whole range (psm_create, psm_create_u16 / "
-                        "psm_create_blocked over [0, max_disp), psm_create_multi or psm_create_range)", c->d_begin,
-                        c->d_begin + c->d_count, c->D);
-        if (int rc = value ? alloc_costs(c, true) : PSM_OK) return rc;
-        apply_costs(c, value);
-        return PSM_OK;
-    case PSM_OPT_RUNNER_UP:
-        if (int rc = check_runner_up_value(c, value)) return rc;
-        if (value && !c->owns_problem())
-            return fail(c, PSM_EINVAL, "PSM_OPT_RUNNER_UP on a context that owns slices [%d,%d) of %d: the runner-up and "
-                        "the winner may lie on different contexts; use a context over the whole range (psm_create, "
-                        "psm_create_u16 / psm_create_blocked over [0, max_disp), psm_create_multi or psm_create_range)", c->d_begin,
-                        c->d_begin + c->d_count, c->D);
-        if (int rc = value ? alloc_runner_up(c, true, 0) : PSM_OK) return rc;
-        apply_runner_up(c, value);
         return PSM_OK;
     case PSM_OPT_CVF_MODE:
         if (value != PSM_CVF_EXACT && value != PSM_CVF_MIXED && value != PSM_CVF_NAIVE)
@@ -1834,9 +1819,9 @@ static int select_maps(psm_ctx* c)
     }
     for (int v = 0; v < c->views; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        if (c->runner_up)   // the map and the runner-up in one read of the volume
+        if (c->outs[kOutRunnerUp].on)   // the map and the runner-up in one read of the volume
             wta_runner_up_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
-                                                                reinterpret_cast<T*>(c->dis[v]), runner_up_planes(c, v));
+                                                                reinterpret_cast<T*>(c->dis[v]), out_planes(c, kOutRunnerUp, v));
         else
             wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
                                                       reinterpret_cast<T*>(c->dis[v]), nullptr);
@@ -1896,15 +1881,11 @@ int psm_disp_select_device(psm_ctx* c)
     if (int rc = stage_begin(c, 3)) return rc;
     if (int rc = c->map_bytes == 2 ? select_maps<uint16_t>(c) : select_maps<uint8_t>(c)) return rc;
     selection_ran(c, true);
-    if (c->costs) {   // from the volume, or from a blocked context's tracking planes, which its next walk rewrites
+    for (int o = 0; o < kNumOuts; ++o) {
+        if (!c->outs[o].on) continue;
         for (int v = 0; v < c->views; ++v)
-            if (int rc = launch_cost_write(c, v, c->dis[v], cost_planes(c, v))) return rc;
-        c->have_costs = true;
-    }
-    if (c->runner_up) {   // select_maps wrote it on an unblocked context; a blocked one picks it from its running lists
-        for (int v = 0; c->blk_slices && v < c->views; ++v)
-            if (int rc = launch_runner_up_write(c, v, c->dis[v], RunnerUpSlots{}, 0)) return rc;
-        c->have_runner_up = true;
+            if (int rc = launch_out_write(c, o, v, c->dis[v], c, 0, 0)) return rc;
+        c->outs[o].have = true;
     }
     return stage_end(c, 3);
 }
@@ -1937,8 +1918,7 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
     if (!d_keys_left || (c->views == 2 && !d_keys_right)) return fail(c, PSM_EINVAL, "null key buffer");
     if (!c->filtered) return fail(c, PSM_ESTATE, "psm_disp_select_keys before psm_cost_filter");
     if (int rc = stage_begin(c, 3)) return rc;
-    c->have_costs = false;   // keys carry no costs beside the winner, and no runner-up
-    c->have_runner_up = false;
+    for (psm_ctx::OutState& o : c->outs) o.have = false;   // keys carry no output beside the winner
     uint64_t* keys[2] = {d_keys_left, d_keys_right};
     if (c->blk_slices) {   // the running keys are this context's minima already
         for (int v = 0; v < c->views; ++v)
@@ -2135,31 +2115,22 @@ static int p2p_wait_done(psm_ctx* c)
 //   4. every reduce writes the first shard's maps, which what the first shard enqueued before this select (a previous
 //      post-filter, an asynchronous D2H) may still read: the wait of 2 on the first shard's scatter, queued behind
 //      that work, covers it.
-// With PSM_OPT_COSTS, every shard then writes the cost entries it owns into the first shard's cost planes:
-//   5. shard k's gather reads its copy of the complete maps, which every shard's reduce writes: it waits for them;
-//   6. the first shard's stream, which carries every reader of the costs (psm_copy_costs_device, psm_read_costs), waits
-//      for every gather;
-//   7. the gathers overwrite cost planes that a copy-out of the previous frame on the first shard's stream may still
-//      read: each gather follows its shard's reduce, which waits for the first shard's scatter (2), queued behind that
-//      copy-out;
-//   8. a gather reads its shard's map, which the next frame's reduces overwrite: they wait for that shard's next
-//      scatter (2), queued behind the gather; and the volumes or tracking planes it reads are rewritten only by later
-//      stages on its own stream.
-// The first shard's result planes are written by these gathers alone, never by a filter stage (its tracking planes are
-// separate), so they hold frame f's costs until the next select, as on a single-device context.
-// With PSM_OPT_RUNNER_UP, every shard then writes its pick into its own slot on the first shard, and the first shard
-// reduces the slots into its result planes:
-//   9. shard k's pick reads its copy of the complete maps, which every shard's reduce writes: it waits for them;
-//  10. the first shard's slot reduce reads every shard's slot: it waits for every pick.  Its stream carries every reader
-//      of the result planes (psm_copy_runner_up_device, psm_read_runner_up), queued behind the reduce;
-//  11. the picks overwrite slots that the first shard's slot reduce of frame f - 1 read: each pick follows its shard's
-//      reduce, which waits for the first shard's scatter (2), queued behind that slot reduce;
-//  12. a pick reads its shard's map, which the next frame's reduces overwrite: they wait for that shard's next scatter
-//      (2), queued behind the pick; and the volume or running lists it reads are rewritten only by later stages on its
-//      own stream.
-// Every slot has one writer and the reduce takes the first slot of the lowest key, so the result does not depend on the
-// order in which the picks land.  The result planes are written by the slot reduce alone, so they hold frame f's
-// runner-up until the next select.
+// With outputs on (kSelOut), every shard then writes, per enabled output, what it owns into the first shard: the cost
+// entries into its cost planes, its runner-up pick into its own slot, which the first shard then reduces into its
+// runner-up planes:
+//   5. shard k's writes read its copy of the complete maps, which every shard's reduce writes: they wait for them;
+//   6. the first shard's stream waits for every shard's writes.  It carries the slot reduce and every reader of the
+//      result planes (psm_copy_*_device, psm_read_*), queued behind them;
+//   7. the writes overwrite cost planes and slots that a copy-out or the slot reduce of frame f - 1 on the first shard's
+//      stream may still read: each shard's writes follow its reduce, which waits for the first shard's scatter (2),
+//      queued behind that work;
+//   8. a shard's writes read its map, which the next frame's reduces overwrite: they wait for that shard's next scatter
+//      (2), queued behind the writes; and the volumes, tracking planes or running lists they read are rewritten only by
+//      later stages on its own stream.
+// Every cost entry and every slot has one writer, and the slot reduce takes the first slot of the lowest key, so the
+// result does not depend on the order in which the writes land.  The first shard's result planes are written by these
+// writes and the slot reduce alone, never by a filter stage (its tracking planes and running lists are separate), so they
+// hold frame f's outputs until the next select, as on a single-device context.
 // No kernel waits for another queued behind it, so shards on one device are as safe as shards on several.
 static int multi_select(psm_ctx* c)
 {
@@ -2187,47 +2158,29 @@ static int multi_select(psm_ctx* c)
     }
     c->reduced_valid = true;
     psm_ctx* s0 = c->shard[0];
-    if (c->costs) {
-        for (int k = 0; k < n; ++k) {
-            psm_ctx* s = c->shard[k];
-            if (int rc = bind(s)) return relay(c, k, rc);
-            for (int j = 0; j < n; ++j)
-                if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_reduced[j], 0));   // 5
-            const P2pLayout L = p2p_layout(s, s->p2p_nranks);
-            for (int v = 0; v < s->views; ++v)   // peer stores between distinct devices
-                if (int rc = launch_cost_write(s, v, L.maps(s->p2p_own, v), cost_planes(s0, v))) return relay(c, k, rc);
-            PSM_CUDA(c, cudaEventRecord(c->ev_gathered[k], s->stream));
-        }
-    }
-    if (c->runner_up) {
-        for (int k = 0; k < n; ++k) {
-            psm_ctx* s = c->shard[k];
-            if (int rc = bind(s)) return relay(c, k, rc);
-            for (int j = 0; j < n; ++j)
-                if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_reduced[j], 0));   // 9
-            const P2pLayout L = p2p_layout(s, s->p2p_nranks);
-            for (int v = 0; v < s->views; ++v)   // peer stores between distinct devices
-                if (int rc = launch_runner_up_write(s, v, L.maps(s->p2p_own, v), runner_up_slots(s0, v, n), k))
-                    return relay(c, k, rc);
-            PSM_CUDA(c, cudaEventRecord(c->ev_picked[k], s->stream));
-        }
+    for (int k = 0; c->outs_on() && k < n; ++k) {
+        psm_ctx* s = c->shard[k];
+        if (int rc = bind(s)) return relay(c, k, rc);
+        for (int j = 0; j < n; ++j)
+            if (j != k) PSM_CUDA(c, cudaStreamWaitEvent(s->stream, c->ev_reduced[j], 0));   // 5
+        const P2pLayout L = p2p_layout(s, s->p2p_nranks);
+        for (int o = 0; o < kNumOuts; ++o)
+            for (int v = 0; c->outs[o].on && v < s->views; ++v)   // peer stores between distinct devices
+                if (int rc = launch_out_write(s, o, v, L.maps(s->p2p_own, v), s0, k, n)) return relay(c, k, rc);
+        PSM_CUDA(c, cudaEventRecord(c->ev_written[k], s->stream));
     }
     if (int rc = bind(s0)) return relay(c, 0, rc);
     for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_reduced[j], 0));   // 3
-    if (c->costs) {
-        for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_gathered[j], 0));   // 6
-        s0->have_costs = true;
-    }
-    if (c->runner_up) {
-        for (int j = 1; j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_picked[j], 0));   // 10
+    for (int j = 1; c->outs_on() && j < n; ++j) PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_written[j], 0));   // 6
+    if (c->outs[kOutRunnerUp].on) {
         const size_t npix = (size_t)s0->W * s0->H;
         for (int v = 0; v < s0->views; ++v) {
             runner_up_reduce_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, s0->stream>>>(runner_up_slots(s0, v, n),
-                                                                                           runner_up_planes(s0, v));
+                                                                                           out_planes(s0, kOutRunnerUp, v));
             PSM_LAUNCH_CHECK(s0);
         }
-        s0->have_runner_up = true;
     }
+    for (int o = 0; o < kNumOuts; ++o) s0->outs[o].have = c->outs[o].on;   // its reduce cleared them (selection_ran)
     return relay(c, 0, stage_end(s0, 3));
 }
 
@@ -2444,13 +2397,24 @@ int psm_copy_maps_device(psm_ctx* c, int which, void* d_left, size_t left_step, 
     return copy_maps_out(c, maps, d_left, left_step, d_right, right_step, cudaMemcpyDefault, false);
 }
 
-// the costs of the last selection stage for psm_copy_costs_device and psm_read_costs
-static int check_costs_ready(psm_ctx* c, const char* call)
+// output o of the last selection stage, for its copy-out call `call`
+static int check_out_ready(psm_ctx* c, int o, const char* call)
 {
     if (int rc = check_stages_reset(c, call)) return rc;
-    if (!c->have_costs)
-        return fail(c, PSM_ESTATE, "%s: no costs; the last selection stage since the context was created or the last "
-                    "PSM_OPT_VIEWS / PSM_OPT_COSTS change did not write them (psm_disp_select* with PSM_OPT_COSTS = 1)", call);
+    if (!c->outs[o].have)
+        return fail(c, PSM_ESTATE, "%s: no %s; the last selection stage since the context was created or the last "
+                    "PSM_OPT_VIEWS / PSM_OPT_COSTS / PSM_OPT_RUNNER_UP change did not write the %s (psm_disp_select* with "
+                    "%s = 1)", call, kSelOut[o].noun, kSelOut[o].noun, kSelOut[o].option);
+    return PSM_OK;
+}
+
+// the destination of a copy-out call of output o: `given` (its pointers are set) and rows of at least W floats
+static int check_out_dst(psm_ctx* c, int o, const char* call, bool given, size_t row_step)
+{
+    const size_t row = (size_t)c->W * sizeof(float);
+    if (!given || row_step < row)
+        return fail(c, PSM_EINVAL, "%s: bad %s plane pointer/step (row_step must be at least %zu bytes)", call,
+                    kSelOut[o].noun, row);
     return PSM_OK;
 }
 
@@ -2463,91 +2427,58 @@ static int copy_planes_out(psm_ctx* c, const float* src, int nplanes, float* dst
     return PSM_OK;
 }
 
-// view v's kCostOut planes -> dst
-static int copy_costs_out(psm_ctx* c, int v, float* dst, size_t row_step, cudaMemcpyKind kind)
+// psm_copy_*_device: both views' result planes of output o -> device memory, asynchronously
+static int copy_out_device(psm_ctx* c, int o, const char* call, float* d_left, float* d_right, size_t row_step)
 {
-    return copy_planes_out(c, c->win_cost[v], kCostOut, dst, row_step, kind);
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (int rc = check_right_arg(c, d_right, call)) return rc;
+    if (int rc = check_out_dst(c, o, call, d_left && (c->views == 1 || d_right), row_step)) return rc;
+    // a multi-device context's outputs are the first shard's
+    if (is_multi(c)) return relay(c, 0, copy_out_device(c->shard[0], o, call, d_left, d_right, row_step));
+    if (int rc = bind(c)) return rc;
+    if (int rc = check_out_ready(c, o, call)) return rc;
+    float* dst[2] = {d_left, d_right};
+    for (int v = 0; v < c->views; ++v)
+        if (int rc = copy_planes_out(c, c->outs[o].planes[v], kSelOut[o].planes, dst[v], row_step, cudaMemcpyDefault))
+            return rc;
+    return PSM_OK;
+}
+
+// psm_read_*: one view's result planes of output o -> host memory, then waits for the copy
+static int read_out(psm_ctx* c, int o, const char* call, int view, float* dst, size_t row_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
+    if (int rc = check_out_dst(c, o, call, dst, row_step)) return rc;
+    if (is_multi(c)) return relay(c, 0, read_out(c->shard[0], o, call, view, dst, row_step));
+    if (int rc = bind(c)) return rc;
+    if (view == PSM_RIGHT)
+        if (int rc = check_right_view(c, call)) return rc;
+    if (int rc = check_out_ready(c, o, call)) return rc;
+    if (int rc = copy_planes_out(c, c->outs[o].planes[view], kSelOut[o].planes, dst, row_step, cudaMemcpyDeviceToHost))
+        return rc;
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
 }
 
 int psm_copy_costs_device(psm_ctx* c, float* d_left, float* d_right, size_t row_step)
 {
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (int rc = check_right_arg(c, d_right, "psm_copy_costs_device")) return rc;
-    const size_t row = (size_t)c->W * sizeof(float);
-    if (!d_left || (c->views == 2 && !d_right) || row_step < row)
-        return fail(c, PSM_EINVAL, "psm_copy_costs_device: bad cost plane pointer/step (row_step must be at least %zu bytes)", row);
-    // a multi-device context's costs are the first shard's
-    if (is_multi(c)) return relay(c, 0, psm_copy_costs_device(c->shard[0], d_left, d_right, row_step));
-    if (int rc = bind(c)) return rc;
-    if (int rc = check_costs_ready(c, "psm_copy_costs_device")) return rc;
-    float* dst[2] = {d_left, d_right};
-    for (int v = 0; v < c->views; ++v)
-        if (int rc = copy_costs_out(c, v, dst[v], row_step, cudaMemcpyDefault)) return rc;
-    return PSM_OK;
+    return copy_out_device(c, kOutCosts, "psm_copy_costs_device", d_left, d_right, row_step);
 }
 
 int psm_read_costs(psm_ctx* c, int view, float* dst, size_t row_step)
 {
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
-    const size_t row = (size_t)c->W * sizeof(float);
-    if (!dst || row_step < row)
-        return fail(c, PSM_EINVAL, "psm_read_costs: bad cost plane pointer/step (row_step must be at least %zu bytes)", row);
-    if (is_multi(c)) return relay(c, 0, psm_read_costs(c->shard[0], view, dst, row_step));
-    if (int rc = bind(c)) return rc;
-    if (view == PSM_RIGHT)
-        if (int rc = check_right_view(c, "psm_read_costs")) return rc;
-    if (int rc = check_costs_ready(c, "psm_read_costs")) return rc;
-    if (int rc = copy_costs_out(c, view, dst, row_step, cudaMemcpyDeviceToHost)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
-}
-
-// the runner-up of the last selection stage for psm_copy_runner_up_device and psm_read_runner_up
-static int check_runner_up_ready(psm_ctx* c, const char* call)
-{
-    if (int rc = check_stages_reset(c, call)) return rc;
-    if (!c->have_runner_up)
-        return fail(c, PSM_ESTATE, "%s: no runner-up; the last selection stage since the context was created or the last "
-                    "PSM_OPT_VIEWS / PSM_OPT_COSTS / PSM_OPT_RUNNER_UP change did not write it (psm_disp_select* with "
-                    "PSM_OPT_RUNNER_UP = 1)", call);
-    return PSM_OK;
+    return read_out(c, kOutCosts, "psm_read_costs", view, dst, row_step);
 }
 
 int psm_copy_runner_up_device(psm_ctx* c, float* d_left, float* d_right, size_t row_step)
 {
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (int rc = check_right_arg(c, d_right, "psm_copy_runner_up_device")) return rc;
-    const size_t row = (size_t)c->W * sizeof(float);
-    if (!d_left || (c->views == 2 && !d_right) || row_step < row)
-        return fail(c, PSM_EINVAL, "psm_copy_runner_up_device: bad runner-up plane pointer/step (row_step must be at "
-                    "least %zu bytes)", row);
-    // a multi-device context's runner-up is the first shard's
-    if (is_multi(c)) return relay(c, 0, psm_copy_runner_up_device(c->shard[0], d_left, d_right, row_step));
-    if (int rc = bind(c)) return rc;
-    if (int rc = check_runner_up_ready(c, "psm_copy_runner_up_device")) return rc;
-    float* dst[2] = {d_left, d_right};
-    for (int v = 0; v < c->views; ++v)
-        if (int rc = copy_planes_out(c, c->ru_out[v], kRunnerUpOut, dst[v], row_step, cudaMemcpyDefault)) return rc;
-    return PSM_OK;
+    return copy_out_device(c, kOutRunnerUp, "psm_copy_runner_up_device", d_left, d_right, row_step);
 }
 
 int psm_read_runner_up(psm_ctx* c, int view, float* dst, size_t row_step)
 {
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
-    const size_t row = (size_t)c->W * sizeof(float);
-    if (!dst || row_step < row)
-        return fail(c, PSM_EINVAL, "psm_read_runner_up: bad runner-up plane pointer/step (row_step must be at least %zu "
-                    "bytes)", row);
-    if (is_multi(c)) return relay(c, 0, psm_read_runner_up(c->shard[0], view, dst, row_step));
-    if (int rc = bind(c)) return rc;
-    if (view == PSM_RIGHT)
-        if (int rc = check_right_view(c, "psm_read_runner_up")) return rc;
-    if (int rc = check_runner_up_ready(c, "psm_read_runner_up")) return rc;
-    if (int rc = copy_planes_out(c, c->ru_out[view], kRunnerUpOut, dst, row_step, cudaMemcpyDeviceToHost)) return rc;
-    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
-    return PSM_OK;
+    return read_out(c, kOutRunnerUp, "psm_read_runner_up", view, dst, row_step);
 }
 
 static int check_slice(psm_ctx* c, int view, int d)

@@ -225,18 +225,9 @@ class DispEst:
         0x7FC00000 where m + k - 1 lies outside [0, maxDis).  rCosts is None on left-only frames.  Changing it restarts
         the frame at CostConst_GPU.  Raises TypeError unless on is a bool, PsmError on a context that owns part of the
         disparity range (d_begin / d_count)."""
-        if not isinstance(on, bool):
-            raise TypeError(f"setCostOutput takes True or False (got {on!r})")
-        self._need_gpu()
-        capi.check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_COSTS, int(on)), self._ctx)
-        self.cost_output = on
+        self.cost_output = self._set_output("setCostOutput", capi.PSM_OPT_COSTS, on)
         self.lCosts = self.rCosts = None
         return 0
-
-    def _read_costs(self, view):
-        out = np.empty((3, self.hei, self.wid), np.float32)
-        capi.check(self._lib.psm_read_costs(self._ctx, view, _ptr(out), out.strides[1]), self._ctx)
-        return out
 
     def setRunnerUpOutput(self, on):
         """Whether DispSelect_GPU also fills lRunnerUp / rRunnerUp (PSM_OPT_RUNNER_UP): numpy float32 (2, H, W), plane 0
@@ -244,18 +235,26 @@ class DispEst:
         plane 1 its filtered cost bit for bit (the quiet NaN 0x7FC00000 where r = 0).  rRunnerUp is None on left-only
         frames.  Changing it restarts the frame at CostConst_GPU.  Raises TypeError unless on is a bool, PsmError on a
         context that owns part of the disparity range (d_begin / d_count)."""
-        if not isinstance(on, bool):
-            raise TypeError(f"setRunnerUpOutput takes True or False (got {on!r})")
-        self._need_gpu()
-        capi.check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_RUNNER_UP, int(on)), self._ctx)
-        self.runner_up_output = on
+        self.runner_up_output = self._set_output("setRunnerUpOutput", capi.PSM_OPT_RUNNER_UP, on)
         self.lRunnerUp = self.rRunnerUp = None
         return 0
 
-    def _read_runner_up(self, view):
-        out = np.empty((2, self.hei, self.wid), np.float32)
-        capi.check(self._lib.psm_read_runner_up(self._ctx, view, _ptr(out), out.strides[1]), self._ctx)
-        return out
+    def _set_output(self, name, key, on):
+        """the option `key` of a per-pixel output = on (a bool), through the setter `name` -> on"""
+        if not isinstance(on, bool):
+            raise TypeError(f"{name} takes True or False (got {on!r})")
+        self._need_gpu()
+        capi.check(self._lib.psm_set_option(self._ctx, key, int(on)), self._ctx)
+        return on
+
+    def _read_output(self, read, n):
+        """both views' n result planes of a per-pixel output (read: psm_read_costs or psm_read_runner_up) -> (left,
+        right), right None on left-only frames"""
+        out = [None, None]
+        for view in (capi.PSM_LEFT,) if self.rDisMap is None else (capi.PSM_LEFT, capi.PSM_RIGHT):
+            out[view] = np.empty((n, self.hei, self.wid), np.float32)
+            capi.check(read(self._ctx, view, _ptr(out[view]), out[view].strides[1]), self._ctx)
+        return tuple(out)
 
     @staticmethod
     def _map_arg(m):
@@ -301,11 +300,9 @@ class DispEst:
         sel = self._lib.psm_disp_select_u16 if self.map_bits == 16 else self._lib.psm_disp_select
         capi.check(sel(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
         if self.cost_output:
-            self.lCosts = self._read_costs(capi.PSM_LEFT)
-            self.rCosts = None if self.rDisMap is None else self._read_costs(capi.PSM_RIGHT)
+            self.lCosts, self.rCosts = self._read_output(self._lib.psm_read_costs, 3)
         if self.runner_up_output:
-            self.lRunnerUp = self._read_runner_up(capi.PSM_LEFT)
-            self.rRunnerUp = None if self.rDisMap is None else self._read_runner_up(capi.PSM_RIGHT)
+            self.lRunnerUp, self.rRunnerUp = self._read_output(self._lib.psm_read_runner_up, 2)
         return 0
 
     def PostProcess_GPU(self):

@@ -98,19 +98,16 @@ int DispEst::setViews(int v)
     return rc;
 }
 
-int DispEst::setCostOutput(bool on)
-{
-    if (!ctx) return -1;
-    const int rc = psm_set_option(ctx, PSM_OPT_COSTS, on ? 1 : 0);
-    if (rc == PSM_OK) cost_output = on;
-    return rc;
-}
+int DispEst::setCostOutput(bool on) { return set_output(PSM_OPT_COSTS, on, cost_output); }
 
-int DispEst::setRunnerUpOutput(bool on)
+int DispEst::setRunnerUpOutput(bool on) { return set_output(PSM_OPT_RUNNER_UP, on, runner_up_output); }
+
+// a per-pixel output's option `key` = on; `flag` (what DispSelect_GPU reads) follows it where the context accepts it
+int DispEst::set_output(int key, bool on, bool& flag)
 {
     if (!ctx) return -1;
-    const int rc = psm_set_option(ctx, PSM_OPT_RUNNER_UP, on ? 1 : 0);
-    if (rc == PSM_OK) runner_up_output = on;
+    const int rc = psm_set_option(ctx, key, on ? 1 : 0);
+    if (rc == PSM_OK) flag = on;
     return rc;
 }
 
@@ -125,9 +122,6 @@ int DispEst::read_planes(int view, int n, int (*read)(psm_ctx*, int, float*, siz
     }
     return 0;
 }
-
-// one view's three cost planes -> three CV_32FC1 matrices
-int DispEst::read_costs(int view, cv::Mat* planes) { return read_planes(view, 3, psm_read_costs, planes); }
 
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::printCV(void)
@@ -182,9 +176,9 @@ int DispEst::DispSelect_GPU()
         : psm_disp_select(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
     if (rc) return rc;
     if (cost_output) {
-        if (int e = read_costs(PSM_LEFT, lCosts)) return e;
+        if (int e = read_planes(PSM_LEFT, 3, psm_read_costs, lCosts)) return e;
         if (both)
-            if (int e = read_costs(PSM_RIGHT, rCosts)) return e;
+            if (int e = read_planes(PSM_RIGHT, 3, psm_read_costs, rCosts)) return e;
     }
     if (runner_up_output) {
         if (int e = read_planes(PSM_LEFT, 2, psm_read_runner_up, lRunnerUp)) return e;

@@ -155,7 +155,7 @@ private:
     int views = PSM_VIEWS_BOTH;
     bool cost_output = false;
     bool runner_up_output = false;
-    int read_costs(int view, cv::Mat* planes);
+    int set_output(int key, bool on, bool& flag);
     int read_planes(int view, int n, int (*read)(psm_ctx*, int, float*, size_t), cv::Mat* planes);
     psm_ctx* ctx = nullptr;
 };

@@ -16,6 +16,9 @@ from .dispest import DispEst, create_context, resolve_map_bits
 
 _PIX = {torch.uint8: capi.PSM_PIX_U8, torch.float32: capi.PSM_PIX_F32}
 _ORDER = {"bgr": (0, 1, 2), "rgb": (2, 1, 0)}   # the tensor channel that holds B, G and R
+# the per-pixel outputs of match, in their return order: argument (and attribute) name, option, planes, device copy-out
+_OUTPUTS = (("costs", capi.PSM_OPT_COSTS, 3, "psm_copy_costs_device"),
+            ("runner_up", capi.PSM_OPT_RUNNER_UP, 2, "psm_copy_runner_up_device"))
 
 
 def frame_layout(t, height, width, channels="bgr"):
@@ -164,10 +167,10 @@ class TorchStereo:
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
         with post_process=True, and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
         host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
-        if not isinstance(costs, bool):
-            raise TypeError(f"costs must be True or False (got {costs!r})")
-        if not isinstance(runner_up, bool):
-            raise TypeError(f"runner_up must be True or False (got {runner_up!r})")
+        wanted = (costs, runner_up)
+        for (name, *_), on in zip(_OUTPUTS, wanted):
+            if not isinstance(on, bool):
+                raise TypeError(f"{name} must be True or False (got {on!r})")
         pix, lf, rf, row_step, col_step, batched = self._layout(left, right, channels)
         L, ctx = self._lib, self._ctx
         H, W = self.height, self.width
@@ -177,18 +180,15 @@ class TorchStereo:
         lmap = torch.empty(shape, dtype=mdt, device=self.device)
         rmap = torch.empty(shape, dtype=mdt, device=self.device) if self.views == capi.PSM_VIEWS_BOTH else None
         row = W * lmap.element_size()
-        if costs != self.costs:
-            self._check(L.psm_set_option(ctx, capi.PSM_OPT_COSTS, int(costs)))
-            self.costs = costs
-        cshape = (len(lf), 3, H, W) if batched else (3, H, W)
-        lcost = torch.empty(cshape, dtype=torch.float32, device=self.device) if costs else None
-        rcost = torch.empty(cshape, dtype=torch.float32, device=self.device) if costs and rmap is not None else None
-        if runner_up != self.runner_up:
-            self._check(L.psm_set_option(ctx, capi.PSM_OPT_RUNNER_UP, int(runner_up)))
-            self.runner_up = runner_up
-        rshape = (len(lf), 2, H, W) if batched else (2, H, W)
-        lrun = torch.empty(rshape, dtype=torch.float32, device=self.device) if runner_up else None
-        rrun = torch.empty(rshape, dtype=torch.float32, device=self.device) if runner_up and rmap is not None else None
+        outs = []   # (copy-out call, left planes, right planes) of each output asked for
+        for (name, key, n, copy), on in zip(_OUTPUTS, wanted):
+            if on != getattr(self, name):
+                self._check(L.psm_set_option(ctx, key, int(on)))
+                setattr(self, name, on)
+            if on:
+                oshape = (len(lf), n, H, W) if batched else (n, H, W)
+                outs.append((getattr(L, copy), torch.empty(oshape, dtype=torch.float32, device=self.device),
+                             None if rmap is None else torch.empty(oshape, dtype=torch.float32, device=self.device)))
         self._check(L.psm_wait_stream(ctx, stream))
         for b in range(len(lf)):
             lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
@@ -202,16 +202,12 @@ class TorchStereo:
             rm = None if rmap is None else (rmap[b] if batched else rmap)
             self._check(L.psm_copy_maps_device(ctx, 1 if post_process else 0, lm.data_ptr(), row,
                                                None if rm is None else rm.data_ptr(), row))
-            if costs:
-                lc = lcost[b] if batched else lcost
-                rc = None if rcost is None else (rcost[b] if batched else rcost)
-                self._check(L.psm_copy_costs_device(ctx, lc.data_ptr(), None if rc is None else rc.data_ptr(), W * 4))
-            if runner_up:
-                lu = lrun[b] if batched else lrun
-                ru = None if rrun is None else (rrun[b] if batched else rrun)
-                self._check(L.psm_copy_runner_up_device(ctx, lu.data_ptr(), None if ru is None else ru.data_ptr(), W * 4))
+            for copy, lo, ro in outs:
+                lo = lo[b] if batched else lo
+                ro = None if ro is None else (ro[b] if batched else ro)
+                self._check(copy(ctx, lo.data_ptr(), None if ro is None else ro.data_ptr(), W * 4))
         self._check(L.psm_signal_stream(ctx, stream))
-        return (lmap, rmap) + ((lcost, rcost) if costs else ()) + ((lrun, rrun) if runner_up else ())
+        return (lmap, rmap) + tuple(t for _, lo, ro in outs for t in (lo, ro))
 
     # -- measurement helpers ------------------------------------------------------------------
     def stage_ms(self, stage):

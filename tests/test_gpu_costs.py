@@ -16,23 +16,12 @@ import mixed_model as MM
 import test_gpu_selection_seams as SEAMS
 from gif_cases import assert_same
 from oracle import oracle as O
+from output_checks import assert_bits, expect, frame_counts, ptr
 from primestereomatch_b200 import DispEst, capi, synth
 
 pytestmark = pytest.mark.gpu
 
 U8, U16, U32 = np.uint8, np.uint16, np.uint32
-
-
-def assert_bits(got, want, what, nan_any=False):
-    """equal bit patterns; nan_any: a NaN equals a NaN of any sign and payload (the oracle's volume has the host's NaNs)"""
-    got = np.ascontiguousarray(got)
-    got = got.view(U32) if got.dtype == np.float32 else got
-    diff = got != want
-    if nan_any:
-        diff &= ~(((got & 0x7FFFFFFF) > 0x7F800000) & ((want & 0x7FFFFFFF) > 0x7F800000))
-    bad = np.argwhere(diff)
-    assert bad.size == 0, f"{what}: {len(bad)} of {got.size} cost entries differ, first at {tuple(bad[0])}: " \
-                          f"{got[tuple(bad[0])]:#010x} vs {want[tuple(bad[0])]:#010x}"
 
 
 def run(l, r, D, dtype=U8, *, setup=None, fgf=None, left_only=False, volumes=False, **kw):
@@ -187,18 +176,6 @@ def test_full_hd_late_blocks():
 
 
 # ---- launches and state rules ---------------------------------------------------------------------------------------------
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-def frame_counts(de, costs_on):
-    """launch counts of CostConst_GPU, the filter and DispSelect_GPU, and the maps"""
-    c = []
-    for stage in (de.CostConst_GPU, de.CostFilter_GPU, de.DispSelect_GPU):
-        n = de.launch_count(); stage(); c.append(de.launch_count() - n)
-    return c, de.lDisMap.copy(), None if de.rDisMap is None else de.rDisMap.copy()
-
-
 @pytest.mark.parametrize("kw,extra", [({}, 2), (dict(block_slices=7), 2), (dict(devices=[0, 0]), 4),
                                       (dict(devices=[0, 0, 0], block_slices=4), 6)])
 def test_launches_and_maps(kw, extra):
@@ -210,21 +187,14 @@ def test_launches_and_maps(kw, extra):
     with DispEst(l, r, D, **kw) as plain, DispEst(l, r, D, **kw) as toggled:
         toggled.setCostOutput(True)
         toggled.setCostOutput(False)
-        base = frame_counts(plain, False)
-        off = frame_counts(toggled, False)
+        base = frame_counts(plain)
+        off = frame_counts(toggled)
         assert off[0] == base[0]
         assert_same(off[1], base[1], "off: left"); assert_same(off[2], base[2], "off: right")
         toggled.setCostOutput(True)
-        on = frame_counts(toggled, True)
+        on = frame_counts(toggled)
         assert on[0] == [base[0][0], base[0][1], base[0][2] + extra], (on[0], base[0])
         assert_same(on[1], base[1], "on: left"); assert_same(on[2], base[2], "on: right")
-
-
-def expect(rc, code, de, *words):
-    text = capi.lib().psm_last_error(de.handle).decode()
-    assert rc == code, (rc, code, text)
-    for w in words:
-        assert w in text, (w, text)
 
 
 @pytest.mark.parametrize("kw", [{}, dict(block_slices=4), dict(devices=[0, 0])])

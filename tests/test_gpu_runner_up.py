@@ -19,25 +19,12 @@ import runner_up_cases as RU
 import test_gpu_selection_seams as SEAMS
 from gif_cases import assert_same
 from oracle import oracle as O
+from output_checks import assert_bits, expect, frame_counts, ptr
 from primestereomatch_b200 import DispEst, capi, synth
 
 pytestmark = pytest.mark.gpu
 
-U8, U16, U32 = np.uint8, np.uint16, np.uint32
-
-
-def assert_bits(got, want, what, nan_any=False):
-    """equal bit patterns; nan_any: a NaN equals a NaN of any sign and payload (the oracle's volume has the host's NaNs)"""
-    got = np.ascontiguousarray(got)
-    got = got.view(U32) if got.dtype == np.float32 else got
-    want = np.ascontiguousarray(want)
-    want = want.view(U32) if want.dtype == np.float32 else want
-    diff = got != want
-    if nan_any:
-        diff &= ~(((got & 0x7FFFFFFF) > 0x7F800000) & ((want & 0x7FFFFFFF) > 0x7F800000))
-    bad = np.argwhere(diff)
-    assert bad.size == 0, f"{what}: {len(bad)} of {got.size} entries differ, first at {tuple(bad[0])}: " \
-                          f"{got[tuple(bad[0])]:#010x} vs {want[tuple(bad[0])]:#010x}"
+U8, U16 = np.uint8, np.uint16
 
 
 def run(l, r, D, dtype=U8, *, setup=None, fgf=None, left_only=False, volumes=False, costs=False, runner_up=True, **kw):
@@ -184,14 +171,6 @@ def test_distinct_devices():
 
 
 # ---- maps, launches, both options ---------------------------------------------------------------------------------------------
-def frame_counts(de):
-    """launch counts of CostConst_GPU, the filter and DispSelect_GPU, and the maps"""
-    c = []
-    for stage in (de.CostConst_GPU, de.CostFilter_GPU, de.DispSelect_GPU):
-        n = de.launch_count(); stage(); c.append(de.launch_count() - n)
-    return c, de.lDisMap.copy(), None if de.rDisMap is None else de.rDisMap.copy()
-
-
 @pytest.mark.parametrize("kw,extra", [({}, 0), (dict(block_slices=7), 2), (dict(devices=[0, 0]), 6),
                                       (dict(devices=[0, 0, 0], block_slices=4), 8)])
 def test_launches_and_maps(kw, extra):
@@ -224,20 +203,20 @@ def test_both_options(kw):
         assert_same(both["maps"][v], alone["maps"][v], f"view {v} maps")
         assert_bits(both["runner"][v], alone["runner"][v], f"view {v} runner-up with the costs on")
         assert_bits(both["costs"][v], costs["costs"][v], f"view {v} costs with the runner-up on")
+    # stage 3 adds both options' launches: the costs one write per view and shard, the runner-up one pick per view on a
+    # blocked context, and a pick per view and shard plus one slot reduce per view on a multi-device one (the extras
+    # test_launches_and_maps pins here and in test_gpu_costs)
+    shards = len(kw.get("devices", [0]))
+    costs_extra = 2 * shards
+    runner_up_extra = 2 * shards + 2 if "devices" in kw else 2 if kw.get("block_slices") else 0
+    with DispEst(l, r, D, **kw) as plain, DispEst(l, r, D, **kw) as de:
+        de.setCostOutput(True)
+        de.setRunnerUpOutput(True)
+        base, on = frame_counts(plain)[0], frame_counts(de)[0]
+    assert on == [base[0], base[1], base[2] + costs_extra + runner_up_extra], (on, base)
 
 
 # ---- state rules ------------------------------------------------------------------------------------------------------------
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-def expect(rc, code, de, *words):
-    text = capi.lib().psm_last_error(de.handle).decode()
-    assert rc == code, (rc, code, text)
-    for w in words:
-        assert w in text, (w, text)
-
-
 @pytest.mark.parametrize("kw", [{}, dict(block_slices=4), dict(devices=[0, 0])])
 def test_state_rules(kw):
     import torch
