@@ -22,6 +22,8 @@
  *   psm_post_process      <-> DispEst::PostProcess_GPU -> PP::processDM -> JointWMF::filter
  *                                                                 src/DispEst.cpp:338-344, src/PP.cpp:402-425
  *   psm_set_lr_check      <-> PP::processDM's lrCheck + fillInv (commented out there)  src/PP.cpp:17-143, :405-406
+ *   psm_set_speckle_filter <-> cv::filterSpeckles, as the reference's StereoSGBM matcher configures it (speckleWindowSize,
+ *                             speckleRange)                       src/StereoMatch.cpp:654-655
  *   psm_read_cost_slice   <-> DispEst::printCV (cost-slice dump) src/DispEst.cpp:181-194
  *   psm_stage_ms          <-> cvc_time/cvf_time/dispsel_time     src/StereoMatch.cpp:209-241
  *
@@ -52,7 +54,9 @@
  * blocking uploads): psm_set_images_async / _u8_async (the second staging set), psm_cost_filter and psm_read_ab_slice
  * (the scratch of the reference-order pass: float frames, a non-default guided filter, PSM_CVF_NAIVE, flagged slices),
  * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
- * (its buffers and, after a change of sigma or weight type, the weight table), psm_set_option(PSM_OPT_COSTS, 1) (the
+ * (its buffers and, after a change of sigma or weight type, the weight table; with psm_set_speckle_filter on, the
+ * labels and counts, 8 * W * H bytes per view, and with PSM_SPECKLE_FIRST and a check mode, a map pair between the
+ * removal and the check), psm_set_option(PSM_OPT_COSTS, 1) (the
  * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots).  Run them once before a
  * latency-critical
  * loop.  psm_set_stream always waits for the stream it leaves.
@@ -330,6 +334,32 @@ int psm_set_lr_check(psm_ctx* ctx, int mode);
 /* The left-right check's mask of one view (0 / 1, W x H, row step in bytes >= W) to HOST memory; synchronises.
  * PSM_ESTATE unless the last post-process call since the last selection stage ran the check. */
 int psm_read_valid_mask(psm_ctx* ctx, int view, uint8_t* dst, size_t dst_step);
+
+/* Speckle filter modes of psm_set_speckle_filter */
+enum { PSM_SPECKLE_OFF = 0, PSM_SPECKLE_FIRST = 1, PSM_SPECKLE_ONLY = 2 };
+
+/* Speckle removal (OpenCV's cv::filterSpeckles(map, 0, max_size, max_diff), as StereoBM / StereoSGBM users configure it
+ * with speckleWindowSize and speckleRange) for every later psm_post_process / _u16 / _device of this context:
+ *   PSM_SPECKLE_OFF (default): the stage exactly as psm_set_lr_check and psm_set_post_filter configure it, launch for
+ *                     launch;
+ *   PSM_SPECKLE_FIRST: speckle removal on the selection maps, then the configured check and / or post-filter on its
+ *                     result (4 more launches);
+ *   PSM_SPECKLE_ONLY: speckle removal alone; its maps are the result and neither the check nor the post-filter runs, so
+ *                     psm_read_valid_mask returns PSM_ESTATE (4 launches).
+ * Definition, on each view's map on its own (u8, or u16 on a 16-bit context; cv::filterSpeckles on the map as CV_16S):
+ * pixels of value 0 belong to no blob; two 4-neighbours p, q, both non-zero, are in the same blob when
+ * |m(p) - m(q)| <= max_diff (in whole disparities, compared as int); blobs are the connected components of that graph;
+ * every pixel of a blob of at most max_size pixels becomes 0, every other pixel keeps its value.  The result does not
+ * depend on any visiting order.  Removed pixels are 0, which the check never accepts: with PSM_LR_FILL_WMF / PSM_LR_FILL
+ * they are filled like occlusions and psm_read_valid_mask shows them as invalid.  With PSM_LR_OFF and
+ * PSM_SPECKLE_FIRST the post-filter sees them as disparity 0 (a removed blob pulls its neighbours' medians down).  Range
+ * contexts filter their absolute maps; left-only contexts filter the left map (PSM_SPECKLE_FIRST with a check mode keeps
+ * the check's PSM_ESTATE).  The stage reads the maps of the last selection stage and never writes them, the costs or the
+ * runner-up; the result goes to psm_device_ptr selectors 4 / 5 and psm_copy_maps_device(which = 1).  Stage 5 of
+ * psm_stage_ms covers it.  Valid: one of the three modes and, unless the mode is PSM_SPECKLE_OFF, max_size >= 1 and
+ * max_diff >= 0; anything else returns PSM_EINVAL and leaves the context unchanged.  Multi-device contexts forward it to
+ * every shard.  See DESIGN.md section 23. */
+int psm_set_speckle_filter(psm_ctx* ctx, int mode, int max_size, int max_diff);
 
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream.  Waits for the work already enqueued

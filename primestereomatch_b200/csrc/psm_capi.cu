@@ -4,6 +4,7 @@
 #include "../../include/prime_stereo_b200.h"
 
 #include <algorithm>
+#include <climits>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -19,6 +20,7 @@
 #include "psm_pp_param.cuh"
 #include "psm_fgf.cuh"
 #include "psm_lr.cuh"
+#include "psm_speckle.cuh"
 
 #ifndef PSM_BUILD_FLAGS
 #define PSM_BUILD_FLAGS "unknown"
@@ -115,6 +117,11 @@ struct psm_ctx {
     int lr_mode = PSM_LR_OFF;               // left-right check and fill in front of the post-filter, psm_set_lr_check
     uint8_t* lr_valid[2] = {nullptr, nullptr};  // the check's masks (W x H, 0/1), lazy
     bool lr_masks_ok = false;               // lr_valid holds the masks of the current maps (psm_read_valid_mask)
+    int sp_mode = PSM_SPECKLE_OFF;          // speckle removal in the post-process stage, psm_set_speckle_filter
+    int sp_max_size = 0, sp_max_diff = 0;
+    int* sp_lab = nullptr;                  // speckle removal's labels and counts: 2 x W x H each (view v at v * W * H), lazy
+    int* sp_cnt = nullptr;
+    uint8_t* sp_maps[2] = {nullptr, nullptr};  // PSM_SPECKLE_FIRST with the check: the filtered maps the check reads, lazy
     // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
     // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
     int blk_slices = 0;
@@ -1453,7 +1460,9 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->guide_flags);
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
+    cudaFree(c->sp_lab); cudaFree(c->sp_cnt);
     for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]);
+                                   cudaFree(c->sp_maps[v]);
                                    cudaFree(c->track[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]);
                                    for (psm_ctx::OutState& o : c->outs) cudaFree(o.planes[v]); }
     for (int s = 0; s < kNumStages; ++s) {
@@ -1668,6 +1677,21 @@ int psm_set_lr_check(psm_ctx* c, int mode)
     if (mode != PSM_LR_OFF && mode != PSM_LR_FILL_WMF && mode != PSM_LR_FILL)
         return fail(c, PSM_EINVAL, "left-right check mode %d is not off (0), fill + post-filter (1) or fill (2)", mode);
     c->lr_mode = mode;
+    return PSM_OK;
+}
+
+int psm_set_speckle_filter(psm_ctx* c, int mode, int max_size, int max_diff)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_speckle_filter(s, mode, max_size, max_diff); });
+    if (mode != PSM_SPECKLE_OFF && mode != PSM_SPECKLE_FIRST && mode != PSM_SPECKLE_ONLY)
+        return fail(c, PSM_EINVAL, "speckle filter mode %d is not off (0), first (1) or only (2)", mode);
+    if (mode != PSM_SPECKLE_OFF && (max_size < 1 || max_diff < 0))
+        return fail(c, PSM_EINVAL, "speckle filter max_size %d / max_diff %d: need max_size >= 1 and max_diff >= 0",
+                    max_size, max_diff);
+    c->sp_mode = mode;
+    c->sp_max_size = max_size;
+    c->sp_max_diff = max_diff;
     return PSM_OK;
 }
 
@@ -2257,6 +2281,29 @@ static int pp_weight_table(float sigma, int type, uint32_t* t)
 
 }  // extern "C"
 
+// speckle removal (psm_speckle.cuh) of the maps in[view] into out[view], both views in each of its four launches
+template <typename T>
+static int speckle_filter(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
+{
+    const SpeckleArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])}, c->sp_lab, c->sp_cnt,
+                              c->W, c->H, c->sp_max_diff};
+    const unsigned ntx = (unsigned)(c->W + kSpTile - 1) / kSpTile, nty = (unsigned)(c->H + kSpTile - 1) / kSpTile;
+    const dim3 blk(kSpTile, kSpRows);
+    speckle_local_kernel<T><<<dim3(ntx, nty, c->views), blk, 0, c->stream>>>(a);
+    PSM_LAUNCH_CHECK(c);
+    const int nv = (int)(ntx - 1) * c->H, nh = (int)(nty - 1) * c->W;   // edges across vertical / horizontal seams
+    const unsigned sgrid = std::max(1u, (unsigned)((nv + nh + kSpSeamThreads - 1) / kSpSeamThreads));
+    speckle_seam_kernel<T><<<dim3(sgrid, 1, c->views), kSpSeamThreads, 0, c->stream>>>(a, nv, nh);
+    PSM_LAUNCH_CHECK(c);
+    const dim3 grd(ntx, (unsigned)(c->H + kSpRows - 1) / kSpRows, c->views);
+    speckle_count_kernel<T><<<grd, blk, 0, c->stream>>>(a);
+    PSM_LAUNCH_CHECK(c);
+    speckle_paint_kernel<T><<<grd, blk, 0, c->stream>>>(a, c->sp_max_size, reinterpret_cast<T*>(out[0]),
+                                                         reinterpret_cast<T*>(out[1]));
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
 // the post-filter stage on maps of type T
 template <typename T>
 static int post_process_maps(psm_ctx* c)
@@ -2271,11 +2318,15 @@ static int post_process_maps(psm_ctx* c)
     const uint8_t* maps[2];
     if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
-    const bool lr = c->lr_mode != PSM_LR_OFF, wmf = c->lr_mode != PSM_LR_FILL;
+    // PSM_SPECKLE_ONLY: the removal is the whole stage; the check and the post-filter do not run
+    const bool sp = c->sp_mode != PSM_SPECKLE_OFF, only = c->sp_mode == PSM_SPECKLE_ONLY;
+    const bool lr = !only && c->lr_mode != PSM_LR_OFF, wmf = !only && c->lr_mode != PSM_LR_FILL;
     if (lr && c->views == 1)
         return fail(c, PSM_ESTATE, "psm_post_process: the left-right check (psm_set_lr_check mode %d) needs both maps, and "
                     "this context computes the left view alone (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): set PSM_LR_OFF or "
                     "PSM_VIEWS_BOTH", c->lr_mode);
+    if (sp && npix > (size_t)INT_MAX)
+        return fail(c, PSM_EINVAL, "psm_post_process: speckle removal labels pixels with int32 indices (W * H <= 2^31 - 1)");
     // Each buffer is allocated while its own pointer is null and the table is marked valid only once it is on the
     // device, so a call that failed part-way leaves nothing a launch could trip over: the next call completes the set-up
     // or fails in turn.
@@ -2286,6 +2337,12 @@ static int post_process_maps(psm_ctx* c)
     for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->dis_pp[v], npix * c->map_bytes));
     if (lr)
         for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->lr_valid[v], npix));
+    if (sp) {
+        PSM_CUDA(c, alloc_if_null(c->sp_lab, 2 * npix * sizeof(int)));
+        PSM_CUDA(c, alloc_if_null(c->sp_cnt, 2 * npix * sizeof(int)));
+        if (lr)
+            for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->sp_maps[v], npix * c->map_bytes));
+    }
     if (wmf && !c->pp_lut_valid) {
         const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
         PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -2302,6 +2359,14 @@ static int post_process_maps(psm_ctx* c)
     const bool tuned = c->pp_tuned();
     if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
+    if (sp) {
+        // the removal reads the selection maps and writes the stage's result (PSM_SPECKLE_ONLY), the check's input, or
+        // the post-filter's first input (in place: each pass packs its input before it writes dis_pp)
+        uint8_t* const out[2] = {lr ? c->sp_maps[0] : c->dis_pp[0], lr ? c->sp_maps[1] : c->dis_pp[1]};
+        if (int rc = speckle_filter<T>(c, maps, out)) return rc;
+        if (only) return stage_end(c, 5);
+        maps[0] = out[0]; maps[1] = out[1];
+    }
     if (lr) {
         // lrCheck + fillInv (PP.cpp:405-406): reads the selection maps, writes the filled maps into dis_pp
         const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;

@@ -105,6 +105,7 @@ class DispEst:
         self.lValid = np.zeros((self.hei, self.wid), np.uint8)  # DispEst.cpp:48-49
         self.rValid = np.zeros((self.hei, self.wid), np.uint8)
         self.lr_mode = capi.PSM_LR_OFF
+        self.speckle_mode = capi.PSM_SPECKLE_OFF
         self.cost_output = False
         self.lCosts = self.rCosts = None   # setCostOutput(True): DispSelect_GPU's (3, H, W) float32 costs
         self.runner_up_output = False
@@ -200,6 +201,17 @@ class DispEst:
         self._need_gpu()
         capi.check(self._lib.psm_set_lr_check(self._ctx, int(mode)), self._ctx)
         self.lr_mode = int(mode)
+        return 0
+
+    def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
+        """Speckle removal (OpenCV's filterSpeckles(map, 0, max_size, max_diff)) for every later PostProcess_GPU call:
+        0 off (default), 1 first (then the check and / or post-filter of setLRCheck / setPostFilter on its result), 2 only
+        (its maps are the result; lValid / rValid are not read).  Every 4-connected blob of non-zero pixels whose
+        neighbours differ by at most max_diff, of at most max_size pixels, becomes 0 (invalid).  Raises PsmError on any
+        other mode, or unless max_size >= 1 and max_diff >= 0 with the filter on."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)), self._ctx)
+        self.speckle_mode = int(mode)
         return 0
 
     _VIEWS = {"left": capi.PSM_VIEWS_LEFT, "both": capi.PSM_VIEWS_BOTH}
@@ -308,11 +320,12 @@ class DispEst:
     def PostProcess_GPU(self):
         """DispEst.cpp:338-344 -> PP::processDM (PP.cpp:402-425): joint weighted-median filter of both maps (after the
         left-right check and fill, or instead of the filter, as setLRCheck selects); the reference runs it on the CPU even
-        in GPU mode, here it is a device stage.  Results replace lDisMap / rDisMap."""
+        in GPU mode, here it is a device stage.  Speckle removal runs first, or alone, as setSpeckleFilter selects.
+        Results replace lDisMap / rDisMap."""
         self._need_gpu()
         pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
         capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
-        if self.lr_mode != capi.PSM_LR_OFF:
+        if self.lr_mode != capi.PSM_LR_OFF and self.speckle_mode != capi.PSM_SPECKLE_ONLY:   # the check ran
             for view, mask in ((capi.PSM_LEFT, self.lValid), (capi.PSM_RIGHT, self.rValid)):
                 capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)
         return 0

@@ -88,7 +88,7 @@ public:
                       // whose low byte is the reference's uchar map
     cv::Mat rDisMap;
     cv::Mat lValid;   // CV_8UC1 masks of the left-right check (reference DispEst.h:81-82), 0/1; PostProcess_GPU fills them
-    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF
+    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF (and setSpeckleFilter not PSM_SPECKLE_ONLY)
     cv::Mat lCosts[3];  // setCostOutput(true): CV_32FC1 filtered costs at disparity m - 1, m, m + 1 of the selection map's
     cv::Mat rCosts[3];  // m (psm_read_costs); DispSelect_GPU fills them, rCosts not on a left-only context
     cv::Mat lRunnerUp[2];  // setRunnerUpOutput(true): CV_32FC1 runner-up disparity r (0 where none exists) and its
@@ -110,6 +110,10 @@ public:
     // post-filter for every later PostProcess call; see psm_set_lr_check.  INTEGRATION.md: a build that restores
     // PP.cpp:405-406 calls setLRCheck(PSM_LR_FILL_WMF).
     int setLRCheck(int mode);
+    // Speckle removal (cv::filterSpeckles(map, 0, max_size, max_diff)) in front of (PSM_SPECKLE_FIRST) or instead of
+    // (PSM_SPECKLE_ONLY) the check and post-filter for every later PostProcess call; see psm_set_speckle_filter.  A port
+    // of a StereoSGBM pipeline calls setSpeckleFilter(PSM_SPECKLE_FIRST, speckleWindowSize, speckleRange).
+    int setSpeckleFilter(int mode, int max_size, int max_diff);
     // PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT (PSM_OPT_VIEWS): with PSM_VIEWS_LEFT the later frames compute the left
     // map alone; DispSelect_GPU and PostProcess_GPU then leave rDisMap (and rValid) untouched.  The next stage after a
     // change must be CostConst_GPU.
@@ -152,6 +156,7 @@ private:
     bool useOCL;
     unsigned int subsample_rate = 4;
     int lr_mode = PSM_LR_OFF;
+    int speckle_mode = PSM_SPECKLE_OFF;
     int views = PSM_VIEWS_BOTH;
     bool cost_output = false;
     bool runner_up_output = false;

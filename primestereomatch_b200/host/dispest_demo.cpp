@@ -10,7 +10,8 @@
 // maps are CV_16UC1 and the output files hold 2-byte (native-endian uint16) disparities.  A leading
 // `--block-slices N` runs a blocked context (psm_create_blocked) that holds N disparity slices at a time, a leading
 // `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat), a leading
-// `--min-disp N` a context over disparities [N, D) alone (psm_create_range; the maps hold absolute disparities).  A leading
+// `--min-disp N` a context over disparities [N, D) alone (psm_create_range; the maps hold absolute disparities), a
+// leading `--speckle MODE SIZE DIFF` speckle removal (setSpeckleFilter: MODE 0 off, 1 first, 2 only).  A leading
 // `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.
 #include <cstdio>
 #include <cstdlib>
@@ -31,6 +32,7 @@ static bool read_all(const char* path, void* dst, size_t n)
 int main(int argc, char** argv)
 {
     int block_slices = 0, min_disp = 0;
+    int speckle[3] = {0, 0, 0};   // mode, max_size, max_diff
     std::vector<int> devices;
     const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
     if (left_only) {
@@ -39,7 +41,15 @@ int main(int argc, char** argv)
         --argc;
     }
     while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices") ||
-                         !std::strcmp(argv[1], "--min-disp"))) {
+                         !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle"))) {
+        if (!std::strcmp(argv[1], "--speckle")) {
+            if (argc < 5) break;
+            for (int k = 0; k < 3; ++k) speckle[k] = std::atoi(argv[2 + k]);
+            argv[4] = argv[0];
+            argv += 4;
+            argc -= 4;
+            continue;
+        }
         if (!std::strcmp(argv[1], "--block-slices")) {
             block_slices = std::atoi(argv[2]);
         } else if (!std::strcmp(argv[1], "--min-disp")) {
@@ -57,7 +67,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -80,6 +90,7 @@ int main(int argc, char** argv)
         rc = SMDE->setPostFilter(std::atoi(argv[13]), (float)std::atof(argv[14]), std::atoi(argv[15]), wt);
     }
     if (!rc && argc == 18) rc = SMDE->setLRCheck(std::atoi(argv[17]));
+    if (!rc && speckle[0]) rc = SMDE->setSpeckleFilter(speckle[0], speckle[1], speckle[2]);
     if (!rc) rc = SMDE->CostConst_GPU();
     if (!rc) rc = SMDE->CostFilter_GPU();
     if (!rc) rc = SMDE->DispSelect_GPU();

@@ -128,6 +128,9 @@ class TorchStereo:
     def setLRCheck(self, mode):
         self._check(self._lib.psm_set_lr_check(self._ctx, int(mode)))
 
+    def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
+        self._check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)))
+
     def setViews(self, views):
         value = DispEst._VIEWS.get(views, -1) if isinstance(views, str) else -1
         self._check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_VIEWS, value))
@@ -165,7 +168,7 @@ class TorchStereo:
 
         After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
-        with post_process=True, and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
+        with post_process=True (the chain setSpeckleFilter, setLRCheck and setPostFilter configure), and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
         host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
         wanted = (costs, runner_up)
         for (name, *_), on in zip(_OUTPUTS, wanted):
