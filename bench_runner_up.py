@@ -2,12 +2,13 @@
 
 Workload: the synthetic 1920 x 1080 pair of bench.py (synth.stereo_pair_u8), both views, default filter, u8 frames
 uploaded from the host; a frame is ingest -> CVC -> CVF -> WTA (maps left on the device), and with the option on also
-the runner-up into device tensors (psm_copy_runner_up_device).  Five configurations, the ones whose path differs:
+the runner-up into device tensors (psm_copy_runner_up_device).  Six configurations, the ones whose path differs:
   - D = 128 unblocked (the selection kernel keeps the four-lowest lists in its one read of the volume);
   - D = 2048 at block_slices 128 and D = 128 at block_slices 16 (the block fold keeps the running lists; the small
     blocks move them most often per slice);
   - two shards co-located on device 0 at D = 256 (a list scan of every shard's slices, the slots and their reduce);
-  - D = 128 unblocked with PSM_OPT_COSTS on in both contexts (what the runner-up adds to the costs).
+  - D = 128 unblocked and D = 128 at block_slices 16 with PSM_OPT_COSTS on in both contexts (what the runner-up adds
+    to the costs; blocked, the block fold tracks the costs and the running lists in one read).
 For each, one context with the option off and one with it on are alive at once and run in turn, one frame each per
 round, so that drift on a shared card hits both alike.  Medians over the rounds of the frame time (CUDA events around
 the frame on the first device's stream after psm_wait_stream, psm_signal_stream back).  Before the line is printed, the
@@ -29,7 +30,8 @@ sys.path.insert(0, ROOT)
 W, H = 1920, 1080
 CONFIGS = [("unblocked D=128", 128, {}, False), ("blocked D=2048 B=128", 2048, dict(block_slices=128), False),
            ("blocked D=128 B=16", 128, dict(block_slices=16), False), ("2 shards D=256", 256, dict(devices=[0, 0]), False),
-           ("unblocked D=128, costs on in both", 128, {}, True)]
+           ("unblocked D=128, costs on in both", 128, {}, True),
+           ("blocked D=128 B=16, costs on in both", 128, dict(block_slices=16), True)]
 
 
 def main():

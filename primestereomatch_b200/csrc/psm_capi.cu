@@ -805,18 +805,17 @@ RunnerUpSlots runner_up_slots(const psm_ctx* c, int v, int nslots) { return {c->
 int launch_fold(psm_ctx* c, bool first)
 {
     FoldParams P;
-    for (int v = 0; v < 2; ++v) { P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; }
+    for (int v = 0; v < 2; ++v) {
+        P.vol[v] = c->vol[v]; P.keys[v] = c->run_keys[v]; P.track[v] = track_planes(c, v); P.list[v] = list_planes(c, v);
+    }
     P.W = c->W; P.H = c->H; P.Wp = c->Wp; P.d_begin = c->res.begin; P.d_count = c->res.count; P.first = first ? 1 : 0;
+    P.write_first = c->track_planes() > kCostFirst;
     dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H, c->views);
+    const bool costs = c->outs[kOutCosts].on;
     if (c->outs[kOutRunnerUp].on)
-        (c->outs[kOutCosts].on ? wta_fold_list_kernel<true> : wta_fold_list_kernel<false>)<<<grd, blk, 0, c->stream>>>(
-            FoldListParams{P, {list_planes(c, 0), list_planes(c, 1)}, {track_planes(c, 0), track_planes(c, 1)},
-                           c->track_planes() > kCostFirst});
-    else if (c->outs[kOutCosts].on)
-        wta_fold_costs_kernel<<<grd, blk, 0, c->stream>>>(
-            FoldCostParams{P, {track_planes(c, 0), track_planes(c, 1)}, c->track_planes() > kCostFirst});
+        (costs ? wta_fold_kernel<true, true> : wta_fold_kernel<false, true>)<<<grd, blk, 0, c->stream>>>(P);
     else
-        wta_fold_kernel<<<grd, blk, 0, c->stream>>>(P);
+        (costs ? wta_fold_kernel<true, false> : wta_fold_kernel<false, false>)<<<grd, blk, 0, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
@@ -1843,12 +1842,10 @@ static int select_maps(psm_ctx* c)
     }
     for (int v = 0; v < c->views; ++v) {
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        if (c->outs[kOutRunnerUp].on)   // the map and the runner-up in one read of the volume
-            wta_runner_up_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
-                                                                reinterpret_cast<T*>(c->dis[v]), out_planes(c, kOutRunnerUp, v));
-        else
-            wta_kernel<T><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count,
-                                                      reinterpret_cast<T*>(c->dis[v]), nullptr);
+        // with the runner-up, the map and the runner-up in one read of the volume
+        (c->outs[kOutRunnerUp].on ? wta_kernel<T, true> : wta_kernel<T, false>)<<<grd, blk, 0, c->stream>>>(
+            c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, reinterpret_cast<T*>(c->dis[v]), nullptr,
+            out_planes(c, kOutRunnerUp, v));
         PSM_LAUNCH_CHECK(c);
     }
     return PSM_OK;
@@ -1952,8 +1949,8 @@ int psm_disp_select_keys(psm_ctx* c, uint64_t* d_keys_left, uint64_t* d_keys_rig
     }
     for (int v = 0; v < c->views; ++v) {   // keys only, on either map format
         dim3 blk(256), grd(((c->W + 3) / 4 + 255) / 256, c->H);
-        wta_kernel<uint8_t><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, nullptr,
-                                                        reinterpret_cast<unsigned long long*>(keys[v]));
+        wta_kernel<uint8_t, false><<<grd, blk, 0, c->stream>>>(c->vol[v], c->W, c->H, c->Wp, c->d_begin, c->d_count, nullptr,
+                                                               reinterpret_cast<unsigned long long*>(keys[v]), CostPlanes{});
         PSM_LAUNCH_CHECK(c);
     }
     return stage_end(c, 3);

@@ -559,89 +559,13 @@ __device__ __forceinline__ void gif_coeffs(float mp, float mIp0, float mIp1, flo
 
 // ------------------------------------------------------------------------------------------
 // K4 WTA (DispSel.cpp:83-109): per pixel argmin over global d in [1, D), strict <, ties -> lowest d,
-// minCost starts at +inf, result 0 when nothing compares below +inf.  One thread = 4 pixels.  wta_scan4 is the scan of
-// every selection kernel, wta_key the packed (cost, d) key in which every shard, block and rank exchanges its minima.
+// minCost starts at +inf, result 0 when nothing compares below +inf.  One thread = 4 pixels.  wta_scan4 (below) is the
+// scan of every selection kernel, wta_key the packed (cost, d) key in which every shard, block and rank exchanges its
+// minima.
 // ------------------------------------------------------------------------------------------
-// the scan of slices [d_begin, d_begin + d_count), slice dl at p + dl * plane, into the caller's mc / md (set to +inf / 0;
-// returning them in a struct instead changes the kernels' SASS); an inactive lane scans nothing
-__device__ __forceinline__ void wta_scan4(const float* p, size_t plane, int d_begin, int d_count, bool active, float (&mc)[4],
-                                          int (&md)[4])
-{
-    int dl = (d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (DispSel.cpp:96)
-#pragma unroll 8
-    for (; active && dl < d_count; ++dl) {
-        const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
-        const int d = d_begin + dl;
-        if (c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
-        if (c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
-        if (c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
-        if (c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
-    }
-}
-
 __device__ __forceinline__ unsigned long long wta_key(float cost, int d)
 {
     return ((unsigned long long)float_order_key(cost) << 32) | (unsigned)d;
-}
-
-// the scan of one volume: the map (T = uint8_t or uint16_t) and/or the keys used by the disparity-sharded reduction
-template <typename T>
-__global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin, int d_count,
-                                                  T* __restrict__ dis /* [H][W] or null */,
-                                                  unsigned long long* __restrict__ keys /* [H][W] or null */)
-{
-    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    const int y = blockIdx.y;
-    if (x4 >= W) return;
-    const size_t plane = (size_t)H * Wp;
-    const float* p = vol + (size_t)y * Wp + x4;
-    float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
-    int md[4] = {0, 0, 0, 0};
-    wta_scan4(p, plane, d_begin, d_count, true, mc, md);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int x = x4 + j;
-        if (x < W) {
-            if (dis) dis[(size_t)y * W + x] = (T)md[j];
-            if (keys) keys[(size_t)y * W + x] = wta_key(mc[j], md[j]);
-        }
-    }
-}
-
-// WTA of one block of slices of a blocked context (psm_create_blocked), both views in one launch (blockIdx.z = view):
-// wta_scan4 over the block's d_count slices starting at global d_begin, then its wta_key is stored (first block) or
-// folded into the running key by min.  The min over keys of consecutive blocks is the
-// selection over their union: the strict <, the lowest-d tie-break and +inf / NaN costs behave as in one scan.
-struct FoldParams {
-    const float* vol[2];             // the block's filtered volumes [d_count][H][Wp]
-    unsigned long long* keys[2];     // running keys [H][W]
-    int W, H, Wp, d_begin, d_count, first;
-};
-
-__global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
-{
-    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    const int y = blockIdx.y, view = blockIdx.z;
-    if (x4 >= P.W) return;
-    const size_t plane = (size_t)P.H * P.Wp;
-    // views selected, not indexed: a parameter array indexed by a run-time value is copied to the stack
-    const float* p = (view ? P.vol[1] : P.vol[0]) + (size_t)y * P.Wp + x4;
-    float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
-    int md[4] = {0, 0, 0, 0};
-    wta_scan4(p, plane, P.d_begin, P.d_count, true, mc, md);
-    unsigned long long* k = (view ? P.keys[1] : P.keys[0]) + (size_t)y * P.W;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int x = x4 + j;
-        if (x < P.W) {
-            unsigned long long v = wta_key(mc[j], md[j]);
-            if (!P.first) {
-                const unsigned long long old = k[x];
-                v = old < v ? old : v;
-            }
-            k[x] = v;
-        }
-    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -664,11 +588,22 @@ struct CostPlanes {
     __host__ __device__ unsigned* uplane(int k) const { return reinterpret_cast<unsigned*>(plane(k)); }
 };
 
-// The runner-up (PSM_OPT_RUNNER_UP), in planes of the same shape.  The result: kRunnerUpOut planes, r as a float and
-// q(r) bit for bit (kCostNaN where r = 0); only the selection stages write them.  A blocked context's running list
-// (kListPlanes, beside the head's key in its running keys): planes kListCost + e hold the cost bits of entries e = 0..3,
-// planes kListD + e - 1 the d of entries e = 1..3.  A multi-device context's slots on the first shard (RunnerUpSlots):
-// per shard and pixel, the candidate's key and its cost bits.
+// ------------------------------------------------------------------------------------------
+// The runner-up away from the winner (PSM_OPT_RUNNER_UP).  The candidates are the arg-min's: d in [1, D) whose cost
+// compares below +inf, in the order of wta_key (the cost, -0 equal to +0, then the lowest d).  The runner-up r of a pixel
+// with map m is the first candidate with |d - m| >= 2, 0 when there is none; the result planes hold (float)r and q(r)
+// bit for bit (kCostNaN where r = 0).
+// Every path keeps, per pixel, the list of its four lowest candidates, lowest first, empty entries (+inf, 0) behind them.
+// Four are enough: at most three entries lie in {m - 1, m, m + 1}, so the first entry outside them is the lowest
+// candidate outside them.  The list is mergeable: the four lowest of a union of disjoint slice ranges are the four
+// lowest of the ranges' lists.  So a blocked walk folds each block's list into a running one, and the shards of a
+// multi-device context each pick from their own list and the first shard takes the lowest key of the picks.
+// ------------------------------------------------------------------------------------------
+// Planes of the same shape.  The result: kRunnerUpOut planes, r as a float and q(r) bit for bit (kCostNaN where r = 0);
+// only the selection stages write them.  A blocked context's running list (kListPlanes, beside the head's key in its
+// running keys): planes kListCost + e hold the cost bits of entries e = 0..3, planes kListD + e - 1 the d of entries
+// e = 1..3.  A multi-device context's slots on the first shard (RunnerUpSlots): per shard and pixel, the candidate's key
+// and its cost bits.
 constexpr int kRunnerUpOut = 2, kListLen = 4, kListCost = 0, kListD = 4, kListPlanes = 7;
 
 struct RunnerUpSlots {
@@ -683,92 +618,246 @@ struct RunnerUpSlots {
     }
 };
 
-// wta_scan4 over slices [d_begin, d_begin + d_count), tracking the costs beside the running minimum: on a new minimum at
-// d, lo = the previous slice's cost (`prev`, seeded with the cost before the range) and hi waits for slice d + 1.  Slice
-// 0 is scanned but is never a candidate: the no-winner state (md = 0) takes ce = q(0) and, from the md == d - 1 rule,
-// hi = q(1).  `first` and `prev` end as the range's first and last costs.
-__device__ __forceinline__ void wta_scan4_costs(const float* p, size_t plane, int d_begin, int d_count, float (&mc)[4],
-                                                int (&md)[4], float (&lo)[4], float (&ce)[4], float (&hi)[4],
-                                                float (&prev)[4], float (&first)[4])
+// c at slice d into entries 1.. of a sorted list whose head (c0, d0) c replaces where `head`; every entry comes from a
+// slice below d or costs less: the strict < puts c behind every entry of equal cost, as the arg-min's lowest-d rule does,
+// and a +inf or NaN cost never enters
+__device__ __forceinline__ void list_insert_tail(float (&lc)[kListLen], int (&ld)[kListLen], float c, int d, bool head, float c0,
+                                                 int d0)
 {
-    const float nan = __uint_as_float(kCostNaNBits);
-    for (int dl = 0; dl < d_count; ++dl) {
-        const float4 c4 = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
-        const float c[4] = {c4.x, c4.y, c4.z, c4.w};
-        const int d = d_begin + dl;
+    const bool b1 = c < lc[1], b2 = c < lc[2], b3 = c < lc[3];
+    lc[3] = b2 ? lc[2] : (b3 ? c : lc[3]);  ld[3] = b2 ? ld[2] : (b3 ? d : ld[3]);
+    lc[2] = b1 ? lc[1] : (b2 ? c : lc[2]);  ld[2] = b1 ? ld[1] : (b2 ? d : ld[2]);
+    lc[1] = head ? c0 : (b1 ? c : lc[1]);   ld[1] = head ? d0 : (b1 ? d : ld[1]);
+}
+
+// c at slice d into a whole sorted list
+__device__ __forceinline__ void list_insert(float (&lc)[kListLen], int (&ld)[kListLen], float c, int d)
+{
+    const bool b0 = c < lc[0];
+    list_insert_tail(lc, ld, c, d, b0, lc[0], ld[0]);
+    lc[0] = b0 ? c : lc[0];                 ld[0] = b0 ? d : ld[0];
+}
+
+// pixel i's running list in planes L, whose head's d is in its running key
+__device__ __forceinline__ void list_load(const CostPlanes& L, unsigned long long key, size_t i, float (&lc)[kListLen],
+                                          int (&ld)[kListLen])
+{
+    ld[0] = (int)(unsigned)key;
+#pragma unroll
+    for (int e = 0; e < kListLen; ++e) {
+        lc[e] = L.plane(kListCost + e)[i];
+        if (e > 0) ld[e] = (int)L.uplane(kListD + e - 1)[i];
+    }
+}
+
+// the list back into planes L (the head's key is the caller's to write)
+__device__ __forceinline__ void list_store(const CostPlanes& L, size_t i, const float (&lc)[kListLen], const int (&ld)[kListLen])
+{
+#pragma unroll
+    for (int e = 0; e < kListLen; ++e) {
+        L.plane(kListCost + e)[i] = lc[e];
+        if (e > 0) L.uplane(kListD + e - 1)[i] = (unsigned)ld[e];
+    }
+}
+
+// the runner-up of a pixel with map m from its list: (r, q(r)), or (0, kCostNaN)
+__device__ __forceinline__ void runner_up_pick(const float (&lc)[kListLen], const int (&ld)[kListLen], int m, int& r, float& q)
+{
+    r = 0;
+    q = __uint_as_float(kCostNaNBits);
+#pragma unroll
+    for (int e = kListLen - 1; e >= 0; --e)
+        if (ld[e] != 0 && abs(ld[e] - m) >= 2) { r = ld[e]; q = lc[e]; }
+}
+
+// ------------------------------------------------------------------------------------------
+// The selection scan.  Per pixel j of its four, what wta_scan4 tracks beside the arg-min (mc, md):
+//   kCosts: the costs beside the running minimum.  On a new minimum at d, lo = the previous slice's cost (`prev`, seeded
+//           with the cost before the range) and hi waits for slice d + 1.  Slice 0 is read but is never a candidate:
+//           the no-winner state (md = 0) takes ce = q(0) and, from the md == d - 1 rule, hi = q(1).  `first` and
+//           `prev` end as the range's first and last costs.
+//   kList:  the list of the four lowest candidates.  Its head is the arg-min itself, so during the scan only entries 1..
+//           are kept here; wta_scan4 copies (mc, md) into entry 0 at its end.
+// ------------------------------------------------------------------------------------------
+template <bool kCosts, bool kList>
+struct ScanTrack {
+    float lo[4], ce[4], hi[4], prev[4], first[4];
+    float lc[4][kListLen];
+    int ld[4][kListLen];
+
+    __device__ __forceinline__ ScanTrack()
+    {
+        const float nan = __uint_as_float(kCostNaNBits);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            if (md[j] == d - 1) hi[j] = c[j];
-            if (d == 0) ce[j] = c[j];
-            else if (c[j] < mc[j]) { mc[j] = c[j]; md[j] = d; lo[j] = prev[j]; ce[j] = c[j]; hi[j] = nan; }
-            prev[j] = c[j];
-            if (dl == 0) first[j] = c[j];
+            if constexpr (kCosts) lo[j] = ce[j] = hi[j] = prev[j] = nan;
+            if constexpr (kList)
+#pragma unroll
+                for (int e = 0; e < kListLen; ++e) { lc[j][e] = INFINITY; ld[j][e] = 0; }
+        }
+    }
+
+    // pixel j's cost c at slice d, the dl-th of the range, before the arg-min (mc, md) sees it
+    __device__ __forceinline__ void step(int j, float c, int d, int dl, bool cand, float mc, int md)
+    {
+        const bool take = cand && c < mc;   // the arg-min's test: c becomes the new minimum
+        if constexpr (kCosts) {
+            if (md == d - 1) hi[j] = c;
+            if (!cand) ce[j] = c;
+            else if (take) { lo[j] = prev[j]; ce[j] = c; hi[j] = __uint_as_float(kCostNaNBits); }
+            prev[j] = c;
+            if (dl == 0) first[j] = c;
+        }
+        if constexpr (kList)
+            if (cand) list_insert_tail(lc[j], ld[j], c, d, take, mc, md);
+    }
+};
+
+// The scan of slices [d_begin, d_begin + d_count), slice dl at p + dl * plane, into the caller's mc / md (set to +inf / 0;
+// returning them in a struct instead changes the kernels' SASS) and t; an inactive lane scans nothing.  Global d = 0 is
+// never a candidate (DispSel.cpp:96); only the costs read its slice.  Each pixel's tracker step sees the slice before the
+// arg-min, whose strict < keeps the lowest d, takes it.  The four pixels stay four statements on the float4's components:
+// a loop over an array of them, or a helper taking mc / md by reference, changes the SASS of the kernels without a
+// tracker.
+template <bool kCosts, bool kList>
+__device__ __forceinline__ void wta_scan4(const float* p, size_t plane, int d_begin, int d_count, bool active, float (&mc)[4],
+                                          int (&md)[4], ScanTrack<kCosts, kList>& t)
+{
+    int dl = (!kCosts && d_begin == 0) ? 1 : 0;
+#pragma unroll 8
+    for (; active && dl < d_count; ++dl) {
+        const float4 c = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
+        const int d = d_begin + dl;
+        const bool cand = !kCosts || d != 0;
+        t.step(0, c.x, d, dl, cand, mc[0], md[0]); if (cand && c.x < mc[0]) { mc[0] = c.x; md[0] = d; }
+        t.step(1, c.y, d, dl, cand, mc[1], md[1]); if (cand && c.y < mc[1]) { mc[1] = c.y; md[1] = d; }
+        t.step(2, c.z, d, dl, cand, mc[2], md[2]); if (cand && c.z < mc[2]) { mc[2] = c.z; md[2] = d; }
+        t.step(3, c.w, d, dl, cand, mc[3], md[3]); if (cand && c.w < mc[3]) { mc[3] = c.w; md[3] = d; }
+    }
+    if constexpr (kList)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { t.lc[j][0] = mc[j]; t.ld[j][0] = md[j]; }
+}
+
+// The selection of one volume: the map (T = uint8_t or uint16_t) and/or the keys used by the disparity-sharded
+// reduction; kList (an unblocked single-device context with the runner-up) also the runner-up into its result planes
+// ru, in the same read
+template <typename T, bool kList>
+__global__ void __launch_bounds__(256) wta_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin, int d_count,
+                                                  T* __restrict__ dis /* [H][W] or null */,
+                                                  unsigned long long* __restrict__ keys /* [H][W] or null */, const CostPlanes ru)
+{
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y;
+    if (x4 >= W) return;
+    const size_t plane = (size_t)H * Wp;
+    const float* p = vol + (size_t)y * Wp + x4;
+    float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+    int md[4] = {0, 0, 0, 0};
+    ScanTrack<false, kList> t;
+    wta_scan4(p, plane, d_begin, d_count, true, mc, md, t);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int x = x4 + j;
+        if (x < W) {
+            const size_t i = (size_t)y * W + x;
+            if (dis) dis[i] = (T)md[j];
+            if (keys) keys[i] = wta_key(mc[j], md[j]);
+            if constexpr (kList) {
+                int r;
+                float q;
+                runner_up_pick(t.lc[j], t.ld[j], md[j], r, q);
+                ru.plane(0)[i] = (float)r;
+                ru.plane(1)[i] = q;
+            }
         }
     }
 }
 
-// one pixel's step of wta_scan4_costs at slice d, the dl-th of the range, for the list scan (list_scan4) that tracks the
-// costs in the same read.  wta_scan4_costs keeps its own copy of these lines: calling this from it changes the SASS of
-// wta_fold_costs_kernel.
-__device__ __forceinline__ void costs_step(float c, int d, int dl, float nan, float& mc, int& md, float& lo, float& ce,
-                                           float& hi, float& prev, float& first)
-{
-    if (md == d - 1) hi = c;
-    if (d == 0) ce = c;
-    else if (c < mc) { mc = c; md = d; lo = prev; ce = c; hi = nan; }
-    prev = c;
-    if (dl == 0) first = c;
-}
-
-// wta_fold_kernel with the costs tracked in track[view] (the tracking planes).  Planes 0..2 hold the running winner's
-// (lo, ce, hi).  A block whose key is below the running key (the fold's own comparison) replaces them; its lo at its
-// first slice is the previous block's last cost (kCostLast).  A running winner on the previous block's last slice takes
-// hi from this block's first slice.  The first block starts from the no-winner state and, if write_first, records
-// kCostFirst.
-struct FoldCostParams {
-    FoldParams f;
-    CostPlanes track[2];
-    int write_first;
+// WTA of one block of slices of a blocked context (psm_create_blocked), both views in one launch (blockIdx.z = view):
+// wta_scan4 over the block's d_count slices starting at global d_begin, then its wta_key is stored (first block) or
+// folded into the running key by min.  The min over keys of consecutive blocks is the
+// selection over their union: the strict <, the lowest-d tie-break and +inf / NaN costs behave as in one scan.
+// kCosts: the costs in track[view] (the tracking planes).  Planes 0..2 hold the running winner's (lo, ce, hi).  A block
+// whose key is below the running key replaces them; its lo at its first slice is the previous block's last cost
+// (kCostLast).  A running winner on the previous block's last slice takes hi from this block's first slice.  The first
+// block starts from the no-winner state and, if write_first, records kCostFirst.
+// kList: the running list in list[view] (the head's key stays in the running keys): the block's list folds into it,
+// entry by entry, and only a list that changes is written back.
+struct FoldParams {
+    const float* vol[2];             // the block's filtered volumes [d_count][H][Wp]
+    unsigned long long* keys[2];     // running keys [H][W]
+    int W, H, Wp, d_begin, d_count, first;
+    CostPlanes track[2];             // kCosts
+    int write_first;                 // kCosts
+    CostPlanes list[2];              // kList
 };
 
-__global__ void __launch_bounds__(256) wta_fold_costs_kernel(const FoldCostParams P)
+template <bool kCosts, bool kList>
+__global__ void __launch_bounds__(256) wta_fold_kernel(const FoldParams P)
 {
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y, view = blockIdx.z;
-    if (x4 >= P.f.W) return;
-    const size_t plane = (size_t)P.f.H * P.f.Wp;
-    const float* p = (view ? P.f.vol[1] : P.f.vol[0]) + (size_t)y * P.f.Wp + x4;
-    unsigned long long* k = (view ? P.f.keys[1] : P.f.keys[0]) + (size_t)y * P.f.W;
-    const CostPlanes t = view ? P.track[1] : P.track[0];
-    const size_t row = (size_t)y * P.f.W;
-    const float nan = __uint_as_float(kCostNaNBits);
+    if (x4 >= P.W) return;
+    const size_t plane = (size_t)P.H * P.Wp;
+    const size_t row = (size_t)y * P.W;
+    // views selected, not indexed: a parameter array indexed by a run-time value is copied to the stack
+    const float* p = (view ? P.vol[1] : P.vol[0]) + (size_t)y * P.Wp + x4;
+    const CostPlanes tr = view ? P.track[1] : P.track[0];
     float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
     int md[4] = {0, 0, 0, 0};
-    float lo[4] = {nan, nan, nan, nan}, ce[4] = {nan, nan, nan, nan}, hi[4] = {nan, nan, nan, nan};
-    float prev[4] = {nan, nan, nan, nan}, first[4];
-    if (!P.f.first)
+    ScanTrack<kCosts, kList> t;
+    if constexpr (kCosts)
+        if (!P.first)
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-            if (x4 + j < P.f.W) prev[j] = t.plane(kCostLast)[row + x4 + j];
-    wta_scan4_costs(p, plane, P.f.d_begin, P.f.d_count, mc, md, lo, ce, hi, prev, first);
+            for (int j = 0; j < 4; ++j)
+                if (x4 + j < P.W) t.prev[j] = tr.plane(kCostLast)[row + x4 + j];
+    wta_scan4(p, plane, P.d_begin, P.d_count, true, mc, md, t);
+    unsigned long long* k = (view ? P.keys[1] : P.keys[0]) + row;
+    const CostPlanes L = view ? P.list[1] : P.list[0];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const int x = x4 + j;
-        if (x >= P.f.W) continue;
+        if (x >= P.W) continue;
         const size_t i = row + x;
-        const unsigned long long v = wta_key(mc[j], md[j]);
-        t.plane(kCostLast)[i] = prev[j];
-        bool win = true;
-        if (P.f.first) {
-            if (P.write_first) t.plane(kCostFirst)[i] = first[j];
-        } else {
-            const unsigned long long old = k[x];
-            win = v < old;
-            if (!win && (int)(unsigned)old == P.f.d_begin - 1) t.plane(2)[i] = first[j];
-        }
-        if (win) {
+        unsigned long long v = wta_key(mc[j], md[j]);
+        if constexpr (!kCosts && !kList) {
+            if (!P.first) {
+                const unsigned long long old = k[x];
+                v = old < v ? old : v;
+            }
             k[x] = v;
-            t.plane(0)[i] = lo[j]; t.plane(1)[i] = ce[j]; t.plane(2)[i] = hi[j];
+            continue;
+        }
+        const unsigned long long old = P.first ? 0ull : k[x];
+        if constexpr (kCosts) {
+            tr.plane(kCostLast)[i] = t.prev[j];
+            bool win = true;
+            if (P.first) {
+                if (P.write_first) tr.plane(kCostFirst)[i] = t.first[j];
+            } else {
+                win = v < old;
+                if (!win && (int)(unsigned)old == P.d_begin - 1) tr.plane(2)[i] = t.first[j];
+            }
+            if (win) {
+                if constexpr (!kList) k[x] = v;   // with the list, the merged head's key is written below
+                tr.plane(0)[i] = t.lo[j]; tr.plane(1)[i] = t.ce[j]; tr.plane(2)[i] = t.hi[j];
+            }
+        }
+        if constexpr (kList) {
+            float rc[kListLen];
+            int rd[kListLen];
+            if (P.first) {
+#pragma unroll
+                for (int e = 0; e < kListLen; ++e) { rc[e] = t.lc[j][e]; rd[e] = t.ld[j][e]; }
+            } else {
+                if (!(t.lc[j][0] < L.plane(kListCost + 3)[i])) continue;   // no entry of the block enters the running list
+                list_load(L, old, i, rc, rd);
+#pragma unroll
+                for (int e = 0; e < kListLen; ++e) list_insert(rc, rd, t.lc[j][e], t.ld[j][e]);
+            }
+            k[x] = wta_key(rc[0], rd[0]);
+            list_store(L, i, rc, rd);
         }
     }
 }
@@ -814,182 +903,6 @@ __global__ void __launch_bounds__(256) cost_write_kernel(const CostWriteParams P
     }
 }
 
-// ------------------------------------------------------------------------------------------
-// The runner-up away from the winner (PSM_OPT_RUNNER_UP).  The candidates are the arg-min's: d in [1, D) whose cost
-// compares below +inf, in the order of wta_key (the cost, -0 equal to +0, then the lowest d).  The runner-up r of a pixel
-// with map m is the first candidate with |d - m| >= 2, 0 when there is none; the result planes hold (float)r and q(r)
-// bit for bit (kCostNaN where r = 0).
-// Every path keeps, per pixel, the list of its four lowest candidates, lowest first, empty entries (+inf, 0) behind them.
-// Four are enough: at most three entries lie in {m - 1, m, m + 1}, so the first entry outside them is the lowest
-// candidate outside them.  The list is mergeable: the four lowest of a union of disjoint slice ranges are the four
-// lowest of the ranges' lists.  So a blocked walk folds each block's list into a running one, and the shards of a
-// multi-device context each pick from their own list and the first shard takes the lowest key of the picks.
-// ------------------------------------------------------------------------------------------
-// c at slice d into a sorted list whose entries all come from slices below d or cost less: the strict < puts it behind
-// every entry of equal cost, as the arg-min's lowest-d rule does, and a +inf or NaN cost never enters
-__device__ __forceinline__ void list_insert(float (&lc)[kListLen], int (&ld)[kListLen], float c, int d)
-{
-    const bool b0 = c < lc[0], b1 = c < lc[1], b2 = c < lc[2], b3 = c < lc[3];
-    lc[3] = b2 ? lc[2] : (b3 ? c : lc[3]);  ld[3] = b2 ? ld[2] : (b3 ? d : ld[3]);
-    lc[2] = b1 ? lc[1] : (b2 ? c : lc[2]);  ld[2] = b1 ? ld[1] : (b2 ? d : ld[2]);
-    lc[1] = b0 ? lc[0] : (b1 ? c : lc[1]);  ld[1] = b0 ? ld[0] : (b1 ? d : ld[1]);
-    lc[0] = b0 ? c : lc[0];                 ld[0] = b0 ? d : ld[0];
-}
-
-__device__ __forceinline__ void list_clear(float (&lc)[4][kListLen], int (&ld)[4][kListLen])
-{
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int e = 0; e < kListLen; ++e) { lc[j][e] = INFINITY; ld[j][e] = 0; }
-}
-
-// wta_scan4_costs's state of four pixels, for a list scan that also tracks the costs beside the winner
-struct CostTrack4 {
-    float mc[4];
-    int md[4];
-    float lo[4], ce[4], hi[4], prev[4], first[4];
-};
-
-// The lists of four pixels over slices [d_begin, d_begin + d_count), as wta_scan4 reads them (slice dl at p + dl * plane).
-// The head of each list is wta_scan4's (mc, md).  kCosts: t also takes wta_scan4_costs's steps, in the same read.
-template <bool kCosts>
-__device__ __forceinline__ void list_scan4(const float* p, size_t plane, int d_begin, int d_count, float (&lc)[4][kListLen],
-                                           int (&ld)[4][kListLen], CostTrack4* t)
-{
-    const float nan = __uint_as_float(kCostNaNBits);
-    int dl = (!kCosts && d_begin == 0) ? 1 : 0;  // global d = 0 is never a candidate (the costs scan still reads it)
-#pragma unroll 8
-    for (; dl < d_count; ++dl) {
-        const float4 c4 = __ldg(reinterpret_cast<const float4*>(p + (size_t)dl * plane));
-        const float c[4] = {c4.x, c4.y, c4.z, c4.w};
-        const int d = d_begin + dl;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            if constexpr (kCosts)
-                costs_step(c[j], d, dl, nan, t->mc[j], t->md[j], t->lo[j], t->ce[j], t->hi[j], t->prev[j], t->first[j]);
-            if (!kCosts || d != 0) list_insert(lc[j], ld[j], c[j], d);
-        }
-    }
-}
-
-// the runner-up of a pixel with map m from its list: (r, q(r)), or (0, kCostNaN)
-__device__ __forceinline__ void runner_up_pick(const float (&lc)[kListLen], const int (&ld)[kListLen], int m, int& r, float& q)
-{
-    r = 0;
-    q = __uint_as_float(kCostNaNBits);
-#pragma unroll
-    for (int e = kListLen - 1; e >= 0; --e)
-        if (ld[e] != 0 && abs(ld[e] - m) >= 2) { r = ld[e]; q = lc[e]; }
-}
-
-// The selection of an unblocked single-device context with the runner-up: wta_kernel's map (the lists' heads) and the
-// result planes, in one read of the volume.
-template <typename T>
-__global__ void __launch_bounds__(256) wta_runner_up_kernel(const float* __restrict__ vol, int W, int H, int Wp, int d_begin,
-                                                            int d_count, T* __restrict__ dis, const CostPlanes dst)
-{
-    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    const int y = blockIdx.y;
-    if (x4 >= W) return;
-    float lc[4][kListLen];
-    int ld[4][kListLen];
-    list_clear(lc, ld);
-    list_scan4<false>(vol + (size_t)y * Wp + x4, (size_t)H * Wp, d_begin, d_count, lc, ld, nullptr);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int x = x4 + j;
-        if (x >= W) continue;
-        const size_t i = (size_t)y * W + x;
-        int r;
-        float q;
-        runner_up_pick(lc[j], ld[j], ld[j][0], r, q);
-        dis[i] = (T)ld[j][0];
-        dst.plane(0)[i] = (float)r;
-        dst.plane(1)[i] = q;
-    }
-}
-
-// wta_fold_kernel with the running list in list[view] (the head's key stays in the running keys): the block's list
-// folds into it, entry by entry, and only a list that changes is written back.  kCosts: wta_fold_costs_kernel's
-// tracking too, from the same read, with its own key comparison.
-struct FoldListParams {
-    FoldParams f;
-    CostPlanes list[2];
-    CostPlanes track[2];   // kCosts
-    int write_first;       // kCosts
-};
-
-template <bool kCosts>
-__global__ void __launch_bounds__(256) wta_fold_list_kernel(const FoldListParams P)
-{
-    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-    const int y = blockIdx.y, view = blockIdx.z;
-    if (x4 >= P.f.W) return;
-    const size_t plane = (size_t)P.f.H * P.f.Wp;
-    const float* p = (view ? P.f.vol[1] : P.f.vol[0]) + (size_t)y * P.f.Wp + x4;
-    unsigned long long* k = (view ? P.f.keys[1] : P.f.keys[0]) + (size_t)y * P.f.W;
-    const CostPlanes L = view ? P.list[1] : P.list[0];
-    const size_t row = (size_t)y * P.f.W;
-    float lc[4][kListLen];
-    int ld[4][kListLen];
-    list_clear(lc, ld);
-    CostTrack4 t;
-    if constexpr (kCosts) {
-        const CostPlanes tr = view ? P.track[1] : P.track[0];
-        const float nan = __uint_as_float(kCostNaNBits);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            t.mc[j] = INFINITY; t.md[j] = 0; t.lo[j] = t.ce[j] = t.hi[j] = t.prev[j] = nan;
-            if (!P.f.first && x4 + j < P.f.W) t.prev[j] = tr.plane(kCostLast)[row + x4 + j];
-        }
-    }
-    list_scan4<kCosts>(p, plane, P.f.d_begin, P.f.d_count, lc, ld, &t);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int x = x4 + j;
-        if (x >= P.f.W) continue;
-        const size_t i = row + x;
-        const unsigned long long old = P.f.first ? 0ull : k[x];
-        if constexpr (kCosts) {   // wta_fold_costs_kernel's epilogue, but the key is written below
-            const CostPlanes tr = view ? P.track[1] : P.track[0];
-            tr.plane(kCostLast)[i] = t.prev[j];
-            bool win = true;
-            if (P.f.first) {
-                if (P.write_first) tr.plane(kCostFirst)[i] = t.first[j];
-            } else {
-                win = wta_key(t.mc[j], t.md[j]) < old;
-                if (!win && (int)(unsigned)old == P.f.d_begin - 1) tr.plane(2)[i] = t.first[j];
-            }
-            if (win) { tr.plane(0)[i] = t.lo[j]; tr.plane(1)[i] = t.ce[j]; tr.plane(2)[i] = t.hi[j]; }
-        }
-        float rc[kListLen];
-        int rd[kListLen];
-        if (P.f.first) {
-#pragma unroll
-            for (int e = 0; e < kListLen; ++e) { rc[e] = lc[j][e]; rd[e] = ld[j][e]; }
-        } else {
-            rc[3] = L.plane(kListCost + 3)[i];
-            if (!(lc[j][0] < rc[3])) continue;   // no entry of the block enters the running list
-            rd[0] = (int)(unsigned)old;
-            rc[0] = L.plane(kListCost)[i];
-#pragma unroll
-            for (int e = 1; e < kListLen; ++e) {
-                if (e < 3) rc[e] = L.plane(kListCost + e)[i];
-                rd[e] = (int)L.uplane(kListD + e - 1)[i];
-            }
-#pragma unroll
-            for (int e = 0; e < kListLen; ++e) list_insert(rc, rd, lc[j][e], ld[j][e]);
-        }
-        k[x] = wta_key(rc[0], rd[0]);
-#pragma unroll
-        for (int e = 0; e < kListLen; ++e) {
-            L.plane(kListCost + e)[i] = rc[e];
-            if (e > 0) L.uplane(kListD + e - 1)[i] = (unsigned)rd[e];
-        }
-    }
-}
-
 // The runner-up of the slices a context owns, from the complete selection map (T): from a list scan of its resident
 // volume (kTracked = false: an unblocked shard) or from its running list (kTracked = true: a blocked context).  Into the
 // result planes, or, where slots.base is set (a shard of a multi-device context), into slot `slot` of the first shard's
@@ -1011,23 +924,15 @@ __global__ void __launch_bounds__(256) runner_up_write_kernel(const RunnerUpWrit
     const int y = blockIdx.y;
     if (x4 >= P.W) return;
     const size_t row = (size_t)y * P.W;
-    float lc[4][kListLen];
-    int ld[4][kListLen];
-    list_clear(lc, ld);
+    ScanTrack<false, true> t;
     if constexpr (!kTracked) {
-        list_scan4<false>(P.vol + (size_t)y * P.Wp + x4, (size_t)P.H * P.Wp, P.d_begin, P.d_count, lc, ld, nullptr);
+        float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
+        int md[4] = {0, 0, 0, 0};
+        wta_scan4(P.vol + (size_t)y * P.Wp + x4, (size_t)P.H * P.Wp, P.d_begin, P.d_count, true, mc, md, t);
     } else {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            if (x4 + j >= P.W) continue;
-            const size_t i = row + x4 + j;
-            ld[j][0] = (int)(unsigned)P.keys[i];
-#pragma unroll
-            for (int e = 0; e < kListLen; ++e) {
-                lc[j][e] = P.list.plane(kListCost + e)[i];
-                if (e > 0) ld[j][e] = (int)P.list.uplane(kListD + e - 1)[i];
-            }
-        }
+        for (int j = 0; j < 4; ++j)
+            if (x4 + j < P.W) list_load(P.list, P.keys[row + x4 + j], row + x4 + j, t.lc[j], t.ld[j]);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -1036,7 +941,7 @@ __global__ void __launch_bounds__(256) runner_up_write_kernel(const RunnerUpWrit
         const size_t i = row + x;
         int r;
         float q;
-        runner_up_pick(lc[j], ld[j], static_cast<const T*>(P.map)[i], r, q);
+        runner_up_pick(t.lc[j], t.ld[j], static_cast<const T*>(P.map)[i], r, q);
         if (P.slots.base) {
             P.slots.key(P.slot)[i] = r ? wta_key(q, r) : wta_key(INFINITY, 0);
             P.slots.cost(P.slot)[i] = q;
@@ -1181,7 +1086,8 @@ __global__ void __launch_bounds__(256) wta_scatter_kernel(const float* __restric
         const float* p = vol + (size_t)y * Wp + (active ? x4 : 0);
         float mc[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
         int md[4] = {0, 0, 0, 0};
-        wta_scan4(p, plane, d_begin, d_count, active, mc, md);
+        ScanTrack<false, false> none;
+        wta_scan4(p, plane, d_begin, d_count, active, mc, md, none);
         p2p_store_row(stage[warp], peers, W, y, x4 - 4 * lane, lane,
                       [&](int j) { return wta_key(mc[j], md[j]); });
     }

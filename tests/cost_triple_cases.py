@@ -5,9 +5,10 @@ The definition is a gather from the filtered volume: for the selection map m, pl
 and the quiet NaN 0x7FC00000 where m + k - 1 lies outside [0, D).  The library never holds the whole volume on a blocked
 or multi-device context, so it computes the same planes in pieces.  This module restates both:
   - gather: the definition;
-  - track: wta_fold_costs_kernel's walk of a blocked context (block folds with the seam rules: a block winning on its first
-    slice takes q(m - 1) from the previous block's last slice, a running winner on the previous block's last slice takes
-    q(m + 1) from this block's first slice, the first block starts from the no-winner state (NaN, q(0), q(1)));
+  - track: wta_fold_kernel<kCosts>'s walk of a blocked context (block folds with the seam rules: a block winning on its
+    first slice takes q(m - 1) from the previous block's last slice, a running winner on the previous block's last
+    slice takes q(m + 1) from this block's first slice, the first block starts from the no-winner state (NaN, q(0),
+    q(1)));
   - multi: cost_write_kernel's ownership on a multi-device context, every shard writing the entries it owns (unblocked
     shards from their slices, blocked shards from their tracking planes and first / last slice costs), each entry counted.
 Every plane is a uint32 bit pattern, so NaN payloads and the sign of zero are compared exactly."""
@@ -43,7 +44,7 @@ def gather(vol, m, d0=0, D=None):
 
 
 def track(vol, blocks, d0=0):
-    """wta_fold_costs_kernel over blocks [(d_begin, d_count), ...] (ascending, contiguous) of vol (slices d0 ..) ->
+    """wta_fold_kernel<kCosts> over blocks [(d_begin, d_count), ...] (ascending, contiguous) of vol (slices d0 ..) ->
     (running keys, uint32 planes [5, H, W]: lo, ce, hi, the last slice's cost, the first slice's cost)"""
     f = np.ascontiguousarray(vol, np.float32)
     b32 = f.view(U32)

@@ -7,8 +7,8 @@ candidate with |d - m| >= 2, 0 when there is none.  The planes hold r as a float
 0x7FC00000 where r = 0.  The library never scans for r directly: every path keeps a per-pixel list of the four lowest
 candidates and picks r from it.  This module restates both:
   - definition: a direct scan given m;
-  - scan_list / pick: the list of one scan (list_scan4) and the pick from it (runner_up_pick);
-  - fold: a blocked walk (wta_fold_list_kernel), each block's list inserted entry by entry into the running one;
+  - scan_list / pick: the list of one scan (wta_scan4 with the list tracked) and the pick from it (runner_up_pick);
+  - fold: a blocked walk (wta_fold_kernel<kList>), each block's list inserted entry by entry into the running one;
   - multi: a multi-device context, every shard picking from its own list into its slot and the first shard taking the
     first slot of the lowest key (runner_up_write_kernel, runner_up_reduce_kernel).
 Every plane is a uint32 bit pattern, so NaN payloads and the sign of zero are compared exactly."""
@@ -79,7 +79,7 @@ def head_key(lc, ld):
 
 
 def fold(vol, blocks, d0=0):
-    """wta_fold_list_kernel over blocks [(d_begin, d_count), ...] (ascending, contiguous) of vol (slices d0 ..) -> the
+    """wta_fold_kernel<kList> over blocks [(d_begin, d_count), ...] (ascending, contiguous) of vol (slices d0 ..) -> the
     running list; a block whose head does not compare below the running list's last entry leaves it as it is"""
     f = np.ascontiguousarray(vol, np.float32)
     run = None

@@ -1,10 +1,11 @@
 """CPU model of disparity selection through packed keys (test_selection_model.py on the CPU, test_gpu_selection_seams.py on
 the device).
 
-Every selection path of the library ends in a packed key per pixel, (float_order_key(cost) << 32) | d: wta_kernel's keys
-for disparity shards, wta_fold_kernel's running keys of a blocked context, the keys a multi-device context's shards
-exchange.  The min over keys of disjoint slice ranges is claimed to be the winner-take-all over their union (strict <,
-lowest d on ties, +inf and NaN never win, global d = 0 never a candidate).  This module restates the key
+Every selection path of the library ends in a packed key per pixel, (float_order_key(cost) << 32) | d:
+wta_kernel<T, false>'s keys for disparity shards, wta_fold_kernel<false, false>'s running keys of a blocked context, the
+keys a multi-device context's shards exchange.  The min over keys of disjoint slice ranges is claimed to be the
+winner-take-all over their union (strict <, lowest d on ties, +inf and NaN never win, global d = 0 never a candidate).
+This module restates the key
 (psm_common.cuh::float_order_key), the one-scan key of a range of slices, the fold over a partition of the range, and
 the partitions the library makes: blocks of a blocked context (block_at) and shards (sharding.shard_range)."""
 import numpy as np

@@ -1,6 +1,6 @@
 """CPU-only, world_size 2 over gloo: the host-side logic of the disparity-sharded path --
 shard ranges and the packed-key exchange whose min reproduces the reference's WTA tie-break.
-The key packing below emulates, in numpy, what wta_kernel emits on the device."""
+The key packing below emulates, in numpy, what wta_kernel<T, false> emits on the device."""
 import os
 
 import numpy as np
