@@ -24,6 +24,8 @@
  *   psm_set_lr_check      <-> PP::processDM's lrCheck + fillInv (commented out there)  src/PP.cpp:17-143, :405-406
  *   psm_set_speckle_filter <-> cv::filterSpeckles, as the reference's StereoSGBM matcher configures it (speckleWindowSize,
  *                             speckleRange)                       src/StereoMatch.cpp:654-655
+ *   psm_reproject_device  <-> cv::reprojectImageTo3D with the rig's Q (camProps.Q, computed and never read there)
+ *                                                                 src/StereoMatch.cpp:456-457
  *   psm_read_cost_slice   <-> DispEst::printCV (cost-slice dump) src/DispEst.cpp:181-194
  *   psm_stage_ms          <-> cvc_time/cvf_time/dispsel_time     src/StereoMatch.cpp:209-241
  *
@@ -57,7 +59,8 @@
  * (its buffers and, after a change of sigma or weight type, the weight table; with psm_set_speckle_filter on, the
  * labels and counts, 8 * W * H bytes per view, and with PSM_SPECKLE_FIRST and a check mode, a map pair between the
  * removal and the check), psm_set_option(PSM_OPT_COSTS, 1) (the
- * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots).  Run them once before a
+ * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots), psm_reproject_device with
+ * handle_missing (8 bytes of scratch).  Run them once before a
  * latency-critical
  * loop.  psm_set_stream always waits for the stream it leaves.
  */
@@ -566,6 +569,33 @@ int psm_read_costs(psm_ctx* ctx, int view, float* dst, size_t row_step);
  * psm_copy_costs_device / psm_read_costs, with PSM_OPT_RUNNER_UP in place of PSM_OPT_COSTS. */
 int psm_copy_runner_up_device(psm_ctx* ctx, float* d_left, float* d_right, size_t row_step);
 int psm_read_runner_up(psm_ctx* ctx, int view, float* dst, size_t row_step);
+
+/* The 3D point of every pixel of a map (OpenCV's cv::reprojectImageTo3D(map, xyz, Q, handleMissingValues) with a map of
+ * integer disparities), for the rig's 4 x 4 reprojection matrix Q (row-major doubles, as cv::stereoRectify returns it);
+ * the reference computes Q (src/StereoMatch.cpp:456-457, camProps.Q) and never reads it.  Per requested view, X, Y, Z
+ * interleaved as float32 (CV_32FC3: 12 bytes per pixel), rows row_step bytes apart.  For pixel (x, y) with map value d,
+ * in fp64 with each product and sum rounded on its own (no fused multiply-add) and the sum started from +0.0:
+ *     h[i] = (((+0.0 + Q[i][0] x) + Q[i][1] y) + Q[i][2] d) + Q[i][3],  r = 1 / h[3] (correctly rounded),
+ *     X = (float)((double)(float)h[0] * r), Y and Z likewise from h[1] and h[2];
+ * with handle_missing = 1, Z = 10000 wherever d equals the minimum of that view's map (OpenCV takes the minimum for the
+ * missing value, zero or not).  This is cv2's result bit for bit, except that a NaN (0 * inf, a NaN in Q) may carry
+ * another payload.  Q may hold any doubles (0, +-inf, NaN): the result is what IEEE arithmetic gives.
+ * which = 0: the maps of the last selection stage (a fused-exchange context's complete maps; a range context's absolute
+ * disparities); which = 1: the post-processed maps -- as psm_copy_maps_device reads them.  A multi-device context
+ * reprojects the first shard's.  The maps, masks, costs and runner-up are not touched.
+ * psm_reproject_device: a view is reprojected when both its Q and its DEVICE point buffer are given; one launch covers
+ * every requested view, plus one launch in front of it with handle_missing (the maps' minima, into context scratch), on
+ * the context's stream, asynchronous; psm_launch_count counts them (a fused-exchange context's first reader of a frame
+ * also enqueues the exchange wait, as psm_copy_maps_device does).  psm_read_points: one view into HOST memory through
+ * a context-owned device buffer of 12 * W * H bytes (allocated on first use), then synchronises.
+ *   - PSM_EINVAL before any CUDA work, with nothing changed: a Q without a point buffer or a buffer without a Q, no view
+ *     requested, which not 0 / 1, handle_missing not 0 / 1, a bad view, row_step below 12 * W, a buffer or row_step that
+ *     is not a multiple of 4 bytes.
+ *   - PSM_ESTATE: no selection (which = 0) or post-process (which = 1) yet, as for psm_copy_maps_device; the right view
+ *     on a left-only context.  See DESIGN.md section 24. */
+int psm_reproject_device(psm_ctx* ctx, int which, const double* q_left, const double* q_right, int handle_missing,
+                         float* d_left, float* d_right, size_t row_step);
+int psm_read_points(psm_ctx* ctx, int which, int view, const double q[16], int handle_missing, float* dst, size_t row_step);
 
 /* Sharded stage 3a: per-pixel packed minima over this context's slices, written to DEVICE
  * buffers of H*W uint64 each:  key = (order_preserving_u32(cost) << 32) | global_d.

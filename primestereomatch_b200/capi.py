@@ -24,7 +24,7 @@ SYMBOLS = [
     "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
     "psm_create_blocked", "psm_create_multi", "psm_set_images_device_planes", "psm_wait_stream", "psm_signal_stream",
     "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs", "psm_copy_runner_up_device", "psm_read_runner_up",
-    "psm_create_range", "psm_set_speckle_filter",
+    "psm_create_range", "psm_set_speckle_filter", "psm_reproject_device", "psm_read_points",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -93,6 +93,8 @@ def lib():
     L.psm_read_costs.argtypes = [vp, i, fp, sz]
     L.psm_copy_runner_up_device.argtypes = [vp, fp, fp, sz]
     L.psm_read_runner_up.argtypes = [vp, i, fp, sz]
+    L.psm_reproject_device.argtypes = [vp, i, vp, vp, i, fp, fp, sz]
+    L.psm_read_points.argtypes = [vp, i, i, vp, i, fp, sz]
     L.psm_set_images_async.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_u8_async.argtypes = [vp, u8p, sz, u8p, sz]
     L.psm_set_images_commit.argtypes = [vp]

@@ -21,6 +21,7 @@
 #include "psm_fgf.cuh"
 #include "psm_lr.cuh"
 #include "psm_speckle.cuh"
+#include "psm_reproject.cuh"
 
 #ifndef PSM_BUILD_FLAGS
 #define PSM_BUILD_FLAGS "unknown"
@@ -166,6 +167,8 @@ struct psm_ctx {
     unsigned p2p_seq_right = 0;                // frames whose exchange included the right view (p2p_seq counts every frame)
     bool p2p_right_current = false;            // the last frame's exchange included the right view
     bool have_pp = false;                      // dis_pp holds the maps of a post-process since the last PSM_OPT_VIEWS change
+    unsigned* rp_min = nullptr;                // psm_reproject_device with handle_missing: each requested map's minimum, lazy
+    float* rp_buf = nullptr;                   // psm_read_points: one view's points (12 * W * H bytes), lazy
     cudaEvent_t ev_user = nullptr;             // psm_wait_stream: the caller's stream, recorded
     cudaEvent_t ev_signal[2] = {nullptr, nullptr};  // psm_signal_stream: the compute and the copy stream, recorded
     uint64_t launches = 0;
@@ -1460,6 +1463,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->pp_packed); cudaFree(c->pp_lut);
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
     cudaFree(c->sp_lab); cudaFree(c->sp_cnt);
+    cudaFree(c->rp_min); cudaFree(c->rp_buf);
     for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]);
                                    cudaFree(c->sp_maps[v]);
                                    cudaFree(c->track[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]);
@@ -2439,24 +2443,151 @@ int psm_post_process_u16(psm_ctx* c, uint16_t* left, size_t left_step, uint16_t*
     return post_process(c, left, left_step, right, right_step);
 }
 
+// `which` of a map call `call`: PSM_EINVAL unless 0 (the selection maps) or 1 (the post-processed maps)
+static int check_which(psm_ctx* c, const char* call, int which)
+{
+    if (which != 0 && which != 1)
+        return fail(c, PSM_EINVAL, "%s: which %d is neither 0 (selection maps) nor 1 (post-processed maps)", call, which);
+    return PSM_OK;
+}
+
+// the maps `which` names for a reader `call` on a single-device context (bound): the selection maps, with the wait for
+// the exchanged maps enqueued in front of the reader, or the post-processed maps
+static int result_maps(psm_ctx* c, const char* call, int which, const uint8_t* maps[2])
+{
+    if (int rc = check_stages_reset(c, call)) return rc;
+    maps[0] = c->dis_pp[0]; maps[1] = c->dis_pp[1];
+    if (which == 0) {
+        if (int rc = selection_maps(c, call, maps)) return rc;
+        return p2p_wait_done(c);
+    }
+    if (!c->have_pp) return fail(c, PSM_ESTATE, "%s of the post-processed maps before a post-process", call);
+    return PSM_OK;
+}
+
 int psm_copy_maps_device(psm_ctx* c, int which, void* d_left, size_t left_step, void* d_right, size_t right_step)
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (which != 0 && which != 1)
-        return fail(c, PSM_EINVAL, "psm_copy_maps_device: which %d is neither 0 (selection maps) nor 1 (post-processed maps)", which);
+    if (int rc = check_which(c, "psm_copy_maps_device", which)) return rc;
     if (int rc = check_map_dst(c, "psm_copy_maps_device", d_left, left_step, d_right, right_step)) return rc;
     // a multi-device context's maps are the first shard's (its exchange block, and its post-filter's outputs)
     if (is_multi(c)) return relay(c, 0, psm_copy_maps_device(c->shard[0], which, d_left, left_step, d_right, right_step));
     if (int rc = bind(c)) return rc;
-    if (int rc = check_stages_reset(c, "psm_copy_maps_device")) return rc;
-    const uint8_t* maps[2] = {c->dis_pp[0], c->dis_pp[1]};
-    if (which == 0) {
-        if (int rc = selection_maps(c, "psm_copy_maps_device", maps)) return rc;
-        if (int rc = p2p_wait_done(c)) return rc;
-    } else if (!c->have_pp) {
-        return fail(c, PSM_ESTATE, "psm_copy_maps_device of the post-processed maps before a post-process");
-    }
+    const uint8_t* maps[2];
+    if (int rc = result_maps(c, "psm_copy_maps_device", which, maps)) return rc;
     return copy_maps_out(c, maps, d_left, left_step, d_right, right_step, cudaMemcpyDefault, false);
+}
+
+}  // extern "C"
+
+// the points of each requested view v (q[v] given) of maps[v] into out[v]: with handle_missing the maps' minima first,
+// then one launch over every requested view
+template <typename T>
+static int reproject_maps(psm_ctx* c, const uint8_t* const maps[2], const double* const q[2], int handle_missing,
+                          float* const out[2], size_t row_step)
+{
+    ReprojArgs<T> a = {};
+    unsigned nz = 0;   // the launch's slots: the requested views in order
+    for (int v = 0; v < 2; ++v) {
+        if (!q[v]) continue;
+        a.map[nz] = reinterpret_cast<const T*>(maps[v]);
+        a.out[nz] = out[v];
+        std::memcpy(a.q[nz], q[v], sizeof a.q[nz]);
+        ++nz;
+    }
+    a.row_step = row_step;
+    a.W = c->W;
+    a.H = c->H;
+    if (handle_missing) {
+        PSM_CUDA(c, alloc_if_null(c->rp_min, 2 * sizeof(unsigned)));
+        PSM_CUDA(c, cudaMemsetAsync(c->rp_min, 0xff, 2 * sizeof(unsigned), c->stream));
+        const size_t npix = (size_t)c->W * c->H;
+        const unsigned grid = (unsigned)std::min<size_t>(kRpMinBlocks, (npix + kRpThreads - 1) / kRpThreads);
+        reproject_min_kernel<T><<<dim3(grid, 1, nz), kRpThreads, 0, c->stream>>>(a, c->rp_min);
+        PSM_LAUNCH_CHECK(c);
+        a.minv = c->rp_min;
+    }
+    const unsigned segs = (unsigned)((c->W + kRpPix - 1) / kRpPix);
+    reproject_kernel<T><<<dim3(segs * (unsigned)c->H, 1, nz), kRpThreads, 0, c->stream>>>(a, segs);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
+// the arguments of psm_reproject_device / psm_read_points `call`, before any CUDA work: a view is requested when its Q
+// and its point buffer are both given
+static int check_reproject_args(psm_ctx* c, const char* call, int which, const double* const q[2], int handle_missing,
+                                float* const out[2], size_t row_step)
+{
+    if (int rc = check_which(c, call, which)) return rc;
+    if (handle_missing != 0 && handle_missing != 1)
+        return fail(c, PSM_EINVAL, "%s: handle_missing %d is neither 0 nor 1", call, handle_missing);
+    for (int v = 0; v < 2; ++v)
+        if (!q[v] != !out[v])
+            return fail(c, PSM_EINVAL, "%s: the %s view has %s; give both or neither", call, v ? "right" : "left",
+                        q[v] ? "a Q without a point buffer" : "a point buffer without a Q");
+    if (!q[0] && !q[1]) return fail(c, PSM_EINVAL, "%s: no view requested (no Q and point buffer given)", call);
+    const size_t row = (size_t)c->W * 3 * sizeof(float);
+    const auto misaligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; };
+    if (row_step < row || row_step % 4 || misaligned(out[0]) || misaligned(out[1]))
+        return fail(c, PSM_EINVAL, "%s: bad point buffer/row_step (row_step must be a multiple of 4 and at least 12 * W = "
+                    "%zu bytes, buffers 4-byte aligned)", call, row);
+    return PSM_OK;
+}
+
+// the maps `which` names and the requested views' state, on a bound single-device context
+static int reproject_maps_of(psm_ctx* c, const char* call, int which, const double* const q[2], const uint8_t* maps[2])
+{
+    if (q[1])
+        if (int rc = check_right_view(c, call)) return rc;
+    return result_maps(c, call, which, maps);
+}
+
+static int reproject_run(psm_ctx* c, const uint8_t* const maps[2], const double* const q[2], int handle_missing,
+                         float* const out[2], size_t row_step)
+{
+    return c->map_bytes == 2 ? reproject_maps<uint16_t>(c, maps, q, handle_missing, out, row_step)
+                             : reproject_maps<uint8_t>(c, maps, q, handle_missing, out, row_step);
+}
+
+extern "C" {
+
+int psm_reproject_device(psm_ctx* c, int which, const double* q_left, const double* q_right, int handle_missing,
+                         float* d_left, float* d_right, size_t row_step)
+{
+    static const char* call = "psm_reproject_device";
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    const double* const q[2] = {q_left, q_right};
+    float* const out[2] = {d_left, d_right};
+    if (int rc = check_reproject_args(c, call, which, q, handle_missing, out, row_step)) return rc;
+    if (is_multi(c))
+        return relay(c, 0, psm_reproject_device(c->shard[0], which, q_left, q_right, handle_missing, d_left, d_right, row_step));
+    if (int rc = bind(c)) return rc;
+    const uint8_t* maps[2];
+    if (int rc = reproject_maps_of(c, call, which, q, maps)) return rc;
+    return reproject_run(c, maps, q, handle_missing, out, row_step);
+}
+
+int psm_read_points(psm_ctx* c, int which, int view, const double q_view[16], int handle_missing, float* dst, size_t row_step)
+{
+    static const char* call = "psm_read_points";
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "%s: bad view %d", call, view);
+    const double* q[2] = {nullptr, nullptr};
+    float* out[2] = {nullptr, nullptr};
+    q[view] = q_view;
+    out[view] = dst;
+    if (int rc = check_reproject_args(c, call, which, q, handle_missing, out, row_step)) return rc;
+    if (is_multi(c)) return relay(c, 0, psm_read_points(c->shard[0], which, view, q_view, handle_missing, dst, row_step));
+    if (int rc = bind(c)) return rc;
+    const uint8_t* maps[2];
+    if (int rc = reproject_maps_of(c, call, which, q, maps)) return rc;
+    const size_t row = (size_t)c->W * 3 * sizeof(float);
+    PSM_CUDA(c, alloc_if_null(c->rp_buf, row * c->H));
+    out[view] = c->rp_buf;
+    if (int rc = reproject_run(c, maps, q, handle_missing, out, row)) return rc;
+    PSM_CUDA(c, cudaMemcpy2DAsync(dst, row_step, c->rp_buf, row, row, c->H, cudaMemcpyDeviceToHost, c->stream));
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    return PSM_OK;
 }
 
 // output o of the last selection stage, for its copy-out call `call`

@@ -330,6 +330,26 @@ class DispEst:
                 capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)
         return 0
 
+    _VIEW = {"left": capi.PSM_LEFT, "right": capi.PSM_RIGHT}
+    _WHICH = {"selection": 0, "post": 1}
+
+    def reproject(self, Q, view="left", which="post", handle_missing=False):
+        """OpenCV's reprojectImageTo3D(map, xyz, Q, handleMissingValues) of one view's map on the device
+        (psm_read_points) -> (H, W, 3) float32 X, Y, Z, bit for bit as cv2 computes them (NaN payloads aside).  Q: the
+        rig's 4 x 4 reprojection matrix (stereoRectify's Q); view: "left" or "right"; which: "post" (the maps of the
+        last PostProcess_GPU) or "selection" (those of the last DispSelect_GPU); handle_missing: Z = 10000 wherever the
+        map holds its minimum.  Raises PsmError (PSM_ESTATE) before the stage that makes the maps has run."""
+        self._need_gpu()
+        q = np.ascontiguousarray(np.asarray(Q, np.float64).reshape(4, 4))
+        if not isinstance(handle_missing, bool):
+            raise TypeError(f"handle_missing must be True or False (got {handle_missing!r})")
+        view_id = self._VIEW.get(view, -1) if isinstance(view, str) else -1
+        which_id = self._WHICH.get(which, -1) if isinstance(which, str) else -1
+        out = np.empty((self.hei, self.wid, 3), np.float32)
+        capi.check(self._lib.psm_read_points(self._ctx, which_id, view_id, _ptr(q), int(handle_missing), _ptr(out),
+                                             out.strides[0]), self._ctx)
+        return out
+
     def CostConst(self):
         raise NotImplementedError("CPU stage (reference src/CVC.cpp) is not part of this package")
 

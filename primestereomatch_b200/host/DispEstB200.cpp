@@ -132,6 +132,13 @@ int DispEst::read_planes(int view, int n, int (*read)(psm_ctx*, int, float*, siz
 }
 
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
+int DispEst::reprojectImageTo3D(cv::Mat& xyz, const double Q[16], bool handleMissingValues, int view, bool postProcessed)
+{
+    if (!ctx) return -1;
+    if (xyz.rows != hei || xyz.cols != wid || xyz.type() != CV_32FC3 || !xyz.data) xyz.create(hei, wid, CV_32FC3);
+    return psm_read_points(ctx, postProcessed ? 1 : 0, view, Q, handleMissingValues ? 1 : 0, xyz.ptr<float>(), xyz.step);
+}
+
 int DispEst::printCV(void)
 {
     if (!ctx) return -1;

@@ -125,6 +125,12 @@ public:
     // be CostConst_GPU.  Fails on a context that owns part of the disparity range.
     int setRunnerUpOutput(bool on);
     int printCV(void);
+    // OpenCV's reprojectImageTo3D(disp, xyz, Q, handleMissingValues) of one view's map (PSM_LEFT / PSM_RIGHT) on the
+    // device, bit for bit (psm_read_points): xyz becomes H x W CV_32FC3 (X, Y, Z).  Q: the rig's 4 x 4 reprojection
+    // matrix, row-major (stereoRectify's Q, the reference's camProps.Q).  postProcessed: the maps of the last
+    // PostProcess_GPU, else those of the last DispSelect_GPU.
+    int reprojectImageTo3D(cv::Mat& xyz, const double Q[16], bool handleMissingValues = false, int view = PSM_LEFT,
+                           bool postProcessed = true);
 
     // GPU stages (the path behind the `m` toggle): 0 = success, as in the reference
     int CostConst_GPU();

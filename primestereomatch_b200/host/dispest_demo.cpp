@@ -11,7 +11,9 @@
 // `--block-slices N` runs a blocked context (psm_create_blocked) that holds N disparity slices at a time, a leading
 // `--devices 0,1,...` a context over those CUDA devices (two or more ids: psm_create_multi; ids may repeat), a leading
 // `--min-disp N` a context over disparities [N, D) alone (psm_create_range; the maps hold absolute disparities), a
-// leading `--speckle MODE SIZE DIFF` speckle removal (setSpeckleFilter: MODE 0 off, 1 first, 2 only).  A leading
+// leading `--speckle MODE SIZE DIFF` speckle removal (setSpeckleFilter: MODE 0 off, 1 first, 2 only), a leading
+// `--points Q.f64 out.xyz` the left view's 3D points of the final maps (reprojectImageTo3D with the 16 native-endian
+// doubles of Q.f64, row-major): out.xyz holds H x W x 3 native float32 X, Y, Z.  A leading
 // `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.
 #include <cstdio>
 #include <cstdlib>
@@ -33,6 +35,7 @@ int main(int argc, char** argv)
 {
     int block_slices = 0, min_disp = 0;
     int speckle[3] = {0, 0, 0};   // mode, max_size, max_diff
+    const char* points[2] = {nullptr, nullptr};   // Q file, output file
     std::vector<int> devices;
     const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
     if (left_only) {
@@ -41,7 +44,17 @@ int main(int argc, char** argv)
         --argc;
     }
     while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices") ||
-                         !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle"))) {
+                         !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle") ||
+                         !std::strcmp(argv[1], "--points"))) {
+        if (!std::strcmp(argv[1], "--points")) {
+            if (argc < 4) break;
+            points[0] = argv[2];
+            points[1] = argv[3];
+            argv[3] = argv[0];
+            argv += 3;
+            argc -= 3;
+            continue;
+        }
         if (!std::strcmp(argv[1], "--speckle")) {
             if (argc < 5) break;
             for (int k = 0; k < 3; ++k) speckle[k] = std::atoi(argv[2 + k]);
@@ -67,7 +80,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--points Q.f64 out.xyz] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -95,11 +108,18 @@ int main(int argc, char** argv)
     if (!rc) rc = SMDE->CostFilter_GPU();
     if (!rc) rc = SMDE->DispSelect_GPU();
     if (!rc) rc = SMDE->PostProcess_GPU();
+    cv::Mat xyz;
+    if (!rc && points[0]) {
+        double Q[16];
+        if (!read_all(points[0], Q, sizeof Q)) { std::fprintf(stderr, "bad Q file %s\n", points[0]); return 2; }
+        rc = SMDE->reprojectImageTo3D(xyz, Q);
+    }
     if (rc) { std::fprintf(stderr, "stage failed (%d): %s\n", rc, SMDE->last_error()); return 1; }
     std::printf("CVC %.3f ms  CVF %.3f ms  DispSel %.3f ms  PP %.3f ms\n", SMDE->stage_ms(1), SMDE->stage_ms(2), SMDE->stage_ms(3), SMDE->stage_ms(5));
     const size_t bytes = SMDE->lDisMap.step * H;   // dense rows: W * 1 or W * 2 bytes
     FILE* f = std::fopen(argv[6], "wb"); std::fwrite(SMDE->lDisMap.data, 1, bytes, f); std::fclose(f);
     if (!left_only) { f = std::fopen(argv[7], "wb"); std::fwrite(SMDE->rDisMap.data, 1, bytes, f); std::fclose(f); }
+    if (points[1]) { f = std::fopen(points[1], "wb"); std::fwrite(xyz.data, 1, xyz.step * H, f); std::fclose(f); }
     delete SMDE;
     return 0;
 }

@@ -9,6 +9,7 @@ the host upload of the same pixels.  Importing this module imports torch; the pa
 """
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import capi
@@ -152,7 +153,8 @@ class TorchStereo:
                 raise ValueError(f"{name} is on {t.device}: frames must be CUDA tensors on the context's device {self.device}")
         return pix, lf, other[1], row_step, col_step, batched
 
-    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False, costs=False, runner_up=False):
+    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False, costs=False, runner_up=False,
+              points=None, handle_missing=False):
         """Disparity maps of one frame pair or a batch -> (lmap, rmap): new uint8 / uint16 tensors of shape (H, W) or
         (B, H, W) on the context's device; rmap is None on a left-only context.
 
@@ -166,14 +168,32 @@ class TorchStereo:
         disparity r (0 where none exists), plane 1 its filtered cost bit for bit (the quiet NaN 0x7FC00000 where r = 0);
         rrunner is None on a left-only context.  The option is set when runner_up differs from the last call's.
 
+        points=(Q_left, Q_right) -> also (lpts, rpts), appended last: OpenCV's reprojectImageTo3D of the maps this call
+        returns (post-processed or selection) with each view's 4 x 4 reprojection matrix (psm_reproject_device), new
+        float32 tensors (H, W, 3) or (B, H, W, 3) of X, Y, Z; either Q may be None, and its tensor is then None.
+        handle_missing=True sets Z = 10000 wherever a map holds its minimum.
+
         After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
-        with post_process=True (the chain setSpeckleFilter, setLRCheck and setPostFilter configure), and psm_copy_maps_device of each frame of a batch in turn; then psm_signal_stream.  No
+        with post_process=True (the chain setSpeckleFilter, setLRCheck and setPostFilter configure), psm_copy_maps_device
+        and, with points, psm_reproject_device of each frame of a batch in turn; then psm_signal_stream.  No
         host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
         wanted = (costs, runner_up)
         for (name, *_), on in zip(_OUTPUTS, wanted):
             if not isinstance(on, bool):
                 raise TypeError(f"{name} must be True or False (got {on!r})")
+        if not isinstance(handle_missing, bool):
+            raise TypeError(f"handle_missing must be True or False (got {handle_missing!r})")
+        qs = None
+        if points is not None:
+            if not isinstance(points, (tuple, list)) or len(points) != 2:
+                raise TypeError("points must be a pair (Q_left, Q_right), either of them None")
+            qs = [None if q is None else (C.c_double * 16)(*np.asarray(q, np.float64).reshape(4, 4).ravel())
+                  for q in points]
+            if qs[1] is not None and self.views != capi.PSM_VIEWS_BOTH:
+                raise ValueError("points: a right Q on a left-only context (setViews('left'))")
+            if qs[0] is None and qs[1] is None:
+                raise ValueError("points: give a Q for at least one view")
         pix, lf, rf, row_step, col_step, batched = self._layout(left, right, channels)
         L, ctx = self._lib, self._ctx
         H, W = self.height, self.width
@@ -192,6 +212,10 @@ class TorchStereo:
                 oshape = (len(lf), n, H, W) if batched else (n, H, W)
                 outs.append((getattr(L, copy), torch.empty(oshape, dtype=torch.float32, device=self.device),
                              None if rmap is None else torch.empty(oshape, dtype=torch.float32, device=self.device)))
+        pts = [None, None]
+        if qs is not None:
+            pshape = (len(lf), H, W, 3) if batched else (H, W, 3)
+            pts = [None if q is None else torch.empty(pshape, dtype=torch.float32, device=self.device) for q in qs]
         self._check(L.psm_wait_stream(ctx, stream))
         for b in range(len(lf)):
             lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
@@ -209,8 +233,13 @@ class TorchStereo:
                 lo = lo[b] if batched else lo
                 ro = None if ro is None else (ro[b] if batched else ro)
                 self._check(copy(ctx, lo.data_ptr(), None if ro is None else ro.data_ptr(), W * 4))
+            if qs is not None:
+                lp, rp = ((None if p is None else (p[b] if batched else p).data_ptr()) for p in pts)
+                self._check(L.psm_reproject_device(ctx, 1 if post_process else 0, qs[0], qs[1], int(handle_missing),
+                                                   lp, rp, W * 12))
         self._check(L.psm_signal_stream(ctx, stream))
-        return (lmap, rmap) + tuple(t for _, lo, ro in outs for t in (lo, ro))
+        return (lmap, rmap) + tuple(t for _, lo, ro in outs for t in (lo, ro)) + \
+            (tuple(pts) if qs is not None else ())
 
     # -- measurement helpers ------------------------------------------------------------------
     def stage_ms(self, stage):
