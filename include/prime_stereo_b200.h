@@ -426,6 +426,31 @@ enum { PSM_PIX_U8 = 1, PSM_PIX_F32 = 2 };
 int psm_set_images_device_planes(psm_ctx* ctx, int pix_type, const void* const left[3], const void* const right[3],
                                  size_t row_step, size_t col_step);
 
+/* Rectify raw camera frames in ingest (the reference's video-mode remap and crop, src/StereoMatch.cpp:149-153, 464-478).
+ * The maps are those initUndistortRectifyMap(..., CV_16SC2) returns for each view, cropped to the context's W x H: xy
+ * holds W x H int16 pairs (sx, sy) (map[0], CV_16SC2), a holds W x H uint16 values (map[1], CV_16UC1), in HOST memory
+ * with row steps in bytes.  They are copied once into device memory (6 bytes per pixel per view); synchronous.  From then
+ * on every frame is 8-bit BGR of src_width x src_height, and output pixel (x, y) of each channel is
+ *   a' = a[y][x] & 1023, fx = a' & 31, fy = a' >> 5,  taps (sx, sy), (sx + 1, sy), (sx, sy + 1), (sx + 1, sy + 1) with
+ *   weights (32 - fx)(32 - fy) * 32, fx (32 - fy) * 32, (32 - fx) fy * 32, fx fy * 32;  a tap outside the frame reads 0;
+ *   out = (sum of weight * sample + 16384) >> 15
+ * -- cv::remap(frame, xy, a, INTER_LINEAR) with its default BORDER_CONSTANT 0, bit for bit -- and that u8 frame is
+ * ingested as psm_set_images_u8 ingests a W x H frame (the gradient mirrors at the crop's borders).
+ *   - psm_set_images_u8, _u8_async and psm_set_images_device_planes with PSM_PIX_U8 take src_width x src_height frames
+ *     (steps checked against src_width); float frames (psm_set_images, _device, _async, PSM_PIX_F32 planes) return
+ *     PSM_EINVAL.  One ingest_kernel launch and one halo pass per view, as without it.  The staging sets grow to hold
+ *     the source frame here, so no frame allocates.
+ *   - src_width = src_height = 0 with null maps and zero steps turns it off and frees the maps; the context then behaves
+ *     as one that never rectified.
+ *   - PSM_EINVAL before any CUDA work, context unchanged: a null map, a step below W * 4 (xy) or W * 2 (a) bytes, a source
+ *     side outside 1..32767, or any other mix of zero and non-zero arguments.  PSM_ESTATE while a psm_set_images_async
+ *     upload is pending.
+ *   - Multi-device contexts keep the maps on the first shard; every kind of frame reaches the other shards as the first
+ *     shard's ingested planes.  See DESIGN.md section 25. */
+int psm_set_rectify(psm_ctx* ctx, int src_width, int src_height,
+                    const int16_t* xy_left, size_t xy_left_step, const uint16_t* a_left, size_t a_left_step,
+                    const int16_t* xy_right, size_t xy_right_step, const uint16_t* a_right, size_t a_right_step);
+
 /* Pipelined upload (extension; the reference's DispEst is synchronous per frame): start the H2D copy
  * of the NEXT frame on the context's copy stream into a second staging set while the current frame
  * is still being computed, then make it the current frame.  Host buffers must be page-locked for the

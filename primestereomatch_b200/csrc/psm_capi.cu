@@ -66,6 +66,14 @@ struct psm_ctx {
     float* vol_alt[2] = {nullptr, nullptr}; // the other half of the ping-pong
     void* stage_in[2] = {nullptr, nullptr}; // device staging for the interleaved upload (the set the synchronous calls use)
     void* stage_alt[2] = {nullptr, nullptr};// second staging set: psm_set_images_async uploads frame k+1 while frame k is in flight
+    size_t stage_bytes = 0;                 // bytes per view of each staging set: a float frame of W x H, or more (psm_set_rectify)
+    // psm_set_rectify: frames are rect_sw x rect_sh and ingest remaps each view through its maps (W x H entries each) into
+    // the context's W x H; 0 x 0 = off.  A multi-device context keeps the maps on its first shard.
+    int rect_sw = 0, rect_sh = 0;
+    short2* rect_xy[2] = {nullptr, nullptr};
+    uint16_t* rect_a[2] = {nullptr, nullptr};
+    int frame_w() const { return rect_sw ? rect_sw : W; }   // the size of the frames the psm_set_images* calls take
+    int frame_h() const { return rect_sw ? rect_sh : H; }
     cudaStream_t copy_stream = nullptr;     // H2D stream of every host upload
     cudaEvent_t up_done = nullptr;          // async upload finished (recorded on copy_stream)
     cudaEvent_t host_copied = nullptr;      // H2D of a synchronous host upload finished (recorded on copy_stream)
@@ -285,7 +293,8 @@ void images_ingested(psm_ctx* c, bool float_images)
 
 size_t pix_bytes(int pix) { return pix == PSM_PIX_U8 ? 1 : sizeof(float); }
 
-// the frame's planes, gradients and ingest flags: one ingest_kernel launch and one pad_rows per view on the context's stream
+// the frame's planes, gradients and ingest flags: one ingest_kernel launch and one pad_rows per view on the context's
+// stream.  With psm_set_rectify on, the frame (u8, checked by the caller) is read through each view's maps.
 int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
 {
     PSM_CUDA(c, cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
@@ -293,8 +302,15 @@ int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
     for (int v = 0; v < 2; ++v) {
         float* g = c->guide[v];
         dim3 blk(128), grd((c->W + 3 + 127) / 128, c->H);
-        kernel<<<grd, blk, 0, c->stream>>>(src[v], c->W, c->H, c->Wp, g, g + c->plane, g + 2 * c->plane, c->grd[v],
-                                           c->gray_mode, c->guide_flags + v);
+        auto launch = [&](auto k, const auto& s) {
+            k<<<grd, blk, 0, c->stream>>>(s, c->W, c->H, c->Wp, g, g + c->plane, g + 2 * c->plane, c->grd[v], c->gray_mode,
+                                          c->guide_flags + v);
+        };
+        if (c->rect_sw)
+            launch(ingest_kernel<uint8_t, RectifySrc>,
+                   RectifySrc{src[v], c->rect_xy[v], c->rect_a[v], c->rect_sw, c->rect_sh, c->W});
+        else
+            launch(kernel, src[v]);
         PSM_LAUNCH_CHECK(c);
         if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
     }
@@ -306,11 +322,11 @@ int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
 // starts once the last ingest from that set has read it, so that it does not queue behind the compute stream's backlog.
 int upload(psm_ctx* c, int set, int pix, const PlanesSrc src[2], cudaEvent_t done)
 {
-    const size_t row_bytes = (size_t)c->W * 3 * pix_bytes(pix);
+    const size_t row_bytes = (size_t)c->frame_w() * 3 * pix_bytes(pix);
     if (c->ingest_done_valid[set]) PSM_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ingest_done[set], 0));
     for (int v = 0; v < 2; ++v)
-        PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v].ch[0], src[v].row_step, row_bytes, c->H,
-                                      cudaMemcpyHostToDevice, c->copy_stream));
+        PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v].ch[0], src[v].row_step, row_bytes,
+                                      c->frame_h(), cudaMemcpyHostToDevice, c->copy_stream));
     PSM_CUDA(c, cudaEventRecord(done, c->copy_stream));
     return PSM_OK;
 }
@@ -319,12 +335,21 @@ int upload(psm_ctx* c, int set, int pix, const PlanesSrc src[2], cudaEvent_t don
 int ingest_staged(psm_ctx* c, int set, int pix, cudaEvent_t copied)
 {
     PSM_CUDA(c, cudaStreamWaitEvent(c->stream, copied, 0));
-    const size_t elem = pix_bytes(pix), row_bytes = (size_t)c->W * 3 * elem;
+    const size_t elem = pix_bytes(pix), row_bytes = (size_t)c->frame_w() * 3 * elem;
     const PlanesSrc src[2] = {interleaved_src(stage_buf(c, set, 0), elem, row_bytes),
                               interleaved_src(stage_buf(c, set, 1), elem, row_bytes)};
     if (int rc = ingest(c, pix, src)) return rc;
     PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
     c->ingest_done_valid[set] = true;
+    return PSM_OK;
+}
+
+// a frame of pixel type pix while psm_set_rectify is on: the maps remap 8-bit frames alone
+int check_rectify_pix(psm_ctx* c, int pix)
+{
+    if (c->rect_sw && pix != PSM_PIX_U8)
+        return fail(c, PSM_EINVAL, "float frame on a context that rectifies (psm_set_rectify): rectification reads 8-bit "
+                    "frames only, as OpenCV's remap of the camera frame does; pass the u8 frame, or turn it off");
     return PSM_OK;
 }
 
@@ -334,11 +359,13 @@ int check_interleaved(psm_ctx* c, int pix, bool device, const void* l, size_t ls
                       PlanesSrc src[2])
 {
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (int rc = check_rectify_pix(c, pix)) return rc;
     const void* p[2] = {l, r};
     const size_t step[2] = {lstep, rstep};
     const size_t elem = pix_bytes(pix);
     for (int v = 0; v < 2; ++v) {
-        if (!p[v] || step[v] < (size_t)c->W * 3 * elem) return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
+        if (!p[v] || step[v] < (size_t)c->frame_w() * 3 * elem)
+            return fail(c, PSM_EINVAL, "bad image pointer/step for view %d", v);
         if (device && ((uintptr_t)p[v] % elem || step[v] % elem))
             return fail(c, PSM_EINVAL, "pointer or step %zu of view %d is not a multiple of the %zu bytes of a float sample",
                         step[v], v, elem);
@@ -354,6 +381,7 @@ int check_planes(psm_ctx* c, int pix_type, const void* const left[3], const void
     if (!c) return fail(nullptr, PSM_EINVAL, "null context");
     if (pix_type != PSM_PIX_U8 && pix_type != PSM_PIX_F32)
         return fail(c, PSM_EINVAL, "unknown pixel type %d (PSM_PIX_U8 = 1, PSM_PIX_F32 = 2)", pix_type);
+    if (int rc = check_rectify_pix(c, pix_type)) return rc;
     const size_t elem = pix_bytes(pix_type);
     const void* const* ch[2] = {left, right};
     for (int v = 0; v < 2; ++v) {
@@ -368,10 +396,10 @@ int check_planes(psm_ctx* c, int pix_type, const void* const left[3], const void
         src[v].col_step = col_step;
     }
     if (col_step < elem) return fail(c, PSM_EINVAL, "col_step %zu is below the %zu bytes of one sample", col_step, elem);
-    const size_t span = (size_t)(c->W - 1);
+    const size_t span = (size_t)(c->frame_w() - 1);
     if ((span && col_step > (SIZE_MAX - elem) / span) || row_step < span * col_step + elem)
         return fail(c, PSM_EINVAL, "row_step %zu is below the (W - 1) * col_step + %zu bytes a row of W = %d spans", row_step,
-                    elem, c->W);
+                    elem, c->frame_w());
     if (row_step % elem || col_step % elem)
         return fail(c, PSM_EINVAL, "row_step %zu / col_step %zu are not multiples of the %zu bytes of a float sample",
                     row_step, col_step, elem);
@@ -1041,12 +1069,13 @@ int multi_send_planes(psm_ctx* c, int pix)
 }
 
 // the body of every synchronous psm_set_images* call once its frame is checked.  A multi-device context runs stage 0 on
-// its first shard and sends the other shards the frame, or the planes the first shard ingested.
+// its first shard and sends the other shards the frame, or the planes the first shard ingested.  With psm_set_rectify on,
+// only the first shard holds the maps, so every kind of frame reaches the others as its planes.
 int set_images(psm_ctx* c, Frame kind, int pix, const PlanesSrc src[2])
 {
     if (!is_multi(c)) return set_images_one(c, kind, pix, src);
     if (int rc = set_images_one(c->shard[0], kind, pix, src)) return relay(c, 0, rc);
-    return kind == Frame::planes ? multi_send_planes(c, pix) : multi_send_frame(c, kind, pix, src);
+    return kind == Frame::planes || c->rect_sw ? multi_send_planes(c, pix) : multi_send_frame(c, kind, pix, src);
 }
 
 // psm_set_images[_u8]_async: the frame is uploaded into the staging set that is not in use, on the copy stream
@@ -1058,7 +1087,7 @@ int set_images_async(psm_ctx* c, int pix, const void* l, size_t lstep, const voi
     PlanesSrc src[2];
     if (int rc = check_interleaved(c, pix, false, l, lstep, r, rstep, src)) return rc;
     if (!c->stage_alt[0]) {  // allocated on first use: synchronous callers never pay for the second set
-        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->stage_alt[v], (size_t)c->W * c->H * 3 * sizeof(float)));
+        for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->stage_alt[v], c->stage_bytes));
     }
     if (int rc = upload(c, c->stage_cur ^ 1, pix, src, c->up_done)) return rc;
     c->up_pending = pix;
@@ -1211,12 +1240,13 @@ static int create_ctx(psm_ctx** out, int width, int height, int max_disp, int d_
         return e;
     };
     const size_t vol_rows = (size_t)c->vol_slices() * c->H;
+    c->stage_bytes = (size_t)c->W * c->H * 3 * sizeof(float);
     for (int v = 0; v < 2; ++v) {
         PSM_CREATE_CUDA(halo_alloc(&c->guide[v], (size_t)kGuidePlanes * c->H));
         PSM_CREATE_CUDA(halo_alloc(&c->grd[v], (size_t)c->H));
         PSM_CREATE_CUDA(halo_alloc(&c->vol[v], vol_rows));
         PSM_CREATE_CUDA(halo_alloc(&c->vol_alt[v], vol_rows));
-        PSM_CREATE_CUDA(cudaMalloc(&c->stage_in[v], (size_t)c->W * c->H * 3 * sizeof(float)));
+        PSM_CREATE_CUDA(cudaMalloc(&c->stage_in[v], c->stage_bytes));
         PSM_CREATE_CUDA(cudaMalloc(&c->dis[v], (size_t)c->W * c->H * map_bytes));
         PSM_CREATE_CUDA(cudaMemsetAsync(c->dis[v], 0, (size_t)c->W * c->H * map_bytes, c->stream));
         if (block_slices) PSM_CREATE_CUDA(cudaMalloc(&c->run_keys[v], (size_t)c->W * c->H * sizeof(unsigned long long)));
@@ -1464,6 +1494,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->fgf_lo[0]); cudaFree(c->fgf_lo[1]); cudaFree(c->fgf_mean); cudaFree(c->fgf_plan);
     cudaFree(c->sp_lab); cudaFree(c->sp_cnt);
     cudaFree(c->rp_min); cudaFree(c->rp_buf);
+    for (int v = 0; v < 2; ++v) { cudaFree(c->rect_xy[v]); cudaFree(c->rect_a[v]); }
     for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]);
                                    cudaFree(c->sp_maps[v]);
                                    cudaFree(c->track[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]);
@@ -1695,6 +1726,83 @@ int psm_set_speckle_filter(psm_ctx* c, int mode, int max_size, int max_diff)
     c->sp_mode = mode;
     c->sp_max_size = max_size;
     c->sp_max_diff = max_diff;
+    return PSM_OK;
+}
+
+int psm_set_rectify(psm_ctx* c, int src_width, int src_height, const int16_t* xy_left, size_t xy_left_step,
+                    const uint16_t* a_left, size_t a_left_step, const int16_t* xy_right, size_t xy_right_step,
+                    const uint16_t* a_right, size_t a_right_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    const void* map[4] = {xy_left, a_left, xy_right, a_right};
+    const size_t step[4] = {xy_left_step, a_left_step, xy_right_step, a_right_step};
+    const bool off = !src_width && !src_height && std::none_of(map, map + 4, [](const void* p) { return p; }) &&
+                     std::none_of(step, step + 4, [](size_t s) { return s; });
+    if (!off) {
+        if (src_width < 1 || src_width > 32767 || src_height < 1 || src_height > 32767)
+            return fail(c, PSM_EINVAL, "rectify source size %d x %d: each side must lie in 1..32767 (the int16 coordinate "
+                        "range), or both be 0 with null maps and zero steps to turn rectification off", src_width, src_height);
+        for (int k = 0; k < 4; ++k) {
+            const char* what = k % 2 ? "a (CV_16UC1)" : "xy (CV_16SC2)";
+            const char* view = k < 2 ? "left" : "right";
+            const size_t row = (size_t)c->W * (k % 2 ? 2 : 4);
+            if (!map[k]) return fail(c, PSM_EINVAL, "null %s map of the %s view", what, view);
+            if (step[k] < row)
+                return fail(c, PSM_EINVAL, "row step %zu of the %s map of the %s view is below the %zu bytes of a row of W = %d "
+                            "entries", step[k], what, view, row, c->W);
+        }
+    }
+    if (c->up_pending)
+        return fail(c, PSM_ESTATE, "psm_set_rectify with an asynchronous upload pending: call psm_set_images_commit first");
+    if (c->nshards) {
+        if (int rc = psm_set_rectify(c->shard[0], src_width, src_height, xy_left, xy_left_step, a_left, a_left_step, xy_right,
+                                     xy_right_step, a_right, a_right_step))
+            return relay(c, 0, rc);
+        c->rect_sw = src_width;
+        c->rect_sh = src_height;
+        return PSM_OK;
+    }
+    if (int rc = bind(c)) return rc;
+    // the last ingest may still read the maps and the staging sets, and the last upload may still fill a staging set
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    PSM_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+    if (off) {
+        for (int v = 0; v < 2; ++v) {
+            PSM_CUDA(c, cudaFree(c->rect_xy[v]));
+            PSM_CUDA(c, cudaFree(c->rect_a[v]));
+            c->rect_xy[v] = nullptr;
+            c->rect_a[v] = nullptr;
+        }
+        c->rect_sw = c->rect_sh = 0;
+        return PSM_OK;
+    }
+    const size_t n = (size_t)c->W * c->H;
+    for (int v = 0; v < 2; ++v) {
+        PSM_CUDA(c, alloc_if_null(c->rect_xy[v], n * sizeof(short2)));
+        PSM_CUDA(c, alloc_if_null(c->rect_a[v], n * sizeof(uint16_t)));
+    }
+    // the staging sets hold a u8 source frame as well as a float frame of W x H, so no frame allocates
+    const size_t need = std::max(c->stage_bytes, (size_t)src_width * src_height * 3);
+    if (need > c->stage_bytes) {
+        for (void** set : {c->stage_in, c->stage_alt})
+            for (int v = 0; v < 2; ++v) {
+                if (!set[v]) continue;
+                void* p = nullptr;
+                PSM_CUDA(c, cudaMalloc(&p, need));
+                cudaFree(set[v]);
+                set[v] = p;
+            }
+        c->stage_bytes = need;
+    }
+    for (int v = 0; v < 2; ++v) {
+        PSM_CUDA(c, cudaMemcpy2DAsync(c->rect_xy[v], (size_t)c->W * sizeof(short2), map[2 * v], step[2 * v],
+                                      (size_t)c->W * sizeof(short2), c->H, cudaMemcpyHostToDevice, c->stream));
+        PSM_CUDA(c, cudaMemcpy2DAsync(c->rect_a[v], (size_t)c->W * sizeof(uint16_t), map[2 * v + 1], step[2 * v + 1],
+                                      (size_t)c->W * sizeof(uint16_t), c->H, cudaMemcpyHostToDevice, c->stream));
+    }
+    PSM_CUDA(c, cudaStreamSynchronize(c->stream));
+    c->rect_sw = src_width;
+    c->rect_sh = src_height;
     return PSM_OK;
 }
 

@@ -8,6 +8,8 @@
 // pad_cols_kernel), which lets the streaming CVF kernel use plain 128-bit loads everywhere.
 // Planes are [H][Wp], volumes [d_local][H][Wp]; "W4" below is W rounded up to 4.
 #pragma once
+#include <type_traits>
+
 #include "psm_common.cuh"
 
 namespace psm {
@@ -42,7 +44,8 @@ __global__ void pad_cols_kernel(float* __restrict__ base, size_t nrows, int W, i
 }
 
 // ------------------------------------------------------------------------------------------
-// Ingest: a BGR frame (float or u8) in any PlanesSrc layout -> 3 planar channels + x-gradient of the gray image.
+// Ingest: a BGR frame (float or u8) in any PlanesSrc layout, or a u8 frame read through rectification maps (RectifySrc)
+// -> 3 planar channels + x-gradient of the gray image.
 // Restates StereoMatch.cpp:193-197 (u8 * (1/255.0f)), CVF.cpp:47 (split) and CVC.cpp:41-46
 // (cvtColor RGB2GRAY on the BGR image, Sobel dx=1 ksize=1 with BORDER_REFLECT_101).
 // ------------------------------------------------------------------------------------------
@@ -84,8 +87,49 @@ inline PlanesSrc interleaved_src(const void* p, size_t elem, size_t step)
     return PlanesSrc{{b, b + elem, b + 2 * elem}, step, 3 * elem};
 }
 
+// A u8 frame of SW x SH read through the rectification maps of one view (psm_set_rectify): output pixel (x, y) of the
+// W x H crop is OpenCV's remap(frame, xy, a, INTER_LINEAR, BORDER_CONSTANT 0) with the fixed-point maps of
+// initUndistortRectifyMap(..., CV_16SC2), cropped (DESIGN.md section 25).  The maps are dense: entry (x, y) at y * W + x.
+struct RectifySrc {
+    PlanesSrc frame;           // the source frame, SW x SH
+    const short2* xy;          // map[0]: the integer tap (sx, sy)
+    const uint16_t* a;         // map[1]: the 5 + 5-bit fraction (fy << 5 | fx); bits above 10 are ignored
+    int SW, SH, W;
+};
+
+// channel c of the sample at (x, y), as to_f32 sees it
 template <typename T>
-__global__ void ingest_kernel(PlanesSrc src, int W, int H, int Wp,
+__device__ __forceinline__ float read_sample(const PlanesSrc& src, size_t row, int c, int x, int)
+{
+    return to_f32(*reinterpret_cast<const T*>(src.ch[c] + row + (size_t)x * src.col_step));
+}
+
+// channel c of rectified pixel (x, y): the four taps' weights sum to 32768, a tap outside the frame reads 0, and the
+// integer sum is rounded like OpenCV's FixedPtCast (+ 2^14, >> 15), so the value is the u8 remap writes.  Every tap is
+// bounds-checked before it is read, so any map is memory-safe.
+template <typename T>
+__device__ __forceinline__ float read_sample(const RectifySrc& src, size_t, int c, int x, int y)
+{
+    static_assert(std::is_same<T, uint8_t>::value, "rectification reads 8-bit frames");
+    const size_t i = (size_t)y * src.W + x;
+    const short2 p = src.xy[i];
+    const int a = src.a[i] & 1023, fx = a & 31, fy = a >> 5;
+    const int wx[2] = {32 - fx, fx}, wy[2] = {32 - fy, fy};
+    int acc = 0;
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+        for (int dx = 0; dx < 2; ++dx) {
+            const int sx = p.x + dx, sy = p.y + dy;
+            if ((unsigned)sx < (unsigned)src.SW && (unsigned)sy < (unsigned)src.SH)
+                acc += wx[dx] * wy[dy] * 32 * *reinterpret_cast<const uint8_t*>(
+                           src.frame.ch[c] + (size_t)sy * src.frame.row_step + (size_t)sx * src.frame.col_step);
+        }
+    return to_f32((uint8_t)((acc + 16384) >> 15));
+}
+
+template <typename T, class Src = PlanesSrc>
+__global__ void ingest_kernel(Src src, int W, int H, int Wp,
                               float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
                               float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
 {
@@ -94,10 +138,9 @@ __global__ void ingest_kernel(PlanesSrc src, int W, int H, int Wp,
     if (x >= ((W + 3) & ~3) || y >= H) return;
     const size_t o = (size_t)y * Wp + x;
     if (x >= W) { I0[o] = 0.f; I1[o] = 0.f; I2[o] = 0.f; grd[o] = 0.f; return; }
-    const size_t row = (size_t)y * src.row_step;
-    auto sample = [&](int c, int xx) {
-        return to_f32(*reinterpret_cast<const T*>(src.ch[c] + row + (size_t)xx * src.col_step));
-    };
+    size_t row = 0;
+    if constexpr (std::is_same<Src, PlanesSrc>::value) row = (size_t)y * src.row_step;
+    auto sample = [&](int c, int xx) { return read_sample<T>(src, row, c, xx, y); };
     const float v0 = sample(0, x), v1 = sample(1, x), v2 = sample(2, x);
     I0[o] = v0;
     I1[o] = v1;

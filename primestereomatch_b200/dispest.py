@@ -66,6 +66,40 @@ def create_context(width, height, max_disp, map_bits, *, device=0, d_begin=0, d_
     return ctx
 
 
+def rectify_args(left_maps, right_maps, src_size, width, height):
+    """The psm_set_rectify arguments after the context's size and ctx: (args, arrays) -- args = (SW, SH, then a pointer
+    and a byte row step for each of xy_left, a_left, xy_right, a_right), arrays = the numpy arrays they point into (keep
+    them alive for the call).  left_maps / right_maps: (xy, a), xy int16 (H, W, 2) (initUndistortRectifyMap's map[0],
+    CV_16SC2), a uint16 (H, W) (map[1], CV_16UC1), both already cropped to the context's W x H; rows may lie any step
+    apart (a cropped view of the full map is taken as it is).  src_size: (SW, SH), the size of the camera frames.  All
+    three None: rectification off (0 x 0, null maps).  Raises TypeError or ValueError before any device work."""
+    if left_maps is None and right_maps is None and src_size is None:
+        return (0, 0, None, 0, None, 0, None, 0, None, 0), ()
+    if left_maps is None or right_maps is None or src_size is None:
+        raise ValueError("setRectify takes both views' maps and the source size, or None for all three (off)")
+    try:
+        sw, sh = (int(v) for v in src_size)
+    except (TypeError, ValueError):
+        raise TypeError(f"src_size must be (width, height) (got {src_size!r})") from None
+    if not (1 <= sw <= 32767 and 1 <= sh <= 32767):
+        raise ValueError(f"source size {sw} x {sh}: each side must lie in 1..32767 (the int16 map coordinates)")
+    args, arrays = [sw, sh], []
+    for name, maps in (("left", left_maps), ("right", right_maps)):
+        if not isinstance(maps, (tuple, list)) or len(maps) != 2:
+            raise TypeError(f"{name} maps must be a pair (xy, a)")
+        for what, m, dtype, shape, inner in (("xy", maps[0], np.int16, (height, width, 2), (4, 2)),
+                                             ("a", maps[1], np.uint16, (height, width), (2,))):
+            m = np.asarray(m)
+            if m.dtype != dtype or m.shape != shape:
+                raise ValueError(f"{name} {what} map must be {np.dtype(dtype).name} of shape {shape} (the maps cropped to the "
+                                 f"context's {width} x {height}; got {m.dtype} {m.shape})")
+            if m.strides[1:] != inner or m.strides[0] < 0:
+                m = np.ascontiguousarray(m)   # each row is read as a dense run of entries
+            arrays.append(m)
+            args += [_ptr(m), m.strides[0]]
+    return tuple(args), tuple(arrays)
+
+
 class DispEst:
     """DispEst(l, r, d, t, ocl) -- reference src/DispEst.cpp:10-143.
 
@@ -115,6 +149,7 @@ class DispEst:
         if min_disp and (d_begin != 0 or d_count is not None):
             raise ValueError("min_disp (a range context over [min_disp, max_disp)) excludes d_begin / d_count")
         self.min_disp = int(min_disp)
+        self.src_size = None   # setRectify: (SW, SH) of the camera frames CostConst_GPU takes
         self._lImg, self._rImg = l, r
         self._ctx = C.c_void_p()
         self._lib = None
@@ -214,6 +249,19 @@ class DispEst:
         self.speckle_mode = int(mode)
         return 0
 
+    def setRectify(self, left_maps, right_maps, src_size):
+        """Rectify every later frame on the device (psm_set_rectify): the reference's video-mode remap(frame, rec,
+        map[0], map[1], INTER_LINEAR) and crop, bit for bit.  left_maps / right_maps: (xy, a) of each view as
+        initUndistortRectifyMap(..., CV_16SC2) returns them, cropped to the constructor's W x H (xy int16 (H, W, 2), a
+        uint16 (H, W)); src_size: (SW, SH) of the camera frames.  setInputImages then takes uint8 frames of SH x SW x 3;
+        float frames raise PsmError.  None for all three turns it off.  Raises TypeError / ValueError on malformed maps
+        before any device work."""
+        args, _keep = rectify_args(left_maps, right_maps, src_size, self.wid, self.hei)
+        self._need_gpu()
+        capi.check(self._lib.psm_set_rectify(self._ctx, *args), self._ctx)
+        self.src_size = None if src_size is None else (args[0], args[1])
+        return 0
+
     _VIEWS = {"left": capi.PSM_VIEWS_LEFT, "both": capi.PSM_VIEWS_BOTH}
 
     def setViews(self, views):
@@ -284,8 +332,10 @@ class DispEst:
         self._need_gpu()
         l = np.ascontiguousarray(self._lImg)
         r = np.ascontiguousarray(self._rImg)
-        if l.shape != (self.hei, self.wid, 3) or r.shape != l.shape:
-            raise ValueError("input image size differs from the size DispEst was constructed with")
+        w, h = self.src_size or (self.wid, self.hei)
+        if l.shape != (h, w, 3) or r.shape != l.shape:
+            raise ValueError(f"input images must be {h} x {w} x 3: the size DispEst was constructed with, or the source "
+                             "size of setRectify")
         if l.dtype == np.uint8:
             capi.check(self._lib.psm_set_images_u8(self._ctx, _ptr(l), l.strides[0], _ptr(r), r.strides[0]), self._ctx)
         else:

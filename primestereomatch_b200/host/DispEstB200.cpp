@@ -131,6 +131,28 @@ int DispEst::read_planes(int view, int n, int (*read)(psm_ctx*, int, float*, siz
     return 0;
 }
 
+// reference src/StereoMatch.cpp:149-153 (remap of each camera frame, then the crop) as a device step of CostConst_GPU
+int DispEst::setRectify(const cv::Mat& lxy, const cv::Mat& la, const cv::Mat& rxy, const cv::Mat& ra, int src_width,
+                        int src_height)
+{
+    if (!ctx) return -1;
+    if (!src_width && !src_height && lxy.empty() && la.empty() && rxy.empty() && ra.empty()) {
+        const int rc = psm_set_rectify(ctx, 0, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0);
+        if (rc == PSM_OK) src_w = src_h = 0;
+        return rc;
+    }
+    for (const cv::Mat* m : {&lxy, &la, &rxy, &ra})
+        if (m->rows != hei || m->cols != wid || m->type() != (m == &lxy || m == &rxy ? CV_16SC2 : CV_16UC1)) {
+            std::fprintf(stderr, "DispEst::setRectify: the maps must be %dx%d CV_16SC2 (xy) and CV_16UC1 (a), cropped to "
+                                 "the disparity maps' size\n", wid, hei);
+            return -1;
+        }
+    const int rc = psm_set_rectify(ctx, src_width, src_height, lxy.ptr<int16_t>(), lxy.step, la.ptr<uint16_t>(), la.step,
+                                   rxy.ptr<int16_t>(), rxy.step, ra.ptr<uint16_t>(), ra.step);
+    if (rc == PSM_OK) { src_w = src_width; src_h = src_height; }
+    return rc;
+}
+
 // reference src/DispEst.cpp:181-194 dumps every slice as PNG; here: slice statistics on stdout
 int DispEst::reprojectImageTo3D(cv::Mat& xyz, const double Q[16], bool handleMissingValues, int view, bool postProcessed)
 {
@@ -160,9 +182,11 @@ int DispEst::CostConst_GPU()
     if (!ctx) return -1;
     // the context was sized at construction: a differently shaped or typed Mat from setInputImages must not reach
     // the 2-D copy (the reference re-creates DispEst on every dataset change, StereoMatch.cpp:601-602)
-    if (lImg.rows != hei || lImg.cols != wid || rImg.rows != hei || rImg.cols != wid || lImg.type() != rImg.type() ||
+    // with setRectify on, the frames are the camera's (src_w x src_h, 8-bit)
+    const int fw = src_w ? src_w : wid, fh = src_w ? src_h : hei;
+    if (lImg.rows != fh || lImg.cols != fw || rImg.rows != fh || rImg.cols != fw || lImg.type() != rImg.type() ||
         lImg.channels() != 3) {
-        std::fprintf(stderr, "DispEst::CostConst_GPU: input images must be %dx%d, 3 channels, equal types\n", wid, hei);
+        std::fprintf(stderr, "DispEst::CostConst_GPU: input images must be %dx%d, 3 channels, equal types\n", fw, fh);
         return -1;
     }
     int rc;

@@ -28,12 +28,14 @@
 // Minimal stand-in for the handful of cv::Mat members the facade touches.
 #define CV_8U 0
 #define CV_16U 2
+#define CV_16S 3
 #define CV_32F 5
 #define CV_MAT_DEPTH_MASK 7
 #define CV_MAKETYPE(depth, cn) ((depth) + (((cn)-1) << 3))
 #define CV_8UC1 CV_MAKETYPE(CV_8U, 1)
 #define CV_8UC3 CV_MAKETYPE(CV_8U, 3)
 #define CV_16UC1 CV_MAKETYPE(CV_16U, 1)
+#define CV_16SC2 CV_MAKETYPE(CV_16S, 2)
 #define CV_32FC1 CV_MAKETYPE(CV_32F, 1)
 #define CV_32FC3 CV_MAKETYPE(CV_32F, 3)
 namespace cv {
@@ -55,7 +57,7 @@ public:
     }
     int type() const { return type_; }
     int channels() const { return (type_ >> 3) + 1; }
-    size_t elemSize() const { return (size_t)channels() * ((type_ & CV_MAT_DEPTH_MASK) == CV_32F ? 4 : (type_ & CV_MAT_DEPTH_MASK) == CV_16U ? 2 : 1); }
+    size_t elemSize() const { return (size_t)channels() * ((type_ & CV_MAT_DEPTH_MASK) == CV_32F ? 4 : (type_ & CV_MAT_DEPTH_MASK) == CV_16U || (type_ & CV_MAT_DEPTH_MASK) == CV_16S ? 2 : 1); }
     bool empty() const { return data == nullptr; }
     template <typename T> T* ptr(int y = 0) { return (T*)(data + step * y); }
     template <typename T> const T* ptr(int y = 0) const { return (const T*)(data + step * y); }
@@ -124,6 +126,12 @@ public:
     // PSM_OPT_RUNNER_UP: with true, DispSelect_GPU also fills lRunnerUp / rRunnerUp.  The next stage after a change must
     // be CostConst_GPU.  Fails on a context that owns part of the disparity range.
     int setRunnerUpOutput(bool on);
+    // Rectify every later frame on the device (psm_set_rectify): the reference's video-mode remap(frame, rec, map[0],
+    // map[1], INTER_LINEAR) and crop.  xy / a: each view's CV_16SC2 / CV_16UC1 maps from initUndistortRectifyMap, cropped
+    // to the context's W x H (map(cropBox)); src_width x src_height: the camera frames' size.  setInputImages then takes
+    // CV_8UC3 frames of that size.  src_width = src_height = 0 with empty maps turns it off.
+    int setRectify(const cv::Mat& lxy, const cv::Mat& la, const cv::Mat& rxy, const cv::Mat& ra, int src_width,
+                   int src_height);
     int printCV(void);
     // OpenCV's reprojectImageTo3D(disp, xyz, Q, handleMissingValues) of one view's map (PSM_LEFT / PSM_RIGHT) on the
     // device, bit for bit (psm_read_points): xyz becomes H x W CV_32FC3 (X, Y, Z).  Q: the rig's 4 x 4 reprojection
@@ -164,6 +172,7 @@ private:
     int lr_mode = PSM_LR_OFF;
     int speckle_mode = PSM_SPECKLE_OFF;
     int views = PSM_VIEWS_BOTH;
+    int src_w = 0, src_h = 0;   // setRectify: the size of the frames CostConst_GPU takes, 0 = the context's
     bool cost_output = false;
     bool runner_up_output = false;
     int set_output(int key, bool on, bool& flag);

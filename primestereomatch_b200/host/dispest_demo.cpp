@@ -14,7 +14,10 @@
 // leading `--speckle MODE SIZE DIFF` speckle removal (setSpeckleFilter: MODE 0 off, 1 first, 2 only), a leading
 // `--points Q.f64 out.xyz` the left view's 3D points of the final maps (reprojectImageTo3D with the 16 native-endian
 // doubles of Q.f64, row-major): out.xyz holds H x W x 3 native float32 X, Y, Z.  A leading
-// `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.
+// `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.  A
+// leading `--rectify SW SH left.map right.map` rectifies raw camera frames on the device (setRectify): each .map file
+// holds W x H native-endian int16 pairs (map[0], CV_16SC2), then W x H uint16 (map[1], CV_16UC1), both cropped to W x H,
+// and left / right are then 8-bit BGR frames of SW x SH instead of float frames of W x H.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -36,6 +39,8 @@ int main(int argc, char** argv)
     int block_slices = 0, min_disp = 0;
     int speckle[3] = {0, 0, 0};   // mode, max_size, max_diff
     const char* points[2] = {nullptr, nullptr};   // Q file, output file
+    int src_size[2] = {0, 0};                     // --rectify: SW, SH
+    const char* map_files[2] = {nullptr, nullptr};
     std::vector<int> devices;
     const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
     if (left_only) {
@@ -45,7 +50,18 @@ int main(int argc, char** argv)
     }
     while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices") ||
                          !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle") ||
-                         !std::strcmp(argv[1], "--points"))) {
+                         !std::strcmp(argv[1], "--points") || !std::strcmp(argv[1], "--rectify"))) {
+        if (!std::strcmp(argv[1], "--rectify")) {
+            if (argc < 6) break;
+            src_size[0] = std::atoi(argv[2]);
+            src_size[1] = std::atoi(argv[3]);
+            map_files[0] = argv[4];
+            map_files[1] = argv[5];
+            argv[5] = argv[0];
+            argv += 5;
+            argc -= 5;
+            continue;
+        }
         if (!std::strcmp(argv[1], "--points")) {
             if (argc < 4) break;
             points[0] = argv[2];
@@ -80,19 +96,38 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--points Q.f64 out.xyz] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
     const int W = std::atoi(argv[1]), H = std::atoi(argv[2]), D = std::atoi(argv[3]);
     if (b200devicepoll() == 0) { std::fprintf(stderr, "no CUDA device\n"); return 3; }
-    cv::Mat l(H, W, CV_32FC3), r(H, W, CV_32FC3);
-    if (!read_all(argv[4], l.data, l.step * H) || !read_all(argv[5], r.data, r.step * H)) { std::fprintf(stderr, "bad input\n"); return 2; }
-    DispEst* SMDE = new DispEst(l, r, D, MAX_CPU_THREADS, true, block_slices, devices, min_disp);
+    // the frames: float W x H, or with --rectify the camera's 8-bit SW x SH
+    const bool rectify = map_files[0] != nullptr;
+    const int fw = rectify ? src_size[0] : W, fh = rectify ? src_size[1] : H;
+    if (fw < 1 || fh < 1) { std::fprintf(stderr, "bad --rectify source size\n"); return 2; }
+    cv::Mat l(fh, fw, rectify ? CV_8UC3 : CV_32FC3), r(fh, fw, rectify ? CV_8UC3 : CV_32FC3);
+    if (!read_all(argv[4], l.data, l.step * fh) || !read_all(argv[5], r.data, r.step * fh)) { std::fprintf(stderr, "bad input\n"); return 2; }
+    cv::Mat sized(H, W, l.type());   // the facade takes the context's size from its first frames
+    DispEst* SMDE = new DispEst(rectify ? sized : l, rectify ? sized : r, D, MAX_CPU_THREADS, true, block_slices, devices,
+                                min_disp);
     SMDE->setInputImages(l, r);
     SMDE->setThreads(MAX_CPU_THREADS);
     SMDE->setSubsampleRate(4);
     int rc = left_only ? SMDE->setViews(PSM_VIEWS_LEFT) : 0;
+    if (!rc && rectify) {
+        cv::Mat xy[2], a[2];
+        for (int v = 0; v < 2; ++v) {
+            xy[v].create(H, W, CV_16SC2);
+            a[v].create(H, W, CV_16UC1);
+            FILE* f = std::fopen(map_files[v], "rb");
+            const bool ok = f && std::fread(xy[v].data, 1, xy[v].step * H, f) == xy[v].step * H &&
+                            std::fread(a[v].data, 1, a[v].step * H, f) == a[v].step * H;
+            if (f) std::fclose(f);
+            if (!ok) { std::fprintf(stderr, "bad map file %s\n", map_files[v]); return 2; }
+        }
+        rc = SMDE->setRectify(xy[0], a[0], xy[1], a[1], fw, fh);
+    }
     if (!rc && argc >= 10) rc = SMDE->setGuidedFilter(std::atoi(argv[8]), (float)std::atof(argv[9]));
     if (!rc && argc >= 13)
         rc = SMDE->setMatchingCost((float)std::atof(argv[10]), (float)std::atof(argv[11]), (float)std::atof(argv[12]));

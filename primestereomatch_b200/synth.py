@@ -44,3 +44,23 @@ def to_f32(img_u8):
 def stereo_pair_f32(W, H, D, seed=None):
     l, r, d = stereo_pair_u8(W, H, D, seed)
     return to_f32(l), to_f32(r), d
+
+
+def rectify_maps(W, H, SW, SH, view=0, k1=-0.17, k2=0.027):
+    """Fixed-point rectification maps of a closed-form rig, for callers without cv2: the W x H crop centred in an SW x SH
+    rectified image, seen by a pinhole camera of focal length 0.5 * SW with radial distortion (k1, k2), turned by a small
+    in-plane angle that differs per view.  -> (xy int16 (H, W, 2), a uint16 (H, W)), the CV_16SC2 / CV_16UC1 layout of
+    initUndistortRectifyMap: each coordinate is rounded to 1/32 px, xy holds its integer part and a = fy * 32 + fx its
+    fraction."""
+    f, cx, cy = 0.5 * SW, (SW - 1) / 2.0, (SH - 1) / 2.0
+    ang = 0.004 if view == 0 else -0.003
+    x = np.arange(W, dtype=np.float64)[None, :] + (SW - W) // 2
+    y = np.arange(H, dtype=np.float64)[:, None] + (SH - H) // 2
+    u, v = (x - cx) / f, (y - cy) / f
+    u, v = np.cos(ang) * u - np.sin(ang) * v, np.sin(ang) * u + np.cos(ang) * v
+    r2 = u * u + v * v
+    d = 1.0 + k1 * r2 + k2 * r2 * r2
+    ix = np.rint((f * u * d + cx) * 32).astype(np.int64)
+    iy = np.rint((f * v * d + cy) * 32).astype(np.int64)
+    xy = np.stack([np.clip(ix >> 5, -32768, 32767), np.clip(iy >> 5, -32768, 32767)], -1).astype(np.int16)
+    return xy, ((iy & 31) * 32 + (ix & 31)).astype(np.uint16)

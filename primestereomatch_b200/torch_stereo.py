@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import capi
-from .dispest import DispEst, create_context, resolve_map_bits
+from .dispest import DispEst, create_context, rectify_args, resolve_map_bits
 
 _PIX = {torch.uint8: capi.PSM_PIX_U8, torch.float32: capi.PSM_PIX_F32}
 _ORDER = {"bgr": (0, 1, 2), "rgb": (2, 1, 0)}   # the tensor channel that holds B, G and R
@@ -70,6 +70,8 @@ class TorchStereo:
     `devices` (a multi-device context whose frames and maps live on devices[0]), `min_disp` (a range context over
     [min_disp, max_disp), psm_create_range).  The setters pass their values straight to the C-ABI, which rejects bad ones
     with PsmError."""
+
+    src_size = None   # setRectify: (SW, SH) of the raw frames match takes; None = frames of (height, width)
 
     def __init__(self, width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None, min_disp=0):
         self.width, self.height, self.max_disp = int(width), int(height), int(max_disp)
@@ -132,6 +134,14 @@ class TorchStereo:
     def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
         self._check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)))
 
+    def setRectify(self, left_maps, right_maps, src_size):
+        """DispEst.setRectify: from then on match takes uint8 camera frames of (SH, SW) in any layout frame_layout reads
+        -- the two halves of one side-by-side tensor included -- and rectifies them on the device; float frames raise
+        ValueError before any device work.  None for all three turns it off."""
+        args, _keep = rectify_args(left_maps, right_maps, src_size, self.width, self.height)
+        self._check(self._lib.psm_set_rectify(self._ctx, *args))
+        self.src_size = None if src_size is None else (args[0], args[1])
+
     def setViews(self, views):
         value = DispEst._VIEWS.get(views, -1) if isinstance(views, str) else -1
         self._check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_VIEWS, value))
@@ -143,9 +153,13 @@ class TorchStereo:
 
     # -- frames -------------------------------------------------------------------------------
     def _layout(self, left, right, channels):
-        """Both frames' layout, checked in full before any device work."""
-        pix, lf, row_step, col_step, batched = frame_layout(left, self.height, self.width, channels)
-        other = frame_layout(right, self.height, self.width, channels)
+        """Both frames' layout, checked in full before any device work: (H, W) frames, or uint8 frames of the source
+        size while setRectify is on."""
+        w, h = self.src_size or (self.width, self.height)
+        pix, lf, row_step, col_step, batched = frame_layout(left, h, w, channels)
+        other = frame_layout(right, h, w, channels)
+        if self.src_size is not None and pix != capi.PSM_PIX_U8:
+            raise ValueError("setRectify is on: rectification reads uint8 camera frames only (got float32)")
         if left.shape != right.shape or left.dtype != right.dtype or (pix, row_step, col_step) != (other[0], other[2], other[3]):
             raise ValueError("left and right must have the same shape, dtype and strides")
         for name, t in (("left", left), ("right", right)):
