@@ -24,6 +24,7 @@
  *   psm_set_lr_check      <-> PP::processDM's lrCheck + fillInv (commented out there)  src/PP.cpp:17-143, :405-406
  *   psm_set_speckle_filter <-> cv::filterSpeckles, as the reference's StereoSGBM matcher configures it (speckleWindowSize,
  *                             speckleRange)                       src/StereoMatch.cpp:654-655
+ *   psm_set_disparity_check <-> cv::validateDisparity, the same matcher's disp12MaxDiff = 1  src/StereoMatch.cpp:651
  *   psm_reproject_device  <-> cv::reprojectImageTo3D with the rig's Q (camProps.Q, computed and never read there)
  *                                                                 src/StereoMatch.cpp:456-457
  *   psm_read_cost_slice   <-> DispEst::printCV (cost-slice dump) src/DispEst.cpp:181-194
@@ -58,7 +59,8 @@
  * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
  * (its buffers and, after a change of sigma or weight type, the weight table; with psm_set_speckle_filter on, the
  * labels and counts, 8 * W * H bytes per view, and with PSM_SPECKLE_FIRST and a check mode, a map pair between the
- * removal and the check), psm_set_option(PSM_OPT_COSTS, 1) (the
+ * removal and the check; with psm_set_disparity_check on, a map per computed view between the check and the next step and,
+ * on rows over 6144 columns, its claim words), psm_set_option(PSM_OPT_COSTS, 1) (the
  * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots), psm_reproject_device with
  * handle_missing (8 bytes of scratch).  Run them once before a
  * latency-critical
@@ -123,9 +125,10 @@ enum { PSM_VIEWS_LEFT = 1, PSM_VIEWS_BOTH = 2 };
  *     psm_disp_reduce_keys* must be NULL: a non-NULL one returns PSM_EINVAL.  The fused exchange moves and reduces the
  *     left keys only; every rank must use the same setting.  Multi-device contexts forward the option to every shard.
  *   - psm_post_process* filters the left map only.  With a left-right check mode (psm_set_lr_check 1 or 2) it returns
- *     PSM_ESTATE: the check needs both maps.  psm_set_lr_check itself may be called at any time.
+ *     PSM_ESTATE: the check needs both maps; psm_set_disparity_check(PSM_DCHECK_FIRST) replaces it with the one-view
+ *     check and fills the left map.  psm_set_lr_check itself may be called at any time.
  *   - PSM_ESTATE: psm_read_cost_slice, psm_read_ab_slice and psm_read_guide_plane planes 3-11 of the right view, and
- *     psm_read_valid_mask.
+ *     psm_read_valid_mask (of the left view too, unless the last post-process filled with the one-view check).
  *   - Nothing else is written: the right volume, the right map, the right post-filtered map and the right mask keep
  *     their contents.  psm_device_ptr returns the same addresses, and no device memory is freed or allocated.
  *     psm_stage_ms reports the left view's work, psm_launch_count the kernels that ran. */
@@ -363,6 +366,38 @@ enum { PSM_SPECKLE_OFF = 0, PSM_SPECKLE_FIRST = 1, PSM_SPECKLE_ONLY = 2 };
  * max_diff >= 0; anything else returns PSM_EINVAL and leaves the context unchanged.  Multi-device contexts forward it to
  * every shard.  See DESIGN.md section 23. */
 int psm_set_speckle_filter(psm_ctx* ctx, int mode, int max_size, int max_diff);
+
+/* Disparity check modes of psm_set_disparity_check */
+enum { PSM_DCHECK_OFF = 0, PSM_DCHECK_FIRST = 1, PSM_DCHECK_ONLY = 2 };
+
+/* One-view disparity check (OpenCV's cv::validateDisparity, StereoSGBM's disp12MaxDiff, which the reference's SGBM
+ * matcher sets to 1) for every later psm_post_process / _u16 / _device of this context:
+ *   PSM_DCHECK_OFF (default): the stage exactly as psm_set_speckle_filter, psm_set_lr_check and psm_set_post_filter
+ *                     configure it, launch for launch;
+ *   PSM_DCHECK_FIRST: the check on the selection maps, then the configured speckle removal, left-right check / fill and
+ *                     post-filter on its result, in that order (one more launch);
+ *   PSM_DCHECK_ONLY:  the check alone; its maps are the result, nothing else runs and psm_read_valid_mask returns
+ *                     PSM_ESTATE (one launch).
+ * Definition, per row of one view's selection map m (u8 or u16), c = plane 1 of PSM_OPT_COSTS (the winner's cost q(m))
+ * of the same selection, W = width, D = max_disp:
+ *   1. only columns x in [D, W) with m[x] != 0 take part; every other pixel keeps its value;
+ *   2. every participating x claims column x - m[x] with cost c[x]; per column the lowest cost wins, compared in the
+ *      arg-min's order (-0 equal to +0), and on equal costs the lowest x; d2[column] is the winner's m;
+ *   3. a participating x becomes 0 when |d2[x - m[x]] - m[x]| > max_diff (as int);
+ *   4. the right view is the mirror image: fliplr(check(fliplr(r), fliplr(c_right))).
+ * This equals cv::validateDisparity(m * 16 as CV_16S, c's order as CV_32S, 1, D - 1, max_diff) with 0 for 0; it does not
+ * depend on min_disp.  With PSM_DCHECK_FIRST and PSM_LR_FILL / PSM_LR_FILL_WMF, a left-only context fills with the mask
+ * valid[x] = v[x] >= 2 of its checked (and speckle-filtered) map v instead of the two-view check, and psm_read_valid_mask
+ * of the left view returns that mask; two-view contexts run the left-right check on the checked maps, so the pixels
+ * the check zeroed are filled like occlusions.  The stage reads the costs the last selection wrote: without them
+ * (PSM_OPT_COSTS off for that selection) psm_post_process* returns PSM_ESTATE.  It writes nothing but the post-processed
+ * maps and the masks.  Stage 5 of psm_stage_ms covers it.  Valid: one of the three modes and max_diff in [0, 4095];
+ * anything else returns PSM_EINVAL and leaves the context unchanged, as does a mode other than PSM_DCHECK_OFF on a
+ * context that owns part of the range (psm_create_sharded).  Multi-device contexts forward it to every shard; the stage
+ * runs on the first.  Rows wider than 6144 columns use 8 * W * H bytes of scratch per computed view, allocated on first
+ * use.
+ * See DESIGN.md section 26. */
+int psm_set_disparity_check(psm_ctx* ctx, int mode, int max_diff);
 
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream.  Waits for the work already enqueued

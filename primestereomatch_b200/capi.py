@@ -24,7 +24,7 @@ SYMBOLS = [
     "psm_disp_reduce_keys_u16", "psm_disp_fetch_p2p_u16", "psm_post_process_u16", "psm_set_lr_check", "psm_read_valid_mask",
     "psm_create_blocked", "psm_create_multi", "psm_set_images_device_planes", "psm_wait_stream", "psm_signal_stream",
     "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs", "psm_copy_runner_up_device", "psm_read_runner_up",
-    "psm_create_range", "psm_set_speckle_filter", "psm_reproject_device", "psm_read_points", "psm_set_rectify",
+    "psm_create_range", "psm_set_speckle_filter", "psm_set_disparity_check", "psm_reproject_device", "psm_read_points", "psm_set_rectify",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -38,6 +38,7 @@ PSM_CVF_EXACT, PSM_CVF_MIXED, PSM_CVF_NAIVE = 0, 1, 2
 PSM_WMF_EXP, PSM_WMF_IV1, PSM_WMF_IV2, PSM_WMF_OFF = 0, 1, 2, 5
 PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL = 0, 1, 2
 PSM_SPECKLE_OFF, PSM_SPECKLE_FIRST, PSM_SPECKLE_ONLY = 0, 1, 2
+PSM_DCHECK_OFF, PSM_DCHECK_FIRST, PSM_DCHECK_ONLY = 0, 1, 2
 PSM_PIX_U8, PSM_PIX_F32 = 1, 2
 
 _lib = None
@@ -80,6 +81,7 @@ def lib():
     L.psm_set_post_filter.argtypes = [vp, i, C.c_float, i, i]
     L.psm_set_lr_check.argtypes = [vp, i]
     L.psm_set_speckle_filter.argtypes = [vp, i, i, i]
+    L.psm_set_disparity_check.argtypes = [vp, i, i]
     L.psm_set_rectify.argtypes = [vp, i, i, vp, sz, vp, sz, vp, sz, vp, sz]
     L.psm_read_valid_mask.argtypes = [vp, i, u8p, sz]
     L.psm_set_stream.argtypes = [vp, vp]

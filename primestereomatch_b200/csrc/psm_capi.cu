@@ -21,6 +21,7 @@
 #include "psm_fgf.cuh"
 #include "psm_lr.cuh"
 #include "psm_speckle.cuh"
+#include "psm_dcheck.cuh"
 #include "psm_reproject.cuh"
 
 #ifndef PSM_BUILD_FLAGS
@@ -131,6 +132,12 @@ struct psm_ctx {
     int* sp_lab = nullptr;                  // speckle removal's labels and counts: 2 x W x H each (view v at v * W * H), lazy
     int* sp_cnt = nullptr;
     uint8_t* sp_maps[2] = {nullptr, nullptr};  // PSM_SPECKLE_FIRST with the check: the filtered maps the check reads, lazy
+    int dc_mode = PSM_DCHECK_OFF;           // one-view disparity check in the post-process stage, psm_set_disparity_check
+    int dc_max_diff = 1;
+    // per computed view, lazy: PSM_DCHECK_FIRST with speckle removal or the check: its result; rows wider than
+    // kDcStageCols: the claim words, W x H
+    uint8_t* dc_maps[2] = {nullptr, nullptr};
+    unsigned long long* dc_claims[2] = {nullptr, nullptr};
     // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
     // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
     int blk_slices = 0;
@@ -1496,7 +1503,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->rp_min); cudaFree(c->rp_buf);
     for (int v = 0; v < 2; ++v) { cudaFree(c->rect_xy[v]); cudaFree(c->rect_a[v]); }
     for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]);
-                                   cudaFree(c->sp_maps[v]);
+                                   cudaFree(c->sp_maps[v]); cudaFree(c->dc_maps[v]); cudaFree(c->dc_claims[v]);
                                    cudaFree(c->track[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]);
                                    for (psm_ctx::OutState& o : c->outs) cudaFree(o.planes[v]); }
     for (int s = 0; s < kNumStages; ++s) {
@@ -1726,6 +1733,26 @@ int psm_set_speckle_filter(psm_ctx* c, int mode, int max_size, int max_diff)
     c->sp_mode = mode;
     c->sp_max_size = max_size;
     c->sp_max_diff = max_diff;
+    return PSM_OK;
+}
+
+int psm_set_disparity_check(psm_ctx* c, int mode, int max_diff)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (mode != PSM_DCHECK_OFF && mode != PSM_DCHECK_FIRST && mode != PSM_DCHECK_ONLY)
+        return fail(c, PSM_EINVAL, "disparity check mode %d is not off (0), first (1) or only (2)", mode);
+    if (max_diff < 0 || max_diff > 4095) return fail(c, PSM_EINVAL, "disparity check max_diff %d outside 0..4095", max_diff);
+    // a multi-device context spans the range, and its first shard holds the complete maps and the cost planes
+    if (c->nshards) {
+        for (int k = 0; k < c->nshards; ++k) { c->shard[k]->dc_mode = mode; c->shard[k]->dc_max_diff = max_diff; }
+        return PSM_OK;
+    }
+    if (mode != PSM_DCHECK_OFF && !c->owns_problem())
+        return fail(c, PSM_EINVAL, "psm_set_disparity_check on a context that owns slices [%d,%d) of %d: the check reads "
+                    "the winners' costs (PSM_OPT_COSTS), which such a context cannot write; use a context over the whole "
+                    "range", c->d_begin, c->d_begin + c->d_count, c->D);
+    c->dc_mode = mode;
+    c->dc_max_diff = max_diff;
     return PSM_OK;
 }
 
@@ -2413,6 +2440,21 @@ static int speckle_filter(psm_ctx* c, const uint8_t* const in[2], uint8_t* const
     return PSM_OK;
 }
 
+// the one-view disparity check (psm_dcheck.cuh) of the maps in[view] into out[view], every computed view in one launch
+template <typename T>
+static int disparity_check(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
+{
+    const float* q[2];
+    for (int v = 0; v < 2; ++v) q[v] = c->outs[kOutCosts].planes[v] ? c->outs[kOutCosts].planes[v] + (size_t)c->W * c->H : nullptr;
+    const DcheckArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])}, {q[0], q[1]},
+                             {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, {c->dc_claims[0], c->dc_claims[1]}, c->W, c->H, c->D,
+                             c->dc_max_diff};
+    const size_t smem = c->W <= kDcStageCols ? (size_t)c->W * sizeof(unsigned long long) : 0;
+    dcheck_kernel<T><<<dim3((unsigned)c->H, (unsigned)c->views), kDcThreads, smem, c->stream>>>(a);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
 // the post-filter stage on maps of type T
 template <typename T>
 static int post_process_maps(psm_ctx* c)
@@ -2427,10 +2469,18 @@ static int post_process_maps(psm_ctx* c)
     const uint8_t* maps[2];
     if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
-    // PSM_SPECKLE_ONLY: the removal is the whole stage; the check and the post-filter do not run
-    const bool sp = c->sp_mode != PSM_SPECKLE_OFF, only = c->sp_mode == PSM_SPECKLE_ONLY;
+    // PSM_DCHECK_ONLY: the disparity check is the whole stage; PSM_SPECKLE_ONLY: the removal (after the disparity
+    // check) is; the left-right check and the post-filter do not run
+    const bool dc = c->dc_mode != PSM_DCHECK_OFF, dc_only = c->dc_mode == PSM_DCHECK_ONLY;
+    const bool sp = !dc_only && c->sp_mode != PSM_SPECKLE_OFF, only = dc_only || c->sp_mode == PSM_SPECKLE_ONLY;
     const bool lr = !only && c->lr_mode != PSM_LR_OFF, wmf = !only && c->lr_mode != PSM_LR_FILL;
-    if (lr && c->views == 1)
+    // a left-only context fills with the disparity check's result in place of the two-view check
+    const bool own_fill = lr && dc && c->views == 1;
+    if (dc && !c->outs[kOutCosts].have)
+        return fail(c, PSM_ESTATE, "psm_post_process: the disparity check (psm_set_disparity_check mode %d) reads the "
+                    "winners' costs, and the last selection stage did not write them: set PSM_OPT_COSTS = 1 before it",
+                    c->dc_mode);
+    if (lr && c->views == 1 && !own_fill)
         return fail(c, PSM_ESTATE, "psm_post_process: the left-right check (psm_set_lr_check mode %d) needs both maps, and "
                     "this context computes the left view alone (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): set PSM_LR_OFF or "
                     "PSM_VIEWS_BOTH", c->lr_mode);
@@ -2446,6 +2496,10 @@ static int post_process_maps(psm_ctx* c)
     for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->dis_pp[v], npix * c->map_bytes));
     if (lr)
         for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->lr_valid[v], npix));
+    if (dc && (sp || lr))
+        for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->dc_maps[v], npix * c->map_bytes));
+    if (dc && c->W > kDcStageCols)
+        for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->dc_claims[v], npix * sizeof(unsigned long long)));
     if (sp) {
         PSM_CUDA(c, alloc_if_null(c->sp_lab, 2 * npix * sizeof(int)));
         PSM_CUDA(c, alloc_if_null(c->sp_cnt, 2 * npix * sizeof(int)));
@@ -2468,6 +2522,14 @@ static int post_process_maps(psm_ctx* c)
     const bool tuned = c->pp_tuned();
     if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
+    if (dc) {
+        // the check reads the selection maps and writes the stage's result (PSM_DCHECK_ONLY, or the post-filter's first
+        // input) or the input of the removal or of the left-right check
+        uint8_t* const out[2] = {sp || lr ? c->dc_maps[0] : c->dis_pp[0], sp || lr ? c->dc_maps[1] : c->dis_pp[1]};
+        if (int rc = disparity_check<T>(c, maps, out)) return rc;
+        if (dc_only) return stage_end(c, 5);
+        maps[0] = out[0]; maps[1] = out[1];
+    }
     if (sp) {
         // the removal reads the selection maps and writes the stage's result (PSM_SPECKLE_ONLY), the check's input, or
         // the post-filter's first input (in place: each pass packs its input before it writes dis_pp)
@@ -2478,10 +2540,16 @@ static int post_process_maps(psm_ctx* c)
     }
     if (lr) {
         // lrCheck + fillInv (PP.cpp:405-406): reads the selection maps, writes the filled maps into dis_pp
+        // (own_fill: the left view alone, its mask from the map itself; the right view's buffers are not touched)
         const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;
-        lr_check_fill_kernel<T><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
-            reinterpret_cast<const T*>(maps[0]), reinterpret_cast<const T*>(maps[1]), c->W,
-            reinterpret_cast<T*>(c->dis_pp[0]), reinterpret_cast<T*>(c->dis_pp[1]), c->lr_valid[0], c->lr_valid[1]);
+        if (own_fill)
+            lr_check_fill_kernel<T, true><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
+                reinterpret_cast<const T*>(maps[0]), nullptr, c->W, reinterpret_cast<T*>(c->dis_pp[0]), nullptr,
+                c->lr_valid[0], nullptr);
+        else
+            lr_check_fill_kernel<T, false><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
+                reinterpret_cast<const T*>(maps[0]), reinterpret_cast<const T*>(maps[1]), c->W,
+                reinterpret_cast<T*>(c->dis_pp[0]), reinterpret_cast<T*>(c->dis_pp[1]), c->lr_valid[0], c->lr_valid[1]);
         PSM_LAUNCH_CHECK(c);
         c->lr_masks_ok = true;
         if (!wmf) return stage_end(c, 5);
@@ -2916,9 +2984,11 @@ int psm_read_valid_mask(psm_ctx* c, int view, uint8_t* dst, size_t dst_step)
     if (int rc = bind(c)) return rc;
     if (view != PSM_LEFT && view != PSM_RIGHT) return fail(c, PSM_EINVAL, "bad view %d", view);
     if (!dst || dst_step < (size_t)c->W) return fail(c, PSM_EINVAL, "bad dst/step");
-    if (c->views == 1)   // the left-right check never runs on a left-only context
+    // the left-right check never runs on a left-only context; the fill after the disparity check masks the left view
+    if (c->views == 1 && (view == PSM_RIGHT || !c->lr_masks_ok))
         return fail(c, PSM_ESTATE, "psm_read_valid_mask on a left-only context (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): the "
-                    "left-right check needs both maps; set PSM_VIEWS_BOTH");
+                    "left-right check needs both maps; set PSM_VIEWS_BOTH, or fill the left view after "
+                    "psm_set_disparity_check(PSM_DCHECK_FIRST)");
     if (!c->lr_masks_ok)
         return fail(c, PSM_ESTATE, "no valid mask: the last post-process since the last selection stage did not run the left-right check");
     PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->lr_valid[view], c->W, c->W, c->H, cudaMemcpyDeviceToHost, c->stream));

@@ -63,9 +63,12 @@ __device__ __forceinline__ int2 lr_block_scan(int2 v, int2& carry, int2* warp_pa
 
 // l, r: the maps to check (read only); out_l, out_r: the filled maps; valid_l, valid_r: the masks (0/1).  One CTA of
 // kLrThreads threads per row, bounded for eight CTAs per SM (without the bound ptxas spills a register on u16 maps);
-// dynamic shared memory W * (2 * sizeof(T) + 2) bytes when W <= kLrStageCols, else none.
-template <typename T>
-__global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* __restrict__ l, const T* __restrict__ r, int W,
+// dynamic shared memory W * (2 * sizeof(T) + 2) bytes when W <= kLrStageCols, else none.  kOwn: the left view alone,
+// its mask its own map >= 2 instead of the check against the right view (the fill of a left-only context after
+// psm_set_disparity_check); r, out_r and valid_r are never touched and may be null.  It is bounded for six CTAs per SM:
+// at eight ptxas spills.
+template <typename T, bool kOwn>
+__global__ void __launch_bounds__(kLrThreads, kOwn ? 6 : 8) lr_check_fill_kernel(const T* __restrict__ l, const T* __restrict__ r, int W,
                                                                    T* __restrict__ out_l, T* __restrict__ out_r,
                                                                    uint8_t* valid_l, uint8_t* valid_r)
 {
@@ -74,13 +77,17 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
     const size_t row = (size_t)blockIdx.x * W;
     const bool staged = W <= kLrStageCols;
     const T* ml = l + row;
-    const T* mr = r + row;
+    constexpr bool kRight = !kOwn;   // the right view's half of every step
+    const T* mr = kRight ? r + row : nullptr;
     uint8_t* vl = valid_l + row;
-    uint8_t* vr = valid_r + row;
+    uint8_t* vr = kRight ? valid_r + row : nullptr;
     if (staged) {
         T* sl = reinterpret_cast<T*>(lr_smem);
         T* sr = sl + W;
-        for (int x = threadIdx.x; x < W; x += kLrThreads) { sl[x] = __ldg(ml + x); sr[x] = __ldg(mr + x); }
+        for (int x = threadIdx.x; x < W; x += kLrThreads) {
+            sl[x] = __ldg(ml + x);
+            if constexpr (kRight) sr[x] = __ldg(mr + x);
+        }
         ml = sl; mr = sr;
         vl = reinterpret_cast<uint8_t*>(sr + W);
         vr = vl + W;
@@ -89,13 +96,24 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
     // the check, on the unmodified maps
     int2 own_last = make_int2(-1, -1);
     for (int x = threadIdx.x; x < W; x += kLrThreads) {
-        const int dl = ml[x], dr = mr[x];
-        int xl = (x - dl) % W;
-        if (xl < 0) xl += W;
-        const int xr = (int)(((unsigned)x + (unsigned)dr) % (unsigned)W);
-        const uint8_t okl = dl >= 2 && dl == (int)mr[xl], okr = dr >= 2 && dr == (int)ml[xr];
-        vl[x] = okl; vr[x] = okr;
-        if (staged) { valid_l[row + x] = okl; valid_r[row + x] = okr; }
+        const int dl = ml[x], dr = kRight ? mr[x] : 0;
+        uint8_t okl, okr;
+        if constexpr (kOwn) {
+            okl = dl >= 2;
+            okr = 0;
+        } else {
+            int xl = (x - dl) % W;
+            if (xl < 0) xl += W;
+            const int xr = (int)(((unsigned)x + (unsigned)dr) % (unsigned)W);
+            okl = dl >= 2 && dl == (int)mr[xl];
+            okr = dr >= 2 && dr == (int)ml[xr];
+        }
+        vl[x] = okl;
+        if constexpr (kRight) vr[x] = okr;
+        if (staged) {
+            valid_l[row + x] = okl;
+            if constexpr (kRight) valid_r[row + x] = okr;
+        }
         if (okl) own_last.x = x;
         if (okr) own_last.y = x;
     }
@@ -105,7 +123,7 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
     lr_block_scan<true>(own_last, last, warp_part);
     // right to left: R = the nearest valid column at or right of x (W: none); out = map[R], or map[x] without an R
     T* ol = out_l + row;
-    T* orr = out_r + row;
+    T* orr = kRight ? out_r + row : nullptr;
     const int nchunks = (W + kLrChunk - 1) / kLrChunk;
     int2 carry = make_int2(W, W);
     for (int c = nchunks - 1; c >= 0; --c) {
@@ -116,7 +134,7 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
             const int x = x0 + i;
             if (x < W) {
                 if (vl[x]) own.x = x;
-                if (vr[x]) own.y = x;
+                if (kRight && vr[x]) own.y = x;
             }
         }
         int2 nxt = lr_block_scan<false>(own, carry, warp_part);
@@ -125,9 +143,9 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
             const int x = x0 + i;
             if (x < W) {
                 if (vl[x]) nxt.x = x;
-                if (vr[x]) nxt.y = x;
+                if (kRight && vr[x]) nxt.y = x;
                 ol[x] = ml[nxt.x < W ? nxt.x : x];
-                orr[x] = mr[nxt.y < W ? nxt.y : x];
+                if constexpr (kRight) orr[x] = mr[nxt.y < W ? nxt.y : x];
             }
         }
     }
@@ -141,7 +159,7 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
             const int x = x0 + i;
             if (x < W) {
                 if (vl[x]) own.x = x;
-                if (vr[x]) own.y = x;
+                if (kRight && vr[x]) own.y = x;
             }
         }
         int2 prv = lr_block_scan<true>(own, carry, warp_part);
@@ -149,7 +167,7 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
         for (int i = 0; i < kLrItems; ++i) {
             const int x = x0 + i;
             if (x < W) {
-                const bool gl = vl[x], gr = vr[x];
+                const bool gl = vl[x], gr = kRight && vr[x];
                 if (gl) prv.x = x;
                 if (gr) prv.y = x;
                 // ol[x] holds map[R] where x <= last, else map[x]: then map[L] alone
@@ -157,7 +175,7 @@ __global__ void __launch_bounds__(kLrThreads, 8) lr_check_fill_kernel(const T* _
                     const T a = ml[prv.x], b = ol[x];
                     ol[x] = x <= last.x && b < a ? b : a;
                 }
-                if (!gr && prv.y >= 0) {
+                if (kRight && !gr && prv.y >= 0) {
                     const T a = mr[prv.y], b = orr[x];
                     orr[x] = x <= last.y && b < a ? b : a;
                 }

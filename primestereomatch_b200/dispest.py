@@ -140,6 +140,7 @@ class DispEst:
         self.rValid = np.zeros((self.hei, self.wid), np.uint8)
         self.lr_mode = capi.PSM_LR_OFF
         self.speckle_mode = capi.PSM_SPECKLE_OFF
+        self.dcheck_mode = capi.PSM_DCHECK_OFF
         self.cost_output = False
         self.lCosts = self.rCosts = None   # setCostOutput(True): DispSelect_GPU's (3, H, W) float32 costs
         self.runner_up_output = False
@@ -247,6 +248,20 @@ class DispEst:
         self._need_gpu()
         capi.check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)), self._ctx)
         self.speckle_mode = int(mode)
+        return 0
+
+    def setDisparityCheck(self, mode, max_diff=1):
+        """One-view disparity check (OpenCV's validateDisparity, StereoSGBM's disp12MaxDiff) for every later
+        PostProcess_GPU call: 0 off (default), 1 first (then setSpeckleFilter's removal and the check and / or post-filter
+        of setLRCheck / setPostFilter on its result), 2 only (its maps are the result; lValid / rValid are not read).  In
+        each row, the pixels at x >= maxDis claim the other view's column their disparity points at, the lowest cost of
+        setCostOutput's centre plane winning; a pixel whose disparity differs from its column's winner's by more than
+        max_diff becomes 0 (invalid).  Needs setCostOutput(True) for the selection it checks.  On a left-only context,
+        mode 1 with setLRCheck 1 or 2 fills the left map where it is below 2 and fills lValid.  Raises PsmError on any
+        other mode, on max_diff outside [0, 4095], or on a context that owns part of the range with the check on."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_disparity_check(self._ctx, int(mode), int(max_diff)), self._ctx)
+        self.dcheck_mode = int(mode)
         return 0
 
     def setRectify(self, left_maps, right_maps, src_size):
@@ -370,13 +385,15 @@ class DispEst:
     def PostProcess_GPU(self):
         """DispEst.cpp:338-344 -> PP::processDM (PP.cpp:402-425): joint weighted-median filter of both maps (after the
         left-right check and fill, or instead of the filter, as setLRCheck selects); the reference runs it on the CPU even
-        in GPU mode, here it is a device stage.  Speckle removal runs first, or alone, as setSpeckleFilter selects.
-        Results replace lDisMap / rDisMap."""
+        in GPU mode, here it is a device stage.  The disparity check and then speckle removal run first, or alone, as
+        setDisparityCheck and setSpeckleFilter select.  Results replace lDisMap / rDisMap."""
         self._need_gpu()
         pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
         capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
-        if self.lr_mode != capi.PSM_LR_OFF and self.speckle_mode != capi.PSM_SPECKLE_ONLY:   # the check ran
-            for view, mask in ((capi.PSM_LEFT, self.lValid), (capi.PSM_RIGHT, self.rValid)):
+        if self.lr_mode != capi.PSM_LR_OFF and self.speckle_mode != capi.PSM_SPECKLE_ONLY \
+                and self.dcheck_mode != capi.PSM_DCHECK_ONLY:   # the check ran (a left-only fill masks the left view)
+            masks = ((capi.PSM_LEFT, self.lValid),) + (((capi.PSM_RIGHT, self.rValid),) if self.rDisMap is not None else ())
+            for view, mask in masks:
                 capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)
         return 0
 

@@ -90,7 +90,9 @@ public:
                       // whose low byte is the reference's uchar map
     cv::Mat rDisMap;
     cv::Mat lValid;   // CV_8UC1 masks of the left-right check (reference DispEst.h:81-82), 0/1; PostProcess_GPU fills them
-    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF (and setSpeckleFilter not PSM_SPECKLE_ONLY)
+    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF (and setSpeckleFilter not PSM_SPECKLE_ONLY,
+                      // setDisparityCheck not PSM_DCHECK_ONLY); lValid alone on a left-only context that fills after
+                      // setDisparityCheck(PSM_DCHECK_FIRST)
     cv::Mat lCosts[3];  // setCostOutput(true): CV_32FC1 filtered costs at disparity m - 1, m, m + 1 of the selection map's
     cv::Mat rCosts[3];  // m (psm_read_costs); DispSelect_GPU fills them, rCosts not on a left-only context
     cv::Mat lRunnerUp[2];  // setRunnerUpOutput(true): CV_32FC1 runner-up disparity r (0 where none exists) and its
@@ -116,6 +118,11 @@ public:
     // (PSM_SPECKLE_ONLY) the check and post-filter for every later PostProcess call; see psm_set_speckle_filter.  A port
     // of a StereoSGBM pipeline calls setSpeckleFilter(PSM_SPECKLE_FIRST, speckleWindowSize, speckleRange).
     int setSpeckleFilter(int mode, int max_size, int max_diff);
+    // One-view disparity check (cv::validateDisparity, StereoSGBM's disp12MaxDiff) in front of (PSM_DCHECK_FIRST) or
+    // instead of (PSM_DCHECK_ONLY) the speckle removal, check and post-filter for every later PostProcess call; see
+    // psm_set_disparity_check.  It reads the winners' costs: call setCostOutput(true) before DispSelect_GPU.  A port of a
+    // StereoSGBM pipeline calls setDisparityCheck(PSM_DCHECK_FIRST, disp12MaxDiff).
+    int setDisparityCheck(int mode, int max_diff);
     // PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT (PSM_OPT_VIEWS): with PSM_VIEWS_LEFT the later frames compute the left
     // map alone; DispSelect_GPU and PostProcess_GPU then leave rDisMap (and rValid) untouched.  The next stage after a
     // change must be CostConst_GPU.
@@ -171,6 +178,7 @@ private:
     unsigned int subsample_rate = 4;
     int lr_mode = PSM_LR_OFF;
     int speckle_mode = PSM_SPECKLE_OFF;
+    int dcheck_mode = PSM_DCHECK_OFF;
     int views = PSM_VIEWS_BOTH;
     int src_w = 0, src_h = 0;   // setRectify: the size of the frames CostConst_GPU takes, 0 = the context's
     bool cost_output = false;

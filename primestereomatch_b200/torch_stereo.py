@@ -87,6 +87,7 @@ class TorchStereo:
         self.views = capi.PSM_VIEWS_BOTH
         self.costs = False   # PSM_OPT_COSTS as match() last set it
         self.runner_up = False   # PSM_OPT_RUNNER_UP as match() last set it
+        self.dcheck = capi.PSM_DCHECK_OFF   # setDisparityCheck's mode
         self._lib = capi.lib()
         self._ctx = C.c_void_p()
         self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
@@ -134,6 +135,12 @@ class TorchStereo:
     def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
         self._check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)))
 
+    def setDisparityCheck(self, mode, max_diff=1):
+        """DispEst.setDisparityCheck.  match(post_process=True) then turns PSM_OPT_COSTS on itself, since the check reads
+        the winners' costs; it returns them only with costs=True."""
+        self._check(self._lib.psm_set_disparity_check(self._ctx, int(mode), int(max_diff)))
+        self.dcheck = int(mode)
+
     def setRectify(self, left_maps, right_maps, src_size):
         """DispEst.setRectify: from then on match takes uint8 camera frames of (SH, SW) in any layout frame_layout reads
         -- the two halves of one side-by-side tensor included -- and rectifies them on the device; float frames raise
@@ -175,7 +182,8 @@ class TorchStereo:
         costs=True -> (lmap, rmap, lcosts, rcosts): also the filtered costs beside each winner of the selection maps
         (PSM_OPT_COSTS, psm_copy_costs_device), new float32 tensors (3, H, W) or (B, 3, H, W) whose plane k holds the cost
         at disparity m + k - 1, bit for bit (the quiet NaN 0x7FC00000 outside [min_disp, max_disp)); rcosts is None on a
-        left-only context.  The option is set when costs differs from the last call's, which restarts the frame.
+        left-only context.  The option is set when it differs from the last call's, which restarts the frame; with
+        setDisparityCheck on and post_process=True it is on whatever costs says.
 
         runner_up=True -> also (lrunner, rrunner), appended after any costs: each pixel's runner-up away from the winner
         (PSM_OPT_RUNNER_UP, psm_copy_runner_up_device), new float32 tensors (2, H, W) or (B, 2, H, W): plane 0 the
@@ -189,9 +197,9 @@ class TorchStereo:
 
         After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
-        with post_process=True (the chain setSpeckleFilter, setLRCheck and setPostFilter configure), psm_copy_maps_device
-        and, with points, psm_reproject_device of each frame of a batch in turn; then psm_signal_stream.  No
-        host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
+        with post_process=True (the chain setDisparityCheck, setSpeckleFilter, setLRCheck and setPostFilter configure),
+        psm_copy_maps_device and, with points, psm_reproject_device of each frame of a batch in turn; then
+        psm_signal_stream.  No host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
         wanted = (costs, runner_up)
         for (name, *_), on in zip(_OUTPUTS, wanted):
             if not isinstance(on, bool):
@@ -219,9 +227,11 @@ class TorchStereo:
         row = W * lmap.element_size()
         outs = []   # (copy-out call, left planes, right planes) of each output asked for
         for (name, key, n, copy), on in zip(_OUTPUTS, wanted):
-            if on != getattr(self, name):
-                self._check(L.psm_set_option(ctx, key, int(on)))
-                setattr(self, name, on)
+            # the disparity check of the post-process reads the costs
+            option = on or (key == capi.PSM_OPT_COSTS and post_process and self.dcheck != capi.PSM_DCHECK_OFF)
+            if option != getattr(self, name):
+                self._check(L.psm_set_option(ctx, key, int(option)))
+                setattr(self, name, option)
             if on:
                 oshape = (len(lf), n, H, W) if batched else (n, H, W)
                 outs.append((getattr(L, copy), torch.empty(oshape, dtype=torch.float32, device=self.device),
