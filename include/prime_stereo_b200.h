@@ -486,6 +486,43 @@ int psm_set_rectify(psm_ctx* ctx, int src_width, int src_height,
                     const int16_t* xy_left, size_t xy_left_step, const uint16_t* a_left, size_t a_left_step,
                     const int16_t* xy_right, size_t xy_right_step, const uint16_t* a_right, size_t a_right_step);
 
+/* YUV frames (NVDEC surfaces, UVC cameras), converted to BGR in ingest.  A frame of Wf x Hf (the context's W x H, or the
+ * source size while psm_set_rectify is on) has luma Y(x, y) and chroma U, V at (x >> 1, y >> vs), vs = 1 for 4:2:0 and 0
+ * for 4:2:2.  Its BGR pixel is OpenCV's cvtColor(COLOR_YUV2BGR_*) (BT.601 limited range, fixed point, cv2 4.13.0), each
+ * value clamped to 0..255:
+ *   y' = max(0, Y - 16) * 1220542,  u = U - 128,  v = V - 128,  h = 1 << 19
+ *   R = (y' + h + 1673527 v) >> 20,  G = (y' + h - 852492 v - 409993 u) >> 20,  B = (y' + h + 2116026 u) >> 20
+ * and that u8 frame is ingested exactly as psm_set_images_u8 ingests it; with psm_set_rectify on, the frame is
+ * remap(cvtColor(yuv), xy, a, INTER_LINEAR), each tap the converted pixel at its source position.  Wf must be even, and
+ * Hf too for 4:2:0, as cv2 requires.  BT.709, full-range and 10-bit (P010 / P016) frames are not accepted: cv2 defines no
+ * such conversion to pin them to.  One ingest_kernel launch and one halo pass per view, as for u8 frames.
+ *
+ * psm_set_images_device_yuv: device frames read in place, ordered like psm_set_images_device_planes (psm_wait_stream /
+ * psm_signal_stream).  left[k] / right[k] point at Y, U, V of pixel (0, 0): Y(x, y) at p[0] + y * y_row_step + x *
+ * y_col_step, U and V at p[1] / p[2] + (y >> vs) * c_row_step + (x >> 1) * c_col_step (bytes).  Separate luma and chroma
+ * pitches (NVDEC) and the two halves of one side-by-side frame fit:
+ *   NV12   Y p, 1;  U uv + 0, V uv + 1, c_col_step 2        I420   Y, U, V planes, c_col_step 1
+ *   YUYV   Y p + 0, y_col_step 2;  U p + 1, V p + 3, c_col_step 4 (UYVY: U p, Y p + 1, V p + 2; YVYU: V p + 1, U p + 3)
+ * psm_set_images_yuv / _yuv_async (finished by psm_set_images_commit): HOST frames in cv2's contiguous layouts, rows
+ * `step` bytes apart: 4:2:0 formats are Hf * 3 / 2 rows (the luma rows, then the chroma; I420 and YV12 need step == Wf),
+ * 4:2:2 formats Hf rows of 2 * Wf bytes.  They are copied into the u8 staging sets (1.5 or 2 bytes per pixel), so no
+ * frame allocates, and converted in ingest; buffers reusable as for psm_set_images_u8 / _u8_async.
+ *   - PSM_EINVAL before any CUDA work, context unchanged: an unknown format or sampling, a null pointer, an odd Wf or (4:2:0)
+ *     Hf, a step below what a row spans (y_row_step < (Wf - 1) * y_col_step + 1, c_row_step < (Wf / 2 - 1) * c_col_step
+ *     + 1, a zero column step, a host step below Wf or 2 * Wf).  psm_set_images_yuv_async returns PSM_ESTATE while
+ *     another asynchronous upload is pending, and PSM_EINVAL on a multi-device context, as psm_set_images_u8_async does.
+ *   - Multi-device contexts read the frame on the first device; the other shards receive its ingested planes.
+ * See DESIGN.md section 27. */
+enum { PSM_YUV_420 = 1, PSM_YUV_422 = 2 };
+enum { PSM_YUV_NV12 = 1, PSM_YUV_NV21 = 2, PSM_YUV_I420 = 3, PSM_YUV_YV12 = 4, PSM_YUV_YUYV = 5, PSM_YUV_UYVY = 6,
+       PSM_YUV_YVYU = 7 };
+int psm_set_images_device_yuv(psm_ctx* ctx, int sampling, const void* const left[3], const void* const right[3],
+                              size_t y_row_step, size_t y_col_step, size_t c_row_step, size_t c_col_step);
+int psm_set_images_yuv(psm_ctx* ctx, int format, const uint8_t* left, size_t left_step, const uint8_t* right,
+                       size_t right_step);
+int psm_set_images_yuv_async(psm_ctx* ctx, int format, const uint8_t* left, size_t left_step, const uint8_t* right,
+                             size_t right_step);
+
 /* Pipelined upload (extension; the reference's DispEst is synchronous per frame): start the H2D copy
  * of the NEXT frame on the context's copy stream into a second staging set while the current frame
  * is still being computed, then make it the current frame.  Host buffers must be page-locked for the

@@ -25,6 +25,7 @@ SYMBOLS = [
     "psm_create_blocked", "psm_create_multi", "psm_set_images_device_planes", "psm_wait_stream", "psm_signal_stream",
     "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs", "psm_copy_runner_up_device", "psm_read_runner_up",
     "psm_create_range", "psm_set_speckle_filter", "psm_set_disparity_check", "psm_reproject_device", "psm_read_points", "psm_set_rectify",
+    "psm_set_images_device_yuv", "psm_set_images_yuv", "psm_set_images_yuv_async",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -40,6 +41,12 @@ PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL = 0, 1, 2
 PSM_SPECKLE_OFF, PSM_SPECKLE_FIRST, PSM_SPECKLE_ONLY = 0, 1, 2
 PSM_DCHECK_OFF, PSM_DCHECK_FIRST, PSM_DCHECK_ONLY = 0, 1, 2
 PSM_PIX_U8, PSM_PIX_F32 = 1, 2
+PSM_YUV_420, PSM_YUV_422 = 1, 2
+PSM_YUV_NV12, PSM_YUV_NV21, PSM_YUV_I420, PSM_YUV_YV12, PSM_YUV_YUYV, PSM_YUV_UYVY, PSM_YUV_YVYU = 1, 2, 3, 4, 5, 6, 7
+# the YUV formats by cv2's name (COLOR_YUV2BGR_<name>), and which are 4:2:0
+YUV_FORMATS = {"nv12": PSM_YUV_NV12, "nv21": PSM_YUV_NV21, "i420": PSM_YUV_I420, "yv12": PSM_YUV_YV12,
+               "yuyv": PSM_YUV_YUYV, "uyvy": PSM_YUV_UYVY, "yvyu": PSM_YUV_YVYU}
+YUV_420 = ("nv12", "nv21", "i420", "yv12")
 
 _lib = None
 
@@ -89,6 +96,9 @@ def lib():
     L.psm_set_images_u8.argtypes = [vp, u8p, sz, u8p, sz]
     L.psm_set_images_device.argtypes = [vp, fp, sz, fp, sz]
     L.psm_set_images_device_planes.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), sz, sz]
+    L.psm_set_images_device_yuv.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), sz, sz, sz, sz]
+    L.psm_set_images_yuv.argtypes = [vp, i, u8p, sz, u8p, sz]
+    L.psm_set_images_yuv_async.argtypes = [vp, i, u8p, sz, u8p, sz]
     L.psm_wait_stream.argtypes = [vp, vp]
     L.psm_signal_stream.argtypes = [vp, vp]
     L.psm_copy_maps_device.argtypes = [vp, i, vp, sz, vp, sz]

@@ -81,7 +81,7 @@ struct psm_ctx {
     cudaEvent_t ingest_done[2] = {nullptr, nullptr};  // ingest kernels consumed staging set k (recorded on the compute stream)
     bool ingest_done_valid[2] = {false, false};
     int stage_cur = 0;                      // staging set holding the current frame: 0 = stage_in, 1 = stage_alt
-    int up_pending = 0;                     // pixel type (PSM_PIX_*) of the pending asynchronous upload, 0 none
+    int up_pending = 0;                     // frame format (PSM_PIX_* or kFmtYuv + PSM_YUV_*) of the pending asynchronous upload, 0 none
     uint8_t* dis[2] = {nullptr, nullptr};    // disparity maps: u8, or u16 (map_bytes = 2, psm_create_u16) behind the same pointer
     int map_bytes = 1;                       // bytes per disparity-map element
     // Fast Guided Filter branch (lazy): low-res guide planes per view, low-res coefficient scratch, up-sampling plan
@@ -300,12 +300,45 @@ void images_ingested(psm_ctx* c, bool float_images)
 
 size_t pix_bytes(int pix) { return pix == PSM_PIX_U8 ? 1 : sizeof(float); }
 
+// A host frame's format: PSM_PIX_U8 or PSM_PIX_F32 for interleaved BGR, kFmtYuv + PSM_YUV_* for a YUV frame in cv2's
+// contiguous layout (psm_set_images_yuv).  Uploads, staging sets and the asynchronous commit go by it.
+constexpr int kFmtYuv = 16;
+bool is_yuv(int fmt) { return fmt > kFmtYuv; }
+int yuv_vs(int format) { return format <= PSM_YUV_YV12 ? 1 : 0; }   // the chroma row shift: 1 for 4:2:0, 0 for 4:2:2
+
+// bytes of one row, and rows, of a host frame of format fmt as the staging sets hold it
+size_t host_row_bytes(psm_ctx* c, int fmt)
+{
+    if (is_yuv(fmt)) return (size_t)c->frame_w() * (yuv_vs(fmt - kFmtYuv) ? 1 : 2);
+    return (size_t)c->frame_w() * 3 * pix_bytes(fmt);
+}
+int host_rows(psm_ctx* c, int fmt) { return is_yuv(fmt) && yuv_vs(fmt - kFmtYuv) ? c->frame_h() / 2 * 3 : c->frame_h(); }
+
+// the YuvSrc of a YUV frame of format PSM_YUV_* in cv2's layout at p, rows `step` bytes apart, of the context's frame
+// size: 4:2:0 frames are the luma rows followed by the chroma (NV12 / NV21: interleaved U, V rows of `step` bytes; I420 /
+// YV12: two planes of Wf / 2 x Hf / 2, step == Wf), 4:2:2 frames rows of packed pairs (YUYV: Y0 U Y1 V)
+YuvSrc yuv_host_src(psm_ctx* c, int format, const void* p, size_t step)
+{
+    const char* b = static_cast<const char*>(p);
+    const char* uv = b + (size_t)c->frame_h() * step;
+    const size_t cw = (size_t)c->frame_w() / 2, q = cw * (c->frame_h() / 2);
+    switch (format) {
+    case PSM_YUV_NV12: return YuvSrc{{b, uv, uv + 1}, step, 1, step, 2, 1};
+    case PSM_YUV_NV21: return YuvSrc{{b, uv + 1, uv}, step, 1, step, 2, 1};
+    case PSM_YUV_I420: return YuvSrc{{b, uv, uv + q}, step, 1, cw, 1, 1};
+    case PSM_YUV_YV12: return YuvSrc{{b, uv + q, uv}, step, 1, cw, 1, 1};
+    case PSM_YUV_YUYV: return YuvSrc{{b, b + 1, b + 3}, step, 2, step, 4, 0};
+    case PSM_YUV_UYVY: return YuvSrc{{b + 1, b, b + 2}, step, 2, step, 4, 0};
+    default: return YuvSrc{{b, b + 3, b + 1}, step, 2, step, 4, 0};   // PSM_YUV_YVYU
+    }
+}
+
 // the frame's planes, gradients and ingest flags: one ingest_kernel launch and one pad_rows per view on the context's
-// stream.  With psm_set_rectify on, the frame (u8, checked by the caller) is read through each view's maps.
-int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
+// stream.  With psm_set_rectify on, the frame (u8 or YUV, checked by the caller) is read through each view's maps.
+template <typename T, class Src>
+int ingest(psm_ctx* c, const Src src[2])
 {
     PSM_CUDA(c, cudaMemsetAsync(c->guide_flags, 0, 2 * sizeof(int), c->stream));
-    const auto kernel = pix == PSM_PIX_U8 ? ingest_kernel<uint8_t> : ingest_kernel<float>;
     for (int v = 0; v < 2; ++v) {
         float* g = c->guide[v];
         dim3 blk(128), grd((c->W + 3 + 127) / 128, c->H);
@@ -314,38 +347,52 @@ int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
                                           c->guide_flags + v);
         };
         if (c->rect_sw)
-            launch(ingest_kernel<uint8_t, RectifySrc>,
-                   RectifySrc{src[v], c->rect_xy[v], c->rect_a[v], c->rect_sw, c->rect_sh, c->W});
+            launch(ingest_kernel<uint8_t, RectifySrc<Src>>,
+                   RectifySrc<Src>{src[v], c->rect_xy[v], c->rect_a[v], c->rect_sw, c->rect_sh, c->W});
         else
-            launch(kernel, src[v]);
+            launch(ingest_kernel<T, Src>, src[v]);
         PSM_LAUNCH_CHECK(c);
         if (int rc = pad_rows(c, g, (size_t)3 * c->H)) return rc;  // mirrored halo of the 3 guide channels
     }
-    images_ingested(c, pix != PSM_PIX_U8);
+    images_ingested(c, !std::is_same<T, uint8_t>::value);
     return PSM_OK;
 }
 
-// Copy a checked interleaved host frame into staging set `set` on the copy stream and record `done` there.  The copy
-// starts once the last ingest from that set has read it, so that it does not queue behind the compute stream's backlog.
-int upload(psm_ctx* c, int set, int pix, const PlanesSrc src[2], cudaEvent_t done)
+int ingest(psm_ctx* c, int pix, const PlanesSrc src[2])
 {
-    const size_t row_bytes = (size_t)c->frame_w() * 3 * pix_bytes(pix);
+    return pix == PSM_PIX_U8 ? ingest<uint8_t>(c, src) : ingest<float>(c, src);
+}
+
+// Copy a checked host frame of format fmt (src[v].ch[0] its first byte, src[v].row_step its row step) into staging set
+// `set` on the copy stream and record `done` there.  The copy starts once the last ingest from that set has read it, so
+// that it does not queue behind the compute stream's backlog.
+int upload(psm_ctx* c, int set, int fmt, const PlanesSrc src[2], cudaEvent_t done)
+{
+    const size_t row_bytes = host_row_bytes(c, fmt);
     if (c->ingest_done_valid[set]) PSM_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ingest_done[set], 0));
     for (int v = 0; v < 2; ++v)
         PSM_CUDA(c, cudaMemcpy2DAsync(stage_buf(c, set, v), row_bytes, src[v].ch[0], src[v].row_step, row_bytes,
-                                      c->frame_h(), cudaMemcpyHostToDevice, c->copy_stream));
+                                      host_rows(c, fmt), cudaMemcpyHostToDevice, c->copy_stream));
     PSM_CUDA(c, cudaEventRecord(done, c->copy_stream));
     return PSM_OK;
 }
 
-// ingest staging set `set` once the copy that filled it (`copied`) is done; the next copy into the set waits for this
-int ingest_staged(psm_ctx* c, int set, int pix, cudaEvent_t copied)
+// ingest staging set `set`, which holds a frame of format fmt, once the copy that filled it (`copied`) is done; the next
+// copy into the set waits for this
+int ingest_staged(psm_ctx* c, int set, int fmt, cudaEvent_t copied)
 {
     PSM_CUDA(c, cudaStreamWaitEvent(c->stream, copied, 0));
-    const size_t elem = pix_bytes(pix), row_bytes = (size_t)c->frame_w() * 3 * elem;
-    const PlanesSrc src[2] = {interleaved_src(stage_buf(c, set, 0), elem, row_bytes),
-                              interleaved_src(stage_buf(c, set, 1), elem, row_bytes)};
-    if (int rc = ingest(c, pix, src)) return rc;
+    const size_t row_bytes = host_row_bytes(c, fmt);
+    if (is_yuv(fmt)) {
+        const YuvSrc src[2] = {yuv_host_src(c, fmt - kFmtYuv, stage_buf(c, set, 0), row_bytes),
+                               yuv_host_src(c, fmt - kFmtYuv, stage_buf(c, set, 1), row_bytes)};
+        if (int rc = ingest<uint8_t>(c, src)) return rc;
+    } else {
+        const size_t elem = pix_bytes(fmt);
+        const PlanesSrc src[2] = {interleaved_src(stage_buf(c, set, 0), elem, row_bytes),
+                                  interleaved_src(stage_buf(c, set, 1), elem, row_bytes)};
+        if (int rc = ingest(c, fmt, src)) return rc;
+    }
     PSM_CUDA(c, cudaEventRecord(c->ingest_done[set], c->stream));
     c->ingest_done_valid[set] = true;
     return PSM_OK;
@@ -413,21 +460,83 @@ int check_planes(psm_ctx* c, int pix_type, const void* const left[3], const void
     return PSM_OK;
 }
 
+// a YUV frame of the context's frame size with chroma rows y >> vs: cv2 converts even widths, and even heights for 4:2:0
+int check_yuv_size(psm_ctx* c, int vs)
+{
+    if (c->frame_w() % 2 || (vs && c->frame_h() % 2))
+        return fail(c, PSM_EINVAL, "YUV frame of %d x %d: the width must be even%s", c->frame_w(), c->frame_h(),
+                    vs ? ", and the height too for 4:2:0" : "");
+    return PSM_OK;
+}
+
+// psm_set_images_yuv[_async]: two host frames of format PSM_YUV_* -> src (ch[0] and row_step, as upload reads them), or
+// PSM_EINVAL before any CUDA call
+int check_yuv_host(psm_ctx* c, int format, const void* l, size_t lstep, const void* r, size_t rstep, PlanesSrc src[2])
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (format < PSM_YUV_NV12 || format > PSM_YUV_YVYU)
+        return fail(c, PSM_EINVAL, "unknown YUV format %d (PSM_YUV_NV12 = 1 .. PSM_YUV_YVYU = 7)", format);
+    if (int rc = check_yuv_size(c, yuv_vs(format))) return rc;
+    const void* p[2] = {l, r};
+    const size_t step[2] = {lstep, rstep};
+    const size_t row = host_row_bytes(c, kFmtYuv + format);
+    const bool planar = format == PSM_YUV_I420 || format == PSM_YUV_YV12;
+    for (int v = 0; v < 2; ++v) {
+        if (!p[v]) return fail(c, PSM_EINVAL, "null frame pointer for view %d", v);
+        if (step[v] < row) return fail(c, PSM_EINVAL, "step %zu of view %d is below the %zu bytes of a row", step[v], v, row);
+        if (planar && step[v] != row)
+            return fail(c, PSM_EINVAL, "step %zu of view %d: I420 / YV12 frames are contiguous (step == width %zu)", step[v],
+                        v, row);
+        src[v] = PlanesSrc{{static_cast<const char*>(p[v]), nullptr, nullptr}, step[v], 0};
+    }
+    return PSM_OK;
+}
+
+// psm_set_images_device_yuv: the caller's two frames and their layout -> src, or PSM_EINVAL before any CUDA call
+int check_yuv_device(psm_ctx* c, int sampling, const void* const left[3], const void* const right[3], size_t y_row_step,
+                     size_t y_col_step, size_t c_row_step, size_t c_col_step, YuvSrc src[2])
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (sampling != PSM_YUV_420 && sampling != PSM_YUV_422)
+        return fail(c, PSM_EINVAL, "unknown YUV sampling %d (PSM_YUV_420 = 1, PSM_YUV_422 = 2)", sampling);
+    const int vs = sampling == PSM_YUV_420;
+    if (int rc = check_yuv_size(c, vs)) return rc;
+    const void* const* p[2] = {left, right};
+    for (int v = 0; v < 2; ++v) {
+        if (!p[v]) return fail(c, PSM_EINVAL, "null Y, U, V pointer array for view %d", v);
+        for (int k = 0; k < 3; ++k)
+            if (!p[v][k]) return fail(c, PSM_EINVAL, "null %c pointer of view %d", "YUV"[k], v);
+        src[v] = YuvSrc{{static_cast<const char*>(p[v][0]), static_cast<const char*>(p[v][1]),
+                         static_cast<const char*>(p[v][2])}, y_row_step, y_col_step, c_row_step, c_col_step, vs};
+    }
+    // a row of n samples col_step apart spans (n - 1) * col_step + 1 bytes
+    auto short_row = [](size_t row_step, size_t col_step, size_t n) {
+        return !col_step || (n > 1 && col_step > (SIZE_MAX - 1) / (n - 1)) || row_step < (n - 1) * col_step + 1;
+    };
+    if (short_row(y_row_step, y_col_step, c->frame_w()))
+        return fail(c, PSM_EINVAL, "y_row_step %zu / y_col_step %zu: the column step must be nonzero and a row of %d luma "
+                    "samples fit in the row step", y_row_step, y_col_step, c->frame_w());
+    if (short_row(c_row_step, c_col_step, c->frame_w() / 2))
+        return fail(c, PSM_EINVAL, "c_row_step %zu / c_col_step %zu: the column step must be nonzero and a row of %d chroma "
+                    "samples fit in the row step", c_row_step, c_col_step, c->frame_w() / 2);
+    return PSM_OK;
+}
+
 // how a checked frame reaches the context: host buffers through a staging set, or device memory read in place
 enum class Frame { host, device, planes };
 
 // stage 0 of one context.  A host frame is copied into the current staging set and ingested from there; the call returns
 // once the copy has read the caller's buffers (from page-locked memory it would otherwise still be reading them after the
 // return).  A device frame is ingested in place.
-int set_images_one(psm_ctx* c, Frame kind, int pix, const PlanesSrc src[2])
+int set_images_one(psm_ctx* c, Frame kind, int fmt, const PlanesSrc src[2])
 {
     if (int rc = bind(c)) return rc;
     if (int rc = stage_begin(c, 0)) return rc;
     if (kind == Frame::host) {
-        if (int rc = upload(c, c->stage_cur, pix, src, c->host_copied)) return rc;
-        if (int rc = ingest_staged(c, c->stage_cur, pix, c->host_copied)) return rc;
+        if (int rc = upload(c, c->stage_cur, fmt, src, c->host_copied)) return rc;
+        if (int rc = ingest_staged(c, c->stage_cur, fmt, c->host_copied)) return rc;
         PSM_CUDA(c, cudaEventSynchronize(c->host_copied));
-    } else if (int rc = ingest(c, pix, src)) {
+    } else if (int rc = ingest(c, fmt, src)) {
         return rc;
     }
     return stage_end(c, 0);
@@ -1069,7 +1178,7 @@ int multi_send_planes(psm_ctx* c, int pix)
         PSM_CUDA(c, cudaMemcpyAsync(s->guide_flags, s0->guide_flags, 2 * sizeof(int), cudaMemcpyDefault, s->stream));
         PSM_CUDA(c, cudaEventRecord(c->ev_copied[k], s->stream));
         PSM_CUDA(c, cudaStreamWaitEvent(s0->stream, c->ev_copied[k], 0));
-        images_ingested(s, pix != PSM_PIX_U8);
+        images_ingested(s, pix == PSM_PIX_F32);
         if ((rc = stage_end(s, 0))) return relay(c, k, rc);
     }
     return PSM_OK;
@@ -1077,27 +1186,43 @@ int multi_send_planes(psm_ctx* c, int pix)
 
 // the body of every synchronous psm_set_images* call once its frame is checked.  A multi-device context runs stage 0 on
 // its first shard and sends the other shards the frame, or the planes the first shard ingested.  With psm_set_rectify on,
-// only the first shard holds the maps, so every kind of frame reaches the others as its planes.
-int set_images(psm_ctx* c, Frame kind, int pix, const PlanesSrc src[2])
+// only the first shard holds the maps, so every kind of frame reaches the others as its planes; so does a YUV frame.
+int set_images(psm_ctx* c, Frame kind, int fmt, const PlanesSrc src[2])
 {
-    if (!is_multi(c)) return set_images_one(c, kind, pix, src);
-    if (int rc = set_images_one(c->shard[0], kind, pix, src)) return relay(c, 0, rc);
-    return kind == Frame::planes || c->rect_sw ? multi_send_planes(c, pix) : multi_send_frame(c, kind, pix, src);
+    if (!is_multi(c)) return set_images_one(c, kind, fmt, src);
+    if (int rc = set_images_one(c->shard[0], kind, fmt, src)) return relay(c, 0, rc);
+    return kind == Frame::planes || c->rect_sw || is_yuv(fmt) ? multi_send_planes(c, fmt)
+                                                              : multi_send_frame(c, kind, fmt, src);
 }
 
-// psm_set_images[_u8]_async: the frame is uploaded into the staging set that is not in use, on the copy stream
-int set_images_async(psm_ctx* c, int pix, const void* l, size_t lstep, const void* r, size_t rstep, const char* call)
+// psm_set_images_device_yuv once its frames are checked: stage 0 on the context (a multi-device context's first shard,
+// whose ingested planes the other shards receive)
+int set_images_device_yuv(psm_ctx* c, const YuvSrc src[2])
+{
+    psm_ctx* s = is_multi(c) ? c->shard[0] : c;
+    int rc = bind(s);
+    if (!rc) rc = stage_begin(s, 0);
+    if (!rc) rc = ingest<uint8_t>(s, src);
+    if (!rc) rc = stage_end(s, 0);
+    if (!is_multi(c)) return rc;
+    return rc ? relay(c, 0, rc) : multi_send_planes(c, PSM_PIX_U8);
+}
+
+// psm_set_images[_u8|_yuv]_async: the frame of format fmt that check(src) checks is uploaded into the staging set that is
+// not in use, on the copy stream
+template <class Check>
+int set_images_async(psm_ctx* c, int fmt, const char* call, Check check)
 {
     if (is_multi(c)) return reject_multi(c, call, "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
     if (int rc = bind(c)) return rc;
     if (c->up_pending) return fail(c, PSM_ESTATE, "an asynchronous upload is already pending: call psm_set_images_commit first");
     PlanesSrc src[2];
-    if (int rc = check_interleaved(c, pix, false, l, lstep, r, rstep, src)) return rc;
+    if (int rc = check(src)) return rc;
     if (!c->stage_alt[0]) {  // allocated on first use: synchronous callers never pay for the second set
         for (int v = 0; v < 2; ++v) PSM_CUDA(c, cudaMalloc(&c->stage_alt[v], c->stage_bytes));
     }
-    if (int rc = upload(c, c->stage_cur ^ 1, pix, src, c->up_done)) return rc;
-    c->up_pending = pix;
+    if (int rc = upload(c, c->stage_cur ^ 1, fmt, src, c->up_done)) return rc;
+    c->up_pending = fmt;
     return PSM_OK;
 }
 
@@ -1909,12 +2034,41 @@ int psm_signal_stream(psm_ctx* c, void* cuda_stream)
 
 int psm_set_images_async(psm_ctx* c, const float* left, size_t left_step, const float* right, size_t right_step)
 {
-    return set_images_async(c, PSM_PIX_F32, left, left_step, right, right_step, "psm_set_images_async");
+    return set_images_async(c, PSM_PIX_F32, "psm_set_images_async", [&](PlanesSrc* src) {
+        return check_interleaved(c, PSM_PIX_F32, false, left, left_step, right, right_step, src);
+    });
 }
 
 int psm_set_images_u8_async(psm_ctx* c, const uint8_t* left, size_t left_step, const uint8_t* right, size_t right_step)
 {
-    return set_images_async(c, PSM_PIX_U8, left, left_step, right, right_step, "psm_set_images_u8_async");
+    return set_images_async(c, PSM_PIX_U8, "psm_set_images_u8_async", [&](PlanesSrc* src) {
+        return check_interleaved(c, PSM_PIX_U8, false, left, left_step, right, right_step, src);
+    });
+}
+
+int psm_set_images_yuv(psm_ctx* c, int format, const uint8_t* left, size_t left_step, const uint8_t* right,
+                       size_t right_step)
+{
+    PlanesSrc src[2];
+    if (int rc = check_yuv_host(c, format, left, left_step, right, right_step, src)) return rc;
+    return set_images(c, Frame::host, kFmtYuv + format, src);
+}
+
+int psm_set_images_yuv_async(psm_ctx* c, int format, const uint8_t* left, size_t left_step, const uint8_t* right,
+                             size_t right_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    return set_images_async(c, kFmtYuv + format, "psm_set_images_yuv_async", [&](PlanesSrc* src) {
+        return check_yuv_host(c, format, left, left_step, right, right_step, src);
+    });
+}
+
+int psm_set_images_device_yuv(psm_ctx* c, int sampling, const void* const left[3], const void* const right[3],
+                              size_t y_row_step, size_t y_col_step, size_t c_row_step, size_t c_col_step)
+{
+    YuvSrc src[2];
+    if (int rc = check_yuv_device(c, sampling, left, right, y_row_step, y_col_step, c_row_step, c_col_step, src)) return rc;
+    return set_images_device_yuv(c, src);
 }
 
 int psm_set_images_commit(psm_ctx* c)
@@ -1922,11 +2076,11 @@ int psm_set_images_commit(psm_ctx* c)
     if (is_multi(c)) return reject_multi(c, "psm_set_images_commit", "the asynchronous upload pipeline is not available on it; use psm_set_images / _u8");
     if (int rc = bind(c)) return rc;
     if (!c->up_pending) return fail(c, PSM_ESTATE, "psm_set_images_commit without a pending psm_set_images_async");
-    const int set = c->stage_cur ^ 1, pix = c->up_pending;
+    const int set = c->stage_cur ^ 1, fmt = c->up_pending;
     if (int rc = stage_begin(c, 0)) return rc;
     c->stage_cur = set;
     c->up_pending = 0;
-    if (int rc = ingest_staged(c, set, pix, c->up_done)) return rc;
+    if (int rc = ingest_staged(c, set, fmt, c->up_done)) return rc;
     if (int rc = stage_end(c, 0)) return rc;
     // the caller may reuse its host buffers once this returns: wait for the copy that reads them (it may still be
     // waiting for the frame before last to leave this staging set); the ingest kernels are already queued behind it

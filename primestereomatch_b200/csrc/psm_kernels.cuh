@@ -44,8 +44,8 @@ __global__ void pad_cols_kernel(float* __restrict__ base, size_t nrows, int W, i
 }
 
 // ------------------------------------------------------------------------------------------
-// Ingest: a BGR frame (float or u8) in any PlanesSrc layout, or a u8 frame read through rectification maps (RectifySrc)
-// -> 3 planar channels + x-gradient of the gray image.
+// Ingest: a BGR frame (float or u8) in any PlanesSrc layout or a YUV frame (YuvSrc); an 8-bit frame of either kind may be
+// read through rectification maps (RectifySrc) -> 3 planar channels + x-gradient of the gray image.
 // Restates StereoMatch.cpp:193-197 (u8 * (1/255.0f)), CVF.cpp:47 (split) and CVC.cpp:41-46
 // (cvtColor RGB2GRAY on the BGR image, Sobel dx=1 ksize=1 with BORDER_REFLECT_101).
 // ------------------------------------------------------------------------------------------
@@ -87,11 +87,22 @@ inline PlanesSrc interleaved_src(const void* p, size_t elem, size_t step)
     return PlanesSrc{{b, b + elem, b + 2 * elem}, step, 3 * elem};
 }
 
-// A u8 frame of SW x SH read through the rectification maps of one view (psm_set_rectify): output pixel (x, y) of the
-// W x H crop is OpenCV's remap(frame, xy, a, INTER_LINEAR, BORDER_CONSTANT 0) with the fixed-point maps of
-// initUndistortRectifyMap(..., CV_16SC2), cropped (DESIGN.md section 25).  The maps are dense: entry (x, y) at y * W + x.
+// A YUV frame (psm_set_images_yuv / psm_set_images_device_yuv): luma Y(x, y) at p[0] + y * y_row_step + x * y_col_step,
+// chroma U and V at (x >> 1, y >> vs) of p[1] / p[2] with the chroma steps; vs = 1 for 4:2:0, 0 for 4:2:2.  NV12 / NV21,
+// I420 / YV12 and the packed YUYV / UYVY / YVYU layouts differ only in these offsets and steps (DESIGN.md section 27).
+struct YuvSrc {
+    const char* p[3];   // Y, U, V
+    size_t y_row_step, y_col_step, c_row_step, c_col_step;
+    int vs;
+};
+
+// A u8 frame of SW x SH, BGR (PlanesSrc) or YUV (YuvSrc), read through the rectification maps of one view
+// (psm_set_rectify): output pixel (x, y) of the W x H crop is OpenCV's remap(frame, xy, a, INTER_LINEAR, BORDER_CONSTANT 0)
+// with the fixed-point maps of initUndistortRectifyMap(..., CV_16SC2), cropped (DESIGN.md section 25); a YUV frame is
+// remapped as the BGR frame cvtColor makes of it.  The maps are dense: entry (x, y) at y * W + x.
+template <class F>
 struct RectifySrc {
-    PlanesSrc frame;           // the source frame, SW x SH
+    F frame;                   // the source frame, SW x SH
     const short2* xy;          // map[0]: the integer tap (sx, sy)
     const uint16_t* a;         // map[1]: the 5 + 5-bit fraction (fy << 5 | fx); bits above 10 are ignored
     int SW, SH, W;
@@ -104,28 +115,76 @@ __device__ __forceinline__ float read_sample(const PlanesSrc& src, size_t row, i
     return to_f32(*reinterpret_cast<const T*>(src.ch[c] + row + (size_t)x * src.col_step));
 }
 
-// channel c of rectified pixel (x, y): the four taps' weights sum to 32768, a tap outside the frame reads 0, and the
-// integer sum is rounded like OpenCV's FixedPtCast (+ 2^14, >> 15), so the value is the u8 remap writes.  Every tap is
-// bounds-checked before it is read, so any map is memory-safe.
-template <typename T>
-__device__ __forceinline__ float read_sample(const RectifySrc& src, size_t, int c, int x, int y)
+// tap(sx, sy, w) for each tap of rectified pixel (x, y) inside the frame: the four taps' weights w sum to 32768 and a tap
+// outside the frame reads 0.  Every tap is bounds-checked before it is read, so any map is memory-safe.
+template <class F, class Tap>
+__device__ __forceinline__ void remap_taps(const RectifySrc<F>& src, int x, int y, Tap tap)
 {
-    static_assert(std::is_same<T, uint8_t>::value, "rectification reads 8-bit frames");
     const size_t i = (size_t)y * src.W + x;
     const short2 p = src.xy[i];
     const int a = src.a[i] & 1023, fx = a & 31, fy = a >> 5;
     const int wx[2] = {32 - fx, fx}, wy[2] = {32 - fy, fy};
-    int acc = 0;
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy)
 #pragma unroll
         for (int dx = 0; dx < 2; ++dx) {
             const int sx = p.x + dx, sy = p.y + dy;
-            if ((unsigned)sx < (unsigned)src.SW && (unsigned)sy < (unsigned)src.SH)
-                acc += wx[dx] * wy[dy] * 32 * *reinterpret_cast<const uint8_t*>(
-                           src.frame.ch[c] + (size_t)sy * src.frame.row_step + (size_t)sx * src.frame.col_step);
+            if ((unsigned)sx < (unsigned)src.SW && (unsigned)sy < (unsigned)src.SH) tap(sx, sy, wx[dx] * wy[dy] * 32);
         }
+}
+
+// channel c of rectified pixel (x, y): the integer sum is rounded like OpenCV's FixedPtCast (+ 2^14, >> 15), so the
+// value is the u8 remap writes
+template <typename T>
+__device__ __forceinline__ float read_sample(const RectifySrc<PlanesSrc>& src, size_t, int c, int x, int y)
+{
+    static_assert(std::is_same<T, uint8_t>::value, "rectification reads 8-bit frames");
+    int acc = 0;
+    remap_taps(src, x, y, [&](int sx, int sy, int w) {
+        acc += w * *reinterpret_cast<const uint8_t*>(src.frame.ch[c] + (size_t)sy * src.frame.row_step +
+                                                     (size_t)sx * src.frame.col_step);
+    });
     return to_f32((uint8_t)((acc + 16384) >> 15));
+}
+
+// B, G, R of pixel (x, y) of a YUV frame: OpenCV's BT.601 limited-range fixed-point conversion (cvtColor
+// COLOR_YUV2BGR_NV12 / NV21 / I420 / YV12 / YUYV / UYVY / YVYU), each value clamped to 0..255.  The sums stay below 2^31.
+__device__ __forceinline__ void read_bgr(const YuvSrc& src, int x, int y, int bgr[3])
+{
+    const size_t co = (size_t)(y >> src.vs) * src.c_row_step + (size_t)(x >> 1) * src.c_col_step;
+    const int Y = *reinterpret_cast<const uint8_t*>(src.p[0] + (size_t)y * src.y_row_step + (size_t)x * src.y_col_step);
+    const int u = *reinterpret_cast<const uint8_t*>(src.p[1] + co) - 128;
+    const int v = *reinterpret_cast<const uint8_t*>(src.p[2] + co) - 128;
+    const int yy = max(0, Y - 16) * 1220542 + (1 << 19);
+    bgr[0] = min(max((yy + 2116026 * u) >> 20, 0), 255);
+    bgr[1] = min(max((yy - 852492 * v - 409993 * u) >> 20, 0), 255);
+    bgr[2] = min(max((yy + 1673527 * v) >> 20, 0), 255);
+}
+
+// B, G, R of rectified pixel (x, y) of a YUV frame: each tap's BGR once, then remap's rounding per channel
+__device__ __forceinline__ void read_bgr(const RectifySrc<YuvSrc>& src, int x, int y, int bgr[3])
+{
+    int acc[3] = {0, 0, 0};
+    remap_taps(src, x, y, [&](int sx, int sy, int w) {
+        int t[3];
+        read_bgr(src.frame, sx, sy, t);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[c] += w * t[c];
+    });
+#pragma unroll
+    for (int c = 0; c < 3; ++c) bgr[c] = (acc[c] + 16384) >> 15;
+}
+
+template <class Src> constexpr bool kYuvSrc = std::is_same<Src, YuvSrc>::value || std::is_same<Src, RectifySrc<YuvSrc>>::value;
+
+// the three channels of pixel (x, y) of a YUV source, as to_f32 sees them
+template <class Src>
+__device__ __forceinline__ void read_pixel(const Src& src, int x, int y, float v[3])
+{
+    int bgr[3];
+    read_bgr(src, x, y, bgr);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = to_f32((uint8_t)bgr[c]);
 }
 
 template <typename T, class Src = PlanesSrc>
@@ -133,6 +192,7 @@ __global__ void ingest_kernel(Src src, int W, int H, int Wp,
                               float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
                               float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
 {
+    static_assert(!kYuvSrc<Src> || std::is_same<T, uint8_t>::value, "YUV frames are 8-bit");
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= ((W + 3) & ~3) || y >= H) return;
@@ -140,8 +200,25 @@ __global__ void ingest_kernel(Src src, int W, int H, int Wp,
     if (x >= W) { I0[o] = 0.f; I1[o] = 0.f; I2[o] = 0.f; grd[o] = 0.f; return; }
     size_t row = 0;
     if constexpr (std::is_same<Src, PlanesSrc>::value) row = (size_t)y * src.row_step;
-    auto sample = [&](int c, int xx) { return read_sample<T>(src, row, c, xx, y); };
-    const float v0 = sample(0, x), v1 = sample(1, x), v2 = sample(2, x);
+    // A BGR source reads the channels one by one (sample(c, xx): channel c of pixel (xx, y)); a YUV source converts each
+    // pixel it reads once (read_pixel).  gray_at(xx): the gray value of pixel (xx, y).
+    auto sample = [&](int c, int xx) {
+        if constexpr (kYuvSrc<Src>) return 0.f;
+        else return read_sample<T>(src, row, c, xx, y);
+    };
+    auto gray_at = [&](int xx) {
+        if constexpr (kYuvSrc<Src>) {
+            float p[3];
+            read_pixel(src, xx, y, p);
+            return gray_of(p[0], p[1], p[2], gray_mode);
+        } else {
+            return gray_of(sample(0, xx), sample(1, xx), sample(2, xx), gray_mode);
+        }
+    };
+    float v[3];
+    if constexpr (kYuvSrc<Src>) read_pixel(src, x, y, v);
+    else v[0] = sample(0, x), v[1] = sample(1, x), v[2] = sample(2, x);
+    const float v0 = v[0], v1 = v[1], v2 = v[2];
     I0[o] = v0;
     I1[o] = v1;
     I2[o] = v2;
@@ -156,8 +233,8 @@ __global__ void ingest_kernel(Src src, int W, int H, int Wp,
     // recomputed in OpenCV's order (psm_cvf_ref.cuh).  u8 images (0 or 1/255 .. 1) never raise it.
     ingest_flags(v0, v1, v2, guide_flag);
     const int xr = reflect101(x + 1, W), xl = reflect101(x - 1, W);
-    const float gr = gray_of(sample(0, xr), sample(1, xr), sample(2, xr), gray_mode);
-    const float gl = gray_of(sample(0, xl), sample(1, xl), sample(2, xl), gray_mode);
+    const float gr = gray_at(xr);
+    const float gl = gray_at(xl);
     grd[o] = fsub(gr, gl);
 }
 

@@ -100,6 +100,24 @@ def rectify_args(left_maps, right_maps, src_size, width, height):
     return tuple(args), tuple(arrays)
 
 
+def yuv_format(format):
+    """PSM_YUV_* of a format name ("nv12", "nv21", "i420", "yv12", "yuyv", "uyvy" or "yvyu", cv2's COLOR_YUV2BGR_<NAME>)
+    -> (format code, True for 4:2:0); ValueError on any other value"""
+    name = format.lower() if isinstance(format, str) else format
+    if name not in capi.YUV_FORMATS:
+        raise ValueError(f"unknown YUV format {format!r}: one of {', '.join(capi.YUV_FORMATS)}")
+    return capi.YUV_FORMATS[name], name in capi.YUV_420
+
+
+def yuv_shape(format, width, height):
+    """the shape of a YUV frame of width x height in cv2's layout: (H * 3 / 2, W) for 4:2:0, (H, W, 2) for 4:2:2.
+    ValueError on an unknown format, an odd width or (4:2:0) an odd height."""
+    _, is420 = yuv_format(format)
+    if width % 2 or (is420 and height % 2):
+        raise ValueError(f"YUV frames of {width} x {height}: the width must be even, and the height too for 4:2:0")
+    return (height * 3 // 2, width) if is420 else (height, width, 2)
+
+
 class DispEst:
     """DispEst(l, r, d, t, ocl) -- reference src/DispEst.cpp:10-143.
 
@@ -152,6 +170,7 @@ class DispEst:
         self.min_disp = int(min_disp)
         self.src_size = None   # setRectify: (SW, SH) of the camera frames CostConst_GPU takes
         self._lImg, self._rImg = l, r
+        self._yuv = None   # setInputImagesYUV's format code while its frames are the input
         self._ctx = C.c_void_p()
         self._lib = None
         if self.useOCL:
@@ -188,6 +207,21 @@ class DispEst:
         leftImg, rightImg = np.asarray(leftImg), np.asarray(rightImg)
         assert leftImg.dtype == rightImg.dtype
         self._lImg, self._rImg = leftImg, rightImg
+        self._yuv = None
+        return 0
+
+    def setInputImagesYUV(self, left, right, format):
+        """YUV frames as input (psm_set_images_yuv): uint8 numpy arrays in cv2's shapes, (H * 3 / 2, W) for the 4:2:0
+        formats "nv12", "nv21", "i420", "yv12" and (H, W, 2) for the 4:2:2 formats "yuyv", "uyvy", "yvyu", of the
+        constructor's size or setRectify's source size.  CostConst_GPU converts them to BGR on the device as
+        cv2.cvtColor(frame, COLOR_YUV2BGR_<FORMAT>) does, bit for bit.  Raises ValueError on an unknown format and TypeError
+        on frames that are not uint8; CostConst_GPU checks the shape."""
+        code, _ = yuv_format(format)
+        left, right = np.asarray(left), np.asarray(right)
+        if left.dtype != np.uint8 or right.dtype != np.uint8:
+            raise TypeError(f"YUV frames must be uint8 (got {left.dtype}, {right.dtype})")
+        self._lImg, self._rImg = left, right
+        self._yuv = (code, format)
         return 0
 
     def setThreads(self, newThreads):
@@ -348,6 +382,16 @@ class DispEst:
         l = np.ascontiguousarray(self._lImg)
         r = np.ascontiguousarray(self._rImg)
         w, h = self.src_size or (self.wid, self.hei)
+        if self._yuv is not None:
+            code, name = self._yuv
+            shape = yuv_shape(name, w, h)
+            if l.shape != shape or r.shape != shape:
+                raise ValueError(f"{name} frames must be {shape}: the size DispEst was constructed with, or the source size "
+                                 f"of setRectify (got {l.shape}, {r.shape})")
+            capi.check(self._lib.psm_set_images_yuv(self._ctx, code, _ptr(l), l.strides[0], _ptr(r), r.strides[0]),
+                       self._ctx)
+            capi.check(self._lib.psm_cost_const(self._ctx), self._ctx)
+            return 0
         if l.shape != (h, w, 3) or r.shape != l.shape:
             raise ValueError(f"input images must be {h} x {w} x 3: the size DispEst was constructed with, or the source "
                              "size of setRectify")

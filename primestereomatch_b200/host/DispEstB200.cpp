@@ -53,6 +53,19 @@ int DispEst::setInputImages(cv::Mat leftImg, cv::Mat rightImg)
     assert(leftImg.type() == rightImg.type());
     lImg = leftImg;
     rImg = rightImg;
+    yuv_format = 0;
+    return 0;
+}
+
+int DispEst::setInputImagesYUV(cv::Mat leftImg, cv::Mat rightImg, int format)
+{
+    if (format < PSM_YUV_NV12 || format > PSM_YUV_YVYU) {
+        std::fprintf(stderr, "DispEst::setInputImagesYUV: unknown format %d\n", format);
+        return -1;
+    }
+    lImg = leftImg;
+    rImg = rightImg;
+    yuv_format = format;
     return 0;
 }
 
@@ -192,6 +205,19 @@ int DispEst::CostConst_GPU()
     // the 2-D copy (the reference re-creates DispEst on every dataset change, StereoMatch.cpp:601-602)
     // with setRectify on, the frames are the camera's (src_w x src_h, 8-bit)
     const int fw = src_w ? src_w : wid, fh = src_w ? src_h : hei;
+    if (yuv_format) {
+        const bool is420 = yuv_format <= PSM_YUV_YV12;
+        const int rows = is420 ? fh / 2 * 3 : fh, type = is420 ? CV_8UC1 : CV_8UC2;
+        for (const cv::Mat* m : {&lImg, &rImg})
+            if (m->rows != rows || m->cols != fw || m->type() != type) {
+                std::fprintf(stderr, "DispEst::CostConst_GPU: YUV frames must be %dx%d %s\n", fw, rows,
+                             is420 ? "CV_8UC1" : "CV_8UC2");
+                return -1;
+            }
+        if (int rc = psm_set_images_yuv(ctx, yuv_format, lImg.ptr<uint8_t>(), lImg.step, rImg.ptr<uint8_t>(), rImg.step))
+            return rc;
+        return psm_cost_const(ctx);
+    }
     if (lImg.rows != fh || lImg.cols != fw || rImg.rows != fh || rImg.cols != fw || lImg.type() != rImg.type() ||
         lImg.channels() != 3) {
         std::fprintf(stderr, "DispEst::CostConst_GPU: input images must be %dx%d, 3 channels, equal types\n", fw, fh);

@@ -33,6 +33,7 @@
 #define CV_MAT_DEPTH_MASK 7
 #define CV_MAKETYPE(depth, cn) ((depth) + (((cn)-1) << 3))
 #define CV_8UC1 CV_MAKETYPE(CV_8U, 1)
+#define CV_8UC2 CV_MAKETYPE(CV_8U, 2)
 #define CV_8UC3 CV_MAKETYPE(CV_8U, 3)
 #define CV_16UC1 CV_MAKETYPE(CV_16U, 1)
 #define CV_16SC2 CV_MAKETYPE(CV_16S, 2)
@@ -99,6 +100,10 @@ public:
     cv::Mat rRunnerUp[2];  // filtered cost (psm_read_runner_up); DispSelect_GPU fills them, rRunnerUp not when left-only
 
     int setInputImages(cv::Mat l, cv::Mat r);
+    // YUV frames as input (psm_set_images_yuv): format PSM_YUV_NV12 ... PSM_YUV_YVYU, frames in cv2's layouts -- CV_8UC1
+    // of (H * 3 / 2) x W for the 4:2:0 formats, CV_8UC2 of H x W for the 4:2:2 ones, of the context's size or setRectify's
+    // source size.  CostConst_GPU converts them to BGR on the device as cvtColor(COLOR_YUV2BGR_*) does.
+    int setInputImagesYUV(cv::Mat l, cv::Mat r, int format);
     int setThreads(unsigned int newThreads);
     void setSubsampleRate(unsigned int newRate) { subsample_rate = newRate; }
     // guided-filter window and eps (the reference's GIF_R_WIN / GIF_EPS) for the later CostFilter calls; see
@@ -181,6 +186,7 @@ private:
     int dcheck_mode = PSM_DCHECK_OFF;
     int views = PSM_VIEWS_BOTH;
     int src_w = 0, src_h = 0;   // setRectify: the size of the frames CostConst_GPU takes, 0 = the context's
+    int yuv_format = 0;         // setInputImagesYUV: the PSM_YUV_* format of lImg / rImg, 0 = BGR frames
     bool cost_output = false;
     bool runner_up_output = false;
     int set_output(int key, bool on, bool& flag);

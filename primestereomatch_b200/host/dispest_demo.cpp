@@ -19,7 +19,10 @@
 // `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.  A
 // leading `--rectify SW SH left.map right.map` rectifies raw camera frames on the device (setRectify): each .map file
 // holds W x H native-endian int16 pairs (map[0], CV_16SC2), then W x H uint16 (map[1], CV_16UC1), both cropped to W x H,
-// and left / right are then 8-bit BGR frames of SW x SH instead of float frames of W x H.
+// and left / right are then 8-bit BGR frames of SW x SH instead of float frames of W x H.  A leading `--yuv FORMAT`
+// (nv12, nv21, i420, yv12, yuyv, uyvy or yvyu) reads left / right as raw YUV frames in cv2's layout of W x H (or SW x SH
+// with --rectify): (H * 3 / 2) rows of W bytes for the 4:2:0 formats, H rows of 2 * W bytes for the 4:2:2 ones, converted
+// to BGR on the device (setInputImagesYUV).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -44,6 +47,7 @@ int main(int argc, char** argv)
     const char* points[2] = {nullptr, nullptr};   // Q file, output file
     int src_size[2] = {0, 0};                     // --rectify: SW, SH
     const char* map_files[2] = {nullptr, nullptr};
+    int yuv = 0;                                  // --yuv: PSM_YUV_* of the frames, 0 = BGR
     std::vector<int> devices;
     const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
     if (left_only) {
@@ -54,7 +58,18 @@ int main(int argc, char** argv)
     while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices") ||
                          !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle") ||
                          !std::strcmp(argv[1], "--disp-check") ||
-                         !std::strcmp(argv[1], "--points") || !std::strcmp(argv[1], "--rectify"))) {
+                         !std::strcmp(argv[1], "--points") || !std::strcmp(argv[1], "--rectify") ||
+                         !std::strcmp(argv[1], "--yuv"))) {
+        if (!std::strcmp(argv[1], "--yuv")) {
+            static const char* const names[] = {"nv12", "nv21", "i420", "yv12", "yuyv", "uyvy", "yvyu"};
+            for (int k = 0; k < 7; ++k)
+                if (!std::strcmp(argv[2], names[k])) yuv = PSM_YUV_NV12 + k;
+            if (!yuv) { std::fprintf(stderr, "unknown --yuv format %s\n", argv[2]); return 2; }
+            argv[2] = argv[0];
+            argv += 2;
+            argc -= 2;
+            continue;
+        }
         if (!std::strcmp(argv[1], "--rectify")) {
             if (argc < 6) break;
             src_size[0] = std::atoi(argv[2]);
@@ -109,7 +124,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--disp-check MODE MAXDIFF] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--disp-check MODE MAXDIFF] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] [--yuv FORMAT] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -119,12 +134,19 @@ int main(int argc, char** argv)
     const bool rectify = map_files[0] != nullptr;
     const int fw = rectify ? src_size[0] : W, fh = rectify ? src_size[1] : H;
     if (fw < 1 || fh < 1) { std::fprintf(stderr, "bad --rectify source size\n"); return 2; }
-    cv::Mat l(fh, fw, rectify ? CV_8UC3 : CV_32FC3), r(fh, fw, rectify ? CV_8UC3 : CV_32FC3);
-    if (!read_all(argv[4], l.data, l.step * fh) || !read_all(argv[5], r.data, r.step * fh)) { std::fprintf(stderr, "bad input\n"); return 2; }
-    cv::Mat sized(H, W, l.type());   // the facade takes the context's size from its first frames
-    DispEst* SMDE = new DispEst(rectify ? sized : l, rectify ? sized : r, D, MAX_CPU_THREADS, true, block_slices, devices,
+    // with --yuv: CV_8UC1 of (fh * 3 / 2) x fw (4:2:0) or CV_8UC2 of fh x fw (4:2:2)
+    const int type = yuv ? (yuv <= PSM_YUV_YV12 ? CV_8UC1 : CV_8UC2) : rectify ? CV_8UC3 : CV_32FC3;
+    const int rows = yuv && yuv <= PSM_YUV_YV12 ? fh / 2 * 3 : fh;
+    cv::Mat l(rows, fw, type), r(rows, fw, type);
+    if (!read_all(argv[4], l.data, l.step * rows) || !read_all(argv[5], r.data, r.step * rows)) { std::fprintf(stderr, "bad input\n"); return 2; }
+    const bool framed = rectify || yuv;   // the frames do not give the context's size
+    cv::Mat sized(H, W, framed ? CV_8UC3 : l.type());   // the facade takes the context's size from its first frames
+    DispEst* SMDE = new DispEst(framed ? sized : l, framed ? sized : r, D, MAX_CPU_THREADS, true, block_slices, devices,
                                 min_disp);
-    SMDE->setInputImages(l, r);
+    if (yuv)
+        SMDE->setInputImagesYUV(l, r, yuv);
+    else
+        SMDE->setInputImages(l, r);
     SMDE->setThreads(MAX_CPU_THREADS);
     SMDE->setSubsampleRate(4);
     int rc = left_only ? SMDE->setViews(PSM_VIEWS_LEFT) : 0;

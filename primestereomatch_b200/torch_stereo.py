@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import capi
-from .dispest import DispEst, create_context, rectify_args, resolve_map_bits
+from .dispest import DispEst, create_context, rectify_args, resolve_map_bits, yuv_format, yuv_shape
 
 _PIX = {torch.uint8: capi.PSM_PIX_U8, torch.float32: capi.PSM_PIX_F32}
 _ORDER = {"bgr": (0, 1, 2), "rgb": (2, 1, 0)}   # the tensor channel that holds B, G and R
@@ -60,6 +60,56 @@ def frame_layout(t, height, width, channels="bgr"):
     order = _ORDER[channels]
     frames = [tuple(base + b * bstride + order[c] * sch * elem for c in range(3)) for b in range(n)]
     return _PIX[t.dtype], frames, row_step, col_step, batched
+
+
+def yuv_layout(t, height, width, format):
+    """The psm_set_images_device_yuv arguments of a YUV frame tensor, or of each frame of a batch.
+
+    t: uint8, in cv2's shape for the format -- (H * 3 / 2, W) for "nv12", "nv21", "i420", "yv12", (H, W, 2) for "yuyv",
+    "uyvy", "yvyu" -- optionally with a leading batch dimension, any strides (the halves of one side-by-side frame
+    included), except that I420 / YV12 frames, whose chroma planes are packed rows of W / 2 samples, must be contiguous.
+    -> (sampling, [(Y, U, V) byte addresses] per frame, y_row_step, y_col_step, c_row_step, c_col_step, batched).  Raises
+    TypeError or ValueError on anything the layout cannot express; the tensor's device is not looked at."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"expected a torch.Tensor (got {type(t).__name__})")
+    if t.dtype != torch.uint8:
+        raise TypeError(f"YUV frames must be uint8 tensors (got {t.dtype})")
+    code, is420 = yuv_format(format)
+    shape = yuv_shape(format, width, height)
+    if t.dim() not in (len(shape), len(shape) + 1) or tuple(t.shape[-len(shape):]) != shape:
+        raise ValueError(f"{format} frames must be {shape}, optionally with a leading batch dimension "
+                         f"(got shape {tuple(t.shape)})")
+    s = t.stride()[-len(shape):]
+    sr, sc = s[0], s[1]
+    if sc < 1:
+        raise ValueError(f"the column stride is {sc} elements: pixels of a row must not share samples")
+    if sr < (width - 1) * sc + 1:
+        raise ValueError(f"the row stride ({sr} elements) is shorter than a row ({width} pixels {sc} elements apart)")
+    name = format.lower()
+    if is420:
+        uv = height * sr   # the chroma rows follow the luma rows
+        if name in ("i420", "yv12"):
+            if (sr, sc) != (width, 1):
+                raise ValueError(f"{name} frames must be contiguous: their chroma planes are packed rows of {width // 2} "
+                                 f"samples (got strides {tuple(s)})")
+            q = (width // 2) * (height // 2)
+            u, v = (uv, uv + q) if name == "i420" else (uv + q, uv)
+            offsets, steps = (0, u, v), (sr, 1, width // 2, 1)
+        else:
+            u, v = (uv, uv + sc) if name == "nv12" else (uv + sc, uv)
+            offsets, steps = (0, u, v), (sr, sc, sr, 2 * sc)
+    else:
+        sch = s[2]   # (H, W, 2): sample k of pixel x; the chroma pair (U, V or V, U) spans pixels 2i and 2i + 1
+        offsets = {"yuyv": (0, sch, sc + sch), "uyvy": (sch, 0, sc), "yvyu": (0, sc + sch, sch)}[name]
+        steps = (sr, sc, sr, 2 * sc)
+    sampling = capi.PSM_YUV_420 if is420 else capi.PSM_YUV_422
+    batched = t.dim() == len(shape) + 1
+    n, bstride = (t.shape[0], t.stride(0)) if batched else (1, 0)
+    if n < 1:
+        raise ValueError("empty batch")
+    base = t.data_ptr()
+    frames = [tuple(base + b * bstride + o for o in offsets) for b in range(n)]
+    return (sampling, frames) + steps + (batched,)
 
 
 class TorchStereo:
@@ -159,25 +209,40 @@ class TorchStereo:
         self.subsample_rate = int(rate)
 
     # -- frames -------------------------------------------------------------------------------
-    def _layout(self, left, right, channels):
+    def _layout(self, left, right, channels, yuv=None):
         """Both frames' layout, checked in full before any device work: (H, W) frames, or uint8 frames of the source
-        size while setRectify is on."""
+        size while setRectify is on -> (the C-ABI call that takes them, its argument before the pointers, left frames,
+        right frames, its steps, batched)"""
         w, h = self.src_size or (self.width, self.height)
+        if yuv is not None:
+            sampling, lf, *steps, batched = yuv_layout(left, h, w, yuv)
+            other = yuv_layout(right, h, w, yuv)
+            if left.shape != right.shape or tuple(steps) != tuple(other[2:6]):
+                raise ValueError("left and right must have the same shape and strides")
+            self._check_devices(left, right)
+            return "psm_set_images_device_yuv", sampling, lf, other[1], tuple(steps), batched
         pix, lf, row_step, col_step, batched = frame_layout(left, h, w, channels)
         other = frame_layout(right, h, w, channels)
         if self.src_size is not None and pix != capi.PSM_PIX_U8:
             raise ValueError("setRectify is on: rectification reads uint8 camera frames only (got float32)")
         if left.shape != right.shape or left.dtype != right.dtype or (pix, row_step, col_step) != (other[0], other[2], other[3]):
             raise ValueError("left and right must have the same shape, dtype and strides")
+        self._check_devices(left, right)
+        return "psm_set_images_device_planes", pix, lf, other[1], (row_step, col_step), batched
+
+    def _check_devices(self, left, right):
         for name, t in (("left", left), ("right", right)):
             if t.device != self.device:
                 raise ValueError(f"{name} is on {t.device}: frames must be CUDA tensors on the context's device {self.device}")
-        return pix, lf, other[1], row_step, col_step, batched
 
-    def match(self, left, right, *, channels="bgr", fgf=False, post_process=False, costs=False, runner_up=False,
-              points=None, handle_missing=False):
+    def match(self, left, right, *, channels="bgr", yuv=None, fgf=False, post_process=False, costs=False,
+              runner_up=False, points=None, handle_missing=False):
         """Disparity maps of one frame pair or a batch -> (lmap, rmap): new uint8 / uint16 tensors of shape (H, W) or
         (B, H, W) on the context's device; rmap is None on a left-only context.
+
+        yuv="nv12" (or "nv21", "i420", "yv12", "yuyv", "uyvy", "yvyu"): the frames are uint8 YUV tensors in cv2's shapes
+        (yuv_layout; the halves of one side-by-side frame included), converted to BGR on the device as
+        cv2.cvtColor(frame, COLOR_YUV2BGR_<FORMAT>) does (psm_set_images_device_yuv); channels is not read.
 
         costs=True -> (lmap, rmap, lcosts, rcosts): also the filtered costs beside each winner of the selection maps
         (PSM_OPT_COSTS, psm_copy_costs_device), new float32 tensors (3, H, W) or (B, 3, H, W) whose plane k holds the cost
@@ -195,7 +260,7 @@ class TorchStereo:
         float32 tensors (H, W, 3) or (B, H, W, 3) of X, Y, Z; either Q may be None, and its tensor is then None.
         handle_missing=True sets Z = 10000 wherever a map holds its minimum.
 
-        After psm_wait_stream on torch's current stream: psm_set_images_device_planes, psm_cost_const, the guided filter
+        After psm_wait_stream on torch's current stream: psm_set_images_device_planes (or _device_yuv), psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
         with post_process=True (the chain setDisparityCheck, setSpeckleFilter, setLRCheck and setPostFilter configure),
         psm_copy_maps_device and, with points, psm_reproject_device of each frame of a batch in turn; then
@@ -216,7 +281,7 @@ class TorchStereo:
                 raise ValueError("points: a right Q on a left-only context (setViews('left'))")
             if qs[0] is None and qs[1] is None:
                 raise ValueError("points: give a Q for at least one view")
-        pix, lf, rf, row_step, col_step, batched = self._layout(left, right, channels)
+        set_images, kind, lf, rf, steps, batched = self._layout(left, right, channels, yuv)
         L, ctx = self._lib, self._ctx
         H, W = self.height, self.width
         mdt = torch.uint16 if self.map_bits == 16 else torch.uint8
@@ -243,7 +308,7 @@ class TorchStereo:
         self._check(L.psm_wait_stream(ctx, stream))
         for b in range(len(lf)):
             lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
-            self._check(L.psm_set_images_device_planes(ctx, pix, lp, rp, row_step, col_step))
+            self._check(getattr(L, set_images)(ctx, kind, lp, rp, *steps))
             self._check(L.psm_cost_const(ctx))
             self._check(L.psm_cost_filter_fgf(ctx, self.subsample_rate) if fgf else L.psm_cost_filter(ctx))
             self._check(L.psm_disp_select_device(ctx))
