@@ -523,6 +523,45 @@ int psm_set_images_yuv(psm_ctx* ctx, int format, const uint8_t* left, size_t lef
 int psm_set_images_yuv_async(psm_ctx* ctx, int format, const uint8_t* left, size_t left_step, const uint8_t* right,
                              size_t right_step);
 
+/* Bayer raw frames (machine-vision and CSI cameras), demosaiced to BGR in ingest.  A frame of Wf x Hf (the context's
+ * W x H, or the source size while psm_set_rectify is on) has one u8 sample raw(x, y) per pixel; the pattern names the
+ * colours of the 2 x 2 cell at (0, 0) in reading order (PSM_BAYER_RGGB is cv2's COLOR_BayerRGGB2BGR = COLOR_BayerBG2BGR,
+ * BGGR = BayerRG, GRBG = BayerGB, GBRG = BayerGR: cv2's two-letter names are shifted by one cell).  Its BGR pixel is
+ * OpenCV's cvtColor(COLOR_Bayer<PATTERN>2BGR) (PSM_DEMOSAIC_BILINEAR) or _EA (PSM_DEMOSAIC_EA), cv2 4.13.0:
+ *   - interior pixel (1 <= x <= Wf - 2, 1 <= y <= Hf - 2) of colour c: channel c is raw(x, y).  At an R or B site
+ *     G = (n4 + 2) >> 2 and the opposite colour = (d4 + 2) >> 2, n4 / d4 the sums of the four edge / diagonal neighbours.
+ *     At a G site the colour of the horizontal neighbours is (raw(x - 1, y) + raw(x + 1, y) + 1) >> 1, the other colour
+ *     (raw(x, y - 1) + raw(x, y + 1) + 1) >> 1.
+ *   - edge-aware: G at an R or B site is the horizontal pair's (a + b + 1) >> 1 when |raw(x - 1, y) - raw(x + 1, y)| <=
+ *     |raw(x, y - 1) - raw(x, y + 1)| (ties go horizontal), the vertical pair's otherwise; R and B as bilinear.
+ *   - border: BGR(x, y) = interior(clamp(x, 1, Wf - 2), clamp(y, 1, Hf - 2)); every pixel is 0 when Wf < 3 or Hf < 3.
+ * That u8 frame is ingested exactly as psm_set_images_u8 ingests it; with psm_set_rectify on, the frame is
+ * remap(cvtColor(bayer), xy, a, INTER_LINEAR), each tap the demosaiced pixel at its source position.  One ingest_kernel
+ * launch and one halo pass per view, as for u8 frames.
+ *
+ * Side-by-side frames: each view is demosaiced as a frame of its own, equal to cvtColor on the half as a separate array,
+ * with borders at the half's own edges (demosaicing the whole side-by-side frame first differs at the two seam columns).
+ * `pattern` names each view's own pixel (0, 0): a half that starts at an odd column has the horizontally shifted pattern.
+ *
+ * psm_set_images_device_bayer: device frames read in place, raw(x, y) at p + y * row_step + x * col_step (bytes), ordered
+ * like psm_set_images_device_planes (psm_wait_stream / psm_signal_stream).
+ * psm_set_images_bayer / _bayer_async (finished by psm_set_images_commit): HOST frames of Hf rows of Wf bytes, `step`
+ * bytes apart, copied into the u8 staging sets (1 byte per pixel), so no frame allocates; buffers reusable as for
+ * psm_set_images_u8 / _u8_async.
+ *   - PSM_EINVAL before any CUDA work, context unchanged: an unknown pattern or method, a null pointer, a zero column
+ *     step, row_step < (Wf - 1) * col_step + 1, a host step below Wf.  psm_set_images_bayer_async returns PSM_ESTATE while
+ *     another asynchronous upload is pending, and PSM_EINVAL on a multi-device context, as psm_set_images_u8_async does.
+ *   - Multi-device contexts read the frame on the first device; the other shards receive its ingested planes.
+ * See DESIGN.md section 28. */
+enum { PSM_BAYER_RGGB = 1, PSM_BAYER_BGGR = 2, PSM_BAYER_GRBG = 3, PSM_BAYER_GBRG = 4 };
+enum { PSM_DEMOSAIC_BILINEAR = 1, PSM_DEMOSAIC_EA = 2 };
+int psm_set_images_device_bayer(psm_ctx* ctx, int pattern, int method, const void* left, const void* right,
+                                size_t row_step, size_t col_step);
+int psm_set_images_bayer(psm_ctx* ctx, int pattern, int method, const uint8_t* left, size_t left_step,
+                         const uint8_t* right, size_t right_step);
+int psm_set_images_bayer_async(psm_ctx* ctx, int pattern, int method, const uint8_t* left, size_t left_step,
+                               const uint8_t* right, size_t right_step);
+
 /* Pipelined upload (extension; the reference's DispEst is synchronous per frame): start the H2D copy
  * of the NEXT frame on the context's copy stream into a second staging set while the current frame
  * is still being computed, then make it the current frame.  Host buffers must be page-locked for the

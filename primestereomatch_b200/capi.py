@@ -26,6 +26,7 @@ SYMBOLS = [
     "psm_copy_maps_device", "psm_copy_costs_device", "psm_read_costs", "psm_copy_runner_up_device", "psm_read_runner_up",
     "psm_create_range", "psm_set_speckle_filter", "psm_set_disparity_check", "psm_reproject_device", "psm_read_points", "psm_set_rectify",
     "psm_set_images_device_yuv", "psm_set_images_yuv", "psm_set_images_yuv_async",
+    "psm_set_images_device_bayer", "psm_set_images_bayer", "psm_set_images_bayer_async",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -47,6 +48,11 @@ PSM_YUV_NV12, PSM_YUV_NV21, PSM_YUV_I420, PSM_YUV_YV12, PSM_YUV_YUYV, PSM_YUV_UY
 YUV_FORMATS = {"nv12": PSM_YUV_NV12, "nv21": PSM_YUV_NV21, "i420": PSM_YUV_I420, "yv12": PSM_YUV_YV12,
                "yuyv": PSM_YUV_YUYV, "uyvy": PSM_YUV_UYVY, "yvyu": PSM_YUV_YVYU}
 YUV_420 = ("nv12", "nv21", "i420", "yv12")
+PSM_BAYER_RGGB, PSM_BAYER_BGGR, PSM_BAYER_GRBG, PSM_BAYER_GBRG = 1, 2, 3, 4
+PSM_DEMOSAIC_BILINEAR, PSM_DEMOSAIC_EA = 1, 2
+# the Bayer patterns by the colours of the 2 x 2 cell at (0, 0) in reading order, and the demosaicing methods
+BAYER_PATTERNS = {"rggb": PSM_BAYER_RGGB, "bggr": PSM_BAYER_BGGR, "grbg": PSM_BAYER_GRBG, "gbrg": PSM_BAYER_GBRG}
+DEMOSAIC_METHODS = {"bilinear": PSM_DEMOSAIC_BILINEAR, "ea": PSM_DEMOSAIC_EA}
 
 _lib = None
 
@@ -99,6 +105,9 @@ def lib():
     L.psm_set_images_device_yuv.argtypes = [vp, i, C.POINTER(vp), C.POINTER(vp), sz, sz, sz, sz]
     L.psm_set_images_yuv.argtypes = [vp, i, u8p, sz, u8p, sz]
     L.psm_set_images_yuv_async.argtypes = [vp, i, u8p, sz, u8p, sz]
+    L.psm_set_images_device_bayer.argtypes = [vp, i, i, vp, vp, sz, sz]
+    L.psm_set_images_bayer.argtypes = [vp, i, i, u8p, sz, u8p, sz]
+    L.psm_set_images_bayer_async.argtypes = [vp, i, i, u8p, sz, u8p, sz]
     L.psm_wait_stream.argtypes = [vp, vp]
     L.psm_signal_stream.argtypes = [vp, vp]
     L.psm_copy_maps_device.argtypes = [vp, i, vp, sz, vp, sz]

@@ -81,7 +81,7 @@ struct psm_ctx {
     cudaEvent_t ingest_done[2] = {nullptr, nullptr};  // ingest kernels consumed staging set k (recorded on the compute stream)
     bool ingest_done_valid[2] = {false, false};
     int stage_cur = 0;                      // staging set holding the current frame: 0 = stage_in, 1 = stage_alt
-    int up_pending = 0;                     // frame format (PSM_PIX_* or kFmtYuv + PSM_YUV_*) of the pending asynchronous upload, 0 none
+    int up_pending = 0;                     // frame format (PSM_PIX_*, kFmtYuv + PSM_YUV_* or bayer_fmt) of the pending asynchronous upload, 0 none
     uint8_t* dis[2] = {nullptr, nullptr};    // disparity maps: u8, or u16 (map_bytes = 2, psm_create_u16) behind the same pointer
     int map_bytes = 1;                       // bytes per disparity-map element
     // Fast Guided Filter branch (lazy): low-res guide planes per view, low-res coefficient scratch, up-sampling plan
@@ -301,15 +301,19 @@ void images_ingested(psm_ctx* c, bool float_images)
 size_t pix_bytes(int pix) { return pix == PSM_PIX_U8 ? 1 : sizeof(float); }
 
 // A host frame's format: PSM_PIX_U8 or PSM_PIX_F32 for interleaved BGR, kFmtYuv + PSM_YUV_* for a YUV frame in cv2's
-// contiguous layout (psm_set_images_yuv).  Uploads, staging sets and the asynchronous commit go by it.
-constexpr int kFmtYuv = 16;
-bool is_yuv(int fmt) { return fmt > kFmtYuv; }
+// contiguous layout (psm_set_images_yuv), bayer_fmt(PSM_BAYER_*, PSM_DEMOSAIC_*) for a Bayer frame
+// (psm_set_images_bayer).  Uploads, staging sets and the asynchronous commit go by it.
+constexpr int kFmtYuv = 16, kFmtBayer = 32;
+bool is_yuv(int fmt) { return fmt > kFmtYuv && fmt < kFmtBayer; }
 int yuv_vs(int format) { return format <= PSM_YUV_YV12 ? 1 : 0; }   // the chroma row shift: 1 for 4:2:0, 0 for 4:2:2
+int bayer_fmt(int pattern, int method) { return kFmtBayer | (method & 3) << 3 | (pattern & 7); }
+bool is_bayer(int fmt) { return fmt > kFmtBayer; }
 
 // bytes of one row, and rows, of a host frame of format fmt as the staging sets hold it
 size_t host_row_bytes(psm_ctx* c, int fmt)
 {
     if (is_yuv(fmt)) return (size_t)c->frame_w() * (yuv_vs(fmt - kFmtYuv) ? 1 : 2);
+    if (is_bayer(fmt)) return (size_t)c->frame_w();
     return (size_t)c->frame_w() * 3 * pix_bytes(fmt);
 }
 int host_rows(psm_ctx* c, int fmt) { return is_yuv(fmt) && yuv_vs(fmt - kFmtYuv) ? c->frame_h() / 2 * 3 : c->frame_h(); }
@@ -333,8 +337,18 @@ YuvSrc yuv_host_src(psm_ctx* c, int format, const void* p, size_t step)
     }
 }
 
+// the BayerSrc of a checked Bayer frame of the context's frame size at p, samples col_step and rows row_step bytes apart,
+// whose pixel (0, 0) has pattern PSM_BAYER_*'s first colour
+BayerSrc bayer_src(psm_ctx* c, int pattern, int method, const void* p, size_t row_step, size_t col_step)
+{
+    const int rx = pattern == PSM_BAYER_BGGR || pattern == PSM_BAYER_GRBG;
+    const int ry = pattern == PSM_BAYER_BGGR || pattern == PSM_BAYER_GBRG;
+    return BayerSrc{static_cast<const char*>(p), row_step, col_step, c->frame_w(), c->frame_h(), rx, ry,
+                    method == PSM_DEMOSAIC_EA};
+}
+
 // the frame's planes, gradients and ingest flags: one ingest_kernel launch and one pad_rows per view on the context's
-// stream.  With psm_set_rectify on, the frame (u8 or YUV, checked by the caller) is read through each view's maps.
+// stream.  With psm_set_rectify on, the frame (u8, YUV or Bayer, checked by the caller) is read through each view's maps.
 template <typename T, class Src>
 int ingest(psm_ctx* c, const Src src[2])
 {
@@ -386,6 +400,11 @@ int ingest_staged(psm_ctx* c, int set, int fmt, cudaEvent_t copied)
     if (is_yuv(fmt)) {
         const YuvSrc src[2] = {yuv_host_src(c, fmt - kFmtYuv, stage_buf(c, set, 0), row_bytes),
                                yuv_host_src(c, fmt - kFmtYuv, stage_buf(c, set, 1), row_bytes)};
+        if (int rc = ingest<uint8_t>(c, src)) return rc;
+    } else if (is_bayer(fmt)) {
+        const int pattern = fmt & 7, method = fmt >> 3 & 3;
+        const BayerSrc src[2] = {bayer_src(c, pattern, method, stage_buf(c, set, 0), row_bytes, 1),
+                                 bayer_src(c, pattern, method, stage_buf(c, set, 1), row_bytes, 1)};
         if (int rc = ingest<uint8_t>(c, src)) return rc;
     } else {
         const size_t elem = pix_bytes(fmt);
@@ -519,6 +538,51 @@ int check_yuv_device(psm_ctx* c, int sampling, const void* const left[3], const 
     if (short_row(c_row_step, c_col_step, c->frame_w() / 2))
         return fail(c, PSM_EINVAL, "c_row_step %zu / c_col_step %zu: the column step must be nonzero and a row of %d chroma "
                     "samples fit in the row step", c_row_step, c_col_step, c->frame_w() / 2);
+    return PSM_OK;
+}
+
+// a Bayer pattern and demosaicing method, or PSM_EINVAL
+int check_bayer_kind(psm_ctx* c, int pattern, int method)
+{
+    if (pattern < PSM_BAYER_RGGB || pattern > PSM_BAYER_GBRG)
+        return fail(c, PSM_EINVAL, "unknown Bayer pattern %d (PSM_BAYER_RGGB = 1 .. PSM_BAYER_GBRG = 4)", pattern);
+    if (method != PSM_DEMOSAIC_BILINEAR && method != PSM_DEMOSAIC_EA)
+        return fail(c, PSM_EINVAL, "unknown demosaicing method %d (PSM_DEMOSAIC_BILINEAR = 1, PSM_DEMOSAIC_EA = 2)", method);
+    return PSM_OK;
+}
+
+// psm_set_images_bayer[_async]: two host frames -> src (ch[0] and row_step, as upload reads them), or PSM_EINVAL before
+// any CUDA call
+int check_bayer_host(psm_ctx* c, int pattern, int method, const void* l, size_t lstep, const void* r, size_t rstep,
+                     PlanesSrc src[2])
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (int rc = check_bayer_kind(c, pattern, method)) return rc;
+    const void* p[2] = {l, r};
+    const size_t step[2] = {lstep, rstep};
+    for (int v = 0; v < 2; ++v) {
+        if (!p[v]) return fail(c, PSM_EINVAL, "null frame pointer for view %d", v);
+        if (step[v] < (size_t)c->frame_w())
+            return fail(c, PSM_EINVAL, "step %zu of view %d is below the %d bytes of a row", step[v], v, c->frame_w());
+        src[v] = PlanesSrc{{static_cast<const char*>(p[v]), nullptr, nullptr}, step[v], 0};
+    }
+    return PSM_OK;
+}
+
+// psm_set_images_device_bayer: the caller's two frames and their layout -> src, or PSM_EINVAL before any CUDA call
+int check_bayer_device(psm_ctx* c, int pattern, int method, const void* left, const void* right, size_t row_step,
+                       size_t col_step, BayerSrc src[2])
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (int rc = check_bayer_kind(c, pattern, method)) return rc;
+    if (!left || !right) return fail(c, PSM_EINVAL, "null frame pointer for view %d", left ? 1 : 0);
+    // a row of Wf samples col_step apart spans (Wf - 1) * col_step + 1 bytes
+    const size_t span = (size_t)(c->frame_w() - 1);
+    if (!col_step || (span && col_step > (SIZE_MAX - 1) / span) || row_step < span * col_step + 1)
+        return fail(c, PSM_EINVAL, "row_step %zu / col_step %zu: the column step must be nonzero and a row of %d samples "
+                    "fit in the row step", row_step, col_step, c->frame_w());
+    src[0] = bayer_src(c, pattern, method, left, row_step, col_step);
+    src[1] = bayer_src(c, pattern, method, right, row_step, col_step);
     return PSM_OK;
 }
 
@@ -1186,18 +1250,20 @@ int multi_send_planes(psm_ctx* c, int pix)
 
 // the body of every synchronous psm_set_images* call once its frame is checked.  A multi-device context runs stage 0 on
 // its first shard and sends the other shards the frame, or the planes the first shard ingested.  With psm_set_rectify on,
-// only the first shard holds the maps, so every kind of frame reaches the others as its planes; so does a YUV frame.
+// only the first shard holds the maps, so every kind of frame reaches the others as its planes; so does a YUV or Bayer
+// frame.
 int set_images(psm_ctx* c, Frame kind, int fmt, const PlanesSrc src[2])
 {
     if (!is_multi(c)) return set_images_one(c, kind, fmt, src);
     if (int rc = set_images_one(c->shard[0], kind, fmt, src)) return relay(c, 0, rc);
-    return kind == Frame::planes || c->rect_sw || is_yuv(fmt) ? multi_send_planes(c, fmt)
-                                                              : multi_send_frame(c, kind, fmt, src);
+    return kind == Frame::planes || c->rect_sw || is_yuv(fmt) || is_bayer(fmt) ? multi_send_planes(c, fmt)
+                                                                                : multi_send_frame(c, kind, fmt, src);
 }
 
-// psm_set_images_device_yuv once its frames are checked: stage 0 on the context (a multi-device context's first shard,
-// whose ingested planes the other shards receive)
-int set_images_device_yuv(psm_ctx* c, const YuvSrc src[2])
+// psm_set_images_device_yuv / _device_bayer once its frames are checked: stage 0 on the context (a multi-device context's
+// first shard, whose ingested planes the other shards receive)
+template <class Src>
+int set_images_device_converted(psm_ctx* c, const Src src[2])
 {
     psm_ctx* s = is_multi(c) ? c->shard[0] : c;
     int rc = bind(s);
@@ -1208,7 +1274,7 @@ int set_images_device_yuv(psm_ctx* c, const YuvSrc src[2])
     return rc ? relay(c, 0, rc) : multi_send_planes(c, PSM_PIX_U8);
 }
 
-// psm_set_images[_u8|_yuv]_async: the frame of format fmt that check(src) checks is uploaded into the staging set that is
+// psm_set_images[_u8|_yuv|_bayer]_async: the frame of format fmt that check(src) checks is uploaded into the staging set that is
 // not in use, on the copy stream
 template <class Check>
 int set_images_async(psm_ctx* c, int fmt, const char* call, Check check)
@@ -2068,7 +2134,32 @@ int psm_set_images_device_yuv(psm_ctx* c, int sampling, const void* const left[3
 {
     YuvSrc src[2];
     if (int rc = check_yuv_device(c, sampling, left, right, y_row_step, y_col_step, c_row_step, c_col_step, src)) return rc;
-    return set_images_device_yuv(c, src);
+    return set_images_device_converted(c, src);
+}
+
+int psm_set_images_bayer(psm_ctx* c, int pattern, int method, const uint8_t* left, size_t left_step, const uint8_t* right,
+                         size_t right_step)
+{
+    PlanesSrc src[2];
+    if (int rc = check_bayer_host(c, pattern, method, left, left_step, right, right_step, src)) return rc;
+    return set_images(c, Frame::host, bayer_fmt(pattern, method), src);
+}
+
+int psm_set_images_bayer_async(psm_ctx* c, int pattern, int method, const uint8_t* left, size_t left_step,
+                               const uint8_t* right, size_t right_step)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    return set_images_async(c, bayer_fmt(pattern, method), "psm_set_images_bayer_async", [&](PlanesSrc* src) {
+        return check_bayer_host(c, pattern, method, left, left_step, right, right_step, src);
+    });
+}
+
+int psm_set_images_device_bayer(psm_ctx* c, int pattern, int method, const void* left, const void* right, size_t row_step,
+                                size_t col_step)
+{
+    BayerSrc src[2];
+    if (int rc = check_bayer_device(c, pattern, method, left, right, row_step, col_step, src)) return rc;
+    return set_images_device_converted(c, src);
 }
 
 int psm_set_images_commit(psm_ctx* c)

@@ -44,8 +44,8 @@ __global__ void pad_cols_kernel(float* __restrict__ base, size_t nrows, int W, i
 }
 
 // ------------------------------------------------------------------------------------------
-// Ingest: a BGR frame (float or u8) in any PlanesSrc layout or a YUV frame (YuvSrc); an 8-bit frame of either kind may be
-// read through rectification maps (RectifySrc) -> 3 planar channels + x-gradient of the gray image.
+// Ingest: a BGR frame (float or u8) in any PlanesSrc layout, a YUV frame (YuvSrc) or a Bayer frame (BayerSrc); an 8-bit
+// frame of any kind may be read through rectification maps (RectifySrc) -> 3 planar channels + x-gradient of the gray image.
 // Restates StereoMatch.cpp:193-197 (u8 * (1/255.0f)), CVF.cpp:47 (split) and CVC.cpp:41-46
 // (cvtColor RGB2GRAY on the BGR image, Sobel dx=1 ksize=1 with BORDER_REFLECT_101).
 // ------------------------------------------------------------------------------------------
@@ -96,10 +96,21 @@ struct YuvSrc {
     int vs;
 };
 
-// A u8 frame of SW x SH, BGR (PlanesSrc) or YUV (YuvSrc), read through the rectification maps of one view
-// (psm_set_rectify): output pixel (x, y) of the W x H crop is OpenCV's remap(frame, xy, a, INTER_LINEAR, BORDER_CONSTANT 0)
-// with the fixed-point maps of initUndistortRectifyMap(..., CV_16SC2), cropped (DESIGN.md section 25); a YUV frame is
-// remapped as the BGR frame cvtColor makes of it.  The maps are dense: entry (x, y) at y * W + x.
+// A Bayer frame of Wf x Hf (psm_set_images_bayer / psm_set_images_device_bayer): raw sample (x, y) at p + y * row_step +
+// x * col_step, one byte per pixel, the colour of each site given by the red site's column and row parity (DESIGN.md
+// section 28).  The four patterns differ only in (rx, ry).
+struct BayerSrc {
+    const char* p;
+    size_t row_step, col_step;
+    int Wf, Hf;
+    int rx, ry;   // the red site's column and row parity: RGGB (0, 0), BGGR (1, 1), GRBG (1, 0), GBRG (0, 1)
+    int ea;       // 1: the edge-aware method (COLOR_Bayer*2BGR_EA), 0: bilinear (COLOR_Bayer*2BGR)
+};
+
+// A u8 frame of SW x SH, BGR (PlanesSrc), YUV (YuvSrc) or Bayer (BayerSrc), read through the rectification maps of one
+// view (psm_set_rectify): output pixel (x, y) of the W x H crop is OpenCV's remap(frame, xy, a, INTER_LINEAR,
+// BORDER_CONSTANT 0) with the fixed-point maps of initUndistortRectifyMap(..., CV_16SC2), cropped (DESIGN.md section 25);
+// a YUV or Bayer frame is remapped as the BGR frame cvtColor makes of it.  The maps are dense: entry (x, y) at y * W + x.
 template <class F>
 struct RectifySrc {
     F frame;                   // the source frame, SW x SH
@@ -161,8 +172,53 @@ __device__ __forceinline__ void read_bgr(const YuvSrc& src, int x, int y, int bg
     bgr[2] = min(max((yy + 1673527 * v) >> 20, 0), 255);
 }
 
-// B, G, R of rectified pixel (x, y) of a YUV frame: each tap's BGR once, then remap's rounding per channel
-__device__ __forceinline__ void read_bgr(const RectifySrc<YuvSrc>& src, int x, int y, int bgr[3])
+// B, G, R of pixel (x, y) of a Bayer frame: OpenCV's demosaicing (cvtColor COLOR_Bayer<PATTERN>2BGR, or _EA), each pixel
+// the interior pixel at (clamp(x, 1, Wf - 2), clamp(y, 1, Hf - 2)) and every pixel 0 when Wf < 3 or Hf < 3, as cv2 does.
+// At the interior pixel, of colour c: c is its own sample; at an R or B site G is (n4 + 2) >> 2 over the four edge
+// neighbours (edge-aware: the horizontal pair's rounded mean when |left - right| <= |up - down|, else the vertical
+// pair's) and the opposite colour (d4 + 2) >> 2 over the four diagonal ones; at a G site the colour of its row's other
+// sites is the horizontal pair's (a + b + 1) >> 1, the third colour the vertical pair's.  Only samples of the 3 x 3
+// neighbourhood of the clamped pixel are read, all inside the frame.
+__device__ __forceinline__ void read_bgr(const BayerSrc& src, int x, int y, int bgr[3])
+{
+    if (src.Wf < 3 || src.Hf < 3) {
+        bgr[0] = bgr[1] = bgr[2] = 0;
+        return;
+    }
+    const int cx = min(max(x, 1), src.Wf - 2), cy = min(max(y, 1), src.Hf - 2);
+    const char* row[3];
+    row[1] = src.p + (size_t)cy * src.row_step + (size_t)cx * src.col_step;
+    row[0] = row[1] - src.row_step;
+    row[2] = row[1] + src.row_step;
+    int s[3][3];   // s[dy + 1][dx + 1] = raw(cx + dx, cy + dy)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        s[k][0] = *reinterpret_cast<const uint8_t*>(row[k] - src.col_step);
+        s[k][1] = *reinterpret_cast<const uint8_t*>(row[k]);
+        s[k][2] = *reinterpret_cast<const uint8_t*>(row[k] + src.col_step);
+    }
+    const int l = s[1][0], r = s[1][2], u = s[0][1], d = s[2][1];
+    const int hor = (l + r + 1) >> 1, ver = (u + d + 1) >> 1;
+    const bool red_row = ((cy ^ src.ry) & 1) == 0, red_col = ((cx ^ src.rx) & 1) == 0;
+    int R, G, B;
+    if (red_row == red_col) {   // an R (both) or B (neither) site
+        G = !src.ea ? (l + r + u + d + 2) >> 2 : abs(l - r) <= abs(u - d) ? hor : ver;
+        const int opp = (s[0][0] + s[0][2] + s[2][0] + s[2][2] + 2) >> 2;
+        R = red_row ? s[1][1] : opp;
+        B = red_row ? opp : s[1][1];
+    } else {   // a G site
+        G = s[1][1];
+        R = red_row ? hor : ver;
+        B = red_row ? ver : hor;
+    }
+    bgr[0] = B;
+    bgr[1] = G;
+    bgr[2] = R;
+}
+
+// B, G, R of rectified pixel (x, y) of a YUV or Bayer frame: each tap's BGR once, then remap's rounding per channel
+template <class F>
+__device__ __forceinline__ void read_bgr(const RectifySrc<F>& src, int x, int y, int bgr[3])
 {
     int acc[3] = {0, 0, 0};
     remap_taps(src, x, y, [&](int sx, int sy, int w) {
@@ -175,9 +231,13 @@ __device__ __forceinline__ void read_bgr(const RectifySrc<YuvSrc>& src, int x, i
     for (int c = 0; c < 3; ++c) bgr[c] = (acc[c] + 16384) >> 15;
 }
 
-template <class Src> constexpr bool kYuvSrc = std::is_same<Src, YuvSrc>::value || std::is_same<Src, RectifySrc<YuvSrc>>::value;
+// source kinds that convert whole pixels (read_bgr) instead of reading the channels one by one (read_sample)
+template <class Src> constexpr bool kPixelSrc = false;
+template <> constexpr bool kPixelSrc<YuvSrc> = true;
+template <> constexpr bool kPixelSrc<BayerSrc> = true;
+template <class F> constexpr bool kPixelSrc<RectifySrc<F>> = kPixelSrc<F>;
 
-// the three channels of pixel (x, y) of a YUV source, as to_f32 sees them
+// the three channels of pixel (x, y) of a YUV or Bayer source, as to_f32 sees them
 template <class Src>
 __device__ __forceinline__ void read_pixel(const Src& src, int x, int y, float v[3])
 {
@@ -192,7 +252,7 @@ __global__ void ingest_kernel(Src src, int W, int H, int Wp,
                               float* __restrict__ I0, float* __restrict__ I1, float* __restrict__ I2,
                               float* __restrict__ grd, int gray_mode, int* __restrict__ guide_flag)
 {
-    static_assert(!kYuvSrc<Src> || std::is_same<T, uint8_t>::value, "YUV frames are 8-bit");
+    static_assert(!kPixelSrc<Src> || std::is_same<T, uint8_t>::value, "YUV and Bayer frames are 8-bit");
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= ((W + 3) & ~3) || y >= H) return;
@@ -200,14 +260,14 @@ __global__ void ingest_kernel(Src src, int W, int H, int Wp,
     if (x >= W) { I0[o] = 0.f; I1[o] = 0.f; I2[o] = 0.f; grd[o] = 0.f; return; }
     size_t row = 0;
     if constexpr (std::is_same<Src, PlanesSrc>::value) row = (size_t)y * src.row_step;
-    // A BGR source reads the channels one by one (sample(c, xx): channel c of pixel (xx, y)); a YUV source converts each
-    // pixel it reads once (read_pixel).  gray_at(xx): the gray value of pixel (xx, y).
+    // A BGR source reads the channels one by one (sample(c, xx): channel c of pixel (xx, y)); a YUV or Bayer source
+    // converts each pixel it reads once (read_pixel).  gray_at(xx): the gray value of pixel (xx, y).
     auto sample = [&](int c, int xx) {
-        if constexpr (kYuvSrc<Src>) return 0.f;
+        if constexpr (kPixelSrc<Src>) return 0.f;
         else return read_sample<T>(src, row, c, xx, y);
     };
     auto gray_at = [&](int xx) {
-        if constexpr (kYuvSrc<Src>) {
+        if constexpr (kPixelSrc<Src>) {
             float p[3];
             read_pixel(src, xx, y, p);
             return gray_of(p[0], p[1], p[2], gray_mode);
@@ -216,7 +276,7 @@ __global__ void ingest_kernel(Src src, int W, int H, int Wp,
         }
     };
     float v[3];
-    if constexpr (kYuvSrc<Src>) read_pixel(src, x, y, v);
+    if constexpr (kPixelSrc<Src>) read_pixel(src, x, y, v);
     else v[0] = sample(0, x), v[1] = sample(1, x), v[2] = sample(2, x);
     const float v0 = v[0], v1 = v[1], v2 = v[2];
     I0[o] = v0;

@@ -118,6 +118,20 @@ def yuv_shape(format, width, height):
     return (height * 3 // 2, width) if is420 else (height, width, 2)
 
 
+def bayer_kind(pattern, method="bilinear"):
+    """(PSM_BAYER_*, PSM_DEMOSAIC_*) of a pattern name ("rggb", "bggr", "grbg" or "gbrg": the colours of the 2 x 2 cell at
+    (0, 0) in reading order) and a method name ("bilinear" or "ea", cv2's COLOR_Bayer<PATTERN>2BGR and _EA); ValueError on
+    any other value"""
+    names = []
+    for value, table, what in ((pattern, capi.BAYER_PATTERNS, "Bayer pattern"),
+                               (method, capi.DEMOSAIC_METHODS, "demosaicing method")):
+        name = value.lower() if isinstance(value, str) else value
+        if name not in table:
+            raise ValueError(f"unknown {what} {value!r}: one of {', '.join(table)}")
+        names.append(table[name])
+    return tuple(names)
+
+
 class DispEst:
     """DispEst(l, r, d, t, ocl) -- reference src/DispEst.cpp:10-143.
 
@@ -171,6 +185,7 @@ class DispEst:
         self.src_size = None   # setRectify: (SW, SH) of the camera frames CostConst_GPU takes
         self._lImg, self._rImg = l, r
         self._yuv = None   # setInputImagesYUV's format code while its frames are the input
+        self._bayer = None   # setInputImagesBayer's (pattern, method) codes while its frames are the input
         self._ctx = C.c_void_p()
         self._lib = None
         if self.useOCL:
@@ -207,7 +222,7 @@ class DispEst:
         leftImg, rightImg = np.asarray(leftImg), np.asarray(rightImg)
         assert leftImg.dtype == rightImg.dtype
         self._lImg, self._rImg = leftImg, rightImg
-        self._yuv = None
+        self._yuv = self._bayer = None
         return 0
 
     def setInputImagesYUV(self, left, right, format):
@@ -222,6 +237,22 @@ class DispEst:
             raise TypeError(f"YUV frames must be uint8 (got {left.dtype}, {right.dtype})")
         self._lImg, self._rImg = left, right
         self._yuv = (code, format)
+        self._bayer = None
+        return 0
+
+    def setInputImagesBayer(self, left, right, pattern, method="bilinear"):
+        """Bayer raw frames as input (psm_set_images_bayer): uint8 numpy arrays (H, W) of the constructor's size or
+        setRectify's source size, whose pixel (0, 0) starts the pattern ("rggb", "bggr", "grbg" or "gbrg").  CostConst_GPU
+        demosaics them on the device as cv2.cvtColor(frame, COLOR_Bayer<PATTERN>2BGR) (method "bilinear") or _EA ("ea")
+        does, bit for bit.  Raises ValueError on an unknown pattern or method and TypeError on frames that are not uint8;
+        CostConst_GPU checks the shape."""
+        codes = bayer_kind(pattern, method)
+        left, right = np.asarray(left), np.asarray(right)
+        if left.dtype != np.uint8 or right.dtype != np.uint8:
+            raise TypeError(f"Bayer frames must be uint8 (got {left.dtype}, {right.dtype})")
+        self._lImg, self._rImg = left, right
+        self._yuv = None
+        self._bayer = codes
         return 0
 
     def setThreads(self, newThreads):
@@ -390,6 +421,14 @@ class DispEst:
                                  f"of setRectify (got {l.shape}, {r.shape})")
             capi.check(self._lib.psm_set_images_yuv(self._ctx, code, _ptr(l), l.strides[0], _ptr(r), r.strides[0]),
                        self._ctx)
+            capi.check(self._lib.psm_cost_const(self._ctx), self._ctx)
+            return 0
+        if self._bayer is not None:
+            if l.shape != (h, w) or r.shape != (h, w):
+                raise ValueError(f"Bayer frames must be {(h, w)}: the size DispEst was constructed with, or the source size "
+                                 f"of setRectify (got {l.shape}, {r.shape})")
+            capi.check(self._lib.psm_set_images_bayer(self._ctx, *self._bayer, _ptr(l), l.strides[0], _ptr(r),
+                                                      r.strides[0]), self._ctx)
             capi.check(self._lib.psm_cost_const(self._ctx), self._ctx)
             return 0
         if l.shape != (h, w, 3) or r.shape != l.shape:

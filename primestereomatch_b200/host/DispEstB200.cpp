@@ -54,6 +54,7 @@ int DispEst::setInputImages(cv::Mat leftImg, cv::Mat rightImg)
     lImg = leftImg;
     rImg = rightImg;
     yuv_format = 0;
+    bayer_pattern = 0;
     return 0;
 }
 
@@ -66,6 +67,21 @@ int DispEst::setInputImagesYUV(cv::Mat leftImg, cv::Mat rightImg, int format)
     lImg = leftImg;
     rImg = rightImg;
     yuv_format = format;
+    bayer_pattern = 0;
+    return 0;
+}
+
+int DispEst::setInputImagesBayer(cv::Mat leftImg, cv::Mat rightImg, int pattern, int method)
+{
+    if (pattern < PSM_BAYER_RGGB || pattern > PSM_BAYER_GBRG || (method != PSM_DEMOSAIC_BILINEAR && method != PSM_DEMOSAIC_EA)) {
+        std::fprintf(stderr, "DispEst::setInputImagesBayer: unknown pattern %d or method %d\n", pattern, method);
+        return -1;
+    }
+    lImg = leftImg;
+    rImg = rightImg;
+    yuv_format = 0;
+    bayer_pattern = pattern;
+    bayer_method = method;
     return 0;
 }
 
@@ -215,6 +231,17 @@ int DispEst::CostConst_GPU()
                 return -1;
             }
         if (int rc = psm_set_images_yuv(ctx, yuv_format, lImg.ptr<uint8_t>(), lImg.step, rImg.ptr<uint8_t>(), rImg.step))
+            return rc;
+        return psm_cost_const(ctx);
+    }
+    if (bayer_pattern) {
+        for (const cv::Mat* m : {&lImg, &rImg})
+            if (m->rows != fh || m->cols != fw || m->type() != CV_8UC1) {
+                std::fprintf(stderr, "DispEst::CostConst_GPU: Bayer frames must be %dx%d CV_8UC1\n", fw, fh);
+                return -1;
+            }
+        if (int rc = psm_set_images_bayer(ctx, bayer_pattern, bayer_method, lImg.ptr<uint8_t>(), lImg.step,
+                                          rImg.ptr<uint8_t>(), rImg.step))
             return rc;
         return psm_cost_const(ctx);
     }

@@ -104,6 +104,10 @@ public:
     // of (H * 3 / 2) x W for the 4:2:0 formats, CV_8UC2 of H x W for the 4:2:2 ones, of the context's size or setRectify's
     // source size.  CostConst_GPU converts them to BGR on the device as cvtColor(COLOR_YUV2BGR_*) does.
     int setInputImagesYUV(cv::Mat l, cv::Mat r, int format);
+    // Bayer raw frames as input (psm_set_images_bayer): pattern PSM_BAYER_RGGB ... PSM_BAYER_GBRG (the colours of the
+    // 2 x 2 cell at (0, 0)), method PSM_DEMOSAIC_BILINEAR or PSM_DEMOSAIC_EA, CV_8UC1 frames of the context's size or
+    // setRectify's source size.  CostConst_GPU demosaics them on the device as cvtColor(COLOR_Bayer*2BGR[_EA]) does.
+    int setInputImagesBayer(cv::Mat l, cv::Mat r, int pattern, int method = PSM_DEMOSAIC_BILINEAR);
     int setThreads(unsigned int newThreads);
     void setSubsampleRate(unsigned int newRate) { subsample_rate = newRate; }
     // guided-filter window and eps (the reference's GIF_R_WIN / GIF_EPS) for the later CostFilter calls; see
@@ -187,6 +191,8 @@ private:
     int views = PSM_VIEWS_BOTH;
     int src_w = 0, src_h = 0;   // setRectify: the size of the frames CostConst_GPU takes, 0 = the context's
     int yuv_format = 0;         // setInputImagesYUV: the PSM_YUV_* format of lImg / rImg, 0 = BGR frames
+    int bayer_pattern = 0;      // setInputImagesBayer: the PSM_BAYER_* pattern of lImg / rImg, 0 = not Bayer frames
+    int bayer_method = PSM_DEMOSAIC_BILINEAR;
     bool cost_output = false;
     bool runner_up_output = false;
     int set_output(int key, bool on, bool& flag);

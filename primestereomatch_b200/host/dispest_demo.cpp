@@ -22,7 +22,9 @@
 // and left / right are then 8-bit BGR frames of SW x SH instead of float frames of W x H.  A leading `--yuv FORMAT`
 // (nv12, nv21, i420, yv12, yuyv, uyvy or yvyu) reads left / right as raw YUV frames in cv2's layout of W x H (or SW x SH
 // with --rectify): (H * 3 / 2) rows of W bytes for the 4:2:0 formats, H rows of 2 * W bytes for the 4:2:2 ones, converted
-// to BGR on the device (setInputImagesYUV).
+// to BGR on the device (setInputImagesYUV).  A leading `--bayer PATTERN` (rggb, bggr, grbg or gbrg) reads left / right
+// as Bayer raw frames of W x H (or SW x SH with --rectify), H rows of W bytes, demosaiced on the device
+// (setInputImagesBayer) as cvtColor(COLOR_Bayer<PATTERN>2BGR) does, or as _EA with a following `--ea`.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -48,6 +50,7 @@ int main(int argc, char** argv)
     int src_size[2] = {0, 0};                     // --rectify: SW, SH
     const char* map_files[2] = {nullptr, nullptr};
     int yuv = 0;                                  // --yuv: PSM_YUV_* of the frames, 0 = BGR
+    int bayer = 0, demosaic = PSM_DEMOSAIC_BILINEAR;   // --bayer: PSM_BAYER_* of the frames, 0 = not Bayer; --ea
     std::vector<int> devices;
     const bool left_only = argc >= 2 && !std::strcmp(argv[1], "--left-only");
     if (left_only) {
@@ -59,7 +62,25 @@ int main(int argc, char** argv)
                          !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle") ||
                          !std::strcmp(argv[1], "--disp-check") ||
                          !std::strcmp(argv[1], "--points") || !std::strcmp(argv[1], "--rectify") ||
-                         !std::strcmp(argv[1], "--yuv"))) {
+                         !std::strcmp(argv[1], "--yuv") || !std::strcmp(argv[1], "--bayer") ||
+                         !std::strcmp(argv[1], "--ea"))) {
+        if (!std::strcmp(argv[1], "--ea")) {
+            demosaic = PSM_DEMOSAIC_EA;
+            argv[1] = argv[0];
+            ++argv;
+            --argc;
+            continue;
+        }
+        if (!std::strcmp(argv[1], "--bayer")) {
+            static const char* const names[] = {"rggb", "bggr", "grbg", "gbrg"};
+            for (int k = 0; k < 4; ++k)
+                if (!std::strcmp(argv[2], names[k])) bayer = PSM_BAYER_RGGB + k;
+            if (!bayer) { std::fprintf(stderr, "unknown --bayer pattern %s\n", argv[2]); return 2; }
+            argv[2] = argv[0];
+            argv += 2;
+            argc -= 2;
+            continue;
+        }
         if (!std::strcmp(argv[1], "--yuv")) {
             static const char* const names[] = {"nv12", "nv21", "i420", "yv12", "yuyv", "uyvy", "yvyu"};
             for (int k = 0; k < 7; ++k)
@@ -124,7 +145,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--disp-check MODE MAXDIFF] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] [--yuv FORMAT] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--disp-check MODE MAXDIFF] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] [--yuv FORMAT | --bayer PATTERN [--ea]] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -134,16 +155,19 @@ int main(int argc, char** argv)
     const bool rectify = map_files[0] != nullptr;
     const int fw = rectify ? src_size[0] : W, fh = rectify ? src_size[1] : H;
     if (fw < 1 || fh < 1) { std::fprintf(stderr, "bad --rectify source size\n"); return 2; }
-    // with --yuv: CV_8UC1 of (fh * 3 / 2) x fw (4:2:0) or CV_8UC2 of fh x fw (4:2:2)
-    const int type = yuv ? (yuv <= PSM_YUV_YV12 ? CV_8UC1 : CV_8UC2) : rectify ? CV_8UC3 : CV_32FC3;
+    if (yuv && bayer) { std::fprintf(stderr, "--yuv and --bayer: the frames are one or the other\n"); return 2; }
+    // with --yuv: CV_8UC1 of (fh * 3 / 2) x fw (4:2:0) or CV_8UC2 of fh x fw (4:2:2); with --bayer: CV_8UC1 of fh x fw
+    const int type = bayer ? CV_8UC1 : yuv ? (yuv <= PSM_YUV_YV12 ? CV_8UC1 : CV_8UC2) : rectify ? CV_8UC3 : CV_32FC3;
     const int rows = yuv && yuv <= PSM_YUV_YV12 ? fh / 2 * 3 : fh;
     cv::Mat l(rows, fw, type), r(rows, fw, type);
     if (!read_all(argv[4], l.data, l.step * rows) || !read_all(argv[5], r.data, r.step * rows)) { std::fprintf(stderr, "bad input\n"); return 2; }
-    const bool framed = rectify || yuv;   // the frames do not give the context's size
+    const bool framed = rectify || yuv || bayer;   // the frames do not give the context's size
     cv::Mat sized(H, W, framed ? CV_8UC3 : l.type());   // the facade takes the context's size from its first frames
     DispEst* SMDE = new DispEst(framed ? sized : l, framed ? sized : r, D, MAX_CPU_THREADS, true, block_slices, devices,
                                 min_disp);
-    if (yuv)
+    if (bayer)
+        SMDE->setInputImagesBayer(l, r, bayer, demosaic);
+    else if (yuv)
         SMDE->setInputImagesYUV(l, r, yuv);
     else
         SMDE->setInputImages(l, r);

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import capi
-from .dispest import DispEst, create_context, rectify_args, resolve_map_bits, yuv_format, yuv_shape
+from .dispest import DispEst, bayer_kind, create_context, rectify_args, resolve_map_bits, yuv_format, yuv_shape
 
 _PIX = {torch.uint8: capi.PSM_PIX_U8, torch.float32: capi.PSM_PIX_F32}
 _ORDER = {"bgr": (0, 1, 2), "rgb": (2, 1, 0)}   # the tensor channel that holds B, G and R
@@ -110,6 +110,39 @@ def yuv_layout(t, height, width, format):
     base = t.data_ptr()
     frames = [tuple(base + b * bstride + o for o in offsets) for b in range(n)]
     return (sampling, frames) + steps + (batched,)
+
+
+def bayer_layout(t, height, width, pattern, method="bilinear"):
+    """The psm_set_images_device_bayer arguments of a Bayer frame tensor, or of each frame of a batch.
+
+    t: uint8 (H, W), optionally with a leading batch dimension, any strides (the halves of one side-by-side (H, 2W) frame
+    included; each half is demosaiced as a frame of its own, and pattern names its own pixel (0, 0)).  -> (pattern code,
+    method code, [byte address] per frame, row_step, col_step, batched).  Raises TypeError or ValueError on anything the
+    layout cannot express; the tensor's device is not looked at."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"expected a torch.Tensor (got {type(t).__name__})")
+    if t.dtype != torch.uint8:
+        raise TypeError(f"Bayer frames must be uint8 tensors (got {t.dtype})")
+    codes = bayer_kind(pattern, method)
+    if t.dim() not in (2, 3) or tuple(t.shape[-2:]) != (height, width):
+        raise ValueError(f"Bayer frames must be ({height}, {width}), optionally with a leading batch dimension "
+                         f"(got shape {tuple(t.shape)})")
+    sr, sc = t.stride()[-2:]
+    if sc < 1:
+        raise ValueError(f"the column stride is {sc} elements: pixels of a row must not share samples")
+    if sr < (width - 1) * sc + 1:
+        raise ValueError(f"the row stride ({sr} elements) is shorter than a row ({width} pixels {sc} elements apart)")
+    batched = t.dim() == 3
+    n, bstride = (t.shape[0], t.stride(0)) if batched else (1, 0)
+    if n < 1:
+        raise ValueError("empty batch")
+    base = t.data_ptr()
+    return codes + ([base + b * bstride for b in range(n)], sr, sc, batched)
+
+
+def _pointers(frame):
+    """the C argument of one frame's addresses: three channel or plane pointers, or one frame pointer"""
+    return C.c_void_p(frame) if isinstance(frame, int) else (C.c_void_p * 3)(*frame)
 
 
 class TorchStereo:
@@ -209,18 +242,27 @@ class TorchStereo:
         self.subsample_rate = int(rate)
 
     # -- frames -------------------------------------------------------------------------------
-    def _layout(self, left, right, channels, yuv=None):
+    def _layout(self, left, right, channels, yuv=None, bayer=None, demosaic="bilinear"):
         """Both frames' layout, checked in full before any device work: (H, W) frames, or uint8 frames of the source
-        size while setRectify is on -> (the C-ABI call that takes them, its argument before the pointers, left frames,
+        size while setRectify is on -> (the C-ABI call that takes them, its arguments before the pointers, left frames,
         right frames, its steps, batched)"""
         w, h = self.src_size or (self.width, self.height)
+        if yuv is not None and bayer is not None:
+            raise ValueError("yuv and bayer: a frame is one or the other")
+        if bayer is not None:
+            pattern, method, lf, row_step, col_step, batched = bayer_layout(left, h, w, bayer, demosaic)
+            other = bayer_layout(right, h, w, bayer, demosaic)
+            if left.shape != right.shape or (row_step, col_step) != other[3:5]:
+                raise ValueError("left and right must have the same shape and strides")
+            self._check_devices(left, right)
+            return "psm_set_images_device_bayer", (pattern, method), lf, other[2], (row_step, col_step), batched
         if yuv is not None:
             sampling, lf, *steps, batched = yuv_layout(left, h, w, yuv)
             other = yuv_layout(right, h, w, yuv)
             if left.shape != right.shape or tuple(steps) != tuple(other[2:6]):
                 raise ValueError("left and right must have the same shape and strides")
             self._check_devices(left, right)
-            return "psm_set_images_device_yuv", sampling, lf, other[1], tuple(steps), batched
+            return "psm_set_images_device_yuv", (sampling,), lf, other[1], tuple(steps), batched
         pix, lf, row_step, col_step, batched = frame_layout(left, h, w, channels)
         other = frame_layout(right, h, w, channels)
         if self.src_size is not None and pix != capi.PSM_PIX_U8:
@@ -228,21 +270,26 @@ class TorchStereo:
         if left.shape != right.shape or left.dtype != right.dtype or (pix, row_step, col_step) != (other[0], other[2], other[3]):
             raise ValueError("left and right must have the same shape, dtype and strides")
         self._check_devices(left, right)
-        return "psm_set_images_device_planes", pix, lf, other[1], (row_step, col_step), batched
+        return "psm_set_images_device_planes", (pix,), lf, other[1], (row_step, col_step), batched
 
     def _check_devices(self, left, right):
         for name, t in (("left", left), ("right", right)):
             if t.device != self.device:
                 raise ValueError(f"{name} is on {t.device}: frames must be CUDA tensors on the context's device {self.device}")
 
-    def match(self, left, right, *, channels="bgr", yuv=None, fgf=False, post_process=False, costs=False,
-              runner_up=False, points=None, handle_missing=False):
+    def match(self, left, right, *, channels="bgr", yuv=None, bayer=None, demosaic="bilinear", fgf=False,
+              post_process=False, costs=False, runner_up=False, points=None, handle_missing=False):
         """Disparity maps of one frame pair or a batch -> (lmap, rmap): new uint8 / uint16 tensors of shape (H, W) or
         (B, H, W) on the context's device; rmap is None on a left-only context.
 
         yuv="nv12" (or "nv21", "i420", "yv12", "yuyv", "uyvy", "yvyu"): the frames are uint8 YUV tensors in cv2's shapes
         (yuv_layout; the halves of one side-by-side frame included), converted to BGR on the device as
         cv2.cvtColor(frame, COLOR_YUV2BGR_<FORMAT>) does (psm_set_images_device_yuv); channels is not read.
+
+        bayer="rggb" (or "bggr", "grbg", "gbrg"): the frames are uint8 Bayer tensors (H, W) (bayer_layout; the halves of
+        one side-by-side frame included, each demosaiced as a frame of its own), demosaiced on the device as
+        cv2.cvtColor(frame, COLOR_Bayer<PATTERN>2BGR) does with demosaic="bilinear", or _EA with demosaic="ea"
+        (psm_set_images_device_bayer); channels is not read.
 
         costs=True -> (lmap, rmap, lcosts, rcosts): also the filtered costs beside each winner of the selection maps
         (PSM_OPT_COSTS, psm_copy_costs_device), new float32 tensors (3, H, W) or (B, 3, H, W) whose plane k holds the cost
@@ -260,7 +307,7 @@ class TorchStereo:
         float32 tensors (H, W, 3) or (B, H, W, 3) of X, Y, Z; either Q may be None, and its tensor is then None.
         handle_missing=True sets Z = 10000 wherever a map holds its minimum.
 
-        After psm_wait_stream on torch's current stream: psm_set_images_device_planes (or _device_yuv), psm_cost_const, the guided filter
+        After psm_wait_stream on torch's current stream: psm_set_images_device_planes (or _device_yuv, _device_bayer), psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
         with post_process=True (the chain setDisparityCheck, setSpeckleFilter, setLRCheck and setPostFilter configure),
         psm_copy_maps_device and, with points, psm_reproject_device of each frame of a batch in turn; then
@@ -281,7 +328,7 @@ class TorchStereo:
                 raise ValueError("points: a right Q on a left-only context (setViews('left'))")
             if qs[0] is None and qs[1] is None:
                 raise ValueError("points: give a Q for at least one view")
-        set_images, kind, lf, rf, steps, batched = self._layout(left, right, channels, yuv)
+        set_images, lead, lf, rf, steps, batched = self._layout(left, right, channels, yuv, bayer, demosaic)
         L, ctx = self._lib, self._ctx
         H, W = self.height, self.width
         mdt = torch.uint16 if self.map_bits == 16 else torch.uint8
@@ -307,8 +354,7 @@ class TorchStereo:
             pts = [None if q is None else torch.empty(pshape, dtype=torch.float32, device=self.device) for q in qs]
         self._check(L.psm_wait_stream(ctx, stream))
         for b in range(len(lf)):
-            lp, rp = (C.c_void_p * 3)(*lf[b]), (C.c_void_p * 3)(*rf[b])
-            self._check(getattr(L, set_images)(ctx, kind, lp, rp, *steps))
+            self._check(getattr(L, set_images)(ctx, *lead, _pointers(lf[b]), _pointers(rf[b]), *steps))
             self._check(L.psm_cost_const(ctx))
             self._check(L.psm_cost_filter_fgf(ctx, self.subsample_rate) if fgf else L.psm_cost_filter(ctx))
             self._check(L.psm_disp_select_device(ctx))
