@@ -58,9 +58,9 @@
  * (the scratch of the reference-order pass: float frames, a non-default guided filter, PSM_CVF_NAIVE, flagged slices),
  * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
  * (its buffers and, after a change of sigma or weight type, the weight table; with psm_set_speckle_filter on, the
- * labels and counts, 8 * W * H bytes per view, and with PSM_SPECKLE_FIRST and a check mode, a map pair between the
- * removal and the check; with psm_set_disparity_check on, a map per computed view between the check and the next step and,
- * on rows over 6144 columns, its claim words), psm_set_option(PSM_OPT_COSTS, 1) (the
+ * labels and counts, 8 * W * H bytes per view; with psm_set_disparity_check on rows over 6144 columns, its claim words;
+ * with two or more of the check, removal and left-right steps, one map per computed view between them),
+ * psm_set_option(PSM_OPT_COSTS, 1) (the
  * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots), psm_reproject_device with
  * handle_missing (8 bytes of scratch).  Run them once before a
  * latency-critical

@@ -90,6 +90,7 @@ struct psm_ctx {
     void* fgf_plan = nullptr;               // FgfTap x[W], y[H]: INTER_LINEAR source indices and weights
     int fgf_s = 0;                          // sub-sampling rate the buffers / plan were built for
     uint8_t* dis_pp[2] = {nullptr, nullptr}; // post-processed maps (map_bytes per element)
+    uint8_t* pp_tmp[2] = {nullptr, nullptr}; // per computed view, lazy: the maps between two post-process steps
     uint32_t* pp_packed = nullptr;          // packed (disparity, 6-bit colour) image of one view, lazy
     uint32_t* pp_lut = nullptr;             // weight table of the current post-filter setting (kPpMaxD2 + 1 entries), lazy
     bool pp_lut_valid = false;              // pp_lut holds the table of (pp_sigma, pp_type)
@@ -131,13 +132,9 @@ struct psm_ctx {
     int sp_max_size = 0, sp_max_diff = 0;
     int* sp_lab = nullptr;                  // speckle removal's labels and counts: 2 x W x H each (view v at v * W * H), lazy
     int* sp_cnt = nullptr;
-    uint8_t* sp_maps[2] = {nullptr, nullptr};  // PSM_SPECKLE_FIRST with the check: the filtered maps the check reads, lazy
     int dc_mode = PSM_DCHECK_OFF;           // one-view disparity check in the post-process stage, psm_set_disparity_check
     int dc_max_diff = 1;
-    // per computed view, lazy: PSM_DCHECK_FIRST with speckle removal or the check: its result; rows wider than
-    // kDcStageCols: the claim words, W x H
-    uint8_t* dc_maps[2] = {nullptr, nullptr};
-    unsigned long long* dc_claims[2] = {nullptr, nullptr};
+    unsigned long long* dc_claims[2] = {nullptr, nullptr};  // W > kDcStageCols: the claim words, W x H per computed view, lazy
     // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
     // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
     int blk_slices = 0;
@@ -1694,7 +1691,7 @@ int psm_destroy(psm_ctx* c)
     cudaFree(c->rp_min); cudaFree(c->rp_buf);
     for (int v = 0; v < 2; ++v) { cudaFree(c->rect_xy[v]); cudaFree(c->rect_a[v]); }
     for (int v = 0; v < 2; ++v) { cudaFree(c->dis_pp[v]); cudaFree(c->lr_valid[v]); cudaFree(c->run_keys[v]);
-                                   cudaFree(c->sp_maps[v]); cudaFree(c->dc_maps[v]); cudaFree(c->dc_claims[v]);
+                                   cudaFree(c->pp_tmp[v]); cudaFree(c->dc_claims[v]);
                                    cudaFree(c->track[v]); cudaFree(c->ru_list[v]); cudaFree(c->ru_slots[v]);
                                    for (psm_ctx::OutState& o : c->outs) cudaFree(o.planes[v]); }
     for (int s = 0; s < kNumStages; ++s) {
@@ -2700,7 +2697,42 @@ static int disparity_check(psm_ctx* c, const uint8_t* const in[2], uint8_t* cons
     return PSM_OK;
 }
 
-// the post-filter stage on maps of type T
+// lrCheck + fillInv (PP.cpp:405-406) of in[view] into out[view] and lr_valid; kOwn: the left view alone, its mask from the map itself
+template <typename T, bool kOwn>
+static int lr_check_fill(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
+{
+    const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;
+    lr_check_fill_kernel<T, kOwn><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
+        reinterpret_cast<const T*>(in[0]), kOwn ? nullptr : reinterpret_cast<const T*>(in[1]), c->W,
+        reinterpret_cast<T*>(out[0]), kOwn ? nullptr : reinterpret_cast<T*>(out[1]), c->lr_valid[0], kOwn ? nullptr : c->lr_valid[1]);
+    PSM_LAUNCH_CHECK(c);
+    c->lr_masks_ok = true;
+    return PSM_OK;
+}
+
+// psm_post_process's steps in front of the post-filter: the disparity check, speckle removal and the left-right check
+// and fill, each when on and in that order.  PSM_DCHECK_ONLY, PSM_SPECKLE_ONLY and PSM_LR_FILL end the chain after their
+// step, and then the post-filter (wmf) does not run.  With the check on, a left-only context fills from its result.
+template <typename T>
+struct PpChain {
+    using Step = int (*)(psm_ctx*, const uint8_t* const*, uint8_t* const*);
+    Step step[3];
+    int n = 0;
+    bool wmf = false;
+    explicit PpChain(const psm_ctx* c)
+    {
+        if (c->dc_mode != PSM_DCHECK_OFF) step[n++] = disparity_check<T>;
+        if (c->dc_mode == PSM_DCHECK_ONLY) return;
+        if (c->sp_mode != PSM_SPECKLE_OFF) step[n++] = speckle_filter<T>;
+        if (c->sp_mode == PSM_SPECKLE_ONLY) return;
+        if (c->lr_mode != PSM_LR_OFF)
+            step[n++] = c->views == 1 && has(disparity_check<T>) ? lr_check_fill<T, true> : lr_check_fill<T, false>;
+        wmf = c->lr_mode != PSM_LR_FILL;
+    }
+    bool has(Step s) const { return std::find(step, step + n, s) != step + n; }
+};
+
+// the post-process stage on maps of type T
 template <typename T>
 static int post_process_maps(psm_ctx* c)
 {
@@ -2714,44 +2746,36 @@ static int post_process_maps(psm_ctx* c)
     const uint8_t* maps[2];
     if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
-    // PSM_DCHECK_ONLY: the disparity check is the whole stage; PSM_SPECKLE_ONLY: the removal (after the disparity
-    // check) is; the left-right check and the post-filter do not run
-    const bool dc = c->dc_mode != PSM_DCHECK_OFF, dc_only = c->dc_mode == PSM_DCHECK_ONLY;
-    const bool sp = !dc_only && c->sp_mode != PSM_SPECKLE_OFF, only = dc_only || c->sp_mode == PSM_SPECKLE_ONLY;
-    const bool lr = !only && c->lr_mode != PSM_LR_OFF, wmf = !only && c->lr_mode != PSM_LR_FILL;
-    // a left-only context fills with the disparity check's result in place of the two-view check
-    const bool own_fill = lr && dc && c->views == 1;
-    if (dc && !c->outs[kOutCosts].have)
+    const PpChain<T> p(c);
+    if (p.has(disparity_check<T>) && !c->outs[kOutCosts].have)
         return fail(c, PSM_ESTATE, "psm_post_process: the disparity check (psm_set_disparity_check mode %d) reads the "
                     "winners' costs, and the last selection stage did not write them: set PSM_OPT_COSTS = 1 before it",
                     c->dc_mode);
-    if (lr && c->views == 1 && !own_fill)
+    if (p.has(lr_check_fill<T, false>) && c->views == 1)
         return fail(c, PSM_ESTATE, "psm_post_process: the left-right check (psm_set_lr_check mode %d) needs both maps, and "
                     "this context computes the left view alone (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): set PSM_LR_OFF or "
                     "PSM_VIEWS_BOTH", c->lr_mode);
-    if (sp && npix > (size_t)INT_MAX)
+    if (p.has(speckle_filter<T>) && npix > (size_t)INT_MAX)
         return fail(c, PSM_EINVAL, "psm_post_process: speckle removal labels pixels with int32 indices (W * H <= 2^31 - 1)");
     // Each buffer is allocated while its own pointer is null and the table is marked valid only once it is on the
     // device, so a call that failed part-way leaves nothing a launch could trip over: the next call completes the set-up
     // or fails in turn.
-    if (wmf) {
+    if (p.wmf) {
         PSM_CUDA(c, alloc_if_null(c->pp_lut, (kPpMaxD2 + 1) * sizeof(uint32_t)));
         PSM_CUDA(c, alloc_if_null(c->pp_packed, npix * sizeof(uint32_t)));
     }
     for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->dis_pp[v], npix * c->map_bytes));
-    if (lr)
+    if (p.has(lr_check_fill<T, false>) || p.has(lr_check_fill<T, true>))
         for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->lr_valid[v], npix));
-    if (dc && (sp || lr))
-        for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->dc_maps[v], npix * c->map_bytes));
-    if (dc && c->W > kDcStageCols)
+    if (p.n >= 2)
+        for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->pp_tmp[v], npix * c->map_bytes));
+    if (p.has(disparity_check<T>) && c->W > kDcStageCols)
         for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->dc_claims[v], npix * sizeof(unsigned long long)));
-    if (sp) {
+    if (p.has(speckle_filter<T>)) {
         PSM_CUDA(c, alloc_if_null(c->sp_lab, 2 * npix * sizeof(int)));
         PSM_CUDA(c, alloc_if_null(c->sp_cnt, 2 * npix * sizeof(int)));
-        if (lr)
-            for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->sp_maps[v], npix * c->map_bytes));
     }
-    if (wmf && !c->pp_lut_valid) {
+    if (p.wmf && !c->pp_lut_valid) {
         const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
         PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
@@ -2767,38 +2791,13 @@ static int post_process_maps(psm_ctx* c)
     const bool tuned = c->pp_tuned();
     if (int rc = p2p_wait_done(c)) return rc;
     if (int rc = stage_begin(c, 5)) return rc;
-    if (dc) {
-        // the check reads the selection maps and writes the stage's result (PSM_DCHECK_ONLY, or the post-filter's first
-        // input) or the input of the removal or of the left-right check
-        uint8_t* const out[2] = {sp || lr ? c->dc_maps[0] : c->dis_pp[0], sp || lr ? c->dc_maps[1] : c->dis_pp[1]};
-        if (int rc = disparity_check<T>(c, maps, out)) return rc;
-        if (dc_only) return stage_end(c, 5);
+    // the last step writes dis_pp, the ones before alternate back through pp_tmp: no step writes the maps it reads
+    for (int i = 0; i < p.n; ++i) {
+        uint8_t* const* out = (p.n - 1 - i) % 2 ? c->pp_tmp : c->dis_pp;
+        if (int rc = p.step[i](c, maps, out)) return rc;
         maps[0] = out[0]; maps[1] = out[1];
     }
-    if (sp) {
-        // the removal reads the selection maps and writes the stage's result (PSM_SPECKLE_ONLY), the check's input, or
-        // the post-filter's first input (in place: each pass packs its input before it writes dis_pp)
-        uint8_t* const out[2] = {lr ? c->sp_maps[0] : c->dis_pp[0], lr ? c->sp_maps[1] : c->dis_pp[1]};
-        if (int rc = speckle_filter<T>(c, maps, out)) return rc;
-        if (only) return stage_end(c, 5);
-        maps[0] = out[0]; maps[1] = out[1];
-    }
-    if (lr) {
-        // lrCheck + fillInv (PP.cpp:405-406): reads the selection maps, writes the filled maps into dis_pp
-        // (own_fill: the left view alone, its mask from the map itself; the right view's buffers are not touched)
-        const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;
-        if (own_fill)
-            lr_check_fill_kernel<T, true><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
-                reinterpret_cast<const T*>(maps[0]), nullptr, c->W, reinterpret_cast<T*>(c->dis_pp[0]), nullptr,
-                c->lr_valid[0], nullptr);
-        else
-            lr_check_fill_kernel<T, false><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
-                reinterpret_cast<const T*>(maps[0]), reinterpret_cast<const T*>(maps[1]), c->W,
-                reinterpret_cast<T*>(c->dis_pp[0]), reinterpret_cast<T*>(c->dis_pp[1]), c->lr_valid[0], c->lr_valid[1]);
-        PSM_LAUNCH_CHECK(c);
-        c->lr_masks_ok = true;
-        if (!wmf) return stage_end(c, 5);
-    }
+    if (!p.wmf) return stage_end(c, 5);
     int nsm = 0;
     PSM_CUDA(c, cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, c->device));
     const int lut_n = pp_weight_table_size(c->pp_type);
@@ -2812,9 +2811,9 @@ static int post_process_maps(psm_ctx* c)
         T* dst = reinterpret_cast<T*>(c->dis_pp[v]);
         dim3 blk(256), grd((c->W + 255) / 256, c->H);
         // JointWMF.h:126-131: the feature image stays the original, each pass filters the previous pass's output (after
-        // the left-right fill, the first pass filters the filled map)
+        // the earlier steps, the first pass filters their result; it packs its input before it writes dis_pp)
         for (int it = 0; it < c->pp_iter; ++it) {
-            const T* src = reinterpret_cast<const T*>(it == 0 && !lr ? maps[v] : c->dis_pp[v]);
+            const T* src = reinterpret_cast<const T*>(it == 0 ? maps[v] : c->dis_pp[v]);
             pp_pack_kernel<T><<<grd, blk, 0, c->stream>>>(g, g + c->plane, g + 2 * c->plane, c->Wp, src, c->W, c->H, c->pp_packed);
             PSM_LAUNCH_CHECK(c);
             if (tuned)

@@ -29,14 +29,12 @@ import random
 import numpy as np
 
 import cost_triple_cases as CT
-import dcheck_oracle as DC
-import lr_oracle as LR
 import mixed_model as MM
+import pp_chain as PP
 import range_cases as RC
 import rectify_oracle as RO
 import reproject_oracle as RP
 import runner_up_cases as RU
-import speckle_oracle as SP
 from oracle import oracle as O
 from primestereomatch_b200 import synth
 
@@ -328,10 +326,9 @@ def expect(config, fr, D=None):
     post = POSTS[config["post"]]
     if post is not None:
         dcheck, speckle, lr, setting = post
-        ld, rd, masks = DC.chain(l, r, out["selection", 0], out.get(("selection", 1)), costs[0][1].view(np.float32),
-                                 None if costs[1] is None else costs[1][1].view(np.float32), D, dcheck, speckle, lr,
-                                 setting, post_process=O.post_process, lr_check_fill=LR.lr_check_fill,
-                                 filter_speckles=SP.filter_speckles, fill=LR.fill)
+        q = [None if c is None else c[1].view(np.float32) for c in costs]
+        ld, rd, masks = PP.chain(l, r, out["selection", 0], out.get(("selection", 1)), dcheck=dcheck, costs=q, D=D,
+                                 speckle=speckle, lr=lr, setting=setting)
         for v, m in zip(views, (ld, rd)):
             out["post", v] = m
             if masks is not None:

@@ -88,32 +88,3 @@ def winner_costs(vol, m):
     """plane 1 of PSM_OPT_COSTS from a filtered volume [D, H, W]: q(m) at each pixel (q(0) where m = 0)"""
     return np.take_along_axis(vol, m.astype(np.int64)[None], axis=0)[0]
 
-
-def chain(l_img, r_img, ld, rd, lc, rc, D, dcheck, speckle=(0, 0, 0), lr_mode=0, setting=(9, 25.5, 1, "exp"),
-          post_process=None, lr_check_fill=None, filter_speckles=None, fill=None):
-    """What psm_post_process computes with psm_set_disparity_check(dcheck = (mode, max_diff)), speckle (mode, max_size,
-    max_diff), left-right check mode lr_mode and post-filter `setting` -> (left, right, (lValid, rValid) or None); right
-    None when rd is None (a left-only context, which fills with valid = v >= 2).  The callables are the oracle's
-    post-filter and the lr / speckle restatements."""
-    mode, diff = dcheck
-    if mode:
-        ld = check(ld, lc, D, diff)
-        rd = None if rd is None else check(rd, rc, D, diff, view=1)
-        if mode == 2:
-            return ld, rd, None
-    if speckle[0]:
-        ld = filter_speckles(ld, *speckle[1:])
-        rd = None if rd is None else filter_speckles(rd, *speckle[1:])
-        if speckle[0] == 2:
-            return ld, rd, None
-    masks = None
-    if lr_mode:
-        if rd is None:
-            lv = (ld >= 2).astype(np.uint8)
-            ld, masks = fill(ld, lv), (lv, None)
-        else:
-            lv, rv, ld, rd = lr_check_fill(ld, rd)
-            masks = (lv, rv)
-        if lr_mode == 2:
-            return ld, rd, masks
-    return (post_process(l_img, ld, *setting), None if rd is None else post_process(r_img, rd, *setting), masks)

@@ -36,6 +36,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 from conftest import read_png  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 import lr_oracle as LR  # noqa: E402
+import pp_chain as PP  # noqa: E402
 
 REF = os.environ.get("REF", "/root/reference")
 
@@ -135,7 +136,7 @@ def main():
                 H, W = ld.shape
                 want_l, want_r = np.empty((H, W), np.uint8), np.empty((H, W), np.uint8)
                 assert L.ref_process_dm_lr(li, ri, ld, rd, W, H, radius, sigma, it, O.WEIGHTS[weight], want_l, want_r) == 0
-                got_l, got_r = LR.post_process(li, ri, ld, rd, 1, (radius, sigma, it, weight))
+                got_l, got_r, _ = PP.chain(li, ri, ld, rd, lr=1, setting=(radius, sigma, it, weight))
                 ent["scenes"][name] = {v: {"sha": sha(g), "ref_sha": sha(w), "differ": int((g != w).sum())}
                                        for v, g, w in (("l", got_l, want_l), ("r", got_r, want_r))}
             print((radius, sigma, it, weight), {k: [v["differ"] for v in s.values()] for k, s in ent["scenes"].items()},

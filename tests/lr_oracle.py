@@ -11,8 +11,6 @@ unchanged.
 """
 import numpy as np
 
-from oracle import oracle as O
-
 MODES = {"off": 0, "fill_wmf": 1, "fill": 2}   # PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL
 
 
@@ -46,12 +44,3 @@ def lr_check_fill(l, r):
     lv, rv = lr_check(l, r)
     return lv, rv, fill(l, lv), fill(r, rv)
 
-
-def post_process(l_img, r_img, ld, rd, mode, setting=(9, 25.5, 1, "exp")):
-    """What psm_post_process computes in lr-check mode `mode` (0, 1, 2) at post-filter `setting` -> (left, right)"""
-    if mode == 0:
-        return O.post_process(l_img, ld, *setting), O.post_process(r_img, rd, *setting)
-    _, _, lf, rf = lr_check_fill(ld, rd)
-    if mode == 2:
-        return lf, rf
-    return O.post_process(l_img, lf, *setting), O.post_process(r_img, rf, *setting)

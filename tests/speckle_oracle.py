@@ -75,22 +75,5 @@ def filter_speckles_flood(m, max_size, max_diff):
     return out
 
 
-def chain(l_img, r_img, ld, rd, speckle, lr_mode, setting=(9, 25.5, 1, "exp"), post_process=None, lr_check_fill=None):
-    """What psm_post_process computes with psm_set_speckle_filter(speckle = (mode, max_size, max_diff)), left-right
-    check mode lr_mode and post-filter `setting` -> (left, right); right None when rd is None.  post_process and
-    lr_check_fill are the oracle's post-filter and tests/lr_oracle.py's check."""
-    mode, size, diff = speckle
-    if mode:
-        ld = filter_speckles(ld, size, diff)
-        rd = None if rd is None else filter_speckles(rd, size, diff)
-        if mode == 2:
-            return ld, rd
-    if lr_mode:
-        _, _, ld, rd = lr_check_fill(ld, rd)
-        if lr_mode == 2:
-            return ld, rd
-    return post_process(l_img, ld, *setting), None if rd is None else post_process(r_img, rd, *setting)
-
-
 def sha(a):
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()

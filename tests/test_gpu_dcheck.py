@@ -13,10 +13,10 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, ROOT
-from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
 import dcheck_oracle as DC
 import lr_oracle as LR
+import pp_chain as PP
 import speckle_oracle as SP
 
 pytestmark = pytest.mark.gpu
@@ -59,11 +59,9 @@ def post(de, dcheck, speckle=(0, 0, 0), lr=0, setting=DEFAULT):
     return de.lDisMap.copy(), None if de.rDisMap is None else de.rDisMap.copy()
 
 
-def want(l, r, sel, D, dcheck, speckle=(0, 0, 0), lr=0, setting=DEFAULT, wmf=True):
+def want(l, r, sel, D, dcheck, speckle=(0, 0, 0), lr=0, setting=DEFAULT):
     ld, rd, lc, rc = sel
-    return DC.chain(l, r, ld, rd, lc, rc, D, dcheck, speckle, lr, setting,
-                    post_process=O.post_process if wmf else None, lr_check_fill=LR.lr_check_fill,
-                    filter_speckles=SP.filter_speckles, fill=LR.fill)
+    return PP.chain(l, r, ld, rd, dcheck=dcheck, costs=(lc, rc), D=D, speckle=speckle, lr=lr, setting=setting)
 
 
 def check_against(de, l, r, sel, D, what, **kw):
@@ -110,13 +108,10 @@ def test_every_mode_with_every_speckle_and_check_mode(bits):
                 for sp in ((0, 0, 0), (1, 6, 1), (2, 6, 1)):
                     for lr in (0, 1, 2):
                         what = f"u{bits} dcheck {dc} speckle {sp} lr {lr} {setting}"
-                        check_against(de, l, r, sel, D, what, dcheck=dc, speckle=sp, lr=lr, setting=setting)
+                        _, ref = check_against(de, l, r, sel, D, what, dcheck=dc, speckle=sp, lr=lr, setting=setting)
                         ran = lr and dc[0] != ONLY and sp[0] != 2
                         if ran:
-                            v = DC.check(sel[0], sel[2], D, dc[1]), DC.check(sel[1], sel[3], D, dc[1], view=1)
-                            if sp[0]:
-                                v = SP.filter_speckles(v[0], *sp[1:]), SP.filter_speckles(v[1], *sp[1:])
-                            lv, rv = LR.lr_check(*v)
+                            lv, rv = ref[2]
                             assert_same(de.lValid, lv, what + " left mask"); assert_same(de.rValid, rv, what + " right mask")
 
 
@@ -364,7 +359,7 @@ def test_cpp_demo_disp_check_flag(tmp_path, scenes, oracle_scene_results):
                          capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stderr
     sel = (ref["ld"], ref["rd"], DC.winner_costs(ref["lf"], ref["ld"]), DC.winner_costs(ref["rf"], ref["rd"]))
-    exp = want(l, r, sel, 64, (FIRST, 1), (1, 100, 1), 2, wmf=False)
+    exp = want(l, r, sel, 64, (FIRST, 1), (1, 100, 1), 2)
     assert_same(got()[0], exp[0], "demo first + speckle + fill left"); assert_same(got()[1], exp[1], "demo right")
     bad = subprocess.run([exe, "--disp-check", "1", "-3"] + tail, capture_output=True, text=True, timeout=300)
     assert bad.returncode == 1 and "disparity check" in bad.stderr

@@ -19,6 +19,7 @@ from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
 from primestereomatch_b200.sharding import shard_range
 import lr_oracle as LR
+import pp_chain as PP
 
 pytestmark = pytest.mark.gpu
 
@@ -125,7 +126,7 @@ def test_full_scenes_against_the_golden(scene, scenes, oracle_scene_results):
         gl, gr = run(de, 2)
         assert [sha(de.lValid), sha(de.rValid), sha(gl), sha(gr)] == [g["lValid"], g["rValid"], g["lFill"], g["rFill"]]
         gl, gr = run(de, 1)
-        want = LR.post_process(l, r, ref["ld"], ref["rd"], 1)
+        want = PP.chain(l, r, ref["ld"], ref["rd"], lr=1)
         assert_same(gl, want[0], "mode 1 left"); assert_same(gr, want[1], "mode 1 right")
     pl, pr = f32(posterise(l8)), f32(posterise(r8))
     with DispEst(pl, pr, 64) as de:
@@ -163,7 +164,7 @@ def test_u16_context_at_d64_equals_u8(scenes, oracle_scene_results):
             assert gb[0].dtype == np.uint16
             assert_same(gb[0], ga[0].astype(np.uint16), f"mode {mode} left"); assert_same(gb[1], ga[1].astype(np.uint16), f"mode {mode} right")
             assert_same(b.lValid, a.lValid, "left mask"); assert_same(b.rValid, a.rValid, "right mask")
-        assert_same(ga[0], LR.post_process(l, r, ref["ld"], ref["rd"], 1)[0], "u8 mode 1 left")
+        assert_same(ga[0], PP.chain(l, r, ref["ld"], ref["rd"], lr=1)[0], "u8 mode 1 left")
 
 
 @pytest.mark.parametrize("W,H,D", [(150, 10, 300), (97, 6, 600)])
@@ -293,7 +294,7 @@ def test_sharded_p2p_exchange_untouched(G):
 def test_switching_modes_between_frames_and_back():
     ld, rd = random_pair(64, 30, 24, seed=9)
     l, r = images(64, 30, seed=9)
-    want = {m: LR.post_process(l, r, ld, rd, m) for m in (0, 1, 2)}
+    want = {m: PP.chain(l, r, ld, rd, lr=m) for m in (0, 1, 2)}
     with DispEst(l, r, 24) as de:
         inject_maps(de, ld, rd)
         first = run(de, None)
@@ -393,7 +394,7 @@ def test_cpp_demo_mode_argument(tmp_path, scenes, oracle_scene_results):
     for mode in (1, 2, 0):
         out = subprocess.run(base + [str(mode)], capture_output=True, text=True, timeout=300)
         assert out.returncode == 0, out.stderr
-        want = LR.post_process(l, r, ref["ld"], ref["rd"], mode)
+        want = PP.chain(l, r, ref["ld"], ref["rd"], lr=mode)
         assert_same(np.fromfile(tmp_path / "l.u8", np.uint8).reshape(H, W), want[0], f"C++ facade left, mode {mode}")
         assert_same(np.fromfile(tmp_path / "r.u8", np.uint8).reshape(H, W), want[1], f"C++ facade right, mode {mode}")
     bad = subprocess.run(base + ["3"], capture_output=True, text=True, timeout=300)

@@ -9,7 +9,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import lr_oracle as LR
+import pp_chain as PP
 from conftest import ROOT
 from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
@@ -152,7 +152,7 @@ def test_settings(name):
     assert want[0].any()
     if name == "post":
         ref = O.pipeline(l, r, D)
-        same_maps(want, LR.post_process(l, r, ref["lDis"], ref["rDis"], 0, (4, 10.0, 2, "iv1")), "post vs oracle")
+        same_maps(want, PP.chain(l, r, ref["lDis"], ref["rDis"], setting=(4, 10.0, 2, "iv1"))[:2], "post vs oracle")
 
 
 @pytest.mark.parametrize("mode", [capi.PSM_LR_FILL_WMF, capi.PSM_LR_FILL])
@@ -170,9 +170,9 @@ def test_lr_check_and_valid_masks(mode, devices, scenes):
     got = run(l8, r8, 64, setup=setup, post=True, devices=devices)
     same_maps(got, want, f"lr {mode} on {devices}")
     ref = O.pipeline(l, r, 64)
-    lv, rv, _, _ = LR.lr_check_fill(ref["lDis"], ref["rDis"])
+    pl, pr, (lv, rv) = PP.chain(l, r, ref["lDis"], ref["rDis"], lr=mode)
     assert_same(got[2], lv, "left mask vs oracle"); assert_same(got[3], rv, "right mask vs oracle")
-    same_maps(got[:2], LR.post_process(l, r, ref["lDis"], ref["rDis"], mode), "post-processed vs oracle")
+    same_maps(got[:2], (pl, pr), "post-processed vs oracle")
 
 
 # ---- 4. frames in a row: host (float, u8) and device frames, no host wait between frames ------------------------------

@@ -14,6 +14,7 @@ import pytest
 
 import image_cases as IC
 import lr_oracle as LR
+import pp_chain as PP
 import range_cases as RC
 import selection_cases as S
 from oracle import oracle as O
@@ -227,7 +228,7 @@ def test_lr_check_and_post_filter(kw):
             ld, rd = de.lDisMap.copy(), de.rDisMap.copy()
             assert ((ld == 0) | (ld >= lo)).all() and (ld >= lo).mean() > 0.9
             assert de.PostProcess_GPU() == 0
-            want = LR.post_process(l, r, ld, rd, mode)
+            want = PP.chain(l, r, ld, rd, lr=mode)
             assert_bits(de.lDisMap, want[0], f"mode {mode} left")
             assert_bits(de.rDisMap, want[1], f"mode {mode} right")
             if mode:

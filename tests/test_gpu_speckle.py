@@ -15,9 +15,9 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN, ROOT
-from oracle import oracle as O
 from primestereomatch_b200 import DispEst, capi, synth
 import lr_oracle as LR
+import pp_chain as PP
 import speckle_oracle as SP
 
 pytestmark = pytest.mark.gpu
@@ -136,8 +136,7 @@ def test_full_scenes_against_the_golden(scene, scenes, oracle_scene_results):
         for lr in (1, 2, 0):
             de.setLRCheck(lr)
             gl, gr = speckle(de, FIRST, 400, 2)
-            want = SP.chain(l, r, ref["ld"], ref["rd"], (FIRST, 400, 2), lr, post_process=O.post_process,
-                            lr_check_fill=LR.lr_check_fill)
+            want = PP.chain(l, r, ref["ld"], ref["rd"], speckle=(FIRST, 400, 2), lr=lr)
             assert_same(gl, want[0], f"{scene} first + lr {lr} left"); assert_same(gr, want[1], f"{scene} first + lr {lr} right")
 
 
@@ -247,8 +246,7 @@ def test_every_mode_with_every_check_mode(bits):
                 for lr in (0, 1, 2):
                     de.setLRCheck(lr)
                     gl, gr = speckle(de, *sp)
-                    want = SP.chain(l, r, ld, rd, sp, lr, setting, post_process=O.post_process,
-                                    lr_check_fill=LR.lr_check_fill)
+                    want = PP.chain(l, r, ld, rd, speckle=sp, lr=lr, setting=setting)
                     what = f"u{bits} speckle {sp} lr {lr} {setting}"
                     assert_same(gl, want[0], what + " left"); assert_same(gr, want[1], what + " right")
                     if lr and sp[0] != ONLY:
@@ -286,8 +284,7 @@ def test_context_kinds(kind, kw):
             check_only(de, ld, rd, size, diff, kind)
         de.setLRCheck(0 if left_only else 1)
         gl, gr = speckle(de, FIRST, 20, 1)
-        want = SP.chain(l, r, ld, rd, (FIRST, 20, 1), 0 if left_only else 1, post_process=O.post_process,
-                        lr_check_fill=LR.lr_check_fill)
+        want = PP.chain(l, r, ld, rd, speckle=(FIRST, 20, 1), lr=0 if left_only else 1)
         assert_same(gl, want[0], f"{kind} first left")
         if not left_only:
             assert_same(gr, want[1], f"{kind} first right")
@@ -403,7 +400,7 @@ def test_cpp_demo_speckle_flag(tmp_path, scenes, oracle_scene_results):
     assert SP.sha(got()[0]) == g[(400, 2)]
     out = subprocess.run([exe, "--speckle", "1", "100", "1"] + tail + ["2"], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stderr
-    want = SP.chain(l, r, ref["ld"], ref["rd"], (FIRST, 100, 1), 2, lr_check_fill=LR.lr_check_fill)
+    want = PP.chain(l, r, ref["ld"], ref["rd"], speckle=(FIRST, 100, 1), lr=2)
     assert_same(got()[0], want[0], "demo first + fill left"); assert_same(got()[1], want[1], "demo first + fill right")
     bad = subprocess.run([exe, "--speckle", "1", "0", "1"] + tail, capture_output=True, text=True, timeout=300)
     assert bad.returncode == 1 and "speckle filter" in bad.stderr

@@ -11,6 +11,7 @@ import pytest
 from conftest import GOLDEN
 from oracle import oracle as O
 import lr_oracle as LR
+import pp_chain as PP
 
 with open(os.path.join(GOLDEN, "golden_lr.json")) as f:
     GOLD = json.load(f)
@@ -88,7 +89,8 @@ def test_process_dm_with_the_check_equals_the_reference(scenes, oracle_scene_res
         for scene in ("Cones", "Teddy"):
             l8, r8, _, _ = scenes[scene]
             ref = oracle_scene_results[scene]
-            gl, gr = LR.post_process(O.u8_to_f32(posterise(l8)), O.u8_to_f32(posterise(r8)), ref["ld"], ref["rd"], 1, setting)
+            gl, gr, _ = PP.chain(O.u8_to_f32(posterise(l8)), O.u8_to_f32(posterise(r8)), ref["ld"], ref["rd"], lr=1,
+                                  setting=setting)
             for v, g in (("l", gl), ("r", gr)):
                 e = ent["scenes"][scene][v]
                 assert sha(g) == e["sha"], (setting, scene, v)
@@ -154,8 +156,8 @@ def test_modes():
     img = O.u8_to_f32(l8)
     l, r = random_pair(30, 20, 16, 7)
     _, _, lf, rf = LR.lr_check_fill(l, r)
-    assert all(np.array_equal(a, b) for a, b in zip(LR.post_process(img, img, l, r, 0), (O.post_process(img, l), O.post_process(img, r))))
-    assert all(np.array_equal(a, b) for a, b in zip(LR.post_process(img, img, l, r, 2), (lf, rf)))
+    assert all(np.array_equal(a, b) for a, b in zip(PP.chain(img, img, l, r), (O.post_process(img, l), O.post_process(img, r))))
+    assert all(np.array_equal(a, b) for a, b in zip(PP.chain(img, img, l, r, lr=2), (lf, rf)))
     s = (4, 10.0, 2, "iv1")
     assert all(np.array_equal(a, b) for a, b in
-               zip(LR.post_process(img, img, l, r, 1, s), (O.post_process(img, lf, *s), O.post_process(img, rf, *s))))
+               zip(PP.chain(img, img, l, r, lr=1, setting=s), (O.post_process(img, lf, *s), O.post_process(img, rf, *s))))
