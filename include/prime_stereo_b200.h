@@ -51,6 +51,11 @@
  * Threading: one psm_ctx must not be used concurrently; it may be used from different
  * host threads over its life (every call binds its CUDA device first), matching how the
  * reference constructs DispEst on the HCI thread and runs stages on the worker thread.
+ * Distinct contexts may be used concurrently from different host threads, on one device or
+ * several: a kernel's dynamic shared-memory limit, which the CUDA runtime keeps once per
+ * process and device, is only ever raised, so no context's setting can make another's launch
+ * fail (DESIGN.md section 29).  psm_last_error(NULL) reports the calling thread's own last
+ * failed creation.
  *
  * Host synchronisation: the calls documented as asynchronous only enqueue work once their first use is behind them.
  * On first use, or on the first call after a setting change, these may wait for the device (allocations, cudaFree,

@@ -8,6 +8,8 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <map>
+#include <mutex>
 #include <new>
 #include <type_traits>
 
@@ -212,6 +214,28 @@ int fail(psm_ctx* c, int code, const char* fmt, ...)
         (c)->launches++;                                                                           \
         PSM_CUDA((c), cudaGetLastError());                                                         \
     } while (0)
+
+// Make `bytes` of dynamic shared memory launchable for `kern` on `device` (the current device).  The limit is one value per
+// kernel per device for the whole process, and setting it then launching is not atomic: a context that lowered it
+// between another thread's set and launch would make that launch fail.  So the limit only ever goes up: a size at or
+// below the one already set is a no-op, and the record moves only once the runtime has accepted the new size.
+cudaError_t raise_smem_limit(const void* kern, size_t bytes, int device)
+{
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> limit;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& have = limit[{device, kern}];
+    if (bytes <= have) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) have = bytes;
+    return e;
+}
+
+template <typename K>
+cudaError_t raise_smem_limit(K* kern, size_t bytes, int device)
+{
+    return raise_smem_limit(reinterpret_cast<const void*>(kern), bytes, device);
+}
 
 // cudaMalloc into p while it is null; p stays null unless the allocation succeeds
 template <typename T>
@@ -734,7 +758,10 @@ int ensure_fgf(psm_ctx* c, int s)
           t.i0 = i < 0 ? 0 : (i > g.h2 - 1 ? g.h2 - 1 : i);
           t.i1 = i + 1 < 0 ? 0 : (i + 1 > g.h2 - 1 ? g.h2 - 1 : i + 1);
           t.f = f; t.pad = 0.f; } }
-    cudaError_t e = cudaMemcpy(c->fgf_plan, hp, (size_t)(c->W + c->H) * sizeof(FgfTap), cudaMemcpyHostToDevice);
+    // on the context's stream: a cudaMemcpy from pageable memory may return before its DMA lands, and it is not ordered
+    // before the kernels of the context's non-blocking stream, which read the plan at once
+    cudaError_t e = cudaMemcpyAsync(c->fgf_plan, hp, (size_t)(c->W + c->H) * sizeof(FgfTap), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     delete[] hp;
     PSM_CUDA(c, e);
     c->fgf_s = s;
@@ -759,7 +786,7 @@ int fgf_views(psm_ctx* c, int s, bool guide, bool slices)
         dim3 blk(128);
         dim3 g3((g.w2 + kFgfTX - 1) / kFgfTX, (g.h2 + kFgfTY - 1) / kFgfTY, c->res.count);
         const size_t fsmem = fgf_smem_bytes(g.K);
-        PSM_CUDA(c, cudaFuncSetAttribute(fgf_lowres_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+        PSM_CUDA(c, raise_smem_limit(fgf_lowres_kernel, fsmem, c->device));
         fgf_lowres_kernel<<<g3, kFgfThreads, fsmem, c->stream>>>(c->vol[v], c->plane, g, c->fgf_lo[v], c->fgf_mean);
         PSM_LAUNCH_CHECK(c);
         dim3 g5((((c->W + 3) / 4) + 127) / 128, c->H, c->res.count);
@@ -915,7 +942,7 @@ int launch_cvf_stream(psm_ctx* c)
     if (smem > (size_t)smem_max)
         return fail(c, PSM_EINVAL, "streaming filter: %zu bytes of shared memory for %d threads exceed the %d a block may have",
                     smem, nthreads, smem_max);
-    PSM_CUDA(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PSM_CUDA(c, raise_smem_limit(kern, smem, c->device));
     P.guide_flags = c->guide_flags;
     P.one = 1.0f; P.mone = -1.0f;
     const unsigned grid = plan.grid;
@@ -947,7 +974,7 @@ int launch_cvf_window(psm_ctx* c)
     const size_t smem = win_smem_bytes(P.K, P.ring_stride);
     if (smem > (size_t)smem_max)
         return fail(c, PSM_EINVAL, "guided filter window %d: %zu bytes of shared memory exceed the %d a block may have", P.K, smem, smem_max);
-    PSM_CUDA(c, cudaFuncSetAttribute(cvf_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PSM_CUDA(c, raise_smem_limit(cvf_window_kernel, smem, c->device));
     cvf_window_kernel<<<(unsigned)(base * P.nseg), kWinThreads, smem, c->stream>>>(P);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
@@ -2777,7 +2804,7 @@ static int post_process_maps(psm_ctx* c)
     }
     if (p.wmf && !c->pp_lut_valid) {
         const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
-        PSM_CUDA(c, cudaFuncSetAttribute(generic, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PSM_CUDA(c, raise_smem_limit(generic, smem, c->device));
         uint32_t* host = new (std::nothrow) uint32_t[kPpMaxD2 + 1];
         if (!host) return fail(c, PSM_ENOMEM, "out of host memory");
         const int n = pp_weight_table(c->pp_sigma, c->pp_type, host);
