@@ -25,6 +25,9 @@
  *   psm_set_speckle_filter <-> cv::filterSpeckles, as the reference's StereoSGBM matcher configures it (speckleWindowSize,
  *                             speckleRange)                       src/StereoMatch.cpp:654-655
  *   psm_set_disparity_check <-> cv::validateDisparity, the same matcher's disp12MaxDiff = 1  src/StereoMatch.cpp:651
+ *   psm_set_uniqueness_check <-> StereoSGBM's uniqueness test, the same matcher's uniquenessRatio = 10
+ *                                                                 src/StereoMatch.cpp:653
+ *   psm_set_median_blur   <-> cv::medianBlur(disp, 3), which StereoSGBM::compute runs on every map it returns
  *   psm_reproject_device  <-> cv::reprojectImageTo3D with the rig's Q (camProps.Q, computed and never read there)
  *                                                                 src/StereoMatch.cpp:456-457
  *   psm_read_cost_slice   <-> DispEst::printCV (cost-slice dump) src/DispEst.cpp:181-194
@@ -64,7 +67,8 @@
  * psm_cost_filter_fgf (buffers and up-sampling plan, rebuilt for every new sub-sampling rate), psm_post_process_device
  * (its buffers and, after a change of sigma or weight type, the weight table; with psm_set_speckle_filter on, the
  * labels and counts, 8 * W * H bytes per view; with psm_set_disparity_check on rows over 6144 columns, its claim words;
- * with two or more of the check, removal and left-right steps, one map per computed view between them),
+ * with two or more of the uniqueness, check, median, removal and left-right steps, one map per computed view between
+ * them),
  * psm_set_option(PSM_OPT_COSTS, 1) (the
  * cost planes), psm_set_option(PSM_OPT_RUNNER_UP, 1) (the runner-up planes, lists and slots), psm_reproject_device with
  * handle_missing (8 bytes of scratch).  Run them once before a
@@ -130,10 +134,11 @@ enum { PSM_VIEWS_LEFT = 1, PSM_VIEWS_BOTH = 2 };
  *     psm_disp_reduce_keys* must be NULL: a non-NULL one returns PSM_EINVAL.  The fused exchange moves and reduces the
  *     left keys only; every rank must use the same setting.  Multi-device contexts forward the option to every shard.
  *   - psm_post_process* filters the left map only.  With a left-right check mode (psm_set_lr_check 1 or 2) it returns
- *     PSM_ESTATE: the check needs both maps; psm_set_disparity_check(PSM_DCHECK_FIRST) replaces it with the one-view
- *     check and fills the left map.  psm_set_lr_check itself may be called at any time.
+ *     PSM_ESTATE: the check needs both maps; psm_set_disparity_check(PSM_DCHECK_FIRST) or
+ *     psm_set_uniqueness_check(PSM_UNIQUE_FIRST) replaces it with the one-view tests and fills the left map.
+ *     psm_set_lr_check itself may be called at any time.
  *   - PSM_ESTATE: psm_read_cost_slice, psm_read_ab_slice and psm_read_guide_plane planes 3-11 of the right view, and
- *     psm_read_valid_mask (of the left view too, unless the last post-process filled with the one-view check).
+ *     psm_read_valid_mask (of the left view too, unless the last post-process filled after the one-view tests).
  *   - Nothing else is written: the right volume, the right map, the right post-filtered map and the right mask keep
  *     their contents.  psm_device_ptr returns the same addresses, and no device memory is freed or allocated.
  *     psm_stage_ms reports the left view's work, psm_launch_count the kernels that ran. */
@@ -353,10 +358,11 @@ enum { PSM_SPECKLE_OFF = 0, PSM_SPECKLE_FIRST = 1, PSM_SPECKLE_ONLY = 2 };
  * with speckleWindowSize and speckleRange) for every later psm_post_process / _u16 / _device of this context:
  *   PSM_SPECKLE_OFF (default): the stage exactly as psm_set_lr_check and psm_set_post_filter configure it, launch for
  *                     launch;
- *   PSM_SPECKLE_FIRST: speckle removal on the selection maps, then the configured check and / or post-filter on its
+ *   PSM_SPECKLE_FIRST: speckle removal on the selection maps (or on the result of the uniqueness test, disparity check
+ *                     and median before it, where those are on), then the configured check and / or post-filter on its
  *                     result (4 more launches);
- *   PSM_SPECKLE_ONLY: speckle removal alone; its maps are the result and neither the check nor the post-filter runs, so
- *                     psm_read_valid_mask returns PSM_ESTATE (4 launches).
+ *   PSM_SPECKLE_ONLY: the chain up to and including speckle removal; its maps are the result and neither the check nor
+ *                     the post-filter runs, so psm_read_valid_mask returns PSM_ESTATE (4 launches).
  * Definition, on each view's map on its own (u8, or u16 on a 16-bit context; cv::filterSpeckles on the map as CV_16S):
  * pixels of value 0 belong to no blob; two 4-neighbours p, q, both non-zero, are in the same blob when
  * |m(p) - m(q)| <= max_diff (in whole disparities, compared as int); blobs are the connected components of that graph;
@@ -379,10 +385,11 @@ enum { PSM_DCHECK_OFF = 0, PSM_DCHECK_FIRST = 1, PSM_DCHECK_ONLY = 2 };
  * matcher sets to 1) for every later psm_post_process / _u16 / _device of this context:
  *   PSM_DCHECK_OFF (default): the stage exactly as psm_set_speckle_filter, psm_set_lr_check and psm_set_post_filter
  *                     configure it, launch for launch;
- *   PSM_DCHECK_FIRST: the check on the selection maps, then the configured speckle removal, left-right check / fill and
- *                     post-filter on its result, in that order (one more launch);
- *   PSM_DCHECK_ONLY:  the check alone; its maps are the result, nothing else runs and psm_read_valid_mask returns
- *                     PSM_ESTATE (one launch).
+ *   PSM_DCHECK_FIRST: the check on the selection maps (or on the uniqueness test's result, where it is on), then the
+ *                     configured median, speckle removal, left-right check / fill and post-filter on its result, in
+ *                     that order (one more launch);
+ *   PSM_DCHECK_ONLY:  the chain up to and including the check; its maps are the result, nothing else runs and
+ *                     psm_read_valid_mask returns PSM_ESTATE (one launch).
  * Definition, per row of one view's selection map m (u8 or u16), c = plane 1 of PSM_OPT_COSTS (the winner's cost q(m))
  * of the same selection, W = width, D = max_disp:
  *   1. only columns x in [D, W) with m[x] != 0 take part; every other pixel keeps its value;
@@ -403,6 +410,57 @@ enum { PSM_DCHECK_OFF = 0, PSM_DCHECK_FIRST = 1, PSM_DCHECK_ONLY = 2 };
  * use.
  * See DESIGN.md section 26. */
 int psm_set_disparity_check(psm_ctx* ctx, int mode, int max_diff);
+
+/* The post-process chain.  psm_post_process* runs the steps that are on in StereoSGBM's order,
+ *   uniqueness test -> disparity check -> median -> speckle removal -> left-right check / fill -> post-filter,
+ * each on the previous step's result.  A step's _ONLY mode (and PSM_LR_FILL) ends the chain after it: its maps are the
+ * result.  With every step but the post-filter off, the stage is the post-filter alone.  Each of the first four adds one
+ * launch (speckle removal four) and writes nothing but the post-processed maps and the masks.  On a left-only context,
+ * PSM_UNIQUE_FIRST or PSM_DCHECK_FIRST with PSM_LR_FILL / PSM_LR_FILL_WMF fills the left map where the chain's map v is
+ * below 2 (valid[x] = v[x] >= 2), and psm_read_valid_mask of the left view returns that mask. */
+
+/* Uniqueness test modes of psm_set_uniqueness_check */
+enum { PSM_UNIQUE_OFF = 0, PSM_UNIQUE_FIRST = 1, PSM_UNIQUE_ONLY = 2 };
+
+/* Uniqueness test (OpenCV StereoSGBM's uniquenessRatio, which the reference's SGBM matcher sets to 10) for every later
+ * psm_post_process / _u16 / _device of this context:
+ *   PSM_UNIQUE_OFF (default): the stage exactly as the other steps configure it, launch for launch;
+ *   PSM_UNIQUE_FIRST: the test on the selection maps, then the rest of the chain on its result (one more launch);
+ *   PSM_UNIQUE_ONLY:  the test alone; its maps are the result and psm_read_valid_mask returns PSM_ESTATE (one launch).
+ * Definition, per pixel of one view's selection map m (u8 or u16), with q(m) = plane 1 of PSM_OPT_COSTS and q(r) =
+ * plane 1 of PSM_OPT_RUNNER_UP of the same selection: a pixel with m != 0 becomes 0 when
+ *   (double)q(r) * (100 - ratio) < (double)q(m) * 100;
+ * every other pixel keeps its value.  Both products are exact, so the comparison is the exact one on finite costs and
+ * IEEE's on the rest: where there is no runner-up (r = 0, q(r) NaN) the pixel is kept.  This is computeDisparitySGBM's
+ * `Sp[d]*(100 - uniquenessRatio) < minS*100 && abs(bestDisp - d) > 1` over the selection's candidates
+ * [max(1, min_disp), max_disp) on float costs: the runner-up is the lowest of them with |d - m| >= 2, and multiplying
+ * by a constant >= 0 keeps their order, so testing r alone tests them all.  Ratio 0 rejects nothing (q(r) >= q(m)).
+ * StereoBM's variant (`<=` on integer sums with an integer division) is not this test.  Rejected pixels are 0, so they
+ * claim no column in the disparity check that follows.  The stage reads the costs and the runner-up the last selection
+ * wrote: without both (PSM_OPT_COSTS or PSM_OPT_RUNNER_UP off for that selection) psm_post_process* returns PSM_ESTATE.
+ * Stage 5 of psm_stage_ms covers it.  Valid: one of the three modes and ratio in [0, 100]; anything else returns
+ * PSM_EINVAL and leaves the context unchanged, as does a mode other than PSM_UNIQUE_OFF on a context that owns part of
+ * the range (psm_create_sharded).  Multi-device contexts forward it to every shard; the stage runs on the first.
+ * See DESIGN.md section 30. */
+int psm_set_uniqueness_check(psm_ctx* ctx, int mode, int ratio);
+
+/* Median modes of psm_set_median_blur */
+enum { PSM_MEDIAN_OFF = 0, PSM_MEDIAN_FIRST = 1, PSM_MEDIAN_ONLY = 2 };
+
+/* ksize x ksize median (OpenCV's cv::medianBlur, which StereoSGBM::compute runs with ksize 3 between its winner-take-all
+ * and filterSpeckles) for every later psm_post_process / _u16 / _device of this context:
+ *   PSM_MEDIAN_OFF (default): the stage exactly as the other steps configure it, launch for launch;
+ *   PSM_MEDIAN_FIRST: the median after the uniqueness test and the disparity check, then speckle removal, the left-right
+ *                     check / fill and the post-filter on its result (one more launch);
+ *   PSM_MEDIAN_ONLY:  the chain up to and including the median; its maps are the result and psm_read_valid_mask
+ *                     returns PSM_ESTATE (one launch).
+ * Definition, per view: out(x, y) = the median of the ksize * ksize map values around (x, y), rows and columns clamped
+ * to the map (BORDER_REPLICATE): exactly cv::medianBlur(map, ksize) on the u8 map, or on the u16 map as CV_16U.  Zeros
+ * (invalid) take part as values, the lowest, as SGBM's invalid (minD - 1) * 16 does, so the result commutes with SGBM's
+ * fixed-point scaling.  Stage 5 of psm_stage_ms covers it.  Valid: one of the three modes and ksize 3 or 5; anything
+ * else returns PSM_EINVAL and leaves the context unchanged.  Multi-device contexts forward it to every shard; the stage
+ * runs on the first.  See DESIGN.md section 30. */
+int psm_set_median_blur(psm_ctx* ctx, int mode, int ksize);
 
 /* Use an existing CUDA stream (cudaStream_t passed as void*) for all work; NULL restores the
  * context's own stream.  Lets a caller time with its own events on that stream.  Waits for the work already enqueued

@@ -27,6 +27,7 @@ SYMBOLS = [
     "psm_create_range", "psm_set_speckle_filter", "psm_set_disparity_check", "psm_reproject_device", "psm_read_points", "psm_set_rectify",
     "psm_set_images_device_yuv", "psm_set_images_yuv", "psm_set_images_yuv_async",
     "psm_set_images_device_bayer", "psm_set_images_bayer", "psm_set_images_bayer_async",
+    "psm_set_uniqueness_check", "psm_set_median_blur",
 ]
 
 PSM_OK, PSM_EINVAL, PSM_ECUDA, PSM_ESTATE, PSM_ENOMEM = 0, 1, 2, 3, 4
@@ -41,6 +42,8 @@ PSM_WMF_EXP, PSM_WMF_IV1, PSM_WMF_IV2, PSM_WMF_OFF = 0, 1, 2, 5
 PSM_LR_OFF, PSM_LR_FILL_WMF, PSM_LR_FILL = 0, 1, 2
 PSM_SPECKLE_OFF, PSM_SPECKLE_FIRST, PSM_SPECKLE_ONLY = 0, 1, 2
 PSM_DCHECK_OFF, PSM_DCHECK_FIRST, PSM_DCHECK_ONLY = 0, 1, 2
+PSM_UNIQUE_OFF, PSM_UNIQUE_FIRST, PSM_UNIQUE_ONLY = 0, 1, 2
+PSM_MEDIAN_OFF, PSM_MEDIAN_FIRST, PSM_MEDIAN_ONLY = 0, 1, 2
 PSM_PIX_U8, PSM_PIX_F32 = 1, 2
 PSM_YUV_420, PSM_YUV_422 = 1, 2
 PSM_YUV_NV12, PSM_YUV_NV21, PSM_YUV_I420, PSM_YUV_YV12, PSM_YUV_YUYV, PSM_YUV_UYVY, PSM_YUV_YVYU = 1, 2, 3, 4, 5, 6, 7
@@ -95,6 +98,8 @@ def lib():
     L.psm_set_lr_check.argtypes = [vp, i]
     L.psm_set_speckle_filter.argtypes = [vp, i, i, i]
     L.psm_set_disparity_check.argtypes = [vp, i, i]
+    L.psm_set_uniqueness_check.argtypes = [vp, i, i]
+    L.psm_set_median_blur.argtypes = [vp, i, i]
     L.psm_set_rectify.argtypes = [vp, i, i, vp, sz, vp, sz, vp, sz, vp, sz]
     L.psm_read_valid_mask.argtypes = [vp, i, u8p, sz]
     L.psm_set_stream.argtypes = [vp, vp]

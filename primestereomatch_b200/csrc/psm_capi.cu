@@ -24,6 +24,8 @@
 #include "psm_lr.cuh"
 #include "psm_speckle.cuh"
 #include "psm_dcheck.cuh"
+#include "psm_unique.cuh"
+#include "psm_median.cuh"
 #include "psm_reproject.cuh"
 
 #ifndef PSM_BUILD_FLAGS
@@ -137,6 +139,10 @@ struct psm_ctx {
     int dc_mode = PSM_DCHECK_OFF;           // one-view disparity check in the post-process stage, psm_set_disparity_check
     int dc_max_diff = 1;
     unsigned long long* dc_claims[2] = {nullptr, nullptr};  // W > kDcStageCols: the claim words, W x H per computed view, lazy
+    int un_mode = PSM_UNIQUE_OFF;           // uniqueness test in the post-process stage, psm_set_uniqueness_check
+    int un_ratio = 10;
+    int md_mode = PSM_MEDIAN_OFF;           // median in the post-process stage, psm_set_median_blur
+    int md_ksize = 3;
     // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
     // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
     int blk_slices = 0;
@@ -1971,6 +1977,38 @@ int psm_set_disparity_check(psm_ctx* c, int mode, int max_diff)
     return PSM_OK;
 }
 
+int psm_set_uniqueness_check(psm_ctx* c, int mode, int ratio)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (mode != PSM_UNIQUE_OFF && mode != PSM_UNIQUE_FIRST && mode != PSM_UNIQUE_ONLY)
+        return fail(c, PSM_EINVAL, "uniqueness check mode %d is not off (0), first (1) or only (2)", mode);
+    if (ratio < 0 || ratio > 100) return fail(c, PSM_EINVAL, "uniqueness ratio %d outside 0..100", ratio);
+    // a multi-device context spans the range, and its first shard holds the complete maps, costs and runner-up
+    if (c->nshards) {
+        for (int k = 0; k < c->nshards; ++k) { c->shard[k]->un_mode = mode; c->shard[k]->un_ratio = ratio; }
+        return PSM_OK;
+    }
+    if (mode != PSM_UNIQUE_OFF && !c->owns_problem())
+        return fail(c, PSM_EINVAL, "psm_set_uniqueness_check on a context that owns slices [%d,%d) of %d: the test reads "
+                    "the winners' costs and the runner-up (PSM_OPT_COSTS, PSM_OPT_RUNNER_UP), which such a context cannot "
+                    "write; use a context over the whole range", c->d_begin, c->d_begin + c->d_count, c->D);
+    c->un_mode = mode;
+    c->un_ratio = ratio;
+    return PSM_OK;
+}
+
+int psm_set_median_blur(psm_ctx* c, int mode, int ksize)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_median_blur(s, mode, ksize); });
+    if (mode != PSM_MEDIAN_OFF && mode != PSM_MEDIAN_FIRST && mode != PSM_MEDIAN_ONLY)
+        return fail(c, PSM_EINVAL, "median blur mode %d is not off (0), first (1) or only (2)", mode);
+    if (ksize != 3 && ksize != 5) return fail(c, PSM_EINVAL, "median blur ksize %d is not 3 or 5", ksize);
+    c->md_mode = mode;
+    c->md_ksize = ksize;
+    return PSM_OK;
+}
+
 int psm_set_rectify(psm_ctx* c, int src_width, int src_height, const int16_t* xy_left, size_t xy_left_step,
                     const uint16_t* a_left, size_t a_left_step, const int16_t* xy_right, size_t xy_right_step,
                     const uint16_t* a_right, size_t a_right_step)
@@ -2724,6 +2762,36 @@ static int disparity_check(psm_ctx* c, const uint8_t* const in[2], uint8_t* cons
     return PSM_OK;
 }
 
+// the uniqueness test (psm_unique.cuh) of the maps in[view] into out[view], every computed view in one launch
+template <typename T>
+static int unique_check(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
+{
+    const size_t npix = (size_t)c->W * c->H;
+    const float* qm[2];
+    const float* qr[2];
+    for (int v = 0; v < 2; ++v) {
+        qm[v] = c->outs[kOutCosts].planes[v] ? c->outs[kOutCosts].planes[v] + npix : nullptr;
+        qr[v] = c->outs[kOutRunnerUp].planes[v] ? c->outs[kOutRunnerUp].planes[v] + npix : nullptr;
+    }
+    const UniqueArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])}, {qm[0], qm[1]},
+                             {qr[0], qr[1]}, {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, npix, c->un_ratio};
+    unique_kernel<T><<<dim3((unsigned)((npix + kUnThreads - 1) / kUnThreads), (unsigned)c->views), kUnThreads, 0, c->stream>>>(a);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
+// the ksize x ksize median (psm_median.cuh) of the maps in[view] into out[view], every computed view in one launch
+template <typename T>
+static int median_blur(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
+{
+    const MedianArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])},
+                             {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, c->W, c->H};
+    const dim3 grd((unsigned)(c->W + kMdTileX - 1) / kMdTileX, (unsigned)(c->H + kMdTileY - 1) / kMdTileY, c->views);
+    (c->md_ksize == 3 ? median_kernel<T, 1> : median_kernel<T, 2>)<<<grd, dim3(kMdTileX, kMdTileY), 0, c->stream>>>(a);
+    PSM_LAUNCH_CHECK(c);
+    return PSM_OK;
+}
+
 // lrCheck + fillInv (PP.cpp:405-406) of in[view] into out[view] and lr_valid; kOwn: the left view alone, its mask from the map itself
 template <typename T, bool kOwn>
 static int lr_check_fill(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
@@ -2737,23 +2805,28 @@ static int lr_check_fill(psm_ctx* c, const uint8_t* const in[2], uint8_t* const 
     return PSM_OK;
 }
 
-// psm_post_process's steps in front of the post-filter: the disparity check, speckle removal and the left-right check
-// and fill, each when on and in that order.  PSM_DCHECK_ONLY, PSM_SPECKLE_ONLY and PSM_LR_FILL end the chain after their
-// step, and then the post-filter (wmf) does not run.  With the check on, a left-only context fills from its result.
+// psm_post_process's steps in front of the post-filter: the uniqueness test, the disparity check, the median, speckle
+// removal and the left-right check and fill, each when on and in that order (StereoSGBM's).  PSM_UNIQUE_ONLY,
+// PSM_DCHECK_ONLY, PSM_MEDIAN_ONLY, PSM_SPECKLE_ONLY and PSM_LR_FILL end the chain after their step, and then the
+// post-filter (wmf) does not run.  With the uniqueness test or the check on, a left-only context fills from the result.
 template <typename T>
 struct PpChain {
     using Step = int (*)(psm_ctx*, const uint8_t* const*, uint8_t* const*);
-    Step step[3];
+    Step step[5];
     int n = 0;
     bool wmf = false;
     explicit PpChain(const psm_ctx* c)
     {
+        if (c->un_mode != PSM_UNIQUE_OFF) step[n++] = unique_check<T>;
+        if (c->un_mode == PSM_UNIQUE_ONLY) return;
         if (c->dc_mode != PSM_DCHECK_OFF) step[n++] = disparity_check<T>;
         if (c->dc_mode == PSM_DCHECK_ONLY) return;
+        if (c->md_mode != PSM_MEDIAN_OFF) step[n++] = median_blur<T>;
+        if (c->md_mode == PSM_MEDIAN_ONLY) return;
         if (c->sp_mode != PSM_SPECKLE_OFF) step[n++] = speckle_filter<T>;
         if (c->sp_mode == PSM_SPECKLE_ONLY) return;
-        if (c->lr_mode != PSM_LR_OFF)
-            step[n++] = c->views == 1 && has(disparity_check<T>) ? lr_check_fill<T, true> : lr_check_fill<T, false>;
+        const bool own = c->views == 1 && (has(unique_check<T>) || has(disparity_check<T>));
+        if (c->lr_mode != PSM_LR_OFF) step[n++] = own ? lr_check_fill<T, true> : lr_check_fill<T, false>;
         wmf = c->lr_mode != PSM_LR_FILL;
     }
     bool has(Step s) const { return std::find(step, step + n, s) != step + n; }
@@ -2774,6 +2847,10 @@ static int post_process_maps(psm_ctx* c)
     if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
     const PpChain<T> p(c);
+    if (p.has(unique_check<T>) && !(c->outs[kOutCosts].have && c->outs[kOutRunnerUp].have))
+        return fail(c, PSM_ESTATE, "psm_post_process: the uniqueness test (psm_set_uniqueness_check mode %d) reads the "
+                    "winners' costs and the runner-up, and the last selection stage did not write both: set PSM_OPT_COSTS = 1 "
+                    "and PSM_OPT_RUNNER_UP = 1 before it", c->un_mode);
     if (p.has(disparity_check<T>) && !c->outs[kOutCosts].have)
         return fail(c, PSM_ESTATE, "psm_post_process: the disparity check (psm_set_disparity_check mode %d) reads the "
                     "winners' costs, and the last selection stage did not write them: set PSM_OPT_COSTS = 1 before it",
@@ -3259,7 +3336,7 @@ int psm_read_valid_mask(psm_ctx* c, int view, uint8_t* dst, size_t dst_step)
     if (c->views == 1 && (view == PSM_RIGHT || !c->lr_masks_ok))
         return fail(c, PSM_ESTATE, "psm_read_valid_mask on a left-only context (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): the "
                     "left-right check needs both maps; set PSM_VIEWS_BOTH, or fill the left view after "
-                    "psm_set_disparity_check(PSM_DCHECK_FIRST)");
+                    "psm_set_disparity_check(PSM_DCHECK_FIRST) or psm_set_uniqueness_check(PSM_UNIQUE_FIRST)");
     if (!c->lr_masks_ok)
         return fail(c, PSM_ESTATE, "no valid mask: the last post-process since the last selection stage did not run the left-right check");
     PSM_CUDA(c, cudaMemcpy2DAsync(dst, dst_step, c->lr_valid[view], c->W, c->W, c->H, cudaMemcpyDeviceToHost, c->stream));

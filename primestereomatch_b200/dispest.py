@@ -173,6 +173,8 @@ class DispEst:
         self.lr_mode = capi.PSM_LR_OFF
         self.speckle_mode = capi.PSM_SPECKLE_OFF
         self.dcheck_mode = capi.PSM_DCHECK_OFF
+        self.unique_mode = capi.PSM_UNIQUE_OFF
+        self.median_mode = capi.PSM_MEDIAN_OFF
         self.cost_output = False
         self.lCosts = self.rCosts = None   # setCostOutput(True): DispSelect_GPU's (3, H, W) float32 costs
         self.runner_up_output = False
@@ -329,6 +331,31 @@ class DispEst:
         self.dcheck_mode = int(mode)
         return 0
 
+    def setUniquenessCheck(self, mode, ratio=10):
+        """Uniqueness test (OpenCV StereoSGBM's uniquenessRatio) for every later PostProcess_GPU call: 0 off (default),
+        1 first (then the rest of the chain -- setDisparityCheck, setMedianBlur, setSpeckleFilter, setLRCheck,
+        setPostFilter -- on its result), 2 only (its maps are the result; lValid / rValid are not read).  A pixel with
+        m != 0 becomes 0 (invalid) when its runner-up's cost q(r) (setRunnerUpOutput's plane 1) is within ratio percent
+        of its winner's cost q(m) (setCostOutput's centre plane): q(r) * (100 - ratio) < q(m) * 100, exactly.  Needs
+        setCostOutput(True) and setRunnerUpOutput(True) for the selection it tests.  On a left-only context, mode 1 with
+        setLRCheck 1 or 2 fills the left map where it is below 2 and fills lValid.  Raises PsmError on any other mode, on
+        ratio outside [0, 100], or on a context that owns part of the range with the test on."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_uniqueness_check(self._ctx, int(mode), int(ratio)), self._ctx)
+        self.unique_mode = int(mode)
+        return 0
+
+    def setMedianBlur(self, mode, ksize=3):
+        """ksize x ksize median (OpenCV's medianBlur, StereoSGBM's fixed medianBlur(disp, 3)) for every later
+        PostProcess_GPU call, after the uniqueness test and the disparity check: 0 off (default), 1 first (then
+        setSpeckleFilter's removal and the check and / or post-filter on its result), 2 only (the chain up to the median;
+        its maps are the result; lValid / rValid are not read).  Equals cv2.medianBlur(map, ksize) on the u8 or u16 map,
+        zeros included as values.  Raises PsmError on any other mode or on ksize other than 3 or 5."""
+        self._need_gpu()
+        capi.check(self._lib.psm_set_median_blur(self._ctx, int(mode), int(ksize)), self._ctx)
+        self.median_mode = int(mode)
+        return 0
+
     def setRectify(self, left_maps, right_maps, src_size):
         """Rectify every later frame on the device (psm_set_rectify): the reference's video-mode remap(frame, rec,
         map[0], map[1], INTER_LINEAR) and crop, bit for bit.  left_maps / right_maps: (xy, a) of each view as
@@ -468,13 +495,14 @@ class DispEst:
     def PostProcess_GPU(self):
         """DispEst.cpp:338-344 -> PP::processDM (PP.cpp:402-425): joint weighted-median filter of both maps (after the
         left-right check and fill, or instead of the filter, as setLRCheck selects); the reference runs it on the CPU even
-        in GPU mode, here it is a device stage.  The disparity check and then speckle removal run first, or alone, as
-        setDisparityCheck and setSpeckleFilter select.  Results replace lDisMap / rDisMap."""
+        in GPU mode, here it is a device stage.  The uniqueness test, the disparity check, the median and speckle
+        removal run first, in that order, or end the chain, as setUniquenessCheck, setDisparityCheck, setMedianBlur and
+        setSpeckleFilter select.  Results replace lDisMap / rDisMap."""
         self._need_gpu()
         pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
         capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
-        if self.lr_mode != capi.PSM_LR_OFF and self.speckle_mode != capi.PSM_SPECKLE_ONLY \
-                and self.dcheck_mode != capi.PSM_DCHECK_ONLY:   # the check ran (a left-only fill masks the left view)
+        ended = capi.PSM_SPECKLE_ONLY in (self.unique_mode, self.dcheck_mode, self.median_mode, self.speckle_mode)
+        if self.lr_mode != capi.PSM_LR_OFF and not ended:   # the check ran (a left-only fill masks the left view)
             masks = ((capi.PSM_LEFT, self.lValid),) + (((capi.PSM_RIGHT, self.rValid),) if self.rDisMap is not None else ())
             for view, mask in masks:
                 capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)

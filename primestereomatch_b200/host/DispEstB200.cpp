@@ -135,6 +135,22 @@ int DispEst::setDisparityCheck(int mode, int max_diff)
     return rc;
 }
 
+int DispEst::setUniquenessCheck(int mode, int ratio)
+{
+    if (!ctx) return -1;
+    const int rc = psm_set_uniqueness_check(ctx, mode, ratio);
+    if (rc == PSM_OK) unique_mode = mode;
+    return rc;
+}
+
+int DispEst::setMedianBlur(int mode, int ksize)
+{
+    if (!ctx) return -1;
+    const int rc = psm_set_median_blur(ctx, mode, ksize);
+    if (rc == PSM_OK) median_mode = mode;
+    return rc;
+}
+
 int DispEst::setViews(int v)
 {
     if (!ctx) return -1;
@@ -290,9 +306,10 @@ int DispEst::DispSelect_GPU()
 
 // reference src/DispEst.cpp:338-344 -> PP::processDM (src/PP.cpp:402-425): the joint weighted-median filter of
 // both maps, after the left-right check and fill that setLRCheck enables (PP.cpp:405-406, psm_lr.cuh) and the speckle
-// removal and disparity check that setSpeckleFilter and setDisparityCheck enable (psm_speckle.cuh, psm_dcheck.cuh).  The
-// reference runs it on the CPU even in GPU mode; here it is a device stage (psm_pp.cuh).  The masks exist only where the
-// check ran (not under PSM_SPECKLE_ONLY or PSM_DCHECK_ONLY), the right one only on a two-view context.
+// removal, disparity check, uniqueness test and median that setSpeckleFilter, setDisparityCheck, setUniquenessCheck and
+// setMedianBlur enable (psm_speckle.cuh, psm_dcheck.cuh, psm_unique.cuh, psm_median.cuh).  The reference runs it on the
+// CPU even in GPU mode; here it is a device stage (psm_pp.cuh).  The masks exist only where the check ran (not under
+// any of the steps' _ONLY modes), the right one only on a two-view context.
 int DispEst::PostProcess_GPU()
 {
     if (!ctx) return -1;
@@ -300,7 +317,9 @@ int DispEst::PostProcess_GPU()
     const int rc = lDisMap.type() == CV_16UC1
         ? psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step)
         : psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
-    if (rc || lr_mode == PSM_LR_OFF || speckle_mode == PSM_SPECKLE_ONLY || dcheck_mode == PSM_DCHECK_ONLY) return rc;
+    if (rc || lr_mode == PSM_LR_OFF || speckle_mode == PSM_SPECKLE_ONLY || dcheck_mode == PSM_DCHECK_ONLY ||
+        unique_mode == PSM_UNIQUE_ONLY || median_mode == PSM_MEDIAN_ONLY)
+        return rc;
     if (int e = psm_read_valid_mask(ctx, PSM_LEFT, lValid.ptr<uint8_t>(), lValid.step)) return e;
     return both ? psm_read_valid_mask(ctx, PSM_RIGHT, rValid.ptr<uint8_t>(), rValid.step) : 0;
 }

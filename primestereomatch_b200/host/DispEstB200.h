@@ -91,9 +91,9 @@ public:
                       // whose low byte is the reference's uchar map
     cv::Mat rDisMap;
     cv::Mat lValid;   // CV_8UC1 masks of the left-right check (reference DispEst.h:81-82), 0/1; PostProcess_GPU fills them
-    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF (and setSpeckleFilter not PSM_SPECKLE_ONLY,
-                      // setDisparityCheck not PSM_DCHECK_ONLY); lValid alone on a left-only context that fills after
-                      // setDisparityCheck(PSM_DCHECK_FIRST)
+    cv::Mat rValid;   // when setLRCheck selected a mode other than PSM_LR_OFF (and no step of the chain an _ONLY mode);
+                      // lValid alone on a left-only context that fills after setDisparityCheck(PSM_DCHECK_FIRST) or
+                      // setUniquenessCheck(PSM_UNIQUE_FIRST)
     cv::Mat lCosts[3];  // setCostOutput(true): CV_32FC1 filtered costs at disparity m - 1, m, m + 1 of the selection map's
     cv::Mat rCosts[3];  // m (psm_read_costs); DispSelect_GPU fills them, rCosts not on a left-only context
     cv::Mat lRunnerUp[2];  // setRunnerUpOutput(true): CV_32FC1 runner-up disparity r (0 where none exists) and its
@@ -132,6 +132,15 @@ public:
     // psm_set_disparity_check.  It reads the winners' costs: call setCostOutput(true) before DispSelect_GPU.  A port of a
     // StereoSGBM pipeline calls setDisparityCheck(PSM_DCHECK_FIRST, disp12MaxDiff).
     int setDisparityCheck(int mode, int max_diff);
+    // Uniqueness test (StereoSGBM's uniquenessRatio) at the head of (PSM_UNIQUE_FIRST) or instead of (PSM_UNIQUE_ONLY)
+    // the rest of the post-process chain for every later PostProcess call; see psm_set_uniqueness_check.  It reads the
+    // winners' costs and the runner-up: call setCostOutput(true) and setRunnerUpOutput(true) before DispSelect_GPU.  A
+    // port of a StereoSGBM pipeline calls setUniquenessCheck(PSM_UNIQUE_FIRST, uniquenessRatio).
+    int setUniquenessCheck(int mode, int ratio);
+    // ksize x ksize median (cv::medianBlur; StereoSGBM::compute's fixed medianBlur(disp, 3)) after the uniqueness test and
+    // disparity check, in front of (PSM_MEDIAN_FIRST) or instead of (PSM_MEDIAN_ONLY) the speckle removal, check and
+    // post-filter for every later PostProcess call; see psm_set_median_blur.
+    int setMedianBlur(int mode, int ksize);
     // PSM_VIEWS_BOTH (default) or PSM_VIEWS_LEFT (PSM_OPT_VIEWS): with PSM_VIEWS_LEFT the later frames compute the left
     // map alone; DispSelect_GPU and PostProcess_GPU then leave rDisMap (and rValid) untouched.  The next stage after a
     // change must be CostConst_GPU.
@@ -188,6 +197,8 @@ private:
     int lr_mode = PSM_LR_OFF;
     int speckle_mode = PSM_SPECKLE_OFF;
     int dcheck_mode = PSM_DCHECK_OFF;
+    int unique_mode = PSM_UNIQUE_OFF;
+    int median_mode = PSM_MEDIAN_OFF;
     int views = PSM_VIEWS_BOTH;
     int src_w = 0, src_h = 0;   // setRectify: the size of the frames CostConst_GPU takes, 0 = the context's
     int yuv_format = 0;         // setInputImagesYUV: the PSM_YUV_* format of lImg / rImg, 0 = BGR frames

@@ -13,7 +13,9 @@
 // `--min-disp N` a context over disparities [N, D) alone (psm_create_range; the maps hold absolute disparities), a
 // leading `--speckle MODE SIZE DIFF` speckle removal (setSpeckleFilter: MODE 0 off, 1 first, 2 only), a leading
 // `--disp-check MODE MAXDIFF` the one-view disparity check (setDisparityCheck: MODE 0 off, 1 first, 2 only; it turns
-// setCostOutput on, which the check reads), a leading
+// setCostOutput on, which the check reads), a leading `--uniqueness MODE RATIO` the uniqueness test
+// (setUniquenessCheck: MODE 0 off, 1 first, 2 only; it turns setCostOutput and setRunnerUpOutput on, which the test
+// reads), a leading `--median MODE KSIZE` the median (setMedianBlur: MODE 0 off, 1 first, 2 only; KSIZE 3 or 5), a leading
 // `--points Q.f64 out.xyz` the left view's 3D points of the final maps (reprojectImageTo3D with the 16 native-endian
 // doubles of Q.f64, row-major): out.xyz holds H x W x 3 native float32 X, Y, Z.  A leading
 // `--left-only` computes the left map alone (setViews(PSM_VIEWS_LEFT)) and writes no right map: outR is not created.  A
@@ -46,6 +48,8 @@ int main(int argc, char** argv)
     int block_slices = 0, min_disp = 0;
     int speckle[3] = {0, 0, 0};   // mode, max_size, max_diff
     int dcheck[2] = {0, 1};       // mode, max_diff
+    int unique[2] = {0, 10};      // mode, ratio
+    int median[2] = {0, 3};       // mode, ksize
     const char* points[2] = {nullptr, nullptr};   // Q file, output file
     int src_size[2] = {0, 0};                     // --rectify: SW, SH
     const char* map_files[2] = {nullptr, nullptr};
@@ -60,7 +64,8 @@ int main(int argc, char** argv)
     }
     while (argc >= 3 && (!std::strcmp(argv[1], "--block-slices") || !std::strcmp(argv[1], "--devices") ||
                          !std::strcmp(argv[1], "--min-disp") || !std::strcmp(argv[1], "--speckle") ||
-                         !std::strcmp(argv[1], "--disp-check") ||
+                         !std::strcmp(argv[1], "--disp-check") || !std::strcmp(argv[1], "--uniqueness") ||
+                         !std::strcmp(argv[1], "--median") ||
                          !std::strcmp(argv[1], "--points") || !std::strcmp(argv[1], "--rectify") ||
                          !std::strcmp(argv[1], "--yuv") || !std::strcmp(argv[1], "--bayer") ||
                          !std::strcmp(argv[1], "--ea"))) {
@@ -111,10 +116,12 @@ int main(int argc, char** argv)
             argc -= 3;
             continue;
         }
-        if (!std::strcmp(argv[1], "--disp-check")) {
+        if (!std::strcmp(argv[1], "--disp-check") || !std::strcmp(argv[1], "--uniqueness") ||
+            !std::strcmp(argv[1], "--median")) {
             if (argc < 4) break;
-            dcheck[0] = std::atoi(argv[2]);
-            dcheck[1] = std::atoi(argv[3]);
+            int* const dst = argv[1][2] == 'd' ? dcheck : argv[1][2] == 'u' ? unique : median;
+            dst[0] = std::atoi(argv[2]);
+            dst[1] = std::atoi(argv[3]);
             argv[3] = argv[0];
             argv += 3;
             argc -= 3;
@@ -145,7 +152,7 @@ int main(int argc, char** argv)
         argc -= 2;
     }
     if (argc != 8 && argc != 10 && argc != 13 && argc != 17 && argc != 18) {
-        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--disp-check MODE MAXDIFF] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] [--yuv FORMAT | --bayer PATTERN [--ea]] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
+        std::fprintf(stderr, "usage: %s [--left-only] [--block-slices N] [--devices i,j,...] [--min-disp N] [--speckle MODE SIZE DIFF] [--disp-check MODE MAXDIFF] [--uniqueness MODE RATIO] [--median MODE KSIZE] [--points Q.f64 out.xyz] [--rectify SW SH left.map right.map] [--yuv FORMAT | --bayer PATTERN [--ea]] W H D left.f32 right.f32 outL.u8 outR.u8 [window eps [alpha tau_color tau_grad"
                              " [radius sigma iterations exp|iv1|iv2|off [lr_mode]]]]\n", argv[0]);
         return 2;
     }
@@ -199,7 +206,10 @@ int main(int argc, char** argv)
     if (!rc && argc == 18) rc = SMDE->setLRCheck(std::atoi(argv[17]));
     if (!rc && speckle[0]) rc = SMDE->setSpeckleFilter(speckle[0], speckle[1], speckle[2]);
     if (!rc && dcheck[0]) rc = SMDE->setDisparityCheck(dcheck[0], dcheck[1]);
-    if (!rc && dcheck[0]) rc = SMDE->setCostOutput(true);
+    if (!rc && unique[0]) rc = SMDE->setUniquenessCheck(unique[0], unique[1]);
+    if (!rc && median[0]) rc = SMDE->setMedianBlur(median[0], median[1]);
+    if (!rc && (dcheck[0] || unique[0])) rc = SMDE->setCostOutput(true);
+    if (!rc && unique[0]) rc = SMDE->setRunnerUpOutput(true);
     if (!rc) rc = SMDE->CostConst_GPU();
     if (!rc) rc = SMDE->CostFilter_GPU();
     if (!rc) rc = SMDE->DispSelect_GPU();

@@ -171,6 +171,7 @@ class TorchStereo:
         self.costs = False   # PSM_OPT_COSTS as match() last set it
         self.runner_up = False   # PSM_OPT_RUNNER_UP as match() last set it
         self.dcheck = capi.PSM_DCHECK_OFF   # setDisparityCheck's mode
+        self.unique = capi.PSM_UNIQUE_OFF   # setUniquenessCheck's mode
         self._lib = capi.lib()
         self._ctx = C.c_void_p()
         self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
@@ -223,6 +224,16 @@ class TorchStereo:
         the winners' costs; it returns them only with costs=True."""
         self._check(self._lib.psm_set_disparity_check(self._ctx, int(mode), int(max_diff)))
         self.dcheck = int(mode)
+
+    def setUniquenessCheck(self, mode, ratio=10):
+        """DispEst.setUniquenessCheck.  match(post_process=True) then turns PSM_OPT_COSTS and PSM_OPT_RUNNER_UP on
+        itself, since the test reads both; it returns them only with costs=True / runner_up=True."""
+        self._check(self._lib.psm_set_uniqueness_check(self._ctx, int(mode), int(ratio)))
+        self.unique = int(mode)
+
+    def setMedianBlur(self, mode, ksize=3):
+        """DispEst.setMedianBlur."""
+        self._check(self._lib.psm_set_median_blur(self._ctx, int(mode), int(ksize)))
 
     def setRectify(self, left_maps, right_maps, src_size):
         """DispEst.setRectify: from then on match takes uint8 camera frames of (SH, SW) in any layout frame_layout reads
@@ -295,12 +306,13 @@ class TorchStereo:
         (PSM_OPT_COSTS, psm_copy_costs_device), new float32 tensors (3, H, W) or (B, 3, H, W) whose plane k holds the cost
         at disparity m + k - 1, bit for bit (the quiet NaN 0x7FC00000 outside [min_disp, max_disp)); rcosts is None on a
         left-only context.  The option is set when it differs from the last call's, which restarts the frame; with
-        setDisparityCheck on and post_process=True it is on whatever costs says.
+        setDisparityCheck or setUniquenessCheck on and post_process=True it is on whatever costs says.
 
         runner_up=True -> also (lrunner, rrunner), appended after any costs: each pixel's runner-up away from the winner
         (PSM_OPT_RUNNER_UP, psm_copy_runner_up_device), new float32 tensors (2, H, W) or (B, 2, H, W): plane 0 the
         disparity r (0 where none exists), plane 1 its filtered cost bit for bit (the quiet NaN 0x7FC00000 where r = 0);
-        rrunner is None on a left-only context.  The option is set when runner_up differs from the last call's.
+        rrunner is None on a left-only context.  The option is set when it differs from the last call's; with
+        setUniquenessCheck on and post_process=True it is on whatever runner_up says.
 
         points=(Q_left, Q_right) -> also (lpts, rpts), appended last: OpenCV's reprojectImageTo3D of the maps this call
         returns (post-processed or selection) with each view's 4 x 4 reprojection matrix (psm_reproject_device), new
@@ -309,7 +321,8 @@ class TorchStereo:
 
         After psm_wait_stream on torch's current stream: psm_set_images_device_planes (or _device_yuv, _device_bayer), psm_cost_const, the guided filter
         (the Fast Guided Filter at setSubsampleRate's rate with fgf=True), psm_disp_select_device, psm_post_process_device
-        with post_process=True (the chain setDisparityCheck, setSpeckleFilter, setLRCheck and setPostFilter configure),
+        with post_process=True (the chain setUniquenessCheck, setDisparityCheck, setMedianBlur, setSpeckleFilter,
+        setLRCheck and setPostFilter configure),
         psm_copy_maps_device and, with points, psm_reproject_device of each frame of a batch in turn; then
         psm_signal_stream.  No host synchronisation: the inputs may be overwritten or freed, and the maps read, on that stream at once."""
         wanted = (costs, runner_up)
@@ -339,8 +352,9 @@ class TorchStereo:
         row = W * lmap.element_size()
         outs = []   # (copy-out call, left planes, right planes) of each output asked for
         for (name, key, n, copy), on in zip(_OUTPUTS, wanted):
-            # the disparity check of the post-process reads the costs
-            option = on or (key == capi.PSM_OPT_COSTS and post_process and self.dcheck != capi.PSM_DCHECK_OFF)
+            # the disparity check of the post-process reads the costs, the uniqueness test the costs and the runner-up
+            needed = self.unique != capi.PSM_UNIQUE_OFF or (key == capi.PSM_OPT_COSTS and self.dcheck != capi.PSM_DCHECK_OFF)
+            option = on or (post_process and needed)
             if option != getattr(self, name):
                 self._check(L.psm_set_option(ctx, key, int(option)))
                 setattr(self, name, option)
