@@ -54,6 +54,15 @@ constexpr SelOutInfo kSelOut[kNumOuts] = {
     {PSM_OPT_RUNNER_UP, "PSM_OPT_RUNNER_UP", "runner-up", kRunnerUpOut},
 };
 
+// The post-process steps in front of the post-filter, in chain order (StereoSGBM's); kPpStep holds what each one is.
+// Every step's modes are 0 (off), 1 and kPpEnd, which ends the chain after the step.
+enum PpStepId { kPpUnique, kPpDcheck, kPpMedian, kPpSpeckle, kPpLr, kNumPpSteps };
+constexpr int kPpEnd = 2;
+static_assert(PSM_UNIQUE_OFF == 0 && PSM_DCHECK_OFF == 0 && PSM_MEDIAN_OFF == 0 && PSM_SPECKLE_OFF == 0 && PSM_LR_OFF == 0,
+              "mode 0 turns a post-process step off");
+static_assert(PSM_UNIQUE_ONLY == kPpEnd && PSM_DCHECK_ONLY == kPpEnd && PSM_MEDIAN_ONLY == kPpEnd &&
+              PSM_SPECKLE_ONLY == kPpEnd && PSM_LR_FILL == kPpEnd, "mode 2 ends the post-process chain");
+
 }  // namespace
 
 struct psm_ctx {
@@ -129,20 +138,14 @@ struct psm_ctx {
     float pp_sigma = 25.5f;
     int pp_iter = 1, pp_type = PSM_WMF_EXP;
     bool pp_tuned() const { return pp_radius == kPpRadius && pp_sigma == 25.5f && pp_type == PSM_WMF_EXP; }   // any pp_iter
-    int lr_mode = PSM_LR_OFF;               // left-right check and fill in front of the post-filter, psm_set_lr_check
-    uint8_t* lr_valid[2] = {nullptr, nullptr};  // the check's masks (W x H, 0/1), lazy
+    // the post-process steps' settings by PpStepId: the mode and the arguments of the step's psm_set_* call (uniqueness
+    // ratio 10, disparity check max_diff 1, median ksize 3, speckle max_size and max_diff 0)
+    struct PpSetting { int mode, a, b; } pp_steps[kNumPpSteps] = {{0, 10, 0}, {0, 1, 0}, {0, 3, 0}, {0, 0, 0}, {0, 0, 0}};
+    uint8_t* lr_valid[2] = {nullptr, nullptr};  // the left-right check's masks (W x H, 0/1), lazy
     bool lr_masks_ok = false;               // lr_valid holds the masks of the current maps (psm_read_valid_mask)
-    int sp_mode = PSM_SPECKLE_OFF;          // speckle removal in the post-process stage, psm_set_speckle_filter
-    int sp_max_size = 0, sp_max_diff = 0;
     int* sp_lab = nullptr;                  // speckle removal's labels and counts: 2 x W x H each (view v at v * W * H), lazy
     int* sp_cnt = nullptr;
-    int dc_mode = PSM_DCHECK_OFF;           // one-view disparity check in the post-process stage, psm_set_disparity_check
-    int dc_max_diff = 1;
     unsigned long long* dc_claims[2] = {nullptr, nullptr};  // W > kDcStageCols: the claim words, W x H per computed view, lazy
-    int un_mode = PSM_UNIQUE_OFF;           // uniqueness test in the post-process stage, psm_set_uniqueness_check
-    int un_ratio = 10;
-    int md_mode = PSM_MEDIAN_OFF;           // median in the post-process stage, psm_set_median_blur
-    int md_ksize = 3;
     // psm_create_blocked: the volumes hold blk_slices slices; the filter stages walk [d_begin, d_begin + d_count) in
     // blocks of that many and fold each into the running keys.  0 = unblocked (the volumes hold every owned slice).
     int blk_slices = 0;
@@ -1932,83 +1935,6 @@ int psm_set_post_filter(psm_ctx* c, int radius, float sigma, int iterations, int
     return PSM_OK;
 }
 
-int psm_set_lr_check(psm_ctx* c, int mode)
-{
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_lr_check(s, mode); });
-    if (mode != PSM_LR_OFF && mode != PSM_LR_FILL_WMF && mode != PSM_LR_FILL)
-        return fail(c, PSM_EINVAL, "left-right check mode %d is not off (0), fill + post-filter (1) or fill (2)", mode);
-    c->lr_mode = mode;
-    return PSM_OK;
-}
-
-int psm_set_speckle_filter(psm_ctx* c, int mode, int max_size, int max_diff)
-{
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_speckle_filter(s, mode, max_size, max_diff); });
-    if (mode != PSM_SPECKLE_OFF && mode != PSM_SPECKLE_FIRST && mode != PSM_SPECKLE_ONLY)
-        return fail(c, PSM_EINVAL, "speckle filter mode %d is not off (0), first (1) or only (2)", mode);
-    if (mode != PSM_SPECKLE_OFF && (max_size < 1 || max_diff < 0))
-        return fail(c, PSM_EINVAL, "speckle filter max_size %d / max_diff %d: need max_size >= 1 and max_diff >= 0",
-                    max_size, max_diff);
-    c->sp_mode = mode;
-    c->sp_max_size = max_size;
-    c->sp_max_diff = max_diff;
-    return PSM_OK;
-}
-
-int psm_set_disparity_check(psm_ctx* c, int mode, int max_diff)
-{
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (mode != PSM_DCHECK_OFF && mode != PSM_DCHECK_FIRST && mode != PSM_DCHECK_ONLY)
-        return fail(c, PSM_EINVAL, "disparity check mode %d is not off (0), first (1) or only (2)", mode);
-    if (max_diff < 0 || max_diff > 4095) return fail(c, PSM_EINVAL, "disparity check max_diff %d outside 0..4095", max_diff);
-    // a multi-device context spans the range, and its first shard holds the complete maps and the cost planes
-    if (c->nshards) {
-        for (int k = 0; k < c->nshards; ++k) { c->shard[k]->dc_mode = mode; c->shard[k]->dc_max_diff = max_diff; }
-        return PSM_OK;
-    }
-    if (mode != PSM_DCHECK_OFF && !c->owns_problem())
-        return fail(c, PSM_EINVAL, "psm_set_disparity_check on a context that owns slices [%d,%d) of %d: the check reads "
-                    "the winners' costs (PSM_OPT_COSTS), which such a context cannot write; use a context over the whole "
-                    "range", c->d_begin, c->d_begin + c->d_count, c->D);
-    c->dc_mode = mode;
-    c->dc_max_diff = max_diff;
-    return PSM_OK;
-}
-
-int psm_set_uniqueness_check(psm_ctx* c, int mode, int ratio)
-{
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (mode != PSM_UNIQUE_OFF && mode != PSM_UNIQUE_FIRST && mode != PSM_UNIQUE_ONLY)
-        return fail(c, PSM_EINVAL, "uniqueness check mode %d is not off (0), first (1) or only (2)", mode);
-    if (ratio < 0 || ratio > 100) return fail(c, PSM_EINVAL, "uniqueness ratio %d outside 0..100", ratio);
-    // a multi-device context spans the range, and its first shard holds the complete maps, costs and runner-up
-    if (c->nshards) {
-        for (int k = 0; k < c->nshards; ++k) { c->shard[k]->un_mode = mode; c->shard[k]->un_ratio = ratio; }
-        return PSM_OK;
-    }
-    if (mode != PSM_UNIQUE_OFF && !c->owns_problem())
-        return fail(c, PSM_EINVAL, "psm_set_uniqueness_check on a context that owns slices [%d,%d) of %d: the test reads "
-                    "the winners' costs and the runner-up (PSM_OPT_COSTS, PSM_OPT_RUNNER_UP), which such a context cannot "
-                    "write; use a context over the whole range", c->d_begin, c->d_begin + c->d_count, c->D);
-    c->un_mode = mode;
-    c->un_ratio = ratio;
-    return PSM_OK;
-}
-
-int psm_set_median_blur(psm_ctx* c, int mode, int ksize)
-{
-    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
-    if (c->nshards) return forward(c, [&](psm_ctx* s) { return psm_set_median_blur(s, mode, ksize); });
-    if (mode != PSM_MEDIAN_OFF && mode != PSM_MEDIAN_FIRST && mode != PSM_MEDIAN_ONLY)
-        return fail(c, PSM_EINVAL, "median blur mode %d is not off (0), first (1) or only (2)", mode);
-    if (ksize != 3 && ksize != 5) return fail(c, PSM_EINVAL, "median blur ksize %d is not 3 or 5", ksize);
-    c->md_mode = mode;
-    c->md_ksize = ksize;
-    return PSM_OK;
-}
-
 int psm_set_rectify(psm_ctx* c, int src_width, int src_height, const int16_t* xy_left, size_t xy_left_step,
                     const uint16_t* a_left, size_t a_left_step, const int16_t* xy_right, size_t xy_right_step,
                     const uint16_t* a_right, size_t a_right_step)
@@ -2728,8 +2654,9 @@ static int pp_weight_table(float sigma, int type, uint32_t* t)
 template <typename T>
 static int speckle_filter(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
 {
+    const int max_size = c->pp_steps[kPpSpeckle].a, max_diff = c->pp_steps[kPpSpeckle].b;
     const SpeckleArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])}, c->sp_lab, c->sp_cnt,
-                              c->W, c->H, c->sp_max_diff};
+                              c->W, c->H, max_diff};
     const unsigned ntx = (unsigned)(c->W + kSpTile - 1) / kSpTile, nty = (unsigned)(c->H + kSpTile - 1) / kSpTile;
     const dim3 blk(kSpTile, kSpRows);
     speckle_local_kernel<T><<<dim3(ntx, nty, c->views), blk, 0, c->stream>>>(a);
@@ -2741,7 +2668,7 @@ static int speckle_filter(psm_ctx* c, const uint8_t* const in[2], uint8_t* const
     const dim3 grd(ntx, (unsigned)(c->H + kSpRows - 1) / kSpRows, c->views);
     speckle_count_kernel<T><<<grd, blk, 0, c->stream>>>(a);
     PSM_LAUNCH_CHECK(c);
-    speckle_paint_kernel<T><<<grd, blk, 0, c->stream>>>(a, c->sp_max_size, reinterpret_cast<T*>(out[0]),
+    speckle_paint_kernel<T><<<grd, blk, 0, c->stream>>>(a, max_size, reinterpret_cast<T*>(out[0]),
                                                          reinterpret_cast<T*>(out[1]));
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
@@ -2755,7 +2682,7 @@ static int disparity_check(psm_ctx* c, const uint8_t* const in[2], uint8_t* cons
     for (int v = 0; v < 2; ++v) q[v] = c->outs[kOutCosts].planes[v] ? c->outs[kOutCosts].planes[v] + (size_t)c->W * c->H : nullptr;
     const DcheckArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])}, {q[0], q[1]},
                              {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, {c->dc_claims[0], c->dc_claims[1]}, c->W, c->H, c->D,
-                             c->dc_max_diff};
+                             c->pp_steps[kPpDcheck].a};
     const size_t smem = c->W <= kDcStageCols ? (size_t)c->W * sizeof(unsigned long long) : 0;
     dcheck_kernel<T><<<dim3((unsigned)c->H, (unsigned)c->views), kDcThreads, smem, c->stream>>>(a);
     PSM_LAUNCH_CHECK(c);
@@ -2774,7 +2701,8 @@ static int unique_check(psm_ctx* c, const uint8_t* const in[2], uint8_t* const o
         qr[v] = c->outs[kOutRunnerUp].planes[v] ? c->outs[kOutRunnerUp].planes[v] + npix : nullptr;
     }
     const UniqueArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])}, {qm[0], qm[1]},
-                             {qr[0], qr[1]}, {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, npix, c->un_ratio};
+                             {qr[0], qr[1]}, {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, npix,
+                             c->pp_steps[kPpUnique].a};
     unique_kernel<T><<<dim3((unsigned)((npix + kUnThreads - 1) / kUnThreads), (unsigned)c->views), kUnThreads, 0, c->stream>>>(a);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
@@ -2787,49 +2715,108 @@ static int median_blur(psm_ctx* c, const uint8_t* const in[2], uint8_t* const ou
     const MedianArgs<T> a = {{reinterpret_cast<const T*>(in[0]), reinterpret_cast<const T*>(in[1])},
                              {reinterpret_cast<T*>(out[0]), reinterpret_cast<T*>(out[1])}, c->W, c->H};
     const dim3 grd((unsigned)(c->W + kMdTileX - 1) / kMdTileX, (unsigned)(c->H + kMdTileY - 1) / kMdTileY, c->views);
-    (c->md_ksize == 3 ? median_kernel<T, 1> : median_kernel<T, 2>)<<<grd, dim3(kMdTileX, kMdTileY), 0, c->stream>>>(a);
+    (c->pp_steps[kPpMedian].a == 3 ? median_kernel<T, 1> : median_kernel<T, 2>)<<<grd, dim3(kMdTileX, kMdTileY), 0, c->stream>>>(a);
     PSM_LAUNCH_CHECK(c);
     return PSM_OK;
 }
 
-// lrCheck + fillInv (PP.cpp:405-406) of in[view] into out[view] and lr_valid; kOwn: the left view alone, its mask from the map itself
-template <typename T, bool kOwn>
+// lrCheck + fillInv (PP.cpp:405-406) of in[view] into out[view] and lr_valid; on a left-only context the left view
+// alone, its mask from the map itself (post_process_maps runs the step there only after a step that reads selection
+// outputs)
+template <typename T>
 static int lr_check_fill(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2])
 {
+    const bool own = c->views == 1;
     const size_t smem = c->W <= kLrStageCols ? (size_t)c->W * (2 * sizeof(T) + 2) : 0;
-    lr_check_fill_kernel<T, kOwn><<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
-        reinterpret_cast<const T*>(in[0]), kOwn ? nullptr : reinterpret_cast<const T*>(in[1]), c->W,
-        reinterpret_cast<T*>(out[0]), kOwn ? nullptr : reinterpret_cast<T*>(out[1]), c->lr_valid[0], kOwn ? nullptr : c->lr_valid[1]);
+    (own ? lr_check_fill_kernel<T, true> : lr_check_fill_kernel<T, false>)<<<(unsigned)c->H, kLrThreads, smem, c->stream>>>(
+        reinterpret_cast<const T*>(in[0]), own ? nullptr : reinterpret_cast<const T*>(in[1]), c->W,
+        reinterpret_cast<T*>(out[0]), own ? nullptr : reinterpret_cast<T*>(out[1]), c->lr_valid[0], own ? nullptr : c->lr_valid[1]);
     PSM_LAUNCH_CHECK(c);
     c->lr_masks_ok = true;
     return PSM_OK;
 }
 
-// psm_post_process's steps in front of the post-filter: the uniqueness test, the disparity check, the median, speckle
-// removal and the left-right check and fill, each when on and in that order (StereoSGBM's).  PSM_UNIQUE_ONLY,
-// PSM_DCHECK_ONLY, PSM_MEDIAN_ONLY, PSM_SPECKLE_ONLY and PSM_LR_FILL end the chain after their step, and then the
-// post-filter (wmf) does not run.  With the uniqueness test or the check on, a left-only context fills from the result.
+// What each post-process step is, by PpStepId: the noun and the setter its messages name, the selection outputs
+// (kSelOut) it reads as a bit mask, and its launcher on maps of type T.  A step that reads selection outputs needs a context over the
+// whole range, and after it a left-only context's left-right step fills from the chain's own map.
 template <typename T>
+struct PpStepInfo {
+    const char* noun;
+    const char* setter;
+    unsigned reads;
+    int (*launch)(psm_ctx* c, const uint8_t* const in[2], uint8_t* const out[2]);
+};
+template <typename T>
+constexpr PpStepInfo<T> kPpStep[kNumPpSteps] = {
+    {"uniqueness check", "psm_set_uniqueness_check", 1u << kOutCosts | 1u << kOutRunnerUp, unique_check<T>},
+    {"disparity check", "psm_set_disparity_check", 1u << kOutCosts, disparity_check<T>},
+    {"median blur", "psm_set_median_blur", 0, median_blur<T>},
+    {"speckle filter", "psm_set_speckle_filter", 0, speckle_filter<T>},
+    {"left-right check", "psm_set_lr_check", 0, lr_check_fill<T>},
+};
+
+// the options of the selection outputs in `reads` (a kSelOut bit mask), joined by " and "
+static const char* reads_text(unsigned reads, char (&buf)[64])
+{
+    buf[0] = 0;
+    for (int o = 0; o < kNumOuts; ++o)
+        if (reads >> o & 1) {
+            const size_t n = strlen(buf);
+            snprintf(buf + n, sizeof(buf) - n, "%s%s", n ? " and " : "", kSelOut[o].option);
+        }
+    return buf;
+}
+
+// psm_set_<step>: mode 0, 1 or kPpEnd and the step's own arguments; a mode other than off, for a step that reads
+// selection outputs, only on a context over the whole range.  A multi-device context spans the range and its first
+// shard holds the complete maps and outputs: it judges the value once, then every shard takes it.
+static int set_pp_step(psm_ctx* c, int step, int mode, int a = 0, int b = 0)
+{
+    if (!c) return fail(nullptr, PSM_EINVAL, "null context");
+    const PpStepInfo<uint8_t>& f = kPpStep<uint8_t>[step];   // everything but the launcher is the same for every map type
+    if (mode < 0 || mode > kPpEnd) return fail(c, PSM_EINVAL, "%s mode %d is not off (0), 1 or 2", f.noun, mode);
+    if (step == kPpUnique && (a < 0 || a > 100)) return fail(c, PSM_EINVAL, "uniqueness ratio %d outside 0..100", a);
+    if (step == kPpDcheck && (a < 0 || a > 4095)) return fail(c, PSM_EINVAL, "disparity check max_diff %d outside 0..4095", a);
+    if (step == kPpMedian && a != 3 && a != 5) return fail(c, PSM_EINVAL, "median blur ksize %d is not 3 or 5", a);
+    if (step == kPpSpeckle && mode && (a < 1 || b < 0))
+        return fail(c, PSM_EINVAL, "speckle filter max_size %d / max_diff %d: need max_size >= 1 and max_diff >= 0", a, b);
+    if (mode && f.reads && !c->owns_problem()) {
+        char outs[64];
+        return fail(c, PSM_EINVAL, "%s on a context that owns slices [%d,%d) of %d: the %s reads %s, which such a "
+                    "context cannot write; use a context over the whole range", f.setter, c->d_begin,
+                    c->d_begin + c->d_count, c->D, f.noun, reads_text(f.reads, outs));
+    }
+    c->pp_steps[step] = {mode, a, b};
+    for (int k = 0; k < c->nshards; ++k) c->shard[k]->pp_steps[step] = c->pp_steps[step];
+    return PSM_OK;
+}
+
+extern "C" {
+
+int psm_set_uniqueness_check(psm_ctx* c, int mode, int ratio) { return set_pp_step(c, kPpUnique, mode, ratio); }
+int psm_set_disparity_check(psm_ctx* c, int mode, int max_diff) { return set_pp_step(c, kPpDcheck, mode, max_diff); }
+int psm_set_median_blur(psm_ctx* c, int mode, int ksize) { return set_pp_step(c, kPpMedian, mode, ksize); }
+int psm_set_speckle_filter(psm_ctx* c, int mode, int max_size, int max_diff)
+{
+    return set_pp_step(c, kPpSpeckle, mode, max_size, max_diff);
+}
+int psm_set_lr_check(psm_ctx* c, int mode) { return set_pp_step(c, kPpLr, mode); }
+
+}  // extern "C"
+
+// psm_post_process's steps in front of the post-filter (wmf): the steps that are on, in chain order, up to the first
+// whose mode is kPpEnd; the post-filter runs when no step ends the chain
 struct PpChain {
-    using Step = int (*)(psm_ctx*, const uint8_t* const*, uint8_t* const*);
-    Step step[5];
+    int step[kNumPpSteps];   // PpStepId
     int n = 0;
-    bool wmf = false;
+    bool wmf = true;
     explicit PpChain(const psm_ctx* c)
     {
-        if (c->un_mode != PSM_UNIQUE_OFF) step[n++] = unique_check<T>;
-        if (c->un_mode == PSM_UNIQUE_ONLY) return;
-        if (c->dc_mode != PSM_DCHECK_OFF) step[n++] = disparity_check<T>;
-        if (c->dc_mode == PSM_DCHECK_ONLY) return;
-        if (c->md_mode != PSM_MEDIAN_OFF) step[n++] = median_blur<T>;
-        if (c->md_mode == PSM_MEDIAN_ONLY) return;
-        if (c->sp_mode != PSM_SPECKLE_OFF) step[n++] = speckle_filter<T>;
-        if (c->sp_mode == PSM_SPECKLE_ONLY) return;
-        const bool own = c->views == 1 && (has(unique_check<T>) || has(disparity_check<T>));
-        if (c->lr_mode != PSM_LR_OFF) step[n++] = own ? lr_check_fill<T, true> : lr_check_fill<T, false>;
-        wmf = c->lr_mode != PSM_LR_FILL;
+        for (int s = 0; s < kNumPpSteps && wmf; ++s) {
+            if (c->pp_steps[s].mode) step[n++] = s;
+            wmf = c->pp_steps[s].mode != kPpEnd;
+        }
     }
-    bool has(Step s) const { return std::find(step, step + n, s) != step + n; }
 };
 
 // the post-process stage on maps of type T
@@ -2846,21 +2833,25 @@ static int post_process_maps(psm_ctx* c)
     const uint8_t* maps[2];
     if (int rc = selection_maps(c, "psm_post_process", maps)) return rc;
     const size_t npix = (size_t)c->W * c->H;
-    const PpChain<T> p(c);
-    if (p.has(unique_check<T>) && !(c->outs[kOutCosts].have && c->outs[kOutRunnerUp].have))
-        return fail(c, PSM_ESTATE, "psm_post_process: the uniqueness test (psm_set_uniqueness_check mode %d) reads the "
-                    "winners' costs and the runner-up, and the last selection stage did not write both: set PSM_OPT_COSTS = 1 "
-                    "and PSM_OPT_RUNNER_UP = 1 before it", c->un_mode);
-    if (p.has(disparity_check<T>) && !c->outs[kOutCosts].have)
-        return fail(c, PSM_ESTATE, "psm_post_process: the disparity check (psm_set_disparity_check mode %d) reads the "
-                    "winners' costs, and the last selection stage did not write them: set PSM_OPT_COSTS = 1 before it",
-                    c->dc_mode);
-    if (p.has(lr_check_fill<T, false>) && c->views == 1)
-        return fail(c, PSM_ESTATE, "psm_post_process: the left-right check (psm_set_lr_check mode %d) needs both maps, and "
-                    "this context computes the left view alone (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): set PSM_LR_OFF or "
-                    "PSM_VIEWS_BOTH", c->lr_mode);
-    if (p.has(speckle_filter<T>) && npix > (size_t)INT_MAX)
-        return fail(c, PSM_EINVAL, "psm_post_process: speckle removal labels pixels with int32 indices (W * H <= 2^31 - 1)");
+    const PpChain p(c);
+    bool read_outs = false;   // a step so far reads selection outputs
+    for (int i = 0; i < p.n; ++i) {
+        const int s = p.step[i], mode = c->pp_steps[s].mode;
+        const PpStepInfo<T>& f = kPpStep<T>[s];
+        for (int o = 0; o < kNumOuts; ++o)
+            if ((f.reads >> o & 1) && !c->outs[o].have) {
+                char outs[64];
+                return fail(c, PSM_ESTATE, "psm_post_process: the %s (%s mode %d) reads %s, and the last selection stage "
+                            "did not write them all: set each to 1 before it", f.noun, f.setter, mode, reads_text(f.reads, outs));
+            }
+        read_outs = read_outs || f.reads;
+        if (s == kPpLr && c->views == 1 && !read_outs)
+            return fail(c, PSM_ESTATE, "psm_post_process: the left-right check (psm_set_lr_check mode %d) needs both maps, "
+                        "and this context computes the left view alone (PSM_OPT_VIEWS = PSM_VIEWS_LEFT): set PSM_LR_OFF or "
+                        "PSM_VIEWS_BOTH", mode);
+        if (s == kPpSpeckle && npix > (size_t)INT_MAX)
+            return fail(c, PSM_EINVAL, "psm_post_process: speckle removal labels pixels with int32 indices (W * H <= 2^31 - 1)");
+    }
     // Each buffer is allocated while its own pointer is null and the table is marked valid only once it is on the
     // device, so a call that failed part-way leaves nothing a launch could trip over: the next call completes the set-up
     // or fails in turn.
@@ -2869,15 +2860,17 @@ static int post_process_maps(psm_ctx* c)
         PSM_CUDA(c, alloc_if_null(c->pp_packed, npix * sizeof(uint32_t)));
     }
     for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->dis_pp[v], npix * c->map_bytes));
-    if (p.has(lr_check_fill<T, false>) || p.has(lr_check_fill<T, true>))
-        for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->lr_valid[v], npix));
     if (p.n >= 2)
         for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->pp_tmp[v], npix * c->map_bytes));
-    if (p.has(disparity_check<T>) && c->W > kDcStageCols)
-        for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->dc_claims[v], npix * sizeof(unsigned long long)));
-    if (p.has(speckle_filter<T>)) {
-        PSM_CUDA(c, alloc_if_null(c->sp_lab, 2 * npix * sizeof(int)));
-        PSM_CUDA(c, alloc_if_null(c->sp_cnt, 2 * npix * sizeof(int)));
+    for (int i = 0; i < p.n; ++i) {   // each step's own scratch
+        if (p.step[i] == kPpLr)
+            for (int v = 0; v < 2; ++v) PSM_CUDA(c, alloc_if_null(c->lr_valid[v], npix));
+        if (p.step[i] == kPpDcheck && c->W > kDcStageCols)
+            for (int v = 0; v < c->views; ++v) PSM_CUDA(c, alloc_if_null(c->dc_claims[v], npix * sizeof(unsigned long long)));
+        if (p.step[i] == kPpSpeckle) {
+            PSM_CUDA(c, alloc_if_null(c->sp_lab, 2 * npix * sizeof(int)));
+            PSM_CUDA(c, alloc_if_null(c->sp_cnt, 2 * npix * sizeof(int)));
+        }
     }
     if (p.wmf && !c->pp_lut_valid) {
         const size_t smem = kPpParamWarps * 256 * sizeof(unsigned long long) + (size_t)(kPpMaxD2 + 1) * sizeof(uint32_t);
@@ -2898,7 +2891,7 @@ static int post_process_maps(psm_ctx* c)
     // the last step writes dis_pp, the ones before alternate back through pp_tmp: no step writes the maps it reads
     for (int i = 0; i < p.n; ++i) {
         uint8_t* const* out = (p.n - 1 - i) % 2 ? c->pp_tmp : c->dis_pp;
-        if (int rc = p.step[i](c, maps, out)) return rc;
+        if (int rc = kPpStep<T>[p.step[i]].launch(c, maps, out)) return rc;
         maps[0] = out[0]; maps[1] = out[1];
     }
     if (!p.wmf) return stage_end(c, 5);

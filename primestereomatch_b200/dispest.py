@@ -132,7 +132,160 @@ def bayer_kind(pattern, method="bilinear"):
     return tuple(names)
 
 
-class DispEst:
+class _Context:
+    """The settings and lifetime DispEst and TorchStereo share.  A subclass sets _lib (the library, or None when it was
+    constructed without the GPU path: every setter then raises RuntimeError), _ctx (the context's handle) and _map_size
+    (the maps' (W, H)).  Each setter passes its values to the C-ABI, which judges them (PsmError), and returns 0.  The
+    docstrings name DispEst's stages; TorchStereo.match runs the same ones."""
+
+    src_size = None   # setRectify: (SW, SH) of the camera frames the frame calls take; None = frames of the maps' size
+    # setLRCheck's last accepted mode, for callers that read it; PostProcess_GPU asks the context whether the check ran
+    lr_mode = capi.PSM_LR_OFF
+
+    # -- lifetime ---------------------------------------------------------------------------
+    def close(self):
+        if self._lib is not None and self._ctx:
+            self._lib.psm_destroy(self._ctx)
+            self._ctx = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    @property
+    def handle(self):
+        return self._ctx
+
+    def _check(self, rc):
+        capi.check(rc, self._ctx)
+
+    def _need_gpu(self):
+        if self._lib is None:
+            raise RuntimeError("DispEst was constructed with ocl=False: the GPU stages are unavailable")
+
+    # -- settings ---------------------------------------------------------------------------
+    def setGuidedFilter(self, window, eps):
+        """Guided-filter window and regulariser (the reference's compile-time GIF_R_WIN and GIF_EPS, include/ComFunc.h:49-50)
+        for every later CostFilter_GPU / CostFilter_FGF_GPU call; default (8, 1e-4).  Raises PsmError on values outside
+        1 <= window <= 32, 0 < eps < inf."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_guided_filter(self._ctx, int(window), float(eps)))
+        return 0
+
+    def setMatchingCost(self, alpha, tau_color, tau_grad):
+        """Matching-cost weight and truncation thresholds (the reference's compile-time ALPHA_32F, TAU_1_32F and TAU_2_32F,
+        include/CVC.h:18-23, with the truncation of src/CVC.cpp:24-25,36-37 applied) for every later CostConst_GPU call;
+        default (0.9, inf, inf), the reference as shipped.  Raises PsmError unless 0 <= alpha <= 1 and each tau is >= 0 or
+        inf (no truncation)."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_matching_cost(self._ctx, float(alpha), float(tau_color), float(tau_grad)))
+        return 0
+
+    _WMF_WEIGHTS = {"exp": capi.PSM_WMF_EXP, "iv1": capi.PSM_WMF_IV1, "iv2": capi.PSM_WMF_IV2, "off": capi.PSM_WMF_OFF}
+
+    def setPostFilter(self, radius, sigma=25.5, iterations=1, weight="exp"):
+        """Joint weighted-median post-filter (JointWMF::filter's r, sigma, iter and weightType; the reference's PP::processDM
+        passes MED_SZ/2 = 9 and the defaults) for every later PostProcess_GPU call; default (9, 25.5, 1, "exp").  weight is
+        "exp", "iv1", "iv2" or "off".  Raises PsmError unless 1 <= radius <= 32, 2^-16 <= sigma <= 2^16 and
+        1 <= iterations <= 16, and on any other weight name."""
+        self._need_gpu()
+        wt = self._WMF_WEIGHTS.get(weight, -1) if isinstance(weight, str) else -1
+        self._check(self._lib.psm_set_post_filter(self._ctx, int(radius), float(sigma), int(iterations), wt))
+        return 0
+
+    def setLRCheck(self, mode):
+        """Left-right consistency check and occlusion fill (the reference's lrCheck / fillInv, commented out in
+        PP::processDM, src/PP.cpp:405-406) for every later PostProcess_GPU call: 0 off (default), 1 check + fill + the
+        post-filter (processDM with those lines restored), 2 check + fill only.  With mode 1 or 2 PostProcess_GPU also
+        fills lValid / rValid (0/1).  Raises PsmError on any other mode."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_lr_check(self._ctx, int(mode)))
+        self.lr_mode = int(mode)
+        return 0
+
+    def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
+        """Speckle removal (OpenCV's filterSpeckles(map, 0, max_size, max_diff)) for every later PostProcess_GPU call:
+        0 off (default), 1 first (then the check and / or post-filter of setLRCheck / setPostFilter on its result), 2 only
+        (its maps are the result; lValid / rValid are not read).  Every 4-connected blob of non-zero pixels whose
+        neighbours differ by at most max_diff, of at most max_size pixels, becomes 0 (invalid).  Raises PsmError on any
+        other mode, or unless max_size >= 1 and max_diff >= 0 with the filter on."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)))
+        return 0
+
+    def setDisparityCheck(self, mode, max_diff=1):
+        """One-view disparity check (OpenCV's validateDisparity, StereoSGBM's disp12MaxDiff) for every later
+        PostProcess_GPU call: 0 off (default), 1 first (then setSpeckleFilter's removal and the check and / or post-filter
+        of setLRCheck / setPostFilter on its result), 2 only (its maps are the result; lValid / rValid are not read).  In
+        each row, the pixels at x >= maxDis claim the other view's column their disparity points at, the lowest cost of
+        setCostOutput's centre plane winning; a pixel whose disparity differs from its column's winner's by more than
+        max_diff becomes 0 (invalid).  Needs setCostOutput(True) for the selection it checks.  On a left-only context,
+        mode 1 with setLRCheck 1 or 2 fills the left map where it is below 2 and fills lValid.  Raises PsmError on any
+        other mode, on max_diff outside [0, 4095], or on a context that owns part of the range with the check on."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_disparity_check(self._ctx, int(mode), int(max_diff)))
+        return 0
+
+    def setUniquenessCheck(self, mode, ratio=10):
+        """Uniqueness test (OpenCV StereoSGBM's uniquenessRatio) for every later PostProcess_GPU call: 0 off (default),
+        1 first (then the rest of the chain -- setDisparityCheck, setMedianBlur, setSpeckleFilter, setLRCheck,
+        setPostFilter -- on its result), 2 only (its maps are the result; lValid / rValid are not read).  A pixel with
+        m != 0 becomes 0 (invalid) when its runner-up's cost q(r) (setRunnerUpOutput's plane 1) is within ratio percent
+        of its winner's cost q(m) (setCostOutput's centre plane): q(r) * (100 - ratio) < q(m) * 100, exactly.  Needs
+        setCostOutput(True) and setRunnerUpOutput(True) for the selection it tests.  On a left-only context, mode 1 with
+        setLRCheck 1 or 2 fills the left map where it is below 2 and fills lValid.  Raises PsmError on any other mode, on
+        ratio outside [0, 100], or on a context that owns part of the range with the test on."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_uniqueness_check(self._ctx, int(mode), int(ratio)))
+        return 0
+
+    def setMedianBlur(self, mode, ksize=3):
+        """ksize x ksize median (OpenCV's medianBlur, StereoSGBM's fixed medianBlur(disp, 3)) for every later
+        PostProcess_GPU call, after the uniqueness test and the disparity check: 0 off (default), 1 first (then
+        setSpeckleFilter's removal and the check and / or post-filter on its result), 2 only (the chain up to the median;
+        its maps are the result; lValid / rValid are not read).  Equals cv2.medianBlur(map, ksize) on the u8 or u16 map,
+        zeros included as values.  Raises PsmError on any other mode or on ksize other than 3 or 5."""
+        self._need_gpu()
+        self._check(self._lib.psm_set_median_blur(self._ctx, int(mode), int(ksize)))
+        return 0
+
+    def setRectify(self, left_maps, right_maps, src_size):
+        """Rectify every later frame on the device (psm_set_rectify): the reference's video-mode remap(frame, rec,
+        map[0], map[1], INTER_LINEAR) and crop, bit for bit.  left_maps / right_maps: (xy, a) of each view as
+        initUndistortRectifyMap(..., CV_16SC2) returns them, cropped to the maps' W x H (xy int16 (H, W, 2), a uint16
+        (H, W)); src_size: (SW, SH) of the camera frames.  setInputImages then takes uint8 frames of SH x SW x 3, and
+        TorchStereo.match uint8 frames of (SH, SW) in any layout frame_layout reads (the two halves of one side-by-side
+        tensor included); float frames raise PsmError (DispEst) or ValueError (TorchStereo).  None for all three turns it
+        off.  Raises TypeError / ValueError on malformed maps before any device work."""
+        args, _keep = rectify_args(left_maps, right_maps, src_size, *self._map_size)
+        self._need_gpu()
+        self._check(self._lib.psm_set_rectify(self._ctx, *args))
+        self.src_size = None if src_size is None else (args[0], args[1])
+        return 0
+
+    _VIEWS = {"left": capi.PSM_VIEWS_LEFT, "both": capi.PSM_VIEWS_BOTH}   # the values of each class's own setViews
+
+    # -- measurement helpers ----------------------------------------------------------------
+    def stage_ms(self, stage):
+        ms = C.c_float()
+        self._check(self._lib.psm_stage_ms(self._ctx, stage, C.byref(ms)))
+        return ms.value
+
+    def launch_count(self):
+        n = C.c_uint64()
+        self._check(self._lib.psm_launch_count(self._ctx, C.byref(n)))
+        return n.value
+
+
+class DispEst(_Context):
     """DispEst(l, r, d, t, ocl) -- reference src/DispEst.cpp:10-143.
 
     l, r : HxWx3 images, both float32 in [0,1] (CV_32FC3) or both uint8 (CV_8UC3), BGR order.
@@ -160,6 +313,7 @@ class DispEst:
         if l.ndim != 3 or l.shape[2] != 3 or l.dtype not in (np.float32, np.uint8):
             raise ValueError("DispEst expects HxWx3 float32 or uint8 images")
         self.hei, self.wid = int(l.shape[0]), int(l.shape[1])
+        self._map_size = (self.wid, self.hei)
         self.maxDis = int(d)
         self.map_bits = resolve_map_bits(self.maxDis, map_bits)
         mdt = np.uint16 if self.map_bits == 16 else np.uint8
@@ -170,11 +324,6 @@ class DispEst:
         self.rDisMap = np.zeros((self.hei, self.wid), mdt)
         self.lValid = np.zeros((self.hei, self.wid), np.uint8)  # DispEst.cpp:48-49
         self.rValid = np.zeros((self.hei, self.wid), np.uint8)
-        self.lr_mode = capi.PSM_LR_OFF
-        self.speckle_mode = capi.PSM_SPECKLE_OFF
-        self.dcheck_mode = capi.PSM_DCHECK_OFF
-        self.unique_mode = capi.PSM_UNIQUE_OFF
-        self.median_mode = capi.PSM_MEDIAN_OFF
         self.cost_output = False
         self.lCosts = self.rCosts = None   # setCostOutput(True): DispSelect_GPU's (3, H, W) float32 costs
         self.runner_up_output = False
@@ -184,7 +333,6 @@ class DispEst:
         if min_disp and (d_begin != 0 or d_count is not None):
             raise ValueError("min_disp (a range context over [min_disp, max_disp)) excludes d_begin / d_count")
         self.min_disp = int(min_disp)
-        self.src_size = None   # setRectify: (SW, SH) of the camera frames CostConst_GPU takes
         self._lImg, self._rImg = l, r
         self._yuv = None   # setInputImagesYUV's format code while its frames are the input
         self._bayer = None   # setInputImagesBayer's (pattern, method) codes while its frames are the input
@@ -199,24 +347,6 @@ class DispEst:
         self.d_begin, self.d_count = d_begin, (self.maxDis - d_begin if d_count is None else d_count)
         self.block_slices = None if devices is not None and not block_slices else block_slices   # 0: unblocked shards
         self.devices = None if devices is None else list(devices)
-
-    # -- lifetime ---------------------------------------------------------------------------
-    def close(self):
-        if self._lib is not None and self._ctx:
-            self._lib.psm_destroy(self._ctx)
-            self._ctx = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
 
     # -- reference public methods -----------------------------------------------------------
     def setInputImages(self, leftImg, rightImg):
@@ -266,110 +396,6 @@ class DispEst:
 
     def setSubsampleRate(self, newRate):
         self.subsample_rate = int(newRate)
-
-    def setGuidedFilter(self, window, eps):
-        """Guided-filter window and regulariser (the reference's compile-time GIF_R_WIN and GIF_EPS, include/ComFunc.h:49-50)
-        for every later CostFilter_GPU / CostFilter_FGF_GPU call; default (8, 1e-4).  Raises PsmError on values outside
-        1 <= window <= 32, 0 < eps < inf."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_guided_filter(self._ctx, int(window), float(eps)), self._ctx)
-        return 0
-
-    def setMatchingCost(self, alpha, tau_color, tau_grad):
-        """Matching-cost weight and truncation thresholds (the reference's compile-time ALPHA_32F, TAU_1_32F and TAU_2_32F,
-        include/CVC.h:18-23, with the truncation of src/CVC.cpp:24-25,36-37 applied) for every later CostConst_GPU call;
-        default (0.9, inf, inf), the reference as shipped.  Raises PsmError unless 0 <= alpha <= 1 and each tau is >= 0 or
-        inf (no truncation)."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_matching_cost(self._ctx, float(alpha), float(tau_color), float(tau_grad)), self._ctx)
-        return 0
-
-    _WMF_WEIGHTS = {"exp": capi.PSM_WMF_EXP, "iv1": capi.PSM_WMF_IV1, "iv2": capi.PSM_WMF_IV2, "off": capi.PSM_WMF_OFF}
-
-    def setPostFilter(self, radius, sigma=25.5, iterations=1, weight="exp"):
-        """Joint weighted-median post-filter (JointWMF::filter's r, sigma, iter and weightType; the reference's PP::processDM
-        passes MED_SZ/2 = 9 and the defaults) for every later PostProcess_GPU call; default (9, 25.5, 1, "exp").  weight is
-        "exp", "iv1", "iv2" or "off".  Raises PsmError unless 1 <= radius <= 32, 2^-16 <= sigma <= 2^16 and
-        1 <= iterations <= 16, and on any other weight name."""
-        self._need_gpu()
-        wt = self._WMF_WEIGHTS.get(weight, -1) if isinstance(weight, str) else -1
-        capi.check(self._lib.psm_set_post_filter(self._ctx, int(radius), float(sigma), int(iterations), wt), self._ctx)
-        return 0
-
-    def setLRCheck(self, mode):
-        """Left-right consistency check and occlusion fill (the reference's lrCheck / fillInv, commented out in
-        PP::processDM, src/PP.cpp:405-406) for every later PostProcess_GPU call: 0 off (default), 1 check + fill + the
-        post-filter (processDM with those lines restored), 2 check + fill only.  With mode 1 or 2 PostProcess_GPU also
-        fills lValid / rValid (0/1).  Raises PsmError on any other mode."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_lr_check(self._ctx, int(mode)), self._ctx)
-        self.lr_mode = int(mode)
-        return 0
-
-    def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
-        """Speckle removal (OpenCV's filterSpeckles(map, 0, max_size, max_diff)) for every later PostProcess_GPU call:
-        0 off (default), 1 first (then the check and / or post-filter of setLRCheck / setPostFilter on its result), 2 only
-        (its maps are the result; lValid / rValid are not read).  Every 4-connected blob of non-zero pixels whose
-        neighbours differ by at most max_diff, of at most max_size pixels, becomes 0 (invalid).  Raises PsmError on any
-        other mode, or unless max_size >= 1 and max_diff >= 0 with the filter on."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)), self._ctx)
-        self.speckle_mode = int(mode)
-        return 0
-
-    def setDisparityCheck(self, mode, max_diff=1):
-        """One-view disparity check (OpenCV's validateDisparity, StereoSGBM's disp12MaxDiff) for every later
-        PostProcess_GPU call: 0 off (default), 1 first (then setSpeckleFilter's removal and the check and / or post-filter
-        of setLRCheck / setPostFilter on its result), 2 only (its maps are the result; lValid / rValid are not read).  In
-        each row, the pixels at x >= maxDis claim the other view's column their disparity points at, the lowest cost of
-        setCostOutput's centre plane winning; a pixel whose disparity differs from its column's winner's by more than
-        max_diff becomes 0 (invalid).  Needs setCostOutput(True) for the selection it checks.  On a left-only context,
-        mode 1 with setLRCheck 1 or 2 fills the left map where it is below 2 and fills lValid.  Raises PsmError on any
-        other mode, on max_diff outside [0, 4095], or on a context that owns part of the range with the check on."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_disparity_check(self._ctx, int(mode), int(max_diff)), self._ctx)
-        self.dcheck_mode = int(mode)
-        return 0
-
-    def setUniquenessCheck(self, mode, ratio=10):
-        """Uniqueness test (OpenCV StereoSGBM's uniquenessRatio) for every later PostProcess_GPU call: 0 off (default),
-        1 first (then the rest of the chain -- setDisparityCheck, setMedianBlur, setSpeckleFilter, setLRCheck,
-        setPostFilter -- on its result), 2 only (its maps are the result; lValid / rValid are not read).  A pixel with
-        m != 0 becomes 0 (invalid) when its runner-up's cost q(r) (setRunnerUpOutput's plane 1) is within ratio percent
-        of its winner's cost q(m) (setCostOutput's centre plane): q(r) * (100 - ratio) < q(m) * 100, exactly.  Needs
-        setCostOutput(True) and setRunnerUpOutput(True) for the selection it tests.  On a left-only context, mode 1 with
-        setLRCheck 1 or 2 fills the left map where it is below 2 and fills lValid.  Raises PsmError on any other mode, on
-        ratio outside [0, 100], or on a context that owns part of the range with the test on."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_uniqueness_check(self._ctx, int(mode), int(ratio)), self._ctx)
-        self.unique_mode = int(mode)
-        return 0
-
-    def setMedianBlur(self, mode, ksize=3):
-        """ksize x ksize median (OpenCV's medianBlur, StereoSGBM's fixed medianBlur(disp, 3)) for every later
-        PostProcess_GPU call, after the uniqueness test and the disparity check: 0 off (default), 1 first (then
-        setSpeckleFilter's removal and the check and / or post-filter on its result), 2 only (the chain up to the median;
-        its maps are the result; lValid / rValid are not read).  Equals cv2.medianBlur(map, ksize) on the u8 or u16 map,
-        zeros included as values.  Raises PsmError on any other mode or on ksize other than 3 or 5."""
-        self._need_gpu()
-        capi.check(self._lib.psm_set_median_blur(self._ctx, int(mode), int(ksize)), self._ctx)
-        self.median_mode = int(mode)
-        return 0
-
-    def setRectify(self, left_maps, right_maps, src_size):
-        """Rectify every later frame on the device (psm_set_rectify): the reference's video-mode remap(frame, rec,
-        map[0], map[1], INTER_LINEAR) and crop, bit for bit.  left_maps / right_maps: (xy, a) of each view as
-        initUndistortRectifyMap(..., CV_16SC2) returns them, cropped to the constructor's W x H (xy int16 (H, W, 2), a
-        uint16 (H, W)); src_size: (SW, SH) of the camera frames.  setInputImages then takes uint8 frames of SH x SW x 3;
-        float frames raise PsmError.  None for all three turns it off.  Raises TypeError / ValueError on malformed maps
-        before any device work."""
-        args, _keep = rectify_args(left_maps, right_maps, src_size, self.wid, self.hei)
-        self._need_gpu()
-        capi.check(self._lib.psm_set_rectify(self._ctx, *args), self._ctx)
-        self.src_size = None if src_size is None else (args[0], args[1])
-        return 0
-
-    _VIEWS = {"left": capi.PSM_VIEWS_LEFT, "both": capi.PSM_VIEWS_BOTH}
 
     def setViews(self, views):
         """Which disparity maps the later frames compute (PSM_OPT_VIEWS): "both" (default) or "left".  "left" skips every
@@ -429,10 +455,6 @@ class DispEst:
 
     def set_option(self, key, value):
         capi.check(self._lib.psm_set_option(self._ctx, int(key), int(value)), self._ctx)
-
-    def _need_gpu(self):
-        if not self.useOCL or self._lib is None:
-            raise RuntimeError("DispEst was constructed with ocl=False: the GPU stages are unavailable")
 
     def CostConst_GPU(self):
         """DispEst.cpp:272-276: upload both images, build both raw cost volumes on the device."""
@@ -501,11 +523,12 @@ class DispEst:
         self._need_gpu()
         pp = self._lib.psm_post_process_u16 if self.map_bits == 16 else self._lib.psm_post_process
         capi.check(pp(self._ctx, _ptr(self.lDisMap), self.lDisMap.strides[0], *self._map_arg(self.rDisMap)), self._ctx)
-        ended = capi.PSM_SPECKLE_ONLY in (self.unique_mode, self.dcheck_mode, self.median_mode, self.speckle_mode)
-        if self.lr_mode != capi.PSM_LR_OFF and not ended:   # the check ran (a left-only fill masks the left view)
-            masks = ((capi.PSM_LEFT, self.lValid),) + (((capi.PSM_RIGHT, self.rValid),) if self.rDisMap is not None else ())
-            for view, mask in masks:
-                capi.check(self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0]), self._ctx)
+        masks = ((capi.PSM_LEFT, self.lValid),) + (((capi.PSM_RIGHT, self.rValid),) if self.rDisMap is not None else ())
+        for view, mask in masks:
+            rc = self._lib.psm_read_valid_mask(self._ctx, view, _ptr(mask), mask.strides[0])
+            if rc == capi.PSM_ESTATE:   # the check did not run (a left-only fill masks the left view alone)
+                break
+            capi.check(rc, self._ctx)
         return 0
 
     _VIEW = {"left": capi.PSM_LEFT, "right": capi.PSM_RIGHT}
@@ -560,19 +583,5 @@ class DispEst:
         capi.check(self._lib.psm_read_ab_slice(self._ctx, view, d, _ptr(a), _ptr(b)), self._ctx)
         return a, b
 
-    def stage_ms(self, stage):
-        ms = C.c_float()
-        capi.check(self._lib.psm_stage_ms(self._ctx, stage, C.byref(ms)), self._ctx)
-        return ms.value
-
-    def launch_count(self):
-        n = C.c_uint64()
-        capi.check(self._lib.psm_launch_count(self._ctx, C.byref(n)), self._ctx)
-        return n.value
-
     def sync(self):
         capi.check(self._lib.psm_sync(self._ctx), self._ctx)
-
-    @property
-    def handle(self):
-        return self._ctx

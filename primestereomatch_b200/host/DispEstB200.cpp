@@ -114,41 +114,31 @@ int DispEst::setPostFilter(int radius, float sigma, int iterations, int weight_t
 int DispEst::setLRCheck(int mode)
 {
     if (!ctx) return -1;
-    const int rc = psm_set_lr_check(ctx, mode);
-    if (rc == PSM_OK) lr_mode = mode;
-    return rc;
+    return psm_set_lr_check(ctx, mode);
 }
 
 int DispEst::setSpeckleFilter(int mode, int max_size, int max_diff)
 {
     if (!ctx) return -1;
-    const int rc = psm_set_speckle_filter(ctx, mode, max_size, max_diff);
-    if (rc == PSM_OK) speckle_mode = mode;
-    return rc;
+    return psm_set_speckle_filter(ctx, mode, max_size, max_diff);
 }
 
 int DispEst::setDisparityCheck(int mode, int max_diff)
 {
     if (!ctx) return -1;
-    const int rc = psm_set_disparity_check(ctx, mode, max_diff);
-    if (rc == PSM_OK) dcheck_mode = mode;
-    return rc;
+    return psm_set_disparity_check(ctx, mode, max_diff);
 }
 
 int DispEst::setUniquenessCheck(int mode, int ratio)
 {
     if (!ctx) return -1;
-    const int rc = psm_set_uniqueness_check(ctx, mode, ratio);
-    if (rc == PSM_OK) unique_mode = mode;
-    return rc;
+    return psm_set_uniqueness_check(ctx, mode, ratio);
 }
 
 int DispEst::setMedianBlur(int mode, int ksize)
 {
     if (!ctx) return -1;
-    const int rc = psm_set_median_blur(ctx, mode, ksize);
-    if (rc == PSM_OK) median_mode = mode;
-    return rc;
+    return psm_set_median_blur(ctx, mode, ksize);
 }
 
 int DispEst::setViews(int v)
@@ -308,8 +298,8 @@ int DispEst::DispSelect_GPU()
 // both maps, after the left-right check and fill that setLRCheck enables (PP.cpp:405-406, psm_lr.cuh) and the speckle
 // removal, disparity check, uniqueness test and median that setSpeckleFilter, setDisparityCheck, setUniquenessCheck and
 // setMedianBlur enable (psm_speckle.cuh, psm_dcheck.cuh, psm_unique.cuh, psm_median.cuh).  The reference runs it on the
-// CPU even in GPU mode; here it is a device stage (psm_pp.cuh).  The masks exist only where the check ran (not under
-// any of the steps' _ONLY modes), the right one only on a two-view context.
+// CPU even in GPU mode; here it is a device stage (psm_pp.cuh).  The masks exist only where the check ran (the context
+// answers PSM_ESTATE otherwise), the right one only on a two-view context.
 int DispEst::PostProcess_GPU()
 {
     if (!ctx) return -1;
@@ -317,9 +307,9 @@ int DispEst::PostProcess_GPU()
     const int rc = lDisMap.type() == CV_16UC1
         ? psm_post_process_u16(ctx, lDisMap.ptr<uint16_t>(), lDisMap.step, both ? rDisMap.ptr<uint16_t>() : nullptr, rDisMap.step)
         : psm_post_process(ctx, lDisMap.ptr<uint8_t>(), lDisMap.step, both ? rDisMap.ptr<uint8_t>() : nullptr, rDisMap.step);
-    if (rc || lr_mode == PSM_LR_OFF || speckle_mode == PSM_SPECKLE_ONLY || dcheck_mode == PSM_DCHECK_ONLY ||
-        unique_mode == PSM_UNIQUE_ONLY || median_mode == PSM_MEDIAN_ONLY)
-        return rc;
-    if (int e = psm_read_valid_mask(ctx, PSM_LEFT, lValid.ptr<uint8_t>(), lValid.step)) return e;
+    if (rc) return rc;
+    const int e = psm_read_valid_mask(ctx, PSM_LEFT, lValid.ptr<uint8_t>(), lValid.step);
+    if (e == PSM_ESTATE) return 0;   // the check did not run
+    if (e) return e;
     return both ? psm_read_valid_mask(ctx, PSM_RIGHT, rValid.ptr<uint8_t>(), rValid.step) : 0;
 }

@@ -194,11 +194,6 @@ private:
     int hei, wid, maxDis, threads;
     bool useOCL;
     unsigned int subsample_rate = 4;
-    int lr_mode = PSM_LR_OFF;
-    int speckle_mode = PSM_SPECKLE_OFF;
-    int dcheck_mode = PSM_DCHECK_OFF;
-    int unique_mode = PSM_UNIQUE_OFF;
-    int median_mode = PSM_MEDIAN_OFF;
     int views = PSM_VIEWS_BOTH;
     int src_w = 0, src_h = 0;   // setRectify: the size of the frames CostConst_GPU takes, 0 = the context's
     int yuv_format = 0;         // setInputImagesYUV: the PSM_YUV_* format of lImg / rImg, 0 = BGR frames

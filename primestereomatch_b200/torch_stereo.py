@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import capi
-from .dispest import DispEst, bayer_kind, create_context, rectify_args, resolve_map_bits, yuv_format, yuv_shape
+from .dispest import _Context, bayer_kind, create_context, resolve_map_bits, yuv_format, yuv_shape
 
 _PIX = {torch.uint8: capi.PSM_PIX_U8, torch.float32: capi.PSM_PIX_F32}
 _ORDER = {"bgr": (0, 1, 2), "rgb": (2, 1, 0)}   # the tensor channel that holds B, G and R
@@ -145,7 +145,7 @@ def _pointers(frame):
     return C.c_void_p(frame) if isinstance(frame, int) else (C.c_void_p * 3)(*frame)
 
 
-class TorchStereo:
+class TorchStereo(_Context):
     """TorchStereo(width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None, min_disp=0)
 
     The context `DispEst` creates for the same arguments: `device` (an index, "cuda:k" or torch.device; None = the
@@ -154,10 +154,9 @@ class TorchStereo:
     [min_disp, max_disp), psm_create_range).  The setters pass their values straight to the C-ABI, which rejects bad ones
     with PsmError."""
 
-    src_size = None   # setRectify: (SW, SH) of the raw frames match takes; None = frames of (height, width)
-
     def __init__(self, width, height, max_disp, *, device=None, map_bits=None, block_slices=None, devices=None, min_disp=0):
         self.width, self.height, self.max_disp = int(width), int(height), int(max_disp)
+        self._map_size = (self.width, self.height)
         self.min_disp = int(min_disp)
         self.map_bits = resolve_map_bits(self.max_disp, map_bits)
         if devices is not None:
@@ -177,74 +176,23 @@ class TorchStereo:
         self._ctx = create_context(self.width, self.height, self.max_disp, self.map_bits, device=index,
                                    block_slices=block_slices, devices=devices, min_disp=self.min_disp)
 
-    # -- lifetime ---------------------------------------------------------------------------
-    def close(self):
-        if self._ctx:
-            self._lib.psm_destroy(self._ctx)
-            self._ctx = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    @property
-    def handle(self):
-        return self._ctx
-
     # -- settings (the C-ABI judges every value) ---------------------------------------------
-    def _check(self, rc):
-        capi.check(rc, self._ctx)
-
-    def setGuidedFilter(self, window, eps):
-        self._check(self._lib.psm_set_guided_filter(self._ctx, int(window), float(eps)))
-
-    def setMatchingCost(self, alpha, tau_color, tau_grad):
-        self._check(self._lib.psm_set_matching_cost(self._ctx, float(alpha), float(tau_color), float(tau_grad)))
-
-    def setPostFilter(self, radius, sigma=25.5, iterations=1, weight="exp"):
-        wt = DispEst._WMF_WEIGHTS.get(weight, -1) if isinstance(weight, str) else -1
-        self._check(self._lib.psm_set_post_filter(self._ctx, int(radius), float(sigma), int(iterations), wt))
-
-    def setLRCheck(self, mode):
-        self._check(self._lib.psm_set_lr_check(self._ctx, int(mode)))
-
-    def setSpeckleFilter(self, mode, max_size=0, max_diff=0):
-        self._check(self._lib.psm_set_speckle_filter(self._ctx, int(mode), int(max_size), int(max_diff)))
-
     def setDisparityCheck(self, mode, max_diff=1):
         """DispEst.setDisparityCheck.  match(post_process=True) then turns PSM_OPT_COSTS on itself, since the check reads
         the winners' costs; it returns them only with costs=True."""
-        self._check(self._lib.psm_set_disparity_check(self._ctx, int(mode), int(max_diff)))
+        super().setDisparityCheck(mode, max_diff)
         self.dcheck = int(mode)
+        return 0
 
     def setUniquenessCheck(self, mode, ratio=10):
         """DispEst.setUniquenessCheck.  match(post_process=True) then turns PSM_OPT_COSTS and PSM_OPT_RUNNER_UP on
         itself, since the test reads both; it returns them only with costs=True / runner_up=True."""
-        self._check(self._lib.psm_set_uniqueness_check(self._ctx, int(mode), int(ratio)))
+        super().setUniquenessCheck(mode, ratio)
         self.unique = int(mode)
-
-    def setMedianBlur(self, mode, ksize=3):
-        """DispEst.setMedianBlur."""
-        self._check(self._lib.psm_set_median_blur(self._ctx, int(mode), int(ksize)))
-
-    def setRectify(self, left_maps, right_maps, src_size):
-        """DispEst.setRectify: from then on match takes uint8 camera frames of (SH, SW) in any layout frame_layout reads
-        -- the two halves of one side-by-side tensor included -- and rectifies them on the device; float frames raise
-        ValueError before any device work.  None for all three turns it off."""
-        args, _keep = rectify_args(left_maps, right_maps, src_size, self.width, self.height)
-        self._check(self._lib.psm_set_rectify(self._ctx, *args))
-        self.src_size = None if src_size is None else (args[0], args[1])
+        return 0
 
     def setViews(self, views):
-        value = DispEst._VIEWS.get(views, -1) if isinstance(views, str) else -1
+        value = self._VIEWS.get(views, -1) if isinstance(views, str) else -1
         self._check(self._lib.psm_set_option(self._ctx, capi.PSM_OPT_VIEWS, value))
         self.views = value
 
@@ -389,14 +337,3 @@ class TorchStereo:
         self._check(L.psm_signal_stream(ctx, stream))
         return (lmap, rmap) + tuple(t for _, lo, ro in outs for t in (lo, ro)) + \
             (tuple(pts) if qs is not None else ())
-
-    # -- measurement helpers ------------------------------------------------------------------
-    def stage_ms(self, stage):
-        ms = C.c_float()
-        self._check(self._lib.psm_stage_ms(self._ctx, stage, C.byref(ms)))
-        return ms.value
-
-    def launch_count(self):
-        n = C.c_uint64()
-        self._check(self._lib.psm_launch_count(self._ctx, C.byref(n)))
-        return n.value
